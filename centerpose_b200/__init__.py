@@ -1,4 +1,4 @@
-"""centerpose_b200 -- B200-native (sm_100a) CenterPose inference hot path.
+"""centerpose_b200 -- H100-native (sm_90a) CenterPose inference hot path.
 
 Public surface (mirrors the reference's, see INTEGRATION.md):
     create_model, load_model, save_model      <- lib.models.model

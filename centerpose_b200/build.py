@@ -1,9 +1,9 @@
-"""Build libcenterpose_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libcenterpose_b200.so in-tree with nvcc for sm_90a (cross-compiles without a GPU).
 
     python -m centerpose_b200.build [--force]
 
 The shared library lands next to this file so that it travels to the GPU box
-with the repository snapshot; nothing is JIT-compiled at run time.
+with the repository; nothing is JIT-compiled at run time.
 """
 import os
 import subprocess
@@ -19,7 +19,7 @@ def _headers():
     return hs + [os.path.join("..", "..", "include", "centerpose_b200.h")]
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "--expt-relaxed-constexpr",
@@ -72,7 +72,7 @@ def build(force=False, verbose=False):
     if verbose and logs:
         print("\n".join(logs))
     if force or procs or _stale(LIB, objs):
-        cmd = [_nvcc(), "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-lcudart"]
+        cmd = [_nvcc(), "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_90a,code=sm_90a", "-lcudart"]
         subprocess.check_call(cmd)
     return LIB
 

@@ -1,4 +1,4 @@
-// Shared declarations for libcenterpose_b200.so (sm_100a only).
+// Shared declarations for libcenterpose_b200.so (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -64,7 +64,7 @@ struct IgemmParams {
   int omStride;
   int mask_is_logit;     // 1: apply sigmoid to channels 18..26
   int mode;
-  const void* wgt_umma;  // tcgen05 path: pre-swizzled weight tiles (igemm_umma.cu), else null
+  const void* wgt_umma;  // tensor-core path: pre-swizzled weight tiles (igemm_umma.cu, conv_tma.cu, dcn_tma.cu), else null
   // conv_tma only: the per-head 1x1 convolutions fused into the epilogue of the merged heads 3x3 conv.  Head h owns the
   // output columns [h * fuse_hidden, (h + 1) * fuse_hidden); its 1x1 weights are [fuse_hidden][16] fp32 (rows = hidden
   // channel, 16 padded outputs), bias [16], output NCHW [B, fuse_cout[h], Hout, Wout].  fuse_n == 0: not fused.
@@ -86,7 +86,7 @@ int launch_conv3_c16(const IgemmParams& p, cudaStream_t stream);
 bool stem_supported(const IgemmParams& p);
 int launch_stem_conv(const IgemmParams& p, cudaStream_t s);
 
-// tcgen05 tensor-core path (igemm_umma.cu).  prec: 0 = bf16 (kind::f16), 1 = tf32 x 3 (kind::tf32, fp32-equivalent)
+// wgmma tensor-core gather path (igemm_umma.cu).  prec: 0 = bf16, 1 = tf32 x 3 (fp32-equivalent)
 bool umma_supported(const IgemmParams& p, int prec);
 size_t umma_weight_bytes(int Kreal, int CoutPad, int prec);
 int launch_pack_umma_weight(const float* src_k_by_ld, int ld, int Kreal, int Cout, int CoutPad, int prec, void* dst,
@@ -113,13 +113,13 @@ int launch_group_norm_relu(float* x, const float* gamma, const float* beta, int 
 int launch_gru_gates(const float* xi, const float* hh, const float* hprev, float* hout, int B_HW, int C,
                      int first_step, cudaStream_t s);
 
-// TMA-fed shifted-window tcgen05 convolution (conv_tma.cu): stride-1 1x1 / 3x3 over NHWC fp32, kind::tf32
+// TMA-fed shifted-window wgmma convolution (conv_tma.cu): stride-1 1x1 / 3x3 over NHWC fp32, tf32 operands
 // x3 = 1: 3-term split with two-level accumulation (fp32-equivalent); x3 = 0: single tf32 pass
 bool tma_conv_supported(const IgemmParams& p, int x3);
 size_t tma_weight_bytes(int Cin, int taps, int CoutPad, int x3);
 int tma_tile_n(int CoutPad, int x3);             // N tile of conv_tma for this output width
 int tma_cslab(const IgemmParams& p, int x3);     // channels per activation slab (32 or 16); needs Cin, kh, Win, CoutPad
-int x3_group_blocks();                           // tf32x3: 32-channel K blocks per TMEM accumulation group
+int x3_group_blocks();                           // tf32x3: 32-channel K blocks per accumulation group
 int launch_pack_tma_weight(const float* src_k_by_ld, int ld, int Cin, int taps, int Cout, int CoutPad, int round_tf32,
                            int x3, int cslab, void* dst, cudaStream_t s, int bn_override = 0);
 int tma_encode_nhwc_box(const float* base, int C, int W, int H, int B, int strideFloats, int boxC, int boxW, int boxH,
@@ -138,11 +138,11 @@ inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
 
 // ---------------------------------------------------------------------------
 // Programmatic dependent launch (PDL).  The forward is ~90 dependent launches; at batch 1 a launch is ~25 us of which the
-// launch latency + the fixed prologue of a tcgen05 CTA (barrier init, TMEM allocation, first weight tiles) is a third.
+// launch latency + the fixed prologue of a tensor-core CTA (barrier init, first weight tiles) is a large share.
 // Every kernel of the forward schedule therefore (a) signals `launch_dependents` at its very start, so the NEXT kernel's
 // CTAs are placed on an SM the moment a CTA of this one retires, and (b) executes `griddep_wait()` before its first
 // read of an activation / first global write.  What runs before the wait touches only per-plan constants (weights,
-// biases) and the CTA's own shared memory / TMEM.  Kernels launched without the attribute see both instructions as no-ops.
+// biases) and the CTA's own shared memory.  Kernels launched without the attribute see both instructions as no-ops.
 // g_pdl is set by run_forward (plan.cu) around the op loop; stand-alone ops (cp_conv2d ...) pack their weights on the
 // stream right before the launch and therefore never use it.  CP_NO_PDL=1 disables it (A/B runs).
 extern thread_local int g_pdl;

@@ -1,20 +1,19 @@
-// TMA-fed tcgen05 convolution ("shifted-window" implicit GEMM) for stride-1 1x1 / 3x3 convolutions
-// over NHWC fp32 activations, kind::tf32.
+// TMA-fed wgmma convolution ("shifted-window" implicit GEMM) for stride-1 1x1 / 3x3 convolutions
+// over NHWC fp32 activations, tf32 operands.
 //
 // Idea: pad the image by one pixel and flatten it to a 1-D sequence of positions with pitch Wt = W + 2.
 // A 3x3 tap (ky, kx) is then a CONSTANT offset (ky-1)*Wt + (kx-1) in that sequence, so the A operand of
 // tap (ky,kx) for 128 consecutive output positions is simply the same shared-memory slab read from a
 // different start row.  One TMA tiled load (box = 32 channels x Wt columns x BOXH rows, out-of-bounds
 // elements zero-filled = the convolution padding) brings a [positions][32 ch] slab of 128-byte rows in
-// SWIZZLE_128B layout; nine UMMA descriptors with different start addresses contract it against nine
+// SWIZZLE_128B layout; nine wgmma descriptors with different start addresses contract it against nine
 // weight tiles.  Outputs computed at the two pad columns of every row are discarded (W/Wt efficiency).
 // The im2col matrix never exists anywhere and no thread touches activation data before the epilogue.
 //
 //   warp 0 : TMA producer for activation slabs            (ring of SA stages)
 //   warp 1 : weight-tile producer, cp.async.bulk          (ring of SB stages, tiles pre-swizzled at load time)
-//   warp 2 : tcgen05.mma issuer (one lane), accumulator in TMEM; also owns the TMEM allocation
-//   warp 3 : idle
-//   warps 4-7 : epilogue, TMEM lane == flattened output position
+//   warpgroups 1, 2 : consumers, rows [0, 64) / [64, 128) of the tile: wgmma into registers + epilogue
+//   warpgroup 3 (x3 only) : hi / lo splitters of the activation slabs
 // Reference semantics: nn.Conv2d(k, stride 1, padding k//2) + folded BatchNorm + residual + ReLU
 // (pose_dla_dcn.py:37-62, 153-168, 496-505).
 #include <cuda.h>
@@ -27,13 +26,13 @@ namespace cp {
 namespace {
 
 constexpr int TM_BM = 128;
-constexpr int TM_THREADS = 256;
+constexpr int TM_THREADS = 384;       // control warpgroup + two consumer warpgroups
+constexpr int TM_THREADS_X3 = 512;    // + the splitter warpgroup
 constexpr int TM_GROUP_X3 = 1;
 }  // namespace
 
-// tf32x3: 32-channel K blocks (12 MMAs each) per TMEM accumulation group.  The tensor core's fp32 accumulator TRUNCATES
-// every add (measured; the error is biased towards zero and grows with the chain length), so a group is promoted into
-// round-to-nearest fp32 sums after this many blocks.  CP_X3_GROUP overrides (diagnostics).
+// tf32x3: 32-channel K blocks (12 MMAs each) chained in the wgmma accumulator before they are added, with
+// round-to-nearest, into fp32 running sums in registers.  CP_X3_GROUP overrides (diagnostics).
 int x3_group_blocks() {
   int g = TM_GROUP_X3;
   if (const char* e = getenv("CP_X3_GROUP")) {
@@ -51,12 +50,11 @@ struct TmaConvParams {
   int srcC[4];
   int B, H, W, Cin, Cout, CoutPad, BN;
   int k;              // 1 or 3
-  int tile_m;         // output positions per tile: 128 (x1) or 256 (x3: two M sub-tiles share every weight tile)
+  int tile_m;         // output positions per tile (128)
   int Wt, boxh;       // padded pitch and slab rows (k == 3)
   int tiles_per_image;
-  long long total_tiles;                // cluster tiles: m groups x n tiles (n fastest)
-  long long m_tiles;                    // real number of 128-position tiles
-  int cluster;                          // CTAs per cluster (1, 2 or 4): same N tile, consecutive M tiles, weight tiles multicast
+  long long total_tiles;                // m tiles x n tiles (n fastest), x split-K factor
+  long long m_tiles;                    // number of 128-position tiles
   uint32_t slab_bytes, slab_stride;   // TMA transaction bytes, 1024-aligned stage stride
   int SA, SB;
   const float* bias;
@@ -64,12 +62,10 @@ struct TmaConvParams {
   int resStride, relu, res_after_relu;
   float* out;
   int outStride, out_nchw;
-  int round_tf32;     // round the stored outputs to tf32 (consumers feed them to kind::tf32 untouched)
+  int round_tf32;     // round the stored outputs to tf32 (consumers feed them to the tf32 MMAs untouched)
   int cslab;          // channels per slab: 32 (128-byte rows, SWIZZLE_128B) or 16 (64-byte rows, SWIZZLE_64B; Cin = 16 layers)
   int x3;             // 3-term split (fp32-equivalent): hi/lo slabs + hi/lo weight tiles, BN <= 128
-  int group;          // x3: K blocks per TMEM accumulation group (promoted into fp32 registers after each group)
-  int nbuf;           // TMEM accumulation buffers of tile_m x BN (2; x3 with narrow N tiles: up to 8, all 512 columns)
-  int cat;            // x3, N tile <= 64: hi and lo weight tiles are ONE 2 BN-row B operand (see issue_tile)
+  int group;          // x3: K blocks per accumulation group (promoted into the fp32 sums after each group)
   const unsigned char* wtiles;
   // split-K (x3, not fused): the K loop of a tile is dealt to `ksplit` CTAs (slab-aligned ranges of `sps` slabs); every
   // CTA stores its promoted partial sums and conv_tma_splitk_finish adds them in split order (deterministic) and runs
@@ -89,31 +85,18 @@ using namespace umma;
 struct TmaCtl {
   unsigned long long a_full[4], a_empty[4], a_split[4];
   unsigned long long b_full[8], b_empty[8];
-  unsigned long long accum_full;
-  unsigned long long p_full[8], p_empty[8];
-  unsigned long long w2_full, w2_empty;      // x3 fused heads: 1x1 weights + 3x3 bias of the current tile in shared memory
-  uint32_t tmem_base;
 };
 static_assert(sizeof(TmaCtl) <= 512, "control block");
-
-// x3 fused heads: [128 hidden][16] fp32 1x1 weights of the tile's (head, part) followed by the 128 biases of the 3x3 conv
-constexpr uint32_t TM_W2_BYTES = 128u * 16u * 4u;
-constexpr uint32_t TM_W2_BUF = TM_W2_BYTES + 128u * 4u;
-
-constexpr int TM_THREADS_X3 = 512;    // x3: warps 4-11 epilogue (two 128-row sub-tiles), warps 12-15 hi/lo splitters
 
 // Tile geometry of one 128-position output tile.
 struct TileGeo {
   int n_tile, img, g0, r_lo;
   long long pos0;
 };
-// cluster tile `ct` -> this CTA's (n tile, m tile); m tiles past the end are clamped (computed redundantly, never stored)
-__device__ __forceinline__ TileGeo decode_tile(const TmaConvParams& p, long long ct, int n_tiles, int rank, bool* live) {
+__device__ __forceinline__ TileGeo decode_tile(const TmaConvParams& p, long long ct, int n_tiles) {
   TileGeo g;
   g.n_tile = (int)(ct % n_tiles);
-  long long m_tile = (ct / n_tiles) * p.cluster + rank;
-  *live = m_tile < p.m_tiles;
-  if (!*live) m_tile = p.m_tiles - 1;
+  const long long m_tile = ct / n_tiles;
   g.img = 0;
   g.g0 = 0;
   g.r_lo = 0;
@@ -129,435 +112,132 @@ __device__ __forceinline__ TileGeo decode_tile(const TmaConvParams& p, long long
   return g;
 }
 
-// fused 1x1 epilogue: outputs of one position of one head -> NCHW [B, Cout, H, W] (+ the 1x1 bias)
-template <int NA>
-__device__ __forceinline__ void fused_store(const TmaConvParams& p, int head, const float (&acc2)[NA], int n, int oy, int ox) {
-  const int co = p.fuse_cout[head];
-  const float* b2 = p.fuse_b[head];
-  float* o = p.fuse_out[head] + ((size_t)n * co * p.H + oy) * p.W + ox;
-  const size_t plane = (size_t)p.H * p.W;
-#pragma unroll
-  for (int j = 0; j < 16; ++j)
-    if (j < co && j < NA) o[j * plane] = acc2[j < NA ? j : 0] + __ldg(b2 + j);
-}
-
-// x3 fused heads: hidden[c] = relu(sums[c] + b1[c]) is multiplied with the [128][16] weight block in shared memory.
-// Every lane reads the SAME address (broadcast, one wavefront); only V = ceil(cout / 4) float4 groups are touched, so the
-// narrow heads (hm 1, wh / reg / hp_offset 2, scale 3 outputs) cost 4 FMAs per hidden channel instead of 16.
-template <int V>
-__device__ __forceinline__ void fused_part_smem(const float (&sums)[128], float (&acc2)[16], uint32_t w2s, uint32_t b1s) {
-#pragma unroll
-  for (int c4 = 0; c4 < 32; ++c4) {
-    const float4 bb = ld_shared_v4f(b1s + (uint32_t)c4 * 16u);
-    const float bq[4] = {bb.x, bb.y, bb.z, bb.w};
-#pragma unroll
-    for (int u = 0; u < 4; ++u) {
-      const int c = c4 * 4 + u;
-      const float v = fmaxf(sums[c] + bq[u], 0.f);
-#pragma unroll
-      for (int q = 0; q < V; ++q) {
-        const float4 w = ld_shared_v4f(w2s + (uint32_t)(c * 64 + q * 16));
-        acc2[q * 4 + 0] = fmaf(v, w.x, acc2[q * 4 + 0]);
-        acc2[q * 4 + 1] = fmaf(v, w.y, acc2[q * 4 + 1]);
-        acc2[q * 4 + 2] = fmaf(v, w.z, acc2[q * 4 + 2]);
-        acc2[q * 4 + 3] = fmaf(v, w.w, acc2[q * 4 + 3]);
-      }
-    }
+// output position i of a tile -> (valid, image, row, column, flat NHWC index)
+__device__ __forceinline__ bool tile_position(const TmaConvParams& p, const TileGeo& g, int i, int* n, int* oy, int* ox, int* m) {
+  bool valid;
+  if (p.k == 3) {
+    const int gg = g.g0 + i;
+    *oy = gg / p.Wt;
+    const int xp = gg - *oy * p.Wt;
+    *ox = xp - 1;
+    *n = g.img;
+    valid = (*oy < p.H) && (xp >= 1) && (xp <= p.W);
+  } else {
+    const long long pix = g.pos0 + i;
+    valid = pix < (long long)p.B * p.H * p.W;
+    const long long pp = valid ? pix : 0;
+    *ox = (int)(pp % p.W);
+    const long long t = pp / p.W;
+    *oy = (int)(t % p.H);
+    *n = (int)(t / p.H);
   }
-}
-
-// ---- MMA issue loop (one warp; see the comment at its call site) --------------------------------------------------------
-struct IssueCtx {
-  uint32_t idesc, dhi, rowu, a_lo_u, b_lo_u, sub_u, a0_u, a_stage_u, b0_u, b_stage_u, tmem_base, buf_cols, bn;
-  uint32_t idesc2, sub_cols;      // cat: instruction descriptor with N = 2 BN; TMEM columns of one sub-tile (BN or 2 BN)
-  int cat;
-  uint32_t bar_a, bar_a_empty, bar_b_full, bar_b_empty, bar_p_full, bar_p_empty;
-  uint32_t tap_u[2];
-  int group, KB, SA, SB, nslab, cluster, nbuf;
-  uint32_t sub0_a, sub0_d;        // descriptor / TMEM column offset of this issuer's first sub-tile (two issuers: sub-tile 1)
-  uint16_t cmask;
-};
-struct IssueState {
-  int sa = 0, sb = 0, buf = 0;
-  uint32_t pa = 0, pb = 0, pe = 0;        // pe bit b: phase of p_empty[b]
-};
-
-template <bool X3, int MSL, int TAPS, int KS>
-__device__ __forceinline__ void issue_tile(const IssueCtx& c, IssueState& st, uint32_t tap0) {
-  int kbi = 0, gk = 0;                     // K-block index inside the tile (slab-major, tap-minor) / inside its group
-  for (int s = 0; s < c.nslab; ++s) {
-    mbar_wait(c.bar_a + 8u * (uint32_t)st.sa, st.pa);
-    tc_fence_after();
-    const uint32_t a_slab = c.a0_u + (uint32_t)st.sa * c.a_stage_u + tap0;
-    // the tap loop stays ROLLED (one copy of the body in the instruction cache); the descriptor offset of tap (ky, kx) =
-    // (ky Wt + kx) rows is stepped: + 1 row inside a kernel row, + (Wt - 2) rows at its end
-    uint32_t tap_off = 0;
-    int kx = 0;
-#pragma unroll 1
-    for (int tap = 0; tap < TAPS; ++tap, ++kbi) {
-      const bool first = X3 ? (gk == 0) : (kbi == 0);
-      if (first)                           // new accumulation group / tile: the epilogue must have drained this TMEM buffer
-        mbar_wait(c.bar_p_empty + 8u * (uint32_t)st.buf, ((st.pe >> st.buf) & 1u) ^ 1u);
-      mbar_wait(c.bar_b_full + 8u * (uint32_t)st.sb, st.pb);
-      tc_fence_after();
-      const uint32_t da = a_slab + tap_off + c.sub0_a;
-      if (++kx == 3) {
-        kx = 0;
-        tap_off += c.tap_u[1];       // (Wt - 2) rows
-      } else {
-        tap_off += c.tap_u[0];       // 1 row
-      }
-      const uint32_t db = c.b0_u + (uint32_t)st.sb * c.b_stage_u;
-      const uint32_t d_tmem = c.tmem_base + (uint32_t)st.buf * c.buf_cols + c.sub0_d;
-      const bool last = X3 ? (gk == c.group - 1 || kbi == c.KB - 1) : (kbi == c.KB - 1);
-      if (elect_one()) {
-        if (X3 && c.cat) {
-          // N tile <= 64.  Measured (scripts/mma_rate.cu): below N = 128 a tf32 MMA is bound by the fetch of its 4 KB A
-          // operand -- 45.5 clk at N = 32, 48 at N = 64 -- so the hi and lo weight tiles, which sit back to back in shared
-          // memory, are read as ONE B operand of 2 BN rows: a_hi x [b_hi | b_lo] costs what a_hi x b_hi cost, and the
-          // 3-term product is two instructions instead of three.  Columns [0, BN) of the accumulator hold
-          // a_lo b_hi + a_hi b_hi (promoted every group), columns [BN, 2 BN) the cross term a_hi b_lo, which is 2^-11 of
-          // the main term: its truncation is harmless, so it keeps accumulating and is drained once per tile.  The
-          // epilogue zeroes what it drains (tcgen05.st), every MMA accumulates.
-#pragma unroll
-          for (int ks = 0; ks < KS; ++ks) {
-#pragma unroll
-            for (int sub = 0; sub < MSL; ++sub)
-              umma_tf32_lohi(d_tmem + (uint32_t)sub * c.sub_cols, da + (uint32_t)sub * c.sub_u + 2u * ks + c.a_lo_u, db + 2u * ks,
-                             c.dhi, c.idesc, 1u);
-          }
-#pragma unroll
-          for (int ks = 0; ks < KS; ++ks) {
-#pragma unroll
-            for (int sub = 0; sub < MSL; ++sub)
-              umma_tf32_lohi(d_tmem + (uint32_t)sub * c.sub_cols, da + (uint32_t)sub * c.sub_u + 2u * ks, db + 2u * ks, c.dhi,
-                             c.idesc2, 1u);
-          }
-        } else if (X3) {
-          // The accumulator truncates every add (error ~ its magnitude x chain length): the two cross terms of all K
-          // slices go first, while the accumulator still holds small values, the hi x hi terms last.
-#pragma unroll
-          for (int ks = 0; ks < KS; ++ks) {
-            const uint32_t acc = (first && ks == 0) ? 0u : 1u;
-#pragma unroll
-            for (int sub = 0; sub < MSL; ++sub) {         // rows [128 sub, 128 sub + 128) of the tile
-              const uint32_t das = da + (uint32_t)sub * c.sub_u + 2u * ks;
-              const uint32_t dt = d_tmem + (uint32_t)sub * c.sub_cols;
-              umma_tf32_lohi(dt, das + c.a_lo_u, db + 2u * ks, c.dhi, c.idesc, acc);
-              umma_tf32_lohi(dt, das, db + c.b_lo_u + 2u * ks, c.dhi, c.idesc, 1u);
-            }
-          }
-#pragma unroll
-          for (int ks = 0; ks < KS; ++ks) {
-#pragma unroll
-            for (int sub = 0; sub < MSL; ++sub)
-              umma_tf32_lohi(d_tmem + (uint32_t)sub * c.sub_cols, da + (uint32_t)sub * c.sub_u + 2u * ks, db + 2u * ks, c.dhi,
-                             c.idesc, 1u);
-          }
-        } else {
-#pragma unroll
-          for (int ks = 0; ks < KS; ++ks)
-            umma_tf32_lohi(d_tmem, da + 2u * ks, db + 2u * ks, c.dhi, c.idesc, (first && ks == 0) ? 0u : 1u);
-        }
-        if (c.cluster > 1)
-          umma_commit_multicast(c.bar_b_empty + 8u * (uint32_t)st.sb, c.cmask);
-        else
-          umma_commit(c.bar_b_empty + 8u * (uint32_t)st.sb);
-        if (last) umma_commit(c.bar_p_full + 8u * (uint32_t)st.buf);        // group / tile finished -> epilogue
-        if (tap == TAPS - 1) umma_commit(c.bar_a_empty + 8u * (uint32_t)st.sa);
-      }
-      if (++st.sb == c.SB) {
-        st.sb = 0;
-        st.pb ^= 1u;
-      }
-      if (last) {
-        st.pe ^= 1u << st.buf;
-        if (++st.buf == c.nbuf) st.buf = 0;
-        gk = 0;
-      } else {
-        ++gk;
-      }
-    }
-    if (++st.sa == c.SA) {
-      st.sa = 0;
-      st.pa ^= 1u;
-    }
-  }
-}
-
-struct IssueTiles {            // 32-bit tile arithmetic (the launcher rejects > 2^31 tiles): no 64-bit divisions per tile
-  int cluster_id, num_clusters, tph, total_tiles;
-  int n_tiles, rank, ksplit;
-};
-
-// DUAL: two warps issue, one M sub-tile each (issuer 1 only walks the barriers of a tile whose second sub-tile is empty)
-template <bool X3, int MS, int TAPS, int KS, bool DUAL>
-__device__ __forceinline__ void issue_all_tiles(const TmaConvParams& p, const IssueCtx& c, const IssueTiles& tl, int issuer) {
-  IssueState st;
-  const int Wt = p.Wt, HWt = p.H * p.Wt;
-  const long long total_pos = (long long)p.B * p.H * p.W;
-  for (int it = 0;; ++it) {
-    const int unit = it / tl.tph;
-    const int tile = (tl.cluster_id + unit * tl.num_clusters) * tl.tph + (it - unit * tl.tph);
-    if (tile >= tl.total_tiles) break;
-    bool live;
-    const TileGeo g = decode_tile(p, tile / tl.ksplit, tl.n_tiles, tl.rank, &live);
-    const uint32_t tap0 = (TAPS == 9) ? (uint32_t)(g.g0 - 1 - g.r_lo * Wt) * c.rowu : 0u;
-    // x3: small feature maps end inside the first 128 rows of their last tile; the second accumulator is then skipped.
-    // MSL = sub-tiles with output positions: a compile-time count, so the unrolled MMA list carries no predication
-    const bool sub1_live = (TAPS == 9) ? (g.g0 + TM_BM < HWt) : (g.pos0 + TM_BM < total_pos);
-    if (DUAL) {
-      if (issuer == 0 || sub1_live)
-        issue_tile<X3, 1, TAPS, KS>(c, st, tap0);
-      else
-        issue_tile<X3, 0, TAPS, KS>(c, st, tap0);
-    } else if (MS == 2 && sub1_live) {
-      issue_tile<X3, MS, TAPS, KS>(c, st, tap0);
-    } else {
-      issue_tile<X3, 1, TAPS, KS>(c, st, tap0);
-    }
-  }
+  *m = (int)(((size_t)*n * p.H + *oy) * p.W + *ox);
+  return valid;
 }
 
 // PERSISTENT kernel: gridDim.x = min(#tiles, #SMs); CTA c processes tiles c, c + gridDim.x, ...  Every role keeps its
-// pipeline state across tiles, so the TMA / split / MMA of tile i+1 overlap the epilogue of tile i and the fixed cost
-// of a CTA (barrier init, TMEM allocation, descriptor fetch, pipeline fill) is paid once per SM instead of per tile.
-template <bool X3, bool FUSE>
+// pipeline state across tiles, so the TMA / split of tile i+1 overlap the epilogue of tile i and the fixed cost of a CTA
+// (barrier init, descriptor fetch, pipeline fill) is paid once per SM instead of per tile.
+template <bool X3, bool FUSE, int BN>
 __global__ void __launch_bounds__(X3 ? TM_THREADS_X3 : TM_THREADS, 1) conv_tma_kernel(const __grid_constant__ TmaConvParams p) {
   extern __shared__ __align__(1024) unsigned char smem[];
   TmaCtl* ctl = reinterpret_cast<TmaCtl*>(smem);
   if (threadIdx.x == 0) griddep_launch_dependents();      // PDL (common.cuh): the next launch may take this SM when we retire
-  // x3 computes TWO 128-row M sub-tiles per weight tile (tile = 256 positions): the weight stream from L2, the measured
-  // limiter, is halved per MMA.  The sub-tiles are two accumulators side by side in TMEM and two sets of epilogue warps.
-  constexpr int MS = X3 ? 2 : 1;
-  // x3 without the fused 1x1: warps 2 AND 3 issue MMAs, one sub-tile each.  The issue loop of a single warp (~100 dependent
-  // scalar instructions per K block at ~5 clk each) bounds every layer whose K blocks carry little tensor work.
-  constexpr bool DUAL = X3 && !FUSE;
-  constexpr int NISSUE = DUAL ? 2 : 1;
   const uint32_t slabs0 = (smem_u32(smem) + 512u + 1023u) & ~1023u;
   const uint32_t rowb = (uint32_t)p.cslab * 4u;                               // bytes per position row
-  const int kslices = p.cslab / 8;                                            // tf32 MMA K = 8
-  const uint32_t btile_bytes = (uint32_t)p.BN * rowb * (X3 ? 2u : 1u);         // hi (+ lo) weight tile
+  const uint32_t btile_bytes = (uint32_t)BN * rowb * (X3 ? 2u : 1u);          // hi (+ lo) weight tile
   const uint32_t a_stage = p.slab_stride * (X3 ? 2u : 1u);                    // hi (+ lo) slab
   const uint32_t btiles0 = slabs0 + (uint32_t)p.SA * a_stage;
-  const uint32_t w2buf = btiles0 + (uint32_t)p.SB * btile_bytes;                // x3 fused heads only (TM_W2_BUF bytes)
+  const uint32_t drain0 = btiles0 + (uint32_t)p.SB * btile_bytes;             // epilogue staging, one per consumer warpgroup
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int n_tiles = p.CoutPad / p.BN;
+  const int n_tiles = p.CoutPad / BN;
   const int taps = p.k * p.k;
-  const int nslab = p.Cin / p.cslab;
   const int KS_SPLIT = p.ksplit;                   // split-K factor (1 = off)
   const int sps = p.sps;                           // slabs per split
   const int KB = sps * taps;                       // K blocks THIS CTA runs per tile
-  const int KB_all = nslab * taps;                 // K blocks of the whole contraction (weight-tile addressing)
+  const int KB_all = (p.Cin / p.cslab) * taps;     // K blocks of the whole contraction (weight-tile addressing)
   const long long total_tiles = p.total_tiles;
-  const int rank = (p.cluster > 1) ? (int)cluster_ctarank() : 0;
-  const long long cluster_id = blockIdx.x / p.cluster;
-  const long long num_clusters = gridDim.x / p.cluster;
-  const uint16_t cmask = (uint16_t)((1u << p.cluster) - 1u);
   // Tile order of this CTA: units of `tph` consecutive tiles (same positions, the N tiles of one head when the 1x1 is
   // fused; tph = 1 otherwise), units strided over the CTAs.
   const long long tph = FUSE ? p.tph : 1;
-  auto tile_at = [&](long long it) { return (cluster_id + (it / tph) * num_clusters) * tph + (it % tph); };
+  auto tile_at = [&](long long it) { return ((long long)blockIdx.x + (it / tph) * gridDim.x) * tph + (it % tph); };
 
   if (tid == 0) {
     for (int s = 0; s < p.SA; ++s) {
       mbar_init(smem_u32(&ctl->a_full[s]), 1);
-      mbar_init(smem_u32(&ctl->a_empty[s]), NISSUE);
+      mbar_init(smem_u32(&ctl->a_empty[s]), 2);     // one arrival per consumer warpgroup
       mbar_init(smem_u32(&ctl->a_split[s]), 128);
     }
     for (int s = 0; s < p.SB; ++s) {
       mbar_init(smem_u32(&ctl->b_full[s]), 1);
-      mbar_init(smem_u32(&ctl->b_empty[s]), p.cluster * NISSUE);      // every issuer of every CTA of the cluster releases every CTA's slot
+      mbar_init(smem_u32(&ctl->b_empty[s]), 2);
     }
-    for (int s = 0; s < p.nbuf; ++s) {
-      mbar_init(smem_u32(&ctl->p_full[s]), NISSUE);  // x3: accumulation group ready / x1: tile accumulator ready
-      mbar_init(smem_u32(&ctl->p_empty[s]), 128 * MS);   // drained by the epilogue threads
-    }
-    mbar_init(smem_u32(&ctl->w2_full), 1);
-    mbar_init(smem_u32(&ctl->w2_empty), 4 * MS);         // one arrive per epilogue warp
     fence_mbar_init();
   }
-  // two TMEM accumulator buffers of BN columns: x1 ping-pongs whole tiles, x3 ping-pongs accumulation groups
-  const bool cat = X3 && !FUSE && p.cat;
-  uint32_t tmem_cols = 32;
-  while ((int)tmem_cols < p.BN * p.nbuf * MS * (cat ? 2 : 1)) tmem_cols <<= 1;
-  if (warp == 2) {
-    tmem_alloc(smem_u32(&ctl->tmem_base), tmem_cols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  if (p.cluster > 1) cluster_sync_all();       // remote arrives / multicast writes need every CTA's barriers initialised
-  const uint32_t tmem_base = ctl->tmem_base;
-  if (cat) {
-    // cat: every MMA accumulates and the epilogue zeroes what it has drained, so the accumulators start from zero
-    if (warp >= 4 && warp < 8) {
-      uint32_t z[32];
-#pragma unroll
-      for (int j = 0; j < 32; ++j) z[j] = 0u;
-      for (uint32_t col = 0; col < tmem_cols; col += 32) tmem_st32(tmem_base + ((uint32_t)((warp & 3) * 32) << 16) + col, z);
-      tmem_st_wait();
-    }
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-  }
-  // PDL: everything above touched shared memory / TMEM only.  The weight producer (warp 1) reads per-plan constants and
-  // runs ahead; every other role waits here for the previous launch of the stream to finish before it reads an
-  // activation (TMA slabs, residuals) or writes one.
+  // PDL: everything above touched shared memory only.  The weight producer (warp 1) reads per-plan constants and runs
+  // ahead; every other role waits here for the previous launch of the stream to finish before it reads an activation
+  // (TMA slabs, residuals) or writes one.
   if (warp != 1) griddep_wait();
 
-  // x3: 512 threads leave 128 registers per thread, but an epilogue thread carries the 128 promoted sums of its row.
-  // Warpgroup 0 (control warps) and 3 (splitters) hand registers to warpgroups 1-2 (epilogue) with setmaxnreg; the
-  // role code sits inside the branch that executed it so that ptxas allocates per branch.
+  // x3: 512 threads leave 128 registers per thread, but a consumer thread carries a 64 x BN accumulator AND the promoted
+  // sums.  The control and splitter warpgroups hand registers to the consumers with setmaxnreg; the role code sits
+  // inside the branch that executed it so that ptxas allocates per branch.
   if (warp < 4) {
-  if (X3) {
-    if (FUSE)
-      asm volatile("setmaxnreg.dec.sync.aligned.u32 80;");
-    else
-      asm volatile("setmaxnreg.dec.sync.aligned.u32 80;");
-  }
-  if (warp == 0) {
-    // ===================== activation slabs via TMA =====================
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (long long it = 0, tile = tile_at(0); tile < total_tiles; tile = tile_at(++it)) {
-        bool live;
-        const TileGeo g = decode_tile(p, tile / KS_SPLIT, n_tiles, rank, &live);
-        const int s_begin = (int)(tile % KS_SPLIT) * sps;
-        for (int s = s_begin; s < s_begin + sps; ++s) {
-          int src = 0, cb = 0;
-          while (src + 1 < p.nsrc && s * p.cslab >= cb + p.srcC[src]) {
-            cb += p.srcC[src];
-            ++src;
-          }
-          mbar_wait(smem_u32(&ctl->a_empty[stage]), phase ^ 1u);
-          const uint32_t bar = smem_u32(&ctl->a_full[stage]);
-          mbar_arrive_expect_tx(bar, p.slab_bytes);
-          const uint32_t dst = slabs0 + (uint32_t)stage * a_stage;
-          if (p.k == 3)
-            tma_load_4d(dst, &p.amap[src], s * p.cslab - cb, -1, g.r_lo - 1, g.img, bar);
-          else
-            tma_load_2d(dst, &p.amap[src], s * p.cslab - cb, (int)g.pos0, bar);
-          if (++stage == p.SA) {
-            stage = 0;
-            phase ^= 1u;
+    if (X3) asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (warp == 0) {
+      // ===================== activation slabs via TMA =====================
+      if (lane == 0) {
+        int stage = 0;
+        uint32_t phase = 0;
+        for (long long it = 0, tile = tile_at(0); tile < total_tiles; tile = tile_at(++it)) {
+          const TileGeo g = decode_tile(p, tile / KS_SPLIT, n_tiles);
+          const int s_begin = (int)(tile % KS_SPLIT) * sps;
+          for (int s = s_begin; s < s_begin + sps; ++s) {
+            int src = 0, cb = 0;
+            while (src + 1 < p.nsrc && s * p.cslab >= cb + p.srcC[src]) {
+              cb += p.srcC[src];
+              ++src;
+            }
+            mbar_wait(smem_u32(&ctl->a_empty[stage]), phase ^ 1u);
+            const uint32_t bar = smem_u32(&ctl->a_full[stage]);
+            mbar_arrive_expect_tx(bar, p.slab_bytes);
+            const uint32_t dst = slabs0 + (uint32_t)stage * a_stage;
+            if (p.k == 3)
+              tma_load_4d(dst, &p.amap[src], s * p.cslab - cb, -1, g.r_lo - 1, g.img, bar);
+            else
+              tma_load_2d(dst, &p.amap[src], s * p.cslab - cb, (int)g.pos0, bar);
+            if (++stage == p.SA) {
+              stage = 0;
+              phase ^= 1u;
+            }
           }
         }
       }
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    // ===================== weight tiles =====================
-    if (lane == 0) {
-      int stage = 0;
-      uint32_t phase = 0;
-      for (long long it = 0, tile = tile_at(0); tile < total_tiles; tile = tile_at(++it)) {
-        const int n_tile = (int)((tile / KS_SPLIT) % n_tiles);       // identical for all CTAs of the cluster
-        const unsigned char* wsrc = p.wtiles + ((size_t)n_tile * KB_all + (size_t)(tile % KS_SPLIT) * KB) * btile_bytes;
-        for (int kb = 0; kb < KB; ++kb) {
-          mbar_wait(smem_u32(&ctl->b_empty[stage]), phase ^ 1u);
-          const uint32_t bar = smem_u32(&ctl->b_full[stage]);
-          mbar_arrive_expect_tx(bar, btile_bytes);            // the whole tile lands here: one slice from every CTA
-          if (p.cluster > 1) {
-            const uint32_t slice = btile_bytes / (uint32_t)p.cluster;
-            bulk_g2s_multicast(btiles0 + (uint32_t)stage * btile_bytes + (uint32_t)rank * slice,
-                               wsrc + (size_t)kb * btile_bytes + (size_t)rank * slice, slice, bar, cmask);
-          } else {
+      __syncwarp();
+    } else if (warp == 1) {
+      // ===================== weight tiles =====================
+      if (lane == 0) {
+        int stage = 0;
+        uint32_t phase = 0;
+        for (long long it = 0, tile = tile_at(0); tile < total_tiles; tile = tile_at(++it)) {
+          const int n_tile = (int)((tile / KS_SPLIT) % n_tiles);
+          const unsigned char* wsrc = p.wtiles + ((size_t)n_tile * KB_all + (size_t)(tile % KS_SPLIT) * KB) * btile_bytes;
+          for (int kb = 0; kb < KB; ++kb) {
+            mbar_wait(smem_u32(&ctl->b_empty[stage]), phase ^ 1u);
+            const uint32_t bar = smem_u32(&ctl->b_full[stage]);
+            mbar_arrive_expect_tx(bar, btile_bytes);
             bulk_g2s(btiles0 + (uint32_t)stage * btile_bytes, wsrc + (size_t)kb * btile_bytes, btile_bytes, bar);
-          }
-          if (++stage == p.SB) {
-            stage = 0;
-            phase ^= 1u;
+            if (++stage == p.SB) {
+              stage = 0;
+              phase ^= 1u;
+            }
           }
         }
       }
+      __syncwarp();
     }
-    __syncwarp();
-  } else if (warp == 2 || (DUAL && warp == 3)) {
-    // ===================== MMA issuer(s) =====================
-    // The issue loop of this ONE warp bounds the kernel once the operand pipelines are deep enough (ncu stall sampling:
-    // the warp was busy executing descriptor arithmetic, not waiting).  So: the whole warp walks the warp-uniform loop
-    // (descriptors and barrier addresses stay in uniform registers), one elected lane issues, and a descriptor is a
-    // constant template plus (shared byte address >> 4) - stepping through taps and K slices is one add on the low word
-    // (the 14-bit address field cannot carry: shared addresses stay below 256 KB).
-    // Measured again in round 2 (profiles/r02_l2conv_ncu.md): with every operand pipeline full the warp spends 1500 clk
-    // per 16-channel K block on ~170 dependent instructions (12 % issue rate: constant re-loads, uniform-register chains,
-    // tap arithmetic) for 384 - 768 clk of MMA work -- the heads launch was bound by THIS loop, not by the L2 -> SM
-    // stream.  The loop below is specialised at compile time on (taps, K slices): the nine taps are unrolled with their
-    // descriptor offsets in registers, all parameters are hoisted, and a K block costs two barrier polls + its MMAs.
-    IssueCtx c;
-    c.idesc = make_idesc_tf32(p.BN);
-    const uint64_t dtmpl = make_desc(0, 0, p.cslab);
-    c.dhi = (uint32_t)(dtmpl >> 32);
-    const uint32_t dlo0 = (uint32_t)dtmpl;
-    c.rowu = rowb >> 4;
-    c.a_lo_u = p.slab_stride >> 4;
-    c.b_lo_u = ((uint32_t)p.BN * rowb) >> 4;
-    c.sub_u = (uint32_t)TM_BM * c.rowu;
-    c.a0_u = dlo0 + (slabs0 >> 4);
-    c.a_stage_u = a_stage >> 4;
-    c.b0_u = dlo0 + (btiles0 >> 4);
-    c.b_stage_u = btile_bytes >> 4;
-    c.tmem_base = tmem_base;
-    c.cat = X3 ? p.cat : 0;
-    c.idesc2 = make_idesc_tf32(2 * p.BN);
-    c.sub_cols = (uint32_t)(p.BN * (c.cat ? 2 : 1));
-    c.buf_cols = c.sub_cols * (uint32_t)MS;
-    c.nbuf = p.nbuf;
-    c.bn = (uint32_t)p.BN;
-    c.group = p.group;
-    c.KB = KB;
-    c.SA = p.SA;
-    c.SB = p.SB;
-    c.nslab = sps;
-    c.bar_a = smem_u32(X3 ? &ctl->a_split[0] : &ctl->a_full[0]);
-    c.bar_a_empty = smem_u32(&ctl->a_empty[0]);
-    c.bar_b_full = smem_u32(&ctl->b_full[0]);
-    c.bar_b_empty = smem_u32(&ctl->b_empty[0]);
-    c.bar_p_full = smem_u32(&ctl->p_full[0]);
-    c.bar_p_empty = smem_u32(&ctl->p_empty[0]);
-    c.cluster = p.cluster;
-    c.cmask = cmask;
-    c.tap_u[0] = c.rowu;                                   // step between taps of one kernel row
-    c.tap_u[1] = (uint32_t)(p.Wt - 2) * c.rowu;            // step from the last tap of a kernel row to the next row
-    const int issuer = warp - 2;
-    c.sub0_a = DUAL ? (uint32_t)issuer * c.sub_u : 0u;
-    c.sub0_d = DUAL ? (uint32_t)issuer * c.sub_cols : 0u;
-    // (taps, K slices) are chosen ONCE, outside the tile loop: each combination owns its copy of the loop, so the
-    // register allocation of the hot path is not shared between variants
-    const IssueTiles tl{(int)cluster_id, (int)num_clusters, (int)tph, (int)total_tiles, n_tiles, rank, KS_SPLIT};
-    if (p.k == 3) {
-      if (kslices == 2)
-        issue_all_tiles<X3, MS, 9, 2, DUAL>(p, c, tl, issuer);
-      else
-        issue_all_tiles<X3, MS, 9, 4, DUAL>(p, c, tl, issuer);
-    } else {
-      if (kslices == 2)
-        issue_all_tiles<X3, MS, 1, 2, DUAL>(p, c, tl, issuer);
-      else
-        issue_all_tiles<X3, MS, 1, 4, DUAL>(p, c, tl, issuer);
-    }
-  } else if (X3 && FUSE) {
-    // ===================== warp 3: 1x1 weights + 3x3 bias of every tile -> shared memory (x3 fused heads) =====================
-    if (lane == 0) {
-      uint32_t phase = 0;
-      for (long long it = 0, tile = tile_at(0); tile < total_tiles; tile = tile_at(++it)) {
-        const int n_tile = (int)(tile % n_tiles);
-        const int head = n_tile / p.tph, part = n_tile - head * p.tph;
-        mbar_wait(smem_u32(&ctl->w2_empty), phase ^ 1u);
-        const uint32_t bar = smem_u32(&ctl->w2_full);
-        mbar_arrive_expect_tx(bar, TM_W2_BUF);
-        bulk_g2s(w2buf, p.fuse_w[head] + (size_t)part * 128 * 16, TM_W2_BYTES, bar);
-        bulk_g2s(w2buf + TM_W2_BYTES, p.bias + (size_t)n_tile * 128, 128u * 4u, bar);
-        phase ^= 1u;
-      }
-    }
-    __syncwarp();
-  }
   } else if (X3 && warp >= 12) {
     asm volatile("setmaxnreg.dec.sync.aligned.u32 48;");
     // ===================== hi / lo splitters (x3): slab -> tf32-exact hi (in place) + lo slab =====================
@@ -596,21 +276,15 @@ __global__ void __launch_bounds__(X3 ? TM_THREADS_X3 : TM_THREADS, 1) conv_tma_k
         }
       }
     }
-  } else if (warp >= 4 && warp < 4 + 4 * MS) {
-    if (X3) {
-      if (FUSE)
-        asm volatile("setmaxnreg.inc.sync.aligned.u32 192;");
-      else
-        asm volatile("setmaxnreg.inc.sync.aligned.u32 192;");
-    }
-    // ===================== epilogue: TMEM lane == flattened output position =====================
-    const int q = warp & 3;                       // TMEM lane quadrant this warp may read
-    const int sub = (warp - 4) >> 2;              // M sub-tile (x3 only: 0 / 1)
-    const int i = sub * TM_BM + q * 32 + lane;    // position inside the tile
-    const uint32_t sub_cols = (uint32_t)(p.BN * (cat ? 2 : 1));      // TMEM columns of one sub-tile of one buffer
-    const uint32_t buf_cols = sub_cols * (uint32_t)MS;
-    const uint32_t lane_base = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)sub * sub_cols;
-    float* stage = nullptr;                       // (the direct store path needs no scratch)
+  } else {
+    if (X3) asm volatile("setmaxnreg.inc.sync.aligned.u32 208;");
+    // ===================== consumers: warpgroup c multiplies rows [64 c, 64 c + 64) of every tile =====================
+    const int c = (warp - 4) >> 2, wt = tid & 127;
+    float* dstage = reinterpret_cast<float*>(smem + (drain0 - smem_u32(smem))) + (size_t)c * (DRAIN_STAGE_BYTES / 4);
+    const uint32_t bar_a = smem_u32(X3 ? &ctl->a_split[0] : &ctl->a_full[0]);
+    const uint32_t bar_a_empty = smem_u32(&ctl->a_empty[0]);
+    const uint32_t bar_b_full = smem_u32(&ctl->b_full[0]), bar_b_empty = smem_u32(&ctl->b_empty[0]);
+    const uint32_t a_lo_u = p.slab_stride >> 4, b_lo_u = ((uint32_t)BN * rowb) >> 4;
     EpiParams ep;
     ep.bias = p.bias;
     ep.residual = p.residual;
@@ -625,214 +299,121 @@ __global__ void __launch_bounds__(X3 ? TM_THREADS_X3 : TM_THREADS, 1) conv_tma_k
     ep.CoutPad = p.CoutPad;
     ep.H = p.H;
     ep.W = p.W;
-    int buf = 0;
-    uint32_t pf = 0;                     // bit b: phase of p_full[b]
-    uint32_t w2_phase = 0;               // x3 fused heads: phase of w2_full
-    float acc2[FUSE ? 16 : 1];           // fused 1x1: the 16 (padded) outputs of this position's head
+    int sa = 0, sb = 0;
+    uint32_t pa = 0, pb = 0;
+    float acc[BN / 2];
+    float sums[X3 ? BN / 2 : 1];
+    float acc2[FUSE ? 16 : 1];           // fused 1x1: partial outputs (this thread's half of the hidden channels) of its row
+#pragma unroll
+    for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
 #pragma unroll
     for (int j = 0; j < (FUSE ? 16 : 1); ++j) acc2[j] = 0.f;
     for (long long it = 0, tile = tile_at(0); tile < total_tiles; tile = tile_at(++it)) {
-      bool live;
-      const TileGeo g = decode_tile(p, tile / KS_SPLIT, n_tiles, rank, &live);
-      bool valid;
-      int n, oy, ox;
-      if (p.k == 3) {
-        const int gg = g.g0 + i;
-        oy = gg / p.Wt;
-        const int xp = gg - oy * p.Wt;
-        ox = xp - 1;
-        n = g.img;
-        valid = live && (oy < p.H) && (xp >= 1) && (xp <= p.W);
-      } else {
-        const long long pix = g.pos0 + i;
-        valid = live && pix < (long long)p.B * p.H * p.W;
-        const long long pp = valid ? pix : 0;
-        ox = (int)(pp % p.W);
-        const long long t = pp / p.W;
-        oy = (int)(t % p.H);
-        n = (int)(t / p.H);
-      }
-      const int m = (int)(((size_t)n * p.H + oy) * p.W + ox);
-      const int col_end = min(p.Cout, (g.n_tile + 1) * p.BN);
-      if (X3) {
-        // two-level accumulation: the tensor core only ever sums `group` K blocks in TMEM (its accumulator truncates,
-        // error ~ chain length); every finished group is added into fp32 registers with round-to-nearest
-        float sums[X3 ? 128 : 1];
+      const TileGeo g = decode_tile(p, tile / KS_SPLIT, n_tiles);
+      // A row of tap (ky, kx) for tile row 64 c: start of the slab + (g0 - 1 - r_lo Wt) + ky Wt + kx + 64 c
+      const uint32_t row0 = (p.k == 3 ? (uint32_t)(g.g0 - 1 - g.r_lo * p.Wt) : 0u) + (uint32_t)c * 64u;
 #pragma unroll
-        for (int j = 0; j < (X3 ? 128 : 1); ++j) sums[j] = 0.f;
-        const int ngroups = (KB + p.group - 1) / p.group;
-        for (int gi = 0; gi < ngroups; ++gi) {
-          mbar_wait(smem_u32(&ctl->p_full[buf]), (pf >> buf) & 1u);
-          tc_fence_after();
-          // 32 columns per tcgen05.ld: with one accumulation group = 12 MMAs the drain of a TMEM buffer has to finish inside
-          // the ~1500 clk the tensor pipe needs for the next group, and every ld + wait round trip costs ~150 clk
-          if (cat) {
-            // main half [0, BN): promoted and zeroed every group; cross half [BN, 2 BN): only when this is the last group
-            // of the tile that uses this buffer (the last nbuf groups touch every buffer once)
-            const int halves = (gi >= ngroups - p.nbuf) ? 2 : 1;
-            for (int hf = 0; hf < halves; ++hf) {
+      for (int j = 0; j < (X3 ? BN / 2 : 1); ++j) sums[j] = 0.f;
+      int kbi = 0, gk = 0;
+      for (int s = 0; s < sps; ++s) {
+        mbar_wait(bar_a + 8u * (uint32_t)sa, pa);
+        const uint32_t a_slab = slabs0 + (uint32_t)sa * a_stage;
+        for (int tap = 0; tap < taps; ++tap, ++kbi) {
+          const int ky = tap / 3, kx = tap - ky * 3;
+          const uint32_t arow = row0 + (p.k == 3 ? (uint32_t)(ky * p.Wt + kx) : 0u);
+          mbar_wait(bar_b_full + 8u * (uint32_t)sb, pb);
+          const uint64_t da = make_desc(a_slab + arow * rowb, p.cslab);
+          const uint64_t db = make_desc(btiles0 + (uint32_t)sb * btile_bytes, p.cslab);
+          const bool fresh = X3 ? gk == 0 : kbi == 0;
+          if (p.cslab == 32)
+            mma_kblock<BN, X3, false, 4>(acc, da, db, a_lo_u, b_lo_u, fresh);
+          else
+            mma_kblock<BN, X3, false, 2>(acc, da, db, a_lo_u, b_lo_u, fresh);
+          if (wt == 0) {
+            mbar_arrive(bar_b_empty + 8u * (uint32_t)sb);
+            if (tap == taps - 1) mbar_arrive(bar_a_empty + 8u * (uint32_t)sa);
+          }
+          if (++sb == p.SB) {
+            sb = 0;
+            pb ^= 1u;
+          }
+          if (X3) {
+            // two-level accumulation: the tensor core sums `group` K blocks, every finished group is added into fp32
+            // registers with round-to-nearest
+            if (gk == p.group - 1 || kbi == KB - 1) {
 #pragma unroll
-              for (int c = 0; c < 2; ++c) {
-                if (c * 32 < p.BN) {
-                  const uint32_t ta = lane_base + (uint32_t)buf * buf_cols + (uint32_t)(hf * p.BN + c * 32);
-                  uint32_t rr[32], z[32];
-#pragma unroll
-                  for (int j = 0; j < 32; ++j) z[j] = 0u;
-                  if (c * 32 + 16 < p.BN) {
-                    tmem_ld32(ta, rr);
-                    tmem_ld_wait();
-                    tmem_st32(ta, z);
-                  } else {
-                    tmem_ld16(ta, rr);
-#pragma unroll
-                    for (int j = 16; j < 32; ++j) rr[j] = 0u;
-                    tmem_ld_wait();
-                    tmem_st16(ta, z);
-                  }
-#pragma unroll
-                  for (int j = 0; j < 32; ++j) sums[(X3 ? c * 32 + j : 0)] += __uint_as_float(rr[j]);
-                }
-              }
-            }
-            tmem_st_wait();
-          } else {
-#pragma unroll
-          for (int c = 0; c < 4; ++c) {
-            if (c * 32 < p.BN) {
-              uint32_t rr[32];
-              if (c * 32 + 16 < p.BN) {
-                tmem_ld32(lane_base + (uint32_t)(buf * p.BN * MS + c * 32), rr);
-              } else {
-                tmem_ld16(lane_base + (uint32_t)(buf * p.BN * MS + c * 32), rr);
-#pragma unroll
-                for (int j = 16; j < 32; ++j) rr[j] = 0u;
-              }
-              tmem_ld_wait();
-#pragma unroll
-              for (int j = 0; j < 32; ++j) sums[(X3 ? c * 32 + j : 0)] += __uint_as_float(rr[j]);
+              for (int j = 0; j < (X3 ? BN / 2 : 1); ++j) sums[j] += acc[X3 ? j : 0];
+              gk = 0;
+            } else {
+              ++gk;
             }
           }
-          }
-          tc_fence_before();
-          mbar_arrive(smem_u32(&ctl->p_empty[buf]));
-          pf ^= 1u << buf;
-          if (++buf == p.nbuf) buf = 0;
         }
+        if (++sa == p.SA) {
+          sa = 0;
+          pa ^= 1u;
+        }
+      }
+      // ---- epilogue: rows of this warpgroup, 32 columns at a time through shared memory (drain_rows)
+      const int r_me = wt >> 1;
+      int n, oy, ox, m;
+      const bool valid = tile_position(p, g, c * 64 + r_me, &n, &oy, &ox, &m);
+      const int col_end = min(p.Cout, (g.n_tile + 1) * BN);
+      const int head = FUSE ? g.n_tile / p.tph : 0, part = FUSE ? g.n_tile - head * p.tph : 0;
+      if (FUSE && part == 0) {
+#pragma unroll
+        for (int j = 0; j < (FUSE ? 16 : 1); ++j) acc2[j] = 0.f;
+      }
+      auto fn = [&](int r, int cb, float (&v)[16]) {
+        if (cb >= BN) return;
         if (!FUSE && KS_SPLIT > 1) {
-          // split-K: park the partial sums of this K range, [mn tile][split][float4 column group][row] so that the 32
-          // lanes of a warp (32 consecutive rows) write one 512 B run; conv_tma_splitk_finish adds the ranges in split
-          // order (a fixed summation order) and runs the epilogue
+          // split-K: park the partial sums of this K range, [mn tile][split][float4 column group][row];
+          // conv_tma_splitk_finish adds the ranges in split order (a fixed summation order) and runs the epilogue
           const long long mn = tile / KS_SPLIT;
           const int ks = (int)(tile % KS_SPLIT);
-          const int G = p.BN >> 2;
-          float4* mine = reinterpret_cast<float4*>(p.part) + ((size_t)mn * KS_SPLIT + ks) * G * p.tile_m + i;
+          float4* mine = reinterpret_cast<float4*>(p.part) + (((size_t)mn * KS_SPLIT + ks) * (BN >> 2) + (cb >> 2)) * p.tile_m +
+                         c * 64 + r;
 #pragma unroll
-          for (int c = 0; c < 32; ++c)
-            if (c < G)
-              __stcg(mine + (size_t)c * p.tile_m, make_float4(sums[(X3 ? c * 4 : 0)], sums[(X3 ? c * 4 + 1 : 0)],
-                                                              sums[(X3 ? c * 4 + 2 : 0)], sums[(X3 ? c * 4 + 3 : 0)]));
-          continue;
-        }
-        if (FUSE) {
-          // hidden = relu(conv3x3 + bias) never leaves the SM: multiply it with this head's 1x1 weights right here.
-          // The [128][16] weight block + the 128 biases of this (head, part) were staged in shared memory by warp 3;
-          // only the float4 groups that hold real output channels are read.
-          const int head = g.n_tile / p.tph, part = g.n_tile - head * p.tph;
-          if (part == 0) {
+          for (int q = 0; q < 4; ++q) __stcg(mine + (size_t)q * p.tile_m, make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]));
+        } else if (FUSE) {
+          // hidden = relu(conv3x3 + bias) never leaves the SM: multiply it with this head's 1x1 weights right here
+          const float* b1 = p.bias + (size_t)g.n_tile * BN + cb;
+          const float4* w2 = reinterpret_cast<const float4*>(p.fuse_w[head]) + ((size_t)part * BN + cb) * 4;
 #pragma unroll
-            for (int j = 0; j < (FUSE ? 16 : 1); ++j) acc2[j] = 0.f;
+          for (int q = 0; q < 16; ++q) {
+            const float h = fmaxf(v[q] + __ldg(b1 + q), 0.f);
+#pragma unroll
+            for (int u = 0; u < 4; ++u) {
+              const float4 w = __ldg(w2 + q * 4 + u);
+              acc2[FUSE ? 4 * u + 0 : 0] = fmaf(h, w.x, acc2[FUSE ? 4 * u + 0 : 0]);
+              acc2[FUSE ? 4 * u + 1 : 0] = fmaf(h, w.y, acc2[FUSE ? 4 * u + 1 : 0]);
+              acc2[FUSE ? 4 * u + 2 : 0] = fmaf(h, w.z, acc2[FUSE ? 4 * u + 2 : 0]);
+              acc2[FUSE ? 4 * u + 3 : 0] = fmaf(h, w.w, acc2[FUSE ? 4 * u + 3 : 0]);
+            }
           }
-          if constexpr (X3 && FUSE) {
-            mbar_wait(smem_u32(&ctl->w2_full), w2_phase);
-            w2_phase ^= 1u;
-            const int co = p.fuse_cout[head];
-            if (co <= 4)
-              fused_part_smem<1>(sums, acc2, w2buf, w2buf + TM_W2_BYTES);
-            else if (co <= 8)
-              fused_part_smem<2>(sums, acc2, w2buf, w2buf + TM_W2_BYTES);
-            else
-              fused_part_smem<4>(sums, acc2, w2buf, w2buf + TM_W2_BYTES);
-            __syncwarp();
-            if (lane == 0) mbar_arrive(smem_u32(&ctl->w2_empty));
-          }
-          if (part == p.tph - 1 && valid) fused_store(p, head, acc2, n, oy, ox);
         } else {
-#pragma unroll
-          for (int cc = 0; cc < 4; ++cc) {
-            const int c0 = cc * 32;
-            if (c0 < p.BN) {
-              float vv[32];
-#pragma unroll
-              for (int j = 0; j < 32; ++j) vv[j] = sums[(X3 ? cc * 32 + j : 0)];
-              epilogue_sub_tile(ep, stage, vv, lane, valid, m, n, oy, ox, g.n_tile * p.BN + c0, col_end);
-            }
-          }
+          epilogue_row<16>(ep, v, valid, m, n, oy, ox, g.n_tile * BN + cb, col_end);
         }
-      } else {
-        mbar_wait(smem_u32(&ctl->p_full[buf]), (pf >> buf) & 1u);
-        tc_fence_after();
-        for (int c0 = 0; c0 < p.BN; c0 += 32) {
-          uint32_t rr[32];
-          tmem_ld16(lane_base + (uint32_t)(buf * p.BN + c0), rr);
-          if (c0 + 16 < p.BN) {
-            tmem_ld16(lane_base + (uint32_t)(buf * p.BN + c0 + 16), rr + 16);
-          } else {
+      };
+      if constexpr (X3)
+        drain_rows<BN>(sums, dstage, wt, 1 + c, fn);
+      else
+        drain_rows<BN>(acc, dstage, wt, 1 + c, fn);
+      if (FUSE && part == p.tph - 1) {
+        // the two threads of a row (lanes 2 r, 2 r + 1) each hold half of the hidden channels
 #pragma unroll
-            for (int j = 16; j < 32; ++j) rr[j] = 0u;
-          }
-          tmem_ld_wait();
-          if (c0 + 32 >= p.BN) {          // last chunk read: hand the TMEM buffer back before the (slow) global stores
-            tc_fence_before();
-            mbar_arrive(smem_u32(&ctl->p_empty[buf]));
-          }
-          float vv[32];
+        for (int j = 0; j < (FUSE ? 16 : 1); ++j) acc2[j] += __shfl_xor_sync(0xffffffffu, acc2[j], 1);
+        if ((wt & 1) == 0 && valid) {
+          const int co = p.fuse_cout[head];
+          float* o = p.fuse_out[head] + ((size_t)n * co * p.H + oy) * p.W + ox;
+          const size_t plane = (size_t)p.H * p.W;
 #pragma unroll
-          for (int j = 0; j < 32; ++j) vv[j] = __uint_as_float(rr[j]);
-          if (FUSE) {
-            const int head = g.n_tile / p.tph, part = g.n_tile - head * p.tph;
-            if (part == 0 && c0 == 0) {
-#pragma unroll
-              for (int j = 0; j < (FUSE ? 16 : 1); ++j) acc2[j] = 0.f;
-            }
-            const float* b1 = p.bias + (size_t)g.n_tile * p.BN + c0;
-            const float4* w2 = reinterpret_cast<const float4*>(p.fuse_w[head]) + ((size_t)part * p.BN + c0) * 4;
-#pragma unroll
-            for (int c = 0; c < 32; ++c) {
-              const float v = fmaxf(vv[c] + __ldg(b1 + c), 0.f);
-              const float4 wa = __ldg(w2 + c * 4), wb = __ldg(w2 + c * 4 + 1), wc = __ldg(w2 + c * 4 + 2),
-                           wd = __ldg(w2 + c * 4 + 3);
-              acc2[FUSE ? 0 : 0] = fmaf(v, wa.x, acc2[FUSE ? 0 : 0]);
-              acc2[FUSE ? 1 : 0] = fmaf(v, wa.y, acc2[FUSE ? 1 : 0]);
-              acc2[FUSE ? 2 : 0] = fmaf(v, wa.z, acc2[FUSE ? 2 : 0]);
-              acc2[FUSE ? 3 : 0] = fmaf(v, wa.w, acc2[FUSE ? 3 : 0]);
-              acc2[FUSE ? 4 : 0] = fmaf(v, wb.x, acc2[FUSE ? 4 : 0]);
-              acc2[FUSE ? 5 : 0] = fmaf(v, wb.y, acc2[FUSE ? 5 : 0]);
-              acc2[FUSE ? 6 : 0] = fmaf(v, wb.z, acc2[FUSE ? 6 : 0]);
-              acc2[FUSE ? 7 : 0] = fmaf(v, wb.w, acc2[FUSE ? 7 : 0]);
-              acc2[FUSE ? 8 : 0] = fmaf(v, wc.x, acc2[FUSE ? 8 : 0]);
-              acc2[FUSE ? 9 : 0] = fmaf(v, wc.y, acc2[FUSE ? 9 : 0]);
-              acc2[FUSE ? 10 : 0] = fmaf(v, wc.z, acc2[FUSE ? 10 : 0]);
-              acc2[FUSE ? 11 : 0] = fmaf(v, wc.w, acc2[FUSE ? 11 : 0]);
-              acc2[FUSE ? 12 : 0] = fmaf(v, wd.x, acc2[FUSE ? 12 : 0]);
-              acc2[FUSE ? 13 : 0] = fmaf(v, wd.y, acc2[FUSE ? 13 : 0]);
-              acc2[FUSE ? 14 : 0] = fmaf(v, wd.z, acc2[FUSE ? 14 : 0]);
-              acc2[FUSE ? 15 : 0] = fmaf(v, wd.w, acc2[FUSE ? 15 : 0]);
-            }
-            if (part == p.tph - 1 && c0 + 32 >= p.BN && valid) fused_store(p, head, acc2, n, oy, ox);
-          } else {
-            epilogue_sub_tile(ep, stage, vv, lane, valid, m, n, oy, ox, g.n_tile * p.BN + c0, col_end);
-          }
+          for (int j = 0; j < 16; ++j)
+            if (j < co) o[j * plane] = acc2[FUSE ? j : 0] + __ldg(p.fuse_b[head] + j);
         }
-        pf ^= 1u << buf;
-        if (++buf == p.nbuf) buf = 0;
       }
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (p.cluster > 1) cluster_sync_all();       // nobody leaves while a peer may still multicast into / arrive on its smem
-  if (warp == 2) tmem_dealloc(tmem_base, tmem_cols);
 }
 
 // weight tiles for the slab-major K order:  kb = slab * taps + tap,  element j of the row = channel slab*32 + j
@@ -914,26 +495,9 @@ __global__ void __launch_bounds__(256) conv_tma_splitk_finish(const __grid_const
     a.z += v.z;
     a.w += v.w;
   }
-  bool live;
-  const TileGeo g = decode_tile(p, mn, p.CoutPad / p.BN, 0, &live);
-  bool valid;
-  int n, oy, ox;
-  if (p.k == 3) {
-    const int gg = g.g0 + i;
-    oy = gg / p.Wt;
-    const int xp = gg - oy * p.Wt;
-    ox = xp - 1;
-    n = g.img;
-    valid = live && (oy < p.H) && (xp >= 1) && (xp <= p.W);
-  } else {
-    const long long pix = g.pos0 + i;
-    valid = live && pix < (long long)p.B * p.H * p.W;
-    const long long pp = valid ? pix : 0;
-    ox = (int)(pp % p.W);
-    const long long t = pp / p.W;
-    oy = (int)(t % p.H);
-    n = (int)(t / p.H);
-  }
+  const TileGeo g = decode_tile(p, mn, p.CoutPad / p.BN);
+  int n, oy, ox, mi;
+  const bool valid = tile_position(p, g, i, &n, &oy, &ox, &mi);
   if (!valid) return;
   const size_t m = ((size_t)n * p.H + oy) * p.W + ox;
   const int col0 = g.n_tile * p.BN + c4 * 4;
@@ -967,14 +531,16 @@ __global__ void __launch_bounds__(256) conv_tma_splitk_finish(const __grid_const
 // ---------------------------------------------------------------------------------------------------- host side
 // Channels per activation slab.  32 (128-byte rows) by default; 16 (64-byte rows, SWIZZLE_64B) when Cin is not a
 // multiple of 32, or when the 3-term split (hi + lo slabs) could not be double-buffered with 32-channel slabs.
-static int tma_tile_m(int x3) { return x3 ? 256 : TM_BM; }
+static int tma_tile_m(int) { return TM_BM; }
 static int tma_boxh(int Wt, int x3) { return (tma_tile_m(x3) + 1 + 2 * Wt + Wt - 1) / Wt + 1; }
 
-// Stage counts of the slab ring (SA) and the weight-tile ring (SB) inside the 227 KB of dynamic shared memory
-// (512 B control block + up to 1024 B alignment + 1536 B slack are reserved).
-static int tma_smem_layout(uint32_t a_stage, uint32_t btile, int k, bool fuse_x3, int* SA, int* SB, size_t* smem) {
-  const size_t extra = fuse_x3 ? TM_W2_BUF : 0;
-  const size_t budget = 222 * 1024 - (fuse_x3 ? 6 * 1024 : 0);      // fused x3: 227 KB - 2.5 KB control - 8.5 KB weights
+// Shared memory for the slab and weight-tile rings: 227 KB less the control block, alignment, slack and the two
+// epilogue staging buffers.
+constexpr size_t TM_BUDGET = 222 * 1024 - 2 * (size_t)DRAIN_STAGE_BYTES;
+
+// Stage counts of the slab ring (SA) and the weight-tile ring (SB).
+static int tma_smem_layout(uint32_t a_stage, uint32_t btile, int k, int* SA, int* SB, size_t* smem) {
+  const size_t budget = TM_BUDGET;
   int sa = 2;
   if ((size_t)sa * a_stage + 2 * (size_t)btile > budget) sa = 1;
   if ((size_t)sa * a_stage + 2 * (size_t)btile > budget) return fail(CP_ERR_INVALID, "conv_tma: slab does not fit shared memory");
@@ -989,7 +555,7 @@ static int tma_smem_layout(uint32_t a_stage, uint32_t btile, int k, bool fuse_x3
   }
   *SA = sa;
   *SB = sb;
-  *smem = 512 + 2048 + (size_t)sa * a_stage + (size_t)sb * btile + extra;
+  *smem = 512 + 2048 + (size_t)sa * a_stage + (size_t)sb * btile + 2 * (size_t)DRAIN_STAGE_BYTES;
   return CP_OK;
 }
 
@@ -999,15 +565,14 @@ int tma_cslab(const IgemmParams& p, int x3) {
   const int Wt = p.Win + 2;
   const int boxh = tma_boxh(Wt, x3);
   const size_t slab32 = ((size_t)boxh * Wt * 128 + 1023) / 1024 * 1024;
-  const int bn = p.CoutPad <= 128 ? p.CoutPad : 128;
+  const int bn = tma_tile_n(p.CoutPad, x3);
   const size_t need = 2 * (2 * slab32) + 2 * ((size_t)bn * 128 * 2);
-  return need > (size_t)222 * 1024 ? 16 : 32;
+  return need > TM_BUDGET ? 16 : 32;
 }
 
-int tma_tile_n(int CoutPad, int x3) {
-  const int cap = x3 ? 128 : 256;     // x3 keeps the promoted sums of one row in 128 registers
-  return CoutPad <= cap ? CoutPad : cap;
-}
+// wgmma N of the consumer warpgroups: the accumulator takes BN / 2 registers per thread (x3: twice that with the sums);
+// N = 256 would spill
+int tma_tile_n(int CoutPad, int) { return wgmma_tile_n(CoutPad, 128); }
 
 bool tma_conv_supported(const IgemmParams& p, int x3) {
   if (p.mode != IGEMM_NHWC_VEC) return false;
@@ -1019,12 +584,12 @@ bool tma_conv_supported(const IgemmParams& p, int x3) {
     if (p.srcC[s] % cs || p.srcStride[s] % 4) return false;
   if (p.kh == 3 && p.Win + 2 > 256) return false;
   const int bn = tma_tile_n(p.CoutPad, x3);
-  if (bn % 16 || p.CoutPad % bn) return false;
+  if (bn == 0) return false;
   // one single-buffered slab stage (+ its lo copy in x3) and two weight tiles must fit shared memory
   const size_t slab = p.kh == 3 ? (size_t)tma_boxh(p.Win + 2, x3) * (p.Win + 2) * cs * 4 : (size_t)tma_tile_m(x3) * cs * 4;
   const size_t a_stage = ((slab + 1023) / 1024 * 1024) * (x3 ? 2 : 1);
   const size_t btile = (size_t)bn * cs * 4 * (x3 ? 2 : 1);
-  if (a_stage + 2 * btile > (size_t)222 * 1024) return false;
+  if (a_stage + 2 * btile > TM_BUDGET) return false;
   return get_encode() != nullptr;
 }
 
@@ -1039,7 +604,7 @@ int launch_pack_tma_weight(const float* src, int ld, int Cin, int taps, int Cout
   const int nt = CoutPad / bn;
   size_t total = (size_t)nt * (Cin / cs) * taps * bn * (cs / 4);
   int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 32) blocks = 148 * 32;
+  if (blocks > 132 * 32) blocks = 132 * 32;
   pack_tma_weight_kernel<<<blocks, 256, 0, s>>>(src, ld, Cin, taps, Cout, bn, nt, round_tf32, x3, cs, (unsigned char*)dst);
   CP_LAUNCH_CHECK("pack_tma_weight_kernel");
   return CP_OK;
@@ -1096,9 +661,31 @@ int tma_conv_encode(const IgemmParams& p, int Bmax, int x3, void* maps_out) {
   return CP_OK;
 }
 
-static int num_sms_hint() {
-  int n = 0;
-  return device_sm_count(&n) == CP_OK ? n : 148;
+template <bool X3, bool FUSE>
+static int launch_conv_tma_kernel(const TmaConvParams& q, const cudaLaunchConfig_t& cfg0) {
+  void (*kern)(TmaConvParams) = nullptr;
+  switch (q.BN) {
+    case 16: kern = conv_tma_kernel<X3, FUSE, 16>; break;
+    case 32: kern = conv_tma_kernel<X3, FUSE, 32>; break;
+    case 64: kern = conv_tma_kernel<X3, FUSE, 64>; break;
+    case 128: kern = conv_tma_kernel<X3, FUSE, 128>; break;
+    default: return fail(CP_ERR_INVALID, "conv_tma: unsupported N tile");
+  }
+  static PerDevice<bool, 4> configured;
+  const int slot = q.BN == 128 ? 3 : (q.BN == 64 ? 2 : (q.BN == 32 ? 1 : 0));
+  if (!configured.here(slot)) {
+    CP_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    configured.here(slot) = true;
+  }
+  cudaLaunchConfig_t cfg = cfg0;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = 1;
+  cfg.attrs = attr;
+  cfg.numAttrs = g_pdl ? 1 : 0;
+  CP_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, q));
+  CP_LAUNCH_CHECK("conv_tma_kernel");
+  return CP_OK;
 }
 
 int launch_conv_tma(const IgemmParams& p, const void* maps, int round_out_tf32, int x3, cudaStream_t stream) {
@@ -1115,25 +702,10 @@ int launch_conv_tma(const IgemmParams& p, const void* maps, int round_out_tf32, 
   q.Cout = p.Cout;
   q.CoutPad = p.CoutPad;
   q.BN = tma_tile_n(p.CoutPad, x3);
+  if (q.BN == 0) return fail(CP_ERR_INVALID, "conv_tma: unsupported output width");
   q.x3 = x3;
   q.cslab = tma_cslab(p, x3);
-  q.group = x3_group_blocks() * (32 / q.cslab);       // same number of MMAs per TMEM accumulation group
-  // x3 hands a buffer to the promoting warps every accumulation group; narrow N tiles leave TMEM columns for more than two
-  // buffers in flight, which hides the commit -> mbarrier -> tcgen05.ld -> arrive round trip (dcn_tma.cu has the numbers)
-  q.nbuf = 2;
-  if (x3) {
-    q.nbuf = 512 / (q.BN * 2);
-    if (q.nbuf > 8) q.nbuf = 8;
-    if (q.nbuf < 2) q.nbuf = 2;
-  }
-  // x3, N tile <= 64 and no fused 1x1: hi | lo weight tiles as one 2 BN-row operand (issue_tile); a buffer is then 2 BN
-  // columns per sub-tile
-  q.cat = (x3 && q.BN <= 64 && p.fuse_n == 0 && !getenv("CP_NO_CAT")) ? 1 : 0;
-  if (q.cat) {
-    q.nbuf = 512 / (q.BN * 4);
-    if (q.nbuf > 8) q.nbuf = 8;
-  }
-  if (const char* e = getenv("CP_TMA_NBUF")) q.nbuf = atoi(e) >= 2 && atoi(e) <= q.nbuf ? atoi(e) : q.nbuf;
+  q.group = x3_group_blocks() * (32 / q.cslab);       // same number of MMAs per accumulation group
   q.k = p.kh;
   q.Wt = p.Win + 2;
   q.tile_m = tma_tile_m(x3);
@@ -1151,9 +723,8 @@ int launch_conv_tma(const IgemmParams& p, const void* maps, int round_out_tf32, 
   q.slab_stride = (q.slab_bytes + 1023u) & ~1023u;
   const uint32_t btile = (uint32_t)q.BN * (uint32_t)q.cslab * 4u * (x3 ? 2u : 1u);
   const uint32_t a_stage = q.slab_stride * (x3 ? 2u : 1u);
-  const bool fuse_x3 = x3 && p.fuse_n > 0;        // + the staged 1x1 weights / 3x3 bias of the current tile
   size_t smem = 0;
-  if (int rc = tma_smem_layout(a_stage, btile, q.k, fuse_x3, &q.SA, &q.SB, &smem)) return rc;
+  if (int rc = tma_smem_layout(a_stage, btile, q.k, &q.SA, &q.SB, &smem)) return rc;
   q.bias = p.bias;
   q.residual = p.residual;
   q.resStride = p.resStride;
@@ -1176,36 +747,22 @@ int launch_conv_tma(const IgemmParams& p, const void* maps, int round_out_tf32, 
       q.fuse_cout[h] = p.fuse_cout[h];
     }
   }
-  void (*kern)(TmaConvParams) = x3 ? (q.fuse ? conv_tma_kernel<true, true> : conv_tma_kernel<true, false>)
-                                   : (q.fuse ? conv_tma_kernel<false, true> : conv_tma_kernel<false, false>);
-  static PerDevice<bool, 4> configured;
-  const int slot = (x3 ? 2 : 0) + (q.fuse ? 1 : 0);
-  if (!configured.here(slot)) {
-    CP_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    configured.here(slot) = true;
-  }
   q.m_tiles = (long long)m_tiles;
   q.ksplit = 1;
   q.sps = q.Cin / q.cslab;
   q.part = p.splitk_ws;
-  int cluster = 1;     // measured: multicast at cluster sizes 2/4 does not cut L2 traffic on this part and couples the CTAs
-  if (const char* e = getenv("CP_TMA_CLUSTER")) cluster = atoi(e);
-  if (cluster != 1 && cluster != 2 && cluster != 4) cluster = 1;
-  while (cluster > 1 && ((long long)m_tiles < cluster || (btile / cluster) % 16)) cluster >>= 1;
-  q.cluster = cluster;
-  const long long m_groups = ((long long)m_tiles + cluster - 1) / cluster;
-  q.total_tiles = m_groups * (p.CoutPad / q.BN);
+  q.total_tiles = (long long)m_tiles * (p.CoutPad / q.BN);
+  int num_sms = 0;
+  if (int rc = device_sm_count(&num_sms)) return rc;
   // split-K (tf32x3, plain epilogue): small feature maps give a persistent kernel fewer tiles than SMs while every tile
-  // walks a long serial K loop (level5 at batch 1: 8 tiles x 144 K blocks).  Deal slab-aligned K ranges to more CTAs.
+  // walks a long serial K loop (level5 at batch 1: 16 tiles x 144 K blocks).  Deal slab-aligned K ranges to more CTAs.
   const char* ks_off = getenv("CP_NO_SPLITK");        // "1": no split-K anywhere, "conv": not here, "dcn": not in dcn_tma
-  if (x3 && !q.fuse && cluster == 1 && p.splitk_ws && !(ks_off && (ks_off[0] == '1' || ks_off[0] == 'c'))) {
+  if (x3 && !q.fuse && p.splitk_ws && !(ks_off && (ks_off[0] == '1' || ks_off[0] == 'c'))) {
     const int nslab = q.Cin / q.cslab;
     const long long mn = q.total_tiles;
     int S = 1;
     for (int cand = 2; cand <= nslab; ++cand)
-      if (nslab % cand == 0 && mn * cand <= num_sms_hint() &&
-          (size_t)mn * cand * q.tile_m * q.BN <= p.splitk_ws_floats)
-        S = cand;
+      if (nslab % cand == 0 && mn * cand <= num_sms && (size_t)mn * cand * q.tile_m * q.BN <= p.splitk_ws_floats) S = cand;
     if (S > 1) {
       q.ksplit = S;
       q.sps = nslab / S;
@@ -1213,26 +770,14 @@ int launch_conv_tma(const IgemmParams& p, const void* maps, int round_out_tf32, 
     }
   }
   if (q.total_tiles >= (1ll << 31)) return fail(CP_ERR_INVALID, "conv_tma: too many tiles");
-  int num_sms = 0;
-  if (int rc = device_sm_count(&num_sms)) return rc;
-  long long nclusters = num_sms / cluster;
-  if (q.total_tiles < nclusters) nclusters = q.total_tiles;
   cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)(nclusters * cluster));
+  cfg.gridDim = dim3((unsigned)(q.total_tiles < num_sms ? q.total_tiles : num_sms));
   cfg.blockDim = dim3(x3 ? TM_THREADS_X3 : TM_THREADS);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = stream;
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = cluster;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = g_pdl ? 2 : 1;
-  CP_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, q));
-  CP_LAUNCH_CHECK("conv_tma_kernel");
+  int rc = x3 ? (q.fuse ? launch_conv_tma_kernel<true, true>(q, cfg) : launch_conv_tma_kernel<true, false>(q, cfg))
+              : (q.fuse ? launch_conv_tma_kernel<false, true>(q, cfg) : launch_conv_tma_kernel<false, false>(q, cfg));
+  if (rc) return rc;
   if (q.ksplit > 1) {
     const long long mn = q.total_tiles / q.ksplit;
     const long long threads = mn * (q.BN / 4) * q.tile_m;

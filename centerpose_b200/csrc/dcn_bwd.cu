@@ -5,7 +5,7 @@
 //
 // Here the whole batch is one pass over NHWC buffers and the column matrix is touched exactly twice:
 //   1. gcol[m][tap * Cp + c] = sum_o W[o][c][tap] * gout[m][o]      -- a 1x1 convolution Co -> 9 Cp over the output
-//      gradient, run by the forward convolution kernels (cp::run_igemm_dispatch: FFMA or tcgen05, like cp_conv2d)
+//      gradient, run by the forward convolution kernels (cp::run_igemm_dispatch: FFMA or wgmma, like cp_conv2d)
 //   2. dcn_bwd_sample_kernel, one warp per (position, tap), lanes over channels: reads its gcol slice, re-samples the
 //      four bilinear corners of the input, accumulates grad_mask / grad_offset (warp reduction, written NCHW), scatters
 //      grad_input with vector atomics (NHWC) and OVERWRITES the gcol slice with the forward column value
@@ -258,7 +258,7 @@ int dcn_v2_backward_impl(const float* input, const float* weight, const float* o
     {
       const size_t total = n_wp;
       int blocks = (int)((total + 255) / 256);
-      if (blocks > 148 * 8) blocks = 148 * 8;
+      if (blocks > 132 * 8) blocks = 132 * 8;
       dcn_bwd_pack_w_kernel<<<blocks, 256, 0, s>>>(weight, wp, Co, C, CoP, Cp, NPad);
       CP_LAUNCH_CHECK("dcn_bwd_pack_w_kernel");
     }
@@ -283,7 +283,7 @@ int dcn_v2_backward_impl(const float* input, const float* weight, const float* o
     p.out = gcol;
     p.outStride = N;
     p.mode = IGEMM_NHWC_VEC;
-    // shapes the tcgen05 kernels do not take (a few channels) run on the FFMA kernel: same result class, fp32
+    // shapes the tensor-core kernels do not take (a few channels) run on the FFMA kernel: same result class, fp32
     if (prec >= 0) {
       const bool tma_ok = (prec == 1 || prec == 2) && tma_conv_supported(p, prec == 1);
       if (!tma_ok && !umma_supported(p, prec == 2 ? 1 : prec)) prec = -1;
@@ -313,7 +313,7 @@ int dcn_v2_backward_impl(const float* input, const float* weight, const float* o
     {
       const size_t total = (size_t)(N + 1) * Co;
       int blocks = (int)((total + 255) / 256);
-      if (blocks > 148 * 8) blocks = 148 * 8;
+      if (blocks > 132 * 8) blocks = 132 * 8;
       dcn_bwd_wgrad_finish<<<blocks, 256, 0, s>>>(part, S, N, CoP, Cp, C, Co, grad_weight, grad_bias);
       CP_LAUNCH_CHECK("dcn_bwd_wgrad_finish");
     }

@@ -10,7 +10,7 @@ constexpr int TPB = 256;
 
 inline int blocks_for(size_t n) {
   size_t b = (n + TPB - 1) / TPB;
-  const size_t cap = 148 * 32;  // grid-stride beyond this
+  const size_t cap = 132 * 32;  // grid-stride beyond this
   return (int)(b < cap ? (b ? b : 1) : cap);
 }
 

@@ -127,7 +127,7 @@ static int run_igemm(IgemmParams& p, int prec, int Kreal, cudaStream_t s) {
       return rc;
     }
   }
-  if (!umma_supported(p, prec)) return fail(CP_ERR_INVALID, "shape not supported by the tcgen05 kernel");
+  if (!umma_supported(p, prec)) return fail(CP_ERR_INVALID, "shape not supported by the wgmma kernel");
   void* tiles = nullptr;
   CP_CUDA_CHECK(cudaMallocAsync(&tiles, umma_weight_bytes(Kreal, p.CoutPad, prec), s));
   int rc = launch_pack_umma_weight(p.wgt, p.CoutPad, Kreal, p.Cout, p.CoutPad, prec, tiles, s);
@@ -303,7 +303,7 @@ int cp_preprocess_affine(const uint8_t* frames, float* out, int32_t B, int32_t s
   M[5] = b2;
   size_t total = (size_t)B * dst_h * dst_w;
   int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > 132 * 16) blocks = 132 * 16;
   preprocess_kernel<<<blocks, 256, 0, (cudaStream_t)stream_>>>(frames, out, B, src_h, src_w, dst_h, dst_w, W, mean[0],
                                                               mean[1], mean[2], stdv[0], stdv[1], stdv[2]);
   CP_LAUNCH_CHECK("preprocess_kernel");

@@ -1,22 +1,20 @@
-// tcgen05 (5th-gen tensor core) implicit-GEMM convolution for sm_100a.
+// wgmma (Hopper warpgroup MMA) implicit-GEMM convolution for sm_90a.
 //
 //   D[m, n] = sum_k A[m, k] * W[n, k]      m = output pixel, n = output channel, k = (tap, ci)
 //
 // Same contract as igemm_fp32.cu (IgemmParams: NHWC fp32 activations, channel-concatenated
 // sources, DCNv2 deformable gather, fused bias / residual / ReLU epilogue) but the contraction
 // runs on the tensor cores:
-//   * warps 0-3 (128 threads, one per tile row) GATHER the A tile -- plain im2col rows or the
+//   * warps 0-7 (two threads per tile row) GATHER the A tile -- plain im2col rows or the
 //     bilinear deformable samples of dcn_v2_im2col_cuda.cu:125-195 -- convert it and write it
-//     straight into shared memory in the canonical K-major SWIZZLE_128B layout the UMMA
-//     descriptor expects (a data-dependent gather cannot come from TMA);
-//   * warp 5 streams the weight tiles, pre-swizzled at load time into exact smem images, with one
-//     cp.async.bulk (UBLKCP) per stage, completing on the stage's mbarrier;
-//   * warp 4 (one elected lane) issues tcgen05.mma (M = 128, N = BN, cta_group::1) with the
-//     accumulator in TMEM and releases stages with tcgen05.commit;
-//   * warps 0-3 then read the accumulator with tcgen05.ld (lane == output row) and run the epilogue.
+//     straight into shared memory in the canonical K-major SWIZZLE_128B layout the wgmma
+//     descriptor expects (a data-dependent gather cannot come from TMA); thread 0 also streams
+//     the weight tile of the stage, pre-swizzled at load time, with one cp.async.bulk;
+//   * warpgroups 2 and 3 each multiply 64 rows of the tile (wgmma m64nBN) into register
+//     accumulators and run the epilogue.
 // Precisions:
-//   PREC_BF16   kind::f16, bf16 operands, fp32 accumulate                       (fast mode)
-//   PREC_TF32X3 kind::tf32, 3-term split  a_hi*b_hi + a_lo*b_hi + a_hi*b_lo     (fp32-equivalent mode)
+//   PREC_BF16   bf16 operands, fp32 accumulate                                  (fast mode)
+//   PREC_TF32X3 tf32, 3-term split  a_hi*b_hi + a_lo*b_hi + a_hi*b_lo           (fp32-equivalent mode)
 // Every mbarrier wait carries a clock64 watchdog that traps instead of hanging the GPU.
 #include "common.cuh"
 #include "umma_common.cuh"
@@ -26,63 +24,31 @@ namespace {
 
 constexpr int UM_BM = 128;
 constexpr int UM_PROD_WARPS = 8;            // A-gather warps: two threads per tile row, 4 chunks each
-constexpr int UM_THREADS = (UM_PROD_WARPS + 2 + 4) * 32;   // + 4 promoter / epilogue warps (tf32x3 only; idle otherwise)
-constexpr int UM_PROMO_WARP0 = UM_PROD_WARPS + 2;
+constexpr int UM_THREADS = (UM_PROD_WARPS + 8) * 32;       // + two consumer warpgroups
 constexpr uint32_t ROW_BYTES = 128;        // one K block = 128 bytes per row (64 bf16 / 32 tf32)
 constexpr uint32_t A_TILE_BYTES = UM_BM * ROW_BYTES;
 
 using namespace umma;
 
-template <int KIND_TF32>
-__device__ __forceinline__ void umma(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-  if (KIND_TF32) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
-        : "memory");
-  } else {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-        "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
-        : "memory");
-  }
-}
-// K-major SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor):
-//   [0,14) start address >> 4, [16,30) LBO >> 4 (ignored for swizzled K-major, 1), [32,46) SBO >> 4 = 1024 B between
-//   8-row groups, [46,48) version = 1, [61,64) layout type = 2 (SWIZZLE_128B)
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr) {
-  return (uint64_t)((saddr >> 4) & 0x3FFFu) | (1ull << 16) | ((uint64_t)(1024 >> 4) << 32) | (1ull << 46) | (2ull << 61);
-}
-// instruction descriptor (cute::UMMA::InstrDescriptor): c_format F32 (1 << 4), a/b format (1 = bf16, 2 = tf32) at
-// [7,10) / [10,13), K-major A and B (bits 15, 16 = 0), N >> 3 at [17,23), M >> 4 at [24,29)
-__device__ __forceinline__ uint32_t make_idesc(int n, int fmt) {
-  return (1u << 4) | ((uint32_t)fmt << 7) | ((uint32_t)fmt << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(UM_BM >> 4) << 24);
-}
-
 struct UmmaSmem {   // control block at the head of dynamic smem (the tiles follow, 1024-byte aligned)
   unsigned long long full[8];
   unsigned long long empty[8];
-  unsigned long long accum_full;
-  unsigned long long p_full[2], p_empty[2];     // tf32x3: accumulation-group buffers (MMA issuer <-> promoter warps)
-  uint32_t tmem_base;
 };
 
 template <int PREC>
 struct PrecTraits;
 template <>
 struct PrecTraits<0> {   // bf16
-  static constexpr int kElems = 64, kChunkCh = 8, kTilesA = 1, kFmt = 1;
+  static constexpr int kElems = 64, kChunkCh = 8, kTilesA = 1;
 };
 template <>
 struct PrecTraits<1> {   // tf32 x 3
-  static constexpr int kElems = 32, kChunkCh = 4, kTilesA = 2, kFmt = 2;
+  static constexpr int kElems = 32, kChunkCh = 4, kTilesA = 2;
 };
 
 // ------------------------------------------------------------------ the kernel
-template <int PREC, int MODE>
-__global__ void __launch_bounds__(UM_THREADS) igemm_umma_kernel(const IgemmParams p, const int BN, const int STAGES, const int NACC) {
+template <int PREC, int MODE, int BN>
+__global__ void __launch_bounds__(UM_THREADS, 1) igemm_umma_kernel(const IgemmParams p, const int STAGES, const int NACC) {
   using T = PrecTraits<PREC>;
   extern __shared__ __align__(1024) unsigned char smem[];
   UmmaSmem* ctl = reinterpret_cast<UmmaSmem*>(smem);
@@ -92,7 +58,7 @@ __global__ void __launch_bounds__(UM_THREADS) igemm_umma_kernel(const IgemmParam
   const uint32_t a_bytes = A_TILE_BYTES * T::kTilesA;
   const uint32_t stage_bytes = a_bytes + b_tile_bytes;
 
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int tid = threadIdx.x, warp = tid >> 5;
   const int M = p.B * p.Hout * p.Wout;
   // 1-D grid, n tile fastest: the CTAs that share an A row block run back to back and hit it in L2
   // (gridDim.y would overflow at 65535 row blocks: B = 32 at 512 x 512 has 65536)
@@ -104,32 +70,18 @@ __global__ void __launch_bounds__(UM_THREADS) igemm_umma_kernel(const IgemmParam
 
   if (tid == 0) {
     for (int s = 0; s < STAGES; ++s) {
-      mbar_init(smem_u32(&ctl->full[s]), UM_PROD_WARPS * 32 + 1);
-      mbar_init(smem_u32(&ctl->empty[s]), 1);
-    }
-    mbar_init(smem_u32(&ctl->accum_full), 1);
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(smem_u32(&ctl->p_full[s]), 1);
-      mbar_init(smem_u32(&ctl->p_empty[s]), 128);
+      mbar_init(smem_u32(&ctl->full[s]), UM_PROD_WARPS * 32 + 1);      // + the weight copy's expect_tx arrival
+      mbar_init(smem_u32(&ctl->empty[s]), 2);                          // one arrival per consumer warpgroup
     }
     fence_mbar_init();
   }
-  uint32_t tmem_cols = 32;
-  // tf32x3: two accumulation-group buffers + BN columns of promoted sums (NACC = K blocks per group); else NACC accumulators
-  while ((int)tmem_cols < BN * (PREC == 1 ? 3 : NACC)) tmem_cols <<= 1;
-  if (warp == UM_PROD_WARPS) {
-    tmem_alloc(smem_u32(&ctl->tmem_base), tmem_cols);
-    tmem_relinquish();
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = ctl->tmem_base;
   griddep_wait();      // PDL: the prologue above is private to the CTA; activations are read from here on
 
   if (warp < UM_PROD_WARPS) {
     // =========================== A producers: two threads per tile row, four 16-byte chunks each ===============
     {
+      const unsigned char* wsrc = reinterpret_cast<const unsigned char*>(p.wgt_umma) + (size_t)n_tile * KB * b_tile_bytes;
       const int r = tid >> 1;
       const int qbase = (tid & 1) * 4;
       const int m = m0 + r;
@@ -224,6 +176,11 @@ __global__ void __launch_bounds__(UM_THREADS) igemm_umma_kernel(const IgemmParam
         }
         // ---- ... then wait for the stage, convert and store into the swizzled K-major tile
         mbar_wait(smem_u32(&ctl->empty[stage]), phase ^ 1u);
+        if (tid == 0) {
+          const uint32_t bar = smem_u32(&ctl->full[stage]);
+          mbar_arrive_expect_tx(bar, b_tile_bytes);
+          bulk_g2s(tiles0 + (uint32_t)stage * stage_bytes + a_bytes, wsrc + (size_t)kb * b_tile_bytes, b_tile_bytes, bar);
+        }
         const uint32_t a_hi = tiles0 + (uint32_t)stage * stage_bytes + row_off;
         const uint32_t a_lo = a_hi + A_TILE_BYTES;
 #pragma unroll
@@ -280,20 +237,40 @@ __global__ void __launch_bounds__(UM_THREADS) igemm_umma_kernel(const IgemmParam
       }
     }
 
-    // =========================== epilogue (warps 0-3): TMEM lane == tile row (bf16; tf32x3: promoter warps) =====
-    if (PREC != 1 && warp < 4) {
-    const int m = m0 + tid;
-    const bool valid = m < M;
-    int ox = 0, oy = 0, n = 0;
-    if (valid) {
-      ox = m % p.Wout;
-      int t = m / p.Wout;
-      oy = t % p.Hout;
-      n = t / p.Hout;
+  } else {
+    // =========================== consumers: warpgroup c multiplies rows [64 c, 64 c + 64) of the tile ============
+    const int c = (warp - UM_PROD_WARPS) >> 2, wt = tid & 127;
+    constexpr bool X3 = PREC == 1;
+    float acc[BN / 2];
+    float sums[X3 ? BN / 2 : 1];
+#pragma unroll
+    for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
+#pragma unroll
+    for (int j = 0; j < (X3 ? BN / 2 : 1); ++j) sums[j] = 0.f;
+    int stage = 0;
+    uint32_t phase = 0;
+    int gk = 0;                              // tf32x3: K block inside its accumulation group
+    for (int kb = 0; kb < KB; ++kb) {
+      mbar_wait(smem_u32(&ctl->full[stage]), phase);
+      const uint32_t a_hi = tiles0 + (uint32_t)stage * stage_bytes;
+      const uint64_t da = make_desc(a_hi + (uint32_t)c * 64u * ROW_BYTES, 32), db = make_desc(a_hi + a_bytes, 32);
+      // tf32x3: NACC K blocks are chained in the accumulator, then added into round-to-nearest fp32 sums
+      mma_kblock<BN, X3, PREC == 0, 4>(acc, da, db, A_TILE_BYTES >> 4, ((uint32_t)BN * ROW_BYTES) >> 4, X3 ? gk == 0 : kb == 0);
+      if (wt == 0) mbar_arrive(smem_u32(&ctl->empty[stage]));
+      if (++stage == STAGES) {
+        stage = 0;
+        phase ^= 1u;
+      }
+      if (X3) {
+        if (gk == NACC - 1 || kb == KB - 1) {
+#pragma unroll
+          for (int j = 0; j < (X3 ? BN / 2 : 1); ++j) sums[j] += acc[X3 ? j : 0];
+          gk = 0;
+        } else {
+          ++gk;
+        }
+      }
     }
-    mbar_wait(smem_u32(&ctl->accum_full), 0u);
-    tc_fence_after();
-    const uint32_t lane_base = tmem_base + ((uint32_t)(warp * 32) << 16);
     EpiParams ep;
     ep.bias = p.bias;
     ep.residual = p.residual;
@@ -309,173 +286,25 @@ __global__ void __launch_bounds__(UM_THREADS) igemm_umma_kernel(const IgemmParam
     ep.H = p.Hout;
     ep.W = p.Wout;
     const int col_end = min(p.Cout, (n_tile + 1) * BN);
-    for (int c0 = 0; c0 < BN; c0 += 32) {
-      float vv[32];
-#pragma unroll
-      for (int j = 0; j < 32; ++j) vv[j] = 0.f;
-      // the K blocks were dealt round-robin to NACC TMEM accumulators (shorter truncating chains); sum them in fp32
-      for (int a = 0; a < NACC; ++a) {
-        uint32_t rr[32];
-        tmem_ld16(lane_base + (uint32_t)(a * BN + c0), rr);
-        if (c0 + 16 < BN) {
-          tmem_ld16(lane_base + (uint32_t)(a * BN + c0 + 16), rr + 16);
-        } else {
-#pragma unroll
-          for (int j = 16; j < 32; ++j) rr[j] = 0u;
-        }
-        tmem_ld_wait();
-#pragma unroll
-        for (int j = 0; j < 32; ++j) vv[j] += __uint_as_float(rr[j]);
-      }
-      epilogue_sub_tile(ep, nullptr, vv, lane, valid, m, n, oy, ox, n_tile * BN + c0, col_end);
-    }
-    }
-  } else if (warp == UM_PROD_WARPS) {
-    // =========================== MMA issuer (one lane) ===========================
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc(BN, T::kFmt);
-      int stage = 0;
-      uint32_t phase = 0;
-      int gk = 0, buf = 0;                   // tf32x3: K block inside its accumulation group / group buffer
-      uint32_t pe = 0;                       // bit b: phase of p_empty[b]
-      for (int kb = 0; kb < KB; ++kb) {
-        if (PREC == 1 && gk == 0) mbar_wait(smem_u32(&ctl->p_empty[buf]), ((pe >> buf) & 1u) ^ 1u);
-        mbar_wait(smem_u32(&ctl->full[stage]), phase);
-        tc_fence_after();
-        const uint32_t a_hi = tiles0 + (uint32_t)stage * stage_bytes;
-        const uint32_t b_hi = a_hi + a_bytes;
-        const uint64_t da_hi = make_desc(a_hi), db_hi = make_desc(b_hi);
-        // tf32x3: the accumulator truncates, so only NACC K blocks are chained in TMEM; every finished group is promoted
-        // into round-to-nearest fp32 sums by the promoter warps (same two-level scheme as conv_tma.cu / dcn_tma.cu)
-        const uint32_t d_tmem = tmem_base + (uint32_t)((PREC == 1 ? buf : (kb % NACC)) * BN);
-        const bool fresh = PREC == 1 ? (gk == 0) : (kb < NACC);        // first K block of this accumulator overwrites it
-        if (PREC == 0) {
-#pragma unroll
-          for (int k = 0; k < 4; ++k)        // 4 x 32-byte K slices per 128-byte row
-            umma<0>(d_tmem, da_hi + (uint64_t)(k * 2), db_hi + (uint64_t)(k * 2), idesc, (!fresh || k > 0) ? 1u : 0u);
-        } else {                            // cross terms first, hi x hi last (see conv_tma.cu)
-          const uint64_t da_lo = make_desc(a_hi + A_TILE_BYTES), db_lo = make_desc(b_hi + (uint32_t)BN * ROW_BYTES);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            const uint64_t adv = (uint64_t)(k * 2);
-            umma<1>(d_tmem, da_lo + adv, db_hi + adv, idesc, (!fresh || k > 0) ? 1u : 0u);
-            umma<1>(d_tmem, da_hi + adv, db_lo + adv, idesc, 1u);
-          }
-#pragma unroll
-          for (int k = 0; k < 4; ++k) umma<1>(d_tmem, da_hi + (uint64_t)(k * 2), db_hi + (uint64_t)(k * 2), idesc, 1u);
-        }
-        umma_commit(smem_u32(&ctl->empty[stage]));     // frees the stage when these MMAs have read it
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1u;
-        }
-        if (PREC == 1) {
-          if (gk == NACC - 1 || kb == KB - 1) {
-            umma_commit(smem_u32(&ctl->p_full[buf]));
-            pe ^= 1u << buf;
-            buf ^= 1;
-            gk = 0;
-          } else {
-            ++gk;
-          }
-        }
-      }
-      if (PREC != 1) umma_commit(smem_u32(&ctl->accum_full));
-    }
-    __syncwarp();
-  } else if (warp >= UM_PROMO_WARP0) {
-    // =========================== tf32x3: promoter + epilogue warps, TMEM lane == tile row ===========================
-    if (PREC == 1) {
-      const int q = warp & 3;                    // TMEM lane quadrant this warp may access
-      const int row = q * 32 + lane;
-      const int m = m0 + row;
+    float* dstage = reinterpret_cast<float*>(smem + (tiles0 - smem_u32(smem)) + (size_t)STAGES * stage_bytes) +
+                    (size_t)c * (DRAIN_STAGE_BYTES / 4);
+    auto fn = [&](int r, int cb, float (&v)[16]) {
+      const int m = m0 + c * 64 + r;
       const bool valid = m < M;
       int ox = 0, oy = 0, n = 0;
       if (valid) {
         ox = m % p.Wout;
-        int t = m / p.Wout;
+        const int t = m / p.Wout;
         oy = t % p.Hout;
         n = t / p.Hout;
       }
-      const uint32_t lane_base = tmem_base + ((uint32_t)(q * 32) << 16);
-      const uint32_t sum_base = lane_base + (uint32_t)(2 * BN);
-      const int ngroups = (KB + NACC - 1) / NACC;
-      int buf = 0;
-      uint32_t pf = 0;
-      for (int gi = 0; gi < ngroups; ++gi) {
-        mbar_wait(smem_u32(&ctl->p_full[buf]), (pf >> buf) & 1u);
-        tc_fence_after();
-        for (int c = 0; c * 16 < BN; ++c) {
-          uint32_t rr[16], ss[16];
-          tmem_ld16(lane_base + (uint32_t)(buf * BN + c * 16), rr);
-          if (gi > 0) tmem_ld16(sum_base + (uint32_t)(c * 16), ss);
-          tmem_ld_wait();
-          if (gi > 0) {
-#pragma unroll
-            for (int j = 0; j < 16; ++j) rr[j] = __float_as_uint(__uint_as_float(ss[j]) + __uint_as_float(rr[j]));
-          }
-          tmem_st16(sum_base + (uint32_t)(c * 16), rr);
-        }
-        tmem_st_wait();
-        tc_fence_before();
-        mbar_arrive(smem_u32(&ctl->p_empty[buf]));
-        pf ^= 1u << buf;
-        buf ^= 1;
-      }
-      EpiParams ep;
-      ep.bias = p.bias;
-      ep.residual = p.residual;
-      ep.resStride = p.resStride;
-      ep.relu = p.relu;
-      ep.res_after_relu = p.res_after_relu;
-      ep.round_tf32 = 0;
-      ep.out = p.out;
-      ep.outStride = p.outStride;
-      ep.out_nchw = p.out_nchw;
-      ep.Cout = p.Cout;
-      ep.CoutPad = p.CoutPad;
-      ep.H = p.Hout;
-      ep.W = p.Wout;
-      const int col_end = min(p.Cout, (n_tile + 1) * BN);
-      for (int c0 = 0; c0 < BN; c0 += 32) {
-        uint32_t rr[32];
-        tmem_ld16(sum_base + (uint32_t)c0, rr);
-        if (c0 + 16 < BN) {
-          tmem_ld16(sum_base + (uint32_t)(c0 + 16), rr + 16);
-        } else {
-#pragma unroll
-          for (int j = 16; j < 32; ++j) rr[j] = 0u;
-        }
-        tmem_ld_wait();
-        float vv[32];
-#pragma unroll
-        for (int j = 0; j < 32; ++j) vv[j] = __uint_as_float(rr[j]);
-        epilogue_sub_tile(ep, nullptr, vv, lane, valid, m, n, oy, ox, n_tile * BN + c0, col_end);
-      }
-    }
-  } else {
-    // =========================== weight-tile loader (one lane) ===========================
-    if (lane == 0) {
-      const unsigned char* wsrc = reinterpret_cast<const unsigned char*>(p.wgt_umma) + (size_t)n_tile * KB * b_tile_bytes;
-      int stage = 0;
-      uint32_t phase = 0;
-      for (int kb = 0; kb < KB; ++kb) {
-        mbar_wait(smem_u32(&ctl->empty[stage]), phase ^ 1u);
-        const uint32_t bar = smem_u32(&ctl->full[stage]);
-        mbar_arrive_expect_tx(bar, b_tile_bytes);
-        bulk_g2s(tiles0 + (uint32_t)stage * stage_bytes + a_bytes, wsrc + (size_t)kb * b_tile_bytes, b_tile_bytes, bar);
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1u;
-        }
-      }
-    }
-    __syncwarp();
+      if (cb < BN) epilogue_row<16>(ep, v, valid, m, n, oy, ox, n_tile * BN + cb, col_end);
+    };
+    if constexpr (X3)
+      drain_rows<BN>(sums, dstage, wt, 1 + c, fn);
+    else
+      drain_rows<BN>(acc, dstage, wt, 1 + c, fn);
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == UM_PROD_WARPS) tmem_dealloc(tmem_base, tmem_cols);
 }
 
 // ------------------------------------------------------------------ weight tiling
@@ -524,11 +353,9 @@ __global__ void pack_umma_weight_kernel(const float* __restrict__ src, int ld, i
 }  // namespace
 
 // ---- host side -----------------------------------------------------------------------------------------------
-// tf32x3 keeps two accumulation-group buffers and the promoted sums in TMEM: 3 BN <= 512 columns
-int umma_tile_n(int CoutPad, int prec) {
-  const int cap = prec == 1 ? 128 : 256;
-  return CoutPad <= cap ? CoutPad : cap;
-}
+// The N tile is the wgmma N of one consumer warpgroup; its accumulator takes BN / 2 registers per thread (tf32x3: twice
+// that with the promoted sums) out of the 128 a thread of this 512-thread kernel has.
+int umma_tile_n(int CoutPad, int prec) { return wgmma_tile_n(CoutPad, prec == 1 ? 64 : 128); }
 
 bool umma_supported(const IgemmParams& p, int prec) {
   if (p.mode != IGEMM_NHWC_VEC && p.mode != IGEMM_DCN) return false;
@@ -536,9 +363,7 @@ bool umma_supported(const IgemmParams& p, int prec) {
   if (p.Cin % ch) return false;
   for (int s = 0; s < p.nsrc; ++s)
     if (p.srcC[s] % ch || p.srcStride[s] % 4) return false;
-  const int bn = umma_tile_n(p.CoutPad, prec);
-  if (bn % 16 || p.CoutPad % bn) return false;
-  return true;
+  return umma_tile_n(p.CoutPad, prec) != 0;
 }
 
 size_t umma_weight_bytes(int Kreal, int CoutPad, int prec) {
@@ -556,12 +381,29 @@ int launch_pack_umma_weight(const float* src, int ld, int Kreal, int Cout, int C
   const int nt = CoutPad / bn;
   size_t total = (size_t)nt * KB * bn * 8;
   int blocks = (int)((total + 255) / 256);
-  if (blocks > 148 * 32) blocks = 148 * 32;
+  if (blocks > 132 * 32) blocks = 132 * 32;
   if (prec == 0)
     pack_umma_weight_kernel<0><<<blocks, 256, 0, s>>>(src, ld, Kreal, Cout, bn, nt, KB, (unsigned char*)dst);
   else
     pack_umma_weight_kernel<1><<<blocks, 256, 0, s>>>(src, ld, Kreal, Cout, bn, nt, KB, (unsigned char*)dst);
   CP_LAUNCH_CHECK("pack_umma_weight_kernel");
+  return CP_OK;
+}
+
+template <int PREC, int BN>
+static int launch_igemm_umma_bn(const IgemmParams& p, int stages, size_t smem, int nacc, cudaStream_t stream) {
+  void (*kern)(const IgemmParams, const int, const int) =
+      (p.mode == IGEMM_DCN) ? igemm_umma_kernel<PREC, IGEMM_DCN, BN> : igemm_umma_kernel<PREC, IGEMM_NHWC_VEC, BN>;
+  static PerDevice<bool, 2> configured;
+  const int slot = p.mode == IGEMM_DCN ? 1 : 0;
+  if (!configured.here(slot)) {
+    CP_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    configured.here(slot) = true;
+  }
+  const int M = p.B * p.Hout * p.Wout;
+  dim3 grid((unsigned)((size_t)(p.CoutPad / BN) * ((M + UM_BM - 1) / UM_BM)));
+  CP_CUDA_CHECK(launch_kernel(kern, grid, dim3(UM_THREADS), smem, stream, p, stages, nacc));
+  CP_LAUNCH_CHECK("igemm_umma_kernel");
   return CP_OK;
 }
 
@@ -571,31 +413,29 @@ int launch_igemm_umma(const IgemmParams& p, int prec, cudaStream_t stream) {
   const int bn = umma_tile_n(p.CoutPad, prec);
   const int tilesA = prec == 0 ? 1 : 2;
   const size_t stage_bytes = (size_t)A_TILE_BYTES * tilesA + (size_t)bn * ROW_BYTES * tilesA;
-  int stages = (int)((204 * 1024) / stage_bytes);
+  const size_t fixed = 512 + 1024 + 2 * (size_t)DRAIN_STAGE_BYTES;     // control block, alignment, epilogue staging
+  int stages = (int)((224 * 1024 - fixed) / stage_bytes);
   if (stages > 6) stages = 6;
   // deformable gather: neighbouring rows / taps sample overlapping 2x2 neighbourhoods (each input pixel is touched by
-  // up to 36 samples); a small pipeline leaves most of the 228 KB for L1 so those re-reads hit on chip
+  // up to 36 samples); a small pipeline leaves most of the shared memory / L1 for those re-reads
   if (p.mode == IGEMM_DCN && stages > 2) stages = 2;
   if (stages < 2) return fail(CP_ERR_INVALID, "igemm_umma: tile does not fit shared memory");
-  const size_t smem = 512 + 2048 + stages * stage_bytes;
-  const int M = p.B * p.Hout * p.Wout;
-  dim3 grid((unsigned)((size_t)(p.CoutPad / bn) * ((M + UM_BM - 1) / UM_BM)));
-  void (*kern)(const IgemmParams, const int, const int, const int) = nullptr;
-  if (prec == 0)
-    kern = (p.mode == IGEMM_DCN) ? igemm_umma_kernel<0, IGEMM_DCN> : igemm_umma_kernel<0, IGEMM_NHWC_VEC>;
-  else
-    kern = (p.mode == IGEMM_DCN) ? igemm_umma_kernel<1, IGEMM_DCN> : igemm_umma_kernel<1, IGEMM_NHWC_VEC>;
-  static PerDevice<bool, 4> configured;
-  const int slot = prec * 2 + (p.mode == IGEMM_DCN ? 1 : 0);
-  if (!configured.here(slot)) {
-    CP_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    configured.here(slot) = true;
-  }
-  // tf32x3: K blocks (12 MMAs each) per TMEM accumulation group, promoted into fp32 sums by the promoter warps
+  const size_t smem = fixed + stages * stage_bytes;
+  // tf32x3: K blocks (12 MMAs each) chained in the accumulator before they are added into the fp32 sums
   const int nacc = prec == 1 ? x3_group_blocks() : 1;
-  CP_CUDA_CHECK(launch_kernel(kern, grid, dim3(UM_THREADS), smem, stream, p, bn, stages, nacc));
-  CP_LAUNCH_CHECK("igemm_umma_kernel");
-  return CP_OK;
+  if (prec == 0) {
+    switch (bn) {
+      case 16: return launch_igemm_umma_bn<0, 16>(p, stages, smem, nacc, stream);
+      case 32: return launch_igemm_umma_bn<0, 32>(p, stages, smem, nacc, stream);
+      case 64: return launch_igemm_umma_bn<0, 64>(p, stages, smem, nacc, stream);
+      default: return launch_igemm_umma_bn<0, 128>(p, stages, smem, nacc, stream);
+    }
+  }
+  switch (bn) {
+    case 16: return launch_igemm_umma_bn<1, 16>(p, stages, smem, nacc, stream);
+    case 32: return launch_igemm_umma_bn<1, 32>(p, stages, smem, nacc, stream);
+    default: return launch_igemm_umma_bn<1, 64>(p, stages, smem, nacc, stream);
+  }
 }
 
 }  // namespace cp

@@ -56,9 +56,9 @@ struct Op {
   int kh = 1, kw = 1, stride = 1, pad = 0, Cin = 0, Cout = 0, CoutPad = 0, Kpad = 0;
   size_t w_off = 0, b_off = 0;
   int w_ld = 0;            // leading dimension of the fp32 packed weight matrix
-  bool use_umma = false;   // run on the tcgen05 gather kernel
-  bool use_tma = false;    // run on the TMA-fed tcgen05 kernel (conv_tma.cu)
-  bool use_dcn_tma = false;   // deformable conv on the TMA-staged tcgen05 kernel (dcn_tma.cu)
+  bool use_umma = false;   // run on the wgmma gather kernel
+  bool use_tma = false;    // run on the TMA-fed wgmma kernel (conv_tma.cu)
+  bool use_dcn_tma = false;   // deformable conv on the TMA-staged wgmma kernel (dcn_tma.cu)
   std::vector<int> head_children;   // merged heads 3x3 conv: indices of the per-head 1x1 ops that read its slices
   bool fuse_heads = false;          // ... which run inside its epilogue (conv_tma.cu), never touching HBM
   bool fused_away = false;          // this 1x1 op is computed by its parent's epilogue
@@ -118,7 +118,7 @@ struct cp_plan {
   void* decode_ws = nullptr;
   size_t decode_ws_bytes = 0;
   double* gn_stats = nullptr;
-  int prec = -1;                 // -1 fp32 CUDA cores, 0 bf16 tcgen05, 1 tf32x3 tcgen05, 2 tf32 (TMA) + tf32x3 elsewhere
+  int prec = -1;                 // -1 fp32 CUDA cores, 0 bf16 wgmma, 1 tf32x3 wgmma, 2 tf32 (TMA) + tf32x3 elsewhere
   int min_tc_cin = 32;           // ops with fewer input channels stay on the CUDA-core kernels (CP_MIN_TC_CIN overrides)
   bool no_fuse_heads = false;    // CP_NO_FUSE_HEADS=1: keep the per-head 1x1 convs as separate launches
   bool no_dcn_tma = false;       // CP_NO_DCN_TMA=1: deformable convs on the global-gather kernel (A/B measurements)
@@ -574,7 +574,7 @@ int build_graph(cp_plan* P) {
       const int gather_prec = P->prec == 2 ? 1 : P->prec;
       if (op.src[0].ext >= 0) continue;
       // 16-channel layers (level0 / level1): 133 K single-tile CTAs of almost no MMA work are dominated by the fixed
-      // per-CTA cost of a tcgen05 kernel (measured 5.2 ms vs 2.5 ms on the FFMA kernel) -> keep them on CUDA cores
+      // per-CTA cost of a tensor-core kernel -> keep them on CUDA cores
       if (op.Cin < P->min_tc_cin) continue;
       q.Hin = op.src[0].H;
       if ((P->prec == 2 || P->prec == 1) && !P->no_dcn_tma && dcn_tma_supported(q, P->prec == 1)) {
@@ -593,11 +593,9 @@ int build_graph(cp_plan* P) {
     }
   }
   // The per-head 1x1 convs move into the epilogue of the merged heads conv when that one runs on conv_tma: hidden =
-  // relu(conv3x3) never reaches HBM (3.7 GB of writes + 3.7 GB of reads and seven launches at batch 32).  Single-pass
-  // tf32: the epilogue thread that owns a position multiplies it with the head's [256][16] weights (3.8 -> 3.4 ms).
-  // tf32x3: the same threads also promote the accumulation groups of the NEXT tile, so the 1x1 weights + 3x3 bias of
-  // the tile are staged in shared memory by a dedicated warp and only the float4 groups holding real output channels are
-  // multiplied (heads 7.7 -> 5.2 ms; the first version, 16 padded outputs through __ldg, stalled the promotion: 9.9 ms).
+  // relu(conv3x3) never reaches HBM (3.7 GB of writes + 3.7 GB of reads and seven launches at batch 32).  In both
+  // tf32 modes the two epilogue threads that own an output row multiply its hidden channels with the head's [256][16]
+  // 1x1 weights (read through __ldg) and combine their halves with one shuffle (conv_tma.cu).
   if (P->prec == 2 || P->prec == 1) {
     for (auto& op : P->ops) {
       if (op.head_children.empty() || !op.use_tma || P->no_fuse_heads) continue;
@@ -815,10 +813,10 @@ struct ProfCtx {
   std::vector<cudaEvent_t> ev;
 };
 
-// PDL hides ~2 us of launch latency + prologue per kernel: a constant ~0.19 ms of the forward (scripts/pdl_sweep.py, ms with /
-// without: batch 1 1.99 / 2.18, 2 2.77 / 2.97, 4 4.45 / 4.64, 8 7.73 / 7.83, 16 14.70 / 14.65, 32 27.42 / 27.17).  Beyond
-// batch 8 the kernels run for 100s of us and the early CTAs of the next launch only add scheduling work, so it is switched
-// on by the amount of work.  CP_PDL=1 / CP_NO_PDL=1 force it.
+// PDL hides launch latency + prologue per kernel, which matters when the kernels are short (small batches); once they
+// run for 100s of us the early CTAs of the next launch only add scheduling work, so it is switched on by the amount of
+// work.  The threshold below has not been re-chosen for the H100 (scripts/pdl_sweep.py sweeps it); results are
+// bit-identical either way.  CP_PDL=1 / CP_NO_PDL=1 force it.
 static bool pdl_wanted(long long pixels) {
   if (getenv("CP_NO_PDL")) return false;
   if (const char* e = getenv("CP_PDL")) return atoi(e) != 0;

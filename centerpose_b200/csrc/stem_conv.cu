@@ -113,7 +113,7 @@ __global__ void __launch_bounds__(ST_TX* ST_TY)
 // ------------------------------------------------------------------------------------------------------------------
 // 3x3 stride-1 pad-1 convolution, 16 -> 16 channels, NHWC fp32 in and out (DLA level0 at full resolution,
 // pose_dla_dcn.py:239-240 + _make_conv_level).  K = 144 is too small for a tensor-core tile to pay for itself at 8.4 M
-// positions (measured: 4.9 ms on the tcgen05 gather kernel, 2.5 ms on the generic FFMA implicit GEMM); a direct
+// positions (it ran at half the speed of the generic FFMA implicit GEMM on the tensor-core gather kernel); a direct
 // convolution with the halo tile transposed into channel planes in shared memory runs at the FFMA rate instead.
 constexpr int C3_TX = 16, C3_TY = 16, C3_PX = 4;
 constexpr int C3_W = C3_TX * C3_PX;                              // 64 x 16 output pixels per CTA

@@ -1,4 +1,4 @@
-// PTX wrappers and epilogue helpers shared by the tcgen05 kernels (igemm_umma.cu, conv_tma.cu).  sm_100a only.
+// PTX wrappers and epilogue helpers shared by the wgmma kernels (igemm_umma.cu, conv_tma.cu, dcn_tma.cu).  sm_90a.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -37,7 +37,7 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   while (!mbar_try_wait(bar, parity)) {
     if (clock64() - t0 > 4000000000LL) {
 #ifdef CP_MBAR_DEBUG
-      printf("tcgen05 kernel: mbarrier watchdog (block %d thread %d bar %u parity %u)\n", blockIdx.x, threadIdx.x, bar, parity);
+      printf("wgmma kernel: mbarrier watchdog (block %d thread %d bar %u parity %u)\n", blockIdx.x, threadIdx.x, bar, parity);
 #endif
       __trap();
     }
@@ -45,64 +45,124 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
 }
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 __device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
 __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
   asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(dst),
                "l"(src), "r"(bytes), "r"(bar)
                : "memory");
 }
-__device__ __forceinline__ void tmem_alloc(uint32_t dst_smem, uint32_t cols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(dst_smem), "r"(cols) : "memory");
-}
-__device__ __forceinline__ void tmem_relinquish() {
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t cols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* r) {
+// named barrier of the 128 threads of one warpgroup (ids 1 .. 15; 0 is __syncthreads)
+__device__ __forceinline__ void wg_bar_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
+
+// ---- wgmma: a warpgroup (128 threads) multiplies a 64-row A tile by an N-row B tile, both K-major in shared memory,
+// into a register accumulator.  Fragment of thread t (warp w = t / 32, lane l): d[4 j + 2 i + c] holds row
+// 16 w + l / 4 + 8 i, column 8 j + 2 (l % 4) + c.
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_tf32(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d);
+template <int N>
+__device__ __forceinline__ void wgmma_bf16(float (&d)[N / 2], uint64_t da, uint64_t db, uint32_t scale_d);
+template <> __device__ __forceinline__ void wgmma_tf32<16>(float (&d)[8], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(da), "l"(db), "r"(scale_d));
 }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* r) {
+template <> __device__ __forceinline__ void wgmma_tf32<32>(float (&d)[16], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]),
-        "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]),
-        "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(da), "l"(db), "r"(scale_d));
 }
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t* r) {
+template <> __device__ __forceinline__ void wgmma_tf32<64>(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]),
-      "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(scale_d));
 }
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t* r) {
+template <> __device__ __forceinline__ void wgmma_tf32<128>(float (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d) {
   asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,"
-      "%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]), "r"(r[10]),
-      "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]), "r"(r[20]),
-      "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]), "r"(r[30]),
-      "r"(r[31])
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(scale_d));
 }
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
+template <> __device__ __forceinline__ void wgmma_tf32<256>(float (&d)[128], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127}, %128, %129, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma_bf16<16>(float (&d)[8], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %10, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7}, %8, %9, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma_bf16<32>(float (&d)[16], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %18, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, %16, %17, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma_bf16<64>(float (&d)[32], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma_bf16<128>(float (&d)[64], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma_bf16<256>(float (&d)[128], uint64_t da, uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %130, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n256k16.f32.bf16.bf16 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127}, %128, %129, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
+      : "l"(da), "l"(db), "r"(scale_d));
+}
+
+// One K block on the tensor cores: KS slices of 32 bytes (8 tf32 / 16 bf16 elements) of a 64-row A tile and a BN-row B
+// tile.  X3: 3-term split a_lo b_hi + a_hi b_lo + a_hi b_hi (lo tiles at a_lo / b_lo descriptor units past the hi tiles),
+// cross terms first.  fresh: the first product overwrites the accumulator.  Returns when the products are in `acc` and
+// the operand tiles may be reused.
+template <int BN, bool X3, bool BF16, int KS>
+__device__ __forceinline__ void mma_kblock(float (&acc)[BN / 2], uint64_t da, uint64_t db, uint32_t a_lo, uint32_t b_lo,
+                                           bool fresh) {
+  wg_fence();
+#pragma unroll
+  for (int ks = 0; ks < KS; ++ks) {
+    const uint32_t sd = (fresh && ks == 0) ? 0u : 1u;
+    if (X3) {
+      wgmma_tf32<BN>(acc, da + a_lo + 2u * ks, db + 2u * ks, sd);
+      wgmma_tf32<BN>(acc, da + 2u * ks, db + b_lo + 2u * ks, 1u);
+    } else if (BF16) {
+      wgmma_bf16<BN>(acc, da + 2u * ks, db + 2u * ks, sd);
+    } else {
+      wgmma_tf32<BN>(acc, da + 2u * ks, db + 2u * ks, sd);
+    }
+  }
+  if (X3) {
+#pragma unroll
+    for (int ks = 0; ks < KS; ++ks) wgmma_tf32<BN>(acc, da + 2u * ks, db + 2u * ks, 1u);
+  }
+  wg_commit();
+  wg_wait<0>();
+}
 
 // Round to tf32 (10 mantissa bits), nearest, ties away from zero == cvt.rna.tf32.f32 for every finite input (the add
 // carries into the exponent exactly like the rounding does; FLT_MAX rounds to inf either way).  ptxas expands the cvt
@@ -128,7 +188,7 @@ __device__ __forceinline__ float4 ld_shared_v4f(uint32_t addr) {
   return v;
 }
 
-// ---- TMA tensor loads, tcgen05.mma kind::tf32, clusters, shared-memory matrix descriptors (conv_tma.cu, dcn_tma.cu)
+// ---- TMA tensor loads and shared-memory matrix descriptors (conv_tma.cu, dcn_tma.cu)
 __device__ __forceinline__ void tma_load_4d(uint32_t dst, const CUtensorMap* map, int c0, int c1, int c2, int c3, uint32_t bar) {
   asm volatile(
       "cp.async.bulk.tensor.4d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3, %4, %5}], [%6];" ::"r"(dst),
@@ -140,71 +200,28 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
                "l"(map), "r"(c0), "r"(c1), "r"(bar)
                : "memory");
 }
-// Same MMA with the two descriptors given as 32-bit low words + one shared high word (both operands use the same
-// layout template, only the 14-bit address field differs): the issuing warp then does 32-bit adds only.
-__device__ __forceinline__ void umma_tf32_lohi(uint32_t d_tmem, uint32_t a_lo, uint32_t b_lo, uint32_t desc_hi, uint32_t idesc,
-                                               uint32_t accum) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\tsetp.ne.b32 p, %5, 0;\n\tmov.b64 da, {%1, %3};\n\tmov.b64 db, {%2, %3};\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], da, db, %4, p;\n\t}" ::"r"(d_tmem),
-      "r"(a_lo), "r"(b_lo), "r"(desc_hi), "r"(idesc), "r"(accum)
-      : "memory");
-}
-__device__ __forceinline__ void umma_tf32(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
-      : "memory");
-}
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
   return pred != 0;
 }
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;\n\tbarrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-// bulk copy global -> the SAME shared-memory offset of every CTA in `mask`, completing on each CTA's own mbarrier
-__device__ __forceinline__ void bulk_g2s_multicast(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar, uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1], %2, [%3], %4;" ::"r"(dst),
-      "l"(src), "r"(bytes), "r"(bar), "h"(mask)
-      : "memory");
-}
-// tcgen05.commit that arrives on the same-offset mbarrier of every CTA in `mask`
-__device__ __forceinline__ void umma_commit_multicast(uint32_t bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar),
-               "h"(mask)
-               : "memory");
-}
 
-// K-major SWIZZLE_128B descriptor; `saddr` may be any multiple of 16 bytes.  Measured on B200
-// (scripts/tma_diag.py): the tensor core applies the 128-byte swizzle to the ABSOLUTE shared-memory address bits
-// [7,10), exactly like TMA does when it writes the slab, so a matrix that starts at an arbitrary 128-byte row of
-// the slab needs NO base-offset correction (setting the field to (addr >> 7) & 7 gives wrong results).
-// cslab = 32: 128-byte rows, SWIZZLE_128B (layout type 2), 8-row groups 1024 bytes apart;
-// cslab = 16:  64-byte rows, SWIZZLE_64B  (layout type 4), 8-row groups  512 bytes apart.
-__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, int use_base_offset, int cslab) {
+// wgmma shared-memory matrix descriptor, K-major and swizzled; `saddr` may be any multiple of 16 bytes.  The swizzle
+// is a function of the shared-memory address bits [7,10) (like the one TMA applies when it writes the slab), so a matrix
+// that starts at an arbitrary row of a slab needs no base-offset correction.
+//   [0,14) start address >> 4, [16,30) leading byte offset >> 4 (unused when swizzled, 1), [32,46) stride byte offset >> 4
+//   = distance of 8-row groups, [62,64) layout: 1 = SWIZZLE_128B, 2 = SWIZZLE_64B
+// cslab = 32: 128-byte rows, SWIZZLE_128B, 8-row groups 1024 bytes apart;
+// cslab = 16:  64-byte rows, SWIZZLE_64B,  8-row groups  512 bytes apart.
+__device__ __forceinline__ uint64_t make_desc(uint32_t saddr, int cslab) {
   const uint64_t sbo = cslab == 32 ? (1024 >> 4) : (512 >> 4);
-  const uint64_t lay = cslab == 32 ? 2ull : 4ull;
-  uint64_t d = (uint64_t)((saddr >> 4) & 0x3FFFu) | (1ull << 16) | (sbo << 32) | (1ull << 46) | (lay << 61);
-  if (use_base_offset) d |= (uint64_t)((saddr >> 7) & 7u) << 49;
-  return d;
+  const uint64_t lay = cslab == 32 ? 1ull : 2ull;
+  return (uint64_t)((saddr >> 4) & 0x3FFFu) | (1ull << 16) | (sbo << 32) | (lay << 62);
 }
-__device__ __forceinline__ uint32_t make_idesc_tf32(int n) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-}
-
 
 // ---------------------------------------------------------------------------------------------------------------
-// The fused epilogue of one [32 x 32] sub-tile: bias, residual (before or after the ReLU), ReLU, optional tf32
-// rounding, then an NHWC store (every lane streams its own row with 16-byte stores; routing the tile through shared
-// memory for fully coalesced stores was measured SLOWER, DESIGN.md section 4) or an NCHW store (coalesced across lanes).
+// The fused epilogue of NV consecutive columns of one output row: bias, residual (before or after the ReLU), ReLU,
+// optional tf32 rounding, then an NHWC store (16-byte stores along the row) or an NCHW store.
 struct EpiParams {
   const float* bias;
   const float* residual;
@@ -214,46 +231,41 @@ struct EpiParams {
   int Cout, CoutPad, H, W;   // Cout/H/W: NCHW addressing; CoutPad: length of the bias vector
 };
 
-__device__ __forceinline__ void epilogue_sub_tile(const EpiParams& e, float* stage, float (&vv)[32], int lane, bool valid,
-                                                  int m, int n, int oy, int ox, int col0, int col_end) {
-  (void)stage;
-  (void)lane;
+template <int NV>
+__device__ __forceinline__ void epilogue_row(const EpiParams& e, float (&vv)[NV], bool valid, int m, int n, int oy, int ox,
+                                             int col0, int col_end) {
 #pragma unroll
-  for (int j = 0; j < 32; ++j)
+  for (int j = 0; j < NV; ++j)
     if (col0 + j < e.CoutPad) vv[j] += __ldg(e.bias + col0 + j);
-  // Measured on B200 (run 9 vs run 8, profiles/): routing the tile through shared memory so that stores are fully
-  // coalesced (warp_store_rows32) is SLOWER than letting every lane stream its own row with 16-byte stores -- the
-  // lane's consecutive float4 stores fill whole sectors back to back and L2 merges them, while the transpose costs
-  // two shared-memory round trips and 16 shuffles per sub-tile.  The direct path is used; the helpers stay for tests.
   if (e.residual && valid && !e.res_after_relu) {
     const float* r = e.residual + (size_t)m * e.resStride + col0;
 #pragma unroll
-    for (int j = 0; j < 32; ++j)
+    for (int j = 0; j < NV; ++j)
       if (col0 + j < col_end) vv[j] += __ldg(r + j);
   }
   if (e.relu) {
 #pragma unroll
-    for (int j = 0; j < 32; ++j) vv[j] = fmaxf(vv[j], 0.f);
+    for (int j = 0; j < NV; ++j) vv[j] = fmaxf(vv[j], 0.f);
   }
   if (e.residual && valid && e.res_after_relu) {
     const float* r = e.residual + (size_t)m * e.resStride + col0;
 #pragma unroll
-    for (int j = 0; j < 32; ++j)
+    for (int j = 0; j < NV; ++j)
       if (col0 + j < col_end) vv[j] += __ldg(r + j);
   }
   if (e.round_tf32) {
 #pragma unroll
-    for (int j = 0; j < 32; ++j) vv[j] = tf32_round(vv[j]);
+    for (int j = 0; j < NV; ++j) vv[j] = tf32_round(vv[j]);
   }
   if (!valid) return;
   if (e.out_nchw) {
 #pragma unroll
-    for (int j = 0; j < 32; ++j)
+    for (int j = 0; j < NV; ++j)
       if (col0 + j < col_end) e.out[(((size_t)n * e.Cout + col0 + j) * e.H + oy) * e.W + ox] = vv[j];
   } else {
     float* o = e.out + (size_t)m * e.outStride + col0;
 #pragma unroll
-    for (int j = 0; j < 32; j += 4) {
+    for (int j = 0; j < NV; j += 4) {
       if (col0 + j + 3 < col_end) {
         *reinterpret_cast<float4*>(o + j) = make_float4(vv[j], vv[j + 1], vv[j + 2], vv[j + 3]);
       } else {
@@ -263,6 +275,42 @@ __device__ __forceinline__ void epilogue_sub_tile(const EpiParams& e, float* sta
       }
     }
   }
+}
+
+// Row-wise drain of a warpgroup's 64 x BN wgmma accumulator: 32 columns at a time go through `stage` (64 x 33 floats of
+// shared memory owned by the warpgroup); thread t then holds row t / 2, columns 16 (t % 2) .. + 16 of the chunk and
+// calls fn(row, first column, values).  fn runs for every thread and chunk, also where the columns lie past BN (BN = 16).
+constexpr uint32_t DRAIN_STAGE_BYTES = 64u * 33u * 4u;
+template <int BN, class Fn>
+__device__ __forceinline__ void drain_rows(const float (&acc)[BN / 2], float* stage, int wt, int bar_id, Fn&& fn) {
+  const int r0 = (wt >> 5) * 16 + ((wt & 31) >> 2), cq = (wt & 3) * 2;
+#pragma unroll
+  for (int c0 = 0; c0 < BN; c0 += 32) {
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      if (j * 8 >= c0 && j * 8 < c0 + 32) {
+        const int c = j * 8 - c0 + cq;
+        stage[r0 * 33 + c] = acc[4 * j];
+        stage[r0 * 33 + c + 1] = acc[4 * j + 1];
+        stage[(r0 + 8) * 33 + c] = acc[4 * j + 2];
+        stage[(r0 + 8) * 33 + c + 1] = acc[4 * j + 3];
+      }
+    }
+    wg_bar_sync(bar_id);
+    const int r = wt >> 1, h = wt & 1;
+    float v[16];
+#pragma unroll
+    for (int j = 0; j < 16; ++j) v[j] = (c0 + 16 * h + j < BN) ? stage[r * 33 + 16 * h + j] : 0.f;
+    fn(r, c0 + 16 * h, v);
+    wg_bar_sync(bar_id);
+  }
+}
+
+// Largest wgmma N (16 .. 256, a power of two, <= cap) that divides CoutPad (16, 32 or a multiple of 64).
+inline int wgmma_tile_n(int CoutPad, int cap) {
+  for (int n = 256; n >= 16; n >>= 1)
+    if (n <= cap && CoutPad % n == 0) return n;
+  return 0;
 }
 
 }  // namespace umma

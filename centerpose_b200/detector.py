@@ -1,4 +1,4 @@
-"""`ObjectPoseDetector` on the B200-native hot path -- the drop-in for
+"""`ObjectPoseDetector` on the H100-native hot path -- the drop-in for
 /root/reference/src/lib/detectors/{base_detector,object_pose,detector_factory}.py.
 
 `run()` keeps the reference's one-image semantics and its 12-key return dict

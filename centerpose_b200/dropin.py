@@ -1,5 +1,5 @@
 """Make the UNMODIFIED reference entry points (src/demo.py, src/test.py) run on
-the B200-native hot path without editing a reference file.
+the H100-native hot path without editing a reference file.
 
     import centerpose_b200.dropin as dropin
     dropin.install()          # before `from lib.detectors.detector_factory import ...`

@@ -1,4 +1,4 @@
-"""`create_model` / `load_model` / `save_model` for the B200-native CenterPose
+"""`create_model` / `load_model` / `save_model` for the H100-native CenterPose
 network -- the drop-in for /root/reference/src/lib/models/model.py:26-105.
 
 `create_model(arch, heads, head_conv, opt)` returns an `nn.Module` whose
@@ -6,7 +6,7 @@ network -- the drop-in for /root/reference/src/lib/models/model.py:26-105.
 Appendix A: 416 / 439 / 450 keys for dla_34 / dlav1_34 / dla_34-tracking), so
 reference checkpoints load unchanged, and whose
 `forward(x, pre_img=None, pre_hm=None, pre_hm_hp=None) -> [ {head: logits} ]`
-(pose_dla_dcn.py:523-570) runs the hand-written sm_100a plan in
+(pose_dla_dcn.py:523-570) runs the hand-written sm_90a plan in
 libcenterpose_b200.so.  The sub-modules below only HOLD parameters under the
 reference's names; no PyTorch operator ever runs on the hot path and there is
 no CPU fallback -- calling forward without CUDA raises.
@@ -117,11 +117,11 @@ def _flag(opt, name):
 
 
 class DLASegB200(nn.Module):
-    """B200-native DLASeg (pose_dla_dcn.py:457-570).
+    """H100-native DLASeg (pose_dla_dcn.py:457-570).
 
-    `precision` selects the kernels of the plan (include/centerpose_b200.h cp_precision): "tf32x3" (default: tcgen05
+    `precision` selects the kernels of the plan (include/centerpose_b200.h cp_precision): "tf32x3" (default: wgmma
     3-term split with promoted accumulation, fp32-equivalent - meets the same parity bar as "fp32"), "fp32" (CUDA-core
-    FFMA), "tf32" (tcgen05 single pass), "bf16"."""
+    FFMA), "tf32" (wgmma single pass), "bf16"."""
 
     def __init__(self, heads, head_conv=256, use_convGRU=False, opt=None, precision="tf32x3"):
         super().__init__()
@@ -197,7 +197,7 @@ class DLASegB200(nn.Module):
         from .engine import Engine
         device = device if device is not None else next(self.parameters()).device
         if device.type != "cuda":
-            raise RuntimeError("centerpose_b200: the network only runs on CUDA (sm_100a); "
+            raise RuntimeError("centerpose_b200: the network only runs on CUDA (sm_90a); "
                                "there is no CPU fallback -- move the model with .to('cuda')")
         key = (height, width, device.index if device.index is not None else torch.cuda.current_device(), self.precision)
         eng = self._engines.get(key)

@@ -2,7 +2,7 @@
 `demo.py` loop is one synchronous frame at a time: base_detector.py:390-772).
 
 A serving loop has three transfers per batch: frames host -> device, the network + decode on the device, pose records
-device -> host.  Run back to back they serialise (the 25 MB upload of a 32-frame batch is 0.5 ms of a 28 ms step); here
+device -> host.  Run back to back they serialise (a 32-frame batch uploads 25 MB of frames); here
 the upload of batch i+1 runs on a copy stream while batch i computes, and the records of batch i are read back into a
 pinned buffer that the caller collects one submit later:
 

@@ -1,5 +1,5 @@
 /*
- * centerpose_b200.h -- C ABI of libcenterpose_b200.so (sm_100a).
+ * centerpose_b200.h -- C ABI of libcenterpose_b200.so (sm_90a).
  *
  * The drop-in boundary for the CenterPose inference hot path
  * (SURVEY.md section 8b).  Plain pointers and sizes only; every function
@@ -66,11 +66,11 @@ enum cp_arch {
 
 enum cp_precision {
   CP_PREC_FP32 = 0,         /* fp32 operands and accumulation on CUDA cores (parity mode)      */
-  CP_PREC_TF32X3 = 1,       /* tcgen05 kind::tf32, 3-term split + promoted accumulation: fp32-equivalent
+  CP_PREC_TF32X3 = 1,       /* wgmma tf32, 3-term split + promoted accumulation: fp32-equivalent
                              * tensor-core mode, meets the same parity bar as CP_PREC_FP32; the Python host's
                              * default                                                                      */
-  CP_PREC_BF16 = 2,         /* tcgen05 kind::f16 bf16 operands, fp32 accumulation (fast mode)  */
-  CP_PREC_TF32 = 3          /* tcgen05 kind::tf32 single pass -- the math PyTorch's cuDNN convolutions use by
+  CP_PREC_BF16 = 2,         /* wgmma bf16 operands, fp32 accumulation (fast mode)  */
+  CP_PREC_TF32 = 3          /* wgmma tf32 single pass -- the math PyTorch's cuDNN convolutions use by
                              * default (allow_tf32); stride-2 convs run the 3-term split gather kernel     */
 };
 
@@ -332,7 +332,7 @@ int cp_dcn_v2_forward(const float* input, const float* weight, const float* bias
                       const float* offset, const float* mask, float* output,
                       int32_t B, int32_t C, int32_t H, int32_t W, int32_t Co, void* stream);
 
-/* Same op with an explicit cp_precision (CP_PREC_FP32: CUDA cores; CP_PREC_TF32X3 / CP_PREC_BF16: tcgen05). */
+/* Same op with an explicit cp_precision (CP_PREC_FP32: CUDA cores; CP_PREC_TF32X3 / CP_PREC_BF16: wgmma). */
 int cp_dcn_v2_forward_ex(const float* input, const float* weight, const float* bias, const float* offset,
                          const float* mask, float* output, int32_t B, int32_t C, int32_t H, int32_t W,
                          int32_t Co, int32_t precision, void* stream);
@@ -341,7 +341,7 @@ int cp_dcn_v2_forward_ex(const float* input, const float* weight, const float* b
  * kernels dcn_v2_im2col_cuda.cu:197-330).  Inputs as in the forward plus grad_output [B,Co,H,W]; the five gradients
  * (grad_input [B,C,H,W], grad_offset [B,18,H,W], grad_mask [B,9,H,W], grad_weight [Co,C,3,3], grad_bias [Co]) are
  * OVERWRITTEN (the reference returns fresh tensors).  `precision` selects the kernel family of the column-gradient GEMM
- * (CP_PREC_FP32: CUDA cores; CP_PREC_TF32X3: tcgen05, fp32-equivalent); the sampling pass and the weight-gradient GEMM
+ * (CP_PREC_FP32: CUDA cores; CP_PREC_TF32X3: wgmma, fp32-equivalent); the sampling pass and the weight-gradient GEMM
  * run in fp32.  grad_input is accumulated with float atomics (as in the reference), everything else in a fixed order.
  * Scratch (about B*H*W*(11*C + Co + 32) floats) comes from the stream-ordered allocator. */
 int cp_dcn_v2_backward(const float* input, const float* weight, const float* offset, const float* mask,

@@ -1,7 +1,8 @@
-"""ncu CSV (one row per launch x metric) of scripts/profile_target.py -> profiles/<tag>_perlayer_tf32x3.md
+"""ncu CSV (one row per launch x metric) of scripts/profile_target.py -> profiles/<tag>_perlayer_tf32x3.md (kept out of git)
    python scripts/perlayer_table.py gpurun_out/perlayer_r02.csv r02"""
 import collections
 import csv
+import os
 import re
 import sys
 
@@ -20,6 +21,7 @@ for r in rows[1:]:
 ids = sorted(L)
 ids = ids[len(ids) // 2:]                      # second of two forwards
 tot = sum(L[i].get("gpu__time_duration.sum", 0) for i in ids)
+os.makedirs("profiles", exist_ok=True)
 with open("profiles/%s_perlayer_tf32x3.md" % tag, "w") as f:
     f.write("# Per-launch metrics of one forward, tf32x3 (default) mode, batch 32 @ 512x512 (%s)\n\n" % tag)
     f.write("`ncu --metrics gpu__time_duration.sum,sm__pipe_tensor_cycles_active...,l1tex__m_xbar2l1tex_read_bytes.sum,dram__bytes_read.sum,"

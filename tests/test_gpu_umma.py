@@ -1,4 +1,4 @@
-"""tcgen05 tensor-core kernels (igemm_umma.cu) against a plain PyTorch fp32 reference of the same op and
+"""wgmma tensor-core kernels (igemm_umma.cu, conv_tma.cu, dcn_tma.cu) against a plain PyTorch fp32 reference of the same op and
 against the fp32 CUDA-core kernel: layer level (cp_conv2d, cp_dcn_v2_forward_ex) and whole network
 (precision = tf32x3 -- fp32-equivalent -- and bf16 -- fast mode, looser stated tolerance)."""
 import numpy as np
@@ -62,7 +62,7 @@ def test_conv2d_tensor_core(shape, prec, cplib):
     assert (ref32 - want).abs().max().item() / mag <= TOL["fp32"]
     err = (got - want).abs().max().item() / mag
     print("conv %s %s: rel err %.3e" % (shape, prec, err))
-    assert err <= TOL[prec], "tcgen05 %s conv off by %.3e (tolerance %.1e)" % (prec, err, TOL[prec])
+    assert err <= TOL[prec], "wgmma %s conv off by %.3e (tolerance %.1e)" % (prec, err, TOL[prec])
 
 
 @pytest.mark.parametrize("prec", ["tf32x3", "bf16"])
@@ -92,7 +92,7 @@ def test_dcn_tma_staged(prec, off_std, cplib):
     g = torch.Generator().manual_seed(23)
     for (B, C, H, W, Co) in ((2, 64, 16, 16, 64), (1, 32, 8, 32, 48), (1, 128, 8, 64, 128), (1, 16, 8, 128, 16),
                              (2, 64, 24, 48, 64), (3, 64, 32, 32, 256),
-                             (4, 48, 64, 128, 32)):     # 256 tiles > 148 CTAs with an odd number of K blocks
+                             (4, 48, 64, 128, 32)):     # 256 tiles > 132 CTAs with an odd number of K blocks
         x = torch.randn(B, C, H, W, generator=g)
         off = torch.randn(B, 18, H, W, generator=g) * off_std
         mask = torch.rand(B, 9, H, W, generator=g)

@@ -22,16 +22,17 @@ def test_state_dict_matches_reference(arch, trk, key, n):
     assert got == want          # same keys, same shapes, same order
 
 
-def test_state_dict_matches_live_reference(reference):
-    from lib.models.model import create_model as ref_create
-    for arch, trk in (("dla_34", False), ("dlav1_34", False), ("dla_34", True)):
-        ropt = reference.make_opt(arch, tracking_task=trk)
-        r = ref_create(ropt.arch, ropt.heads, ropt.head_conv, ropt)
+def test_state_dict_matches_live_reference():
+    """Heads and state-dict keys / shapes of the reference's create_model from its own options (heads stored by
+    oracle/make_golden_live.py, which also checks state_dict_keys.json against that model)."""
+    from oracle.make_golden_live import MODEL_CONFIGS, STATE_DICT_KEYS
+    heads = json.load(open(os.path.join(GOLD, "live_model_api.json")))["heads"]
+    keys = json.load(open(os.path.join(GOLD, "state_dict_keys.json")))
+    for arch, trk in MODEL_CONFIGS:
         opt = cpb.default_opt(arch, tracking_task=trk)
-        assert list(opt.heads.items()) == list(ropt.heads.items())
+        assert [list(kv) for kv in opt.heads.items()] == heads["%s_%d" % (arch, trk)]
         m = cpb.create_model(opt.arch, opt.heads, opt.head_conv, opt)
-        assert [(k, tuple(v.shape)) for k, v in m.state_dict().items()] == \
-               [(k, tuple(v.shape)) for k, v in r.state_dict().items()]
+        assert [[k, list(v.shape)] for k, v in m.state_dict().items()] == keys[STATE_DICT_KEYS[(arch, trk)]]
 
 
 def test_save_load_roundtrip(tmp_path, capsys):
@@ -90,15 +91,15 @@ def test_dropin_registers_reference_module_names():
                 sys.modules[k] = v
 
 
-def test_default_opt_matches_reference(reference):
-    for arch, trk, rep in (("dla_34", False, 1), ("dla_34", True, 1), ("dlav1_34", False, 0)):
-        r = reference.make_opt(arch, tracking_task=trk, rep_mode=rep)
+def test_default_opt_matches_reference():
+    """The reference's default options per configuration (stored by oracle/make_golden_live.py)."""
+    from oracle.make_golden_live import OPT_CONFIGS, OPT_FIELDS, jsonable
+    ref = json.load(open(os.path.join(GOLD, "live_model_api.json")))["opts"]
+    for arch, trk, rep in OPT_CONFIGS:
+        r = ref["%s_%d_%d" % (arch, trk, rep)]
         o = cpb.default_opt(arch, tracking_task=trk, rep_mode=rep)
-        for f in ("K", "rep_mode", "vis_thresh", "nms", "use_pnp", "head_conv", "down_ratio", "mean", "std", "c",
-                  "input_h", "input_w", "num_classes", "test_scales", "fix_res", "hm_hp", "reg_offset",
-                  "reg_hp_offset", "tracking_task", "hps_uncertainty", "obj_scale_uncertainty"):
-            assert getattr(o, f) == getattr(r, f), f
-        assert o.balance_coefficient == r.balance_coefficient
+        for f in OPT_FIELDS:
+            assert jsonable(getattr(o, f)) == r[f], f
 
 
 def test_seeded_weights_are_deterministic():

@@ -1,6 +1,6 @@
-"""Pins oracle/net_ref.py (the CPU fp32 restatement of the network) against
-(a) the golden head tensors the unmodified reference produced
-(tests/golden/net_*.npz) and (b) the live reference when it is present."""
+"""Pins oracle/net_ref.py (the CPU fp32 restatement of the network) against the golden head tensors the unmodified
+reference produced: tests/golden/net_*.npz (oracle/make_golden.py; oracle/make_golden_live.py checks that CASES[0] is
+also what the reference model built from its own default options computes)."""
 import numpy as np
 import pytest
 import torch
@@ -35,17 +35,17 @@ def test_oracle_matches_reference_golden(name):
         assert np.abs(got - want).max() <= 2e-5 * max(1.0, np.abs(want).max()), h
 
 
-def test_oracle_matches_live_reference(reference):
-    from lib.models.model import create_model as ref_create
-    g = golden(CASES[0])
-    out, opt, sd, x, extra = _run_oracle(g)
-    ropt = reference.make_opt("dla_34")
-    ref = ref_create(ropt.arch, ropt.heads, ropt.head_conv, ropt).eval()
-    ref.load_state_dict(sd, strict=True)
-    with torch.no_grad():
-        want = ref(torch.from_numpy(x))[-1]
-    for h in want:
-        assert (want[h] - out[h]).abs().max().item() <= 2e-5 * max(1.0, want[h].abs().max().item())
+def test_oracle_matches_live_reference():
+    """The reference's create_model(arch, heads, head_conv, opt) from its own default options, on the weights and input
+    of CASES[0]: its heads are the ones stored in CASES[0] (checked bit for bit by oracle/make_golden_live.py)."""
+    out, opt, _, _, _ = _run_oracle(golden(CASES[0]))
+    ref = golden(CASES[0])
+    ref = {f: ref[f] for f in ref.files if f.startswith("head_")}
+    assert sorted(f[len("head_"):] for f in ref) == sorted(opt.heads)
+    for h in opt.heads:
+        want = torch.from_numpy(ref["head_" + h])
+        assert want.shape == out[h].shape, h
+        assert (want - out[h]).abs().max().item() <= 2e-5 * max(1.0, want.abs().max().item()), h
 
 
 def test_dcn_restatement_matches_reference_cpp():
