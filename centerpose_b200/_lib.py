@@ -37,6 +37,11 @@ CP_TRACK_RECORD = 320
 T_ID, T_AGE, T_ACTIVE, T_IN_BOXES, T_PNP2_STATUS, T_CONF_AVG = 192, 193, 194, 195, 196, 197
 T_KPS_FUSION_MEAN, T_KPS_FUSION_STD, T_KPS_MEAN_KF, T_KPS_STD_KF = 200, 216, 232, 248
 T_OBJ_SCALE_KF, T_OBJ_SCALE_UNC_KF, T_KPS_PNP_KF, T_KPS_3D_CAM_KF = 264, 267, 270, 288
+# cp_seed_field
+CP_SEED_RECORD = 264
+S_KPS_FUSION_MEAN, S_KPS_FUSION_STD, S_KPS_GT, S_HAS_CT, S_HAS_KPS_GT, S_KPS_PNP_KF, S_HAS_KPS_PNP_KF = 192, 208, 224, 242, 243, 244, 262
+# cp_render_mode
+RENDER_TRACKS, RENDER_GT, RENDER_EMPTY = 0, 1, 2
 # cp_pnp_status
 PNP_NOT_RUN, PNP_OK, PNP_INVISIBLE, PNP_BEHIND, PNP_FEW_POINTS, PNP_SOLVER_FAIL = 0, 1, 2, 3, 4, 5
 
@@ -46,6 +51,7 @@ EXPORTS = [
     "cp_decode_pnp", "cp_infer", "cp_dcn_v2_forward", "cp_preprocess", "cp_plan_num_ops", "cp_plan_profile",
     "cp_dcn_v2_forward_ex", "cp_conv2d", "cp_dcn_v2_backward",
     "cp_preprocess_affine", "cp_tracker_create", "cp_tracker_destroy", "cp_tracker_reset", "cp_tracker_step", "cp_tracker_render",
+    "cp_tracker_render_ex", "cp_tracker_seed",
 ]
 
 
@@ -87,7 +93,8 @@ class CpTrackerConfig(ctypes.Structure):
     _fields_ = [(n, ctypes.c_int32) for n in (
         "streams", "max_tracks", "kalman", "scale_pool", "use_pnp", "hps_uncertainty", "max_age", "visible_thresh",
         "opencv_return", "render_hm_mode", "render_hmhp_mode", "device")] + [
-        (n, ctypes.c_float) for n in ("new_thresh", "pre_thresh", "R", "conf_lo", "conf_hi")]
+        (n, ctypes.c_float) for n in ("new_thresh", "pre_thresh", "R", "conf_lo", "conf_hi")] + [
+        ("hungarian", ctypes.c_int32)]
 
 
 _lib = None
@@ -141,6 +148,8 @@ def load():
     L.cp_tracker_reset.argtypes = [vp, i32, vp]
     L.cp_tracker_step.argtypes = [vp, i32, vp, vp, i32, vp, vp, vp, vp]
     L.cp_tracker_render.argtypes = [vp, i32, vp, vp, i32, i32, vp, vp, vp]
+    L.cp_tracker_render_ex.argtypes = [vp, i32, vp, vp, i32, i32, ctypes.POINTER(i32), vp, vp, vp]
+    L.cp_tracker_seed.argtypes = [vp, i32, vp, vp, i32, vp]
     for name in EXPORTS:
         fn = getattr(L, name)
         if name not in ("cp_version", "cp_last_error", "cp_plan_bytes", "cp_plan_forward_launches",

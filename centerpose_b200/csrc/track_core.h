@@ -7,7 +7,9 @@
 //   utils/tracker.py:55-84               init_kf: 32-state constant-velocity filter = 8 keypoints x (x, y, vx, vy)
 //   utils/tracker.py:86-101              update_kf (measurement = fused keypoints + the negated tracking_hp offsets)
 //   utils/tracker.py:103-116             update_scale_pool (inverse-variance fusion of the scale history)
-//   utils/tracker.py:118-236             step: association (greedy, :304-314), matched / new / lost tracks
+//   utils/tracker.py:21-48               init_track with meta['pre_dets'] (ground-truth seeding)
+//   utils/tracker.py:118-236             step: association (greedy :304-314 or optimal :154-177), matched / new / lost
+//                                        tracks
 //   utils/tracker.py:238-262             filter read-out, keypoint confidence from the filter covariance
 //   utils/image.py:102-150               gaussian_radius / gaussian2D / draw_umich_gaussian (previous-frame heat maps)
 // filterpy.kalman.KalmanFilter (third party, requirements.txt: filterpy>=1.4.5): predict x = F x, P = F P F^T + Q with
@@ -29,6 +31,7 @@ namespace track {
 struct Cfg {
   int kalman, scale_pool, use_pnp, hps_uncertainty, max_age;
   double new_thresh, R, conf_lo, conf_hi;      // opt.new_thresh, opt.R, opt.conf_border[opt.c]
+  int hungarian;                               // opt.hungarian
 };
 
 // per-track filter state that is not part of the fp32 pose record
@@ -198,6 +201,22 @@ CP_HD float cp_f_noinline_add(volatile float a, volatile float b) { return a + b
 #define CP_FADD(a, b) cp_f_noinline_add(a, b)
 #endif
 
+// dist[i][j] of tracker.py:146-152: float32 squared distance, + 1e18 (float64) where the pair is invalid
+CP_HD double pair_cost(const float* det_c, const float* det_size, const int* det_cls, const float* trk_c,
+                       const float* trk_size, const int* trk_cls, int i, int j) {
+  const float dx = CP_FSUB(trk_c[2 * j], det_c[2 * i]), dy = CP_FSUB(trk_c[2 * j + 1], det_c[2 * i + 1]);
+  const float d = CP_FADD(CP_FMUL(dx, dx), CP_FMUL(dy, dy));
+  const bool invalid = (d > trk_size[j]) || (d > det_size[i]) || (det_cls[i] != trk_cls[j]);
+  return (double)d + (invalid ? 1e18 : 0.0);
+}
+
+// the Hungarian branch clips the matrix first (tracker.py:156: dist[dist > 1e18] = 1e18)
+CP_HD double clipped_cost(const float* det_c, const float* det_size, const int* det_cls, const float* trk_c,
+                          const float* trk_size, const int* trk_cls, int i, int j) {
+  const double d = pair_cost(det_c, det_size, det_cls, trk_c, trk_size, trk_cls, i, j);
+  return d > 1e18 ? 1e18 : d;
+}
+
 // det_c: N x 2 (ct + tracking, float32), det_size / det_cls: N;  trk_c: M x 2, trk_size / trk_cls: M
 // match_of_det[i] = matched track or -1;  det_of_trk[j] = matched detection or -1.  `taken` is M bytes of scratch.
 CP_HDN void greedy_associate(const float* det_c, const float* det_size, const int* det_cls, int N, const float* trk_c,
@@ -212,10 +231,7 @@ CP_HDN void greedy_associate(const float* det_c, const float* det_size, const in
     int best = -1;
     double bd = 0.0;
     for (int j = 0; j < M; ++j) {
-      const float dx = CP_FSUB(trk_c[2 * j], det_c[2 * i]), dy = CP_FSUB(trk_c[2 * j + 1], det_c[2 * i + 1]);
-      const float d = CP_FADD(CP_FMUL(dx, dx), CP_FMUL(dy, dy));
-      const bool invalid = (d > trk_size[j]) || (d > det_size[i]) || (det_cls[i] != trk_cls[j]);
-      double dd = (double)d + (invalid ? 1e18 : 0.0);
+      double dd = pair_cost(det_c, det_size, det_cls, trk_c, trk_size, trk_cls, i, j);
       if (taken[j]) dd = 1e18;              // column already assigned (dist[:, j] = 1e18)
       if (best < 0 || dd < bd) {            // argmin keeps the FIRST minimum
         best = j;
@@ -230,6 +246,125 @@ CP_HDN void greedy_associate(const float* det_c, const float* det_size, const in
   }
 }
 
+// ---- optimal association (tracker.py:154-177, opt.hungarian) --------------------------------------------------------
+// The reference calls sklearn 0.22's linear_assignment; the oracle stands in for it with
+// scipy.optimize.linear_sum_assignment, and this is scipy's solver (shortest augmenting paths with potentials, Crouse
+// 2016), restated so that the same pairs come out, ties included: fp64 potentials u / v, one Dijkstra search per row,
+// columns scanned in the order of a `remaining` list that starts reversed and shrinks by swap-with-last, and the scan's
+// tie rule "the first minimum, unless a later equal one is an unassigned column".  Rows are the smaller side (scipy
+// transposes a tall matrix).  The matrix is never stored: the cost functor recomputes entries.
+struct LsaWork {
+  double u[CP_MAX_K], v[CP_MAX_K], spc[CP_MAX_K];      // row / column potentials, shortest path cost per column
+  int path[CP_MAX_K], col4row[CP_MAX_K], row4col[CP_MAX_K], remaining[CP_MAX_K];
+  unsigned char SR[CP_MAX_K], SC[CP_MAX_K];
+};
+
+// the rows x cols view of the clipped N x M dist matrix
+struct LsaCost {
+  const float *det_c, *det_size, *trk_c, *trk_size;
+  const int *det_cls, *trk_cls;
+  int transpose;             // rows = tracks (N > M)
+  CP_HD double operator()(int r, int c) const {
+    return transpose ? clipped_cost(det_c, det_size, det_cls, trk_c, trk_size, trk_cls, c, r)
+                     : clipped_cost(det_c, det_size, det_cls, trk_c, trk_size, trk_cls, r, c);
+  }
+};
+
+CP_HD void lsa_init(LsaWork* w, int nr, int nc) {
+  for (int i = 0; i < nr; ++i) {
+    w->u[i] = 0.0;
+    w->col4row[i] = -1;
+  }
+  for (int j = 0; j < nc; ++j) {
+    w->v[j] = 0.0;
+    w->row4col[j] = -1;
+    w->path[j] = -1;
+  }
+}
+
+CP_HD void lsa_begin_row(LsaWork* w, int nr, int nc) {
+  for (int it = 0; it < nc; ++it) w->remaining[it] = nc - it - 1;
+  for (int i = 0; i < nr; ++i) w->SR[i] = 0;
+  for (int j = 0; j < nc; ++j) {
+    w->SC[j] = 0;
+    w->spc[j] = INFINITY;
+  }
+}
+
+// after the search of row `cur` reached `sink`: update the potentials, then augment along `path`
+CP_HD void lsa_finish_row(LsaWork* w, int nr, int nc, int cur, int sink, double minVal) {
+  w->u[cur] += minVal;
+  for (int i = 0; i < nr; ++i)
+    if (w->SR[i] && i != cur) w->u[i] += minVal - w->spc[w->col4row[i]];
+  for (int j = 0; j < nc; ++j)
+    if (w->SC[j]) w->v[j] -= minVal - w->spc[j];
+  int j = sink;
+  while (true) {
+    const int i = w->path[j];
+    w->row4col[j] = i;
+    const int t = w->col4row[i];
+    w->col4row[i] = j;
+    j = t;
+    if (i == cur) break;
+  }
+}
+
+// serial solver (nr <= nc <= CP_MAX_K): col4row[r] = the column of row r.  Returns false on an infeasible matrix (an
+// infinite cost; never the case for dist, whose entries are at most 1e18)
+template <class Cost>
+CP_HDN bool lsa_solve(const Cost& cost, int nr, int nc, LsaWork* w) {
+  lsa_init(w, nr, nc);
+  for (int cur = 0; cur < nr; ++cur) {
+    lsa_begin_row(w, nr, nc);
+    int nrem = nc, i = cur, sink = -1;
+    double minVal = 0.0;
+    while (sink < 0) {
+      int index = -1;
+      double lowest = INFINITY;
+      w->SR[i] = 1;
+      for (int it = 0; it < nrem; ++it) {
+        const int j = w->remaining[it];
+        const double r = minVal + cost(i, j) - w->u[i] - w->v[j];
+        if (r < w->spc[j]) {
+          w->path[j] = i;
+          w->spc[j] = r;
+        }
+        if (w->spc[j] < lowest || (w->spc[j] == lowest && w->row4col[j] == -1)) {
+          lowest = w->spc[j];
+          index = it;
+        }
+      }
+      minVal = lowest;
+      if (index < 0 || minVal == INFINITY) return false;
+      const int j = w->remaining[index];
+      if (w->row4col[j] == -1)
+        sink = j;
+      else
+        i = w->row4col[j];
+      w->SC[j] = 1;
+      w->remaining[index] = w->remaining[--nrem];
+    }
+    lsa_finish_row(w, nr, nc, cur, sink, minVal);
+  }
+  return true;
+}
+
+// scipy's pairs and the post-filter of tracker.py:166-177 (a pair costing more than 1e16 is dropped).
+// match_of_det[i] = j for a kept pair, -2 - j for a dropped one, -1 when unassigned; det_of_trk[j] likewise.
+CP_HD void lsa_pairs(const LsaCost& cost, int N, int M, const LsaWork* w, int* match_of_det, int* det_of_trk) {
+  for (int i = 0; i < N; ++i) match_of_det[i] = -1;
+  for (int j = 0; j < M; ++j) det_of_trk[j] = -1;
+  if (N == 0 || M == 0) return;
+  const int nr = cost.transpose ? M : N;
+  for (int r = 0; r < nr; ++r) {
+    const int c = w->col4row[r];
+    if (c < 0) continue;
+    const int i = cost.transpose ? c : r, j = cost.transpose ? r : c;
+    const bool drop = cost(r, c) > 1e16;
+    match_of_det[i] = drop ? -2 - j : j;
+    det_of_trk[j] = drop ? -2 - i : i;
+  }
+}
 
 // ---- one track ------------------------------------------------------------------------------------------------------
 struct Slot {
@@ -239,6 +374,8 @@ struct Slot {
   float kps_pnp_kf[18];          // its 9 normalised projected points (centre first)
   double fus_mean[16], fus_std[16];
   Filter f;
+  int has_gt;                    // seeded from a dict with 'kps_gt' (drawn by the ground-truth render)
+  float kps_gt[18];              // its 9 normalised points (centre first)
 };
 
 CP_HD void slot_fusion(const Cfg& c, Slot* s) {
@@ -264,6 +401,7 @@ CP_HDN void entry_matched(const Cfg& c, Slot* dst, const Slot* old, const float*
   dst->active = old->active + 1;
   dst->has_kf = old->has_kf;
   dst->has_pnp_kf = 0;
+  dst->has_gt = 0;
   dst->f = old->f;
   slot_fusion(c, dst);
   if (c.kalman) {
@@ -281,7 +419,39 @@ CP_HDN void entry_new(const Cfg& c, Slot* dst, const float* rec, int id) {
   dst->active = 1;
   dst->has_kf = 0;
   dst->has_pnp_kf = 0;
+  dst->has_gt = 0;
   slot_fusion(c, dst);
+  for (int i = 0; i < 32; ++i) dst->f.x[i] = 0.0;
+  for (int i = 0; i < 8; ++i)
+    for (int e = 0; e < 16; ++e) dst->f.P[i][e] = 0.0;
+  for (int k = 0; k < 3; ++k) dst->f.sp_w[k] = dst->f.sp_m[k] = 0.0;
+  if (c.kalman) {
+    for (int i = 0; i < 8; ++i) kf_init_kp(&dst->f, i, dst->fus_mean, dst->fus_std, dst->rec + CP_P_TRACKING_HP, c.R);
+    dst->has_kf = 1;
+  }
+  if (c.scale_pool) scale_pool_add(dst, true);
+}
+
+// init_track (tracker.py:31-49): one dict of meta['pre_dets'] (cp_seed_field layout) starts track `id`.  The filter
+// starts from the dict's own kps_fusion_mean / kps_fusion_std, which are not re-derived through gaussian_fusion.
+CP_HDN void entry_seed(const Cfg& c, Slot* dst, const float* seed, int id) {
+  for (int i = 0; i < CP_POSE_RECORD; ++i) dst->rec[i] = seed[i];
+  if (seed[CP_S_HAS_CT] == 0.f) {
+    dst->rec[CP_P_CT] = (float)(((double)seed[CP_P_BBOX] + (double)seed[CP_P_BBOX + 2]) / 2);
+    dst->rec[CP_P_CT + 1] = (float)(((double)seed[CP_P_BBOX + 1] + (double)seed[CP_P_BBOX + 3]) / 2);
+  }
+  dst->id = id;
+  dst->age = 1;
+  dst->active = 1;
+  dst->has_kf = 0;
+  dst->has_pnp_kf = seed[CP_S_HAS_KPS_PNP_KF] != 0.f ? 1 : 0;
+  for (int t = 0; t < 18; ++t) dst->kps_pnp_kf[t] = dst->has_pnp_kf ? seed[CP_S_KPS_PNP_KF + t] : 0.f;
+  dst->has_gt = seed[CP_S_HAS_KPS_GT] != 0.f ? 1 : 0;
+  for (int t = 0; t < 18; ++t) dst->kps_gt[t] = seed[CP_S_KPS_GT + t];
+  for (int i = 0; i < 16; ++i) {
+    dst->fus_mean[i] = (double)seed[CP_S_KPS_FUSION_MEAN + i];
+    dst->fus_std[i] = (double)seed[CP_S_KPS_FUSION_STD + i];
+  }
   for (int i = 0; i < 32; ++i) dst->f.x[i] = 0.0;
   for (int i = 0; i < 8; ++i)
     for (int e = 0; e < 16; ++e) dst->f.P[i][e] = 0.0;
@@ -390,11 +560,10 @@ struct Entry {
   int kind, det, trk, id;
 };
 
-// poses: n_valid records of this frame; old: M tracks.  Scratch: det_idx[K], fbuf[3 * (K + M)] floats, ibuf[2 * K + 2 * M]
-// ints, taken[M].  Returns the number of entries written (<= max_entries); *id_count is advanced for every new track.
-CP_HDN int plan_step(const Cfg& c, const float* poses, int n_valid, const Slot* old, int M, int* id_count, Entry* entries,
-                     int max_entries, int* det_idx, float* fbuf, int* ibuf, unsigned char* taken) {
-  // Step 0 (tracker.py:121-130): with PnP on and at least one solved box, only the solved detections are tracked
+// Step 0 (tracker.py:121-130) and the arrays of Step 1: with PnP on and at least one solved box, only the solved
+// detections are tracked.  Scratch: det_idx[K], fbuf[3 * (K + M)] floats, ibuf[2 * K + 2 * M] ints.  Returns N.
+CP_HDN int plan_stage(const Cfg& c, const float* poses, int n_valid, const Slot* old, int M, int* det_idx, float* fbuf,
+                      int* ibuf) {
   int N = 0;
   bool any_box = false;
   if (c.use_pnp)
@@ -407,8 +576,6 @@ CP_HDN int plan_step(const Cfg& c, const float* poses, int n_valid, const Slot* 
   float* trk_size = trk_c + 2 * M;
   int* det_cls = ibuf;
   int* trk_cls = det_cls + N;
-  int* match_of_det = trk_cls + M;
-  int* det_of_trk = match_of_det + N;
   for (int i = 0; i < N; ++i) {
     const float* r = poses + (size_t)det_idx[i] * CP_POSE_RECORD;
     det_c[2 * i] = (float)((double)r[CP_P_CT] + (double)r[CP_P_TRACKING]);
@@ -423,18 +590,61 @@ CP_HDN int plan_step(const Cfg& c, const float* poses, int n_valid, const Slot* 
     trk_size[j] = (float)(((double)r[CP_P_BBOX + 2] - (double)r[CP_P_BBOX]) * ((double)r[CP_P_BBOX + 3] - (double)r[CP_P_BBOX + 1]));
     trk_cls[j] = (int)r[CP_P_CLS];
   }
-  greedy_associate(det_c, det_size, det_cls, N, trk_c, trk_size, trk_cls, M, match_of_det, det_of_trk, taken);
+  return N;
+}
+
+// the staged arrays of plan_stage as the solver's cost view
+CP_HD LsaCost plan_cost(const float* fbuf, const int* ibuf, int N, int M) {
+  LsaCost v;
+  v.det_c = fbuf;
+  v.det_size = fbuf + 2 * N;
+  v.trk_c = v.det_size + N;
+  v.trk_size = v.trk_c + 2 * M;
+  v.det_cls = ibuf;
+  v.trk_cls = ibuf + N;
+  v.transpose = N > M;
+  return v;
+}
+
+// Steps 2-4 as a list: matched pairs in row order; then new tracks over unmatched_dets = the unassigned detections in
+// order followed by those of dropped pairs (in row order); then lost tracks over unmatched_tracks, built the same way.
+// Without dropped pairs (greedy) this is the plain row / column order.  *id_count advances for every new track.
+CP_HDN int plan_entries(const Cfg& c, const float* poses, const int* det_idx, int N, const Slot* old, int M,
+                        const int* match_of_det, const int* det_of_trk, int* id_count, Entry* entries, int max_entries) {
   int n = 0;
   for (int i = 0; i < N && n < max_entries; ++i)
     if (match_of_det[i] >= 0) entries[n++] = Entry{ENTRY_MATCHED, det_idx[i], match_of_det[i], 0};
-  for (int i = 0; i < N && n < max_entries; ++i)
-    if (match_of_det[i] < 0 && (double)poses[(size_t)det_idx[i] * CP_POSE_RECORD + CP_P_SCORE] > c.new_thresh) {
-      *id_count += 1;
-      entries[n++] = Entry{ENTRY_NEW, det_idx[i], -1, *id_count};
-    }
+  for (int pass = 0; pass < 2; ++pass)
+    for (int i = 0; i < N && n < max_entries; ++i)
+      if ((pass == 0 ? match_of_det[i] == -1 : match_of_det[i] < -1) &&
+          (double)poses[(size_t)det_idx[i] * CP_POSE_RECORD + CP_P_SCORE] > c.new_thresh) {
+        *id_count += 1;
+        entries[n++] = Entry{ENTRY_NEW, det_idx[i], -1, *id_count};
+      }
   for (int j = 0; j < M && n < max_entries; ++j)
-    if (det_of_trk[j] < 0 && old[j].age < c.max_age) entries[n++] = Entry{ENTRY_LOST, -1, j, 0};
+    if (det_of_trk[j] == -1 && old[j].age < c.max_age) entries[n++] = Entry{ENTRY_LOST, -1, j, 0};
+  for (int i = 0; i < N && n < max_entries; ++i)
+    if (match_of_det[i] < -1 && old[-2 - match_of_det[i]].age < c.max_age)
+      entries[n++] = Entry{ENTRY_LOST, -1, -2 - match_of_det[i], 0};
   return n;
+}
+
+// poses: n_valid records of this frame; old: M tracks.  Scratch: det_idx[K], fbuf[3 * (K + M)] floats, ibuf[2 * K + 2 * M]
+// ints, taken[M], and with c.hungarian the solver's `lsa`.  Returns the number of entries written (<= max_entries);
+// *id_count is advanced for every new track.
+CP_HDN int plan_step(const Cfg& c, const float* poses, int n_valid, const Slot* old, int M, int* id_count, Entry* entries,
+                     int max_entries, int* det_idx, float* fbuf, int* ibuf, unsigned char* taken, LsaWork* lsa = nullptr) {
+  const int N = plan_stage(c, poses, n_valid, old, M, det_idx, fbuf, ibuf);
+  const LsaCost v = plan_cost(fbuf, ibuf, N, M);
+  int* match_of_det = ibuf + N + M;
+  int* det_of_trk = match_of_det + N;
+  if (c.hungarian) {
+    if (N > 0 && M > 0) lsa_solve(v, v.transpose ? M : N, v.transpose ? N : M, lsa);
+    lsa_pairs(v, N, M, lsa, match_of_det, det_of_trk);
+  } else {
+    greedy_associate(v.det_c, v.det_size, v.det_cls, N, v.trk_c, v.trk_size, v.trk_cls, M, match_of_det, det_of_trk, taken);
+  }
+  return plan_entries(c, poses, det_idx, N, old, M, match_of_det, det_of_trk, id_count, entries, max_entries);
 }
 
 // ---- previous-frame heat maps (base_detector.py:150-388) -----------------------------------------------------------------

@@ -19,6 +19,9 @@ struct cp_tracker {
   Slot* slots[2] = {nullptr, nullptr};      // [streams][max_tracks], ping-pong: slots[cur] = current tracks
   int* n_tracks[2] = {nullptr, nullptr};    // [streams]
   int* id_count = nullptr;                  // [streams]
+  int* modes = nullptr;                     // [streams] render modes of the latest cp_tracker_render_ex
+  void* plan = nullptr;                     // hungarian: [streams][max_tracks] Entry of the association kernel
+  int* plan_n = nullptr;                    // hungarian: [streams]
   int cur = 0;
 };
 
@@ -41,7 +44,141 @@ struct StepArgs {
   int* id_count;
   float* tracks_out;        // [B, T, 320]
   int* n_out;               // [B]
+  Entry* plan;              // hungarian: [B, T] entries written by tracker_assoc_kernel, else nullptr
+  int* plan_n;              // hungarian: [B]
 };
+
+// the Dijkstra scan of lsa_solve spread over the CTA: thread t relaxes column remaining[t] (nc <= CP_MAX_K <=
+// TRK_THREADS) and the serial scan's choice becomes a reduction over (value, key): the smaller value wins, equal values
+// go to the larger key, key = 256 + t for an unassigned column (the last one of the scan wins) and 255 - t otherwise
+// (the first one wins), so the same column is picked as by the left-to-right scan of lsa_solve.
+struct LsaSync {
+  double val[TRK_THREADS / 32];
+  int key[TRK_THREADS / 32];
+  double minVal;
+  int i, sink, nrem;
+};
+static_assert(CP_MAX_K <= TRK_THREADS && CP_MAX_K < 256, "one column per thread, keys below 256");
+
+__device__ __forceinline__ void lsa_pick(double& best, int& key, double ob, int ok) {
+  if (ob < best || (ob == best && ok > key)) {
+    best = ob;
+    key = ok;
+  }
+}
+
+__device__ void lsa_solve_cta(const LsaCost& cost, int nr, int nc, LsaWork* w, LsaSync* sy) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, NW = TRK_THREADS / 32;
+  if (tid == 0) lsa_init(w, nr, nc);
+  for (int cur = 0; cur < nr; ++cur) {
+    __syncthreads();
+    for (int t = tid; t < nc; t += TRK_THREADS) {
+      w->remaining[t] = nc - t - 1;
+      w->SC[t] = 0;
+      w->spc[t] = INFINITY;
+    }
+    for (int t = tid; t < nr; t += TRK_THREADS) w->SR[t] = 0;
+    if (tid == 0) {
+      sy->i = cur;
+      sy->sink = -1;
+      sy->nrem = nc;
+      sy->minVal = 0.0;
+    }
+    __syncthreads();
+    while (true) {
+      const int i = sy->i, nrem = sy->nrem;
+      const double minVal = sy->minVal;
+      double best = INFINITY;
+      int key = -1;
+      if (tid < nrem) {
+        const int j = w->remaining[tid];
+        const double r = minVal + cost(i, j) - w->u[i] - w->v[j];
+        double sp = w->spc[j];
+        if (r < sp) {
+          w->path[j] = i;
+          w->spc[j] = r;
+          sp = r;
+        }
+        best = sp;
+        key = w->row4col[j] == -1 ? 256 + tid : 255 - tid;
+      }
+      for (int o = 16; o > 0; o >>= 1) lsa_pick(best, key, __shfl_down_sync(0xffffffffu, best, o), __shfl_down_sync(0xffffffffu, key, o));
+      if (lane == 0) {
+        sy->val[warp] = best;
+        sy->key[warp] = key;
+      }
+      __syncthreads();
+      if (tid == 0) {
+        for (int q = 1; q < NW; ++q) lsa_pick(best, key, sy->val[q], sy->key[q]);
+        const int index = key >= 256 ? key - 256 : 255 - key;
+        const int j = w->remaining[index];
+        w->SR[i] = 1;
+        sy->minVal = best;
+        if (w->row4col[j] == -1)
+          sy->sink = j;
+        else
+          sy->i = w->row4col[j];
+        w->SC[j] = 1;
+        w->remaining[index] = w->remaining[nrem - 1];
+        sy->nrem = nrem - 1;
+      }
+      __syncthreads();
+      if (sy->sink >= 0) break;
+    }
+    // lsa_finish_row: potentials in parallel, the augmentation (a few steps) on thread 0
+    const double minVal = sy->minVal;
+    for (int t = tid; t < nr; t += TRK_THREADS)
+      if (w->SR[t] && t != cur) w->u[t] += minVal - w->spc[w->col4row[t]];
+    for (int t = tid; t < nc; t += TRK_THREADS)
+      if (w->SC[t]) w->v[t] -= minVal - w->spc[t];
+    __syncthreads();
+    if (tid == 0) {
+      w->u[cur] += minVal;
+      int j = sy->sink;
+      while (true) {
+        const int i = w->path[j];
+        w->row4col[j] = i;
+        const int t = w->col4row[i];
+        w->col4row[i] = j;
+        j = t;
+        if (i == cur) break;
+      }
+    }
+  }
+  __syncthreads();
+}
+
+// Steps 0-1 with the optimal assignment, one CTA per stream: staging and the order of `ret` on thread 0, the solver on
+// the CTA.  A kernel of its own so that the step kernel's register allocation stays as it is; the step kernel then
+// reads the entries from a.plan.
+__global__ void __launch_bounds__(TRK_THREADS, 1) tracker_assoc_kernel(const StepArgs a) {
+  const int b = blockIdx.x, tid = threadIdx.x;
+  __shared__ int det_idx[TRK_MAXK];
+  __shared__ float fbuf[3 * 2 * TRK_MAXK];
+  __shared__ int ibuf[4 * TRK_MAXK];
+  __shared__ LsaWork lsa;
+  __shared__ LsaSync sync;
+  __shared__ int s_N;
+  const float* poses = a.poses + (size_t)b * a.K * CP_POSE_RECORD;
+  const Slot* old = a.old_slots + (size_t)b * a.T;
+  const int M = a.old_n[b];
+  int nv = a.n_valid[b];
+  if (nv > a.K) nv = a.K;
+  if (nv < 0) nv = 0;
+  if (tid == 0) s_N = plan_stage(a.cfg, poses, nv, old, M, det_idx, fbuf, ibuf);
+  __syncthreads();
+  const int N = s_N;
+  const LsaCost v = plan_cost(fbuf, ibuf, N, M);
+  if (N > 0 && M > 0) lsa_solve_cta(v, v.transpose ? M : N, v.transpose ? N : M, &lsa, &sync);
+  if (tid == 0) {
+    int* match_of_det = ibuf + N + M;
+    int* det_of_trk = match_of_det + N;
+    lsa_pairs(v, N, M, &lsa, match_of_det, det_of_trk);
+    int idc = a.id_count[b];
+    a.plan_n[b] = plan_entries(a.cfg, poses, det_idx, N, old, M, match_of_det, det_of_trk, &idc, a.plan + (size_t)b * a.T, a.T);
+    a.id_count[b] = idc;
+  }
+}
 
 __global__ void __launch_bounds__(TRK_THREADS, 1) tracker_step_kernel(const StepArgs a) {
   const int b = blockIdx.x, tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, NW = TRK_THREADS / 32;
@@ -61,8 +198,12 @@ __global__ void __launch_bounds__(TRK_THREADS, 1) tracker_step_kernel(const Step
   if (nv > a.K) nv = a.K;
   if (nv < 0) nv = 0;
 
-  // Steps 0-1 and the order of `ret` (serial, a few hundred operations)
-  if (tid == 0) {
+  if (a.plan) {
+    const int n = a.plan_n[b];
+    for (int e = tid; e < n; e += TRK_THREADS) entries[e] = a.plan[(size_t)b * a.T + e];
+    if (tid == 0) s_n = n;
+  } else if (tid == 0) {
+    // Steps 0-1 and the order of `ret` (serial, a few hundred operations)
     int idc = a.id_count[b];
     s_n = plan_step(a.cfg, poses, nv, old, M, &idc, entries, a.T, det_idx, fbuf, ibuf, taken);
     a.id_count[b] = idc;
@@ -129,6 +270,29 @@ __global__ void tracker_reset_kernel(int* n0, int* n1, int* id_count, int stream
   }
 }
 
+// init_track with meta['pre_dets'] (tracker.py:21-48), one CTA per stream; seeds go into the current slots
+__global__ void __launch_bounds__(128) tracker_seed_kernel(const Cfg cfg, int T, const float* seeds, const int* n_seeds,
+                                                            int S, Slot* slots, int* n_tracks, int* id_count) {
+  const int b = blockIdx.x;
+  int ns = n_seeds[b];
+  if (ns < 0) return;
+  if (ns > S) ns = S;
+  __shared__ int keep[TRK_MAXK];
+  __shared__ int s_n;
+  const float* sb = seeds + (size_t)b * S * CP_SEED_RECORD;
+  if (threadIdx.x == 0) {
+    int n = 0;
+    for (int k = 0; k < ns; ++k)
+      if ((double)sb[(size_t)k * CP_SEED_RECORD + CP_P_SCORE] > cfg.new_thresh) keep[n++] = k;
+    s_n = n;
+    n_tracks[b] = n;
+    id_count[b] = n;
+  }
+  __syncthreads();
+  for (int t = threadIdx.x; t < s_n; t += blockDim.x)
+    entry_seed(cfg, &slots[(size_t)b * T + t], sb + (size_t)keep[t] * CP_SEED_RECORD, t + 1);
+}
+
 // ---- previous-frame heat maps ----------------------------------------------------------------------------------------
 struct RenderArgs {
   Cfg cfg;
@@ -140,6 +304,7 @@ struct RenderArgs {
   const double* trans;     // [B,6]
   float* pre_hm;           // [B,1,h,w]
   float* pre_hm_hp;        // [B,8,h,w]
+  const int* modes;        // [B] cp_render_mode, or nullptr: all CP_RENDER_TRACKS
 };
 
 struct Patch {
@@ -156,7 +321,9 @@ __device__ __forceinline__ void affine_pt(const double* t, float x, float y, dou
 // one CTA per (track, stream): thread 0 derives the nine patches exactly like base_detector.py:213-315, all threads draw
 __global__ void __launch_bounds__(256) tracker_render_kernel(const RenderArgs a) {
   const int t = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
-  if (t >= a.n[b]) return;
+  const int rmode = a.modes ? a.modes[b] : CP_RENDER_TRACKS;
+  if (t >= a.n[b] || rmode == CP_RENDER_EMPTY) return;
+  const bool gt = rmode == CP_RENDER_GT;
   __shared__ Patch pt[9];
   if (tid == 0) {
     for (int i = 0; i < 9; ++i) pt[i].live = 0;
@@ -164,7 +331,7 @@ __global__ void __launch_bounds__(256) tracker_render_kernel(const RenderArgs a)
     const float* r = s.rec;
     const double* tr = a.trans + (size_t)b * 6;
     const double ori_w = a.meta[(size_t)b * CP_META_DOUBLES + 3], ori_h = a.meta[(size_t)b * CP_META_DOUBLES + 4];
-    if (!((double)r[CP_P_SCORE] < a.pre_thresh)) {
+    if (gt || !((double)r[CP_P_SCORE] < a.pre_thresh)) {
       // _trans_bbox (base_detector.py:79-89): float32 box, transformed corners rounded back to float32, clipped
       double x0, y0, x1, y1;
       affine_pt(tr, r[CP_P_BBOX], r[CP_P_BBOX + 1], &x0, &y0);
@@ -184,66 +351,83 @@ __global__ void __launch_bounds__(256) tracker_render_kernel(const RenderArgs a)
         pt[0].x = (int)cx;
         pt[0].y = (int)cy;
         pt[0].r = radius;
-        pt[0].k = a.render_hm_mode == 1 ? (double)r[CP_P_SCORE] : 1.0;
+        pt[0].k = (a.render_hm_mode == 1 && !gt) ? (double)r[CP_P_SCORE] : 1.0;
         pt[0].live = 1;
-        // keypoints: normalised 9-point sets, entry 0 is the centre (base_detector.py:238-251)
-        double px[8], py[8];
-        bool have = true;
-        const int mode = a.render_hmhp_mode;
-        if (mode == 0 || mode == 1) {       // kps_ori: the detection's own keypoints, normalised
-          for (int j = 0; j < 8; ++j) {
-            px[j] = ((double)r[CP_P_KPS + 2 * j] / ori_w) * ori_w;
-            py[j] = ((double)r[CP_P_KPS + 2 * j + 1] / ori_h) * ori_h;
-          }
-        } else if (a.cfg.kalman || a.cfg.scale_pool) {
-          // kps_pnp_kf when the filtered PnP returned a tuple.  The reference's fall-back (kps_mean_kf[1:]: seven PIXEL
-          // coordinates multiplied by the image size) can never land inside the image: nothing is drawn
-          have = s.has_pnp_kf != 0;
-          for (int j = 0; j < 8 && have; ++j) {
-            px[j] = (double)s.kps_pnp_kf[2 * (j + 1)] * ori_w;
-            py[j] = (double)s.kps_pnp_kf[2 * (j + 1) + 1] * ori_h;
-          }
-        } else {
-          // 'kps_pnp' of the first PnP, or zeros when that failed (base_detector.py:248-253)
-          const bool pose = ((int)r[CP_P_STATUS] == CP_PNP_OK || (int)r[CP_P_STATUS] == CP_PNP_INVISIBLE);
-          for (int j = 0; j < 8; ++j) {
-            px[j] = pose ? (double)r[CP_P_KPS_PNP + 2 * (j + 1)] * ori_w : 0.0;
-            py[j] = pose ? (double)r[CP_P_KPS_PNP + 2 * (j + 1) + 1] * ori_h : 0.0;
-          }
-        }
-        if (have) {
-          for (int j = 0; j < 8; ++j) {
-            Patch& q = pt[1 + j];
-            q.live = 0;
-            // COCO-style visibility, int64 truncation, affine of the truncated point, truncation again
-            const bool outside = px[j] >= ori_w || px[j] < 0 || py[j] < 0 || py[j] >= ori_h;
-            if (outside) continue;
-            const long long ix = (long long)px[j], iy = (long long)py[j];
+        if (gt) {
+          // base_detector.py:166-209: kps_gt[1:] in image pixels, int64 truncation, affine, truncation again; every point
+          // is drawn with heat 1 wherever it lands (draw_umich_gaussian's slicing clips it, see the draw loop below)
+          for (int j = 0; j < 8 && s.has_gt; ++j) {
+            const double px = (double)s.kps_gt[2 * (j + 1)] * ori_w, py = (double)s.kps_gt[2 * (j + 1) + 1] * ori_h;
+            const long long ix = (long long)px, iy = (long long)py;
             double ax, ay;
             affine_pt(tr, (float)ix, (float)iy, &ax, &ay);
-            const long long jx = (long long)ax, jy = (long long)ay;
-            if (!(jx >= 0 && jx < a.inp_w && jy >= 0 && jy < a.inp_h)) continue;
-            double k = 1.0;
-            if (mode == 0 || mode == 2) {
-              const double rd = a.cfg.hps_uncertainty ? s.fus_std[2 * j] : (double)r[CP_P_KPS_HM_STD + 2 * j];
-              if (!((int)rd > 0)) continue;                   // radius_detector[j, 0] > 0 (int32 truncation)
-              if (a.cfg.kalman && s.has_kf) {
-                const double std_c = sqrt(s.f.P[j][0] + s.f.P[j][5]);
-                k = 1.0 - pow(exp(log(0.15) / (a.cfg.conf_lo - a.cfg.conf_hi)), std_c - a.cfg.conf_hi);
-                if (k < 0.0) k = 0.0;
-              } else if (a.cfg.hps_uncertainty) {
-                const double std_c = sqrt(s.fus_std[2 * j] + s.fus_std[2 * j + 1]);
-                k = 1.0 - pow(exp(log(0.15) / (a.cfg.conf_lo - a.cfg.conf_hi)), std_c - a.cfg.conf_hi);
-                if (k < 0.0) k = 0.0;
-              } else {
-                k = (double)r[CP_P_KPS_HM_HEIGHT + j];
-              }
-            }
-            q.x = (int)jx;
-            q.y = (int)jy;
+            Patch& q = pt[1 + j];
+            q.x = (int)(long long)ax;
+            q.y = (int)(long long)ay;
             q.r = radius;
-            q.k = k;
+            q.k = 1.0;
             q.live = 1;
+          }
+        } else {
+          // keypoints: normalised 9-point sets, entry 0 is the centre (base_detector.py:238-251)
+          double px[8], py[8];
+          bool have = true;
+          const int mode = a.render_hmhp_mode;
+          if (mode == 0 || mode == 1) {       // kps_ori: the detection's own keypoints, normalised
+            for (int j = 0; j < 8; ++j) {
+              px[j] = ((double)r[CP_P_KPS + 2 * j] / ori_w) * ori_w;
+              py[j] = ((double)r[CP_P_KPS + 2 * j + 1] / ori_h) * ori_h;
+            }
+          } else if (a.cfg.kalman || a.cfg.scale_pool) {
+            // kps_pnp_kf when the filtered PnP returned a tuple.  The reference's fall-back (kps_mean_kf[1:]: seven PIXEL
+            // coordinates multiplied by the image size) can never land inside the image: nothing is drawn
+            have = s.has_pnp_kf != 0;
+            for (int j = 0; j < 8 && have; ++j) {
+              px[j] = (double)s.kps_pnp_kf[2 * (j + 1)] * ori_w;
+              py[j] = (double)s.kps_pnp_kf[2 * (j + 1) + 1] * ori_h;
+            }
+          } else {
+            // 'kps_pnp' of the first PnP, or zeros when that failed (base_detector.py:248-253)
+            const bool pose = ((int)r[CP_P_STATUS] == CP_PNP_OK || (int)r[CP_P_STATUS] == CP_PNP_INVISIBLE);
+            for (int j = 0; j < 8; ++j) {
+              px[j] = pose ? (double)r[CP_P_KPS_PNP + 2 * (j + 1)] * ori_w : 0.0;
+              py[j] = pose ? (double)r[CP_P_KPS_PNP + 2 * (j + 1) + 1] * ori_h : 0.0;
+            }
+          }
+          if (have) {
+            for (int j = 0; j < 8; ++j) {
+              Patch& q = pt[1 + j];
+              q.live = 0;
+              // COCO-style visibility, int64 truncation, affine of the truncated point, truncation again
+              const bool outside = px[j] >= ori_w || px[j] < 0 || py[j] < 0 || py[j] >= ori_h;
+              if (outside) continue;
+              const long long ix = (long long)px[j], iy = (long long)py[j];
+              double ax, ay;
+              affine_pt(tr, (float)ix, (float)iy, &ax, &ay);
+              const long long jx = (long long)ax, jy = (long long)ay;
+              if (!(jx >= 0 && jx < a.inp_w && jy >= 0 && jy < a.inp_h)) continue;
+              double k = 1.0;
+              if (mode == 0 || mode == 2) {
+                const double rd = a.cfg.hps_uncertainty ? s.fus_std[2 * j] : (double)r[CP_P_KPS_HM_STD + 2 * j];
+                if (!((int)rd > 0)) continue;                   // radius_detector[j, 0] > 0 (int32 truncation)
+                if (a.cfg.kalman && s.has_kf) {
+                  const double std_c = sqrt(s.f.P[j][0] + s.f.P[j][5]);
+                  k = 1.0 - pow(exp(log(0.15) / (a.cfg.conf_lo - a.cfg.conf_hi)), std_c - a.cfg.conf_hi);
+                  if (k < 0.0) k = 0.0;
+                } else if (a.cfg.hps_uncertainty) {
+                  const double std_c = sqrt(s.fus_std[2 * j] + s.fus_std[2 * j + 1]);
+                  k = 1.0 - pow(exp(log(0.15) / (a.cfg.conf_lo - a.cfg.conf_hi)), std_c - a.cfg.conf_hi);
+                  if (k < 0.0) k = 0.0;
+                } else {
+                  k = (double)r[CP_P_KPS_HM_HEIGHT + j];
+                }
+              }
+              q.x = (int)jx;
+              q.y = (int)jy;
+              q.r = radius;
+              q.k = k;
+              q.live = 1;
+            }
           }
         }
       }
@@ -255,7 +439,9 @@ __global__ void __launch_bounds__(256) tracker_render_kernel(const RenderArgs a)
     if (!(pt[i].live & 1)) continue;
     const Patch q = pt[i];
     float* map = (i == 0) ? a.pre_hm + (size_t)b * plane : a.pre_hm_hp + ((size_t)b * 8 + (i - 1)) * plane;
-    // draw_umich_gaussian (utils/image.py:135-150): the patch clipped to the map, np.maximum compositing
+    // draw_umich_gaussian (utils/image.py:135-150): the patch clipped to the map, np.maximum compositing.  A centre left
+    // of / above the map gives left / top < 0 and numpy's slices then keep exactly the part of the patch inside the map
+    // (nothing once x < -r); a centre right of / below it gives right / bottom <= 0, the same.
     const int left = min(q.x, q.r), right = min(a.inp_w - q.x, q.r + 1);
     const int top = min(q.y, q.r), bottom = min(a.inp_h - q.y, q.r + 1);
     const int pw = left + right, ph = top + bottom;
@@ -280,6 +466,7 @@ Cfg make_cfg(const cp_tracker_config& c) {
   g.R = (double)c.R;
   g.conf_lo = (double)c.conf_lo;
   g.conf_hi = (double)c.conf_hi;
+  g.hungarian = c.hungarian;
   return g;
 }
 
@@ -312,6 +499,9 @@ int cp_tracker_create(const cp_tracker_config* cfg, cp_tracker** out) {
   }
   if (e == cudaSuccess) e = cudaMalloc(&t->id_count, sizeof(int) * cfg->streams);
   if (e == cudaSuccess) e = cudaMemset(t->id_count, 0, sizeof(int) * cfg->streams);
+  if (e == cudaSuccess) e = cudaMalloc(&t->modes, sizeof(int) * cfg->streams);
+  if (e == cudaSuccess && cfg->hungarian) e = cudaMalloc(&t->plan, ns * sizeof(Entry));
+  if (e == cudaSuccess && cfg->hungarian) e = cudaMalloc(&t->plan_n, sizeof(int) * cfg->streams);
   if (e != cudaSuccess) {
     cp_tracker_destroy(t);
     return fail(CP_ERR_CUDA, std::string("cp_tracker_create: ") + cudaGetErrorString(e));
@@ -327,6 +517,9 @@ int cp_tracker_destroy(cp_tracker* t) {
     if (t->n_tracks[i]) cudaFree(t->n_tracks[i]);
   }
   if (t->id_count) cudaFree(t->id_count);
+  if (t->modes) cudaFree(t->modes);
+  if (t->plan) cudaFree(t->plan);
+  if (t->plan_n) cudaFree(t->plan_n);
   delete t;
   return CP_OK;
 }
@@ -361,6 +554,12 @@ int cp_tracker_step(cp_tracker* t, int32_t batch, const float* poses, const int3
   a.id_count = t->id_count;
   a.tracks_out = tracks_out;
   a.n_out = n_tracks;
+  a.plan = t->cfg.hungarian ? static_cast<Entry*>(t->plan) : nullptr;
+  a.plan_n = t->cfg.hungarian ? t->plan_n : nullptr;
+  if (a.plan) {
+    tracker_assoc_kernel<<<batch, TRK_THREADS, 0, (cudaStream_t)stream>>>(a);
+    CP_LAUNCH_CHECK("tracker_assoc_kernel");
+  }
   tracker_step_kernel<<<batch, TRK_THREADS, 0, (cudaStream_t)stream>>>(a);
   CP_LAUNCH_CHECK("tracker_step_kernel");
   t->cur ^= 1;           // calls are issued in frame order on one stream
@@ -369,12 +568,24 @@ int cp_tracker_step(cp_tracker* t, int32_t batch, const float* poses, const int3
 
 int cp_tracker_render(cp_tracker* t, int32_t batch, const double* meta, const double* trans_input, int32_t inp_h,
                       int32_t inp_w, float* pre_hm, float* pre_hm_hp, void* stream) {
+  return cp_tracker_render_ex(t, batch, meta, trans_input, inp_h, inp_w, nullptr, pre_hm, pre_hm_hp, stream);
+}
+
+int cp_tracker_render_ex(cp_tracker* t, int32_t batch, const double* meta, const double* trans_input, int32_t inp_h,
+                         int32_t inp_w, const int32_t* modes, float* pre_hm, float* pre_hm_hp, void* stream) {
+  bool any_mode = false;
+  for (int b = 0; modes && b < batch; ++b) {
+    if (modes[b] < CP_RENDER_TRACKS || modes[b] > CP_RENDER_EMPTY)
+      return fail(CP_ERR_INVALID, "cp_tracker_render_ex: unknown render mode " + std::to_string(modes[b]) + " (0, 1 or 2)");
+    any_mode = any_mode || modes[b] != CP_RENDER_TRACKS;
+  }
   if (!t || !meta || !trans_input || !pre_hm || !pre_hm_hp) return fail(CP_ERR_INVALID, "cp_tracker_render: null argument");
   if (batch <= 0 || batch > t->cfg.streams || inp_h <= 0 || inp_w <= 0) return fail(CP_ERR_INVALID, "cp_tracker_render: bad shape");
   cudaStream_t s = (cudaStream_t)stream;
   const size_t plane = (size_t)inp_h * inp_w;
   CP_CUDA_CHECK(cudaMemsetAsync(pre_hm, 0, sizeof(float) * plane * batch, s));
   CP_CUDA_CHECK(cudaMemsetAsync(pre_hm_hp, 0, sizeof(float) * plane * 8 * batch, s));
+  if (any_mode) CP_CUDA_CHECK(cudaMemcpyAsync(t->modes, modes, sizeof(int32_t) * batch, cudaMemcpyHostToDevice, s));
   RenderArgs a;
   a.cfg = make_cfg(t->cfg);
   a.T = t->cfg.max_tracks;
@@ -389,9 +600,23 @@ int cp_tracker_render(cp_tracker* t, int32_t batch, const double* meta, const do
   a.trans = trans_input;
   a.pre_hm = pre_hm;
   a.pre_hm_hp = pre_hm_hp;
+  a.modes = any_mode ? t->modes : nullptr;
   dim3 grid(t->cfg.max_tracks, batch);
   tracker_render_kernel<<<grid, 256, 0, s>>>(a);
   CP_LAUNCH_CHECK("tracker_render_kernel");
+  return CP_OK;
+}
+
+int cp_tracker_seed(cp_tracker* t, int32_t batch, const float* seeds, const int32_t* n_seeds, int32_t S, void* stream) {
+  if (S < 0 || S > CP_MAX_K) return fail(CP_ERR_INVALID, "cp_tracker_seed: S must be in 0..128");
+  if (!t || !n_seeds || (S > 0 && !seeds)) return fail(CP_ERR_INVALID, "cp_tracker_seed: null argument");
+  if (batch <= 0 || batch > t->cfg.streams) return fail(CP_ERR_INVALID, "cp_tracker_seed: batch exceeds the tracker's streams");
+  if (S > t->cfg.max_tracks)
+    return fail(CP_ERR_INVALID, "cp_tracker_seed: S = " + std::to_string(S) + " seeds exceed max_tracks = " +
+                                    std::to_string(t->cfg.max_tracks));
+  tracker_seed_kernel<<<batch, 128, 0, (cudaStream_t)stream>>>(make_cfg(t->cfg), t->cfg.max_tracks, seeds, n_seeds, S,
+                                                               t->slots[t->cur], t->n_tracks[t->cur], t->id_count);
+  CP_LAUNCH_CHECK("tracker_seed_kernel");
   return CP_OK;
 }
 

@@ -180,6 +180,22 @@ class ObjectPoseDetector(object):
                 meta[k] = input_meta[k]
         return images, meta
 
+    def _gt_frame(self, frame_id):
+        """base_detector.py:451 / :167: this frame is seeded from and drawn from the ground truth."""
+        if getattr(self.opt, "gt_pre_hm_hmhp", False):
+            return True
+        if getattr(self.opt, "gt_pre_hm_hmhp_first", False):
+            if frame_id is None:
+                raise ValueError("opt.gt_pre_hm_hmhp_first needs the frame index, meta['id']")
+            return int(frame_id) == 0
+        return False
+
+    def _render_mode(self, gt):
+        """_get_additional_inputs (base_detector.py:165-166): empty, ground truth or the tracks."""
+        if getattr(self.opt, "empty_pre_hm", False):
+            return _lib.RENDER_EMPTY
+        return _lib.RENDER_GT if gt else _lib.RENDER_TRACKS
+
     def _meta_tensor(self, meta, batch=1):
         cam = meta.get("camera_matrix")
         if cam is None:
@@ -256,15 +272,19 @@ class ObjectPoseDetector(object):
 
             pre_hms, pre_hm_hp, pre_inds = None, None, None
             if tracking:
+                gt = self._gt_frame(meta.get("id"))
                 if self.pre_images is None:                       # base_detector.py:444-449
                     print("Initialize tracking!")
                     self.pre_images = images
+                    self.tracker.init_track(meta)
+                elif gt:                                          # :451-454, ground-truth seeding
                     self.tracker.init_track(meta)
                 if self.opt.pre_hm or self.opt.pre_hm_hp:         # :456-462, rendered on the device from the tracker state
                     if "trans_input" not in meta:
                         raise ValueError("tracking needs meta['trans_input'] (pre_process provides it)")
                     metat = self._meta_tensor(meta).to(images.device)
-                    pre_hms, pre_hm_hp = self.tracker.render(metat, meta["trans_input"], images.shape[2], images.shape[3])
+                    pre_hms, pre_hm_hp = self.tracker.render(metat, meta["trans_input"], images.shape[2], images.shape[3],
+                                                             modes=[self._render_mode(gt)])
             torch.cuda.synchronize()
             pre_process_time = time.time()
             pre_time += pre_process_time - scale_start_time
@@ -454,7 +474,7 @@ class ObjectPoseDetector(object):
 
     # ------------------------------------------------------------------ batched API (not in the reference)
     def run_batch(self, frames, camera_matrix, pre_images=None, pre_hms=None, pre_hm_hp=None, to_host=True, track=False,
-                  out=None):
+                  out=None, pre_dets=None, frame_ids=None):
         """frames: uint8 [B,H,W,3] (numpy / pinned CPU tensor / CUDA tensor) or a
         pre-processed fp32 [B,3,h,w] CUDA tensor.  One native cp_infer call for the
         whole batch.  Returns (poses [B,K,192], n_valid [B]) -- on the host when
@@ -462,7 +482,10 @@ class ObjectPoseDetector(object):
 
         track=True (tracking models): the batch is B independent VIDEO STREAMS and every call is their next frame.
         The previous frames, the tracker state and the rendered previous-frame heat maps stay on the device; returns
-        (tracks [B,T,320], n_tracks [B]) (layout: cp_track_field) instead.
+        (tracks [B,T,320], n_tracks [B]) (layout: cp_track_field) instead.  pre_dets: None, or per stream the
+        meta['pre_dets'] list of this frame (or None); frame_ids: per stream meta['id'] (needed with
+        opt.gt_pre_hm_hmhp_first).  Per stream, seeding and the heat maps follow run(): seeded on the first frame and on
+        ground-truth frames, drawn from the ground truth on those frames, empty with opt.empty_pre_hm.
 
         out: optional (poses, n_valid) CUDA tensors to write into (e.g. the views of a dist.PoseBuffer, so that the
         records land directly in the buffer of the all-gather / the pinned D2H copy)."""
@@ -499,10 +522,16 @@ class ObjectPoseDetector(object):
             if trk is None or trk.streams != B:
                 trk = self._batch_tracker = Tracker(self.opt, streams=B, device=x.device)
                 self._batch_pre = None
-            if self._batch_pre is None or self._batch_pre.shape != x.shape:
+            gts = [self._gt_frame(frame_ids[b] if frame_ids is not None else None) for b in range(B)]
+            first = self._batch_pre is None or self._batch_pre.shape != x.shape
+            if first:
                 self._batch_pre = x                                   # first frame: pre_images = images (base_detector.py:446)
+            if pre_dets is not None:
+                if len(pre_dets) != B:
+                    raise ValueError("run_batch: %d pre_dets lists for %d streams" % (len(pre_dets), B))
+                trk.seed([pre_dets[b] if (first or gts[b]) else None for b in range(B)])
             trans = affine_from_center_scale(c, s, x.shape[3], x.shape[2])
-            pre_hms, pre_hm_hp = trk.render(meta, trans, x.shape[2], x.shape[3])
+            pre_hms, pre_hm_hp = trk.render(meta, trans, x.shape[2], x.shape[3], modes=[self._render_mode(g) for g in gts])
             _, poses, n_valid = eng.infer(x, meta, prm, self._batch_pre, pre_hms, pre_hm_hp)
             tracks, nt = trk.step_records(poses, n_valid, meta)
             self._batch_pre = x

@@ -55,6 +55,10 @@ def default_opt(arch="dla_34", tracking_task=False, rep_mode=1, c="chair", gpus=
     o.tracking = o.tracking_hp = bool(tracking_task)
     o.obj_scale_uncertainty = o.hps_uncertainty = bool(tracking_task)
     o.kalman = o.scale_pool = bool(tracking_task)
+    o.hungarian = False                    # opts.py:295
+    o.gt_pre_hm_hmhp = False               # opts.py:307-312
+    o.gt_pre_hm_hmhp_first = False
+    o.empty_pre_hm = False
     o.track_thresh = 0.1
     if tracking_task:
         o.vis_thresh = max(o.track_thresh, o.vis_thresh)

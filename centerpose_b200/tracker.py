@@ -3,9 +3,12 @@
 The reference keeps a Python list of dicts per video and runs association, a 32-state filterpy Kalman filter per
 object, the scale pool and a second PnP on the host every frame; here the state of `streams` independent videos lives
 in device memory and one native call (`cp_tracker_step`) advances all of them from the fixed-shape pose records that
-`cp_decode_pnp` / `cp_infer` emit.  `cp_tracker_render` draws the previous-frame heat maps
-(`BaseDetector._get_additional_inputs`, base_detector.py:150-388) straight into the network's `pre_hm` / `pre_hm_hp`
-inputs.  The Python side only rebuilds the reference's dict structures for callers that want them (`tracks`).
+`cp_decode_pnp` / `cp_infer` emit, with the greedy or (opt.hungarian) the optimal association.  `cp_tracker_render_ex`
+draws the previous-frame heat maps (`BaseDetector._get_additional_inputs`, base_detector.py:150-388) straight into the
+network's `pre_hm` / `pre_hm_hp` inputs, from the tracks, from the ground truth (opt.gt_pre_hm_hmhp /
+gt_pre_hm_hmhp_first) or empty (opt.empty_pre_hm).  `cp_tracker_seed` is init_track with meta['pre_dets'].  The Python
+side packs the reference's `pre_dets` dicts into seed records and rebuilds its dict structures for callers that want
+them (`tracks`).
 """
 import ctypes
 
@@ -60,10 +63,66 @@ def tracks_to_results(rows, n, width, height):
     return res, boxes
 
 
+def _need(d, key):
+    if key not in d:
+        raise ValueError("pre_dets entry has no %r, which the reference tracker reads with these options" % key)
+    return d[key]
+
+
+def seed_records(dets, opt):
+    """meta['pre_dets'] (a list of the reference's dicts) -> fp32 [len, CP_SEED_RECORD] (cp_seed_field layout).  A key
+    the reference would read with these options but which the dict lacks raises ValueError naming it."""
+    L = _lib
+    kalman, scale_pool = bool(_opt(opt, "kalman", True)), bool(_opt(opt, "scale_pool", True))
+    use_pnp = bool(_opt(opt, "use_pnp", True))
+    out = np.zeros((len(dets), L.CP_SEED_RECORD), np.float32)
+
+    def put(r, off, n, v):
+        r[off:off + n] = np.asarray(v, np.float64).reshape(-1)[:n]
+    for r, d in zip(out, dets):
+        r[L.P_SCORE] = float(_need(d, "score"))
+        bbox = _need(d, "bbox")
+        put(r, L.P_BBOX, 4, bbox)
+        r[L.P_CLS] = int(_need(d, "cls"))
+        if "ct" in d:
+            put(r, L.P_CT, 2, d["ct"])
+            r[L.S_HAS_CT] = 1
+        if kalman:                               # init_kf (tracker.py:55-79)
+            put(r, L.S_KPS_FUSION_MEAN, 16, _need(d, "kps_fusion_mean"))
+            put(r, L.S_KPS_FUSION_STD, 16, _need(d, "kps_fusion_std"))
+            put(r, L.P_TRACKING_HP, 16, _need(d, "tracking_hp"))
+        if scale_pool:                           # the scale pool (tracker.py:45-47)
+            put(r, L.P_OBJ_SCALE_UNC, 3, _need(d, "obj_scale_uncertainty"))
+        if scale_pool or use_pnp:
+            put(r, L.P_OBJ_SCALE, 3, _need(d, "obj_scale"))
+        if use_pnp and not kalman and scale_pool:
+            put(r, L.P_KPS, 16, _need(d, "kps"))  # the second PnP reads track['kps'] without the filter (tracker.py:246)
+        for key, off, n in (("kps", L.P_KPS, 16), ("kps_displacement_mean", L.P_KPS_DISP_MEAN, 16),
+                            ("kps_heatmap_mean", L.P_KPS_HM_MEAN, 16), ("kps_heatmap_std", L.P_KPS_HM_STD, 16),
+                            ("kps_heatmap_height", L.P_KPS_HM_HEIGHT, 8), ("kps_displacement_std", L.P_KPS_DISP_STD, 16),
+                            ("obj_scale", L.P_OBJ_SCALE, 3), ("obj_scale_uncertainty", L.P_OBJ_SCALE_UNC, 3),
+                            ("tracking", L.P_TRACKING, 2), ("tracking_hp", L.P_TRACKING_HP, 16),
+                            ("kps_fusion_mean", L.S_KPS_FUSION_MEAN, 16), ("kps_fusion_std", L.S_KPS_FUSION_STD, 16),
+                            ("kps_3d_cam", L.P_KPS_3D_CAM, 27), ("kps_pnp", L.P_KPS_PNP, 18)):
+            if key in d:
+                put(r, off, n, d[key])
+        if "location" in d and "quaternion_xyzw" in d:    # a dict that already went through pnp_shell
+            r[L.P_STATUS] = L.PNP_OK
+            put(r, L.P_LOCATION, 3, d["location"])
+            put(r, L.P_QUAT, 4, d["quaternion_xyzw"])
+            if "projected_cuboid" in d:
+                put(r, L.P_PROJ_CUBOID, 16, d["projected_cuboid"])
+        if "kps_gt" in d:
+            put(r, L.S_KPS_GT, 18, d["kps_gt"])
+            r[L.S_HAS_KPS_GT] = 1
+        if "kps_pnp_kf" in d:
+            put(r, L.S_KPS_PNP_KF, 18, d["kps_pnp_kf"])
+            r[L.S_HAS_KPS_PNP_KF] = 1
+    return out
+
+
 class Tracker(object):
     def __init__(self, opt, streams=1, device=None, max_tracks=_lib.CP_MAX_K):
-        if _opt(opt, "hungarian", False):
-            raise NotImplementedError("centerpose_b200 Tracker implements the greedy association (opt.hungarian is off in demo.py)")
         self.L = _lib.load()
         self.opt = opt
         self.streams = int(streams)
@@ -90,6 +149,7 @@ class Tracker(object):
         cfg.pre_thresh = float(_opt(opt, "pre_thresh", -1))
         cfg.R = float(_opt(opt, "R", 20))
         cfg.conf_lo, cfg.conf_hi = float(border[0]), float(border[1])
+        cfg.hungarian = int(bool(_opt(opt, "hungarian", False)))
         self._cfg = cfg
         h = ctypes.c_void_p()
         with torch.cuda.device(self.device):
@@ -99,6 +159,11 @@ class Tracker(object):
         self._rows = None          # host copy of the latest step: (rows [B,T,320], n [B])
         self._dev = None           # device tensors of the latest step
         self._dicts = None
+        # per stream, since the latest seeding and before the next step: None (not seeded), or the missing key that the
+        # reference would raise on when drawing these seeds from the tracks (or "" when none is missing), and whether
+        # every seed carries 'kps_gt'
+        self._seeded = [None] * self.streams
+        self._seeded_gt = [False] * self.streams
 
     def close(self):
         if getattr(self, "_h", None):
@@ -117,13 +182,60 @@ class Tracker(object):
         with torch.cuda.device(self.device):
             _lib.check(self.L.cp_tracker_reset(self._h, int(index), _stream()), "cp_tracker_reset")
         self._rows = self._dev = self._dicts = None
+        for b in range(self.streams):
+            if index < 0 or b == index:
+                self._seeded[b], self._seeded_gt[b] = None, False
 
     def init_track(self, meta):
-        """Tracker.init_track (tracker.py:22-48).  Seeding from meta['pre_dets'] (ground-truth experiments) is not
-        on the accelerated path."""
-        if meta is not None and "pre_dets" in meta and len(meta["pre_dets"]):
-            raise NotImplementedError("seeding the device tracker from meta['pre_dets'] is not supported")
+        """Tracker.init_track (tracker.py:21-48) for stream 0: with meta['pre_dets'] the stream is reset and one track
+        is started per dict with score > new_thresh (ground-truth seeding, eval_video_official.py:422-456)."""
         self.meta = meta
+        if meta is not None and "pre_dets" in meta:
+            self.seed([meta["pre_dets"]] + [None] * (self.streams - 1))
+
+    def seed(self, pre_dets):
+        """init_track with pre_dets for several streams: pre_dets[b] is the list of dicts for stream b, or None to leave
+        stream b untouched (one cp_tracker_seed call)."""
+        pre_dets = list(pre_dets)
+        if len(pre_dets) > self.streams:
+            raise ValueError("%d seed lists for a tracker of %d streams" % (len(pre_dets), self.streams))
+        B = max([b + 1 for b, p in enumerate(pre_dets) if p is not None] or [0])
+        if B == 0:
+            return
+        S = max(1, max(len(p) for p in pre_dets[:B] if p is not None))
+        if S > self.max_tracks:
+            raise ValueError("%d seeds exceed max_tracks = %d" % (S, self.max_tracks))
+        recs = np.zeros((B, S, _lib.CP_SEED_RECORD), np.float32)
+        n = np.full(B, -1, np.int32)
+        hmhp = int(_opt(self.opt, "render_hmhp_mode", 2))
+        filt = bool(_opt(self.opt, "kalman", True)) or bool(_opt(self.opt, "scale_pool", True))
+        pre_thresh, new_thresh = float(_opt(self.opt, "pre_thresh", -1)), float(_opt(self.opt, "new_thresh", 0.3))
+        for b, dets in enumerate(pre_dets[:B]):
+            if dets is None:
+                continue
+            dets = list(dets)
+            if dets:
+                recs[b, :len(dets)] = seed_records(dets, self.opt)
+            n[b] = len(dets)
+            kept = [d for d in dets if float(d["score"]) > new_thresh]
+            missing = ""
+            for d in kept:
+                if float(d["score"]) < pre_thresh:
+                    continue
+                if hmhp in (0, 1) and "kps_ori" not in d:
+                    missing = "kps_ori"
+                elif hmhp in (2, 3) and filt and "kps_pnp_kf" not in d and "kps_mean_kf" not in d:
+                    missing = "kps_mean_kf"          # base_detector.py:245: the reference raises KeyError here
+            self._seeded[b] = missing
+            self._seeded_gt[b] = all("kps_gt" in d for d in kept)
+        seeds = torch.from_numpy(recs).to(self.device)
+        nt = torch.from_numpy(n).to(self.device)
+        with torch.cuda.device(self.device):
+            rc = self.L.cp_tracker_seed(self._h, B, _ptr(seeds), _ptr(nt), S, _stream())
+        _lib.check(rc, "cp_tracker_seed")
+        seeds._cp_keep = nt
+        self._keep = seeds                       # the copy is stream-ordered; keep the buffers alive until the next call
+        self._rows = self._dev = self._dicts = None
 
     @property
     def tracks(self):
@@ -159,11 +271,28 @@ class Tracker(object):
                                         _stream())
         _lib.check(rc, "cp_tracker_step")
         self._dev, self._rows, self._dicts = out, None, None
+        self._seeded = [None] * self.streams
+        self._seeded_gt = [False] * self.streams
         return out
 
-    def render(self, meta, trans_input, inp_h, inp_w, out=None):
-        """Previous-frame heat maps of every stream: (pre_hm [B,1,h,w], pre_hm_hp [B,8,h,w]) fp32 CUDA."""
+    def render(self, meta, trans_input, inp_h, inp_w, out=None, modes=None):
+        """Previous-frame heat maps of every stream: (pre_hm [B,1,h,w], pre_hm_hp [B,8,h,w]) fp32 CUDA.  modes: None
+        (all drawn from the tracks) or one cp_render_mode per stream: RENDER_TRACKS, RENDER_GT (the ground-truth
+        branch, on a stream seeded since its last step) or RENDER_EMPTY (opt.empty_pre_hm)."""
         B = meta.shape[0]
+        mode_arr = None
+        if modes is not None:
+            modes = [int(m) for m in modes]
+            if len(modes) != B:
+                raise ValueError("render: %d modes for %d streams" % (len(modes), B))
+            mode_arr = (ctypes.c_int32 * B)(*modes)
+        for b in range(B):
+            m = modes[b] if modes is not None else _lib.RENDER_TRACKS
+            if m == _lib.RENDER_GT and not (self._seeded[b] is not None and self._seeded_gt[b]):
+                raise ValueError("the ground-truth render of stream %d needs tracks seeded from pre_dets with 'kps_gt'" % b)
+            if m == _lib.RENDER_TRACKS and self._seeded[b]:
+                raise ValueError("drawing the seeds of stream %d from the tracks reads %r, which a pre_dets entry lacks"
+                                 % (b, self._seeded[b]))
         tr = torch.as_tensor(np.asarray(trans_input, np.float64).reshape(-1, 6)) if not torch.is_tensor(trans_input) else trans_input
         if tr.shape[0] == 1 and B > 1:
             tr = tr.expand(B, 6)
@@ -173,8 +302,8 @@ class Tracker(object):
             out = (torch.empty((B, 1, inp_h, inp_w), dtype=torch.float32, device=self.device),
                    torch.empty((B, 8, inp_h, inp_w), dtype=torch.float32, device=self.device))
         with torch.cuda.device(self.device):
-            rc = self.L.cp_tracker_render(self._h, B, _ptr(meta), _ptr(tr), int(inp_h), int(inp_w), _ptr(out[0]), _ptr(out[1]),
-                                          _stream())
-        _lib.check(rc, "cp_tracker_render")
+            rc = self.L.cp_tracker_render_ex(self._h, B, _ptr(meta), _ptr(tr), int(inp_h), int(inp_w), mode_arr, _ptr(out[0]),
+                                             _ptr(out[1]), _stream())
+        _lib.check(rc, "cp_tracker_render_ex")
         out[0]._cp_keep = (meta, tr)
         return out

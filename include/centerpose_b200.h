@@ -267,7 +267,10 @@ enum cp_dets_field {
  * the previous-frame heat maps, base_detector.py:150-388 (_get_additional_inputs, default options: use_pnp,
  * render_hm_mode 1, render_hmhp_mode 0-3).  One tracker holds `streams` independent videos (the batch dimension);
  * state lives in device memory, every call is enqueued on `stream`, calls on one tracker must be issued in frame order
- * on one stream.  Not supported: --hungarian, meta['pre_dets'] seeding, gt_pre_hm_hmhp. */
+ * on one stream.  Association is greedy (tracker.py:305-314) or, with `hungarian`, the minimum-cost assignment that
+ * scipy.optimize.linear_sum_assignment returns (ties included).  Tracks can be seeded from ground truth
+ * (Tracker.init_track with meta['pre_dets'], cp_tracker_seed) and the previous-frame heat maps drawn from that ground
+ * truth (opt.gt_pre_hm_hmhp / gt_pre_hm_hmhp_first) or left empty (opt.empty_pre_hm), see cp_tracker_render_ex. */
 #define CP_TRACK_RECORD 320
 typedef struct cp_tracker cp_tracker;
 typedef struct cp_tracker_config {
@@ -287,6 +290,7 @@ typedef struct cp_tracker_config {
   float pre_thresh;           /* opt.pre_thresh                                                             */
   float R;                    /* opt.R (20)                                                                 */
   float conf_lo, conf_hi;     /* opt.conf_border[opt.c] (3, 9)                                              */
+  int32_t hungarian;          /* opt.hungarian: optimal instead of greedy association (tracker.py:154-177)  */
 } cp_tracker_config;
 
 int cp_tracker_create(const cp_tracker_config* cfg, cp_tracker** out);
@@ -303,6 +307,38 @@ int cp_tracker_step(cp_tracker* trk, int32_t batch, const float* poses, const in
  * meta['trans_input'] (original image -> network input). */
 int cp_tracker_render(cp_tracker* trk, int32_t batch, const double* meta, const double* trans_input, int32_t inp_h,
                       int32_t inp_w, float* pre_hm, float* pre_hm_hp, void* stream);
+/* Per-stream render modes of cp_tracker_render_ex. */
+enum cp_render_mode {
+  CP_RENDER_TRACKS = 0,  /* the tracks (what cp_tracker_render draws)                                              */
+  CP_RENDER_GT = 1,      /* the ground-truth branch of _get_additional_inputs (base_detector.py:166-209): every track,
+                          * no pre_thresh test, centre heat 1, the 8 points of kps_gt[1:] with heat 1 and no
+                          * visibility or in-input gate.  Tracks that were not seeded draw their centre only.          */
+  CP_RENDER_EMPTY = 2    /* all zeros (opt.empty_pre_hm)                                                            */
+};
+/* cp_tracker_render with a mode per stream: `modes` is a HOST int32 [batch] of cp_render_mode values, or NULL for all
+ * CP_RENDER_TRACKS (then identical to cp_tracker_render).  An unknown mode returns CP_ERR_INVALID. */
+int cp_tracker_render_ex(cp_tracker* trk, int32_t batch, const double* meta, const double* trans_input, int32_t inp_h,
+                         int32_t inp_w, const int32_t* modes, float* pre_hm, float* pre_hm_hp, void* stream);
+
+/* Offsets (in floats) inside one CP_SEED_RECORD: one dict of meta['pre_dets'] (eval_video_official.py:422-450). */
+#define CP_SEED_RECORD 264
+enum cp_seed_field {
+  /* [0, CP_POSE_RECORD): the cp_pose_field layout, holding the dict keys of the same names (image pixels).  CP_P_STATUS
+   * is CP_PNP_OK when the dict carries a pose ('location', 'quaternion_xyzw', ...), else CP_PNP_NOT_RUN. */
+  CP_S_KPS_FUSION_MEAN = 192,  /* 16 */
+  CP_S_KPS_FUSION_STD = 208,   /* 16 */
+  CP_S_KPS_GT = 224,           /* 18, normalised, centre first */
+  CP_S_HAS_CT = 242,           /* 0: 'ct' is absent and becomes the bbox centre                         */
+  CP_S_HAS_KPS_GT = 243,       /* 0: no 'kps_gt' (CP_RENDER_GT then draws the centre only)              */
+  CP_S_KPS_PNP_KF = 244,       /* 18, normalised: a 'kps_pnp_kf' the dict already carries               */
+  CP_S_HAS_KPS_PNP_KF = 262
+};
+/* Tracker.init_track(meta) with meta['pre_dets'] (utils/tracker.py:21-48) for `batch` streams.  seeds: device fp32
+ * [batch, S, CP_SEED_RECORD]; n_seeds: device int32 [batch].  n_seeds[b] < 0 leaves stream b untouched; otherwise
+ * stream b is reset (id counter included) and the first min(n_seeds[b], S) seeds with score > new_thresh become tracks
+ * 1, 2, ... in order, their filter initialised from the seed's own kps_fusion_mean / kps_fusion_std / tracking_hp and
+ * their scale pool from obj_scale / obj_scale_uncertainty.  S must be in 0..max_tracks. */
+int cp_tracker_seed(cp_tracker* trk, int32_t batch, const float* seeds, const int32_t* n_seeds, int32_t S, void* stream);
 
 /* Offsets (in floats) inside one CP_TRACK_RECORD slot.  [0, CP_POSE_RECORD) is the pose record of the detection the
  * track carries; its PnP fields hold the SECOND (filtered) solve whenever that produced a pose (pnp_shell mutates the
