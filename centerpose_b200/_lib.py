@@ -51,13 +51,44 @@ EXPORTS = [
     "cp_decode_pnp", "cp_infer", "cp_dcn_v2_forward", "cp_preprocess", "cp_plan_num_ops", "cp_plan_profile",
     "cp_dcn_v2_forward_ex", "cp_conv2d", "cp_dcn_v2_backward",
     "cp_preprocess_affine", "cp_tracker_create", "cp_tracker_destroy", "cp_tracker_reset", "cp_tracker_step", "cp_tracker_render",
-    "cp_tracker_render_ex", "cp_tracker_seed",
+    "cp_tracker_render_ex", "cp_tracker_seed", "cp_plan_op_desc", "cp_plan_arena", "cp_plan_run_ops",
 ]
+
+# cp_op_family
+FAM_NONE, FAM_IGEMM_FP32, FAM_STEM, FAM_CONV3_C16, FAM_IGEMM_UMMA, FAM_CONV_TMA, FAM_DCN_TMA = 0, 1, 2, 3, 4, 5, 6
+FAM_MAXPOOL, FAM_UPADD, FAM_GN_RELU, FAM_GRU = 7, 8, 9, 10
+FAMILY_NAMES = {FAM_NONE: "fused", FAM_IGEMM_FP32: "igemm_fp32", FAM_STEM: "stem", FAM_CONV3_C16: "conv3_c16",
+                FAM_IGEMM_UMMA: "igemm_umma", FAM_CONV_TMA: "conv_tma", FAM_DCN_TMA: "dcn_tma", FAM_MAXPOOL: "maxpool",
+                FAM_UPADD: "upadd", FAM_GN_RELU: "gn_relu", FAM_GRU: "gru"}
 
 
 class CpOpStat(ctypes.Structure):
     _fields_ = [("name", ctypes.c_char * 96), ("kind", ctypes.c_int32), ("ms", ctypes.c_float),
                 ("flops", ctypes.c_double), ("bytes", ctypes.c_double)]
+
+
+class CpActDesc(ctypes.Structure):
+    _fields_ = [("off", ctypes.c_int64), ("ext", ctypes.c_int32), ("C", ctypes.c_int32), ("H", ctypes.c_int32),
+                ("W", ctypes.c_int32), ("stride", ctypes.c_int32)]
+
+
+class CpOpDesc(ctypes.Structure):
+    _fields_ = ([("name", ctypes.c_char * 96)] +
+                [(n, ctypes.c_int32) for n in ("kind", "family", "x3", "nsrc")] +
+                [("src", CpActDesc * 4), ("out", CpActDesc), ("out_head", ctypes.c_int32)] +
+                [(n, ctypes.c_int32) for n in ("kh", "stride", "pad", "Cin", "Cout", "CoutPad", "Kpad")] +
+                [("w", ctypes.c_void_p), ("w_ld", ctypes.c_int32), ("bias", ctypes.c_void_p)] +
+                [(n, ctypes.c_int32) for n in ("relu", "has_res", "res_after_relu")] +
+                [("res", CpActDesc), ("om", CpActDesc), ("up_w", ctypes.c_void_p), ("f", ctypes.c_int32),
+                 ("has_skip", ctypes.c_int32), ("skip", CpActDesc), ("gamma", ctypes.c_void_p),
+                 ("beta", ctypes.c_void_p), ("groups", ctypes.c_int32), ("gx", CpActDesc), ("gh", CpActDesc),
+                 ("gprev", CpActDesc), ("first_step", ctypes.c_int32)] +
+                [(n, ctypes.c_int32) for n in ("fuse_heads", "fused_away", "parent", "n_children")] +
+                [("children", ctypes.c_int32 * CP_MAX_HEADS)])
+
+
+class CpOpLaunch(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_int32) for n in ("family", "BN", "ksplit", "grid")]
 
 
 class CpConfig(ctypes.Structure):
@@ -125,6 +156,9 @@ def load():
     L.cp_plan_num_ops.argtypes = [vp]
     L.cp_plan_profile.argtypes = [vp, i32, vp, vp, vp, vp, ctypes.POINTER(vp), vp, ctypes.POINTER(CpOpStat), i32,
                                   ctypes.POINTER(i32)]
+    L.cp_plan_op_desc.argtypes = [vp, i32, ctypes.POINTER(CpOpDesc)]
+    L.cp_plan_arena.argtypes = [vp, ctypes.POINTER(vp), ctypes.POINTER(i64)]
+    L.cp_plan_run_ops.argtypes = [vp, i32, i32, i32, vp, vp, vp, vp, ctypes.POINTER(vp), vp, ctypes.POINTER(CpOpLaunch)]
     L.cp_plan_bytes.argtypes = [vp]
     L.cp_plan_bytes.restype = i64
     L.cp_plan_forward_launches.argtypes = [vp]

@@ -80,6 +80,13 @@ struct IgemmParams {
 
 int launch_igemm_fp32(const IgemmParams& p, cudaStream_t stream);
 
+// What a tensor-core launcher decided for one launch (reported to cp_plan_run_ops; null = not wanted).
+struct LaunchInfo {
+  int BN = 0;           // N tile
+  int ksplit = 1;       // split-K factor (1 = off)
+  long long grid = 0;   // CTAs of the main kernel
+};
+
 // dedicated 7x7 stem kernel (stem_conv.cu); consumes the same packed fp32 weights as the generic kernel
 bool conv3_c16_supported(const IgemmParams& p);     // direct 3x3 16 -> 16 NHWC convolution (stem_conv.cu)
 int launch_conv3_c16(const IgemmParams& p, cudaStream_t stream);
@@ -91,7 +98,7 @@ bool umma_supported(const IgemmParams& p, int prec);
 size_t umma_weight_bytes(int Kreal, int CoutPad, int prec);
 int launch_pack_umma_weight(const float* src_k_by_ld, int ld, int Kreal, int Cout, int CoutPad, int prec, void* dst,
                             cudaStream_t s);
-int launch_igemm_umma(const IgemmParams& p, int prec, cudaStream_t stream);
+int launch_igemm_umma(const IgemmParams& p, int prec, cudaStream_t stream, LaunchInfo* info = nullptr);
 
 // elementwise / data-movement kernels (elementwise.cu)
 int launch_maxpool2(const float* in, float* out, int B, int H, int W, int C, cudaStream_t s);
@@ -108,8 +115,11 @@ int launch_pack_up_weight(const float* w_c1kk, float* out_kkc, int C, int k, cud
 int launch_nchw_to_nhwc(const float* in, float* out, int B, int C, int H, int W, int outStride,
                         int chanOffset, cudaStream_t s);
 int launch_nhwc_to_nchw(const float* in, float* out, int B, int C, int H, int W, int inStride, cudaStream_t s);
+// GroupNorm+ReLU workspace: gn_workspace_doubles(B) doubles (statistics + per-block partial sums)
+constexpr int kGnBlocks = 64, kGnMaxGroups = 64;
+inline size_t gn_workspace_doubles(int B) { return (size_t)B * kGnMaxGroups * 2 * (1 + kGnBlocks); }
 int launch_group_norm_relu(float* x, const float* gamma, const float* beta, int B, int HW, int C,
-                           int stride, int chanOffset, int groups, float eps, float* stats, cudaStream_t s);
+                           int stride, int chanOffset, int groups, float eps, double* ws, cudaStream_t s);
 int launch_gru_gates(const float* xi, const float* hh, const float* hprev, float* hout, int B_HW, int C,
                      int first_step, cudaStream_t s);
 
@@ -130,9 +140,11 @@ int tma_encode_nhwc_box(const float* base, int C, int W, int H, int B, int strid
 bool dcn_tma_supported(const IgemmParams& p, int x3);
 int dcn_tma_tile_n(int CoutPad, int x3);
 int dcn_tma_encode(const IgemmParams& p, int Bmax, void* map_out /* 128 bytes, 64-byte aligned */);
-int launch_dcn_tma(const IgemmParams& p, const void* map, int x3, int round_out_tf32, cudaStream_t stream);
+int launch_dcn_tma(const IgemmParams& p, const void* map, int x3, int round_out_tf32, cudaStream_t stream,
+                   LaunchInfo* info = nullptr);
 int tma_conv_encode(const IgemmParams& p, int Bmax, int x3, void* maps_out /* 4 x 128 bytes */);
-int launch_conv_tma(const IgemmParams& p, const void* maps, int round_out_tf32, int x3, cudaStream_t stream);
+int launch_conv_tma(const IgemmParams& p, const void* maps, int round_out_tf32, int x3, cudaStream_t stream,
+                    LaunchInfo* info = nullptr);
 
 inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
 

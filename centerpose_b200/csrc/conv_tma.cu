@@ -688,7 +688,8 @@ static int launch_conv_tma_kernel(const TmaConvParams& q, const cudaLaunchConfig
   return CP_OK;
 }
 
-int launch_conv_tma(const IgemmParams& p, const void* maps, int round_out_tf32, int x3, cudaStream_t stream) {
+int launch_conv_tma(const IgemmParams& p, const void* maps, int round_out_tf32, int x3, cudaStream_t stream,
+                    LaunchInfo* info) {
   if (!p.wgt_umma) return fail(CP_ERR_INVALID, "conv_tma: weight tiles missing");
   TmaConvParams q;
   memset(&q, 0, sizeof(q));
@@ -778,6 +779,11 @@ int launch_conv_tma(const IgemmParams& p, const void* maps, int round_out_tf32, 
   int rc = x3 ? (q.fuse ? launch_conv_tma_kernel<true, true>(q, cfg) : launch_conv_tma_kernel<true, false>(q, cfg))
               : (q.fuse ? launch_conv_tma_kernel<false, true>(q, cfg) : launch_conv_tma_kernel<false, false>(q, cfg));
   if (rc) return rc;
+  if (info) {
+    info->BN = q.BN;
+    info->ksplit = q.ksplit;
+    info->grid = cfg.gridDim.x;
+  }
   if (q.ksplit > 1) {
     const long long mn = q.total_tiles / q.ksplit;
     const long long threads = mn * (q.BN / 4) * q.tile_m;

@@ -522,7 +522,8 @@ int dcn_tma_encode(const IgemmParams& p, int Bmax, void* map_out) {
   return tma_encode_nhwc_box(p.src[0], p.srcC[0], p.Win, p.Hin, Bmax, p.srcStride[0], DT_CS, DT_SW, DT_SH, 1, map_out);
 }
 
-int launch_dcn_tma(const IgemmParams& p, const void* map, int x3, int round_out_tf32, cudaStream_t stream) {
+int launch_dcn_tma(const IgemmParams& p, const void* map, int x3, int round_out_tf32, cudaStream_t stream,
+                   LaunchInfo* info) {
   if (!p.wgt_umma) return fail(CP_ERR_INVALID, "dcn_tma: weight tiles missing");
   if (!dcn_tma_supported(p, x3)) return fail(CP_ERR_INVALID, "dcn_tma: unsupported shape");
   DcnTmaParams q;
@@ -605,6 +606,11 @@ int launch_dcn_tma(const IgemmParams& p, const void* map, int x3, int round_out_
   const unsigned grid = (unsigned)(q.total_tiles < num_sms ? q.total_tiles : num_sms);
   CP_CUDA_CHECK(launch_kernel(kern, dim3(grid), dim3(DT_THREADS), smem, stream, q));
   CP_LAUNCH_CHECK("dcn_tma_kernel");
+  if (info) {
+    info->BN = q.BN;
+    info->ksplit = q.ksplit;
+    info->grid = grid;
+  }
   if (q.ksplit > 1) {
     const long long threads = mn * (q.BN / 4) * 128;
     CP_CUDA_CHECK(launch_kernel(dcn_tma_splitk_finish, dim3((unsigned)((threads + 255) / 256)), dim3(256), 0, stream, q, mn));

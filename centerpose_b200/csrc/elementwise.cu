@@ -167,34 +167,53 @@ __global__ void nhwc_to_nchw_kernel(const float* __restrict__ in, float* __restr
 }
 
 // ---- GroupNorm(groups, C) + ReLU over an NHWC channel slice (GN.py:4-9) -------
-// pass 1: per (sample, group) sum / sum-of-squares in double via atomics
+// pass 1: per (sample, block, group) partial sum / sum-of-squares in double, each added in a fixed order so that the
+// statistics -- and the normalised output -- are bit-reproducible from run to run
 __global__ void gn_stats_kernel(const float* __restrict__ x, int HW, int C, int stride, int chanOffset,
-                                int groups, double* __restrict__ stats) {
-  // grid: (chunks, B); each block reduces a slab of pixels for all groups
+                                int groups, double* __restrict__ partial) {
+  // grid: (kGnBlocks, B); each block reduces a slab of pixels for all groups
   const int n = blockIdx.y;
   const int cpg = C / groups;
-  extern __shared__ double sh[];  // [groups][2]
-  for (int i = threadIdx.x; i < groups * 2; i += blockDim.x) sh[i] = 0.0;
-  __syncthreads();
+  __shared__ double sh_s[TPB], sh_q[TPB];
   const int pix_per_block = (HW + gridDim.x - 1) / gridDim.x;
   const int p0 = blockIdx.x * pix_per_block;
   const int p1 = min(HW, p0 + pix_per_block);
   // thread t owns channel t % C and strides over pixels with the other C-lanes
-  {
-    const int c = threadIdx.x % C;
-    const int lane = threadIdx.x / C;
-    const int nl = blockDim.x / C;
-    double s = 0.0, q = 0.0;
-    for (int pidx = p0 + lane; pidx < p1; pidx += nl) {
-      float v = __ldg(x + ((size_t)n * HW + pidx) * stride + chanOffset + c);
-      s += v;
-      q += (double)v * v;
-    }
-    atomicAdd(&sh[(c / cpg) * 2], s);
-    atomicAdd(&sh[(c / cpg) * 2 + 1], q);
+  const int c = threadIdx.x % C;
+  const int lane = threadIdx.x / C;
+  const int nl = blockDim.x / C;
+  double s = 0.0, q = 0.0;
+  for (int pidx = p0 + lane; pidx < p1; pidx += nl) {
+    float v = __ldg(x + ((size_t)n * HW + pidx) * stride + chanOffset + c);
+    s += v;
+    q += (double)v * v;
   }
+  sh_s[threadIdx.x] = s;
+  sh_q[threadIdx.x] = q;
   __syncthreads();
-  for (int i = threadIdx.x; i < groups * 2; i += blockDim.x) atomicAdd(&stats[(size_t)n * groups * 2 + i], sh[i]);
+  if (threadIdx.x < groups) {
+    const int g = threadIdx.x;
+    double ss = 0.0, qq = 0.0;
+    for (int l = 0; l < nl; ++l)
+      for (int cc = g * cpg; cc < (g + 1) * cpg; ++cc) {
+        ss += sh_s[l * C + cc];
+        qq += sh_q[l * C + cc];
+      }
+    double* dst = partial + (((size_t)n * gridDim.x + blockIdx.x) * groups + g) * 2;
+    dst[0] = ss;
+    dst[1] = qq;
+  }
+}
+
+// pass 2: the partials of every (sample, group) added in block order
+__global__ void gn_stats_finish_kernel(const double* __restrict__ partial, int nblocks, int groups,
+                                       double* __restrict__ stats) {
+  const int n = blockIdx.x;
+  for (int i = threadIdx.x; i < groups * 2; i += blockDim.x) {
+    double t = 0.0;
+    for (int b = 0; b < nblocks; ++b) t += partial[((size_t)n * nblocks + b) * groups * 2 + i];
+    stats[(size_t)n * groups * 2 + i] = t;
+  }
 }
 
 __global__ void gn_apply_relu_kernel(float* __restrict__ x, const float* __restrict__ gamma,
@@ -309,14 +328,16 @@ int launch_nhwc_to_nchw(const float* in, float* out, int B, int C, int H, int W,
 }
 
 int launch_group_norm_relu(float* x, const float* gamma, const float* beta, int B, int HW, int C, int stride,
-                           int chanOffset, int groups, float eps, float* stats_f, cudaStream_t s) {
-  double* stats = reinterpret_cast<double*>(stats_f);
+                           int chanOffset, int groups, float eps, double* ws, cudaStream_t s) {
   if (C > 256 || 256 % C != 0) return fail(CP_ERR_INVALID, "group_norm: C must divide 256");
-  cudaError_t e = cudaMemsetAsync(stats, 0, sizeof(double) * (size_t)B * groups * 2, s);
-  if (e != cudaSuccess) return fail(CP_ERR_CUDA, "group_norm memset");
-  dim3 grid(64, B);
-  gn_stats_kernel<<<grid, 256, sizeof(double) * groups * 2, s>>>(x, HW, C, stride, chanOffset, groups, stats);
+  if (groups <= 0 || groups > kGnMaxGroups || C % groups) return fail(CP_ERR_INVALID, "group_norm: bad group count");
+  double* stats = ws;                                   // [B][groups][2]
+  double* partial = ws + (size_t)B * kGnMaxGroups * 2;   // [B][kGnBlocks][groups][2]
+  dim3 grid(kGnBlocks, B);
+  gn_stats_kernel<<<grid, TPB, 0, s>>>(x, HW, C, stride, chanOffset, groups, partial);
   CP_LAUNCH_CHECK("gn_stats_kernel");
+  gn_stats_finish_kernel<<<B, 64, 0, s>>>(partial, kGnBlocks, groups, stats);
+  CP_LAUNCH_CHECK("gn_stats_finish_kernel");
   size_t total = (size_t)B * HW * C;
   gn_apply_relu_kernel<<<blocks_for(total), TPB, 0, s>>>(x, gamma, beta, B, HW, C, stride, chanOffset, groups,
                                                          eps, stats);

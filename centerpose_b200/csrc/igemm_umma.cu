@@ -391,7 +391,8 @@ int launch_pack_umma_weight(const float* src, int ld, int Kreal, int Cout, int C
 }
 
 template <int PREC, int BN>
-static int launch_igemm_umma_bn(const IgemmParams& p, int stages, size_t smem, int nacc, cudaStream_t stream) {
+static int launch_igemm_umma_bn(const IgemmParams& p, int stages, size_t smem, int nacc, cudaStream_t stream,
+                                LaunchInfo* info) {
   void (*kern)(const IgemmParams, const int, const int) =
       (p.mode == IGEMM_DCN) ? igemm_umma_kernel<PREC, IGEMM_DCN, BN> : igemm_umma_kernel<PREC, IGEMM_NHWC_VEC, BN>;
   static PerDevice<bool, 2> configured;
@@ -404,10 +405,15 @@ static int launch_igemm_umma_bn(const IgemmParams& p, int stages, size_t smem, i
   dim3 grid((unsigned)((size_t)(p.CoutPad / BN) * ((M + UM_BM - 1) / UM_BM)));
   CP_CUDA_CHECK(launch_kernel(kern, grid, dim3(UM_THREADS), smem, stream, p, stages, nacc));
   CP_LAUNCH_CHECK("igemm_umma_kernel");
+  if (info) {
+    info->BN = BN;
+    info->ksplit = 1;
+    info->grid = grid.x;
+  }
   return CP_OK;
 }
 
-int launch_igemm_umma(const IgemmParams& p, int prec, cudaStream_t stream) {
+int launch_igemm_umma(const IgemmParams& p, int prec, cudaStream_t stream, LaunchInfo* info) {
   if (!umma_supported(p, prec)) return fail(CP_ERR_INVALID, "igemm_umma: unsupported shape");
   if (!p.wgt_umma) return fail(CP_ERR_INVALID, "igemm_umma: weight tiles missing");
   const int bn = umma_tile_n(p.CoutPad, prec);
@@ -425,16 +431,16 @@ int launch_igemm_umma(const IgemmParams& p, int prec, cudaStream_t stream) {
   const int nacc = prec == 1 ? x3_group_blocks() : 1;
   if (prec == 0) {
     switch (bn) {
-      case 16: return launch_igemm_umma_bn<0, 16>(p, stages, smem, nacc, stream);
-      case 32: return launch_igemm_umma_bn<0, 32>(p, stages, smem, nacc, stream);
-      case 64: return launch_igemm_umma_bn<0, 64>(p, stages, smem, nacc, stream);
-      default: return launch_igemm_umma_bn<0, 128>(p, stages, smem, nacc, stream);
+      case 16: return launch_igemm_umma_bn<0, 16>(p, stages, smem, nacc, stream, info);
+      case 32: return launch_igemm_umma_bn<0, 32>(p, stages, smem, nacc, stream, info);
+      case 64: return launch_igemm_umma_bn<0, 64>(p, stages, smem, nacc, stream, info);
+      default: return launch_igemm_umma_bn<0, 128>(p, stages, smem, nacc, stream, info);
     }
   }
   switch (bn) {
-    case 16: return launch_igemm_umma_bn<1, 16>(p, stages, smem, nacc, stream);
-    case 32: return launch_igemm_umma_bn<1, 32>(p, stages, smem, nacc, stream);
-    default: return launch_igemm_umma_bn<1, 64>(p, stages, smem, nacc, stream);
+    case 16: return launch_igemm_umma_bn<1, 16>(p, stages, smem, nacc, stream, info);
+    case 32: return launch_igemm_umma_bn<1, 32>(p, stages, smem, nacc, stream, info);
+    default: return launch_igemm_umma_bn<1, 64>(p, stages, smem, nacc, stream, info);
   }
 }
 

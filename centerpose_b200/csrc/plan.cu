@@ -669,7 +669,7 @@ int cp_plan_create(const cp_config* cfg, cp_plan** out) {
   CP_CUDA_CHECK(cudaMalloc(&P->act, P->act_floats * sizeof(float)));
   CP_CUDA_CHECK(cudaMalloc(&P->wts, P->w_floats * sizeof(float)));
   CP_CUDA_CHECK(cudaMemset(P->wts, 0, P->w_floats * sizeof(float)));
-  CP_CUDA_CHECK(cudaMalloc(&P->gn_stats, sizeof(double) * (size_t)P->B * 64 * 2));
+  CP_CUDA_CHECK(cudaMalloc(&P->gn_stats, sizeof(double) * gn_workspace_doubles(P->B)));
   if (P->umma_bytes) CP_CUDA_CHECK(cudaMalloc(&P->umma_wts, P->umma_bytes));
   if (P->prec == 1 || P->prec == 2) {
     CP_CUDA_CHECK(cudaMalloc(&P->splitk_ws, kSplitkWsFloats * sizeof(float)));
@@ -710,7 +710,7 @@ int cp_plan_create(const cp_config* cfg, cp_plan** out) {
     if (rc2) return rc2;
   }
   int n = 0;
-  for (auto& op : P->ops) n += op.fused_away ? 0 : ((op.type == OP_GN_RELU) ? 2 : 1);
+  for (auto& op : P->ops) n += op.fused_away ? 0 : ((op.type == OP_GN_RELU) ? 3 : 1);
   P->launches = n;
   *out = P.release();
   return CP_OK;
@@ -823,6 +823,152 @@ static bool pdl_wanted(long long pixels) {
   return pixels <= 8ll * 512 * 512;
 }
 
+// Kernel parameters of conv op `op` at batch `batch`.  ext[] may hold nulls (family queries); run_op rejects them.
+static void igemm_params(const cp_plan* P, const Op& op, int batch, const float* const ext[4], float* const* head_out,
+                         IgemmParams* pp) {
+  IgemmParams& p = *pp;
+  p = IgemmParams{};
+  p.nsrc = op.nsrc;
+  for (int i = 0; i < op.nsrc; ++i) {
+    const Act& a = op.src[i];
+    p.src[i] = a.ext >= 0 ? ext[a.ext] : P->act + a.off;
+    p.srcC[i] = a.C;
+    p.srcStride[i] = a.stride;
+  }
+  p.B = batch;
+  p.Hin = op.src[0].H;
+  p.Win = op.src[0].W;
+  p.Cin = op.Cin;
+  p.kh = op.kh;
+  p.kw = op.kw;
+  p.stride = op.stride;
+  p.pad = op.pad;
+  p.Hout = (p.Hin + 2 * op.pad - op.kh) / op.stride + 1;
+  p.Wout = (p.Win + 2 * op.pad - op.kw) / op.stride + 1;
+  p.Cout = op.Cout;
+  p.CoutPad = op.CoutPad;
+  p.Kpad = op.Kpad;
+  p.wgt = P->wts + op.w_off;
+  p.bias = P->wts + op.b_off;
+  p.residual = op.has_res ? P->act + op.res.off : nullptr;
+  p.resStride = op.res.stride;
+  p.relu = op.relu;
+  p.res_after_relu = op.res_after_relu;
+  if (op.out_head >= 0) {
+    p.out = head_out ? head_out[op.out_head] : nullptr;
+    p.out_nchw = 1;
+    p.outStride = 0;
+  } else {
+    p.out = P->act + op.out.off;
+    p.outStride = op.out.stride;
+  }
+  if (op.mode == IGEMM_DCN) {
+    p.offmask = P->act + op.om.off;
+    p.omStride = op.om.stride;
+    p.mask_is_logit = 1;
+  }
+  p.mode = op.mode;
+  if (op.fuse_heads) {
+    p.fuse_n = (int)op.head_children.size();
+    p.fuse_hidden = P->cfg.head_conv;
+    for (int i = 0; i < p.fuse_n; ++i) {
+      const Op& ch = P->ops[op.head_children[i]];
+      p.fuse_w[i] = P->wts + ch.w_off;
+      p.fuse_b[i] = P->wts + ch.b_off;
+      p.fuse_out[i] = head_out ? head_out[ch.out_head] : nullptr;
+      p.fuse_cout[i] = ch.Cout;
+    }
+  }
+}
+
+// Kernel family of conv op `op` for the launch parameters `p` (the order of the dispatch in run_op).
+static int igemm_family(const Op& op, const IgemmParams& p) {
+  if (op.use_dcn_tma) return CP_FAM_DCN_TMA;
+  if (op.use_tma) return CP_FAM_CONV_TMA;
+  if (op.use_umma) return CP_FAM_IGEMM_UMMA;
+  if (stem_supported(p)) return CP_FAM_STEM;
+  if (conv3_c16_supported(p)) return CP_FAM_CONV3_C16;
+  return CP_FAM_IGEMM_FP32;
+}
+
+// One op of the schedule, as cp_forward runs it.  `info` (may be null) receives what the launcher decided.
+static int run_op(cp_plan* P, size_t idx, int batch, const float* const ext[4], float* const* head_out, cudaStream_t s,
+                  cp_op_launch* info) {
+  int rc;
+  const Op& op = P->ops[idx];
+  cp_op_launch li{};
+  li.ksplit = 1;
+  if (op.fused_away) {          // computed inside the epilogue of the merged heads conv
+    if (info) *info = li;
+    return CP_OK;
+  }
+  switch (op.type) {
+    case OP_IGEMM: {
+      for (int i = 0; i < op.nsrc; ++i)
+        if (op.src[i].ext >= 0 && !ext[op.src[i].ext]) return fail(CP_ERR_INVALID, "cp_forward: a tracking input tensor is null");
+      IgemmParams p;
+      igemm_params(P, op, batch, ext, head_out, &p);
+      LaunchInfo tc;
+      li.family = igemm_family(op, p);
+      if (op.use_dcn_tma) {
+        p.wgt_umma = P->umma_wts + op.umma_off;
+        p.splitk_ws = P->splitk_ws;
+        p.splitk_ws_floats = P->splitk_ws ? kSplitkWsFloats : 0;
+        const unsigned char* mp = (const unsigned char*)(((uintptr_t)op.tma_maps.data() + 63) & ~(uintptr_t)63);
+        if ((rc = launch_dcn_tma(p, mp, P->prec == 1, P->prec == 2, s, &tc))) return rc;
+      } else if (op.use_tma) {
+        p.wgt_umma = P->umma_wts + op.umma_off;
+        p.splitk_ws = P->splitk_ws;
+        p.splitk_ws_floats = P->splitk_ws ? kSplitkWsFloats : 0;
+        const unsigned char* mp = (const unsigned char*)(((uintptr_t)op.tma_maps.data() + 63) & ~(uintptr_t)63);
+        if ((rc = launch_conv_tma(p, mp, P->prec == 2, P->prec == 1, s, &tc))) return rc;
+      } else if (op.use_umma) {
+        p.wgt_umma = P->umma_wts + op.umma_off;
+        if ((rc = launch_igemm_umma(p, P->prec == 2 ? 1 : P->prec, s, &tc))) return rc;
+      } else if (li.family == CP_FAM_STEM) {
+        if ((rc = launch_stem_conv(p, s))) return rc;
+      } else if (li.family == CP_FAM_CONV3_C16) {
+        if ((rc = launch_conv3_c16(p, s))) return rc;
+      } else if ((rc = launch_igemm_fp32(p, s))) {
+        return rc;
+      }
+      li.BN = tc.BN;
+      li.ksplit = tc.ksplit;
+      li.grid = (int32_t)tc.grid;
+      break;
+    }
+    case OP_MAXPOOL:
+      li.family = CP_FAM_MAXPOOL;
+      if ((rc = launch_maxpool2(P->act + op.src[0].off, P->act + op.out.off, batch, op.src[0].H, op.src[0].W,
+                                op.src[0].C, s)))
+        return rc;
+      break;
+    case OP_UPADD:
+      li.family = CP_FAM_UPADD;
+      if ((rc = launch_upsample_add(P->act + op.src[0].off, P->wts + op.upw_off,
+                                    op.has_skip ? P->act + op.skip.off : nullptr, P->act + op.out.off, batch,
+                                    op.src[0].H, op.src[0].W, op.src[0].C, op.f, s)))
+        return rc;
+      break;
+    case OP_GN_RELU:
+      li.family = CP_FAM_GN_RELU;
+      if ((rc = launch_group_norm_relu(P->act + op.out.off, P->wts + op.gamma_off, P->wts + op.beta_off, batch,
+                                       op.out.H * op.out.W, op.out.C, op.out.stride, 0, op.groups, 1e-5f,
+                                       P->gn_stats, s)))
+        return rc;
+      break;
+    case OP_GRU:
+      li.family = CP_FAM_GRU;
+      if ((rc = launch_gru_gates(P->act + op.gx.off, op.first_step ? nullptr : P->act + op.gh.off,
+                                 op.first_step ? nullptr : P->act + op.gprev.off, P->act + op.out.off,
+                                 batch * op.out.H * op.out.W, op.out.C, op.first_step, s)))
+        return rc;
+      break;
+  }
+  if (info) *info = li;
+  return CP_OK;
+}
+
 static int run_forward(cp_plan* P, int batch, const float* const ext[4], float* const* head_out, cudaStream_t s,
                        ProfCtx* prof = nullptr) {
   int rc;
@@ -832,121 +978,14 @@ static int run_forward(cp_plan* P, int batch, const float* const ext[4], float* 
     explicit PdlScope(int on) { g_pdl = on; }
     ~PdlScope() { g_pdl = 0; }
   } pdl_scope(!prof && pdl_wanted((long long)batch * P->H * P->W));
-  for (auto& op : P->ops) {
+  for (size_t i = 0; i < P->ops.size(); ++i) {
     if (prof) {
       cudaEvent_t e;
       CP_CUDA_CHECK(cudaEventCreate(&e));
       CP_CUDA_CHECK(cudaEventRecord(e, s));
       prof->ev.push_back(e);
     }
-    if (op.fused_away) continue;          // computed inside the epilogue of the merged heads conv
-    switch (op.type) {
-      case OP_IGEMM: {
-        IgemmParams p{};
-        p.nsrc = op.nsrc;
-        for (int i = 0; i < op.nsrc; ++i) {
-          const Act& a = op.src[i];
-          if (a.ext >= 0) {
-            if (!ext[a.ext]) return fail(CP_ERR_INVALID, "cp_forward: a tracking input tensor is null");
-            p.src[i] = ext[a.ext];
-          } else {
-            p.src[i] = P->act + a.off;
-          }
-          p.srcC[i] = a.C;
-          p.srcStride[i] = a.stride;
-        }
-        p.B = batch;
-        p.Hin = op.src[0].H;
-        p.Win = op.src[0].W;
-        p.Cin = op.Cin;
-        p.kh = op.kh;
-        p.kw = op.kw;
-        p.stride = op.stride;
-        p.pad = op.pad;
-        p.Hout = (p.Hin + 2 * op.pad - op.kh) / op.stride + 1;
-        p.Wout = (p.Win + 2 * op.pad - op.kw) / op.stride + 1;
-        p.Cout = op.Cout;
-        p.CoutPad = op.CoutPad;
-        p.Kpad = op.Kpad;
-        p.wgt = P->wts + op.w_off;
-        p.bias = P->wts + op.b_off;
-        p.residual = op.has_res ? P->act + op.res.off : nullptr;
-        p.resStride = op.res.stride;
-        p.relu = op.relu;
-        p.res_after_relu = op.res_after_relu;
-        if (op.out_head >= 0) {
-          p.out = head_out[op.out_head];
-          p.out_nchw = 1;
-          p.outStride = 0;
-        } else {
-          p.out = P->act + op.out.off;
-          p.outStride = op.out.stride;
-        }
-        if (op.mode == IGEMM_DCN) {
-          p.offmask = P->act + op.om.off;
-          p.omStride = op.om.stride;
-          p.mask_is_logit = 1;
-        }
-        p.mode = op.mode;
-        if (op.fuse_heads) {
-          p.fuse_n = (int)op.head_children.size();
-          p.fuse_hidden = P->cfg.head_conv;
-          for (int i = 0; i < p.fuse_n; ++i) {
-            const Op& ch = P->ops[op.head_children[i]];
-            p.fuse_w[i] = P->wts + ch.w_off;
-            p.fuse_b[i] = P->wts + ch.b_off;
-            p.fuse_out[i] = head_out[ch.out_head];
-            p.fuse_cout[i] = ch.Cout;
-          }
-        }
-        if (op.use_dcn_tma) {
-          p.wgt_umma = P->umma_wts + op.umma_off;
-          p.splitk_ws = P->splitk_ws;
-          p.splitk_ws_floats = P->splitk_ws ? kSplitkWsFloats : 0;
-          const unsigned char* mp = (const unsigned char*)(((uintptr_t)op.tma_maps.data() + 63) & ~(uintptr_t)63);
-          if ((rc = launch_dcn_tma(p, mp, P->prec == 1, P->prec == 2, s))) return rc;
-        } else if (op.use_tma) {
-          p.wgt_umma = P->umma_wts + op.umma_off;
-          p.splitk_ws = P->splitk_ws;
-          p.splitk_ws_floats = P->splitk_ws ? kSplitkWsFloats : 0;
-          const unsigned char* mp = (const unsigned char*)(((uintptr_t)op.tma_maps.data() + 63) & ~(uintptr_t)63);
-          if ((rc = launch_conv_tma(p, mp, P->prec == 2, P->prec == 1, s))) return rc;
-        } else if (op.use_umma) {
-          p.wgt_umma = P->umma_wts + op.umma_off;
-          if ((rc = launch_igemm_umma(p, P->prec == 2 ? 1 : P->prec, s))) return rc;
-        } else if (stem_supported(p)) {
-          if ((rc = launch_stem_conv(p, s))) return rc;
-        } else if (conv3_c16_supported(p)) {
-          if ((rc = launch_conv3_c16(p, s))) return rc;
-        } else if ((rc = launch_igemm_fp32(p, s))) {
-          return rc;
-        }
-        break;
-      }
-      case OP_MAXPOOL:
-        if ((rc = launch_maxpool2(P->act + op.src[0].off, P->act + op.out.off, batch, op.src[0].H, op.src[0].W,
-                                  op.src[0].C, s)))
-          return rc;
-        break;
-      case OP_UPADD:
-        if ((rc = launch_upsample_add(P->act + op.src[0].off, P->wts + op.upw_off,
-                                      op.has_skip ? P->act + op.skip.off : nullptr, P->act + op.out.off, batch,
-                                      op.src[0].H, op.src[0].W, op.src[0].C, op.f, s)))
-          return rc;
-        break;
-      case OP_GN_RELU:
-        if ((rc = launch_group_norm_relu(P->act + op.out.off, P->wts + op.gamma_off, P->wts + op.beta_off, batch,
-                                         op.out.H * op.out.W, op.out.C, op.out.stride, 0, op.groups, 1e-5f,
-                                         (float*)P->gn_stats, s)))
-          return rc;
-        break;
-      case OP_GRU:
-        if ((rc = launch_gru_gates(P->act + op.gx.off, op.first_step ? nullptr : P->act + op.gh.off,
-                                   op.first_step ? nullptr : P->act + op.gprev.off, P->act + op.out.off,
-                                   batch * op.out.H * op.out.W, op.out.C, op.first_step, s)))
-          return rc;
-        break;
-    }
+    if ((rc = run_op(P, i, batch, ext, head_out, s, nullptr))) return rc;
   }
   if (prof) {
     cudaEvent_t e;
@@ -1031,6 +1070,112 @@ int cp_plan_profile(cp_plan* P, int32_t batch, const float* images, const float*
   }
   for (auto e : ctx.ev) cudaEventDestroy(e);
   return rc;
+}
+
+static void act_desc(const Act& a, cp_act_desc* d) {
+  d->off = a.ext >= 0 || a.C == 0 ? -1 : (int64_t)a.off;
+  d->ext = a.ext;
+  d->C = a.C;
+  d->H = a.H;
+  d->W = a.W;
+  d->stride = a.stride;
+}
+
+int cp_plan_op_desc(const cp_plan* P, int32_t i, cp_op_desc* d) {
+  if (!P || !d) return fail(CP_ERR_INVALID, "cp_plan_op_desc: null argument");
+  if (i < 0 || i >= (int)P->ops.size()) return fail(CP_ERR_INVALID, "cp_plan_op_desc: op index out of range");
+  const Op& op = P->ops[i];
+  memset(d, 0, sizeof(*d));
+  snprintf(d->name, sizeof(d->name), "%s", op.name.c_str());
+  d->kind = (int)op.type * 10 + (op.type == OP_IGEMM ? op.mode : 0);
+  d->nsrc = op.nsrc;
+  for (int k = 0; k < 4; ++k) act_desc(op.src[k], &d->src[k]);
+  if (op.type != OP_IGEMM) act_desc(op.src[0], &d->src[0]);
+  act_desc(op.out, &d->out);
+  d->out_head = op.out_head;
+  if (op.out_head >= 0) d->out.off = -1;
+  d->kh = op.kh;
+  d->stride = op.stride;
+  d->pad = op.pad;
+  d->Cin = op.Cin;
+  d->Cout = op.Cout;
+  d->CoutPad = op.CoutPad;
+  d->Kpad = op.Kpad;
+  d->relu = op.relu;
+  d->has_res = op.has_res;
+  d->res_after_relu = op.res_after_relu;
+  act_desc(op.res, &d->res);
+  act_desc(op.om, &d->om);
+  act_desc(op.skip, &d->skip);
+  act_desc(op.gx, &d->gx);
+  act_desc(op.gh, &d->gh);
+  act_desc(op.gprev, &d->gprev);
+  d->parent = -1;
+  switch (op.type) {
+    case OP_IGEMM: {
+      d->w = P->wts + op.w_off;
+      d->w_ld = op.w_ld;
+      d->bias = P->wts + op.b_off;
+      const float* ext[4] = {nullptr, nullptr, nullptr, nullptr};
+      IgemmParams p;
+      igemm_params(P, op, P->B, ext, nullptr, &p);
+      d->family = igemm_family(op, p);
+      d->x3 = (op.use_tma || op.use_dcn_tma) ? P->prec == 1 : (op.use_umma ? P->prec != 0 : 0);
+      break;
+    }
+    case OP_MAXPOOL: d->family = CP_FAM_MAXPOOL; break;
+    case OP_UPADD:
+      d->family = CP_FAM_UPADD;
+      d->up_w = P->wts + op.upw_off;
+      d->f = op.f;
+      d->has_skip = op.has_skip;
+      break;
+    case OP_GN_RELU:
+      d->family = CP_FAM_GN_RELU;
+      d->gamma = P->wts + op.gamma_off;
+      d->beta = P->wts + op.beta_off;
+      d->groups = op.groups;
+      break;
+    case OP_GRU:
+      d->family = CP_FAM_GRU;
+      d->first_step = op.first_step;
+      break;
+  }
+  d->fuse_heads = op.fuse_heads;
+  d->fused_away = op.fused_away;
+  d->n_children = (int)op.head_children.size();
+  for (int k = 0; k < d->n_children && k < CP_MAX_HEADS; ++k) d->children[k] = op.head_children[k];
+  if (op.fused_away) {
+    d->family = CP_FAM_NONE;
+    for (int j = 0; j < (int)P->ops.size(); ++j)
+      for (int c : P->ops[j].head_children)
+        if (c == i) d->parent = j;
+  }
+  return CP_OK;
+}
+
+int cp_plan_arena(const cp_plan* P, float** act, int64_t* floats) {
+  if (!P || !act || !floats) return fail(CP_ERR_INVALID, "cp_plan_arena: null argument");
+  *act = P->act;
+  *floats = (int64_t)P->act_floats;
+  return CP_OK;
+}
+
+int cp_plan_run_ops(cp_plan* P, int32_t batch, int32_t first, int32_t last, const float* images, const float* pre_img,
+                    const float* pre_hm, const float* pre_hm_hp, float* const* head_out, void* stream,
+                    cp_op_launch* info) {
+  if (!P || !images || !head_out) return fail(CP_ERR_INVALID, "cp_plan_run_ops: null argument");
+  if (!P->loaded) return fail(CP_ERR_NOT_LOADED, "cp_plan_run_ops: call cp_plan_load_weights first");
+  if (batch <= 0 || batch > P->B) return fail(CP_ERR_INVALID, "cp_plan_run_ops: batch exceeds the plan's max_batch");
+  if (first < 0 || last < first || last > (int)P->ops.size())
+    return fail(CP_ERR_INVALID, "cp_plan_run_ops: op range outside the schedule");
+  const float* ext[4] = {images, pre_img, pre_hm, pre_hm_hp};
+  g_pdl = 0;
+  for (int32_t i = first; i < last; ++i) {
+    int rc = run_op(P, (size_t)i, batch, ext, head_out, (cudaStream_t)stream, info ? info + (i - first) : nullptr);
+    if (rc) return rc;
+  }
+  return CP_OK;
 }
 
 int cp_infer(cp_plan* P, int32_t batch, const float* images, const float* pre_img, const float* pre_hm,

@@ -115,6 +115,18 @@ def decode_pnp(heads, meta, prm, want_dets=True):
     return dets, poses, n_valid
 
 
+class _CudaArray(object):
+    """__cuda_array_interface__ of plan-owned fp32 device memory (torch.as_tensor wraps it without a copy)."""
+
+    def __init__(self, ptr, n):
+        self.__cuda_array_interface__ = {"shape": (n,), "typestr": "<f4", "data": (ptr, False), "version": 3}
+
+
+def _device_view(ptr, n, device):
+    with torch.cuda.device(device):
+        return torch.as_tensor(_CudaArray(ptr, n), device=device)
+
+
 class Engine(object):
     def __init__(self, arch, heads, head_conv, max_batch, height, width, device_index, tracking=False,
                  tracking_task_gru=False, precision="fp32"):
@@ -239,6 +251,57 @@ class Engine(object):
         _lib.check(rc, "cp_plan_profile")
         return [dict(name=stats[i].name.decode(), kind=int(stats[i].kind), ms=float(stats[i].ms),
                      flops=float(stats[i].flops), bytes=float(stats[i].bytes)) for i in range(n.value)]
+
+    # ---- diagnostics (per-layer parity tests): the schedule as data, and one op at a time ----
+    @staticmethod
+    def _act(a):
+        return dict(off=int(a.off), ext=int(a.ext), C=int(a.C), H=int(a.H), W=int(a.W), stride=int(a.stride))
+
+    def op_descs(self):
+        """cp_plan_op_desc of every op: list of dicts (device pointers as ints, activations as dicts of cp_act_desc)."""
+        out = []
+        for i in range(int(self.L.cp_plan_num_ops(self.plan))):
+            d = _lib.CpOpDesc()
+            _lib.check(self.L.cp_plan_op_desc(self.plan, i, ctypes.byref(d)), "cp_plan_op_desc")
+            r = {}
+            for name, _ in _lib.CpOpDesc._fields_:
+                v = getattr(d, name)
+                if isinstance(v, _lib.CpActDesc):
+                    v = self._act(v)
+                elif name == "src":
+                    v = [self._act(a) for a in v][:max(1, int(d.nsrc))]
+                elif name == "children":
+                    v = [int(c) for c in v][:int(d.n_children)]
+                elif name == "name":
+                    v = v.decode()
+                elif v is None:
+                    v = 0
+                r[name] = v
+            r["index"] = i
+            out.append(r)
+        return out
+
+    def arena(self):
+        """The activation arena as a flat fp32 CUDA tensor (a view of plan-owned memory, valid while the plan lives)."""
+        p, n = ctypes.c_void_p(), ctypes.c_int64()
+        _lib.check(self.L.cp_plan_arena(self.plan, ctypes.byref(p), ctypes.byref(n)), "cp_plan_arena")
+        return _device_view(p.value, int(n.value), self.device)
+
+    def run_ops(self, x, first, last, out, pre_img=None, pre_hm=None, pre_hm_hp=None):
+        """cp_plan_run_ops: ops [first, last) at batch x.shape[0] into the head tensors `out` (dict, as forward()).
+        Returns one dict(family, BN, ksplit, grid) per op."""
+        B, xs = self._check_inputs(x, pre_img, pre_hm, pre_hm_hp)
+        for n, c in self.heads.items():
+            self._out_tensor(out[n], "out[%s]" % n, (B, c, self.height // 4, self.width // 4), torch.float32)
+        hp = (ctypes.c_void_p * len(self.head_names))(*[out[n].data_ptr() for n in self.head_names])
+        n = max(0, last - first)
+        info = (_lib.CpOpLaunch * max(1, n))()
+        with torch.cuda.device(self.device):
+            rc = self.L.cp_plan_run_ops(self.plan, B, first, last, _ptr(xs[0]), _ptr(xs[1]), _ptr(xs[2]), _ptr(xs[3]),
+                                        hp, _stream(), info)
+        _lib.check(rc, "cp_plan_run_ops")
+        return [dict(family=int(info[i].family), BN=int(info[i].BN), ksplit=int(info[i].ksplit),
+                     grid=int(info[i].grid)) for i in range(n)]
 
     def infer(self, x, meta, prm, pre_img=None, pre_hm=None, pre_hm_hp=None, heads_out=None, want_dets=False,
               poses=None, n_valid=None, dets=None):

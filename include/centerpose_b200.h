@@ -139,6 +139,70 @@ int cp_plan_profile(cp_plan* plan, int32_t batch, const float* images, const flo
                     const float* pre_hm, const float* pre_hm_hp, float* const* head_out, void* stream,
                     cp_op_stat* stats, int32_t max_stats, int32_t* n_stats);
 
+/* ---- diagnostics: inspect and step the schedule (per-layer parity tests) ----------------------------------------
+ * cp_plan_op_desc describes op i of the schedule as the plan stores it; cp_plan_arena gives the activation arena every
+ * cp_act_desc points into; cp_plan_run_ops runs ops [first, last) exactly as cp_forward does (PDL off) and reports for
+ * each one what its launcher decided.  Together they let a test snapshot an op's inputs, run the op alone and compare
+ * its output with an independent evaluation.  Not needed for inference. */
+enum cp_op_family {
+  CP_FAM_NONE = 0,          /* not launched (fused into its parent's epilogue)              */
+  CP_FAM_IGEMM_FP32 = 1,    /* generic fp32 CUDA-core implicit GEMM (igemm_fp32.cu)          */
+  CP_FAM_STEM = 2,          /* 7x7 NCHW stem (stem_conv.cu)                                   */
+  CP_FAM_CONV3_C16 = 3,     /* direct 3x3 16 -> 16 (stem_conv.cu)                             */
+  CP_FAM_IGEMM_UMMA = 4,    /* wgmma gather implicit GEMM (igemm_umma.cu)                     */
+  CP_FAM_CONV_TMA = 5,      /* TMA-fed wgmma convolution (conv_tma.cu)                        */
+  CP_FAM_DCN_TMA = 6,       /* TMA-staged wgmma deformable convolution (dcn_tma.cu)           */
+  CP_FAM_MAXPOOL = 7, CP_FAM_UPADD = 8, CP_FAM_GN_RELU = 9, CP_FAM_GRU = 10
+};
+typedef struct cp_act_desc {
+  int64_t off;              /* floats into the arena: element (n, y, x, c) is at off + ((n*H + y)*W + x)*stride + c,
+                             * n < max_batch; -1 when the slot is unused                                            */
+  int32_t ext;              /* >= 0: external NCHW input instead (0 images, 1 pre_img, 2 pre_hm, 3 pre_hm_hp)       */
+  int32_t C, H, W, stride;
+} cp_act_desc;
+typedef struct cp_op_desc {
+  char name[96];
+  int32_t kind;             /* as cp_op_stat.kind                                                                   */
+  int32_t family;           /* cp_op_family chosen at plan time (fp32 CUDA-core ops: the kernel at max_batch)      */
+  int32_t x3;               /* tensor-core families: 1 = three-term tf32 split, 0 = single pass / bf16              */
+  int32_t nsrc;             /* conv: sources, concatenated along channels in this order                             */
+  cp_act_desc src[4];       /* conv / maxpool / up-sample input (src[0])                                            */
+  cp_act_desc out;          /* output (GroupNorm: the channel slice it normalises in place)                         */
+  int32_t out_head;         /* >= 0: the conv writes head out_head as NCHW instead of `out`                        */
+  int32_t kh, stride, pad, Cin, Cout, CoutPad, Kpad;
+  const float* w;           /* device fp32 [Kpad][w_ld], row k = (ky*kh + kx)*Cin + ci, BN folded               */
+  int32_t w_ld;
+  const float* bias;        /* device fp32 [Cout]                                                                  */
+  int32_t relu, has_res, res_after_relu;   /* out = relu(acc + bias [+ res]) or relu(acc + bias) + res           */
+  cp_act_desc res;
+  cp_act_desc om;           /* deformable conv: raw offset / mask logits (dy, dx of tap k at 2k, 2k+1; mask 18+k) */
+  const float* up_w;        /* up-sample: device fp32 [2f][2f][C] depthwise ConvTranspose weights                 */
+  int32_t f, has_skip;
+  cp_act_desc skip;
+  const float* gamma;       /* GroupNorm+ReLU                                                                      */
+  const float* beta;
+  int32_t groups;
+  cp_act_desc gx, gh, gprev; /* GRU gates: x-side and h-side pre-activations [r | z | n], previous state            */
+  int32_t first_step;
+  int32_t fuse_heads;       /* 1: the per-head 1x1 convs `children` run in this op's epilogue                       */
+  int32_t fused_away;       /* 1: this 1x1 runs inside op `parent`                                                 */
+  int32_t parent;
+  int32_t n_children;
+  int32_t children[CP_MAX_HEADS];
+} cp_op_desc;
+typedef struct cp_op_launch {
+  int32_t family;           /* cp_op_family of the kernel that ran (CP_FAM_NONE: fused away)                        */
+  int32_t BN;               /* N tile (tensor-core families; 0 otherwise)                                          */
+  int32_t ksplit;           /* split-K factor (1 = off)                                                            */
+  int32_t grid;             /* CTAs of the main kernel (tensor-core families; 0 otherwise)                         */
+} cp_op_launch;
+int cp_plan_op_desc(const cp_plan* plan, int32_t i, cp_op_desc* out);
+int cp_plan_arena(const cp_plan* plan, float** act, int64_t* floats);
+/* `info` (may be NULL) receives last - first records. */
+int cp_plan_run_ops(cp_plan* plan, int32_t batch, int32_t first, int32_t last, const float* images, const float* pre_img,
+                    const float* pre_hm, const float* pre_hm_hp, float* const* head_out, void* stream,
+                    cp_op_launch* info);
+
 /* Arena / weight bytes owned by the plan (for logging). */
 int64_t cp_plan_bytes(const cp_plan* plan);
 /* Number of kernel launches one cp_forward enqueues (for bench gpu_launches). */

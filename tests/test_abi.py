@@ -91,3 +91,15 @@ def test_product_never_imports_oracle():
         if fn.endswith(".py"):
             src = open(os.path.join(pkg, fn)).read()
             assert "import oracle" not in src and "from oracle" not in src, fn
+
+
+def test_plan_stepping_argument_validation(cplib):
+    """The diagnostic stepping calls reject null plans / outputs with an error code, like cp_forward."""
+    from centerpose_b200 import _lib
+    d = _lib.CpOpDesc()
+    assert cplib.cp_plan_op_desc(None, 0, ctypes.byref(d)) == -1
+    assert b"null" in cplib.cp_last_error()
+    p, n = ctypes.c_void_p(), ctypes.c_int64()
+    assert cplib.cp_plan_arena(None, ctypes.byref(p), ctypes.byref(n)) == -1
+    assert cplib.cp_plan_run_ops(None, 1, 0, 1, None, None, None, None, None, None, None) == -1
+    assert b"null" in cplib.cp_last_error()

@@ -92,6 +92,27 @@ def test_batch_invariance_and_replay(cplib):
         assert torch.equal(full[h][1:2], single[h]), h
 
 
+@pytest.mark.parametrize("arch,trk", [("dlav1_34", False), ("dla_34", True)])
+def test_batch_invariance_and_replay_gn_and_tracking(arch, trk, cplib):
+    """The same for the dlav1 plan (convGRU, GroupNorm heads: the GroupNorm statistics are summed in a fixed order)
+    and for the tracking plan (pre_img / pre_hm / pre_hm_hp stems): bit-identical on replay and independent of the
+    batch neighbours."""
+    m, opt, _ = _model(arch, trk, 5)
+    x = torch.from_numpy(synth.normalize_frames(synth.synthetic_frames(3, 128, 160, seed=1))).cuda()
+    kw = {}
+    if trk:
+        g = torch.Generator(device="cuda").manual_seed(2)
+        kw = dict(pre_img=torch.randn(3, 3, 128, 160, device="cuda", generator=g),
+                  pre_hm=torch.rand(3, 1, 128, 160, device="cuda", generator=g),
+                  pre_hm_hp=torch.rand(3, 8, 128, 160, device="cuda", generator=g))
+    full = m(x, **kw)[-1]
+    again = m(x, **kw)[-1]
+    single = m(x[1:2].contiguous(), **{k: v[1:2].contiguous() for k, v in kw.items()})[-1]
+    for h in full:
+        assert torch.equal(full[h], again[h]), h
+        assert torch.equal(full[h][1:2], single[h]), h
+
+
 def test_weight_reload_is_picked_up(cplib):
     m, opt, sd = _model("dla_34", False, 6)
     x = torch.randn(1, 3, 64, 64, device="cuda")

@@ -23,6 +23,23 @@ TOL_HEAD_REL = 3e-4
 # (gpu-vs-fp64 <= 4 x reference-fp32-vs-fp64 + 3e-5).
 TOL_HEAD_REL_512 = 1e-3
 
+# Per-layer ceilings (tests/test_gpu_plan_layers.py, tests/layer_ref.py).  One launch, teacher-forced, scored by
+# r = max |got - ref| / S with ref the fp64 op and S the op on absolute values.  A product of two operands rounded to
+# p-bit mantissas and accumulated in fp32 is off by at most about (2 * 2^-p + K * 2^-24) * S in the worst case; random
+# rounding signs make the observed max much smaller, of order 2^-p / sqrt(K) * few for the operand rounding.
+#   fp32:   CUDA-core fp32 and the tf32x3 tensor-core kernels (hi*hi + hi*lo + lo*hi, fp32 sums), one ceiling, since
+#           "fp32-equivalent" means exactly that per layer; also the fp32 elementwise kernels.
+#   tf32:   single-pass tf32 operands (10-bit mantissa, unit roundoff 2^-11) and tf32-rounded outputs: 2 * 2^-10.
+#   bf16:   bf16 operands (7-bit mantissa, unit roundoff 2^-8): 2 * 2^-8.
+#   exact:  max-pool selects one of its inputs.
+# Measured on one H100 80GB HBM3 (700 W power limit), worst op over all configurations of
+# tests/test_gpu_plan_layers.py: fp32 8.6e-7 (dla_up.ida_1.node_2 deformable conv, ceiling 2.3x), tf32 8.8e-4
+# (level2 project 1x1, 2.3x), bf16 3.2e-3 (level2 project 1x1, 2.4x).
+LAYER_CEIL = {"fp32": 2e-6, "tf32": 2 * 2.0 ** -10, "bf16": 2 * 2.0 ** -8, "exact": 0.0}
+# single-pass tf32 must score at least this many fp32 ceilings on every tensor-core launch with K >= 288 (measured:
+# 25x at the least, dla_up.ida_0.proj_1 offset / mask conv)
+LAYER_DISCRIMINATION = 10.0
+
 
 def golden(name):
     return np.load(os.path.join(GOLD, name + ".npz"), allow_pickle=False)
