@@ -52,6 +52,7 @@ EXPORTS = [
     "cp_dcn_v2_forward_ex", "cp_conv2d", "cp_dcn_v2_backward",
     "cp_preprocess_affine", "cp_tracker_create", "cp_tracker_destroy", "cp_tracker_reset", "cp_tracker_step", "cp_tracker_render",
     "cp_tracker_render_ex", "cp_tracker_seed", "cp_plan_op_desc", "cp_plan_arena", "cp_plan_run_ops",
+    "cp_preprocess_ragged", "cp_tracker_step_ex", "cp_tracker_render_ex2", "cp_tracker_seed_ex",
 ]
 
 # cp_op_family
@@ -177,6 +178,9 @@ def load():
                                 ctypes.POINTER(ctypes.c_float), vp]
     L.cp_preprocess_affine.argtypes = [vp, vp, i32, i32, i32, i32, i32, ctypes.POINTER(ctypes.c_double),
                                        ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_float), vp]
+    L.cp_preprocess_ragged.argtypes = [vp, i64, ctypes.POINTER(i64), ctypes.POINTER(i32), vp, i32, i32, i32,
+                                       ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_float),
+                                       ctypes.POINTER(ctypes.c_float), vp]
     L.cp_tracker_create.argtypes = [ctypes.POINTER(CpTrackerConfig), ctypes.POINTER(vp)]
     L.cp_tracker_destroy.argtypes = [vp]
     L.cp_tracker_reset.argtypes = [vp, i32, vp]
@@ -184,6 +188,9 @@ def load():
     L.cp_tracker_render.argtypes = [vp, i32, vp, vp, i32, i32, vp, vp, vp]
     L.cp_tracker_render_ex.argtypes = [vp, i32, vp, vp, i32, i32, ctypes.POINTER(i32), vp, vp, vp]
     L.cp_tracker_seed.argtypes = [vp, i32, vp, vp, i32, vp]
+    L.cp_tracker_step_ex.argtypes = [vp, i32, ctypes.POINTER(i32), vp, vp, i32, vp, vp, vp, vp]
+    L.cp_tracker_render_ex2.argtypes = [vp, i32, ctypes.POINTER(i32), vp, vp, i32, i32, ctypes.POINTER(i32), vp, vp, vp]
+    L.cp_tracker_seed_ex.argtypes = [vp, i32, ctypes.POINTER(i32), vp, vp, i32, vp]
     for name in EXPORTS:
         fn = getattr(L, name)
         if name not in ("cp_version", "cp_last_error", "cp_plan_bytes", "cp_plan_forward_launches",

@@ -3,8 +3,11 @@
 //                        the same implicit-GEMM deformable kernel the plan uses
 //                        (reference: DCNv2/src/cuda/dcn_v2_cuda.cu:42-172).
 //   cp_preprocess     -- batched uint8 HWC frames -> normalised fp32 NCHW network input
-//                        (reference: detectors/base_detector.py:91-148, fix_res branch).
+//                        (reference: detectors/base_detector.py:91-148, fix_res branch); cp_preprocess_ragged does
+//                        the same for frames of different sizes in one launch.
 #include <stdlib.h>
+
+#include <vector>
 
 #include "common.cuh"
 
@@ -25,6 +28,40 @@ struct WarpM {
   double m[6];
 };
 
+// one output pixel (x, y) of frame `img` [sh, sw, 3] under the inverted matrix W, all three channels
+__device__ __forceinline__ void warp_pixel(const uint8_t* __restrict__ img, float* __restrict__ out, size_t plane, int sh,
+                                           int sw, int x, int y, const WarpM& W, const float* mean, const float* stdv) {
+  // unfused double arithmetic (the host code OpenCV runs here has no FMA contraction)
+  const int X0 = __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(W.m[1], (double)y), W.m[2]), 1024.0)) + 16;
+  const int Y0 = __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(W.m[4], (double)y), W.m[5]), 1024.0)) + 16;
+  const int ad = __double2int_rn(__dmul_rn(__dmul_rn(W.m[0], (double)x), 1024.0));
+  const int bd = __double2int_rn(__dmul_rn(__dmul_rn(W.m[3], (double)x), 1024.0));
+  const int X = (X0 + ad) >> 5, Y = (Y0 + bd) >> 5;
+  int ix = X >> 5, iy = Y >> 5;
+  // saturate_cast<short> of the integer coordinates (only matters for absurd scales; keeps the restatement exact)
+  ix = max(-32768, min(32767, ix));
+  iy = max(-32768, min(32767, iy));
+  const int fx = X & 31, fy = Y & 31;
+  const int w00 = (32 - fy) * (32 - fx) * 32, w01 = (32 - fy) * fx * 32, w10 = fy * (32 - fx) * 32, w11 = fy * fx * 32;
+  const bool y0 = iy >= 0 && iy < sh, y1 = iy + 1 >= 0 && iy + 1 < sh;
+  const bool x0 = ix >= 0 && ix < sw, x1 = ix + 1 >= 0 && ix + 1 < sw;
+  for (int c = 0; c < 3; ++c) {
+    int v00 = 0, v01 = 0, v10 = 0, v11 = 0;
+    if (y0) {
+      if (x0) v00 = img[((size_t)iy * sw + ix) * 3 + c];
+      if (x1) v01 = img[((size_t)iy * sw + ix + 1) * 3 + c];
+    }
+    if (y1) {
+      if (x0) v10 = img[((size_t)(iy + 1) * sw + ix) * 3 + c];
+      if (x1) v11 = img[((size_t)(iy + 1) * sw + ix + 1) * 3 + c];
+    }
+    int u8 = (v00 * w00 + v01 * w01 + v10 * w10 + v11 * w11 + (1 << 14)) >> 15;
+    u8 = max(0, min(255, u8));
+    const double r = ((double)u8 / 255.0 - (double)mean[c]) / (double)stdv[c];
+    out[c * plane] = (float)r;
+  }
+}
+
 __global__ void preprocess_kernel(const uint8_t* __restrict__ frames, float* __restrict__ out, int B, int sh,
                                   int sw, int dh, int dw, const WarpM W, float m0, float m1, float m2, float s0, float s1,
                                   float s2) {
@@ -36,37 +73,77 @@ __global__ void preprocess_kernel(const uint8_t* __restrict__ frames, float* __r
     const size_t t = i / dw;
     const int y = (int)(t % dh);
     const int n = (int)(t / dh);
-    // unfused double arithmetic (the host code OpenCV runs here has no FMA contraction)
-    const int X0 = __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(W.m[1], (double)y), W.m[2]), 1024.0)) + 16;
-    const int Y0 = __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(W.m[4], (double)y), W.m[5]), 1024.0)) + 16;
-    const int ad = __double2int_rn(__dmul_rn(__dmul_rn(W.m[0], (double)x), 1024.0));
-    const int bd = __double2int_rn(__dmul_rn(__dmul_rn(W.m[3], (double)x), 1024.0));
-    const int X = (X0 + ad) >> 5, Y = (Y0 + bd) >> 5;
-    int ix = X >> 5, iy = Y >> 5;
-    // saturate_cast<short> of the integer coordinates (only matters for absurd scales; keeps the restatement exact)
-    ix = max(-32768, min(32767, ix));
-    iy = max(-32768, min(32767, iy));
-    const int fx = X & 31, fy = Y & 31;
-    const int w00 = (32 - fy) * (32 - fx) * 32, w01 = (32 - fy) * fx * 32, w10 = fy * (32 - fx) * 32, w11 = fy * fx * 32;
-    const uint8_t* img = frames + (size_t)n * sh * sw * 3;
-    const bool y0 = iy >= 0 && iy < sh, y1 = iy + 1 >= 0 && iy + 1 < sh;
-    const bool x0 = ix >= 0 && ix < sw, x1 = ix + 1 >= 0 && ix + 1 < sw;
-    for (int c = 0; c < 3; ++c) {
-      int v00 = 0, v01 = 0, v10 = 0, v11 = 0;
-      if (y0) {
-        if (x0) v00 = img[((size_t)iy * sw + ix) * 3 + c];
-        if (x1) v01 = img[((size_t)iy * sw + ix + 1) * 3 + c];
-      }
-      if (y1) {
-        if (x0) v10 = img[((size_t)(iy + 1) * sw + ix) * 3 + c];
-        if (x1) v11 = img[((size_t)(iy + 1) * sw + ix + 1) * 3 + c];
-      }
-      int u8 = (v00 * w00 + v01 * w01 + v10 * w10 + v11 * w11 + (1 << 14)) >> 15;
-      u8 = max(0, min(255, u8));
-      const double r = ((double)u8 / 255.0 - (double)mean[c]) / (double)stdv[c];
-      out[(((size_t)n * 3 + c) * dh + y) * dw + x] = (float)r;
-    }
+    warp_pixel(frames + (size_t)n * sh * sw * 3, out + (((size_t)n * 3) * dh + y) * dw + x, (size_t)dh * dw, sh, sw, x, y,
+               W, mean, stdv);
   }
+}
+
+// per-frame parameters of the ragged launch
+struct RaggedFrame {
+  WarpM W;
+  long long offset;     // bytes into the packed frame buffer
+  int sh, sw;
+};
+
+__global__ void preprocess_ragged_kernel(const uint8_t* __restrict__ frames, const RaggedFrame* __restrict__ fr,
+                                         float* __restrict__ out, int B, int dh, int dw, float m0, float m1, float m2,
+                                         float s0, float s1, float s2) {
+  size_t total = (size_t)B * dh * dw;
+  const float mean[3] = {m0, m1, m2};
+  const float stdv[3] = {s0, s1, s2};
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int x = (int)(i % dw);
+    const size_t t = i / dw;
+    const int y = (int)(t % dh);
+    const int n = (int)(t / dh);
+    const RaggedFrame f = fr[n];
+    warp_pixel(frames + f.offset, out + (((size_t)n * 3) * dh + y) * dw + x, (size_t)dh * dw, f.sh, f.sw, x, y, f.W, mean,
+               stdv);
+  }
+}
+
+// cv::warpAffine inverts the forward matrix like this (imgwarp.cpp), in double, before the fixed-point walk
+WarpM invert_affine(const double* trans_input) {
+  WarpM W;
+  double* M = W.m;
+  for (int i = 0; i < 6; ++i) M[i] = trans_input[i];
+  double D = M[0] * M[4] - M[1] * M[3];
+  D = D != 0 ? 1. / D : 0;
+  const double A11 = M[4] * D, A22 = M[0] * D;
+  M[0] = A11;
+  M[1] *= -D;
+  M[3] *= -D;
+  M[4] = A22;
+  const double b1 = -M[0] * M[2] - M[1] * M[5];
+  const double b2 = -M[3] * M[2] - M[4] * M[5];
+  M[2] = b1;
+  M[5] = b2;
+  return W;
+}
+
+// fix_res affine of base_detector.py:109-121 (c = frame centre, s = max side, rot 0) in closed form: the float32 control
+// points of utils/image.py:35-68 give an isotropic scale a = dst_w / s.  (cv2.getAffineTransform solves the same three
+// point pairs by LU; the two agree to <= 3e-14, which the fixed-point walk cannot see except on exact rounding ties.
+// Callers that hold the reference's own `trans_input` pass it to cp_preprocess_affine.)
+void fix_res_affine(int src_h, int src_w, int dst_h, int dst_w, double T[6]) {
+  const float cx = (float)(src_w / 2.0), cy = (float)(src_h / 2.0);
+  const float s = (float)(src_h > src_w ? src_h : src_w);
+  const float src1y = cy + s * -0.5f;                               // float32 control points
+  const float dst0x = (float)(dst_w * 0.5), dst0y = (float)(dst_h * 0.5);
+  const float dst1y = dst0y + (float)(dst_w * -0.5);
+  const double a = ((double)dst1y - (double)dst0y) / ((double)src1y - (double)cy);
+  T[0] = a;
+  T[1] = 0.0;
+  T[2] = (double)dst0x - a * (double)cx;
+  T[3] = 0.0;
+  T[4] = a;
+  T[5] = (double)dst0y - a * (double)cy;
+}
+
+int preprocess_blocks(size_t total) {
+  int blocks = (int)((total + 255) / 256);
+  if (blocks > 132 * 16) blocks = 132 * 16;
+  return blocks;
 }
 
 }  // namespace
@@ -286,45 +363,66 @@ int cp_preprocess_affine(const uint8_t* frames, float* out, int32_t B, int32_t s
   if (!frames || !out || !mean || !stdv || !trans_input) return fail(CP_ERR_INVALID, "cp_preprocess: null argument");
   if (B <= 0 || src_h <= 0 || src_w <= 0 || dst_h <= 0 || dst_w <= 0)
     return fail(CP_ERR_INVALID, "cp_preprocess: bad shape");
-  // cv::warpAffine inverts the forward matrix like this (imgwarp.cpp), in double, before the fixed-point walk
-  WarpM W;
-  double* M = W.m;
-  for (int i = 0; i < 6; ++i) M[i] = trans_input[i];
-  double D = M[0] * M[4] - M[1] * M[3];
-  D = D != 0 ? 1. / D : 0;
-  const double A11 = M[4] * D, A22 = M[0] * D;
-  M[0] = A11;
-  M[1] *= -D;
-  M[3] *= -D;
-  M[4] = A22;
-  const double b1 = -M[0] * M[2] - M[1] * M[5];
-  const double b2 = -M[3] * M[2] - M[4] * M[5];
-  M[2] = b1;
-  M[5] = b2;
-  size_t total = (size_t)B * dst_h * dst_w;
-  int blocks = (int)((total + 255) / 256);
-  if (blocks > 132 * 16) blocks = 132 * 16;
-  preprocess_kernel<<<blocks, 256, 0, (cudaStream_t)stream_>>>(frames, out, B, src_h, src_w, dst_h, dst_w, W, mean[0],
-                                                              mean[1], mean[2], stdv[0], stdv[1], stdv[2]);
+  const WarpM W = invert_affine(trans_input);
+  preprocess_kernel<<<preprocess_blocks((size_t)B * dst_h * dst_w), 256, 0, (cudaStream_t)stream_>>>(
+      frames, out, B, src_h, src_w, dst_h, dst_w, W, mean[0], mean[1], mean[2], stdv[0], stdv[1], stdv[2]);
   CP_LAUNCH_CHECK("preprocess_kernel");
   return CP_OK;
 }
 
-// fix_res affine of base_detector.py:109-121 (c = frame centre, s = max side, rot 0) in closed form: the float32 control
-// points of utils/image.py:35-68 give an isotropic scale a = dst_w / s.  (cv2.getAffineTransform solves the same three
-// point pairs by LU; the two agree to <= 3e-14, which the fixed-point walk cannot see except on exact rounding ties.
-// Callers that hold the reference's own `trans_input` pass it to cp_preprocess_affine.)
+// the fix_res affine of the frame size (fix_res_affine above)
 int cp_preprocess(const uint8_t* frames, float* out, int32_t B, int32_t src_h, int32_t src_w, int32_t dst_h,
                   int32_t dst_w, const float mean[3], const float stdv[3], void* stream_) {
   if (src_h <= 0 || src_w <= 0 || dst_h <= 0 || dst_w <= 0) return fail(CP_ERR_INVALID, "cp_preprocess: bad shape");
-  const float cx = (float)(src_w / 2.0), cy = (float)(src_h / 2.0);
-  const float s = (float)(src_h > src_w ? src_h : src_w);
-  const float src1y = cy + s * -0.5f;                               // float32 control points
-  const float dst0x = (float)(dst_w * 0.5), dst0y = (float)(dst_h * 0.5);
-  const float dst1y = dst0y + (float)(dst_w * -0.5);
-  const double a = ((double)dst1y - (double)dst0y) / ((double)src1y - (double)cy);
-  const double T[6] = {a, 0.0, (double)dst0x - a * (double)cx, 0.0, a, (double)dst0y - a * (double)cy};
+  double T[6];
+  fix_res_affine(src_h, src_w, dst_h, dst_w, T);
   return cp_preprocess_affine(frames, out, B, src_h, src_w, dst_h, dst_w, T, mean, stdv, stream_);
+}
+
+int cp_preprocess_ragged(const uint8_t* frames, int64_t frames_bytes, const int64_t* offsets, const int32_t* src_hw,
+                         float* out, int32_t B, int32_t dst_h, int32_t dst_w, const double* trans_input,
+                         const float mean[3], const float stdv[3], void* stream_) {
+  if (!frames || !offsets || !src_hw || !out || !mean || !stdv) return fail(CP_ERR_INVALID, "cp_preprocess_ragged: null argument");
+  if (B <= 0 || dst_h <= 0 || dst_w <= 0 || frames_bytes <= 0) return fail(CP_ERR_INVALID, "cp_preprocess_ragged: bad shape");
+  std::vector<RaggedFrame> fr(B);
+  for (int b = 0; b < B; ++b) {
+    const int h = src_hw[2 * b], w = src_hw[2 * b + 1];
+    if (h <= 0 || w <= 0)
+      return fail(CP_ERR_INVALID, "cp_preprocess_ragged: frame " + std::to_string(b) + " has size " + std::to_string(h) +
+                                      " x " + std::to_string(w));
+    if (offsets[b] < 0 || offsets[b] > frames_bytes || (int64_t)h * w * 3 > frames_bytes - offsets[b])
+      return fail(CP_ERR_INVALID, "cp_preprocess_ragged: frame " + std::to_string(b) + " (" + std::to_string(h) + " x " +
+                                      std::to_string(w) + " at byte " + std::to_string(offsets[b]) +
+                                      ") lies outside the " + std::to_string(frames_bytes) + "-byte buffer");
+    double T[6];
+    if (trans_input) {
+      for (int i = 0; i < 6; ++i) T[i] = trans_input[6 * b + i];
+    } else {
+      fix_res_affine(h, w, dst_h, dst_w, T);
+    }
+    fr[b].W = invert_affine(T);
+    fr[b].offset = offsets[b];
+    fr[b].sh = h;
+    fr[b].sw = w;
+  }
+  cudaStream_t s = (cudaStream_t)stream_;
+  RaggedFrame* dfr = nullptr;
+  CP_CUDA_CHECK(cudaMallocAsync(&dfr, sizeof(RaggedFrame) * B, s));
+  int rc = CP_OK;
+  // a pageable source: the bytes are staged before cudaMemcpyAsync returns, so `fr` may go out of scope
+  if (cudaMemcpyAsync(dfr, fr.data(), sizeof(RaggedFrame) * B, cudaMemcpyHostToDevice, s) != cudaSuccess) {
+    rc = fail(CP_ERR_CUDA, "cp_preprocess_ragged: parameter upload");
+  } else {
+    preprocess_ragged_kernel<<<preprocess_blocks((size_t)B * dst_h * dst_w), 256, 0, s>>>(
+        frames, dfr, out, B, dst_h, dst_w, mean[0], mean[1], mean[2], stdv[0], stdv[1], stdv[2]);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess)
+      rc = fail(CP_ERR_CUDA, std::string("preprocess_ragged_kernel: ") + cudaGetErrorString(e));
+    else
+      ++g_launch_counter;
+  }
+  cudaFreeAsync(dfr, s);
+  return rc;
 }
 
 }  // extern "C"

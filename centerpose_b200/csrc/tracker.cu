@@ -16,13 +16,14 @@ using namespace cp::track;
 
 struct cp_tracker {
   cp_tracker_config cfg;
-  Slot* slots[2] = {nullptr, nullptr};      // [streams][max_tracks], ping-pong: slots[cur] = current tracks
+  Slot* slots[2] = {nullptr, nullptr};      // [streams][max_tracks], ping-pong: slots[cur[s]] = current tracks of s
   int* n_tracks[2] = {nullptr, nullptr};    // [streams]
+  int* cur = nullptr;                       // [streams] current buffer of each stream, flipped by the step kernel
   int* id_count = nullptr;                  // [streams]
   int* modes = nullptr;                     // [streams] render modes of the latest cp_tracker_render_ex
+  int* ids = nullptr;                       // [streams] stream map of the latest _ex call (batch row -> stream)
   void* plan = nullptr;                     // hungarian: [streams][max_tracks] Entry of the association kernel
   int* plan_n = nullptr;                    // hungarian: [streams]
-  int cur = 0;
 };
 
 namespace cp {
@@ -37,11 +38,13 @@ struct StepArgs {
   const float* poses;       // [B, K, 192]
   const int* n_valid;       // [B]
   const double* meta;       // [B, 16]
-  const Slot* old_slots;
-  const int* old_n;
-  Slot* new_slots;
-  int* new_n;
-  int* id_count;
+  Slot* slots0;             // [streams, T] the two buffers of the track state
+  Slot* slots1;
+  int* n0;                  // [streams]
+  int* n1;
+  int* cur;                 // [streams] which buffer is current
+  const int* ids;           // [B] tracker stream of each batch row, or nullptr: the identity
+  int* id_count;            // [streams]
   float* tracks_out;        // [B, T, 320]
   int* n_out;               // [B]
   Entry* plan;              // hungarian: [B, T] entries written by tracker_assoc_kernel, else nullptr
@@ -52,6 +55,27 @@ struct StepArgs {
 // TRK_THREADS) and the serial scan's choice becomes a reduction over (value, key): the smaller value wins, equal values
 // go to the larger key, key = 256 + t for an unassigned column (the last one of the scan wins) and 255 - t otherwise
 // (the first one wins), so the same column is picked as by the left-to-right scan of lsa_solve.
+// the state a batch row reads and writes: row b is tracker stream s = ids[b]; its current tracks are buffer cur[s]
+struct StreamState {
+  int s, c;
+  const Slot* old;
+  Slot* nxt;
+  int* new_n;
+  int M;
+};
+
+__device__ __forceinline__ StreamState stream_state(const StepArgs& a, int b) {
+  StreamState st;
+  st.s = a.ids ? a.ids[b] : b;
+  st.c = a.cur[st.s];
+  const size_t off = (size_t)st.s * a.T;
+  st.old = (st.c ? a.slots1 : a.slots0) + off;
+  st.nxt = (st.c ? a.slots0 : a.slots1) + off;
+  st.M = (st.c ? a.n1 : a.n0)[st.s];
+  st.new_n = (st.c ? a.n0 : a.n1) + st.s;
+  return st;
+}
+
 struct LsaSync {
   double val[TRK_THREADS / 32];
   int key[TRK_THREADS / 32];
@@ -160,8 +184,9 @@ __global__ void __launch_bounds__(TRK_THREADS, 1) tracker_assoc_kernel(const Ste
   __shared__ LsaSync sync;
   __shared__ int s_N;
   const float* poses = a.poses + (size_t)b * a.K * CP_POSE_RECORD;
-  const Slot* old = a.old_slots + (size_t)b * a.T;
-  const int M = a.old_n[b];
+  const StreamState st = stream_state(a, b);
+  const Slot* old = st.old;
+  const int M = st.M;
   int nv = a.n_valid[b];
   if (nv > a.K) nv = a.K;
   if (nv < 0) nv = 0;
@@ -174,9 +199,9 @@ __global__ void __launch_bounds__(TRK_THREADS, 1) tracker_assoc_kernel(const Ste
     int* match_of_det = ibuf + N + M;
     int* det_of_trk = match_of_det + N;
     lsa_pairs(v, N, M, &lsa, match_of_det, det_of_trk);
-    int idc = a.id_count[b];
+    int idc = a.id_count[st.s];
     a.plan_n[b] = plan_entries(a.cfg, poses, det_idx, N, old, M, match_of_det, det_of_trk, &idc, a.plan + (size_t)b * a.T, a.T);
-    a.id_count[b] = idc;
+    a.id_count[st.s] = idc;
   }
 }
 
@@ -191,9 +216,11 @@ __global__ void __launch_bounds__(TRK_THREADS, 1) tracker_step_kernel(const Step
   __shared__ double pnp_sm[(TRK_THREADS / 32) * PNP_SCRATCH];
 
   const float* poses = a.poses + (size_t)b * a.K * CP_POSE_RECORD;
-  const Slot* old = a.old_slots + (size_t)b * a.T;
-  Slot* nxt = a.new_slots + (size_t)b * a.T;
-  const int M = a.old_n[b];
+  // every thread reads cur[s] here, before the first barrier; thread 0 flips it at the end
+  const StreamState st = stream_state(a, b);
+  const Slot* old = st.old;
+  Slot* nxt = st.nxt;
+  const int M = st.M;
   int nv = a.n_valid[b];
   if (nv > a.K) nv = a.K;
   if (nv < 0) nv = 0;
@@ -204,9 +231,9 @@ __global__ void __launch_bounds__(TRK_THREADS, 1) tracker_step_kernel(const Step
     if (tid == 0) s_n = n;
   } else if (tid == 0) {
     // Steps 0-1 and the order of `ret` (serial, a few hundred operations)
-    int idc = a.id_count[b];
+    int idc = a.id_count[st.s];
     s_n = plan_step(a.cfg, poses, nv, old, M, &idc, entries, a.T, det_idx, fbuf, ibuf, taken);
-    a.id_count[b] = idc;
+    a.id_count[st.s] = idc;
   }
   __syncthreads();
   const int n = s_n;
@@ -256,8 +283,9 @@ __global__ void __launch_bounds__(TRK_THREADS, 1) tracker_step_kernel(const Step
   float* tail = a.tracks_out + ((size_t)b * a.T + n) * CP_TRACK_RECORD;
   for (int i = tid; i < (a.T - n) * CP_TRACK_RECORD; i += TRK_THREADS) tail[i] = 0.f;
   if (tid == 0) {
-    a.new_n[b] = n;
+    *st.new_n = n;
     a.n_out[b] = n;
+    a.cur[st.s] = st.c ^ 1;
   }
 }
 
@@ -271,12 +299,17 @@ __global__ void tracker_reset_kernel(int* n0, int* n1, int* id_count, int stream
 }
 
 // init_track with meta['pre_dets'] (tracker.py:21-48), one CTA per stream; seeds go into the current slots
+// (row b seeds stream ids[b], or b when ids is nullptr)
 __global__ void __launch_bounds__(128) tracker_seed_kernel(const Cfg cfg, int T, const float* seeds, const int* n_seeds,
-                                                            int S, Slot* slots, int* n_tracks, int* id_count) {
+                                                            int S, Slot* slots0, Slot* slots1, int* n0, int* n1,
+                                                            const int* cur, const int* ids, int* id_count) {
   const int b = blockIdx.x;
   int ns = n_seeds[b];
   if (ns < 0) return;
   if (ns > S) ns = S;
+  const int s = ids ? ids[b] : b, c = cur[s];
+  Slot* slots = (c ? slots1 : slots0) + (size_t)s * T;
+  int* n_tracks = (c ? n1 : n0) + s;
   __shared__ int keep[TRK_MAXK];
   __shared__ int s_n;
   const float* sb = seeds + (size_t)b * S * CP_SEED_RECORD;
@@ -285,12 +318,12 @@ __global__ void __launch_bounds__(128) tracker_seed_kernel(const Cfg cfg, int T,
     for (int k = 0; k < ns; ++k)
       if ((double)sb[(size_t)k * CP_SEED_RECORD + CP_P_SCORE] > cfg.new_thresh) keep[n++] = k;
     s_n = n;
-    n_tracks[b] = n;
-    id_count[b] = n;
+    *n_tracks = n;
+    id_count[s] = n;
   }
   __syncthreads();
   for (int t = threadIdx.x; t < s_n; t += blockDim.x)
-    entry_seed(cfg, &slots[(size_t)b * T + t], sb + (size_t)keep[t] * CP_SEED_RECORD, t + 1);
+    entry_seed(cfg, &slots[t], sb + (size_t)keep[t] * CP_SEED_RECORD, t + 1);
 }
 
 // ---- previous-frame heat maps ----------------------------------------------------------------------------------------
@@ -298,8 +331,12 @@ struct RenderArgs {
   Cfg cfg;
   int T, inp_h, inp_w, render_hm_mode, render_hmhp_mode;
   double pre_thresh;
-  const Slot* slots;
-  const int* n;
+  const Slot* slots0;      // [streams, T]
+  const Slot* slots1;
+  const int* n0;           // [streams]
+  const int* n1;
+  const int* cur;          // [streams]
+  const int* ids;          // [B] tracker stream of image b, or nullptr: the identity
   const double* meta;      // [B,16]: [3] original width, [4] original height
   const double* trans;     // [B,6]
   float* pre_hm;           // [B,1,h,w]
@@ -322,12 +359,13 @@ __device__ __forceinline__ void affine_pt(const double* t, float x, float y, dou
 __global__ void __launch_bounds__(256) tracker_render_kernel(const RenderArgs a) {
   const int t = blockIdx.x, b = blockIdx.y, tid = threadIdx.x;
   const int rmode = a.modes ? a.modes[b] : CP_RENDER_TRACKS;
-  if (t >= a.n[b] || rmode == CP_RENDER_EMPTY) return;
+  const int sid = a.ids ? a.ids[b] : b, c = a.cur[sid];
+  if (t >= (c ? a.n1 : a.n0)[sid] || rmode == CP_RENDER_EMPTY) return;
   const bool gt = rmode == CP_RENDER_GT;
   __shared__ Patch pt[9];
   if (tid == 0) {
     for (int i = 0; i < 9; ++i) pt[i].live = 0;
-    const Slot& s = a.slots[(size_t)b * a.T + t];
+    const Slot& s = (c ? a.slots1 : a.slots0)[(size_t)sid * a.T + t];
     const float* r = s.rec;
     const double* tr = a.trans + (size_t)b * 6;
     const double ori_w = a.meta[(size_t)b * CP_META_DOUBLES + 3], ori_h = a.meta[(size_t)b * CP_META_DOUBLES + 4];
@@ -500,6 +538,9 @@ int cp_tracker_create(const cp_tracker_config* cfg, cp_tracker** out) {
   if (e == cudaSuccess) e = cudaMalloc(&t->id_count, sizeof(int) * cfg->streams);
   if (e == cudaSuccess) e = cudaMemset(t->id_count, 0, sizeof(int) * cfg->streams);
   if (e == cudaSuccess) e = cudaMalloc(&t->modes, sizeof(int) * cfg->streams);
+  if (e == cudaSuccess) e = cudaMalloc(&t->ids, sizeof(int) * cfg->streams);
+  if (e == cudaSuccess) e = cudaMalloc(&t->cur, sizeof(int) * cfg->streams);
+  if (e == cudaSuccess) e = cudaMemset(t->cur, 0, sizeof(int) * cfg->streams);
   if (e == cudaSuccess && cfg->hungarian) e = cudaMalloc(&t->plan, ns * sizeof(Entry));
   if (e == cudaSuccess && cfg->hungarian) e = cudaMalloc(&t->plan_n, sizeof(int) * cfg->streams);
   if (e != cudaSuccess) {
@@ -518,6 +559,8 @@ int cp_tracker_destroy(cp_tracker* t) {
   }
   if (t->id_count) cudaFree(t->id_count);
   if (t->modes) cudaFree(t->modes);
+  if (t->ids) cudaFree(t->ids);
+  if (t->cur) cudaFree(t->cur);
   if (t->plan) cudaFree(t->plan);
   if (t->plan_n) cudaFree(t->plan_n);
   delete t;
@@ -533,12 +576,54 @@ int cp_tracker_reset(cp_tracker* t, int32_t index, void* stream) {
   return CP_OK;
 }
 
+}  // extern "C"
+
+namespace {
+
+// A stream map of `batch` rows: every id in 0..streams-1 and none twice.  The range's lower end and duplicates are
+// checked before the tracker is looked at, so a bad map is reported even with a null handle.
+int check_stream_ids(const cp_tracker* t, int32_t batch, const int32_t* ids, const char* fn) {
+  if (!ids || batch <= 0) return CP_OK;
+  for (int i = 0; i < batch; ++i) {
+    if (ids[i] < 0) return fail(CP_ERR_INVALID, std::string(fn) + ": stream id " + std::to_string(ids[i]) + " out of range");
+    for (int j = 0; j < i; ++j)
+      if (ids[j] == ids[i]) return fail(CP_ERR_INVALID, std::string(fn) + ": duplicate stream id " + std::to_string(ids[i]));
+  }
+  if (!t) return CP_OK;
+  for (int i = 0; i < batch; ++i)
+    if (ids[i] >= t->cfg.streams)
+      return fail(CP_ERR_INVALID, std::string(fn) + ": stream id " + std::to_string(ids[i]) + " out of range 0.." +
+                                      std::to_string(t->cfg.streams - 1));
+  return CP_OK;
+}
+
+// the validated host map -> the tracker's device copy (stream-ordered behind the kernels that read the previous map)
+int upload_stream_ids(cp_tracker* t, int32_t batch, const int32_t* ids, cudaStream_t s, const int** dev) {
+  *dev = nullptr;
+  if (!ids) return CP_OK;
+  CP_CUDA_CHECK(cudaMemcpyAsync(t->ids, ids, sizeof(int32_t) * batch, cudaMemcpyHostToDevice, s));
+  *dev = t->ids;
+  return CP_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
 int cp_tracker_step(cp_tracker* t, int32_t batch, const float* poses, const int32_t* n_valid, int32_t K, const double* meta,
                     float* tracks_out, int32_t* n_tracks, void* stream) {
+  return cp_tracker_step_ex(t, batch, nullptr, poses, n_valid, K, meta, tracks_out, n_tracks, stream);
+}
+
+int cp_tracker_step_ex(cp_tracker* t, int32_t batch, const int32_t* stream_ids, const float* poses, const int32_t* n_valid,
+                       int32_t K, const double* meta, float* tracks_out, int32_t* n_tracks, void* stream) {
+  if (int rc = check_stream_ids(t, batch, stream_ids, "cp_tracker_step")) return rc;
   if (!t || !poses || !n_valid || !meta || !tracks_out || !n_tracks) return fail(CP_ERR_INVALID, "cp_tracker_step: null argument");
   if (batch <= 0 || batch > t->cfg.streams) return fail(CP_ERR_INVALID, "cp_tracker_step: batch exceeds the tracker's streams");
   if (K <= 0 || K > CP_MAX_K) return fail(CP_ERR_INVALID, "cp_tracker_step: K must be in 1..128");
+  cudaStream_t s = (cudaStream_t)stream;
   StepArgs a;
+  if (int rc = upload_stream_ids(t, batch, stream_ids, s, &a.ids)) return rc;
   a.cfg = make_cfg(t->cfg);
   a.visible_thresh = t->cfg.visible_thresh;
   a.opencv_return = t->cfg.opencv_return;
@@ -547,46 +632,54 @@ int cp_tracker_step(cp_tracker* t, int32_t batch, const float* poses, const int3
   a.poses = poses;
   a.n_valid = n_valid;
   a.meta = meta;
-  a.old_slots = t->slots[t->cur];
-  a.old_n = t->n_tracks[t->cur];
-  a.new_slots = t->slots[t->cur ^ 1];
-  a.new_n = t->n_tracks[t->cur ^ 1];
+  a.slots0 = t->slots[0];
+  a.slots1 = t->slots[1];
+  a.n0 = t->n_tracks[0];
+  a.n1 = t->n_tracks[1];
+  a.cur = t->cur;
   a.id_count = t->id_count;
   a.tracks_out = tracks_out;
   a.n_out = n_tracks;
   a.plan = t->cfg.hungarian ? static_cast<Entry*>(t->plan) : nullptr;
   a.plan_n = t->cfg.hungarian ? t->plan_n : nullptr;
   if (a.plan) {
-    tracker_assoc_kernel<<<batch, TRK_THREADS, 0, (cudaStream_t)stream>>>(a);
+    tracker_assoc_kernel<<<batch, TRK_THREADS, 0, s>>>(a);
     CP_LAUNCH_CHECK("tracker_assoc_kernel");
   }
-  tracker_step_kernel<<<batch, TRK_THREADS, 0, (cudaStream_t)stream>>>(a);
+  tracker_step_kernel<<<batch, TRK_THREADS, 0, s>>>(a);     // flips cur[] of the streams it steps, and only those
   CP_LAUNCH_CHECK("tracker_step_kernel");
-  t->cur ^= 1;           // calls are issued in frame order on one stream
   return CP_OK;
 }
 
 int cp_tracker_render(cp_tracker* t, int32_t batch, const double* meta, const double* trans_input, int32_t inp_h,
                       int32_t inp_w, float* pre_hm, float* pre_hm_hp, void* stream) {
-  return cp_tracker_render_ex(t, batch, meta, trans_input, inp_h, inp_w, nullptr, pre_hm, pre_hm_hp, stream);
+  return cp_tracker_render_ex2(t, batch, nullptr, meta, trans_input, inp_h, inp_w, nullptr, pre_hm, pre_hm_hp, stream);
 }
 
 int cp_tracker_render_ex(cp_tracker* t, int32_t batch, const double* meta, const double* trans_input, int32_t inp_h,
                          int32_t inp_w, const int32_t* modes, float* pre_hm, float* pre_hm_hp, void* stream) {
+  return cp_tracker_render_ex2(t, batch, nullptr, meta, trans_input, inp_h, inp_w, modes, pre_hm, pre_hm_hp, stream);
+}
+
+int cp_tracker_render_ex2(cp_tracker* t, int32_t batch, const int32_t* stream_ids, const double* meta,
+                          const double* trans_input, int32_t inp_h, int32_t inp_w, const int32_t* modes, float* pre_hm,
+                          float* pre_hm_hp, void* stream) {
   bool any_mode = false;
   for (int b = 0; modes && b < batch; ++b) {
     if (modes[b] < CP_RENDER_TRACKS || modes[b] > CP_RENDER_EMPTY)
       return fail(CP_ERR_INVALID, "cp_tracker_render_ex: unknown render mode " + std::to_string(modes[b]) + " (0, 1 or 2)");
     any_mode = any_mode || modes[b] != CP_RENDER_TRACKS;
   }
+  if (int rc = check_stream_ids(t, batch, stream_ids, "cp_tracker_render")) return rc;
   if (!t || !meta || !trans_input || !pre_hm || !pre_hm_hp) return fail(CP_ERR_INVALID, "cp_tracker_render: null argument");
   if (batch <= 0 || batch > t->cfg.streams || inp_h <= 0 || inp_w <= 0) return fail(CP_ERR_INVALID, "cp_tracker_render: bad shape");
   cudaStream_t s = (cudaStream_t)stream;
   const size_t plane = (size_t)inp_h * inp_w;
+  RenderArgs a;
+  if (int rc = upload_stream_ids(t, batch, stream_ids, s, &a.ids)) return rc;
   CP_CUDA_CHECK(cudaMemsetAsync(pre_hm, 0, sizeof(float) * plane * batch, s));
   CP_CUDA_CHECK(cudaMemsetAsync(pre_hm_hp, 0, sizeof(float) * plane * 8 * batch, s));
   if (any_mode) CP_CUDA_CHECK(cudaMemcpyAsync(t->modes, modes, sizeof(int32_t) * batch, cudaMemcpyHostToDevice, s));
-  RenderArgs a;
   a.cfg = make_cfg(t->cfg);
   a.T = t->cfg.max_tracks;
   a.inp_h = inp_h;
@@ -594,8 +687,11 @@ int cp_tracker_render_ex(cp_tracker* t, int32_t batch, const double* meta, const
   a.render_hm_mode = t->cfg.render_hm_mode;
   a.render_hmhp_mode = t->cfg.render_hmhp_mode;
   a.pre_thresh = (double)t->cfg.pre_thresh;
-  a.slots = t->slots[t->cur];
-  a.n = t->n_tracks[t->cur];
+  a.slots0 = t->slots[0];
+  a.slots1 = t->slots[1];
+  a.n0 = t->n_tracks[0];
+  a.n1 = t->n_tracks[1];
+  a.cur = t->cur;
   a.meta = meta;
   a.trans = trans_input;
   a.pre_hm = pre_hm;
@@ -608,14 +704,23 @@ int cp_tracker_render_ex(cp_tracker* t, int32_t batch, const double* meta, const
 }
 
 int cp_tracker_seed(cp_tracker* t, int32_t batch, const float* seeds, const int32_t* n_seeds, int32_t S, void* stream) {
+  return cp_tracker_seed_ex(t, batch, nullptr, seeds, n_seeds, S, stream);
+}
+
+int cp_tracker_seed_ex(cp_tracker* t, int32_t batch, const int32_t* stream_ids, const float* seeds, const int32_t* n_seeds,
+                       int32_t S, void* stream) {
   if (S < 0 || S > CP_MAX_K) return fail(CP_ERR_INVALID, "cp_tracker_seed: S must be in 0..128");
+  if (int rc = check_stream_ids(t, batch, stream_ids, "cp_tracker_seed")) return rc;
   if (!t || !n_seeds || (S > 0 && !seeds)) return fail(CP_ERR_INVALID, "cp_tracker_seed: null argument");
   if (batch <= 0 || batch > t->cfg.streams) return fail(CP_ERR_INVALID, "cp_tracker_seed: batch exceeds the tracker's streams");
   if (S > t->cfg.max_tracks)
     return fail(CP_ERR_INVALID, "cp_tracker_seed: S = " + std::to_string(S) + " seeds exceed max_tracks = " +
                                     std::to_string(t->cfg.max_tracks));
-  tracker_seed_kernel<<<batch, 128, 0, (cudaStream_t)stream>>>(make_cfg(t->cfg), t->cfg.max_tracks, seeds, n_seeds, S,
-                                                               t->slots[t->cur], t->n_tracks[t->cur], t->id_count);
+  cudaStream_t s = (cudaStream_t)stream;
+  const int* ids = nullptr;
+  if (int rc = upload_stream_ids(t, batch, stream_ids, s, &ids)) return rc;
+  tracker_seed_kernel<<<batch, 128, 0, s>>>(make_cfg(t->cfg), t->cfg.max_tracks, seeds, n_seeds, S, t->slots[0],
+                                            t->slots[1], t->n_tracks[0], t->n_tracks[1], t->cur, ids, t->id_count);
   CP_LAUNCH_CHECK("tracker_seed_kernel");
   return CP_OK;
 }

@@ -17,7 +17,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from .engine import decode_params, decode_pnp, make_meta, preprocess
+from .engine import decode_params, decode_pnp, make_meta, preprocess, preprocess_ragged
 from .model import create_model, load_model
 from .tracker import Tracker, tracks_to_results
 
@@ -103,6 +103,55 @@ def affine_from_center_scale(c, s, out_w, out_h, inv=False):
     return cv2.getAffineTransform(dst, src) if inv else cv2.getAffineTransform(src, dst)
 
 
+def camera_per_frame(camera_matrix, B):
+    """camera_matrix [3,3] (shared) or [B,3,3] / a list of B [3,3] -> B float64 [3,3] matrices."""
+    cam = np.asarray(camera_matrix, np.float64)
+    if cam.shape == (3, 3):
+        return [cam] * B
+    if cam.shape != (B, 3, 3):
+        raise ValueError("camera_matrix must be [3,3] or one [3,3] per frame ([%d,3,3]), got %s" % (B, cam.shape))
+    return list(cam)
+
+
+def check_frames(frames, allow_idle):
+    """The frames of a ragged batch: uint8 [H,W,3] numpy arrays or tensors (None = an idle slot when allowed)."""
+    if len(frames) == 0:
+        raise ValueError("run_batch: an empty list of frames")
+    for b, f in enumerate(frames):
+        if f is None:
+            if not allow_idle:
+                raise ValueError("run_batch: frame %d is None (idle slots need track=True)" % b)
+            continue
+        if not isinstance(f, (np.ndarray, torch.Tensor)):
+            raise TypeError("run_batch: frame %d is a %s, not a numpy array or tensor" % (b, type(f).__name__))
+        dt = f.dtype
+        if dt not in (np.uint8, torch.uint8):
+            raise TypeError("run_batch: frame %d is %s; the ragged path takes uint8 [H,W,3] frames" % (b, dt))
+        if f.ndim != 3 or f.shape[2] != 3 or f.shape[0] < 1 or f.shape[1] < 1:
+            raise ValueError("run_batch: frame %d has shape %s, expected [H,W,3]" % (b, tuple(f.shape)))
+
+
+def check_slot_list(values, S, name, kind=None):
+    """A per-slot argument: None, or a list of S entries."""
+    if values is None:
+        return None
+    values = list(values)
+    if len(values) != S:
+        raise ValueError("run_batch: %d %s entries for %d slots" % (len(values), name, S))
+    return [kind(v) for v in values] if kind is not None else values
+
+
+class _SlotState(object):
+    """run_batch(list, track=True): the tracker of S slot streams and each slot's previous network input (a private
+    device buffer, written by device-to-device copies only)."""
+
+    def __init__(self, opt, S, ih, iw, device):
+        self.streams = S
+        self.tracker = Tracker(opt, streams=S, device=device)
+        self.pre = torch.zeros((S, 3, ih, iw), dtype=torch.float32, device=device)
+        self.started = [False] * S
+
+
 # ----------------------------------------------------------------------------- detector
 class ObjectPoseDetector(object):
     def __init__(self, opt, model=None):
@@ -134,6 +183,9 @@ class ObjectPoseDetector(object):
             self.tracker = Tracker(opt, streams=1, device=opt.device)
         self._batch_tracker = None
         self._batch_pre = None
+        self._slots = None             # run_batch(list, track=True): per-slot tracker and previous frames (_SlotState)
+        self._packed = None            # run_batch(list): device buffer the ragged frames are packed into
+        self._affines = {}             # (h, w) -> fix_res trans_input of that frame size
 
     def _to_device(self, t):
         """base_detector.py:41,436: everything the network touches lives on opt.device (always CUDA here)."""
@@ -474,7 +526,7 @@ class ObjectPoseDetector(object):
 
     # ------------------------------------------------------------------ batched API (not in the reference)
     def run_batch(self, frames, camera_matrix, pre_images=None, pre_hms=None, pre_hm_hp=None, to_host=True, track=False,
-                  out=None, pre_dets=None, frame_ids=None):
+                  out=None, pre_dets=None, frame_ids=None, new_video=None):
         """frames: uint8 [B,H,W,3] (numpy / pinned CPU tensor / CUDA tensor) or a
         pre-processed fp32 [B,3,h,w] CUDA tensor.  One native cp_infer call for the
         whole batch.  Returns (poses [B,K,192], n_valid [B]) -- on the host when
@@ -488,7 +540,22 @@ class ObjectPoseDetector(object):
         ground-truth frames, drawn from the ground truth on those frames, empty with opt.empty_pre_hm.
 
         out: optional (poses, n_valid) CUDA tensors to write into (e.g. the views of a dist.PoseBuffer, so that the
-        records land directly in the buffer of the all-gather / the pinned D2H copy)."""
+        records land directly in the buffer of the all-gather / the pinned D2H copy).
+
+        frames may also be a LIST of uint8 [H_b,W_b,3] frames of mixed sizes (numpy, CPU or CUDA tensors), with
+        camera_matrix [3,3] or one per frame [B,3,3]: one ragged pre-process launch, one network + decode call, and
+        every frame's records in its own pixels (its own c, s and meta row), exactly what run() gives for it.  With
+        track=True the list is indexed by SLOT, each slot an independent video (see `_run_slots`)."""
+        if isinstance(frames, (list, tuple)):
+            if pre_images is not None or pre_hms is not None or pre_hm_hp is not None:
+                raise ValueError("run_batch(list): the previous frames and heat maps are kept per slot (track=True)")
+            if track:
+                return self._run_slots(frames, camera_matrix, to_host, out, pre_dets, frame_ids, new_video)
+            if new_video is not None or pre_dets is not None or frame_ids is not None:
+                raise ValueError("run_batch(list): new_video / pre_dets / frame_ids need track=True")
+            return self._run_list(frames, camera_matrix, to_host, out)
+        if new_video is not None:
+            raise ValueError("run_batch: new_video needs a list of slot frames")
         dev = self.opt.device
         if isinstance(frames, np.ndarray):
             frames = torch.from_numpy(frames)
@@ -544,6 +611,141 @@ class ObjectPoseDetector(object):
             return poses.cpu().numpy(), n_valid.cpu().numpy()
         return poses, n_valid
 
+    # ------------------------------------------------------------------ ragged batches (lists of frames)
+    def _ragged_input(self, frames, camera_matrix):
+        """Validated list of uint8 HWC frames -> (x [B,3,h,w] fp32 CUDA, meta rows [B,16] float64 host, trans_input
+        [B,2,3] host).  The frames are copied into one device buffer and pre-processed by one cp_preprocess_ragged
+        launch with the same fix_res affine (c = frame centre, s = max side) and meta row that pre_process / run() use."""
+        if getattr(self.opt, "fix_short", 0) > 0 or not getattr(self.opt, "fix_res", True):
+            raise NotImplementedError("run_batch(list) pre-processes in the fix_res mode only")
+        if float(self.scales[0]) != 1.0:
+            raise NotImplementedError("run_batch pre-processes at scale 1; use run() for test_scales[0] != 1")
+        B = len(frames)
+        cams = camera_per_frame(camera_matrix, B)
+        dev = self.opt.device
+        ih, iw = self.opt.input_h, self.opt.input_w
+        ts, hw, offs, off = [], np.zeros((B, 2), np.int32), np.zeros(B, np.int64), 0
+        for b, f in enumerate(frames):
+            t = torch.from_numpy(f) if isinstance(f, np.ndarray) else f
+            ts.append(t)
+            hw[b] = t.shape[:2]
+            offs[b] = off
+            off += t.numel()
+        if self._packed is None or self._packed.numel() < off or self._packed.device != torch.device(dev):
+            self._packed = torch.empty((max(off, 1),), dtype=torch.uint8, device=dev)
+        for t, o in zip(ts, offs):
+            self._packed[o:o + t.numel()].copy_(t.reshape(-1), non_blocking=True)
+        trans = np.zeros((B, 2, 3), np.float64)
+        meta = np.zeros((B, _lib.CP_META_DOUBLES), np.float64)
+        for b in range(B):
+            h, w = int(hw[b, 0]), int(hw[b, 1])
+            c, sc = np.array([w / 2., h / 2.], np.float32), float(max(h, w))
+            if (h, w) not in self._affines:
+                self._affines[(h, w)] = affine_from_center_scale(c, sc, iw, ih)
+            trans[b] = self._affines[(h, w)]
+            meta[b] = make_meta(1, c, sc, w, h, cams[b]).numpy()[0]
+        x = preprocess_ragged(self._packed, offs, hw, ih, iw, self.opt.mean, self.opt.std, trans_input=trans)
+        return x, meta, trans
+
+    def _meta_rows(self, meta):
+        """Host meta rows -> a device tensor, uploaded again only when the rows change."""
+        key = meta.tobytes()
+        if getattr(self, "_list_meta_key", None) != key:
+            self._list_meta = torch.from_numpy(meta).to(self.opt.device)
+            self._list_meta_key = key
+        return self._list_meta
+
+    def _run_list(self, frames, camera_matrix, to_host, out):
+        """run_batch on a list of frames of mixed sizes: (poses [B,K,192], n_valid [B]), row b in frame b's pixels."""
+        check_frames(frames, allow_idle=False)
+        x, meta, _ = self._ragged_input(frames, camera_matrix)
+        B = len(frames)
+        metat = self._meta_rows(meta)
+        eng = self.model.engine(B, x.shape[2], x.shape[3], x.device)
+        prm = decode_params(self.opt, test_scale=1.0)
+        _, poses, n_valid = eng.infer(x, metat, prm, poses=out[0] if out is not None else None,
+                                      n_valid=out[1] if out is not None else None)
+        if to_host:
+            return poses.cpu().numpy(), n_valid.cpu().numpy()
+        return poses, n_valid
+
+    def _run_slots(self, frames, camera_matrix, to_host, out, pre_dets, frame_ids, new_video):
+        """run_batch(list, track=True): frames[i] is the next frame of the video in slot i, or None when slot i is idle
+        this step (its tracker stream is not stepped and keeps its state).  new_video[i] marks the first frame of a
+        video in slot i, which then behaves exactly like the first run() call of a fresh detector: the stream is reset,
+        the frame is its own previous frame, it is seeded from pre_dets[i] when given, and its heat maps follow
+        opt.gt_pre_hm_hmhp* / opt.empty_pre_hm.  A slot's first frame always starts a video.  Only the live slots go
+        through the network (as one batch); each slot keeps its previous network input in a persistent device buffer.
+
+        Returns (tracks [S,T,320], n_tracks [S]) for the S slots, idle slots with n_tracks 0 and zero rows; out:
+        optional (tracks, n_tracks) CUDA tensors of those shapes to write into."""
+        if not getattr(self.opt, "tracking_task", False):
+            raise ValueError("run_batch(track=True) needs a tracking model (opt.tracking_task)")
+        S = len(frames)
+        check_frames(frames, allow_idle=True)
+        cams = camera_per_frame(camera_matrix, S)
+        new_video = check_slot_list(new_video, S, "new_video", bool)
+        pre_dets = check_slot_list(pre_dets, S, "pre_dets")
+        frame_ids = check_slot_list(frame_ids, S, "frame_ids")
+        dev = self.opt.device
+        ih, iw = self.opt.input_h, self.opt.input_w
+        st = self._slots
+        if st is None or st.streams != S:
+            st = self._slots = _SlotState(self.opt, S, ih, iw, dev)
+        T = st.tracker.max_tracks
+        if out is None:
+            out = (torch.empty((S, T, _lib.CP_TRACK_RECORD), dtype=torch.float32, device=dev),
+                   torch.empty((S,), dtype=torch.int32, device=dev))
+        elif (tuple(out[0].shape) != (S, T, _lib.CP_TRACK_RECORD) or tuple(out[1].shape) != (S,)
+              or out[0].dtype != torch.float32 or out[1].dtype != torch.int32):
+            raise ValueError("run_batch: out must be (tracks [%d,%d,%d] fp32, n_tracks [%d] int32)" % (S, T, _lib.CP_TRACK_RECORD, S))
+        live = [i for i in range(S) if frames[i] is not None]
+        for i in range(S):
+            if i not in live:
+                out[0][i].zero_()
+                out[1][i:i + 1].zero_()
+        if not live:
+            return (out[0].cpu().numpy(), out[1].cpu().numpy()) if to_host else out
+        trk = st.tracker
+        x, meta, trans = self._ragged_input([frames[i] for i in live], np.stack([cams[i] for i in live]))
+        metat = self._meta_rows(meta)
+        gts, seeds = [], [None] * S
+        for k, i in enumerate(live):
+            gt = self._gt_frame(frame_ids[i] if frame_ids is not None else None)
+            gts.append(gt)
+            start = (new_video is not None and new_video[i]) or not st.started[i]
+            if start:                                         # base_detector.py:444-449: a fresh stream
+                trk.reset(i)
+                st.pre[i].copy_(x[k])
+                st.started[i] = True
+            if pre_dets is not None and pre_dets[i] is not None and (start or gt):
+                seeds[i] = pre_dets[i]
+        trk.seed(seeds)
+        all_live = len(live) == S
+        if all_live:
+            pre = st.pre
+        else:
+            pre = torch.empty_like(x)
+            for k, i in enumerate(live):
+                pre[k].copy_(st.pre[i])
+        pre_hms, pre_hm_hp = trk.render(metat, trans.reshape(-1, 6), ih, iw, modes=[self._render_mode(g) for g in gts],
+                                        stream_ids=live)
+        eng = self.model.engine(S, ih, iw, x.device)
+        prm = decode_params(self.opt, test_scale=1.0)
+        _, poses, n_valid = eng.infer(x, metat, prm, pre, pre_hms, pre_hm_hp)
+        if all_live:
+            trk.step_records(poses, n_valid, metat, out=out, stream_ids=live)
+            st.pre.copy_(x)
+        else:
+            tr, nt = trk.step_records(poses, n_valid, metat, stream_ids=live)
+            for k, i in enumerate(live):
+                out[0][i].copy_(tr[k])
+                out[1][i:i + 1].copy_(nt[k:k + 1])
+                st.pre[i].copy_(x[k])
+        if to_host:
+            return out[0].cpu().numpy(), out[1].cpu().numpy()
+        return out
+
     def reset_tracking(self):
         """base_detector.py:774-776."""
         if self.tracker is not None:
@@ -552,6 +754,7 @@ class ObjectPoseDetector(object):
         self._batch_pre = None
         if self._batch_tracker is not None:
             self._batch_tracker.reset()
+        self._slots = None
 
 
 detector_factory = {"object_pose": ObjectPoseDetector}

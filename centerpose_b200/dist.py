@@ -4,6 +4,10 @@ fixed-shape pose tensor (+ n_valid packed into the same buffer).  Replaces the
 reference's training-only single-process DataParallel
 (models/data_parallel.py:10-84) on the inference path.
 
+Tracking shards video SLOTS the same way (`slot_layout`): each rank steps its own slots and the per-frame exchange is
+one all-gather of [slots/rank, max_tracks, CP_TRACK_RECORD] track records + n_tracks, a `PoseBuffer` with
+K = max_tracks and R = CP_TRACK_RECORD.
+
 `PoseBuffer` is the persistent buffer of that exchange: ONE flat fp32 tensor per rank,
     [ poses  b*K*R floats | n_valid  b int32 (same 4-byte cells) ]
 whose two views are handed to `cp_infer` as its output pointers, so the kernels write the packed layout directly --
@@ -21,6 +25,18 @@ def shard_range(n, rank, world):
     base, rem = divmod(n, world)
     start = rank * base + min(rank, rem)
     return start, start + base + (1 if rank < rem else 0)
+
+
+def slot_layout(slots, world):
+    """Tracking slots over `world` ranks: rank r owns slots shard_range(slots, r, world) and every rank gathers the same
+    number of rows, b = ceil(slots / world) (a rank with fewer slots leaves its last row empty).  Returns (b, order):
+    order[i] is the row of slot i in the gathered [world * b] records."""
+    b = -(-int(slots) // int(world))
+    order = []
+    for r in range(world):
+        lo, hi = shard_range(slots, r, world)
+        order += [r * b + k for k in range(hi - lo)]
+    return b, order
 
 
 class PoseBuffer(object):

@@ -398,6 +398,36 @@ def preprocess(frames_u8, dst_h, dst_w, mean, std, out=None, trans_input=None):
     return out
 
 
+def preprocess_ragged(packed_u8, offsets, src_hw, dst_h, dst_w, mean, std, out=None, trans_input=None):
+    """cp_preprocess_ragged: B frames of different sizes in one launch.  packed_u8: flat uint8 CUDA buffer holding frame b
+    (uint8 [src_hw[b][0], src_hw[b][1], 3]) at byte offsets[b] -> fp32 [B,3,dst_h,dst_w] CUDA, frame b bit for bit what
+    `preprocess` gives for it alone.  trans_input: optional [B,2,3] forward affines; default = each frame's fix_res affine."""
+    L = _lib.load()
+    if not packed_u8.is_cuda or packed_u8.dtype != torch.uint8 or not packed_u8.is_contiguous():
+        raise RuntimeError("preprocess_ragged needs a contiguous uint8 CUDA buffer")
+    offs = np.ascontiguousarray(offsets, np.int64).reshape(-1)
+    hw = np.ascontiguousarray(src_hw, np.int32).reshape(-1, 2)
+    B = offs.shape[0]
+    if hw.shape[0] != B:
+        raise ValueError("preprocess_ragged: %d offsets for %d frame sizes" % (B, hw.shape[0]))
+    if out is None:
+        out = torch.empty((B, 3, dst_h, dst_w), dtype=torch.float32, device=packed_u8.device)
+    tm = None
+    if trans_input is not None:
+        tr = np.ascontiguousarray(trans_input, np.float64).reshape(-1)
+        if tr.shape[0] != 6 * B:
+            raise ValueError("preprocess_ragged: trans_input must hold %d 2x3 matrices" % B)
+        tm = tr.ctypes.data_as(ctypes.POINTER(ctypes.c_double))
+    m = (ctypes.c_float * 3)(*[float(v) for v in mean])
+    s = (ctypes.c_float * 3)(*[float(v) for v in std])
+    with torch.cuda.device(packed_u8.device):
+        rc = L.cp_preprocess_ragged(_ptr(packed_u8), packed_u8.numel(), offs.ctypes.data_as(ctypes.POINTER(ctypes.c_int64)),
+                                    hw.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), _ptr(out), B, dst_h, dst_w, tm, m, s,
+                                    _stream())
+    _lib.check(rc, "cp_preprocess_ragged")
+    return out
+
+
 def conv2d_nhwc(x, weight, bias=None, residual=None, stride=1, pad=0, relu=False, precision="fp32"):
     """cp_conv2d: x [B,H,W,Cin] NHWC fp32 CUDA, weight OIHW -> [B,Ho,Wo,Cout] NHWC."""
     L = _lib.load()

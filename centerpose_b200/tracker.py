@@ -23,6 +23,16 @@ def _opt(opt, name, default):
     return getattr(opt, name, default)
 
 
+def _stream_map(stream_ids, batch):
+    """A host int32 [batch] stream map for the _ex entry points (NULL = the identity).  The library validates it."""
+    if stream_ids is None:
+        return None
+    ids = [int(s) for s in stream_ids]
+    if len(ids) != batch:
+        raise ValueError("%d stream ids for a batch of %d" % (len(ids), batch))
+    return (ctypes.c_int32 * batch)(*ids)
+
+
 def track_to_dict(row):
     """One CP_TRACK_RECORD row -> the reference's track dict (the keys run() / the debugger / the evaluator read)."""
     from .detector import record_to_result
@@ -195,14 +205,15 @@ class Tracker(object):
 
     def seed(self, pre_dets):
         """init_track with pre_dets for several streams: pre_dets[b] is the list of dicts for stream b, or None to leave
-        stream b untouched (one cp_tracker_seed call)."""
+        stream b untouched (one cp_tracker_seed_ex call over the streams that are seeded)."""
         pre_dets = list(pre_dets)
         if len(pre_dets) > self.streams:
             raise ValueError("%d seed lists for a tracker of %d streams" % (len(pre_dets), self.streams))
-        B = max([b + 1 for b, p in enumerate(pre_dets) if p is not None] or [0])
+        ids = [b for b, p in enumerate(pre_dets) if p is not None]
+        B = len(ids)
         if B == 0:
             return
-        S = max(1, max(len(p) for p in pre_dets[:B] if p is not None))
+        S = max(1, max(len(pre_dets[b]) for b in ids))
         if S > self.max_tracks:
             raise ValueError("%d seeds exceed max_tracks = %d" % (S, self.max_tracks))
         recs = np.zeros((B, S, _lib.CP_SEED_RECORD), np.float32)
@@ -210,13 +221,11 @@ class Tracker(object):
         hmhp = int(_opt(self.opt, "render_hmhp_mode", 2))
         filt = bool(_opt(self.opt, "kalman", True)) or bool(_opt(self.opt, "scale_pool", True))
         pre_thresh, new_thresh = float(_opt(self.opt, "pre_thresh", -1)), float(_opt(self.opt, "new_thresh", 0.3))
-        for b, dets in enumerate(pre_dets[:B]):
-            if dets is None:
-                continue
-            dets = list(dets)
+        for i, b in enumerate(ids):
+            dets = list(pre_dets[b])
             if dets:
-                recs[b, :len(dets)] = seed_records(dets, self.opt)
-            n[b] = len(dets)
+                recs[i, :len(dets)] = seed_records(dets, self.opt)
+            n[i] = len(dets)
             kept = [d for d in dets if float(d["score"]) > new_thresh]
             missing = ""
             for d in kept:
@@ -231,7 +240,7 @@ class Tracker(object):
         seeds = torch.from_numpy(recs).to(self.device)
         nt = torch.from_numpy(n).to(self.device)
         with torch.cuda.device(self.device):
-            rc = self.L.cp_tracker_seed(self._h, B, _ptr(seeds), _ptr(nt), S, _stream())
+            rc = self.L.cp_tracker_seed_ex(self._h, B, _stream_map(ids, B), _ptr(seeds), _ptr(nt), S, _stream())
         _lib.check(rc, "cp_tracker_seed")
         seeds._cp_keep = nt
         self._keep = seeds                       # the copy is stream-ordered; keep the buffers alive until the next call
@@ -254,9 +263,10 @@ class Tracker(object):
             self._rows = (tr.cpu().numpy(), n.cpu().numpy())
         return self._rows
 
-    def step_records(self, poses, n_valid, meta, out=None):
+    def step_records(self, poses, n_valid, meta, out=None, stream_ids=None):
         """poses [B,K,192] / n_valid [B] / meta [B,16] CUDA tensors (as cp_infer emits them) -> (tracks [B,T,320],
-        n_tracks [B]) CUDA tensors.  Stream b of the tracker consumes poses[b]."""
+        n_tracks [B]) CUDA tensors.  Stream b of the tracker consumes poses[b], or stream stream_ids[b] when a map is
+        given; streams the map does not list are not stepped and keep their state untouched."""
         B, K, R = poses.shape
         if R != _lib.CP_POSE_RECORD or B > self.streams:
             raise ValueError("poses %s does not fit a tracker of %d streams" % (tuple(poses.shape), self.streams))
@@ -267,32 +277,38 @@ class Tracker(object):
             out = (torch.empty((B, self.max_tracks, _lib.CP_TRACK_RECORD), dtype=torch.float32, device=self.device),
                    torch.empty((B,), dtype=torch.int32, device=self.device))
         with torch.cuda.device(self.device):
-            rc = self.L.cp_tracker_step(self._h, B, _ptr(poses), _ptr(n_valid), K, _ptr(meta), _ptr(out[0]), _ptr(out[1]),
-                                        _stream())
+            rc = self.L.cp_tracker_step_ex(self._h, B, _stream_map(stream_ids, B), _ptr(poses), _ptr(n_valid), K, _ptr(meta),
+                                           _ptr(out[0]), _ptr(out[1]), _stream())
         _lib.check(rc, "cp_tracker_step")
         self._dev, self._rows, self._dicts = out, None, None
-        self._seeded = [None] * self.streams
-        self._seeded_gt = [False] * self.streams
+        for s in (range(B) if stream_ids is None else stream_ids):
+            self._seeded[s], self._seeded_gt[s] = None, False
         return out
 
-    def render(self, meta, trans_input, inp_h, inp_w, out=None, modes=None):
+    def render(self, meta, trans_input, inp_h, inp_w, out=None, modes=None, stream_ids=None):
         """Previous-frame heat maps of every stream: (pre_hm [B,1,h,w], pre_hm_hp [B,8,h,w]) fp32 CUDA.  modes: None
         (all drawn from the tracks) or one cp_render_mode per stream: RENDER_TRACKS, RENDER_GT (the ground-truth
-        branch, on a stream seeded since its last step) or RENDER_EMPTY (opt.empty_pre_hm)."""
+        branch, on a stream seeded since its last step) or RENDER_EMPTY (opt.empty_pre_hm).  stream_ids: image b draws
+        tracker stream stream_ids[b] (default: stream b)."""
         B = meta.shape[0]
+        sid = list(range(B)) if stream_ids is None else [int(s) for s in stream_ids]
+        if len(sid) != B:
+            raise ValueError("render: %d stream ids for %d images" % (len(sid), B))
         mode_arr = None
         if modes is not None:
             modes = [int(m) for m in modes]
             if len(modes) != B:
                 raise ValueError("render: %d modes for %d streams" % (len(modes), B))
             mode_arr = (ctypes.c_int32 * B)(*modes)
-        for b in range(B):
+        for b, s in enumerate(sid):
+            if not 0 <= s < self.streams:
+                raise ValueError("render: stream id %d out of range 0..%d" % (s, self.streams - 1))
             m = modes[b] if modes is not None else _lib.RENDER_TRACKS
-            if m == _lib.RENDER_GT and not (self._seeded[b] is not None and self._seeded_gt[b]):
-                raise ValueError("the ground-truth render of stream %d needs tracks seeded from pre_dets with 'kps_gt'" % b)
-            if m == _lib.RENDER_TRACKS and self._seeded[b]:
+            if m == _lib.RENDER_GT and not (self._seeded[s] is not None and self._seeded_gt[s]):
+                raise ValueError("the ground-truth render of stream %d needs tracks seeded from pre_dets with 'kps_gt'" % s)
+            if m == _lib.RENDER_TRACKS and self._seeded[s]:
                 raise ValueError("drawing the seeds of stream %d from the tracks reads %r, which a pre_dets entry lacks"
-                                 % (b, self._seeded[b]))
+                                 % (s, self._seeded[s]))
         tr = torch.as_tensor(np.asarray(trans_input, np.float64).reshape(-1, 6)) if not torch.is_tensor(trans_input) else trans_input
         if tr.shape[0] == 1 and B > 1:
             tr = tr.expand(B, 6)
@@ -302,8 +318,8 @@ class Tracker(object):
             out = (torch.empty((B, 1, inp_h, inp_w), dtype=torch.float32, device=self.device),
                    torch.empty((B, 8, inp_h, inp_w), dtype=torch.float32, device=self.device))
         with torch.cuda.device(self.device):
-            rc = self.L.cp_tracker_render_ex(self._h, B, _ptr(meta), _ptr(tr), int(inp_h), int(inp_w), mode_arr, _ptr(out[0]),
-                                             _ptr(out[1]), _stream())
+            rc = self.L.cp_tracker_render_ex2(self._h, B, _stream_map(stream_ids, B), _ptr(meta), _ptr(tr), int(inp_h),
+                                              int(inp_w), mode_arr, _ptr(out[0]), _ptr(out[1]), _stream())
         _lib.check(rc, "cp_tracker_render_ex")
         out[0]._cp_keep = (meta, tr)
         return out

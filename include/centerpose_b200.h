@@ -33,7 +33,7 @@
  *       utils/pnp/cuboid_pnp_shell.py:11-93, utils/pnp/cuboid_pnp_solver.py:91-239
  *   cp_infer
  *       detectors/base_detector.py:473-654 (process -> post_process -> merge -> PnP)
- *   cp_preprocess
+ *   cp_preprocess / cp_preprocess_affine / cp_preprocess_ragged
  *       detectors/base_detector.py:91-148 pre_process (resize + affine warp + normalise)
  */
 #ifndef CENTERPOSE_B200_H_
@@ -334,7 +334,15 @@ enum cp_dets_field {
  * on one stream.  Association is greedy (tracker.py:305-314) or, with `hungarian`, the minimum-cost assignment that
  * scipy.optimize.linear_sum_assignment returns (ties included).  Tracks can be seeded from ground truth
  * (Tracker.init_track with meta['pre_dets'], cp_tracker_seed) and the previous-frame heat maps drawn from that ground
- * truth (opt.gt_pre_hm_hmhp / gt_pre_hm_hmhp_first) or left empty (opt.empty_pre_hm), see cp_tracker_render_ex. */
+ * truth (opt.gt_pre_hm_hmhp / gt_pre_hm_hmhp_first) or left empty (opt.empty_pre_hm), see cp_tracker_render_ex.
+ *
+ * Streams are stepped independently: each stream keeps its own current buffer of the double-buffered track state, so a
+ * stream that a step does not list is left bit-for-bit as it was (tracks, ids, ages, filters, scale pool) and resumes
+ * from there.  The _ex variants (cp_tracker_step_ex, cp_tracker_render_ex2, cp_tracker_seed_ex) take a stream map:
+ * `stream_ids` is a HOST int32 [batch], owned by the caller and read before the call returns; batch row i reads and
+ * advances tracker stream stream_ids[i].  Every id must lie in 0..streams-1 and appear once, otherwise the call returns
+ * CP_ERR_INVALID before any work is enqueued.  stream_ids == NULL is the identity (row i = stream i), which is what the
+ * entry points without a map do. */
 #define CP_TRACK_RECORD 320
 typedef struct cp_tracker cp_tracker;
 typedef struct cp_tracker_config {
@@ -366,6 +374,11 @@ int cp_tracker_reset(cp_tracker* trk, int32_t index, void* stream);
  * [0, n_tracks[b]) = the reference's self.tracker.tracks in order (layout: cp_track_field); n_tracks: device int32. */
 int cp_tracker_step(cp_tracker* trk, int32_t batch, const float* poses, const int32_t* n_valid, int32_t K,
                     const double* meta, float* tracks_out, int32_t* n_tracks, void* stream);
+/* cp_tracker_step with a stream map: batch row i (poses[i], meta[i], tracks_out[i], n_tracks[i]) is tracker stream
+ * stream_ids[i].  Only the listed streams are stepped. */
+int cp_tracker_step_ex(cp_tracker* trk, int32_t batch, const int32_t* stream_ids, const float* poses,
+                       const int32_t* n_valid, int32_t K, const double* meta, float* tracks_out, int32_t* n_tracks,
+                       void* stream);
 /* _get_additional_inputs(): render the tracks of every stream into pre_hm [batch,1,inp_h,inp_w] and pre_hm_hp
  * [batch,8,inp_h,inp_w] (device fp32, overwritten).  trans_input: device fp64 [batch,6] = the row-major 2x3 affine
  * meta['trans_input'] (original image -> network input). */
@@ -383,6 +396,11 @@ enum cp_render_mode {
  * CP_RENDER_TRACKS (then identical to cp_tracker_render).  An unknown mode returns CP_ERR_INVALID. */
 int cp_tracker_render_ex(cp_tracker* trk, int32_t batch, const double* meta, const double* trans_input, int32_t inp_h,
                          int32_t inp_w, const int32_t* modes, float* pre_hm, float* pre_hm_hp, void* stream);
+/* cp_tracker_render_ex with a stream map: image i (meta[i], trans_input[i], modes[i], pre_hm[i], pre_hm_hp[i]) draws the
+ * tracks of tracker stream stream_ids[i]. */
+int cp_tracker_render_ex2(cp_tracker* trk, int32_t batch, const int32_t* stream_ids, const double* meta,
+                          const double* trans_input, int32_t inp_h, int32_t inp_w, const int32_t* modes, float* pre_hm,
+                          float* pre_hm_hp, void* stream);
 
 /* Offsets (in floats) inside one CP_SEED_RECORD: one dict of meta['pre_dets'] (eval_video_official.py:422-450). */
 #define CP_SEED_RECORD 264
@@ -403,6 +421,9 @@ enum cp_seed_field {
  * 1, 2, ... in order, their filter initialised from the seed's own kps_fusion_mean / kps_fusion_std / tracking_hp and
  * their scale pool from obj_scale / obj_scale_uncertainty.  S must be in 0..max_tracks. */
 int cp_tracker_seed(cp_tracker* trk, int32_t batch, const float* seeds, const int32_t* n_seeds, int32_t S, void* stream);
+/* cp_tracker_seed with a stream map: row i (seeds[i], n_seeds[i]) seeds tracker stream stream_ids[i]. */
+int cp_tracker_seed_ex(cp_tracker* trk, int32_t batch, const int32_t* stream_ids, const float* seeds,
+                       const int32_t* n_seeds, int32_t S, void* stream);
 
 /* Offsets (in floats) inside one CP_TRACK_RECORD slot.  [0, CP_POSE_RECORD) is the pose record of the detection the
  * track carries; its PnP fields hold the SECOND (filtered) solve whenever that produced a pose (pnp_shell mutates the
@@ -469,6 +490,16 @@ int cp_preprocess(const uint8_t* frames, float* out, int32_t B, int32_t src_h, i
  * meta['trans_input'] (source frame -> network input), e.g. for fix_short / keep_res or rotated crops. */
 int cp_preprocess_affine(const uint8_t* frames, float* out, int32_t B, int32_t src_h, int32_t src_w, int32_t dst_h,
                          int32_t dst_w, const double trans_input[6], const float mean[3], const float std[3], void* stream);
+/* A ragged batch in one launch: B frames of different sizes packed into one device buffer.  Frame b is uint8
+ * [src_hw[b][0], src_hw[b][1], 3] starting `offsets[b]` bytes into `frames` (frames_bytes long); out: device fp32 NCHW
+ * [B,3,dst_h,dst_w].  offsets (int64 [B]), src_hw (int32 [B,2]) and trans_input (double [B,6], row-major 2x3 forward
+ * affines, or NULL) are HOST arrays owned by the caller and read before the call returns.  Frame b's output equals, bit
+ * for bit, cp_preprocess_affine on that frame alone with trans_input[b], or cp_preprocess on it when trans_input is
+ * NULL.  A frame that does not fit inside frames_bytes returns CP_ERR_INVALID before any work is enqueued.  A few
+ * hundred bytes of per-frame parameters come from the stream-ordered allocator. */
+int cp_preprocess_ragged(const uint8_t* frames, int64_t frames_bytes, const int64_t* offsets, const int32_t* src_hw,
+                         float* out, int32_t B, int32_t dst_h, int32_t dst_w, const double* trans_input,
+                         const float mean[3], const float std[3], void* stream);
 
 /* ---- misc ------------------------------------------------------------------ */
 int cp_version(void);
