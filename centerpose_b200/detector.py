@@ -141,14 +141,19 @@ def check_slot_list(values, S, name, kind=None):
     return [kind(v) for v in values] if kind is not None else values
 
 
-class _SlotState(object):
-    """run_batch(list, track=True): the tracker of S slot streams and each slot's previous network input (a private
-    device buffer, written by device-to-device copies only)."""
+def _returned(pair, to_host):
+    return (pair[0].cpu().numpy(), pair[1].cpu().numpy()) if to_host else pair
 
-    def __init__(self, opt, S, ih, iw, device):
+
+class _SlotState(object):
+    """run_batch(track=True): the tracker of S slot streams, each slot's previous network input (`pre`, [S,3,h,w], None
+    before the first step; never written in place, so it may be the network input of the previous step itself) and
+    whether each slot has had a frame since the state was made."""
+
+    def __init__(self, opt, S, device):
         self.streams = S
         self.tracker = Tracker(opt, streams=S, device=device)
-        self.pre = torch.zeros((S, 3, ih, iw), dtype=torch.float32, device=device)
+        self.pre = None
         self.started = [False] * S
 
 
@@ -181,9 +186,9 @@ class ObjectPoseDetector(object):
         if getattr(opt, "tracking_task", False):
             # base_detector.py:53-54: the tracker state lives on the device (centerpose_b200/tracker.py)
             self.tracker = Tracker(opt, streams=1, device=opt.device)
-        self._batch_tracker = None
-        self._batch_pre = None
-        self._slots = None             # run_batch(list, track=True): per-slot tracker and previous frames (_SlotState)
+        self._slots = None             # run_batch(track=True): per-slot tracker and previous frames (_SlotState)
+        self._meta_key = None          # run_batch: bytes of the host meta rows last uploaded to _meta_dev
+        self._meta_dev = None
         self._packed = None            # run_batch(list): device buffer the ragged frames are packed into
         self._affines = {}             # (h, w) -> fix_res trans_input of that frame size
 
@@ -232,21 +237,21 @@ class ObjectPoseDetector(object):
                 meta[k] = input_meta[k]
         return images, meta
 
-    def _gt_frame(self, frame_id):
-        """base_detector.py:451 / :167: this frame is seeded from and drawn from the ground truth."""
-        if getattr(self.opt, "gt_pre_hm_hmhp", False):
-            return True
-        if getattr(self.opt, "gt_pre_hm_hmhp_first", False):
+    def _track_policy(self, start, frame_id, pre_dets):
+        """base_detector.py:440-465 for one stream and frame: (the pre_dets to seed the stream from, or None; the
+        cp_render_mode of its previous-frame heat maps).  A stream is seeded when its video starts and on ground-truth
+        frames (opt.gt_pre_hm_hmhp: every frame; opt.gt_pre_hm_hmhp_first: frame_id 0; :451-454), whose heat maps are
+        drawn from the ground truth; with opt.empty_pre_hm they are empty (_get_additional_inputs, :165-166)."""
+        gt = bool(getattr(self.opt, "gt_pre_hm_hmhp", False))
+        if not gt and getattr(self.opt, "gt_pre_hm_hmhp_first", False):
             if frame_id is None:
                 raise ValueError("opt.gt_pre_hm_hmhp_first needs the frame index, meta['id']")
-            return int(frame_id) == 0
-        return False
-
-    def _render_mode(self, gt):
-        """_get_additional_inputs (base_detector.py:165-166): empty, ground truth or the tracks."""
+            gt = int(frame_id) == 0
         if getattr(self.opt, "empty_pre_hm", False):
-            return _lib.RENDER_EMPTY
-        return _lib.RENDER_GT if gt else _lib.RENDER_TRACKS
+            mode = _lib.RENDER_EMPTY
+        else:
+            mode = _lib.RENDER_GT if gt else _lib.RENDER_TRACKS
+        return (pre_dets if start or gt else None), mode
 
     def _meta_tensor(self, meta, batch=1):
         cam = meta.get("camera_matrix")
@@ -324,19 +329,19 @@ class ObjectPoseDetector(object):
 
             pre_hms, pre_hm_hp, pre_inds = None, None, None
             if tracking:
-                gt = self._gt_frame(meta.get("id"))
-                if self.pre_images is None:                       # base_detector.py:444-449
+                start = self.pre_images is None
+                seed, mode = self._track_policy(start, meta.get("id"), meta.get("pre_dets"))
+                if start:                                         # base_detector.py:444-449
                     print("Initialize tracking!")
                     self.pre_images = images
-                    self.tracker.init_track(meta)
-                elif gt:                                          # :451-454, ground-truth seeding
+                if start or seed is not None:
                     self.tracker.init_track(meta)
                 if self.opt.pre_hm or self.opt.pre_hm_hp:         # :456-462, rendered on the device from the tracker state
                     if "trans_input" not in meta:
                         raise ValueError("tracking needs meta['trans_input'] (pre_process provides it)")
                     metat = self._meta_tensor(meta).to(images.device)
                     pre_hms, pre_hm_hp = self.tracker.render(metat, meta["trans_input"], images.shape[2], images.shape[3],
-                                                             modes=[self._render_mode(gt)])
+                                                             modes=[mode])
             torch.cuda.synchronize()
             pre_process_time = time.time()
             pre_time += pre_process_time - scale_start_time
@@ -532,20 +537,25 @@ class ObjectPoseDetector(object):
         whole batch.  Returns (poses [B,K,192], n_valid [B]) -- on the host when
         `to_host`, else as CUDA tensors.
 
-        track=True (tracking models): the batch is B independent VIDEO STREAMS and every call is their next frame.
-        The previous frames, the tracker state and the rendered previous-frame heat maps stay on the device; returns
-        (tracks [B,T,320], n_tracks [B]) (layout: cp_track_field) instead.  pre_dets: None, or per stream the
-        meta['pre_dets'] list of this frame (or None); frame_ids: per stream meta['id'] (needed with
-        opt.gt_pre_hm_hmhp_first).  Per stream, seeding and the heat maps follow run(): seeded on the first frame and on
-        ground-truth frames, drawn from the ground truth on those frames, empty with opt.empty_pre_hm.
+        frames may also be a LIST of uint8 [H_b,W_b,3] frames of mixed sizes (numpy, CPU or CUDA tensors), with
+        camera_matrix [3,3] or one per frame [B,3,3]: one ragged pre-process launch, one network + decode call, and
+        every frame's records in its own pixels (its own c, s and meta row), exactly what run() gives for it.
 
         out: optional (poses, n_valid) CUDA tensors to write into (e.g. the views of a dist.PoseBuffer, so that the
         records land directly in the buffer of the all-gather / the pinned D2H copy).
 
-        frames may also be a LIST of uint8 [H_b,W_b,3] frames of mixed sizes (numpy, CPU or CUDA tensors), with
-        camera_matrix [3,3] or one per frame [B,3,3]: one ragged pre-process launch, one network + decode call, and
-        every frame's records in its own pixels (its own c, s and meta row), exactly what run() gives for it.  With
-        track=True the list is indexed by SLOT, each slot an independent video (see `_run_slots`)."""
+        track=True (tracking models): the batch is B independent video streams, or SLOTS, and every call is their next
+        frame.  The previous frames, the tracker state and the rendered previous-frame heat maps stay on the device;
+        returns (tracks [B,T,320], n_tracks [B]) (layout: cp_track_field) instead.  pre_dets: None, or per slot the
+        meta['pre_dets'] list of this frame (or None); frame_ids: per slot meta['id'] (needed with
+        opt.gt_pre_hm_hmhp_first).  Per slot, seeding and the heat maps follow run(): seeded when its video starts and
+        on ground-truth frames, drawn from the ground truth on those frames, empty with opt.empty_pre_hm.  A slot's
+        video starts on its first frame after the state is made (first call, a new number of slots, reset_tracking()).
+        Both forms go through one tracking step (`_track_step`); the array form is the case where every slot steps.
+        With a list, a None frame idles its slot this call, new_video[i] starts a new video in slot i, and `out` (see
+        `_run_slots`) is honoured; the array form ignores `out`."""
+        if track and not getattr(self.opt, "tracking_task", False):
+            raise ValueError("run_batch(track=True) needs a tracking model (opt.tracking_task)")
         if isinstance(frames, (list, tuple)):
             if pre_images is not None or pre_hms is not None or pre_hm_hp is not None:
                 raise ValueError("run_batch(list): the previous frames and heat maps are kept per slot (track=True)")
@@ -553,63 +563,40 @@ class ObjectPoseDetector(object):
                 return self._run_slots(frames, camera_matrix, to_host, out, pre_dets, frame_ids, new_video)
             if new_video is not None or pre_dets is not None or frame_ids is not None:
                 raise ValueError("run_batch(list): new_video / pre_dets / frame_ids need track=True")
-            return self._run_list(frames, camera_matrix, to_host, out)
-        if new_video is not None:
-            raise ValueError("run_batch: new_video needs a list of slot frames")
-        dev = self.opt.device
-        if isinstance(frames, np.ndarray):
-            frames = torch.from_numpy(frames)
-        if frames.dtype == torch.uint8:
-            B, sh, sw, _ = frames.shape
-            fr = frames.to(dev, non_blocking=True)
-            x = preprocess(fr, self.opt.input_h, self.opt.input_w, self.opt.mean, self.opt.std)
-            c, s = np.array([sw / 2., sh / 2.], np.float32), float(max(sh, sw))
-            iw, ih = sw, sh
+            check_frames(frames, allow_idle=False)
+            x, meta, _ = self._ragged_input(frames, camera_matrix)
         else:
-            x = frames.to(dev)
-            B, _, ih, iw = x.shape
-            c, s = np.array([iw / 2., ih / 2.], np.float32), float(max(ih, iw))
-        # the per-frame meta (centre / scale / size / camera) of a fixed frame shape and camera is uploaded once
-        cam_key = np.asarray(camera_matrix, np.float64).tobytes()
-        mkey = (B, iw, ih, cam_key, str(dev))
-        if getattr(self, "_meta_key", None) != mkey:
-            self._meta_dev = make_meta(B, c, s, iw, ih, camera_matrix).to(dev)
-            self._meta_key = mkey
-        meta = self._meta_dev
-        eng = self.model.engine(B, x.shape[2], x.shape[3], x.device)
-        # the batched path pre-processes at scale 1 (what every shipped configuration uses); results of a multi-scale
-        # opt are those of test_scales[0] (object_pose.py:188), which run() reproduces frame by frame
-        if float(self.scales[0]) != 1.0:
-            raise NotImplementedError("run_batch pre-processes at scale 1; use run() for test_scales[0] != 1")
-        prm = decode_params(self.opt, test_scale=1.0)
-        if track:
-            if not getattr(self.opt, "tracking_task", False):
-                raise ValueError("run_batch(track=True) needs a tracking model (opt.tracking_task)")
-            trk = self._batch_tracker
-            if trk is None or trk.streams != B:
-                trk = self._batch_tracker = Tracker(self.opt, streams=B, device=x.device)
-                self._batch_pre = None
-            gts = [self._gt_frame(frame_ids[b] if frame_ids is not None else None) for b in range(B)]
-            first = self._batch_pre is None or self._batch_pre.shape != x.shape
-            if first:
-                self._batch_pre = x                                   # first frame: pre_images = images (base_detector.py:446)
-            if pre_dets is not None:
-                if len(pre_dets) != B:
+            if new_video is not None:
+                raise ValueError("run_batch: new_video needs a list of slot frames")
+            dev = self.opt.device
+            if isinstance(frames, np.ndarray):
+                frames = torch.from_numpy(frames)
+            if frames.dtype == torch.uint8:
+                B, sh, sw, _ = frames.shape
+                fr = frames.to(dev, non_blocking=True)
+                x = preprocess(fr, self.opt.input_h, self.opt.input_w, self.opt.mean, self.opt.std)
+                c, s = np.array([sw / 2., sh / 2.], np.float32), float(max(sh, sw))
+                iw, ih = sw, sh
+            else:
+                x = frames.to(dev)
+                B, _, ih, iw = x.shape
+                c, s = np.array([iw / 2., ih / 2.], np.float32), float(max(ih, iw))
+            meta = make_meta(B, c, s, iw, ih, camera_matrix).numpy()
+            # the batched path pre-processes at scale 1 (what every shipped configuration uses); results of a multi-scale
+            # opt are those of test_scales[0] (object_pose.py:188), which run() reproduces frame by frame
+            if float(self.scales[0]) != 1.0:
+                raise NotImplementedError("run_batch pre-processes at scale 1; use run() for test_scales[0] != 1")
+            if track:
+                if pre_dets is not None and len(pre_dets) != B:
                     raise ValueError("run_batch: %d pre_dets lists for %d streams" % (len(pre_dets), B))
-                trk.seed([pre_dets[b] if (first or gts[b]) else None for b in range(B)])
-            trans = affine_from_center_scale(c, s, x.shape[3], x.shape[2])
-            pre_hms, pre_hm_hp = trk.render(meta, trans, x.shape[2], x.shape[3], modes=[self._render_mode(g) for g in gts])
-            _, poses, n_valid = eng.infer(x, meta, prm, self._batch_pre, pre_hms, pre_hm_hp)
-            tracks, nt = trk.step_records(poses, n_valid, meta)
-            self._batch_pre = x
-            if to_host:
-                return tracks.cpu().numpy(), nt.cpu().numpy()
-            return tracks, nt
-        _, poses, n_valid = eng.infer(x, meta, prm, pre_images, pre_hms, pre_hm_hp,
-                                      poses=out[0] if out is not None else None, n_valid=out[1] if out is not None else None)
-        if to_host:
-            return poses.cpu().numpy(), n_valid.cpu().numpy()
-        return poses, n_valid
+                trans = affine_from_center_scale(c, s, x.shape[3], x.shape[2])
+                return self._track_step(B, list(range(B)), x, self._meta_rows(meta), trans, None, pre_dets, frame_ids,
+                                        to_host, None)
+        eng = self.model.engine(x.shape[0], x.shape[2], x.shape[3], x.device)
+        _, poses, n_valid = eng.infer(x, self._meta_rows(meta), decode_params(self.opt, test_scale=1.0), pre_images,
+                                      pre_hms, pre_hm_hp, poses=out[0] if out is not None else None,
+                                      n_valid=out[1] if out is not None else None)
+        return _returned((poses, n_valid), to_host)
 
     # ------------------------------------------------------------------ ragged batches (lists of frames)
     def _ragged_input(self, frames, camera_matrix):
@@ -648,51 +635,30 @@ class ObjectPoseDetector(object):
         return x, meta, trans
 
     def _meta_rows(self, meta):
-        """Host meta rows -> a device tensor, uploaded again only when the rows change."""
+        """Host meta rows -> a device tensor, uploaded again only when the rows change (a fixed frame size and camera
+        are uploaded once)."""
         key = meta.tobytes()
-        if getattr(self, "_list_meta_key", None) != key:
-            self._list_meta = torch.from_numpy(meta).to(self.opt.device)
-            self._list_meta_key = key
-        return self._list_meta
-
-    def _run_list(self, frames, camera_matrix, to_host, out):
-        """run_batch on a list of frames of mixed sizes: (poses [B,K,192], n_valid [B]), row b in frame b's pixels."""
-        check_frames(frames, allow_idle=False)
-        x, meta, _ = self._ragged_input(frames, camera_matrix)
-        B = len(frames)
-        metat = self._meta_rows(meta)
-        eng = self.model.engine(B, x.shape[2], x.shape[3], x.device)
-        prm = decode_params(self.opt, test_scale=1.0)
-        _, poses, n_valid = eng.infer(x, metat, prm, poses=out[0] if out is not None else None,
-                                      n_valid=out[1] if out is not None else None)
-        if to_host:
-            return poses.cpu().numpy(), n_valid.cpu().numpy()
-        return poses, n_valid
+        if self._meta_key != key:
+            self._meta_dev = torch.from_numpy(meta).to(self.opt.device)
+            self._meta_key = key
+        return self._meta_dev
 
     def _run_slots(self, frames, camera_matrix, to_host, out, pre_dets, frame_ids, new_video):
         """run_batch(list, track=True): frames[i] is the next frame of the video in slot i, or None when slot i is idle
         this step (its tracker stream is not stepped and keeps its state).  new_video[i] marks the first frame of a
         video in slot i, which then behaves exactly like the first run() call of a fresh detector: the stream is reset,
         the frame is its own previous frame, it is seeded from pre_dets[i] when given, and its heat maps follow
-        opt.gt_pre_hm_hmhp* / opt.empty_pre_hm.  A slot's first frame always starts a video.  Only the live slots go
-        through the network (as one batch); each slot keeps its previous network input in a persistent device buffer.
+        opt.gt_pre_hm_hmhp* / opt.empty_pre_hm.  Only the live slots go through the network (as one batch).
 
         Returns (tracks [S,T,320], n_tracks [S]) for the S slots, idle slots with n_tracks 0 and zero rows; out:
         optional (tracks, n_tracks) CUDA tensors of those shapes to write into."""
-        if not getattr(self.opt, "tracking_task", False):
-            raise ValueError("run_batch(track=True) needs a tracking model (opt.tracking_task)")
         S = len(frames)
         check_frames(frames, allow_idle=True)
         cams = camera_per_frame(camera_matrix, S)
         new_video = check_slot_list(new_video, S, "new_video", bool)
         pre_dets = check_slot_list(pre_dets, S, "pre_dets")
         frame_ids = check_slot_list(frame_ids, S, "frame_ids")
-        dev = self.opt.device
-        ih, iw = self.opt.input_h, self.opt.input_w
-        st = self._slots
-        if st is None or st.streams != S:
-            st = self._slots = _SlotState(self.opt, S, ih, iw, dev)
-        T = st.tracker.max_tracks
+        dev, T = self.opt.device, _lib.CP_MAX_K
         if out is None:
             out = (torch.empty((S, T, _lib.CP_TRACK_RECORD), dtype=torch.float32, device=dev),
                    torch.empty((S,), dtype=torch.int32, device=dev))
@@ -700,60 +666,72 @@ class ObjectPoseDetector(object):
               or out[0].dtype != torch.float32 or out[1].dtype != torch.int32):
             raise ValueError("run_batch: out must be (tracks [%d,%d,%d] fp32, n_tracks [%d] int32)" % (S, T, _lib.CP_TRACK_RECORD, S))
         live = [i for i in range(S) if frames[i] is not None]
-        for i in range(S):
-            if i not in live:
-                out[0][i].zero_()
-                out[1][i:i + 1].zero_()
         if not live:
-            return (out[0].cpu().numpy(), out[1].cpu().numpy()) if to_host else out
-        trk = st.tracker
+            out[0].zero_()
+            out[1].zero_()
+            return _returned(out, to_host)
         x, meta, trans = self._ragged_input([frames[i] for i in live], np.stack([cams[i] for i in live]))
-        metat = self._meta_rows(meta)
-        gts, seeds = [], [None] * S
+        return self._track_step(S, live, x, self._meta_rows(meta), trans, new_video, pre_dets, frame_ids, to_host, out)
+
+    def _track_step(self, S, live, x, metat, trans, new_video, pre_dets, frame_ids, to_host, out):
+        """One tracking step of S slots, both forms of run_batch(track=True).  Row k of x (network input [n,3,h,w]),
+        metat (device meta rows [n,16]) and trans (trans_input, [n,2,3] or one [2,3] for all) is the next frame of slot
+        live[k]; new_video / pre_dets / frame_ids: None or per slot.  Writes (tracks [S,T,320], n_tracks [S]) into out
+        (None: new tensors; only when every slot is live), slots not in `live` with n_tracks 0 and zero rows."""
+        if self._slots is None or self._slots.streams != S:
+            self._slots = _SlotState(self.opt, S, self.opt.device)
+        st = self._slots
+        trk = st.tracker
+        # looked up before the render, whose trans_input upload waits for the device: host work between that upload and
+        # the network launch would leave the GPU idle
+        eng = self.model.engine(S, x.shape[2], x.shape[3], x.device)
+        prm = decode_params(self.opt, test_scale=1.0)
+        # previous frames of another size (an fp32 array input that changed size): every slot takes this frame as its
+        # previous frame and is seeded as at a start, but keeps its tracks
+        resized = st.pre is not None and st.pre.shape[1:] != x.shape[1:]
+        if resized and len(live) < S:
+            raise ValueError("run_batch: the network input changed size from %s to %s while slots are idle"
+                             % (tuple(st.pre.shape[2:]), tuple(x.shape[2:])))
+        new = [not st.started[i] or (new_video is not None and new_video[i]) for i in live]
+        starts = [n or resized for n in new]
+        seeds, modes = [None] * S, []
         for k, i in enumerate(live):
-            gt = self._gt_frame(frame_ids[i] if frame_ids is not None else None)
-            gts.append(gt)
-            start = (new_video is not None and new_video[i]) or not st.started[i]
-            if start:                                         # base_detector.py:444-449: a fresh stream
+            seeds[i], mode = self._track_policy(starts[k], frame_ids[i] if frame_ids is not None else None,
+                                                pre_dets[i] if pre_dets is not None else None)
+            modes.append(mode)
+        for k, i in enumerate(live):
+            if new[k]:                                        # base_detector.py:444-449: a fresh stream
                 trk.reset(i)
-                st.pre[i].copy_(x[k])
                 st.started[i] = True
-            if pre_dets is not None and pre_dets[i] is not None and (start or gt):
-                seeds[i] = pre_dets[i]
         trk.seed(seeds)
-        all_live = len(live) == S
-        if all_live:
+        all_live = len(live) == S                             # every slot, in order: stream map NULL (the identity)
+        if all(starts):
+            pre = x
+        elif all_live and not any(starts):
             pre = st.pre
         else:
-            pre = torch.empty_like(x)
-            for k, i in enumerate(live):
-                pre[k].copy_(st.pre[i])
-        pre_hms, pre_hm_hp = trk.render(metat, trans.reshape(-1, 6), ih, iw, modes=[self._render_mode(g) for g in gts],
-                                        stream_ids=live)
-        eng = self.model.engine(S, ih, iw, x.device)
-        prm = decode_params(self.opt, test_scale=1.0)
+            pre = torch.stack([x[k] if starts[k] else st.pre[i] for k, i in enumerate(live)])
+        ids = None if all_live else live
+        pre_hms, pre_hm_hp = trk.render(metat, trans, x.shape[2], x.shape[3], modes=modes, stream_ids=ids)
         _, poses, n_valid = eng.infer(x, metat, prm, pre, pre_hms, pre_hm_hp)
         if all_live:
-            trk.step_records(poses, n_valid, metat, out=out, stream_ids=live)
-            st.pre.copy_(x)
+            out = trk.step_records(poses, n_valid, metat, out=out)
+            st.pre = x
         else:
-            tr, nt = trk.step_records(poses, n_valid, metat, stream_ids=live)
-            for k, i in enumerate(live):
-                out[0][i].copy_(tr[k])
-                out[1][i:i + 1].copy_(nt[k:k + 1])
-                st.pre[i].copy_(x[k])
-        if to_host:
-            return out[0].cpu().numpy(), out[1].cpu().numpy()
-        return out
+            tr, nt = trk.step_records(poses, n_valid, metat, stream_ids=ids)
+            row = {i: k for k, i in enumerate(live)}
+            old = st.pre if st.pre is not None else x.new_zeros((S,) + tuple(x.shape[1:]))
+            st.pre = torch.stack([x[row[i]] if i in row else old[i] for i in range(S)])
+            zt, zn = tr.new_zeros(tr.shape[1:]), nt.new_zeros(())
+            torch.stack([tr[row[i]] if i in row else zt for i in range(S)], out=out[0])
+            torch.stack([nt[row[i]] if i in row else zn for i in range(S)], out=out[1])
+        return _returned(out, to_host)
 
     def reset_tracking(self):
         """base_detector.py:774-776."""
         if self.tracker is not None:
             self.tracker.reset()
         self.pre_images = None
-        self._batch_pre = None
-        if self._batch_tracker is not None:
-            self._batch_tracker.reset()
         self._slots = None
 
 

@@ -168,12 +168,9 @@ class TrackPipeline(object):
         return len(self._queue)
 
     def _local(self, values, name):
-        if values is None:
-            return None
-        values = list(values)
-        if len(values) != self.slots:
-            raise ValueError("TrackPipeline: %d %s entries for %d slots" % (len(values), name, self.slots))
-        return values[self.lo:self.hi]
+        from .detector import check_slot_list
+        values = check_slot_list(values, self.slots, name)
+        return None if values is None else values[self.lo:self.hi]
 
     def submit(self, frames, new_video=None, pre_dets=None, frame_ids=None, camera_matrix=None):
         """frames: one entry per slot (all `slots`, on every rank): uint8 [H,W,3] numpy array or CPU tensor (pinned

@@ -1,7 +1,8 @@
 """Independent video streams on the device: the ragged pre-process (cp_preprocess_ragged) against cv2, the numpy
 restatement and the per-frame kernels; run_batch on mixed-size lists against run(); the tracker's stream maps
 (cp_tracker_*_ex) against the entry points without one; slot schedules with restarts and idle slots against each video
-run alone; and TrackPipeline against the same run_batch sequence."""
+run alone; the array and list forms of run_batch(track=True) against each other and the array form's change of input
+size against the tracker driven by hand; and TrackPipeline against the same run_batch sequence."""
 import ctypes
 import json
 import os
@@ -287,6 +288,73 @@ def test_slot_schedule_matches_each_video_alone(cplib):
                 checked += 1
                 paused += e in ((1, 2), (2, 4))            # the frames right after a two-step pause
         assert checked == sum(e is not None for s in SCHEDULE for e in s) and paused == 2
+
+
+@pytest.mark.parametrize("gt", (False, True), ids=("tracks", "ground_truth"))
+def test_array_and_list_forms_give_identical_tracks(gt, cplib):
+    """The same uniform 512x512 uint8 frames through run_batch(array, track=True) and through run_batch(list,
+    track=True) with new_video on the first step: at 512 -> 512 both pre-process affines are exactly the identity, so
+    every step's tracks agree bit for bit -- also when pre_dets / frame_ids seed the streams from the ground truth."""
+    det, opt = _tracking_detector()
+    opt.gt_pre_hm_hmhp_first = gt
+    cam = _cam(512, 512)
+    S, steps = 3, 4
+    vids = [synth.synthetic_frames(steps, 512, 512, seed=120 + v) for v in range(S)]
+    _, seq = mg.make_sequence()
+    runs = []
+    for form in ("array", "list"):
+        det.reset_tracking()
+        got = []
+        for f in range(steps):
+            batch = np.stack([vids[v][f] for v in range(S)])
+            kw = {"pre_dets": [mgt.gt_list(seq[v]) for v in range(S)], "frame_ids": [f] * S} if gt else {}
+            if form == "list":
+                batch, kw["new_video"] = list(batch), [f == 0] * S
+            got.append(det.run_batch(batch, cam, track=True, **kw))
+        runs.append(got)
+    assert sum(int(n.sum()) for _, n in runs[0]) > 0
+    for f, ((ta, na), (tl, nl)) in enumerate(zip(*runs)):
+        assert np.array_equal(na, nl), f
+        for v in range(S):
+            n = int(na[v])
+            assert np.array_equal(ta[v, :n], tl[v, :n]), (f, v, np.argwhere(ta[v, :n] != tl[v, :n])[:8])
+
+
+@pytest.mark.parametrize("seeded", (False, True))
+def test_array_input_of_a_new_size_keeps_the_tracks(seeded, cplib):
+    """run_batch(fp32 [B,3,h,w], track=True) whose size changes at the same stream count: the new frame is every
+    stream's previous frame and the streams are seeded as at a start, but their tracks are not reset -- the same as
+    driving the tracker, the heat-map render and the network by hand."""
+    from centerpose_b200.engine import decode_params
+    det, opt = _tracking_detector()
+    cam = _cam(512, 512)
+    pre = _seed_dets(det, synth.synthetic_frames(1, 512, 512, seed=5)[0], cam) if seeded else None
+    B = 2
+    sizes = [(512, 512), (512, 512), (384, 448), (384, 448)]
+    xs = [torch.from_numpy(synth.normalize_frames(synth.synthetic_frames(B, h, w, seed=140 + f))).cuda()
+          for f, (h, w) in enumerate(sizes)]
+    got = [det.run_batch(x, cam, track=True, pre_dets=[pre] * B if seeded else None) for x in xs]
+    trk = cpb.Tracker(opt, streams=B)
+    prm = decode_params(opt, test_scale=1.0)
+    prev = None
+    for f, x in enumerate(xs):
+        h, w = x.shape[2:]
+        c, s = np.array([w / 2., h / 2.], np.float32), float(max(h, w))
+        meta = cpb.make_meta(B, c, s, w, h, cam).cuda()
+        if prev is None or prev.shape != x.shape:
+            prev = x
+            if seeded:
+                trk.seed([pre] * B)
+        hms = trk.render(meta, affine_from_center_scale(c, s, w, h), h, w, modes=[L.RENDER_TRACKS] * B)
+        _, poses, nv = det.model.engine(B, h, w, x.device).infer(x, meta, prm, prev, *hms)
+        tr, nt = trk.step_records(poses, nv, meta)
+        tr, nt = tr.cpu().numpy(), nt.cpu().numpy()
+        prev = x
+        assert np.array_equal(nt, got[f][1]), f
+        for b in range(B):
+            n = int(nt[b])
+            assert np.array_equal(tr[b, :n], got[f][0][b, :n]), (f, b)
+    assert int(got[2][1].sum()) > 0
 
 
 def test_track_pipeline_matches_run_batch(cplib):
