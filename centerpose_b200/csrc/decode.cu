@@ -5,6 +5,9 @@
 //   peaks_topk_kernel   one CTA per (image, heat-map channel): sigmoid, 3x3
 //                       equality NMS and an exact top-K (radix select + bitonic
 //                       sort) in shared memory -- each map is read from HBM once.
+//                       Maps over TOPK_SMEM_CELLS cells (keep_res / fix_short
+//                       inputs of ~800 x 600 and up) keep the NMS-ed map in the
+//                       workspace instead; the selection is the same.
 //   group_pose_kernel   one CTA per image: gathers at the K centres, K x K
 //                       nearest-peak match per joint, the decode.py gates, the
 //                       post_process.py affine, soft-NMS and the PnP solve
@@ -28,19 +31,27 @@ namespace {
 constexpr float SENT = -10000.0f;
 constexpr int TOPK_THREADS = 1024;
 constexpr int KM = CP_MAX_K;
+// cells of a heat map whose sigmoid and NMS-ed copies both fit the kernel's shared memory (200 KB of 8 bytes per cell)
+constexpr size_t TOPK_SMEM_CELLS = 200 * 1024 / 8;
+
+__host__ __device__ __forceinline__ bool topk_staged(size_t hw) { return hw <= TOPK_SMEM_CELLS; }
 
 __device__ __forceinline__ float sigmoid_acc(float x) { return 1.0f / (1.0f + expf(-x)); }
 
 // ---------------------------------------------------------------------------
 // kernel 1: per-channel sigmoid + NMS + top-K
+// STAGED: the sigmoid map (raw) and the NMS-ed map (nv) live in shared memory (topk_staged).  Otherwise the NMS reads
+// the map from global memory, recomputing the sigmoid of each neighbour, and nv is this channel's slice of nv_ws
+// ([B][C_hm + J][HW] floats of the workspace); the values and the selection are the same.
 // ---------------------------------------------------------------------------
+template <bool STAGED>
 __global__ void __launch_bounds__(TOPK_THREADS, 1)
 peaks_topk_kernel(const float* __restrict__ hm, const float* __restrict__ hm_hp, int C_hm, int J, int H, int W,
-                  int K, int apply_sigmoid, float* __restrict__ peak_val, int* __restrict__ peak_idx) {
+                  int K, int apply_sigmoid, float* __restrict__ peak_val, int* __restrict__ peak_idx,
+                  float* __restrict__ nv_ws) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const int HW = H * W;
   float* raw = reinterpret_cast<float*>(smem_raw);
-  float* nv = raw + HW;
   __shared__ unsigned int hist[256];
   __shared__ unsigned int s_prefix, s_need, s_cnt;
   __shared__ int warp_tot[TOPK_THREADS / 32];
@@ -53,15 +64,23 @@ peaks_topk_kernel(const float* __restrict__ hm, const float* __restrict__ hm_hp,
   // apply_sigmoid: 0 = both maps are probabilities already, 1 = both are logits, 2 = only hm is a logit
   // (opt.mse_loss: the reference skips the hm_hp sigmoid, object_pose.py:136-138)
   const bool sig = (ch < C_hm) ? (apply_sigmoid != 0) : (apply_sigmoid == 1);
-  for (int i = tid; i < HW; i += TOPK_THREADS) {
-    float v = __ldg(src + i);
-    raw[i] = sig ? sigmoid_acc(v) : v;
+  float* nv = STAGED ? raw + HW : nv_ws + ((size_t)b * CH + ch) * HW;
+  auto heat = [&](int i) -> float {
+    if (STAGED) return raw[i];
+    const float v = __ldg(src + i);
+    return sig ? sigmoid_acc(v) : v;
+  };
+  if (STAGED) {
+    for (int i = tid; i < HW; i += TOPK_THREADS) {
+      float v = __ldg(src + i);
+      raw[i] = sig ? sigmoid_acc(v) : v;
+    }
+    __syncthreads();
   }
-  __syncthreads();
   // 3x3 max-pool (stride 1, -inf padding) equality NMS: keep = (hmax == heat)
   for (int i = tid; i < HW; i += TOPK_THREADS) {
     int y = i / W, x = i - y * W;
-    float v = raw[i];
+    float v = heat(i);
     float m = v;
     for (int dy = -1; dy <= 1; ++dy) {
       int yy = y + dy;
@@ -69,7 +88,7 @@ peaks_topk_kernel(const float* __restrict__ hm, const float* __restrict__ hm_hp,
       for (int dx = -1; dx <= 1; ++dx) {
         int xx = x + dx;
         if (xx < 0 || xx >= W) continue;
-        m = fmaxf(m, raw[yy * W + xx]);
+        m = fmaxf(m, heat(yy * W + xx));
       }
     }
     nv[i] = (m == v) ? v + 0.0f : 0.0f;      // heat * keep; -0 is canonicalised (torch.topk compares it equal to +0)
@@ -576,7 +595,7 @@ __global__ void __launch_bounds__(256, 1) group_pose_kernel(const GroupArgs a) {
 }
 
 struct WsLayout {
-  size_t peak_val, peak_idx, dets, total;
+  size_t peak_val, peak_idx, dets, nv, total;
 };
 
 WsLayout ws_layout(const cp_decode_params* p) {
@@ -589,6 +608,9 @@ WsLayout ws_layout(const cp_decode_params* p) {
   off += (n * sizeof(int) + 255) / 256 * 256;
   w.dets = off;
   off += ((size_t)p->batch * p->K * CP_DETS_RECORD * sizeof(float) + 255) / 256 * 256;
+  w.nv = off;        // the NMS-ed maps of peaks_topk_kernel when they do not fit its shared memory
+  const size_t hw = (size_t)p->out_h * p->out_w;
+  if (!topk_staged(hw)) off += ((size_t)p->batch * (p->num_classes + p->num_joints) * hw * sizeof(float) + 255) / 256 * 256;
   w.total = off;
   return w;
 }
@@ -602,8 +624,7 @@ int validate(const cp_decode_params* p) {
   if (p->num_joints != 8) return fail(CP_ERR_INVALID, "decode: num_joints must be 8");
   if (p->K <= 0 || p->K > CP_MAX_K) return fail(CP_ERR_INVALID, "decode: K must be in 1..128");
   if ((size_t)p->out_h * p->out_w < (size_t)p->K) return fail(CP_ERR_INVALID, "decode: map smaller than K");
-  if ((size_t)p->out_h * p->out_w * 8 > 200 * 1024)
-    return fail(CP_ERR_INVALID, "decode: head map too large for the shared-memory top-K (max 25600 cells)");
+  if ((size_t)p->out_h * p->out_w >= (1u << 30)) return fail(CP_ERR_INVALID, "decode: head map too large");
   if (p->rep_mode == 2)
     return fail(CP_ERR_INVALID, "decode: rep_mode 2 (random GMM sampling, base_detector.py:568-650) is not supported");
   if (p->rep_mode < 0 || p->rep_mode > 4) return fail(CP_ERR_INVALID, "decode: rep_mode must be 0, 1, 3 or 4");
@@ -639,16 +660,22 @@ int cp_decode_pnp(const cp_decode_params* prm, const cp_heads* heads, const doub
   float* dets_buf = dets ? dets : (float*)(ws + w.dets);
 
   const int HW = prm->out_h * prm->out_w;
-  const size_t smem = (size_t)HW * 2 * sizeof(float);
-  static cp::PerDevice<size_t> configured;
-  if (smem > configured.here()) {
-    CP_CUDA_CHECK(cudaFuncSetAttribute(peaks_topk_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    configured.here() = smem;
-  }
   dim3 g1(prm->num_classes + prm->num_joints, prm->batch);
-  peaks_topk_kernel<<<g1, TOPK_THREADS, smem, s>>>(heads->hm, heads->hm_hp, prm->num_classes, prm->num_joints,
-                                                   prm->out_h, prm->out_w, prm->K, prm->apply_sigmoid, peak_val,
-                                                   peak_idx);
+  if (topk_staged(HW)) {
+    const size_t smem = (size_t)HW * 2 * sizeof(float);
+    static cp::PerDevice<size_t> configured;
+    if (smem > configured.here()) {
+      CP_CUDA_CHECK(cudaFuncSetAttribute(peaks_topk_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+      configured.here() = smem;
+    }
+    peaks_topk_kernel<true><<<g1, TOPK_THREADS, smem, s>>>(heads->hm, heads->hm_hp, prm->num_classes, prm->num_joints,
+                                                           prm->out_h, prm->out_w, prm->K, prm->apply_sigmoid, peak_val,
+                                                           peak_idx, nullptr);
+  } else {
+    peaks_topk_kernel<false><<<g1, TOPK_THREADS, 0, s>>>(heads->hm, heads->hm_hp, prm->num_classes, prm->num_joints,
+                                                         prm->out_h, prm->out_w, prm->K, prm->apply_sigmoid, peak_val,
+                                                         peak_idx, (float*)(ws + w.nv));
+  }
   CP_LAUNCH_CHECK("peaks_topk_kernel");
   GroupArgs ga;
   ga.prm = *prm;

@@ -103,6 +103,14 @@ def affine_from_center_scale(c, s, out_w, out_h, inv=False):
     return cv2.getAffineTransform(dst, src) if inv else cv2.getAffineTransform(src, dst)
 
 
+def scale_width(s):
+    """The scale of a pre_process meta as one number: `s` is max(h, w) in the fix_res mode and the (w, h) pair in the
+    keep_res and fix_short modes, of which get_affine_transform uses only the width (image.py:44-45).  The meta row
+    and so the decode's s / max(w, h) ratio take the same width (post_process.py:33,45,48,60 would broadcast a (w, h)
+    pair against the 16 keypoint values and fail)."""
+    return float(s[0]) if isinstance(s, np.ndarray) and s.ndim else float(s)
+
+
 def camera_per_frame(camera_matrix, B):
     """camera_matrix [3,3] (shared) or [B,3,3] / a list of B [3,3] -> B float64 [3,3] matrices."""
     cam = np.asarray(camera_matrix, np.float64)
@@ -220,7 +228,7 @@ class ObjectPoseDetector(object):
             inp_width = (new_width | self.opt.pad) + 1
             c = np.array([new_width // 2, new_height // 2], dtype=np.float32)
             s = np.array([inp_width, inp_height], dtype=np.float32)
-        s0 = float(s[0]) if isinstance(s, np.ndarray) else float(s)      # the affine only uses the width (image.py:44)
+        s0 = scale_width(s)                                                # the affine only uses the width (image.py:44)
         trans_input = affine_from_center_scale(c, s0, inp_width, inp_height)
         out_height = inp_height // self.opt.down_ratio
         out_width = inp_width // self.opt.down_ratio
@@ -259,7 +267,7 @@ class ObjectPoseDetector(object):
             if self.opt.use_pnp:
                 raise ValueError("meta_inp['camera_matrix'] is required when opt.use_pnp is set (demo.py:141-147)")
             cam = np.eye(3)
-        return make_meta(batch, meta["c"], meta["s"], meta["width"], meta["height"], cam)
+        return make_meta(batch, meta["c"], scale_width(meta["s"]), meta["width"], meta["height"], cam)
 
     def process(self, images, pre_images=None, pre_hms=None, pre_hm_hp=None, pre_inds=None, return_time=False,
                 meta=None, scale=1.0):

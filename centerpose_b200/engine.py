@@ -60,7 +60,10 @@ def decode_params(opt=None, **over):
 
 
 def make_meta(batch, c, s, img_w, img_h, cam, device=None, out=None):
-    """[B,16] float64 meta rows (see centerpose_b200.h).  Scalars broadcast over the batch."""
+    """[B,16] float64 meta rows (see centerpose_b200.h).  Scalars broadcast over the batch.  s is one scale for the
+    batch, a 1-D array of exactly `batch` per-image scales, or [B,2] (w, h) pairs; a single (w, h) pair, as
+    pre_process returns in the keep_res and fix_short modes, is reduced to its width by the caller
+    (detector.scale_width)."""
     m = np.zeros((batch, _lib.CP_META_DOUBLES), np.float64)
     c = np.broadcast_to(np.asarray(c, np.float64).reshape(-1, 2), (batch, 2))
     m[:, 0:2] = c
@@ -68,7 +71,10 @@ def make_meta(batch, c, s, img_w, img_h, cam, device=None, out=None):
     if s_arr.ndim == 0:
         m[:, 2] = float(s_arr)                 # one scalar for the whole batch
     elif s_arr.ndim == 1:
-        m[:, 2] = np.broadcast_to(s_arr, (batch,))   # per-image scalar
+        if s_arr.shape[0] != batch:
+            raise ValueError("make_meta: a 1-D s holds one scale per image; got %d values for a batch of %d (reduce a "
+                             "(w, h) pair to its width first)" % (s_arr.shape[0], batch))
+        m[:, 2] = s_arr                        # per-image scalar
     else:
         m[:, 2] = s_arr.reshape(batch, -1)[:, 0]     # [B,2] (w,h) pairs: the affine uses the width only
     m[:, 3] = img_w

@@ -82,9 +82,12 @@ def test_non_square_image_affine(cplib):
         compare_records(poses[b, :n_valid[b]], want, L)
 
 
-@pytest.mark.parametrize("oh,ow,K,nobj", [(96, 128, 100, 3), (128, 128, 128, 5), (64, 64, 20, 2), (160, 96, 100, 3)])
+@pytest.mark.parametrize("oh,ow,K,nobj", [(96, 128, 100, 3), (128, 128, 128, 5), (64, 64, 20, 2), (160, 96, 100, 3),
+                                          (160, 160, 100, 3), (208, 152, 100, 4), (184, 328, 128, 5)])
 def test_map_shapes_and_K(oh, ow, K, nobj, cplib):
-    """Ragged shapes: non-square head maps (keep_res / fix_short inputs), K at CP_MAX_K and a small K, vs the oracle."""
+    """Ragged shapes: non-square head maps (keep_res / fix_short inputs), K at CP_MAX_K and a small K, vs the oracle.
+    160 x 160 is the largest map whose top-K runs in shared memory; the 208 x 152 (keep_res 832 x 608) and 184 x 328
+    (keep_res 736 x 1312) maps keep the NMS-ed map in the workspace."""
     B = 2
     w, h = ow * 4, oh * 4
     hb, truths = synth.planted_batch(B, n_obj=nobj, seed=900 + K, out_h=oh, out_w=ow, disagree_px=0.5)
