@@ -93,8 +93,46 @@ int launch_conv3_c16(const IgemmParams& p, cudaStream_t stream);
 bool stem_supported(const IgemmParams& p);
 int launch_stem_conv(const IgemmParams& p, cudaStream_t s);
 
+// The kernel that runs one convolution and its arithmetic (conv_select.cu).
+struct ConvKernel {
+  int family = CP_FAM_IGEMM_FP32;   // cp_op_family; CP_FAM_NONE: no kernel takes the shape under the policy
+  bool x3 = false;                  // tf32 3-term split (fp32-equivalent); otherwise igemm_umma runs bf16 and the TMA
+                                    // kernels a single tf32 pass
+  bool round_out = false;           // conv_tma / dcn_tma round the stored outputs to tf32
+  int BN = 0;                       // N tile (tensor-core families)
+  int cslab = 0;                    // channels per activation slab (conv_tma / dcn_tma)
+  size_t wbytes = 0;                // bytes of the pre-swizzled weight tiles (0: the kernel reads the fp32 matrix)
+};
+// Where the callers of select_conv_kernel differ.
+struct ConvPolicy {
+  bool small_on_cuda_cores;   // NCHW inputs and Cin < 32 stay on CUDA cores
+  bool dcn_tma;               // deformable convs may run on dcn_tma
+  bool round_out;             // single-pass tf32 TMA kernels round their outputs to tf32
+  bool cuda_core_fallback;    // a tensor-core precision no tensor-core kernel takes runs on CUDA cores (else CP_FAM_NONE)
+};
+inline bool known_precision(int32_t precision) {
+  return precision == CP_PREC_FP32 || precision == CP_PREC_TF32X3 || precision == CP_PREC_BF16 || precision == CP_PREC_TF32;
+}
+// tf32 and tf32x3 run the gather kernel in tf32x3, bf16 in bf16
+inline bool gather_x3(int32_t precision) { return precision == CP_PREC_TF32 || precision == CP_PREC_TF32X3; }
+ConvKernel select_conv_kernel(const IgemmParams& p, int32_t precision, const ConvPolicy& pol);
+// CUtensorMaps of a TMA family, encoded on the host and passed by value at launch
+struct alignas(64) TmaMaps {
+  unsigned char map[4][128];
+};
+int conv_encode(const ConvKernel& k, const IgemmParams& p, int Bmax, TmaMaps* maps);
+int conv_pack(const ConvKernel& k, const IgemmParams& p, int ld, void* tiles, cudaStream_t s);
+int conv_launch(const ConvKernel& k, const IgemmParams& p, const TmaMaps* maps, cudaStream_t s, LaunchInfo* info = nullptr);
+// one stand-alone convolution: select, encode, pack into stream-ordered scratch tiles, launch
+int run_conv(IgemmParams& p, int32_t precision, const ConvPolicy& pol, cudaStream_t s);
+
+// Split-K of the persistent TMA kernels: the largest divisor S of `slabs` such that tiles x S CTAs fit the SMs and their
+// partial sums (tile_floats each) fit the workspace; 1 = off.  CP_NO_SPLITK=1 turns it off; it is read at every launch.
+int splitk_factor(long long tiles, int slabs, int num_sms, size_t tile_floats, size_t ws_floats);
+
 // wgmma tensor-core gather path (igemm_umma.cu).  prec: 0 = bf16, 1 = tf32 x 3 (fp32-equivalent)
 bool umma_supported(const IgemmParams& p, int prec);
+int umma_tile_n(int CoutPad, int prec);
 size_t umma_weight_bytes(int Kreal, int CoutPad, int prec);
 int launch_pack_umma_weight(const float* src_k_by_ld, int ld, int Kreal, int Cout, int CoutPad, int prec, void* dst,
                             cudaStream_t s);
@@ -123,28 +161,29 @@ int launch_group_norm_relu(float* x, const float* gamma, const float* beta, int 
 int launch_gru_gates(const float* xi, const float* hh, const float* hprev, float* hout, int B_HW, int C,
                      int first_step, cudaStream_t s);
 
+// tf32x3: 32-channel K blocks per accumulation group (the tensor core chains them in its accumulator before they are
+// added, with round-to-nearest, into fp32 running sums in registers)
+constexpr int kX3GroupBlocks = 1;
+
 // TMA-fed shifted-window wgmma convolution (conv_tma.cu): stride-1 1x1 / 3x3 over NHWC fp32, tf32 operands
 // x3 = 1: 3-term split with two-level accumulation (fp32-equivalent); x3 = 0: single tf32 pass
 bool tma_conv_supported(const IgemmParams& p, int x3);
 size_t tma_weight_bytes(int Cin, int taps, int CoutPad, int x3);
 int tma_tile_n(int CoutPad, int x3);             // N tile of conv_tma for this output width
 int tma_cslab(const IgemmParams& p, int x3);     // channels per activation slab (32 or 16); needs Cin, kh, Win, CoutPad
-int x3_group_blocks();                           // tf32x3: 32-channel K blocks per accumulation group
-int launch_pack_tma_weight(const float* src_k_by_ld, int ld, int Cin, int taps, int Cout, int CoutPad, int round_tf32,
-                           int x3, int cslab, void* dst, cudaStream_t s, int bn_override = 0);
+int launch_pack_tma_weight(const float* src_k_by_ld, int ld, int Cin, int taps, int Cout, int CoutPad, int x3, int cslab,
+                           int bn, void* dst, cudaStream_t s);
 int tma_encode_nhwc_box(const float* base, int C, int W, int H, int B, int strideFloats, int boxC, int boxW, int boxH,
                         int swizzle64, void* map_out /* 128 bytes, 64-byte aligned */);
+int tma_conv_encode(const IgemmParams& p, int Bmax, int cslab, void* maps_out /* 4 x 128 bytes */);
+int launch_conv_tma(const IgemmParams& p, const void* maps, const ConvKernel& k, cudaStream_t stream, LaunchInfo* info);
 
 // TMA-staged deformable convolution (dcn_tma.cu): DCNv2 3x3 stride 1 pad 1 over one NHWC fp32 source, kind::tf32.
 // x3 = 1: 3-term split + promoted accumulation (fp32-equivalent);  x3 = 0: single pass.
 bool dcn_tma_supported(const IgemmParams& p, int x3);
 int dcn_tma_tile_n(int CoutPad, int x3);
 int dcn_tma_encode(const IgemmParams& p, int Bmax, void* map_out /* 128 bytes, 64-byte aligned */);
-int launch_dcn_tma(const IgemmParams& p, const void* map, int x3, int round_out_tf32, cudaStream_t stream,
-                   LaunchInfo* info = nullptr);
-int tma_conv_encode(const IgemmParams& p, int Bmax, int x3, void* maps_out /* 4 x 128 bytes */);
-int launch_conv_tma(const IgemmParams& p, const void* maps, int round_out_tf32, int x3, cudaStream_t stream,
-                    LaunchInfo* info = nullptr);
+int launch_dcn_tma(const IgemmParams& p, const void* map, const ConvKernel& k, cudaStream_t stream, LaunchInfo* info);
 
 inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
 

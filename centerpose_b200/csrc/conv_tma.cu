@@ -17,7 +17,6 @@
 // Reference semantics: nn.Conv2d(k, stride 1, padding k//2) + folded BatchNorm + residual + ReLU
 // (pose_dla_dcn.py:37-62, 153-168, 496-505).
 #include <cuda.h>
-#include <stdlib.h>
 
 #include "common.cuh"
 #include "umma_common.cuh"
@@ -28,21 +27,6 @@ namespace {
 constexpr int TM_BM = 128;
 constexpr int TM_THREADS = 384;       // control warpgroup + two consumer warpgroups
 constexpr int TM_THREADS_X3 = 512;    // + the splitter warpgroup
-constexpr int TM_GROUP_X3 = 1;
-}  // namespace
-
-// tf32x3: 32-channel K blocks (12 MMAs each) chained in the wgmma accumulator before they are added, with
-// round-to-nearest, into fp32 running sums in registers.  CP_X3_GROUP overrides (diagnostics).
-int x3_group_blocks() {
-  int g = TM_GROUP_X3;
-  if (const char* e = getenv("CP_X3_GROUP")) {
-    const int v = atoi(e);
-    if (v >= 1 && v <= 16) g = v;
-  }
-  return g;
-}
-
-namespace {
 
 struct TmaConvParams {
   CUtensorMap amap[4];
@@ -475,64 +459,18 @@ EncodeTiledFn get_encode() {
 
 }  // namespace
 
-// split-K, second half: one thread per (output position, 4 channels) adds the `ksplit` partial sums in split order and
-// applies the epilogue.  Reads are coalesced (row-fastest layout); the whole grid works, not one CTA per tile.
+// split-K, second half (splitk_finish, umma_common.cuh): tile row i -> output position
 __global__ void __launch_bounds__(256) conv_tma_splitk_finish(const __grid_constant__ TmaConvParams p, long long mn_tiles) {
-  griddep_launch_dependents();
-  griddep_wait();
-  const int G = p.BN >> 2;
-  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= mn_tiles * G * p.tile_m) return;
-  const int i = (int)(idx % p.tile_m);
-  const int c4 = (int)((idx / p.tile_m) % G);
-  const long long mn = idx / ((long long)p.tile_m * G);
-  const float4* src = reinterpret_cast<const float4*>(p.part) + ((size_t)mn * p.ksplit * G + c4) * p.tile_m + i;
-  float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
-  for (int q = 0; q < p.ksplit; ++q) {
-    const float4 v = __ldcg(src + (size_t)q * G * p.tile_m);
-    a.x += v.x;
-    a.y += v.y;
-    a.z += v.z;
-    a.w += v.w;
-  }
-  const TileGeo g = decode_tile(p, mn, p.CoutPad / p.BN);
-  int n, oy, ox, mi;
-  const bool valid = tile_position(p, g, i, &n, &oy, &ox, &mi);
-  if (!valid) return;
-  const size_t m = ((size_t)n * p.H + oy) * p.W + ox;
-  const int col0 = g.n_tile * p.BN + c4 * 4;
-  const int col_end = min(p.Cout, (g.n_tile + 1) * p.BN);
-  float v[4] = {a.x, a.y, a.z, a.w};
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const bool in = col0 + j < col_end;
-    if (col0 + j < p.CoutPad) v[j] += __ldg(p.bias + col0 + j);
-    if (p.residual && in && !p.res_after_relu) v[j] += __ldg(p.residual + m * p.resStride + col0 + j);
-    if (p.relu) v[j] = fmaxf(v[j], 0.f);
-    if (p.residual && in && p.res_after_relu) v[j] += __ldg(p.residual + m * p.resStride + col0 + j);
-    if (p.round_tf32) v[j] = tf32_round(v[j]);
-  }
-  if (p.out_nchw) {
-#pragma unroll
-    for (int j = 0; j < 4; ++j)
-      if (col0 + j < col_end) p.out[(((size_t)n * p.Cout + col0 + j) * p.H + oy) * p.W + ox] = v[j];
-  } else {
-    float* o = p.out + m * p.outStride + col0;
-    if (col0 + 3 < col_end) {
-      *reinterpret_cast<float4*>(o) = make_float4(v[0], v[1], v[2], v[3]);
-    } else {
-#pragma unroll
-      for (int j = 0; j < 4; ++j)
-        if (col0 + j < col_end) o[j] = v[j];
-    }
-  }
+  splitk_finish(p, p.tile_m, mn_tiles, [&](long long mn, int i, int* n, int* oy, int* ox) {
+    int m;
+    return tile_position(p, decode_tile(p, mn, p.CoutPad / p.BN), i, n, oy, ox, &m);
+  });
 }
 
 // ---------------------------------------------------------------------------------------------------- host side
 // Channels per activation slab.  32 (128-byte rows) by default; 16 (64-byte rows, SWIZZLE_64B) when Cin is not a
 // multiple of 32, or when the 3-term split (hi + lo slabs) could not be double-buffered with 32-channel slabs.
-static int tma_tile_m(int) { return TM_BM; }
-static int tma_boxh(int Wt, int x3) { return (tma_tile_m(x3) + 1 + 2 * Wt + Wt - 1) / Wt + 1; }
+static int tma_boxh(int Wt) { return (TM_BM + 1 + 2 * Wt + Wt - 1) / Wt + 1; }
 
 // Shared memory for the slab and weight-tile rings: 227 KB less the control block, alignment, slack and the two
 // epilogue staging buffers.
@@ -563,7 +501,7 @@ int tma_cslab(const IgemmParams& p, int x3) {
   if (p.Cin % 32) return 16;
   if (!x3 || p.kh != 3) return 32;
   const int Wt = p.Win + 2;
-  const int boxh = tma_boxh(Wt, x3);
+  const int boxh = tma_boxh(Wt);
   const size_t slab32 = ((size_t)boxh * Wt * 128 + 1023) / 1024 * 1024;
   const int bn = tma_tile_n(p.CoutPad, x3);
   const size_t need = 2 * (2 * slab32) + 2 * ((size_t)bn * 128 * 2);
@@ -586,7 +524,7 @@ bool tma_conv_supported(const IgemmParams& p, int x3) {
   const int bn = tma_tile_n(p.CoutPad, x3);
   if (bn == 0) return false;
   // one single-buffered slab stage (+ its lo copy in x3) and two weight tiles must fit shared memory
-  const size_t slab = p.kh == 3 ? (size_t)tma_boxh(p.Win + 2, x3) * (p.Win + 2) * cs * 4 : (size_t)tma_tile_m(x3) * cs * 4;
+  const size_t slab = p.kh == 3 ? (size_t)tma_boxh(p.Win + 2) * (p.Win + 2) * cs * 4 : (size_t)TM_BM * cs * 4;
   const size_t a_stage = ((slab + 1023) / 1024 * 1024) * (x3 ? 2 : 1);
   const size_t btile = (size_t)bn * cs * 4 * (x3 ? 2 : 1);
   if (a_stage + 2 * btile > TM_BUDGET) return false;
@@ -597,15 +535,14 @@ size_t tma_weight_bytes(int Cin, int taps, int CoutPad, int x3) {
   return (size_t)CoutPad * Cin * taps * 4 * (x3 ? 2 : 1);
 }
 
-int launch_pack_tma_weight(const float* src, int ld, int Cin, int taps, int Cout, int CoutPad, int round_tf32, int x3,
-                           int cs, void* dst, cudaStream_t s, int bn_override) {
-  const int bn = bn_override > 0 ? bn_override : tma_tile_n(CoutPad, x3);
-  if (x3) round_tf32 = 1;
+// The tiles are tf32-rounded: both TMA kernels feed them to the tf32 MMAs as they are.
+int launch_pack_tma_weight(const float* src, int ld, int Cin, int taps, int Cout, int CoutPad, int x3, int cs, int bn,
+                           void* dst, cudaStream_t s) {
   const int nt = CoutPad / bn;
   size_t total = (size_t)nt * (Cin / cs) * taps * bn * (cs / 4);
   int blocks = (int)((total + 255) / 256);
   if (blocks > 132 * 32) blocks = 132 * 32;
-  pack_tma_weight_kernel<<<blocks, 256, 0, s>>>(src, ld, Cin, taps, Cout, bn, nt, round_tf32, x3, cs, (unsigned char*)dst);
+  pack_tma_weight_kernel<<<blocks, 256, 0, s>>>(src, ld, Cin, taps, Cout, bn, nt, 1, x3, cs, (unsigned char*)dst);
   CP_LAUNCH_CHECK("pack_tma_weight_kernel");
   return CP_OK;
 }
@@ -628,13 +565,12 @@ int tma_encode_nhwc_box(const float* base, int C, int W, int H, int B, int strid
 }
 
 // Encodes the tensor maps of the op's sources into `maps_out` (4 x 128 bytes, host memory, reusable across launches).
-int tma_conv_encode(const IgemmParams& p, int Bmax, int x3, void* maps_out) {
+int tma_conv_encode(const IgemmParams& p, int Bmax, int cs, void* maps_out) {
   EncodeTiledFn enc = get_encode();
   if (!enc) return fail(CP_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
   CUtensorMap* maps = reinterpret_cast<CUtensorMap*>(maps_out);
   const int Wt = p.Win + 2;
-  const int boxh = tma_boxh(Wt, x3);
-  const int cs = tma_cslab(p, x3);
+  const int boxh = tma_boxh(Wt);
   const CUtensorMapSwizzle swz = cs == 32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
   for (int s = 0; s < p.nsrc; ++s) {
     CUresult r;
@@ -650,7 +586,7 @@ int tma_conv_encode(const IgemmParams& p, int Bmax, int x3, void* maps_out) {
     } else {
       cuuint64_t dims[2] = {(cuuint64_t)p.srcC[s], (cuuint64_t)Bmax * p.Hin * p.Win};
       cuuint64_t strides[1] = {(cuuint64_t)p.srcStride[s] * 4};
-      cuuint32_t box[2] = {(cuuint32_t)cs, (cuuint32_t)tma_tile_m(x3)};
+      cuuint32_t box[2] = {(cuuint32_t)cs, (cuuint32_t)TM_BM};
       cuuint32_t es[2] = {1, 1};
       r = enc(&maps[s], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)p.src[s], dims, strides, box, es,
               CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -688,9 +624,9 @@ static int launch_conv_tma_kernel(const TmaConvParams& q, const cudaLaunchConfig
   return CP_OK;
 }
 
-int launch_conv_tma(const IgemmParams& p, const void* maps, int round_out_tf32, int x3, cudaStream_t stream,
-                    LaunchInfo* info) {
+int launch_conv_tma(const IgemmParams& p, const void* maps, const ConvKernel& k, cudaStream_t stream, LaunchInfo* info) {
   if (!p.wgt_umma) return fail(CP_ERR_INVALID, "conv_tma: weight tiles missing");
+  const bool x3 = k.x3;
   TmaConvParams q;
   memset(&q, 0, sizeof(q));
   memcpy(q.amap, maps, sizeof(CUtensorMap) * 4);
@@ -702,15 +638,14 @@ int launch_conv_tma(const IgemmParams& p, const void* maps, int round_out_tf32, 
   q.Cin = p.Cin;
   q.Cout = p.Cout;
   q.CoutPad = p.CoutPad;
-  q.BN = tma_tile_n(p.CoutPad, x3);
-  if (q.BN == 0) return fail(CP_ERR_INVALID, "conv_tma: unsupported output width");
+  q.BN = k.BN;
   q.x3 = x3;
-  q.cslab = tma_cslab(p, x3);
-  q.group = x3_group_blocks() * (32 / q.cslab);       // same number of MMAs per accumulation group
+  q.cslab = k.cslab;
+  q.group = kX3GroupBlocks * (32 / q.cslab);       // same number of MMAs per accumulation group
   q.k = p.kh;
   q.Wt = p.Win + 2;
-  q.tile_m = tma_tile_m(x3);
-  q.boxh = tma_boxh(q.Wt, x3);
+  q.tile_m = TM_BM;
+  q.boxh = tma_boxh(q.Wt);
   size_t m_tiles;
   if (q.k == 3) {
     q.tiles_per_image = (p.Hin * q.Wt + q.tile_m - 1) / q.tile_m;
@@ -734,7 +669,7 @@ int launch_conv_tma(const IgemmParams& p, const void* maps, int round_out_tf32, 
   q.out = p.out;
   q.outStride = p.outStride;
   q.out_nchw = p.out_nchw;
-  q.round_tf32 = round_out_tf32;
+  q.round_tf32 = k.round_out;
   q.wtiles = (const unsigned char*)p.wgt_umma;
   if (p.fuse_n > 0) {
     if (p.fuse_hidden % q.BN || p.CoutPad != p.fuse_n * p.fuse_hidden || !p.relu || p.residual || (x3 && q.BN != 128))
@@ -749,27 +684,16 @@ int launch_conv_tma(const IgemmParams& p, const void* maps, int round_out_tf32, 
     }
   }
   q.m_tiles = (long long)m_tiles;
-  q.ksplit = 1;
-  q.sps = q.Cin / q.cslab;
   q.part = p.splitk_ws;
-  q.total_tiles = (long long)m_tiles * (p.CoutPad / q.BN);
+  const long long mn = (long long)m_tiles * (p.CoutPad / q.BN);
+  const int nslab = q.Cin / q.cslab;
   int num_sms = 0;
   if (int rc = device_sm_count(&num_sms)) return rc;
   // split-K (tf32x3, plain epilogue): small feature maps give a persistent kernel fewer tiles than SMs while every tile
   // walks a long serial K loop (level5 at batch 1: 16 tiles x 144 K blocks).  Deal slab-aligned K ranges to more CTAs.
-  const char* ks_off = getenv("CP_NO_SPLITK");        // "1": no split-K anywhere, "conv": not here, "dcn": not in dcn_tma
-  if (x3 && !q.fuse && p.splitk_ws && !(ks_off && (ks_off[0] == '1' || ks_off[0] == 'c'))) {
-    const int nslab = q.Cin / q.cslab;
-    const long long mn = q.total_tiles;
-    int S = 1;
-    for (int cand = 2; cand <= nslab; ++cand)
-      if (nslab % cand == 0 && mn * cand <= num_sms && (size_t)mn * cand * q.tile_m * q.BN <= p.splitk_ws_floats) S = cand;
-    if (S > 1) {
-      q.ksplit = S;
-      q.sps = nslab / S;
-      q.total_tiles = mn * S;
-    }
-  }
+  q.ksplit = x3 && !q.fuse ? splitk_factor(mn, nslab, num_sms, (size_t)q.tile_m * q.BN, p.splitk_ws_floats) : 1;
+  q.sps = nslab / q.ksplit;
+  q.total_tiles = mn * q.ksplit;
   if (q.total_tiles >= (1ll << 31)) return fail(CP_ERR_INVALID, "conv_tma: too many tiles");
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3((unsigned)(q.total_tiles < num_sms ? q.total_tiles : num_sms));
@@ -785,7 +709,6 @@ int launch_conv_tma(const IgemmParams& p, const void* maps, int round_out_tf32, 
     info->grid = cfg.gridDim.x;
   }
   if (q.ksplit > 1) {
-    const long long mn = q.total_tiles / q.ksplit;
     const long long threads = mn * (q.BN / 4) * q.tile_m;
     CP_CUDA_CHECK(launch_kernel(conv_tma_splitk_finish, dim3((unsigned)((threads + 255) / 256)), dim3(256), 0, stream, q, mn));
     CP_LAUNCH_CHECK("conv_tma_splitk_finish");

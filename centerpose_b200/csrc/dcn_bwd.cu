@@ -5,7 +5,7 @@
 //
 // Here the whole batch is one pass over NHWC buffers and the column matrix is touched exactly twice:
 //   1. gcol[m][tap * Cp + c] = sum_o W[o][c][tap] * gout[m][o]      -- a 1x1 convolution Co -> 9 Cp over the output
-//      gradient, run by the forward convolution kernels (cp::run_igemm_dispatch: FFMA or wgmma, like cp_conv2d)
+//      gradient, run by the forward convolution kernels (cp::run_conv: FFMA or wgmma, like cp_conv2d)
 //   2. dcn_bwd_sample_kernel, one warp per (position, tap), lanes over channels: reads its gcol slice, re-samples the
 //      four bilinear corners of the input, accumulates grad_mask / grad_offset (warp reduction, written NCHW), scatters
 //      grad_input with vector atomics (NHWC) and OVERWRITES the gcol slice with the forward column value
@@ -213,12 +213,13 @@ __global__ void dcn_bwd_wgrad_finish(const float* __restrict__ part, int S, int 
 
 }  // namespace
 
-int run_igemm_dispatch(IgemmParams& p, int prec, int Kreal, cudaStream_t s);      // ext_ops.cu
+// shapes the tensor-core kernels do not take (a few channels) run on the FFMA kernel: same result class, fp32
+constexpr ConvPolicy kColumnGemm{false, true, false, true};
 
 int dcn_v2_backward_impl(const float* input, const float* weight, const float* offset, const float* mask,
                          const float* grad_output, float* grad_input, float* grad_offset, float* grad_mask,
-                         float* grad_weight, float* grad_bias, int B, int C, int H, int W, int Co, int prec,
-                         cudaStream_t s) {
+                         float* grad_weight, float* grad_bias, int B, int C, int H, int W, int Co,
+                         int32_t precision, cudaStream_t s) {
   const int Cp = round_up(C, 16), CoP = round_up(Co, 16);
   const int N = 9 * Cp, NPad = round_up(N, 64);
   const long long M = (long long)B * H * W;
@@ -283,12 +284,7 @@ int dcn_v2_backward_impl(const float* input, const float* weight, const float* o
     p.out = gcol;
     p.outStride = N;
     p.mode = IGEMM_NHWC_VEC;
-    // shapes the tensor-core kernels do not take (a few channels) run on the FFMA kernel: same result class, fp32
-    if (prec >= 0) {
-      const bool tma_ok = (prec == 1 || prec == 2) && tma_conv_supported(p, prec == 1);
-      if (!tma_ok && !umma_supported(p, prec == 2 ? 1 : prec)) prec = -1;
-    }
-    if ((rc = run_igemm_dispatch(p, prec, CoP, s))) break;
+    if ((rc = run_conv(p, precision, kColumnGemm, s))) break;
     // 2. sampling pass
     SampleArgs a;
     a.x = x;

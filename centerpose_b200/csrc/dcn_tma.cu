@@ -24,7 +24,6 @@
 //                   (hi, lo) tf32 split -> A tile in the SWIZZLE_64B K-major layout, AH A stages
 //   warps 12-15   : consumer of tile rows [64, 128)
 #include <cuda.h>
-#include <stdlib.h>
 
 #include "common.cuh"
 #include "umma_common.cuh"
@@ -450,58 +449,16 @@ __global__ void __launch_bounds__(DT_THREADS, 1) dcn_tma_kernel(const __grid_con
   }
 }
 
-// split-K, second half: one thread per (position, 4 channels) adds the partial sums in split order + epilogue
+// split-K, second half (splitk_finish, umma_common.cuh): tile row i -> position i of the 8 x 16 patch
 __global__ void __launch_bounds__(256) dcn_tma_splitk_finish(const __grid_constant__ DcnTmaParams p, long long mn_tiles) {
-  griddep_launch_dependents();
-  griddep_wait();
-  const int G = p.BN >> 2;
-  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= mn_tiles * G * 128) return;
-  const int i = (int)(idx & 127);
-  const int c4 = (int)((idx >> 7) % G);
-  const long long mn = idx / (128ll * G);
-  const float4* src = reinterpret_cast<const float4*>(p.part) + ((size_t)mn * p.ksplit * G + c4) * 128 + i;
-  float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
-  for (int q = 0; q < p.ksplit; ++q) {
-    const float4 v = __ldcg(src + (size_t)q * G * 128);
-    a.x += v.x;
-    a.y += v.y;
-    a.z += v.z;
-    a.w += v.w;
-  }
-  const int n_tiles = p.CoutPad / p.BN;
-  const int n_tile = (int)(mn % n_tiles);
-  const long long m_tile = mn / n_tiles;
-  const int n = (int)(m_tile / p.tiles_per_image);
-  const int pt = (int)(m_tile - (long long)n * p.tiles_per_image);
-  const int oy = (pt / p.tiles_x) * DT_PH + (i >> 4), ox = (pt % p.tiles_x) * DT_PW + (i & 15);
-  const size_t m = ((size_t)n * p.H + oy) * p.W + ox;
-  const int col0 = n_tile * p.BN + c4 * 4;
-  const int col_end = min(p.Cout, (n_tile + 1) * p.BN);
-  float v[4] = {a.x, a.y, a.z, a.w};
-#pragma unroll
-  for (int j = 0; j < 4; ++j) {
-    const bool in = col0 + j < col_end;
-    if (col0 + j < p.CoutPad) v[j] += __ldg(p.bias + col0 + j);
-    if (p.residual && in && !p.res_after_relu) v[j] += __ldg(p.residual + m * p.resStride + col0 + j);
-    if (p.relu) v[j] = fmaxf(v[j], 0.f);
-    if (p.residual && in && p.res_after_relu) v[j] += __ldg(p.residual + m * p.resStride + col0 + j);
-    if (p.round_tf32) v[j] = tf32_round(v[j]);
-  }
-  if (p.out_nchw) {
-#pragma unroll
-    for (int j = 0; j < 4; ++j)
-      if (col0 + j < col_end) p.out[(((size_t)n * p.Cout + col0 + j) * p.H + oy) * p.W + ox] = v[j];
-  } else {
-    float* o = p.out + m * p.outStride + col0;
-    if (col0 + 3 < col_end) {
-      *reinterpret_cast<float4*>(o) = make_float4(v[0], v[1], v[2], v[3]);
-    } else {
-#pragma unroll
-      for (int j = 0; j < 4; ++j)
-        if (col0 + j < col_end) o[j] = v[j];
-    }
-  }
+  splitk_finish(p, DT_BM, mn_tiles, [&](long long mn, int i, int* n, int* oy, int* ox) {
+    const long long m_tile = mn / (p.CoutPad / p.BN);
+    *n = (int)(m_tile / p.tiles_per_image);
+    const int pt = (int)(m_tile - (long long)*n * p.tiles_per_image);
+    *oy = (pt / p.tiles_x) * DT_PH + (i >> 4);
+    *ox = (pt % p.tiles_x) * DT_PW + (i & 15);
+    return true;
+  });
 }
 
 }  // namespace
@@ -522,8 +479,8 @@ int dcn_tma_encode(const IgemmParams& p, int Bmax, void* map_out) {
   return tma_encode_nhwc_box(p.src[0], p.srcC[0], p.Win, p.Hin, Bmax, p.srcStride[0], DT_CS, DT_SW, DT_SH, 1, map_out);
 }
 
-int launch_dcn_tma(const IgemmParams& p, const void* map, int x3, int round_out_tf32, cudaStream_t stream,
-                   LaunchInfo* info) {
+int launch_dcn_tma(const IgemmParams& p, const void* map, const ConvKernel& k, cudaStream_t stream, LaunchInfo* info) {
+  const bool x3 = k.x3;
   if (!p.wgt_umma) return fail(CP_ERR_INVALID, "dcn_tma: weight tiles missing");
   if (!dcn_tma_supported(p, x3)) return fail(CP_ERR_INVALID, "dcn_tma: unsupported shape");
   DcnTmaParams q;
@@ -540,12 +497,12 @@ int launch_dcn_tma(const IgemmParams& p, const void* map, int x3, int round_out_
   q.Cin = p.Cin;
   q.Cout = p.Cout;
   q.CoutPad = p.CoutPad;
-  q.BN = dcn_tma_tile_n(p.CoutPad, x3);
+  q.BN = k.BN;
   q.tiles_x = p.Win / DT_PW;
   q.tiles_per_image = q.tiles_x * (p.Hin / DT_PH);
-  q.total_tiles = (long long)q.tiles_per_image * p.B * (p.CoutPad / q.BN);
+  const long long mn = (long long)q.tiles_per_image * p.B * (p.CoutPad / q.BN);
   const uint32_t a_stage = x3 ? 16384u : 8192u;
-  q.group = x3_group_blocks() * 2;      // 16-channel K blocks: same MMA count per group as conv_tma.cu
+  q.group = kX3GroupBlocks * 2;      // 16-channel K blocks: same MMA count per group as conv_tma.cu
   const uint32_t btile = (uint32_t)q.BN * 64u * (x3 ? 2u : 1u);
   const size_t budget = 226 * 1024;
   // two A stages where >= 3 weight stages still fit, else one
@@ -567,7 +524,7 @@ int launch_dcn_tma(const IgemmParams& p, const void* map, int x3, int round_out_
   q.out = p.out;
   q.outStride = p.outStride;
   q.out_nchw = p.out_nchw;
-  q.round_tf32 = round_out_tf32;
+  q.round_tf32 = k.round_out;
   q.wtiles = (const unsigned char*)p.wgt_umma;
   const size_t smem = fixed + (size_t)q.SB * btile;
   void (*kern)(DcnTmaParams) = nullptr;
@@ -587,22 +544,11 @@ int launch_dcn_tma(const IgemmParams& p, const void* map, int x3, int round_out_
   int num_sms = 0;
   if (int rc = device_sm_count(&num_sms)) return rc;
   // split-K: at batch 1 the 512 -> 256 DCN at 16 x 16 is 4 tiles of 288 K blocks; deal slab ranges to idle SMs
-  q.ksplit = 1;
-  q.sps = p.Cin / DT_CS;
+  const int nslab = p.Cin / DT_CS;
   q.part = p.splitk_ws;
-  const long long mn = q.total_tiles;
-  const char* ks_off = getenv("CP_NO_SPLITK");        // "1": no split-K anywhere, "dcn": not here, "conv": not in conv_tma
-  if (p.splitk_ws && !(ks_off && (ks_off[0] == '1' || ks_off[0] == 'd'))) {
-    const int nslab = p.Cin / DT_CS;
-    int S = 1;
-    for (int cand = 2; cand <= nslab; ++cand)
-      if (nslab % cand == 0 && mn * cand <= num_sms && (size_t)mn * cand * 128 * q.BN <= p.splitk_ws_floats) S = cand;
-    if (S > 1) {
-      q.ksplit = S;
-      q.sps = nslab / S;
-      q.total_tiles = mn * S;
-    }
-  }
+  q.ksplit = splitk_factor(mn, nslab, num_sms, (size_t)DT_BM * q.BN, p.splitk_ws_floats);
+  q.sps = nslab / q.ksplit;
+  q.total_tiles = mn * q.ksplit;
   const unsigned grid = (unsigned)(q.total_tiles < num_sms ? q.total_tiles : num_sms);
   CP_CUDA_CHECK(launch_kernel(kern, dim3(grid), dim3(DT_THREADS), smem, stream, q));
   CP_LAUNCH_CHECK("dcn_tma_kernel");
@@ -612,7 +558,7 @@ int launch_dcn_tma(const IgemmParams& p, const void* map, int x3, int round_out_
     info->grid = grid;
   }
   if (q.ksplit > 1) {
-    const long long threads = mn * (q.BN / 4) * 128;
+    const long long threads = mn * (q.BN / 4) * DT_BM;
     CP_CUDA_CHECK(launch_kernel(dcn_tma_splitk_finish, dim3((unsigned)((threads + 255) / 256)), dim3(256), 0, stream, q, mn));
     CP_LAUNCH_CHECK("dcn_tma_splitk_finish");
   }

@@ -5,8 +5,6 @@
 //   cp_preprocess     -- batched uint8 HWC frames -> normalised fp32 NCHW network input
 //                        (reference: detectors/base_detector.py:91-148, fix_res branch); cp_preprocess_ragged does
 //                        the same for frames of different sizes in one launch.
-#include <stdlib.h>
-
 #include <vector>
 
 #include "common.cuh"
@@ -150,76 +148,15 @@ int preprocess_blocks(size_t total) {
 
 int dcn_v2_backward_impl(const float* input, const float* weight, const float* offset, const float* mask,
                          const float* grad_output, float* grad_input, float* grad_offset, float* grad_mask,
-                         float* grad_weight, float* grad_bias, int B, int C, int H, int W, int Co, int prec,
-                         cudaStream_t s);      // dcn_bwd.cu
+                         float* grad_weight, float* grad_bias, int B, int C, int H, int W, int Co,
+                         int32_t precision, cudaStream_t s);      // dcn_bwd.cu
 }  // namespace cp
 
 using namespace cp;
 
-extern "C" {
+// cp_conv2d / cp_dcn_v2_forward_ex store unrounded outputs and fail when a tensor-core precision has no kernel for the shape
+constexpr ConvPolicy kStandAlone{false, true, false, false};
 
-static int prec_code(int32_t precision, int* prec) {
-  if (precision == CP_PREC_FP32) *prec = -1;
-  else if (precision == CP_PREC_BF16) *prec = 0;
-  else if (precision == CP_PREC_TF32X3) *prec = 1;
-  else if (precision == CP_PREC_TF32) *prec = 2;
-  else return fail(CP_ERR_INVALID, "unknown precision");
-  return CP_OK;
-}
-
-// run one implicit-GEMM launch with the kernel family selected by `prec` (weights already packed as fp32 [K][CoutPad])
-static int run_igemm(IgemmParams& p, int prec, int Kreal, cudaStream_t s) {
-  if (prec < 0) return conv3_c16_supported(p) ? launch_conv3_c16(p, s) : launch_igemm_fp32(p, s);
-  if (prec == 2 || prec == 1) {
-    const int x3 = prec == 1;
-    const char* force_gather = getenv("CP_FORCE_GATHER");
-    if (p.mode == IGEMM_DCN && dcn_tma_supported(p, x3) && !(force_gather && atoi(force_gather))) {
-      void* tiles = nullptr;
-      CP_CUDA_CHECK(cudaMallocAsync(&tiles, tma_weight_bytes(p.Cin, 9, p.CoutPad, x3), s));
-      alignas(64) unsigned char map[128];
-      int rc = dcn_tma_encode(p, p.B, map);
-      if (!rc) rc = launch_pack_tma_weight(p.wgt, p.CoutPad, p.Cin, 9, p.Cout, p.CoutPad, 1, x3, 16, tiles, s,
-                                           dcn_tma_tile_n(p.CoutPad, x3));
-      if (!rc) {
-        p.wgt_umma = tiles;
-        rc = launch_dcn_tma(p, map, x3, 0, s);
-      }
-      cudaFreeAsync(tiles, s);
-      return rc;
-    }
-    if (!tma_conv_supported(p, x3) || (force_gather && atoi(force_gather))) {
-      prec = 1;     // deformable / strided ops: 3-term split gather kernel
-    } else {
-      void* tiles = nullptr;
-      const int taps = p.kh * p.kw;
-      CP_CUDA_CHECK(cudaMallocAsync(&tiles, tma_weight_bytes(p.Cin, taps, p.CoutPad, x3), s));
-      alignas(64) unsigned char maps[512];
-      int rc = tma_conv_encode(p, p.B, x3, maps);
-      if (!rc) rc = launch_pack_tma_weight(p.wgt, p.CoutPad, p.Cin, taps, p.Cout, p.CoutPad, 1, x3, tma_cslab(p, x3), tiles, s);
-      if (!rc) {
-        p.wgt_umma = tiles;
-        rc = launch_conv_tma(p, maps, 0, x3, s);
-      }
-      cudaFreeAsync(tiles, s);
-      return rc;
-    }
-  }
-  if (!umma_supported(p, prec)) return fail(CP_ERR_INVALID, "shape not supported by the wgmma kernel");
-  void* tiles = nullptr;
-  CP_CUDA_CHECK(cudaMallocAsync(&tiles, umma_weight_bytes(Kreal, p.CoutPad, prec), s));
-  int rc = launch_pack_umma_weight(p.wgt, p.CoutPad, Kreal, p.Cout, p.CoutPad, prec, tiles, s);
-  if (!rc) {
-    p.wgt_umma = tiles;
-    rc = launch_igemm_umma(p, prec, s);
-  }
-  cudaFreeAsync(tiles, s);
-  return rc;
-}
-
-}  // extern "C"
-namespace cp {
-int run_igemm_dispatch(IgemmParams& p, int prec, int Kreal, cudaStream_t s) { return run_igemm(p, prec, Kreal, s); }
-}  // namespace cp
 extern "C" {
 
 int cp_conv2d(const float* x, const float* weight, const float* bias, const float* residual, float* out, int32_t B,
@@ -229,9 +166,8 @@ int cp_conv2d(const float* x, const float* weight, const float* bias, const floa
   if (B <= 0 || H <= 0 || W <= 0 || Cin <= 0 || Cout <= 0 || k <= 0 || stride <= 0 || pad < 0)
     return fail(CP_ERR_INVALID, "cp_conv2d: bad shape");
   if (Cin % 16 || Cout % 4) return fail(CP_ERR_INVALID, "cp_conv2d: Cin must be a multiple of 16 and Cout of 4");
-  int prec;
-  int rc = prec_code(precision, &prec);
-  if (rc) return rc;
+  if (!known_precision(precision)) return fail(CP_ERR_INVALID, "unknown precision");
+  int rc;
   cudaStream_t s = (cudaStream_t)stream_;
   const int CoPad = round_up(Cout, Cout > 32 ? 64 : (Cout > 16 ? 32 : 16));
   const int K = k * k * Cin;
@@ -267,7 +203,7 @@ int cp_conv2d(const float* x, const float* weight, const float* bias, const floa
     p.out = out;
     p.outStride = Cout;
     p.mode = IGEMM_NHWC_VEC;
-    rc = run_igemm(p, prec, K, s);
+    rc = run_conv(p, precision, kStandAlone, s);
   } while (0);
   cudaFreeAsync(scratch, s);
   return rc;
@@ -277,17 +213,13 @@ int cp_dcn_v2_backward(const float* input, const float* weight, const float* off
                        const float* grad_output, float* grad_input, float* grad_offset, float* grad_mask,
                        float* grad_weight, float* grad_bias, int32_t B, int32_t C, int32_t H, int32_t W, int32_t Co,
                        int32_t precision, void* stream_) {
-  int prec;
-  {
-    int rcp = prec_code(precision, &prec);
-    if (rcp) return rcp;
-  }
+  if (!known_precision(precision)) return fail(CP_ERR_INVALID, "unknown precision");
   if (!input || !weight || !offset || !mask || !grad_output || !grad_input || !grad_offset || !grad_mask || !grad_weight ||
       !grad_bias)
     return fail(CP_ERR_INVALID, "cp_dcn_v2_backward: null argument");
   if (B <= 0 || C <= 0 || H <= 0 || W <= 0 || Co <= 0) return fail(CP_ERR_INVALID, "cp_dcn_v2_backward: bad shape");
   return dcn_v2_backward_impl(input, weight, offset, mask, grad_output, grad_input, grad_offset, grad_mask, grad_weight,
-                              grad_bias, B, C, H, W, Co, prec, (cudaStream_t)stream_);
+                              grad_bias, B, C, H, W, Co, precision, (cudaStream_t)stream_);
 }
 
 int cp_dcn_v2_forward(const float* input, const float* weight, const float* bias, const float* offset,
@@ -299,11 +231,7 @@ int cp_dcn_v2_forward(const float* input, const float* weight, const float* bias
 int cp_dcn_v2_forward_ex(const float* input, const float* weight, const float* bias, const float* offset,
                          const float* mask, float* output, int32_t B, int32_t C, int32_t H, int32_t W, int32_t Co,
                          int32_t precision, void* stream_) {
-  int prec;
-  {
-    int rcp = prec_code(precision, &prec);
-    if (rcp) return rcp;
-  }
+  if (!known_precision(precision)) return fail(CP_ERR_INVALID, "unknown precision");
   if (!input || !weight || !bias || !offset || !mask || !output)
     return fail(CP_ERR_INVALID, "cp_dcn_v2_forward: null argument");
   if (B <= 0 || C <= 0 || H <= 0 || W <= 0 || Co <= 0) return fail(CP_ERR_INVALID, "cp_dcn_v2_forward: bad shape");
@@ -352,7 +280,7 @@ int cp_dcn_v2_forward_ex(const float* input, const float* weight, const float* b
     p.omStride = 32;
     p.mask_is_logit = 0;
     p.mode = IGEMM_DCN;
-    rc = run_igemm(p, prec, 9 * Cp, s);
+    rc = run_conv(p, precision, kStandAlone, s);
   } while (0);
   cudaFreeAsync(scratch, s);
   return rc;

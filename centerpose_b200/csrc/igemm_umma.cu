@@ -428,7 +428,7 @@ int launch_igemm_umma(const IgemmParams& p, int prec, cudaStream_t stream, Launc
   if (stages < 2) return fail(CP_ERR_INVALID, "igemm_umma: tile does not fit shared memory");
   const size_t smem = fixed + stages * stage_bytes;
   // tf32x3: K blocks (12 MMAs each) chained in the accumulator before they are added into the fp32 sums
-  const int nacc = prec == 1 ? x3_group_blocks() : 1;
+  const int nacc = prec == 1 ? kX3GroupBlocks : 1;
   if (prec == 0) {
     switch (bn) {
       case 16: return launch_igemm_umma_bn<0, 16>(p, stages, smem, nacc, stream, info);

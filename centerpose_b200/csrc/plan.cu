@@ -56,15 +56,12 @@ struct Op {
   int kh = 1, kw = 1, stride = 1, pad = 0, Cin = 0, Cout = 0, CoutPad = 0, Kpad = 0;
   size_t w_off = 0, b_off = 0;
   int w_ld = 0;            // leading dimension of the fp32 packed weight matrix
-  bool use_umma = false;   // run on the wgmma gather kernel
-  bool use_tma = false;    // run on the TMA-fed wgmma kernel (conv_tma.cu)
-  bool use_dcn_tma = false;   // deformable conv on the TMA-staged wgmma kernel (dcn_tma.cu)
+  ConvKernel kernel;       // chosen once the arena exists (choose_kernels)
+  size_t tile_off = 0;     // bytes into the plan's tensor-core weight-tile buffer
+  TmaMaps maps;            // conv_tma / dcn_tma: encoded once the arena exists
   std::vector<int> head_children;   // merged heads 3x3 conv: indices of the per-head 1x1 ops that read its slices
   bool fuse_heads = false;          // ... which run inside its epilogue (conv_tma.cu), never touching HBM
   bool fused_away = false;          // this 1x1 op is computed by its parent's epilogue
-  int tma_cslab = 32;
-  std::vector<unsigned char> tma_maps;   // 4 CUtensorMap, encoded once the arena exists
-  size_t umma_off = 0;     // bytes into the plan's tensor-core weight-tile buffer
   Act om;
   // up-sample
   int f = 0;
@@ -118,11 +115,7 @@ struct cp_plan {
   void* decode_ws = nullptr;
   size_t decode_ws_bytes = 0;
   double* gn_stats = nullptr;
-  int prec = -1;                 // -1 fp32 CUDA cores, 0 bf16 wgmma, 1 tf32x3 wgmma, 2 tf32 (TMA) + tf32x3 elsewhere
-  int min_tc_cin = 32;           // ops with fewer input channels stay on the CUDA-core kernels (CP_MIN_TC_CIN overrides)
-  bool no_fuse_heads = false;    // CP_NO_FUSE_HEADS=1: keep the per-head 1x1 convs as separate launches
   bool no_dcn_tma = false;       // CP_NO_DCN_TMA=1: deformable convs on the global-gather kernel (A/B measurements)
-  bool no_umma = false;          // CP_NO_UMMA=1: ops the TMA kernels do not take stay on the fp32 CUDA-core kernel (diagnostics)
   unsigned char* umma_wts = nullptr;
   size_t umma_bytes = 0;
   float* splitk_ws = nullptr;      // conv_tma / dcn_tma split-K partial sums (kSplitkWsFloats)
@@ -552,68 +545,104 @@ int build_graph(cp_plan* P) {
   }
   P->act_floats = b.act_cur;
   P->w_floats = b.w_cur;
-  // tensor-core eligibility + weight-tile storage
-  P->umma_bytes = 0;
-  if (P->prec >= 0) {
-    for (auto& op : P->ops) {
-      if (op.type != OP_IGEMM) continue;
-      IgemmParams q{};
-      q.mode = op.mode;
-      q.nsrc = op.nsrc;
-      q.Cin = op.Cin;
-      q.CoutPad = op.CoutPad;
-      for (int i = 0; i < op.nsrc; ++i) {
-        q.srcC[i] = op.src[i].C;
-        q.srcStride[i] = op.src[i].stride;
-      }
-      q.kh = op.kh;
-      q.kw = op.kw;
-      q.stride = op.stride;
-      q.pad = op.pad;
-      q.Win = op.src[0].W;
-      const int gather_prec = P->prec == 2 ? 1 : P->prec;
-      if (op.src[0].ext >= 0) continue;
-      // 16-channel layers (level0 / level1): 133 K single-tile CTAs of almost no MMA work are dominated by the fixed
-      // per-CTA cost of a tensor-core kernel -> keep them on CUDA cores
-      if (op.Cin < P->min_tc_cin) continue;
-      q.Hin = op.src[0].H;
-      if ((P->prec == 2 || P->prec == 1) && !P->no_dcn_tma && dcn_tma_supported(q, P->prec == 1)) {
-        op.use_dcn_tma = true;
-        op.umma_off = P->umma_bytes;
-        P->umma_bytes += (tma_weight_bytes(op.Cin, 9, op.CoutPad, P->prec == 1) + 1023) / 1024 * 1024;
-      } else if ((P->prec == 2 || P->prec == 1) && tma_conv_supported(q, P->prec == 1)) {
-        op.use_tma = true;
-        op.umma_off = P->umma_bytes;
-        P->umma_bytes += (tma_weight_bytes(op.Cin, op.kh * op.kw, op.CoutPad, P->prec == 1) + 1023) / 1024 * 1024;
-      } else if (!P->no_umma && umma_supported(q, gather_prec)) {
-        op.use_umma = true;
-        op.umma_off = P->umma_bytes;
-        P->umma_bytes += (umma_weight_bytes(op.kh * op.kw * op.Cin, op.CoutPad, gather_prec) + 1023) / 1024 * 1024;
-      }
+  return CP_OK;
+}
+
+// Kernel parameters of conv op `op` at batch `batch`.  ext[] may hold nulls (family queries); run_op rejects them.
+void igemm_params(const cp_plan* P, const Op& op, int batch, const float* const ext[4], float* const* head_out,
+                  IgemmParams* pp) {
+  IgemmParams& p = *pp;
+  p = IgemmParams{};
+  p.nsrc = op.nsrc;
+  for (int i = 0; i < op.nsrc; ++i) {
+    const Act& a = op.src[i];
+    p.src[i] = a.ext >= 0 ? ext[a.ext] : P->act + a.off;
+    p.srcC[i] = a.C;
+    p.srcStride[i] = a.stride;
+  }
+  p.B = batch;
+  p.Hin = op.src[0].H;
+  p.Win = op.src[0].W;
+  p.Cin = op.Cin;
+  p.kh = op.kh;
+  p.kw = op.kw;
+  p.stride = op.stride;
+  p.pad = op.pad;
+  p.Hout = (p.Hin + 2 * op.pad - op.kh) / op.stride + 1;
+  p.Wout = (p.Win + 2 * op.pad - op.kw) / op.stride + 1;
+  p.Cout = op.Cout;
+  p.CoutPad = op.CoutPad;
+  p.Kpad = op.Kpad;
+  p.wgt = P->wts + op.w_off;
+  p.bias = P->wts + op.b_off;
+  p.residual = op.has_res ? P->act + op.res.off : nullptr;
+  p.resStride = op.res.stride;
+  p.relu = op.relu;
+  p.res_after_relu = op.res_after_relu;
+  if (op.out_head >= 0) {
+    p.out = head_out ? head_out[op.out_head] : nullptr;
+    p.out_nchw = 1;
+    p.outStride = 0;
+  } else {
+    p.out = P->act + op.out.off;
+    p.outStride = op.out.stride;
+  }
+  if (op.mode == IGEMM_DCN) {
+    p.offmask = P->act + op.om.off;
+    p.omStride = op.om.stride;
+    p.mask_is_logit = 1;
+  }
+  p.mode = op.mode;
+  if (op.fuse_heads) {
+    p.fuse_n = (int)op.head_children.size();
+    p.fuse_hidden = P->cfg.head_conv;
+    for (int i = 0; i < p.fuse_n; ++i) {
+      const Op& ch = P->ops[op.head_children[i]];
+      p.fuse_w[i] = P->wts + ch.w_off;
+      p.fuse_b[i] = P->wts + ch.b_off;
+      p.fuse_out[i] = head_out ? head_out[ch.out_head] : nullptr;
+      p.fuse_cout[i] = ch.Cout;
     }
+  }
+}
+
+// The kernel of every conv op (needs the arena: the choice reads the op's residual), its weight-tile offset, its tensor
+// maps, and which per-head 1x1 convs run inside the epilogue of their merged heads conv.
+int choose_kernels(cp_plan* P) {
+  // 16-channel layers (level0 / level1): 133 K single-tile CTAs of almost no MMA work are dominated by the fixed per-CTA
+  // cost of a tensor-core kernel -> keep them, and the NCHW stems, on CUDA cores
+  const ConvPolicy pol{true, !P->no_dcn_tma, true, true};
+  const float* const no_ext[4] = {nullptr, nullptr, nullptr, nullptr};
+  P->umma_bytes = 0;
+  for (auto& op : P->ops) {
+    if (op.type != OP_IGEMM) continue;
+    IgemmParams p;
+    igemm_params(P, op, P->B, no_ext, nullptr, &p);
+    op.kernel = select_conv_kernel(p, P->cfg.precision, pol);
+    op.tile_off = P->umma_bytes;
+    P->umma_bytes += (op.kernel.wbytes + 1023) / 1024 * 1024;
+    if (int rc = conv_encode(op.kernel, p, P->B, &op.maps)) return rc;
   }
   // The per-head 1x1 convs move into the epilogue of the merged heads conv when that one runs on conv_tma: hidden =
   // relu(conv3x3) never reaches HBM (3.7 GB of writes + 3.7 GB of reads and seven launches at batch 32).  In both
   // tf32 modes the two epilogue threads that own an output row multiply its hidden channels with the head's [256][16]
   // 1x1 weights (read through __ldg) and combine their halves with one shuffle (conv_tma.cu).
-  if (P->prec == 2 || P->prec == 1) {
-    for (auto& op : P->ops) {
-      if (op.head_children.empty() || !op.use_tma || P->no_fuse_heads) continue;
-      const int bn = tma_tile_n(op.CoutPad, P->prec == 1);
-      bool ok = op.relu && !op.has_res && (c.head_conv % bn == 0) && (int)op.head_children.size() <= 16 &&
-                op.CoutPad == (int)op.head_children.size() * c.head_conv && (P->prec != 1 || bn == 128);
-      for (int ci : op.head_children) {
-        const Op& ch = P->ops[ci];
-        ok = ok && ch.CoutPad == 16 && ch.w_ld == 16 && ch.Cin == c.head_conv && ch.out_head >= 0 && !ch.relu && !ch.has_res;
-      }
-      if (!ok) continue;
-      op.fuse_heads = true;
-      for (int ci : op.head_children) P->ops[ci].fused_away = true;
+  const int head_conv = P->cfg.head_conv;
+  for (auto& op : P->ops) {
+    if (op.head_children.empty() || op.kernel.family != CP_FAM_CONV_TMA) continue;
+    const int bn = op.kernel.BN;
+    bool ok = op.relu && !op.has_res && (head_conv % bn == 0) && (int)op.head_children.size() <= 16 &&
+              op.CoutPad == (int)op.head_children.size() * head_conv && (!op.kernel.x3 || bn == 128);
+    for (int ci : op.head_children) {
+      const Op& ch = P->ops[ci];
+      ok = ok && ch.CoutPad == 16 && ch.w_ld == 16 && ch.Cin == head_conv && ch.out_head >= 0 && !ch.relu && !ch.has_res;
     }
+    if (!ok) continue;
+    op.fuse_heads = true;
+    for (int ci : op.head_children) P->ops[ci].fused_away = true;
   }
   return CP_OK;
 }
-
 
 }  // namespace
 }  // namespace cp
@@ -628,8 +657,7 @@ int cp_plan_create(const cp_config* cfg, cp_plan** out) {
   if (!cfg || !out) return fail(CP_ERR_INVALID, "cp_plan_create: null argument");
   if (cfg->arch != CP_ARCH_DLA34 && cfg->arch != CP_ARCH_DLAV1_34)
     return fail(CP_ERR_INVALID, "cp_plan_create: unknown arch");
-  if (cfg->precision != CP_PREC_FP32 && cfg->precision != CP_PREC_TF32X3 && cfg->precision != CP_PREC_BF16 &&
-      cfg->precision != CP_PREC_TF32)
+  if (!known_precision(cfg->precision))
     return fail(CP_ERR_INVALID, "cp_plan_create: unknown precision");
   if (cfg->height % 32 || cfg->width % 32 || cfg->height <= 0 || cfg->width <= 0)
     return fail(CP_ERR_INVALID, "cp_plan_create: height/width must be positive multiples of 32");
@@ -650,11 +678,7 @@ int cp_plan_create(const cp_config* cfg, cp_plan** out) {
   P->B = cfg->max_batch;
   P->H = cfg->height;
   P->W = cfg->width;
-  P->prec = cfg->precision == CP_PREC_BF16 ? 0 : (cfg->precision == CP_PREC_TF32X3 ? 1 : (cfg->precision == CP_PREC_TF32 ? 2 : -1));
-  if (const char* e = getenv("CP_MIN_TC_CIN")) P->min_tc_cin = atoi(e);
-  if (const char* e = getenv("CP_NO_FUSE_HEADS")) P->no_fuse_heads = atoi(e) != 0;
   if (const char* e = getenv("CP_NO_DCN_TMA")) P->no_dcn_tma = atoi(e) != 0;
-  if (const char* e = getenv("CP_NO_UMMA")) P->no_umma = atoi(e) != 0;
   // the plan lives on cfg->device; the caller's current device is restored on every exit path
   struct DeviceGuard {
     int prev = -1;
@@ -670,44 +694,10 @@ int cp_plan_create(const cp_config* cfg, cp_plan** out) {
   CP_CUDA_CHECK(cudaMalloc(&P->wts, P->w_floats * sizeof(float)));
   CP_CUDA_CHECK(cudaMemset(P->wts, 0, P->w_floats * sizeof(float)));
   CP_CUDA_CHECK(cudaMalloc(&P->gn_stats, sizeof(double) * gn_workspace_doubles(P->B)));
+  if ((rc = choose_kernels(P.get()))) return rc;
   if (P->umma_bytes) CP_CUDA_CHECK(cudaMalloc(&P->umma_wts, P->umma_bytes));
-  if (P->prec == 1 || P->prec == 2) {
+  if (cfg->precision == CP_PREC_TF32X3 || cfg->precision == CP_PREC_TF32) {
     CP_CUDA_CHECK(cudaMalloc(&P->splitk_ws, kSplitkWsFloats * sizeof(float)));
-  }
-  for (auto& op : P->ops) {
-    if (!op.use_dcn_tma) continue;
-    IgemmParams q{};
-    q.nsrc = 1;
-    q.src[0] = P->act + op.src[0].off;
-    q.srcC[0] = op.src[0].C;
-    q.srcStride[0] = op.src[0].stride;
-    q.Hin = op.src[0].H;
-    q.Win = op.src[0].W;
-    op.tma_maps.resize(512 + 64);
-    unsigned char* mp = (unsigned char*)(((uintptr_t)op.tma_maps.data() + 63) & ~(uintptr_t)63);
-    int rc2 = dcn_tma_encode(q, P->B, mp);
-    if (rc2) return rc2;
-  }
-  for (auto& op : P->ops) {
-    if (!op.use_tma) continue;
-    IgemmParams q{};
-    q.nsrc = op.nsrc;
-    for (int i = 0; i < op.nsrc; ++i) {
-      q.src[i] = P->act + op.src[i].off;
-      q.srcC[i] = op.src[i].C;
-      q.srcStride[i] = op.src[i].stride;
-    }
-    q.kh = op.kh;
-    q.kw = op.kw;
-    q.Cin = op.Cin;          // Cin / kh / Win / CoutPad select 32- vs 16-channel slabs (tma_cslab)
-    q.CoutPad = op.CoutPad;
-    q.Hin = op.src[0].H;
-    q.Win = op.src[0].W;
-    op.tma_cslab = tma_cslab(q, P->prec == 1);
-    op.tma_maps.resize(512 + 64);
-    unsigned char* mp = (unsigned char*)(((uintptr_t)op.tma_maps.data() + 63) & ~(uintptr_t)63);
-    int rc2 = tma_conv_encode(q, P->B, P->prec == 1, mp);
-    if (rc2) return rc2;
   }
   int n = 0;
   for (auto& op : P->ops) n += op.fused_away ? 0 : ((op.type == OP_GN_RELU) ? 3 : 1);
@@ -789,21 +779,12 @@ int cp_plan_load_weights(cp_plan* P, const char* const* names, const void* const
     }
   }
   // second pass: tensor-core weight tiles are cut from the finished fp32 matrices (merged matrices are complete now)
+  const float* const no_ext[4] = {nullptr, nullptr, nullptr, nullptr};
   for (auto& op : P->ops) {
-    if (op.type != OP_IGEMM) continue;
-    if (op.use_dcn_tma) {
-      if ((rc = launch_pack_tma_weight(P->wts + op.w_off, op.w_ld, op.Cin, 9, op.Cout, op.CoutPad, 1, P->prec == 1, 16,
-                                       P->umma_wts + op.umma_off, s, dcn_tma_tile_n(op.CoutPad, P->prec == 1))))
-        return rc;
-    } else if (op.use_tma) {
-      if ((rc = launch_pack_tma_weight(P->wts + op.w_off, op.w_ld, op.Cin, op.kh * op.kw, op.Cout, op.CoutPad, 1,
-                                       P->prec == 1, op.tma_cslab, P->umma_wts + op.umma_off, s)))
-        return rc;
-    } else if (op.use_umma) {
-      if ((rc = launch_pack_umma_weight(P->wts + op.w_off, op.w_ld, op.kh * op.kw * op.Cin, op.Cout, op.CoutPad,
-                                        P->prec == 2 ? 1 : P->prec, P->umma_wts + op.umma_off, s)))
-        return rc;
-    }
+    if (op.type != OP_IGEMM || !op.kernel.wbytes) continue;
+    IgemmParams p;
+    igemm_params(P, op, P->B, no_ext, nullptr, &p);
+    if ((rc = conv_pack(op.kernel, p, op.w_ld, P->umma_wts + op.tile_off, s))) return rc;
   }
   P->loaded = true;
   return CP_OK;
@@ -823,74 +804,6 @@ static bool pdl_wanted(long long pixels) {
   return pixels <= 8ll * 512 * 512;
 }
 
-// Kernel parameters of conv op `op` at batch `batch`.  ext[] may hold nulls (family queries); run_op rejects them.
-static void igemm_params(const cp_plan* P, const Op& op, int batch, const float* const ext[4], float* const* head_out,
-                         IgemmParams* pp) {
-  IgemmParams& p = *pp;
-  p = IgemmParams{};
-  p.nsrc = op.nsrc;
-  for (int i = 0; i < op.nsrc; ++i) {
-    const Act& a = op.src[i];
-    p.src[i] = a.ext >= 0 ? ext[a.ext] : P->act + a.off;
-    p.srcC[i] = a.C;
-    p.srcStride[i] = a.stride;
-  }
-  p.B = batch;
-  p.Hin = op.src[0].H;
-  p.Win = op.src[0].W;
-  p.Cin = op.Cin;
-  p.kh = op.kh;
-  p.kw = op.kw;
-  p.stride = op.stride;
-  p.pad = op.pad;
-  p.Hout = (p.Hin + 2 * op.pad - op.kh) / op.stride + 1;
-  p.Wout = (p.Win + 2 * op.pad - op.kw) / op.stride + 1;
-  p.Cout = op.Cout;
-  p.CoutPad = op.CoutPad;
-  p.Kpad = op.Kpad;
-  p.wgt = P->wts + op.w_off;
-  p.bias = P->wts + op.b_off;
-  p.residual = op.has_res ? P->act + op.res.off : nullptr;
-  p.resStride = op.res.stride;
-  p.relu = op.relu;
-  p.res_after_relu = op.res_after_relu;
-  if (op.out_head >= 0) {
-    p.out = head_out ? head_out[op.out_head] : nullptr;
-    p.out_nchw = 1;
-    p.outStride = 0;
-  } else {
-    p.out = P->act + op.out.off;
-    p.outStride = op.out.stride;
-  }
-  if (op.mode == IGEMM_DCN) {
-    p.offmask = P->act + op.om.off;
-    p.omStride = op.om.stride;
-    p.mask_is_logit = 1;
-  }
-  p.mode = op.mode;
-  if (op.fuse_heads) {
-    p.fuse_n = (int)op.head_children.size();
-    p.fuse_hidden = P->cfg.head_conv;
-    for (int i = 0; i < p.fuse_n; ++i) {
-      const Op& ch = P->ops[op.head_children[i]];
-      p.fuse_w[i] = P->wts + ch.w_off;
-      p.fuse_b[i] = P->wts + ch.b_off;
-      p.fuse_out[i] = head_out ? head_out[ch.out_head] : nullptr;
-      p.fuse_cout[i] = ch.Cout;
-    }
-  }
-}
-
-// Kernel family of conv op `op` for the launch parameters `p` (the order of the dispatch in run_op).
-static int igemm_family(const Op& op, const IgemmParams& p) {
-  if (op.use_dcn_tma) return CP_FAM_DCN_TMA;
-  if (op.use_tma) return CP_FAM_CONV_TMA;
-  if (op.use_umma) return CP_FAM_IGEMM_UMMA;
-  if (stem_supported(p)) return CP_FAM_STEM;
-  if (conv3_c16_supported(p)) return CP_FAM_CONV3_C16;
-  return CP_FAM_IGEMM_FP32;
-}
-
 // One op of the schedule, as cp_forward runs it.  `info` (may be null) receives what the launcher decided.
 static int run_op(cp_plan* P, size_t idx, int batch, const float* const ext[4], float* const* head_out, cudaStream_t s,
                   cp_op_launch* info) {
@@ -908,30 +821,12 @@ static int run_op(cp_plan* P, size_t idx, int batch, const float* const ext[4], 
         if (op.src[i].ext >= 0 && !ext[op.src[i].ext]) return fail(CP_ERR_INVALID, "cp_forward: a tracking input tensor is null");
       IgemmParams p;
       igemm_params(P, op, batch, ext, head_out, &p);
+      p.wgt_umma = P->umma_wts + op.tile_off;
+      p.splitk_ws = P->splitk_ws;
+      p.splitk_ws_floats = P->splitk_ws ? kSplitkWsFloats : 0;
       LaunchInfo tc;
-      li.family = igemm_family(op, p);
-      if (op.use_dcn_tma) {
-        p.wgt_umma = P->umma_wts + op.umma_off;
-        p.splitk_ws = P->splitk_ws;
-        p.splitk_ws_floats = P->splitk_ws ? kSplitkWsFloats : 0;
-        const unsigned char* mp = (const unsigned char*)(((uintptr_t)op.tma_maps.data() + 63) & ~(uintptr_t)63);
-        if ((rc = launch_dcn_tma(p, mp, P->prec == 1, P->prec == 2, s, &tc))) return rc;
-      } else if (op.use_tma) {
-        p.wgt_umma = P->umma_wts + op.umma_off;
-        p.splitk_ws = P->splitk_ws;
-        p.splitk_ws_floats = P->splitk_ws ? kSplitkWsFloats : 0;
-        const unsigned char* mp = (const unsigned char*)(((uintptr_t)op.tma_maps.data() + 63) & ~(uintptr_t)63);
-        if ((rc = launch_conv_tma(p, mp, P->prec == 2, P->prec == 1, s, &tc))) return rc;
-      } else if (op.use_umma) {
-        p.wgt_umma = P->umma_wts + op.umma_off;
-        if ((rc = launch_igemm_umma(p, P->prec == 2 ? 1 : P->prec, s, &tc))) return rc;
-      } else if (li.family == CP_FAM_STEM) {
-        if ((rc = launch_stem_conv(p, s))) return rc;
-      } else if (li.family == CP_FAM_CONV3_C16) {
-        if ((rc = launch_conv3_c16(p, s))) return rc;
-      } else if ((rc = launch_igemm_fp32(p, s))) {
-        return rc;
-      }
+      li.family = op.kernel.family;
+      if ((rc = conv_launch(op.kernel, p, &op.maps, s, &tc))) return rc;
       li.BN = tc.BN;
       li.ksplit = tc.ksplit;
       li.grid = (int32_t)tc.grid;
@@ -1116,11 +1011,8 @@ int cp_plan_op_desc(const cp_plan* P, int32_t i, cp_op_desc* d) {
       d->w = P->wts + op.w_off;
       d->w_ld = op.w_ld;
       d->bias = P->wts + op.b_off;
-      const float* ext[4] = {nullptr, nullptr, nullptr, nullptr};
-      IgemmParams p;
-      igemm_params(P, op, P->B, ext, nullptr, &p);
-      d->family = igemm_family(op, p);
-      d->x3 = (op.use_tma || op.use_dcn_tma) ? P->prec == 1 : (op.use_umma ? P->prec != 0 : 0);
+      d->family = op.kernel.family;
+      d->x3 = op.kernel.x3;
       break;
     }
     case OP_MAXPOOL: d->family = CP_FAM_MAXPOOL; break;

@@ -277,6 +277,37 @@ __device__ __forceinline__ void epilogue_row(const EpiParams& e, float (&vv)[NV]
   }
 }
 
+// Split-K, second half (conv_tma_splitk_finish, dcn_tma_splitk_finish): one thread per (tile row i, 4 columns) of an
+// (m, n) tile adds the ksplit partial sums ([mn tile][split][BN / 4][rows] float4, row-fastest: coalesced) in split
+// order and runs the epilogue.  row_at(mn, i, &n, &oy, &ox) maps the row to its output position (false: none).
+template <class Params, class RowAt>
+__device__ __forceinline__ void splitk_finish(const Params& p, int rows, long long mn_tiles, RowAt row_at) {
+  griddep_launch_dependents();
+  griddep_wait();
+  const int G = p.BN >> 2;
+  const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= mn_tiles * G * rows) return;
+  const int i = (int)(idx % rows);
+  const int c4 = (int)((idx / rows) % G);
+  const long long mn = idx / ((long long)rows * G);
+  const float4* src = reinterpret_cast<const float4*>(p.part) + ((size_t)mn * p.ksplit * G + c4) * rows + i;
+  float4 a = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int q = 0; q < p.ksplit; ++q) {
+    const float4 v = __ldcg(src + (size_t)q * G * rows);
+    a.x += v.x;
+    a.y += v.y;
+    a.z += v.z;
+    a.w += v.w;
+  }
+  int n, oy, ox;
+  if (!row_at(mn, i, &n, &oy, &ox)) return;
+  const int n_tile = (int)(mn % (p.CoutPad / p.BN));
+  const EpiParams e{p.bias, p.residual, p.resStride, p.relu, p.res_after_relu, p.round_tf32, p.out, p.outStride, p.out_nchw,
+                    p.Cout, p.CoutPad, p.H, p.W};
+  float v[4] = {a.x, a.y, a.z, a.w};
+  epilogue_row<4>(e, v, true, (n * p.H + oy) * p.W + ox, n, oy, ox, n_tile * p.BN + c4 * 4, min(p.Cout, (n_tile + 1) * p.BN));
+}
+
 // Row-wise drain of a warpgroup's 64 x BN wgmma accumulator: 32 columns at a time go through `stage` (64 x 33 floats of
 // shared memory owned by the warpgroup); thread t then holds row t / 2, columns 16 (t % 2) .. + 16 of the chunk and
 // calls fn(row, first column, values).  fn runs for every thread and chunk, also where the columns lie past BN (BN = 16).

@@ -94,7 +94,7 @@ class _env(object):
 def step_and_score(arch, trk, H, W, batch, max_batch, prec, env=None, label=None):
     """Run the schedule op by op; returns one record per op (name, family, BN, ksplit, grid, K, r, ceiling key and the
     op's geometry).  env: environment switches ({name: value}) set while the plan is created, where the plan reads
-    them (CP_NO_DCN_TMA, CP_NO_FUSE_HEADS, ...).  label: the record's config name (default: arch, size, batch, prec)."""
+    them (CP_NO_DCN_TMA).  label: the record's config name (default: arch, size, batch, prec)."""
     with _env(env):
         eng, opt, _ = _engine(arch, trk, H, W, max_batch, prec)
     descs = eng.op_descs()
