@@ -21,7 +21,8 @@
 //   warps 4-7     : consumer of tile rows [0, 64) (wgmma into registers + epilogue); thread i also writes the sampling
 //                   records (one 16-byte record per tap) of position i of the NEXT tile
 //   warps 8-11    : gather, one thread per position: 4 corners x 16 channels from the slab -> bilinear blend * mask ->
-//                   (hi, lo) tf32 split -> A tile in the SWIZZLE_64B K-major layout, AH A stages
+//                   A tile in the SWIZZLE_64B K-major layout (tf32-rounded; fp32 in x3, where the consumers split it
+//                   into hi / lo in registers), AH A stages
 //   warps 12-15   : consumer of tile rows [64, 128)
 #include <cuda.h>
 
@@ -125,7 +126,7 @@ __global__ void __launch_bounds__(DT_THREADS, 1) dcn_tma_kernel(const __grid_con
   const uint32_t sbase = smem_u32(smem);
   const uint32_t coef0 = sbase + 1024u;
   const uint32_t slabs0 = (coef0 + 2u * DT_COEF_BYTES + 1023u) & ~1023u;
-  const uint32_t a_stage = X3 ? 16384u : 8192u;                // hi (+ lo) tile of 128 rows x 64 bytes
+  const uint32_t a_stage = 8192u;                              // A tile of 128 rows x 64 bytes
   const uint32_t atiles0 = slabs0 + 2u * DT_SLAB_BYTES;
   const uint32_t btile_bytes = (uint32_t)BN * 64u * (X3 ? 2u : 1u);
   const uint32_t btiles0 = atiles0 + (uint32_t)p.AH * a_stage;
@@ -212,6 +213,8 @@ __global__ void __launch_bounds__(DT_THREADS, 1) dcn_tma_kernel(const __grid_con
       __syncwarp();
     }
   } else if (warp >= 8 && warp < 12) {
+    // 128 x 40 + 128 x 120 + 256 x 176 = 64 K registers: the consumers also hold the hi / lo A fragments of a K block
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 120;");
     // ===================== gather: thread = one position of the tile; the record of a (position, tap) is decoded once
     // for all 16 channels and a stage is synchronised once per K block =====================
     const int gt = tid - 256;
@@ -309,20 +312,15 @@ __global__ void __launch_bounds__(DT_THREADS, 1) dcn_tma_kernel(const __grid_con
           }
         }
         const int sa = (int)(cnt & (uint32_t)(p.AH - 1));          // barrier index == tile slot
-        const uint32_t a_hi = a_row + (uint32_t)sa * a_stage + (asw << 4);       // chunk c -> a_hi ^ (c << 4)
+        const uint32_t a_dst = a_row + (uint32_t)sa * a_stage + (asw << 4);      // chunk c -> a_dst ^ (c << 4)
         mbar_wait(smem_u32(&ctl->a_empty[sa]), ((cnt >> (p.AH - 1)) & 1u) ^ 1u);
 #pragma unroll
         for (int c = 0; c < 4; ++c) {
           const uint32_t off = (uint32_t)c << 4;
-          float4 h;
-          h.x = tf32_round(v[c].x);
-          h.y = tf32_round(v[c].y);
-          h.z = tf32_round(v[c].z);
-          h.w = tf32_round(v[c].w);
-          st_shared_v4f(a_hi ^ off, h.x, h.y, h.z, h.w);
           if (X3)
-            st_shared_v4f((a_hi ^ off) + 8192u, tf32_round(v[c].x - h.x), tf32_round(v[c].y - h.y), tf32_round(v[c].z - h.z),
-                          tf32_round(v[c].w - h.w));
+            st_shared_v4f(a_dst ^ off, v[c].x, v[c].y, v[c].z, v[c].w);
+          else
+            st_shared_v4f(a_dst ^ off, tf32_round(v[c].x), tf32_round(v[c].y), tf32_round(v[c].z), tf32_round(v[c].w));
         }
         fence_proxy_async_smem();
         __syncwarp();
@@ -345,7 +343,7 @@ __global__ void __launch_bounds__(DT_THREADS, 1) dcn_tma_kernel(const __grid_con
     }
   } else {
     // ===================== consumers: warpgroup c multiplies rows [64 c, 64 c + 64) of every tile =====================
-    asm volatile("setmaxnreg.inc.sync.aligned.u32 168;");
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 176;");
     const int c = warp >= 12 ? 1 : 0, wt = tid & 127;
     float* dstage = reinterpret_cast<float*>(smem + (drain0 - sbase)) + (size_t)c * (DRAIN_STAGE_BYTES / 4);
     EpiParams ep;
@@ -400,9 +398,12 @@ __global__ void __launch_bounds__(DT_THREADS, 1) dcn_tma_kernel(const __grid_con
         const uint32_t sa = cnt & (uint32_t)(p.AH - 1);
         mbar_wait(bar_a_full + 8u * sa, (cnt >> (p.AH - 1)) & 1u);
         mbar_wait(bar_b_full + 8u * (uint32_t)sb, pb);
-        const uint64_t da = make_desc(atiles0 + sa * a_stage + (uint32_t)c * 64u * 64u, DT_CS);
+        const uint32_t a_tile = atiles0 + sa * a_stage + (uint32_t)c * 64u * 64u;
         const uint64_t db = make_desc(btiles0 + (uint32_t)sb * btile_bytes, DT_CS);
-        mma_kblock<BN, X3, false, 2>(acc, da, db, 8192u >> 4, ((uint32_t)BN * 64u) >> 4, X3 ? gk == 0 : kbi == 0);
+        if (X3)
+          mma_kblock_x3<BN, 2>(acc, a_tile, wt, db, ((uint32_t)BN * 64u) >> 4, gk == 0);
+        else
+          mma_kblock<BN, false, false, 2>(acc, make_desc(a_tile, DT_CS), db, 0, 0, kbi == 0);
         if (wt == 0) {
           mbar_arrive(bar_a_empty + 8u * sa);
           mbar_arrive(bar_b_empty + 8u * (uint32_t)sb);
@@ -501,7 +502,7 @@ int launch_dcn_tma(const IgemmParams& p, const void* map, const ConvKernel& k, c
   q.tiles_x = p.Win / DT_PW;
   q.tiles_per_image = q.tiles_x * (p.Hin / DT_PH);
   const long long mn = (long long)q.tiles_per_image * p.B * (p.CoutPad / q.BN);
-  const uint32_t a_stage = x3 ? 16384u : 8192u;
+  const uint32_t a_stage = 8192u;
   q.group = kX3GroupBlocks * 2;      // 16-channel K blocks: same MMA count per group as conv_tma.cu
   const uint32_t btile = (uint32_t)q.BN * 64u * (x3 ? 2u : 1u);
   const size_t budget = 226 * 1024;

@@ -14,7 +14,8 @@
 //     accumulators and run the epilogue.
 // Precisions:
 //   PREC_BF16   bf16 operands, fp32 accumulate                                  (fast mode)
-//   PREC_TF32X3 tf32, 3-term split  a_hi*b_hi + a_lo*b_hi + a_hi*b_lo           (fp32-equivalent mode)
+//   PREC_TF32X3 tf32, 3-term split  a_hi*b_hi + a_lo*b_hi + a_hi*b_lo           (fp32-equivalent mode; the gather
+//               writes fp32 A tiles, the consumers split them into hi / lo in registers: mma_kblock_x3)
 // Every mbarrier wait carries a clock64 watchdog that traps instead of hanging the GPU.
 #include "common.cuh"
 #include "umma_common.cuh"
@@ -39,11 +40,11 @@ template <int PREC>
 struct PrecTraits;
 template <>
 struct PrecTraits<0> {   // bf16
-  static constexpr int kElems = 64, kChunkCh = 8, kTilesA = 1;
+  static constexpr int kElems = 64, kChunkCh = 8, kTilesB = 1;
 };
 template <>
 struct PrecTraits<1> {   // tf32 x 3
-  static constexpr int kElems = 32, kChunkCh = 4, kTilesA = 2;
+  static constexpr int kElems = 32, kChunkCh = 4, kTilesB = 2;     // hi + lo weight tiles
 };
 
 // ------------------------------------------------------------------ the kernel
@@ -54,9 +55,8 @@ __global__ void __launch_bounds__(UM_THREADS, 1) igemm_umma_kernel(const IgemmPa
   UmmaSmem* ctl = reinterpret_cast<UmmaSmem*>(smem);
   if (threadIdx.x == 0) griddep_launch_dependents();      // PDL (common.cuh)
   const uint32_t tiles0 = (smem_u32(smem) + 512u + 1023u) & ~1023u;   // first tile, 1024-aligned
-  const uint32_t b_tile_bytes = (uint32_t)BN * ROW_BYTES * T::kTilesA; // hi (+ lo) weight tiles of one stage
-  const uint32_t a_bytes = A_TILE_BYTES * T::kTilesA;
-  const uint32_t stage_bytes = a_bytes + b_tile_bytes;
+  const uint32_t b_tile_bytes = (uint32_t)BN * ROW_BYTES * T::kTilesB; // hi (+ lo) weight tiles of one stage
+  const uint32_t stage_bytes = A_TILE_BYTES + b_tile_bytes;
 
   const int tid = threadIdx.x, warp = tid >> 5;
   const int M = p.B * p.Hout * p.Wout;
@@ -179,10 +179,9 @@ __global__ void __launch_bounds__(UM_THREADS, 1) igemm_umma_kernel(const IgemmPa
         if (tid == 0) {
           const uint32_t bar = smem_u32(&ctl->full[stage]);
           mbar_arrive_expect_tx(bar, b_tile_bytes);
-          bulk_g2s(tiles0 + (uint32_t)stage * stage_bytes + a_bytes, wsrc + (size_t)kb * b_tile_bytes, b_tile_bytes, bar);
+          bulk_g2s(tiles0 + (uint32_t)stage * stage_bytes + A_TILE_BYTES, wsrc + (size_t)kb * b_tile_bytes, b_tile_bytes, bar);
         }
-        const uint32_t a_hi = tiles0 + (uint32_t)stage * stage_bytes + row_off;
-        const uint32_t a_lo = a_hi + A_TILE_BYTES;
+        const uint32_t a_dst = tiles0 + (uint32_t)stage * stage_bytes + row_off;
 #pragma unroll
         for (int qi = 0; qi < 4; ++qi) {
           float v[8];
@@ -212,21 +211,11 @@ __global__ void __launch_bounds__(UM_THREADS, 1) igemm_umma_kernel(const IgemmPa
             }
           }
           const uint32_t coff = ((uint32_t)(qbase + qi) ^ sw) << 4;
-          if (PREC == 0) {
-            st_shared_v4(a_hi + coff, pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]),
+          if (PREC == 0)
+            st_shared_v4(a_dst + coff, pack_bf16x2(v[0], v[1]), pack_bf16x2(v[2], v[3]), pack_bf16x2(v[4], v[5]),
                          pack_bf16x2(v[6], v[7]));
-          } else {
-            float h[4], l[4];
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              h[j] = tf32_round(v[j]);
-              l[j] = tf32_round(v[j] - h[j]);
-            }
-            st_shared_v4(a_hi + coff, __float_as_uint(h[0]), __float_as_uint(h[1]), __float_as_uint(h[2]),
-                         __float_as_uint(h[3]));
-            st_shared_v4(a_lo + coff, __float_as_uint(l[0]), __float_as_uint(l[1]), __float_as_uint(l[2]),
-                         __float_as_uint(l[3]));
-          }
+          else
+            st_shared_v4f(a_dst + coff, v[0], v[1], v[2], v[3]);
         }
         fence_proxy_async_smem();
         mbar_arrive(smem_u32(&ctl->full[stage]));
@@ -252,10 +241,13 @@ __global__ void __launch_bounds__(UM_THREADS, 1) igemm_umma_kernel(const IgemmPa
     int gk = 0;                              // tf32x3: K block inside its accumulation group
     for (int kb = 0; kb < KB; ++kb) {
       mbar_wait(smem_u32(&ctl->full[stage]), phase);
-      const uint32_t a_hi = tiles0 + (uint32_t)stage * stage_bytes;
-      const uint64_t da = make_desc(a_hi + (uint32_t)c * 64u * ROW_BYTES, 32), db = make_desc(a_hi + a_bytes, 32);
+      const uint32_t a_tile = tiles0 + (uint32_t)stage * stage_bytes + (uint32_t)c * 64u * ROW_BYTES;
+      const uint64_t db = make_desc(tiles0 + (uint32_t)stage * stage_bytes + A_TILE_BYTES, 32);
       // tf32x3: NACC K blocks are chained in the accumulator, then added into round-to-nearest fp32 sums
-      mma_kblock<BN, X3, PREC == 0, 4>(acc, da, db, A_TILE_BYTES >> 4, ((uint32_t)BN * ROW_BYTES) >> 4, X3 ? gk == 0 : kb == 0);
+      if (X3)
+        mma_kblock_x3<BN, 4>(acc, a_tile, wt, db, ((uint32_t)BN * ROW_BYTES) >> 4, gk == 0);
+      else
+        mma_kblock<BN, false, true, 4>(acc, make_desc(a_tile, 32), db, 0, 0, kb == 0);
       if (wt == 0) mbar_arrive(smem_u32(&ctl->empty[stage]));
       if (++stage == STAGES) {
         stage = 0;
@@ -309,7 +301,8 @@ __global__ void __launch_bounds__(UM_THREADS, 1) igemm_umma_kernel(const IgemmPa
 
 // ------------------------------------------------------------------ weight tiling
 // src: fp32 [Ksrc][ld] (k-major rows, BN-folded, the matrix the fp32 kernel consumes);
-// dst: for n_tile, for kb: [hi tile | lo tile], each BN rows x 128 bytes in the SWIZZLE_128B K-major image.
+// dst: for n_tile, for kb: [hi tile | lo tile] (tf32x3) or one bf16 tile, BN rows x 128 bytes in the SWIZZLE_128B
+// K-major image.
 template <int PREC>
 __global__ void pack_umma_weight_kernel(const float* __restrict__ src, int ld, int K, int Cout, int BN, int n_tiles,
                                         int KB, unsigned char* __restrict__ dst) {
@@ -329,7 +322,7 @@ __global__ void pack_umma_weight_kernel(const float* __restrict__ src, int ld, i
       const int k = kb * T::kElems + q * T::kChunkCh + j;
       v[j] = (j < T::kChunkCh && k < K && n < Cout) ? src[(size_t)k * ld + n] : 0.f;
     }
-    const size_t tile = ((size_t)nt * KB + kb) * (size_t)BN * ROW_BYTES * T::kTilesA;
+    const size_t tile = ((size_t)nt * KB + kb) * (size_t)BN * ROW_BYTES * T::kTilesB;
     const size_t off = (size_t)(nr >> 3) * 1024 + (size_t)(nr & 7) * 128 + (size_t)((q ^ (nr & 7)) << 4);
     if (PREC == 0) {
       uint4 w;
@@ -417,8 +410,7 @@ int launch_igemm_umma(const IgemmParams& p, int prec, cudaStream_t stream, Launc
   if (!umma_supported(p, prec)) return fail(CP_ERR_INVALID, "igemm_umma: unsupported shape");
   if (!p.wgt_umma) return fail(CP_ERR_INVALID, "igemm_umma: weight tiles missing");
   const int bn = umma_tile_n(p.CoutPad, prec);
-  const int tilesA = prec == 0 ? 1 : 2;
-  const size_t stage_bytes = (size_t)A_TILE_BYTES * tilesA + (size_t)bn * ROW_BYTES * tilesA;
+  const size_t stage_bytes = (size_t)A_TILE_BYTES + (size_t)bn * ROW_BYTES * (prec == 0 ? 1 : 2);
   const size_t fixed = 512 + 1024 + 2 * (size_t)DRAIN_STAGE_BYTES;     // control block, alignment, epilogue staging
   int stages = (int)((224 * 1024 - fixed) / stage_bytes);
   if (stages > 6) stages = 6;

@@ -136,6 +136,40 @@ template <> __device__ __forceinline__ void wgmma_bf16<256>(float (&d)[128], uin
       : "l"(da), "l"(db), "r"(scale_d));
 }
 
+// Register-A form (tf32 only): thread t of warp w holds the A fragment of rows 16 w + l / 4 (+ 8), columns l % 4
+// (+ 4) of the 64 x 8 slice (PTX ISA, wgmma .m64nNk8 A fragment): a[0] = (r, c), a[1] = (r + 8, c), a[2] = (r, c + 4),
+// a[3] = (r + 8, c + 4).  The registers must stay untouched until the wgmma has been waited for.
+template <int N>
+__device__ __forceinline__ void wgmma_tf32_rs(float (&d)[N / 2], const uint32_t (&a)[4], uint64_t db, uint32_t scale_d);
+template <> __device__ __forceinline__ void wgmma_tf32_rs<16>(float (&d)[8], const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7}, {%8,%9,%10,%11}, %12, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma_tf32_rs<32>(float (&d)[16], const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %21, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, {%16,%17,%18,%19}, %20, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma_tf32_rs<64>(float (&d)[32], const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, {%32,%33,%34,%35}, %36, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
+}
+template <> __device__ __forceinline__ void wgmma_tf32_rs<128>(float (&d)[64], const uint32_t (&a)[4], uint64_t db, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %69, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63}, {%64,%65,%66,%67}, %68, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db), "r"(scale_d));
+}
+
 // One K block on the tensor cores: KS slices of 32 bytes (8 tf32 / 16 bf16 elements) of a 64-row A tile and a BN-row B
 // tile.  X3: 3-term split a_lo b_hi + a_hi b_lo + a_hi b_hi (lo tiles at a_lo / b_lo descriptor units past the hi tiles),
 // cross terms first.  fresh: the first product overwrites the accumulator.  Returns when the products are in `acc` and
@@ -171,6 +205,59 @@ __device__ __forceinline__ void mma_kblock(float (&acc)[BN / 2], uint64_t da, ui
 __device__ __forceinline__ float tf32_round(float x) {
   return __uint_as_float((__float_as_uint(x) + 0x1000u) & 0xffffe000u);
 }
+// Four 8 x 8 b16 matrices; lanes 8 q .. 8 q + 7 give the row addresses of matrix q, register q of lane l gets bytes
+// 4 (l % 4) .. + 4 of row l / 4 of matrix q: one tf32 element.
+__device__ __forceinline__ void ldsm_x4(uint32_t (&r)[4], uint32_t addr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(addr));
+}
+
+// One tf32x3 K block with A in registers: the 3-term split a_lo b_hi + a_hi b_lo + a_hi b_hi in mma_kblock's product
+// order (cross terms first, slice by slice, then the hi products), so the results equal those of the shared-memory
+// hi / lo A tiles.  A (this warpgroup's 64 rows, fp32) is read once per slice from shared memory into registers and
+// split there; B keeps its hi tile at `db` and its lo tile `b_lo` descriptor units further.  The A tile is K-major with
+// rows of 32 KS bytes (KS = 4: SWIZZLE_128B, KS = 2: SWIZZLE_64B), row 0 at `a_tile` (a multiple of the row size; the
+// XOR comes from the address bits, as in make_desc).  wt: thread in the warpgroup.  fresh: the first product
+// overwrites the accumulator.  Returns when the products are in `acc` and the operand tiles may be reused.
+template <int BN, int KS>
+__device__ __forceinline__ void mma_kblock_x3(float (&acc)[BN / 2], uint32_t a_tile, int wt, uint64_t db, uint32_t b_lo,
+                                              bool fresh) {
+  const uint32_t lane = (uint32_t)wt & 31u;
+  // ldmatrix matrices 0..3 = (rows 0-7, k 0-3), (rows 8-15, k 0-3), (rows 0-7, k 4-7), (rows 8-15, k 4-7) of the warp's
+  // 16 rows: the wgmma A fragment a[0..3]
+  const uint32_t row = (uint32_t)(wt >> 5) * 16u + (lane & 7u) + ((lane >> 3) & 1u) * 8u;
+  const uint32_t a_row = a_tile + row * (32u * KS);
+  const uint32_t x = ((lane >> 4) << 4) ^ ((a_row >> 3) & (KS == 4 ? 0x70u : 0x30u));
+  uint32_t hi[KS][4], lo[KS][4];
+#pragma unroll
+  for (int ks = 0; ks < KS; ++ks) {
+    ldsm_x4(hi[ks], a_row + (((uint32_t)ks << 5) ^ x));
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const float v = __uint_as_float(hi[ks][j]);
+      const float h = tf32_round(v);
+      lo[ks][j] = __float_as_uint(tf32_round(v - h));
+      hi[ks][j] = __float_as_uint(h);
+    }
+  }
+  wg_fence();
+#pragma unroll
+  for (int ks = 0; ks < KS; ++ks) {
+    wgmma_tf32_rs<BN>(acc, lo[ks], db + 2u * ks, (fresh && ks == 0) ? 0u : 1u);
+    wgmma_tf32_rs<BN>(acc, hi[ks], db + b_lo + 2u * ks, 1u);
+  }
+#pragma unroll
+  for (int ks = 0; ks < KS; ++ks) wgmma_tf32_rs<BN>(acc, hi[ks], db + 2u * ks, 1u);
+  wg_commit();
+  wg_wait<0>();
+  // the tensor cores read the A registers until the wait: keep them live (and unchanged) up to here
+#pragma unroll
+  for (int ks = 0; ks < KS; ++ks)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) asm volatile("" : "+r"(hi[ks][j]), "+r"(lo[ks][j]));
+}
+
 __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
   uint32_t r;
   asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(b), "f"(a));   // low half <- a
