@@ -15,6 +15,7 @@ CP_POSE_RECORD = 192
 CP_DETS_RECORD = 128
 CP_META_DOUBLES = 16
 CP_MAX_K = 128
+CP_MAX_MODELS = 16
 
 CP_ARCH_DLA34 = 0
 CP_ARCH_DLAV1_34 = 1
@@ -53,6 +54,7 @@ EXPORTS = [
     "cp_preprocess_affine", "cp_tracker_create", "cp_tracker_destroy", "cp_tracker_reset", "cp_tracker_step", "cp_tracker_render",
     "cp_tracker_render_ex", "cp_tracker_seed", "cp_plan_op_desc", "cp_plan_arena", "cp_plan_run_ops",
     "cp_preprocess_ragged", "cp_tracker_step_ex", "cp_tracker_render_ex2", "cp_tracker_seed_ex",
+    "cp_plan_create_multi", "cp_plan_load_weights_model", "cp_plan_num_models", "cp_plan_op_desc_model", "cp_infer_multi",
 ]
 
 # cp_op_family
@@ -191,6 +193,12 @@ def load():
     L.cp_tracker_step_ex.argtypes = [vp, i32, ctypes.POINTER(i32), vp, vp, i32, vp, vp, vp, vp]
     L.cp_tracker_render_ex2.argtypes = [vp, i32, ctypes.POINTER(i32), vp, vp, i32, i32, ctypes.POINTER(i32), vp, vp, vp]
     L.cp_tracker_seed_ex.argtypes = [vp, i32, ctypes.POINTER(i32), vp, vp, i32, vp]
+    L.cp_plan_create_multi.argtypes = [ctypes.POINTER(CpConfig), i32, ctypes.POINTER(vp)]
+    L.cp_plan_load_weights_model.argtypes = [vp, i32, ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(vp),
+                                             ctypes.POINTER(i64), i32, vp]
+    L.cp_plan_num_models.argtypes = [vp]
+    L.cp_plan_op_desc_model.argtypes = [vp, i32, i32, ctypes.POINTER(CpOpDesc)]
+    L.cp_infer_multi.argtypes = [vp, i32, vp, ctypes.POINTER(CpDecodeParams), vp, ctypes.POINTER(vp), vp, vp, vp, vp]
     for name in EXPORTS:
         fn = getattr(L, name)
         if name not in ("cp_version", "cp_last_error", "cp_plan_bytes", "cp_plan_forward_launches",

@@ -76,9 +76,22 @@ struct IgemmParams {
   const float* fuse_b[16];
   float* fuse_out[16];
   int fuse_cout[16];
+  // Several models of one architecture behind one launch (multi-model plans, plan.cu): image n belongs to model
+  // n / ipm, whose fp32 weights and biases (wgt, bias, fuse_w, fuse_b) sit (n / ipm) * wstride floats and whose weight
+  // tiles sit (n / ipm) * tstride bytes after the pointers above.  NCHW sources (the plan's input frames) are shared by
+  // the models: image n reads source image n % ipm.  ipm == 0: one model.
+  int ipm;
+  long long wstride, tstride;
 };
+// images per model of a launch (model_ipm > 0 everywhere in the kernels)
+inline int model_ipm(const IgemmParams& p) { return p.ipm > 0 ? p.ipm : p.B; }
 
 int launch_igemm_fp32(const IgemmParams& p, cudaStream_t stream);
+
+// cp_decode_pnp over the heads of `models` models (decode.cu): prm[0].batch = models x frames, image b is frame
+// b % frames of model b / frames and decodes with prm[b / frames].visible_thresh / .balance; meta holds the frames' rows
+int decode_pnp_models(const cp_decode_params* prm, int models, const cp_heads* heads, const double* meta, float* dets,
+                      float* poses, int32_t* n_valid, void* workspace, size_t workspace_bytes, void* stream);
 
 // What a tensor-core launcher decided for one launch (reported to cp_plan_run_ops; null = not wanted).
 struct LaunchInfo {
@@ -140,8 +153,10 @@ int launch_igemm_umma(const IgemmParams& p, int prec, cudaStream_t stream, Launc
 
 // elementwise / data-movement kernels (elementwise.cu)
 int launch_maxpool2(const float* in, float* out, int B, int H, int W, int C, cudaStream_t s);
+// upsample_add / group_norm_relu: image n uses the weights at (n / ipm) * wstride floats (multi-model plans; ipm = B:
+// one model)
 int launch_upsample_add(const float* in, const float* wgt_kkc, const float* skip, float* out, int B,
-                        int Hin, int Win, int C, int f, cudaStream_t s);
+                        int Hin, int Win, int C, int f, cudaStream_t s, int ipm = 0, long long wstride = 0);
 // writes the [Kpad x CoutPad] block at column `colOff` of a row-major matrix with leading dimension `ld`
 int launch_pack_conv_weight(const float* w_oihw, const float* scale, float* out, int Cout, int Cin,
                             int kh, int kw, int CoutPad, int Kpad, int ld, int colOff, cudaStream_t s,
@@ -157,7 +172,8 @@ int launch_nhwc_to_nchw(const float* in, float* out, int B, int C, int H, int W,
 constexpr int kGnBlocks = 64, kGnMaxGroups = 64;
 inline size_t gn_workspace_doubles(int B) { return (size_t)B * kGnMaxGroups * 2 * (1 + kGnBlocks); }
 int launch_group_norm_relu(float* x, const float* gamma, const float* beta, int B, int HW, int C,
-                           int stride, int chanOffset, int groups, float eps, double* ws, cudaStream_t s);
+                           int stride, int chanOffset, int groups, float eps, double* ws, cudaStream_t s, int ipm = 0,
+                           long long wstride = 0);
 int launch_gru_gates(const float* xi, const float* hh, const float* hprev, float* hout, int B_HW, int C,
                      int first_step, cudaStream_t s);
 

@@ -62,6 +62,10 @@ struct TmaConvParams {
   const float* fuse_b[16];
   float* fuse_out[16];
   int fuse_cout[16];
+  // models (IgemmParams::ipm): image n is model n / ipm's.  The 1x1 position tiles are cut per model (tiles_per_model
+  // of them over its ipm images) so that no tile mixes two models' weights.
+  int ipm;
+  long long wstride, tstride, tiles_per_model;
 };
 
 using namespace umma;
@@ -74,9 +78,11 @@ static_assert(sizeof(TmaCtl) <= 512, "control block");
 
 // Tile geometry of one 128-position output tile.
 struct TileGeo {
-  int n_tile, img, g0, r_lo;
+  int n_tile, img, g0, r_lo, model;
   long long pos0;
 };
+// MULTI: the launch holds several models (TmaConvParams::ipm); otherwise model is 0 and the code is that of one model.
+template <bool MULTI>
 __device__ __forceinline__ TileGeo decode_tile(const TmaConvParams& p, long long ct, int n_tiles) {
   TileGeo g;
   g.n_tile = (int)(ct % n_tiles);
@@ -85,11 +91,16 @@ __device__ __forceinline__ TileGeo decode_tile(const TmaConvParams& p, long long
   g.g0 = 0;
   g.r_lo = 0;
   g.pos0 = 0;
+  g.model = 0;
   if (p.k == 3) {
     g.img = (int)(m_tile / p.tiles_per_image);
     g.g0 = (int)(m_tile - (long long)g.img * p.tiles_per_image) * p.tile_m;
     const int t = g.g0 - 1;
     g.r_lo = (t >= 0) ? t / p.Wt : -((-t + p.Wt - 1) / p.Wt);      // floor((g0 - 1) / Wt)
+    if (MULTI) g.model = g.img / p.ipm;
+  } else if (MULTI) {
+    g.model = (int)(m_tile / p.tiles_per_model);
+    g.pos0 = (long long)g.model * p.ipm * p.H * p.W + (m_tile - g.model * p.tiles_per_model) * p.tile_m;
   } else {
     g.pos0 = m_tile * p.tile_m;
   }
@@ -97,6 +108,7 @@ __device__ __forceinline__ TileGeo decode_tile(const TmaConvParams& p, long long
 }
 
 // output position i of a tile -> (valid, image, row, column, flat NHWC index)
+template <bool MULTI>
 __device__ __forceinline__ bool tile_position(const TmaConvParams& p, const TileGeo& g, int i, int* n, int* oy, int* ox, int* m) {
   bool valid;
   if (p.k == 3) {
@@ -108,7 +120,8 @@ __device__ __forceinline__ bool tile_position(const TmaConvParams& p, const Tile
     valid = (*oy < p.H) && (xp >= 1) && (xp <= p.W);
   } else {
     const long long pix = g.pos0 + i;
-    valid = pix < (long long)p.B * p.H * p.W;
+    // rows past the model's images belong to the next model
+    valid = pix < (MULTI ? (long long)(g.model + 1) * p.ipm : (long long)p.B) * p.H * p.W;
     const long long pp = valid ? pix : 0;
     *ox = (int)(pp % p.W);
     const long long t = pp / p.W;
@@ -122,7 +135,7 @@ __device__ __forceinline__ bool tile_position(const TmaConvParams& p, const Tile
 // PERSISTENT kernel: gridDim.x = min(#tiles, #SMs); CTA c processes tiles c, c + gridDim.x, ...  Every role keeps its
 // pipeline state across tiles, so the TMA / split of tile i+1 overlap the epilogue of tile i and the fixed cost of a CTA
 // (barrier init, descriptor fetch, pipeline fill) is paid once per SM instead of per tile.
-template <bool X3, bool FUSE, int BN>
+template <bool X3, bool FUSE, int BN, bool MULTI>
 __global__ void __launch_bounds__(X3 ? TM_THREADS_X3 : TM_THREADS, 1) conv_tma_kernel(const __grid_constant__ TmaConvParams p) {
   extern __shared__ __align__(1024) unsigned char smem[];
   TmaCtl* ctl = reinterpret_cast<TmaCtl*>(smem);
@@ -176,7 +189,7 @@ __global__ void __launch_bounds__(X3 ? TM_THREADS_X3 : TM_THREADS, 1) conv_tma_k
         int stage = 0;
         uint32_t phase = 0;
         for (long long it = 0, tile = tile_at(0); tile < total_tiles; tile = tile_at(++it)) {
-          const TileGeo g = decode_tile(p, tile / KS_SPLIT, n_tiles);
+          const TileGeo g = decode_tile<MULTI>(p, tile / KS_SPLIT, n_tiles);
           const int s_begin = (int)(tile % KS_SPLIT) * sps;
           for (int s = s_begin; s < s_begin + sps; ++s) {
             int src = 0, cb = 0;
@@ -206,8 +219,15 @@ __global__ void __launch_bounds__(X3 ? TM_THREADS_X3 : TM_THREADS, 1) conv_tma_k
         int stage = 0;
         uint32_t phase = 0;
         for (long long it = 0, tile = tile_at(0); tile < total_tiles; tile = tile_at(++it)) {
-          const int n_tile = (int)((tile / KS_SPLIT) % n_tiles);
-          const unsigned char* wsrc = p.wtiles + ((size_t)n_tile * KB_all + (size_t)(tile % KS_SPLIT) * KB) * btile_bytes;
+          const unsigned char* wsrc;
+          if constexpr (MULTI) {
+            const TileGeo g = decode_tile<MULTI>(p, tile / KS_SPLIT, n_tiles);
+            wsrc = p.wtiles + (size_t)g.model * p.tstride +
+                   ((size_t)g.n_tile * KB_all + (size_t)(tile % KS_SPLIT) * KB) * btile_bytes;
+          } else {
+            const int n_tile = (int)((tile / KS_SPLIT) % n_tiles);
+            wsrc = p.wtiles + ((size_t)n_tile * KB_all + (size_t)(tile % KS_SPLIT) * KB) * btile_bytes;
+          }
           for (int kb = 0; kb < KB; ++kb) {
             mbar_wait(smem_u32(&ctl->b_empty[stage]), phase ^ 1u);
             const uint32_t bar = smem_u32(&ctl->b_full[stage]);
@@ -293,7 +313,7 @@ __global__ void __launch_bounds__(X3 ? TM_THREADS_X3 : TM_THREADS, 1) conv_tma_k
 #pragma unroll
     for (int j = 0; j < (FUSE ? 16 : 1); ++j) acc2[j] = 0.f;
     for (long long it = 0, tile = tile_at(0); tile < total_tiles; tile = tile_at(++it)) {
-      const TileGeo g = decode_tile(p, tile / KS_SPLIT, n_tiles);
+      const TileGeo g = decode_tile<MULTI>(p, tile / KS_SPLIT, n_tiles);
       // A row of tap (ky, kx) for tile row 64 c: start of the slab + (g0 - 1 - r_lo Wt) + ky Wt + kx + 64 c
       const uint32_t row0 = (p.k == 3 ? (uint32_t)(g.g0 - 1 - g.r_lo * p.Wt) : 0u) + (uint32_t)c * 64u;
 #pragma unroll
@@ -341,9 +361,11 @@ __global__ void __launch_bounds__(X3 ? TM_THREADS_X3 : TM_THREADS, 1) conv_tma_k
       // ---- epilogue: rows of this warpgroup, 32 columns at a time through shared memory (drain_rows)
       const int r_me = wt >> 1;
       int n, oy, ox, m;
-      const bool valid = tile_position(p, g, c * 64 + r_me, &n, &oy, &ox, &m);
+      const bool valid = tile_position<MULTI>(p, g, c * 64 + r_me, &n, &oy, &ox, &m);
       const int col_end = min(p.Cout, (g.n_tile + 1) * BN);
       const int head = FUSE ? g.n_tile / p.tph : 0, part = FUSE ? g.n_tile - head * p.tph : 0;
+      const size_t wofs = MULTI ? (size_t)g.model * p.wstride : 0;      // this tile's model's biases and fused 1x1 weights
+      if (MULTI) ep.bias = p.bias + wofs;
       if (FUSE && part == 0) {
 #pragma unroll
         for (int j = 0; j < (FUSE ? 16 : 1); ++j) acc2[j] = 0.f;
@@ -361,8 +383,8 @@ __global__ void __launch_bounds__(X3 ? TM_THREADS_X3 : TM_THREADS, 1) conv_tma_k
           for (int q = 0; q < 4; ++q) __stcg(mine + (size_t)q * p.tile_m, make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]));
         } else if (FUSE) {
           // hidden = relu(conv3x3 + bias) never leaves the SM: multiply it with this head's 1x1 weights right here
-          const float* b1 = p.bias + (size_t)g.n_tile * BN + cb;
-          const float4* w2 = reinterpret_cast<const float4*>(p.fuse_w[head]) + ((size_t)part * BN + cb) * 4;
+          const float* b1 = p.bias + wofs + (size_t)g.n_tile * BN + cb;
+          const float4* w2 = reinterpret_cast<const float4*>(p.fuse_w[head] + wofs) + ((size_t)part * BN + cb) * 4;
 #pragma unroll
           for (int q = 0; q < 16; ++q) {
             const float h = fmaxf(v[q] + __ldg(b1 + q), 0.f);
@@ -393,7 +415,7 @@ __global__ void __launch_bounds__(X3 ? TM_THREADS_X3 : TM_THREADS, 1) conv_tma_k
           const size_t plane = (size_t)p.H * p.W;
 #pragma unroll
           for (int j = 0; j < 16; ++j)
-            if (j < co) o[j * plane] = acc2[FUSE ? j : 0] + __ldg(p.fuse_b[head] + j);
+            if (j < co) o[j * plane] = acc2[FUSE ? j : 0] + __ldg(p.fuse_b[head] + wofs + j);
         }
       }
     }
@@ -460,10 +482,11 @@ EncodeTiledFn get_encode() {
 }  // namespace
 
 // split-K, second half (splitk_finish, umma_common.cuh): tile row i -> output position
+template <bool MULTI>
 __global__ void __launch_bounds__(256) conv_tma_splitk_finish(const __grid_constant__ TmaConvParams p, long long mn_tiles) {
-  splitk_finish(p, p.tile_m, mn_tiles, [&](long long mn, int i, int* n, int* oy, int* ox) {
+  splitk_finish<MULTI>(p, p.tile_m, mn_tiles, [&](long long mn, int i, int* n, int* oy, int* ox) {
     int m;
-    return tile_position(p, decode_tile(p, mn, p.CoutPad / p.BN), i, n, oy, ox, &m);
+    return tile_position<MULTI>(p, decode_tile<MULTI>(p, mn, p.CoutPad / p.BN), i, n, oy, ox, &m);
   });
 }
 
@@ -597,14 +620,14 @@ int tma_conv_encode(const IgemmParams& p, int Bmax, int cs, void* maps_out) {
   return CP_OK;
 }
 
-template <bool X3, bool FUSE>
+template <bool X3, bool FUSE, bool MULTI>
 static int launch_conv_tma_kernel(const TmaConvParams& q, const cudaLaunchConfig_t& cfg0) {
   void (*kern)(TmaConvParams) = nullptr;
   switch (q.BN) {
-    case 16: kern = conv_tma_kernel<X3, FUSE, 16>; break;
-    case 32: kern = conv_tma_kernel<X3, FUSE, 32>; break;
-    case 64: kern = conv_tma_kernel<X3, FUSE, 64>; break;
-    case 128: kern = conv_tma_kernel<X3, FUSE, 128>; break;
+    case 16: kern = conv_tma_kernel<X3, FUSE, 16, MULTI>; break;
+    case 32: kern = conv_tma_kernel<X3, FUSE, 32, MULTI>; break;
+    case 64: kern = conv_tma_kernel<X3, FUSE, 64, MULTI>; break;
+    case 128: kern = conv_tma_kernel<X3, FUSE, 128, MULTI>; break;
     default: return fail(CP_ERR_INVALID, "conv_tma: unsupported N tile");
   }
   static PerDevice<bool, 4> configured;
@@ -626,6 +649,7 @@ static int launch_conv_tma_kernel(const TmaConvParams& q, const cudaLaunchConfig
 
 int launch_conv_tma(const IgemmParams& p, const void* maps, const ConvKernel& k, cudaStream_t stream, LaunchInfo* info) {
   if (!p.wgt_umma) return fail(CP_ERR_INVALID, "conv_tma: weight tiles missing");
+  if (p.B % model_ipm(p)) return fail(CP_ERR_INVALID, "conv_tma: batch is not a whole number of models");
   const bool x3 = k.x3;
   TmaConvParams q;
   memset(&q, 0, sizeof(q));
@@ -646,6 +670,9 @@ int launch_conv_tma(const IgemmParams& p, const void* maps, const ConvKernel& k,
   q.Wt = p.Win + 2;
   q.tile_m = TM_BM;
   q.boxh = tma_boxh(q.Wt);
+  q.ipm = model_ipm(p);
+  q.wstride = p.wstride;
+  q.tstride = p.tstride;
   size_t m_tiles;
   if (q.k == 3) {
     q.tiles_per_image = (p.Hin * q.Wt + q.tile_m - 1) / q.tile_m;
@@ -653,7 +680,8 @@ int launch_conv_tma(const IgemmParams& p, const void* maps, const ConvKernel& k,
     q.slab_bytes = (uint32_t)q.boxh * q.Wt * (uint32_t)q.cslab * 4u;
   } else {
     q.tiles_per_image = 0;
-    m_tiles = ((size_t)p.B * p.Hin * p.Win + q.tile_m - 1) / q.tile_m;
+    q.tiles_per_model = ((long long)q.ipm * p.Hin * p.Win + q.tile_m - 1) / q.tile_m;
+    m_tiles = (size_t)q.tiles_per_model * (p.B / q.ipm);
     q.slab_bytes = (uint32_t)q.tile_m * (uint32_t)q.cslab * 4u;
   }
   q.slab_stride = (q.slab_bytes + 1023u) & ~1023u;
@@ -700,8 +728,15 @@ int launch_conv_tma(const IgemmParams& p, const void* maps, const ConvKernel& k,
   cfg.blockDim = dim3(x3 ? TM_THREADS_X3 : TM_THREADS);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = stream;
-  int rc = x3 ? (q.fuse ? launch_conv_tma_kernel<true, true>(q, cfg) : launch_conv_tma_kernel<true, false>(q, cfg))
-              : (q.fuse ? launch_conv_tma_kernel<false, true>(q, cfg) : launch_conv_tma_kernel<false, false>(q, cfg));
+  // several models in the launch: the model-indexed instantiations; one model runs the one-model code unchanged
+  const bool multi = p.B > q.ipm;
+  int rc;
+  if (multi)
+    rc = x3 ? (q.fuse ? launch_conv_tma_kernel<true, true, true>(q, cfg) : launch_conv_tma_kernel<true, false, true>(q, cfg))
+            : (q.fuse ? launch_conv_tma_kernel<false, true, true>(q, cfg) : launch_conv_tma_kernel<false, false, true>(q, cfg));
+  else
+    rc = x3 ? (q.fuse ? launch_conv_tma_kernel<true, true, false>(q, cfg) : launch_conv_tma_kernel<true, false, false>(q, cfg))
+            : (q.fuse ? launch_conv_tma_kernel<false, true, false>(q, cfg) : launch_conv_tma_kernel<false, false, false>(q, cfg));
   if (rc) return rc;
   if (info) {
     info->BN = q.BN;
@@ -710,7 +745,8 @@ int launch_conv_tma(const IgemmParams& p, const void* maps, const ConvKernel& k,
   }
   if (q.ksplit > 1) {
     const long long threads = mn * (q.BN / 4) * q.tile_m;
-    CP_CUDA_CHECK(launch_kernel(conv_tma_splitk_finish, dim3((unsigned)((threads + 255) / 256)), dim3(256), 0, stream, q, mn));
+    CP_CUDA_CHECK(launch_kernel(multi ? conv_tma_splitk_finish<true> : conv_tma_splitk_finish<false>,
+                                dim3((unsigned)((threads + 255) / 256)), dim3(256), 0, stream, q, mn));
     CP_LAUNCH_CHECK("conv_tma_splitk_finish");
   }
   return CP_OK;

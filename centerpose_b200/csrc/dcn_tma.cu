@@ -65,6 +65,8 @@ struct DcnTmaParams {
   // partial sums to `part` ([mn tile][split][BN / 4][128 rows] float4) and dcn_tma_splitk_finish runs the epilogue
   int ksplit, sps;
   float* part;
+  int ipm;                           // models (IgemmParams::ipm): image n takes model n / ipm's bias and weight tiles
+  long long wstride, tstride;
 };
 
 struct DcnCtl {
@@ -118,7 +120,8 @@ __device__ __forceinline__ void coef_row(const DcnTmaParams& p, const float* __r
   }
 }
 
-template <bool X3, int BN>
+// MULTI: the launch holds several models (DcnTmaParams::ipm); otherwise the code is that of one model
+template <bool X3, int BN, bool MULTI>
 __global__ void __launch_bounds__(DT_THREADS, 1) dcn_tma_kernel(const __grid_constant__ DcnTmaParams p) {
   extern __shared__ __align__(1024) unsigned char smem[];
   DcnCtl* ctl = reinterpret_cast<DcnCtl*>(smem);
@@ -197,7 +200,9 @@ __global__ void __launch_bounds__(DT_THREADS, 1) dcn_tma_kernel(const __grid_con
         uint32_t phase = 0;
         for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
           const int n_tile = (int)((tile / KS_SPLIT) % n_tiles);
-          const unsigned char* wsrc = p.wtiles + ((size_t)n_tile * KB_all + (size_t)(tile % KS_SPLIT) * KB) * btile_bytes;
+          const int model = MULTI ? (int)((tile / KS_SPLIT) / n_tiles / p.tiles_per_image) / p.ipm : 0;
+          const unsigned char* wsrc = p.wtiles + (size_t)model * p.tstride +
+                                      ((size_t)n_tile * KB_all + (size_t)(tile % KS_SPLIT) * KB) * btile_bytes;
           for (int kb = 0; kb < KB; ++kb) {
             mbar_wait(smem_u32(&ctl->b_empty[stage]), phase ^ 1u);
             const uint32_t bar = smem_u32(&ctl->b_full[stage]);
@@ -428,6 +433,7 @@ __global__ void __launch_bounds__(DT_THREADS, 1) dcn_tma_kernel(const __grid_con
       const int n = (int)(m_tile / p.tiles_per_image);
       const int pt = (int)(m_tile - (long long)n * p.tiles_per_image);
       const int col_end = min(p.Cout, (n_tile + 1) * BN);
+      if (MULTI) ep.bias = p.bias + (size_t)(n / p.ipm) * p.wstride;
       auto fn = [&](int r, int cb0, float (&v)[16]) {
         if (cb0 >= BN) return;
         const int i = c * 64 + r;
@@ -451,8 +457,9 @@ __global__ void __launch_bounds__(DT_THREADS, 1) dcn_tma_kernel(const __grid_con
 }
 
 // split-K, second half (splitk_finish, umma_common.cuh): tile row i -> position i of the 8 x 16 patch
+template <bool MULTI>
 __global__ void __launch_bounds__(256) dcn_tma_splitk_finish(const __grid_constant__ DcnTmaParams p, long long mn_tiles) {
-  splitk_finish(p, DT_BM, mn_tiles, [&](long long mn, int i, int* n, int* oy, int* ox) {
+  splitk_finish<MULTI>(p, DT_BM, mn_tiles, [&](long long mn, int i, int* n, int* oy, int* ox) {
     const long long m_tile = mn / (p.CoutPad / p.BN);
     *n = (int)(m_tile / p.tiles_per_image);
     const int pt = (int)(m_tile - (long long)*n * p.tiles_per_image);
@@ -527,17 +534,25 @@ int launch_dcn_tma(const IgemmParams& p, const void* map, const ConvKernel& k, c
   q.out_nchw = p.out_nchw;
   q.round_tf32 = k.round_out;
   q.wtiles = (const unsigned char*)p.wgt_umma;
+  q.ipm = model_ipm(p);
+  q.wstride = p.wstride;
+  q.tstride = p.tstride;
+  const bool multi = p.B > q.ipm;      // several models: the model-indexed instantiations
   const size_t smem = fixed + (size_t)q.SB * btile;
   void (*kern)(DcnTmaParams) = nullptr;
   switch (q.BN) {
-    case 16: kern = x3 ? dcn_tma_kernel<true, 16> : dcn_tma_kernel<false, 16>; break;
-    case 32: kern = x3 ? dcn_tma_kernel<true, 32> : dcn_tma_kernel<false, 32>; break;
-    case 64: kern = x3 ? dcn_tma_kernel<true, 64> : dcn_tma_kernel<false, 64>; break;
-    case 128: kern = x3 ? dcn_tma_kernel<true, 128> : dcn_tma_kernel<false, 128>; break;
+    case 16: kern = multi ? (x3 ? dcn_tma_kernel<true, 16, true> : dcn_tma_kernel<false, 16, true>)
+                          : (x3 ? dcn_tma_kernel<true, 16, false> : dcn_tma_kernel<false, 16, false>); break;
+    case 32: kern = multi ? (x3 ? dcn_tma_kernel<true, 32, true> : dcn_tma_kernel<false, 32, true>)
+                          : (x3 ? dcn_tma_kernel<true, 32, false> : dcn_tma_kernel<false, 32, false>); break;
+    case 64: kern = multi ? (x3 ? dcn_tma_kernel<true, 64, true> : dcn_tma_kernel<false, 64, true>)
+                          : (x3 ? dcn_tma_kernel<true, 64, false> : dcn_tma_kernel<false, 64, false>); break;
+    case 128: kern = multi ? (x3 ? dcn_tma_kernel<true, 128, true> : dcn_tma_kernel<false, 128, true>)
+                           : (x3 ? dcn_tma_kernel<true, 128, false> : dcn_tma_kernel<false, 128, false>); break;
     default: return fail(CP_ERR_INVALID, "dcn_tma: unsupported N tile");
   }
-  static PerDevice<bool, 8> configured;
-  const int slot = (x3 ? 4 : 0) + (q.BN == 128 ? 3 : (q.BN == 64 ? 2 : (q.BN == 32 ? 1 : 0)));
+  static PerDevice<bool, 16> configured;
+  const int slot = (multi ? 8 : 0) + (x3 ? 4 : 0) + (q.BN == 128 ? 3 : (q.BN == 64 ? 2 : (q.BN == 32 ? 1 : 0)));
   if (!configured.here(slot)) {
     CP_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     configured.here(slot) = true;
@@ -560,7 +575,7 @@ int launch_dcn_tma(const IgemmParams& p, const void* map, const ConvKernel& k, c
   }
   if (q.ksplit > 1) {
     const long long threads = mn * (q.BN / 4) * DT_BM;
-    CP_CUDA_CHECK(launch_kernel(dcn_tma_splitk_finish, dim3((unsigned)((threads + 255) / 256)), dim3(256), 0, stream, q, mn));
+    CP_CUDA_CHECK(launch_kernel(multi ? dcn_tma_splitk_finish<true> : dcn_tma_splitk_finish<false>, dim3((unsigned)((threads + 255) / 256)), dim3(256), 0, stream, q, mn));
     CP_LAUNCH_CHECK("dcn_tma_splitk_finish");
   }
   return CP_OK;

@@ -212,6 +212,11 @@ struct GroupArgs {
   float* dets;    // [B,K,CP_DETS_RECORD] (user buffer or workspace)
   float* poses;   // [B,K,CP_POSE_RECORD]
   int* n_valid;
+  // several models' heads in one launch (cp_infer_multi): image b is frame b % ipm of model b / ipm, which decodes
+  // with that model's visible_thresh and balance; the meta rows are the frames'
+  int ipm;
+  int visible_thresh[CP_MAX_MODELS];
+  float balance[CP_MAX_MODELS];
 };
 
 __device__ __forceinline__ float gatherf(const float* base, int b, int C, int c, int HW, int ind) {
@@ -247,7 +252,8 @@ __global__ void __launch_bounds__(256, 1) group_pose_kernel(const GroupArgs a) {
 
   float* dets = a.dets + (size_t)b * K * CP_DETS_RECORD;
   float* poses = a.poses + (size_t)b * K * CP_POSE_RECORD;
-  const double* meta = a.meta + (size_t)b * CP_META_DOUBLES;
+  const double* meta = a.meta + (size_t)(b % a.ipm) * CP_META_DOUBLES;
+  const int model = b / a.ipm;
 
   // ---------------- decode.py:52-68 _topk: the K best of the num_classes x K per-class candidates.  Every per-class list
   // is sorted (value descending, index ascending), so the rank of a candidate in the merged order (value descending,
@@ -322,7 +328,7 @@ __global__ void __launch_bounds__(256, 1) group_pose_kernel(const GroupArgs a) {
     for (int t = 0; t < 2 * J; ++t) {
       d[CP_D_TRACKING_HP + t] = a.h.tracking_hp ? gatherf(a.h.tracking_hp, b, 2 * J, t, HW, ind) : 0.0f;
       d[CP_D_KPS_DISP_STD + t] =
-          a.h.hps_uncertainty ? sqrtf(expf(gatherf(a.h.hps_uncertainty, b, 2 * J, t, HW, ind))) * P.balance : 0.0f;
+          a.h.hps_uncertainty ? sqrtf(expf(gatherf(a.h.hps_uncertainty, b, 2 * J, t, HW, ind))) * a.balance[model] : 0.0f;
     }
   }
   // ---------------- phase B: per-joint heat-map peaks (decode.py:129-144)
@@ -573,7 +579,7 @@ __global__ void __launch_bounds__(256, 1) group_pose_kernel(const GroupArgs a) {
         }
         __syncwarp();
         float sc[3] = {d[CP_D_OBJ_SCALE], d[CP_D_OBJ_SCALE + 1], d[CP_D_OBJ_SCALE + 2]};
-        solve_and_shell_warp(pts, n_in, sc, meta + 5, img_w, img_h, P.visible_thresh, P.opencv_return, &po, sm, lane);
+        solve_and_shell_warp(pts, n_in, sc, meta + 5, img_w, img_h, a.visible_thresh[model], P.opencv_return, &po, sm, lane);
       }
       if (lane == 0) {
         o[CP_P_STATUS] = (float)po.status;
@@ -645,8 +651,20 @@ size_t cp_decode_workspace_bytes(const cp_decode_params* prm) {
 
 int cp_decode_pnp(const cp_decode_params* prm, const cp_heads* heads, const double* meta, float* dets, float* poses,
                   int32_t* n_valid, void* workspace, size_t workspace_bytes, void* stream_) {
+  return cp::decode_pnp_models(prm, 1, heads, meta, dets, poses, n_valid, workspace, workspace_bytes, stream_);
+}
+
+}  // extern "C"
+
+namespace cp {
+
+// prm[0 .. models): prm[0].batch = models x frames; prm[m] gives model m its visible_thresh and balance
+int decode_pnp_models(const cp_decode_params* prm, int models, const cp_heads* heads, const double* meta, float* dets,
+                      float* poses, int32_t* n_valid, void* workspace, size_t workspace_bytes, void* stream_) {
   int rc = validate(prm);
   if (rc) return rc;
+  if (models < 1 || models > CP_MAX_MODELS || prm->batch % models)
+    return fail(CP_ERR_INVALID, "cp_decode_pnp: batch is not a whole number of models");
   if (!heads || !meta || !poses || !n_valid || !workspace) return fail(CP_ERR_INVALID, "cp_decode_pnp: null argument");
   if (!heads->hm || !heads->wh || !heads->hps || !heads->hm_hp)
     return fail(CP_ERR_INVALID, "cp_decode_pnp: hm, wh, hps and hm_hp heads are required");
@@ -686,6 +704,11 @@ int cp_decode_pnp(const cp_decode_params* prm, const cp_heads* heads, const doub
   ga.dets = dets_buf;
   ga.poses = poses;
   ga.n_valid = n_valid;
+  ga.ipm = prm->batch / models;
+  for (int m = 0; m < models; ++m) {
+    ga.visible_thresh[m] = prm[m].visible_thresh;
+    ga.balance[m] = prm[m].balance;
+  }
   static cp::PerDevice<bool> pose_configured;
   if (!pose_configured.here()) {      // static (~29 KB) + dynamic (20 KB) shared memory crosses the 48 KB default
     CP_CUDA_CHECK(cudaFuncSetAttribute(group_pose_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 64 * 1024));
@@ -696,4 +719,4 @@ int cp_decode_pnp(const cp_decode_params* prm, const cp_heads* heads, const doub
   return CP_OK;
 }
 
-}  // extern "C"
+}  // namespace cp

@@ -44,10 +44,10 @@ __global__ void maxpool2_kernel(const float4* __restrict__ in, float4* __restric
 //      2 x 2 taps; weights are packed [ky][kx][C].
 // IDX = unsigned for every shape the network uses (< 2^32 float4 elements): the three divisions of the index decode are
 // then 32-bit (the 64-bit ones were ~100 instructions per 16 bytes moved and held the kernel at half the HBM rate).
-template <typename IDX>
+template <typename IDX, bool MULTI>
 __global__ void upsample_add_kernel(const float4* __restrict__ in, const float4* __restrict__ w,
                                     const float4* __restrict__ skip, float4* __restrict__ out, int B,
-                                    int Hin, int Win, int C4, int f) {
+                                    int Hin, int Win, int C4, int f, int ipm, long long wstride4) {
   griddep_launch_dependents();      // PDL (common.cuh)
   griddep_wait();
   const IDX Ho = (IDX)(Hin * f), Wo = (IDX)(Win * f), C4u = (IDX)C4;
@@ -73,7 +73,7 @@ __global__ void upsample_add_kernel(const float4* __restrict__ in, const float4*
         int ix = ix_hi - b, kx = kx_lo + b * f;
         if (ix < 0 || ix >= Win || kx >= k) continue;
         float4 v = __ldg(in + ((size_t)(n * Hin + iy) * Win + ix) * C4 + c);
-        float4 ww = __ldg(w + (size_t)(ky * k + kx) * C4 + c);
+        float4 ww = __ldg(w + (MULTI ? (size_t)(n / ipm) * wstride4 : 0) + (size_t)(ky * k + kx) * C4 + c);
         up.x = fmaf(v.x, ww.x, up.x);
         up.y = fmaf(v.y, ww.y, up.y);
         up.z = fmaf(v.z, ww.z, up.z);
@@ -216,9 +216,11 @@ __global__ void gn_stats_finish_kernel(const double* __restrict__ partial, int n
   }
 }
 
+template <bool MULTI>
 __global__ void gn_apply_relu_kernel(float* __restrict__ x, const float* __restrict__ gamma,
                                      const float* __restrict__ beta, int B, int HW, int C, int stride,
-                                     int chanOffset, int groups, float eps, const double* __restrict__ stats) {
+                                     int chanOffset, int groups, float eps, const double* __restrict__ stats, int ipm,
+                                     long long wstride) {
   const int cpg = C / groups;
   size_t total = (size_t)B * HW * C;
   const double cnt = (double)HW * cpg;
@@ -233,7 +235,8 @@ __global__ void gn_apply_relu_kernel(float* __restrict__ x, const float* __restr
     if (var < 0) var = 0;
     float rstd = (float)(1.0 / sqrt(var + (double)eps));
     float* p = x + pix * stride + chanOffset + c;
-    float v = (*p - (float)mean) * rstd * __ldg(gamma + c) + __ldg(beta + c);
+    const size_t wo = MULTI ? (size_t)(n / ipm) * wstride : 0;      // model n / ipm's gamma and beta
+    float v = (*p - (float)mean) * rstd * __ldg(gamma + wo + c) + __ldg(beta + wo + c);
     *p = fmaxf(v, 0.f);
   }
 }
@@ -274,15 +277,17 @@ int launch_maxpool2(const float* in, float* out, int B, int H, int W, int C, cud
 }
 
 int launch_upsample_add(const float* in, const float* w, const float* skip, float* out, int B, int Hin,
-                        int Win, int C, int f, cudaStream_t s) {
+                        int Win, int C, int f, cudaStream_t s, int ipm, long long wstride) {
   if (C % 4) return fail(CP_ERR_INVALID, "upsample: C%4");
+  if (ipm <= 0) ipm = B;
+  if (wstride % 4) return fail(CP_ERR_INVALID, "upsample: model weight stride % 4");
   size_t total = (size_t)B * Hin * f * Win * f * (C / 4);
   if (total < (1ull << 31))
-    CP_CUDA_CHECK(launch_kernel(upsample_add_kernel<unsigned>, dim3(blocks_for(total)), dim3(TPB), 0, s, (const float4*)in,
-                                (const float4*)w, (const float4*)skip, (float4*)out, B, Hin, Win, C / 4, f));
+    CP_CUDA_CHECK(launch_kernel(ipm < B ? upsample_add_kernel<unsigned, true> : upsample_add_kernel<unsigned, false>, dim3(blocks_for(total)), dim3(TPB), 0, s, (const float4*)in,
+                                (const float4*)w, (const float4*)skip, (float4*)out, B, Hin, Win, C / 4, f, ipm, wstride / 4));
   else
-    CP_CUDA_CHECK(launch_kernel(upsample_add_kernel<size_t>, dim3(blocks_for(total)), dim3(TPB), 0, s, (const float4*)in,
-                                (const float4*)w, (const float4*)skip, (float4*)out, B, Hin, Win, C / 4, f));
+    CP_CUDA_CHECK(launch_kernel(ipm < B ? upsample_add_kernel<size_t, true> : upsample_add_kernel<size_t, false>, dim3(blocks_for(total)), dim3(TPB), 0, s, (const float4*)in,
+                                (const float4*)w, (const float4*)skip, (float4*)out, B, Hin, Win, C / 4, f, ipm, wstride / 4));
   CP_LAUNCH_CHECK("upsample_add_kernel");
   return CP_OK;
 }
@@ -328,7 +333,7 @@ int launch_nhwc_to_nchw(const float* in, float* out, int B, int C, int H, int W,
 }
 
 int launch_group_norm_relu(float* x, const float* gamma, const float* beta, int B, int HW, int C, int stride,
-                           int chanOffset, int groups, float eps, double* ws, cudaStream_t s) {
+                           int chanOffset, int groups, float eps, double* ws, cudaStream_t s, int ipm, long long wstride) {
   if (C > 256 || 256 % C != 0) return fail(CP_ERR_INVALID, "group_norm: C must divide 256");
   if (groups <= 0 || groups > kGnMaxGroups || C % groups) return fail(CP_ERR_INVALID, "group_norm: bad group count");
   double* stats = ws;                                   // [B][groups][2]
@@ -339,8 +344,10 @@ int launch_group_norm_relu(float* x, const float* gamma, const float* beta, int 
   gn_stats_finish_kernel<<<B, 64, 0, s>>>(partial, kGnBlocks, groups, stats);
   CP_LAUNCH_CHECK("gn_stats_finish_kernel");
   size_t total = (size_t)B * HW * C;
-  gn_apply_relu_kernel<<<blocks_for(total), TPB, 0, s>>>(x, gamma, beta, B, HW, C, stride, chanOffset, groups,
-                                                         eps, stats);
+  if (ipm <= 0) ipm = B;
+  // several models in the launch: the model-indexed instantiation
+  (ipm < B ? gn_apply_relu_kernel<true> : gn_apply_relu_kernel<false>)<<<blocks_for(total), TPB, 0, s>>>(
+      x, gamma, beta, B, HW, C, stride, chanOffset, groups, eps, stats, ipm, wstride);
   CP_LAUNCH_CHECK("gn_apply_relu_kernel");
   return CP_OK;
 }

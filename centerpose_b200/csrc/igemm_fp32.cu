@@ -38,7 +38,8 @@ struct DcnTap {
 };
 
 
-template <int BN, int MODE>
+// MULTI: the launch holds several models (IgemmParams::ipm); otherwise the code is that of one model
+template <int BN, int MODE, bool MULTI>
 __global__ void __launch_bounds__(NT, 2) igemm_fp32_kernel(const IgemmParams p) {
   constexpr int TN = BN / 16;
   __shared__ __align__(16) float As[2][BK][BM + APAD];
@@ -49,9 +50,15 @@ __global__ void __launch_bounds__(NT, 2) igemm_fp32_kernel(const IgemmParams p) 
   const int tid = threadIdx.x;
   const int tx = tid & 15;
   const int ty = tid >> 4;
-  const int M = p.B * p.Hout * p.Wout;
-  const int m0 = blockIdx.x * BM;
+  // row blocks are cut per model (IgemmParams::ipm); rows from M on belong to the next model
+  const int Mm = MULTI ? p.ipm * p.Hout * p.Wout : 0;
+  const int bpm = MULTI ? (Mm + BM - 1) / BM : 1;
+  const int model = MULTI ? blockIdx.x / bpm : 0;
+  const int M = MULTI ? (model + 1) * Mm : p.B * p.Hout * p.Wout;
+  const int m0 = MULTI ? model * Mm + (blockIdx.x - model * bpm) * BM : blockIdx.x * BM;
   const int n0 = blockIdx.y * BN;
+  const float* const wgt = MULTI ? p.wgt + (size_t)model * p.wstride : p.wgt;
+  const int n_shared = MULTI ? model * p.ipm : 0;      // NCHW sources are the models' shared input frames
 
   // ---- A-load assignment: this thread fills k-quad `kq` of rows r0 and r0+64
   const int kq = tid & 3;
@@ -80,7 +87,7 @@ __global__ void __launch_bounds__(NT, 2) igemm_fp32_kernel(const IgemmParams p) 
     if (tid < BK * BN / 4) {
       int k = tid / (BN / 4);
       int n4 = tid % (BN / 4);
-      b_reg = __ldg(reinterpret_cast<const float4*>(p.wgt + (size_t)(kt * BK + k) * p.CoutPad + n0 + n4 * 4));
+      b_reg = __ldg(reinterpret_cast<const float4*>(wgt + (size_t)(kt * BK + k) * p.CoutPad + n0 + n4 * 4));
     }
     // ---------------- A tile
     if (MODE == IGEMM_NCHW_SCALAR) {
@@ -99,7 +106,7 @@ __global__ void __launch_bounds__(NT, 2) igemm_fp32_kernel(const IgemmParams p) 
             int iy = row[i].oy * p.stride - p.pad + ky;
             int ix = row[i].ox * p.stride - p.pad + kx;
             if (iy >= 0 && iy < p.Hin && ix >= 0 && ix < p.Win)
-              x = __ldg(p.src[0] + (((size_t)row[i].n * p.Cin + c) * p.Hin + iy) * p.Win + ix);
+              x = __ldg(p.src[0] + (((size_t)(row[i].n - n_shared) * p.Cin + c) * p.Hin + iy) * p.Win + ix);
           }
           v[j] = x;
         }
@@ -246,7 +253,7 @@ __global__ void __launch_bounds__(NT, 2) igemm_fp32_kernel(const IgemmParams p) 
   // ---------------- epilogue
   float bias[TN];
 #pragma unroll
-  for (int j = 0; j < TN; ++j) bias[j] = __ldg(p.bias + n0 + tx * TN + j);
+  for (int j = 0; j < TN; ++j) bias[j] = __ldg((MULTI ? p.bias + (size_t)model * p.wstride : p.bias) + n0 + tx * TN + j);
 
 #pragma unroll
   for (int i = 0; i < 8; ++i) {
@@ -292,24 +299,33 @@ __global__ void __launch_bounds__(NT, 2) igemm_fp32_kernel(const IgemmParams p) 
   }
 }
 
-template <int BN>
-int launch_bn(const IgemmParams& p, cudaStream_t stream) {
-  const int M = p.B * p.Hout * p.Wout;
-  dim3 grid((M + BM - 1) / BM, p.CoutPad / BN);
+template <int BN, bool MULTI>
+int launch_bn_models(const IgemmParams& p, dim3 grid, cudaStream_t stream) {
   switch (p.mode) {
-    case IGEMM_NCHW_SCALAR: CP_CUDA_CHECK(launch_kernel(igemm_fp32_kernel<BN, IGEMM_NCHW_SCALAR>, grid, dim3(NT), 0, stream, p)); break;
-    case IGEMM_NHWC_VEC: CP_CUDA_CHECK(launch_kernel(igemm_fp32_kernel<BN, IGEMM_NHWC_VEC>, grid, dim3(NT), 0, stream, p)); break;
-    case IGEMM_DCN: CP_CUDA_CHECK(launch_kernel(igemm_fp32_kernel<BN, IGEMM_DCN>, grid, dim3(NT), 0, stream, p)); break;
+    case IGEMM_NCHW_SCALAR: CP_CUDA_CHECK(launch_kernel(igemm_fp32_kernel<BN, IGEMM_NCHW_SCALAR, MULTI>, grid, dim3(NT), 0, stream, p)); break;
+    case IGEMM_NHWC_VEC: CP_CUDA_CHECK(launch_kernel(igemm_fp32_kernel<BN, IGEMM_NHWC_VEC, MULTI>, grid, dim3(NT), 0, stream, p)); break;
+    case IGEMM_DCN: CP_CUDA_CHECK(launch_kernel(igemm_fp32_kernel<BN, IGEMM_DCN, MULTI>, grid, dim3(NT), 0, stream, p)); break;
     default: return fail(CP_ERR_INVALID, "igemm: bad mode");
   }
   CP_LAUNCH_CHECK("igemm_fp32_kernel");
   return CP_OK;
 }
 
+template <int BN>
+int launch_bn(const IgemmParams& p0, cudaStream_t stream) {
+  IgemmParams p = p0;
+  p.ipm = model_ipm(p0);
+  const int Mm = p.ipm * p.Hout * p.Wout;
+  dim3 grid((Mm + BM - 1) / BM * (p.B / p.ipm), p.CoutPad / BN);
+  // several models in the launch: the model-indexed instantiations; one model runs the one-model code unchanged
+  return p.B > p.ipm ? launch_bn_models<BN, true>(p, grid, stream) : launch_bn_models<BN, false>(p, grid, stream);
+}
+
 }  // namespace
 
 int launch_igemm_fp32(const IgemmParams& p, cudaStream_t stream) {
   if (p.Kpad % BK != 0) return fail(CP_ERR_INVALID, "igemm: Kpad must be a multiple of 16");
+  if (p.B % model_ipm(p)) return fail(CP_ERR_INVALID, "igemm: batch is not a whole number of models");
   if (p.mode != IGEMM_NCHW_SCALAR) {
     if (p.Cin % BK != 0) return fail(CP_ERR_INVALID, "igemm: Cin must be a multiple of 16 for NHWC modes");
     for (int s = 0; s < p.nsrc; ++s)

@@ -48,7 +48,8 @@ struct PrecTraits<1> {   // tf32 x 3
 };
 
 // ------------------------------------------------------------------ the kernel
-template <int PREC, int MODE, int BN>
+// MULTI: the launch holds several models (IgemmParams::ipm); otherwise the code is that of one model
+template <int PREC, int MODE, int BN, bool MULTI>
 __global__ void __launch_bounds__(UM_THREADS, 1) igemm_umma_kernel(const IgemmParams p, const int STAGES, const int NACC) {
   using T = PrecTraits<PREC>;
   extern __shared__ __align__(1024) unsigned char smem[];
@@ -59,12 +60,16 @@ __global__ void __launch_bounds__(UM_THREADS, 1) igemm_umma_kernel(const IgemmPa
   const uint32_t stage_bytes = A_TILE_BYTES + b_tile_bytes;
 
   const int tid = threadIdx.x, warp = tid >> 5;
-  const int M = p.B * p.Hout * p.Wout;
   // 1-D grid, n tile fastest: the CTAs that share an A row block run back to back and hit it in L2
-  // (gridDim.y would overflow at 65535 row blocks: B = 32 at 512 x 512 has 65536)
+  // (gridDim.y would overflow at 65535 row blocks: B = 32 at 512 x 512 has 65536).  Row blocks are cut per model
+  // (IgemmParams::ipm) so that a block never mixes two models' weights; rows from M on belong to the next model.
   const int n_tiles = p.CoutPad / BN;
   const int n_tile = blockIdx.x % n_tiles;
-  const int m0 = (blockIdx.x / n_tiles) * UM_BM;
+  const int Mm = MULTI ? p.ipm * p.Hout * p.Wout : 0;
+  const int bpm = MULTI ? (Mm + UM_BM - 1) / UM_BM : 1;
+  const int model = MULTI ? (blockIdx.x / n_tiles) / bpm : 0;
+  const int m0 = MULTI ? model * Mm + ((blockIdx.x / n_tiles) - model * bpm) * UM_BM : (blockIdx.x / n_tiles) * UM_BM;
+  const int M = MULTI ? (model + 1) * Mm : p.B * p.Hout * p.Wout;
   const int K = p.kh * p.kw * p.Cin;
   const int KB = (K + T::kElems - 1) / T::kElems;
 
@@ -81,7 +86,8 @@ __global__ void __launch_bounds__(UM_THREADS, 1) igemm_umma_kernel(const IgemmPa
   if (warp < UM_PROD_WARPS) {
     // =========================== A producers: two threads per tile row, four 16-byte chunks each ===============
     {
-      const unsigned char* wsrc = reinterpret_cast<const unsigned char*>(p.wgt_umma) + (size_t)n_tile * KB * b_tile_bytes;
+      const unsigned char* wsrc =
+          reinterpret_cast<const unsigned char*>(p.wgt_umma) + (size_t)model * p.tstride + (size_t)n_tile * KB * b_tile_bytes;
       const int r = tid >> 1;
       const int qbase = (tid & 1) * 4;
       const int m = m0 + r;
@@ -264,7 +270,7 @@ __global__ void __launch_bounds__(UM_THREADS, 1) igemm_umma_kernel(const IgemmPa
       }
     }
     EpiParams ep;
-    ep.bias = p.bias;
+    ep.bias = MULTI ? p.bias + (size_t)model * p.wstride : p.bias;
     ep.residual = p.residual;
     ep.resStride = p.resStride;
     ep.relu = p.relu;
@@ -383,20 +389,22 @@ int launch_pack_umma_weight(const float* src, int ld, int Kreal, int Cout, int C
   return CP_OK;
 }
 
-template <int PREC, int BN>
+template <int PREC, int BN, bool MULTI>
 static int launch_igemm_umma_bn(const IgemmParams& p, int stages, size_t smem, int nacc, cudaStream_t stream,
                                 LaunchInfo* info) {
   void (*kern)(const IgemmParams, const int, const int) =
-      (p.mode == IGEMM_DCN) ? igemm_umma_kernel<PREC, IGEMM_DCN, BN> : igemm_umma_kernel<PREC, IGEMM_NHWC_VEC, BN>;
+      (p.mode == IGEMM_DCN) ? igemm_umma_kernel<PREC, IGEMM_DCN, BN, MULTI> : igemm_umma_kernel<PREC, IGEMM_NHWC_VEC, BN, MULTI>;
   static PerDevice<bool, 2> configured;
   const int slot = p.mode == IGEMM_DCN ? 1 : 0;
   if (!configured.here(slot)) {
     CP_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     configured.here(slot) = true;
   }
-  const int M = p.B * p.Hout * p.Wout;
-  dim3 grid((unsigned)((size_t)(p.CoutPad / BN) * ((M + UM_BM - 1) / UM_BM)));
-  CP_CUDA_CHECK(launch_kernel(kern, grid, dim3(UM_THREADS), smem, stream, p, stages, nacc));
+  IgemmParams q = p;
+  q.ipm = model_ipm(p);
+  const int Mm = q.ipm * p.Hout * p.Wout;
+  dim3 grid((unsigned)((size_t)(p.CoutPad / BN) * ((Mm + UM_BM - 1) / UM_BM) * (p.B / q.ipm)));
+  CP_CUDA_CHECK(launch_kernel(kern, grid, dim3(UM_THREADS), smem, stream, q, stages, nacc));
   CP_LAUNCH_CHECK("igemm_umma_kernel");
   if (info) {
     info->BN = BN;
@@ -406,9 +414,28 @@ static int launch_igemm_umma_bn(const IgemmParams& p, int stages, size_t smem, i
   return CP_OK;
 }
 
+template <bool MULTI>
+static int launch_igemm_umma_prec(const IgemmParams& p, int prec, int bn, int stages, size_t smem, int nacc,
+                                  cudaStream_t stream, LaunchInfo* info) {
+  if (prec == 0) {
+    switch (bn) {
+      case 16: return launch_igemm_umma_bn<0, 16, MULTI>(p, stages, smem, nacc, stream, info);
+      case 32: return launch_igemm_umma_bn<0, 32, MULTI>(p, stages, smem, nacc, stream, info);
+      case 64: return launch_igemm_umma_bn<0, 64, MULTI>(p, stages, smem, nacc, stream, info);
+      default: return launch_igemm_umma_bn<0, 128, MULTI>(p, stages, smem, nacc, stream, info);
+    }
+  }
+  switch (bn) {
+    case 16: return launch_igemm_umma_bn<1, 16, MULTI>(p, stages, smem, nacc, stream, info);
+    case 32: return launch_igemm_umma_bn<1, 32, MULTI>(p, stages, smem, nacc, stream, info);
+    default: return launch_igemm_umma_bn<1, 64, MULTI>(p, stages, smem, nacc, stream, info);
+  }
+}
+
 int launch_igemm_umma(const IgemmParams& p, int prec, cudaStream_t stream, LaunchInfo* info) {
   if (!umma_supported(p, prec)) return fail(CP_ERR_INVALID, "igemm_umma: unsupported shape");
   if (!p.wgt_umma) return fail(CP_ERR_INVALID, "igemm_umma: weight tiles missing");
+  if (p.B % model_ipm(p)) return fail(CP_ERR_INVALID, "igemm_umma: batch is not a whole number of models");
   const int bn = umma_tile_n(p.CoutPad, prec);
   const size_t stage_bytes = (size_t)A_TILE_BYTES + (size_t)bn * ROW_BYTES * (prec == 0 ? 1 : 2);
   const size_t fixed = 512 + 1024 + 2 * (size_t)DRAIN_STAGE_BYTES;     // control block, alignment, epilogue staging
@@ -421,19 +448,9 @@ int launch_igemm_umma(const IgemmParams& p, int prec, cudaStream_t stream, Launc
   const size_t smem = fixed + stages * stage_bytes;
   // tf32x3: K blocks (12 MMAs each) chained in the accumulator before they are added into the fp32 sums
   const int nacc = prec == 1 ? kX3GroupBlocks : 1;
-  if (prec == 0) {
-    switch (bn) {
-      case 16: return launch_igemm_umma_bn<0, 16>(p, stages, smem, nacc, stream, info);
-      case 32: return launch_igemm_umma_bn<0, 32>(p, stages, smem, nacc, stream, info);
-      case 64: return launch_igemm_umma_bn<0, 64>(p, stages, smem, nacc, stream, info);
-      default: return launch_igemm_umma_bn<0, 128>(p, stages, smem, nacc, stream, info);
-    }
-  }
-  switch (bn) {
-    case 16: return launch_igemm_umma_bn<1, 16>(p, stages, smem, nacc, stream, info);
-    case 32: return launch_igemm_umma_bn<1, 32>(p, stages, smem, nacc, stream, info);
-    default: return launch_igemm_umma_bn<1, 64>(p, stages, smem, nacc, stream, info);
-  }
+  // several models in the launch: the model-indexed instantiations; one model runs the one-model code unchanged
+  if (p.B > model_ipm(p)) return launch_igemm_umma_prec<true>(p, prec, bn, stages, smem, nacc, stream, info);
+  return launch_igemm_umma_prec<false>(p, prec, bn, stages, smem, nacc, stream, info);
 }
 
 }  // namespace cp

@@ -119,6 +119,10 @@ struct cp_plan {
   unsigned char* umma_wts = nullptr;
   size_t umma_bytes = 0;
   float* splitk_ws = nullptr;      // conv_tma / dcn_tma split-K partial sums (kSplitkWsFloats)
+  // multi-model plans (cp_plan_create_multi): model m's fp32 weights are wts + m * w_floats, its weight tiles
+  // umma_wts + m * umma_bytes; the arena holds models * B images, model m's at [m * batch, (m + 1) * batch)
+  int models = 1;
+  std::vector<char> model_loaded;
 };
 
 namespace cp {
@@ -362,7 +366,7 @@ int build_graph(cp_plan* P) {
   const cp_config& c = P->cfg;
   Builder b;
   b.P = P;
-  b.B = P->B;
+  b.B = P->B * P->models;
   P->ops.clear();
   P->jobs.clear();
   const int H = P->H, W = P->W;
@@ -548,11 +552,16 @@ int build_graph(cp_plan* P) {
   return CP_OK;
 }
 
-// Kernel parameters of conv op `op` at batch `batch`.  ext[] may hold nulls (family queries); run_op rejects them.
+// Kernel parameters of conv op `op` at `batch` frames (x every model of the plan).  ext[] may hold nulls (family
+// queries); run_op rejects them.
 void igemm_params(const cp_plan* P, const Op& op, int batch, const float* const ext[4], float* const* head_out,
                   IgemmParams* pp) {
   IgemmParams& p = *pp;
   p = IgemmParams{};
+  p.ipm = batch;
+  p.wstride = (long long)P->w_floats;
+  p.tstride = (long long)P->umma_bytes;
+  batch *= P->models;
   p.nsrc = op.nsrc;
   for (int i = 0; i < op.nsrc; ++i) {
     const Act& a = op.src[i];
@@ -621,7 +630,7 @@ int choose_kernels(cp_plan* P) {
     op.kernel = select_conv_kernel(p, P->cfg.precision, pol);
     op.tile_off = P->umma_bytes;
     P->umma_bytes += (op.kernel.wbytes + 1023) / 1024 * 1024;
-    if (int rc = conv_encode(op.kernel, p, P->B, &op.maps)) return rc;
+    if (int rc = conv_encode(op.kernel, p, P->B * P->models, &op.maps)) return rc;
   }
   // The per-head 1x1 convs move into the epilogue of the merged heads conv when that one runs on conv_tma: hidden =
   // relu(conv3x3) never reaches HBM (3.7 GB of writes + 3.7 GB of reads and seven launches at batch 32).  In both
@@ -653,8 +662,14 @@ extern "C" {
 int cp_version(void) { return CP_ABI_VERSION; }
 const char* cp_last_error(void) { return cp::g_last_error.c_str(); }
 
-int cp_plan_create(const cp_config* cfg, cp_plan** out) {
+int cp_plan_create(const cp_config* cfg, cp_plan** out) { return cp_plan_create_multi(cfg, 1, out); }
+
+int cp_plan_create_multi(const cp_config* cfg, int32_t num_models, cp_plan** out) {
   if (!cfg || !out) return fail(CP_ERR_INVALID, "cp_plan_create: null argument");
+  if (num_models < 1 || num_models > CP_MAX_MODELS)
+    return fail(CP_ERR_INVALID, "cp_plan_create_multi: num_models must be in 1..CP_MAX_MODELS");
+  if (cfg->tracking && num_models > 1)
+    return fail(CP_ERR_INVALID, "cp_plan_create_multi: a tracking plan holds one model (multi-category tracking is not supported)");
   if (cfg->arch != CP_ARCH_DLA34 && cfg->arch != CP_ARCH_DLAV1_34)
     return fail(CP_ERR_INVALID, "cp_plan_create: unknown arch");
   if (!known_precision(cfg->precision))
@@ -676,6 +691,8 @@ int cp_plan_create(const cp_config* cfg, cp_plan** out) {
   }
   for (int i = 0; i < cfg->num_heads; ++i) P->cfg.head_names[i] = P->head_names[i].c_str();
   P->B = cfg->max_batch;
+  P->models = num_models;
+  P->model_loaded.assign(num_models, 0);
   P->H = cfg->height;
   P->W = cfg->width;
   if (const char* e = getenv("CP_NO_DCN_TMA")) P->no_dcn_tma = atoi(e) != 0;
@@ -691,11 +708,11 @@ int cp_plan_create(const cp_config* cfg, cp_plan** out) {
   int rc = build_graph(P.get());
   if (rc) return rc;
   CP_CUDA_CHECK(cudaMalloc(&P->act, P->act_floats * sizeof(float)));
-  CP_CUDA_CHECK(cudaMalloc(&P->wts, P->w_floats * sizeof(float)));
-  CP_CUDA_CHECK(cudaMemset(P->wts, 0, P->w_floats * sizeof(float)));
-  CP_CUDA_CHECK(cudaMalloc(&P->gn_stats, sizeof(double) * gn_workspace_doubles(P->B)));
+  CP_CUDA_CHECK(cudaMalloc(&P->wts, P->w_floats * num_models * sizeof(float)));
+  CP_CUDA_CHECK(cudaMemset(P->wts, 0, P->w_floats * num_models * sizeof(float)));
+  CP_CUDA_CHECK(cudaMalloc(&P->gn_stats, sizeof(double) * gn_workspace_doubles(P->B * num_models)));
   if ((rc = choose_kernels(P.get()))) return rc;
-  if (P->umma_bytes) CP_CUDA_CHECK(cudaMalloc(&P->umma_wts, P->umma_bytes));
+  if (P->umma_bytes) CP_CUDA_CHECK(cudaMalloc(&P->umma_wts, P->umma_bytes * num_models));
   if (cfg->precision == CP_PREC_TF32X3 || cfg->precision == CP_PREC_TF32) {
     CP_CUDA_CHECK(cudaMalloc(&P->splitk_ws, kSplitkWsFloats * sizeof(float)));
   }
@@ -718,13 +735,23 @@ int cp_plan_destroy(cp_plan* P) {
   return CP_OK;
 }
 
-int64_t cp_plan_bytes(const cp_plan* P) { return P ? (int64_t)((P->act_floats + P->w_floats) * sizeof(float)) : 0; }
+int64_t cp_plan_bytes(const cp_plan* P) {
+  return P ? (int64_t)((P->act_floats + P->w_floats * P->models) * sizeof(float)) : 0;
+}
+int32_t cp_plan_num_models(const cp_plan* P) { return P ? P->models : 0; }
 int32_t cp_plan_forward_launches(const cp_plan* P) { return P ? P->launches : 0; }
 
 int cp_plan_load_weights(cp_plan* P, const char* const* names, const void* const* ptrs, const int64_t* numel,
                          int32_t n, void* stream_) {
+  return cp_plan_load_weights_model(P, 0, names, ptrs, numel, n, stream_);
+}
+
+int cp_plan_load_weights_model(cp_plan* P, int32_t model, const char* const* names, const void* const* ptrs,
+                               const int64_t* numel, int32_t n, void* stream_) {
   if (!P || !names || !ptrs || !numel) return fail(CP_ERR_INVALID, "cp_plan_load_weights: null argument");
+  if (model < 0 || model >= P->models) return fail(CP_ERR_INVALID, "cp_plan_load_weights_model: model index out of range");
   cudaStream_t s = (cudaStream_t)stream_;
+  float* const wts = P->wts + (size_t)model * P->w_floats;      // this model's copy of the weight storage
   std::map<std::string, WRef> m;
   for (int i = 0; i < n; ++i) {
     std::string k = names[i];
@@ -752,14 +779,14 @@ int cp_plan_load_weights(cp_plan* P, const char* const* names, const void* const
           if ((rc = get(j.bn + ".running_mean", j.Cout, &mu))) return rc;
           if ((rc = get(j.bn + ".running_var", j.Cout, &var))) return rc;
         }
-        if ((rc = launch_pack_bias(cb, g, be, mu, var, P->wts + j.scale, P->wts + j.dst, j.Cout, j.CoutPad, 1e-5f, s)))
+        if ((rc = launch_pack_bias(cb, g, be, mu, var, wts + j.scale, wts + j.dst, j.Cout, j.CoutPad, 1e-5f, s)))
           return rc;
         break;
       }
       case PACK_CONV: {
         const float* w = nullptr;
         if ((rc = get(j.key, (int64_t)j.Cout * j.Cin * j.kh * j.kw, &w))) return rc;
-        if ((rc = launch_pack_conv_weight(w, j.use_scale ? P->wts + j.scale : nullptr, P->wts + j.dst, j.Cout, j.Cin,
+        if ((rc = launch_pack_conv_weight(w, j.use_scale ? wts + j.scale : nullptr, wts + j.dst, j.Cout, j.Cin,
                                           j.kh, j.kw, j.CoutPad, j.Kpad, j.ld, j.colOff, s)))
           return rc;
         break;
@@ -767,13 +794,13 @@ int cp_plan_load_weights(cp_plan* P, const char* const* names, const void* const
       case PACK_UP: {
         const float* w = nullptr;
         if ((rc = get(j.key, (int64_t)j.Cout * j.kh * j.kh, &w))) return rc;
-        if ((rc = launch_pack_up_weight(w, P->wts + j.dst, j.Cout, j.kh, s))) return rc;
+        if ((rc = launch_pack_up_weight(w, wts + j.dst, j.Cout, j.kh, s))) return rc;
         break;
       }
       case PACK_VEC: {
         const float* w = nullptr;
         if ((rc = get(j.key, j.Cout, &w))) return rc;
-        CP_CUDA_CHECK(cudaMemcpyAsync(P->wts + j.dst, w, sizeof(float) * j.Cout, cudaMemcpyDeviceToDevice, s));
+        CP_CUDA_CHECK(cudaMemcpyAsync(wts + j.dst, w, sizeof(float) * j.Cout, cudaMemcpyDeviceToDevice, s));
         break;
       }
     }
@@ -784,9 +811,12 @@ int cp_plan_load_weights(cp_plan* P, const char* const* names, const void* const
     if (op.type != OP_IGEMM || !op.kernel.wbytes) continue;
     IgemmParams p;
     igemm_params(P, op, P->B, no_ext, nullptr, &p);
-    if ((rc = conv_pack(op.kernel, p, op.w_ld, P->umma_wts + op.tile_off, s))) return rc;
+    p.wgt += (size_t)model * P->w_floats;
+    if ((rc = conv_pack(op.kernel, p, op.w_ld, P->umma_wts + (size_t)model * P->umma_bytes + op.tile_off, s))) return rc;
   }
+  P->model_loaded[model] = 1;
   P->loaded = true;
+  for (char l : P->model_loaded) P->loaded = P->loaded && l;
   return CP_OK;
 }
 
@@ -809,6 +839,8 @@ static int run_op(cp_plan* P, size_t idx, int batch, const float* const ext[4], 
                   cp_op_launch* info) {
   int rc;
   const Op& op = P->ops[idx];
+  const int images = batch * P->models;       // every model's images go through one launch
+  const long long wstride = (long long)P->w_floats;
   cp_op_launch li{};
   li.ksplit = 1;
   if (op.fused_away) {          // computed inside the epilogue of the merged heads conv
@@ -834,29 +866,29 @@ static int run_op(cp_plan* P, size_t idx, int batch, const float* const ext[4], 
     }
     case OP_MAXPOOL:
       li.family = CP_FAM_MAXPOOL;
-      if ((rc = launch_maxpool2(P->act + op.src[0].off, P->act + op.out.off, batch, op.src[0].H, op.src[0].W,
+      if ((rc = launch_maxpool2(P->act + op.src[0].off, P->act + op.out.off, images, op.src[0].H, op.src[0].W,
                                 op.src[0].C, s)))
         return rc;
       break;
     case OP_UPADD:
       li.family = CP_FAM_UPADD;
       if ((rc = launch_upsample_add(P->act + op.src[0].off, P->wts + op.upw_off,
-                                    op.has_skip ? P->act + op.skip.off : nullptr, P->act + op.out.off, batch,
-                                    op.src[0].H, op.src[0].W, op.src[0].C, op.f, s)))
+                                    op.has_skip ? P->act + op.skip.off : nullptr, P->act + op.out.off, images,
+                                    op.src[0].H, op.src[0].W, op.src[0].C, op.f, s, batch, wstride)))
         return rc;
       break;
     case OP_GN_RELU:
       li.family = CP_FAM_GN_RELU;
-      if ((rc = launch_group_norm_relu(P->act + op.out.off, P->wts + op.gamma_off, P->wts + op.beta_off, batch,
+      if ((rc = launch_group_norm_relu(P->act + op.out.off, P->wts + op.gamma_off, P->wts + op.beta_off, images,
                                        op.out.H * op.out.W, op.out.C, op.out.stride, 0, op.groups, 1e-5f,
-                                       P->gn_stats, s)))
+                                       P->gn_stats, s, batch, wstride)))
         return rc;
       break;
     case OP_GRU:
       li.family = CP_FAM_GRU;
       if ((rc = launch_gru_gates(P->act + op.gx.off, op.first_step ? nullptr : P->act + op.gh.off,
                                  op.first_step ? nullptr : P->act + op.gprev.off, P->act + op.out.off,
-                                 batch * op.out.H * op.out.W, op.out.C, op.first_step, s)))
+                                 images * op.out.H * op.out.W, op.out.C, op.first_step, s)))
         return rc;
       break;
   }
@@ -872,7 +904,7 @@ static int run_forward(cp_plan* P, int batch, const float* const ext[4], float* 
   struct PdlScope {
     explicit PdlScope(int on) { g_pdl = on; }
     ~PdlScope() { g_pdl = 0; }
-  } pdl_scope(!prof && pdl_wanted((long long)batch * P->H * P->W));
+  } pdl_scope(!prof && pdl_wanted((long long)batch * P->models * P->H * P->W));
   for (size_t i = 0; i < P->ops.size(); ++i) {
     if (prof) {
       cudaEvent_t e;
@@ -959,7 +991,7 @@ int cp_plan_profile(cp_plan* P, int32_t batch, const float* images, const float*
       snprintf(st.name, sizeof(st.name), "%s", op.name.c_str());
       st.kind = (int)op.type * 10 + (op.type == OP_IGEMM ? op.mode : 0);
       cudaEventElapsedTime(&st.ms, ctx.ev[i], ctx.ev[i + 1]);
-      op_work(op, batch, &st.flops, &st.bytes);
+      op_work(op, batch * P->models, &st.flops, &st.bytes);
     }
     *n_stats = n;
   }
@@ -967,8 +999,9 @@ int cp_plan_profile(cp_plan* P, int32_t batch, const float* images, const float*
   return rc;
 }
 
-static void act_desc(const Act& a, cp_act_desc* d) {
-  d->off = a.ext >= 0 || a.C == 0 ? -1 : (int64_t)a.off;
+// `first`: the arena offset of the image the description starts at (model m of a multi-model plan: m * max_batch)
+static void act_desc(const Act& a, cp_act_desc* d, size_t first = 0) {
+  d->off = a.ext >= 0 || a.C == 0 ? -1 : (int64_t)(a.off + first * a.H * a.W * a.stride);
   d->ext = a.ext;
   d->C = a.C;
   d->H = a.H;
@@ -976,10 +1009,16 @@ static void act_desc(const Act& a, cp_act_desc* d) {
   d->stride = a.stride;
 }
 
-int cp_plan_op_desc(const cp_plan* P, int32_t i, cp_op_desc* d) {
+int cp_plan_op_desc(const cp_plan* P, int32_t i, cp_op_desc* d) { return cp_plan_op_desc_model(P, 0, i, d); }
+
+int cp_plan_op_desc_model(const cp_plan* P, int32_t model, int32_t i, cp_op_desc* d) {
   if (!P || !d) return fail(CP_ERR_INVALID, "cp_plan_op_desc: null argument");
+  if (model < 0 || model >= P->models) return fail(CP_ERR_INVALID, "cp_plan_op_desc_model: model index out of range");
   if (i < 0 || i >= (int)P->ops.size()) return fail(CP_ERR_INVALID, "cp_plan_op_desc: op index out of range");
   const Op& op = P->ops[i];
+  const float* const wts = P->wts + (size_t)model * P->w_floats;
+  const size_t first = (size_t)model * P->B;
+  auto act_desc = [first](const Act& a, cp_act_desc* ad) { ::act_desc(a, ad, first); };
   memset(d, 0, sizeof(*d));
   snprintf(d->name, sizeof(d->name), "%s", op.name.c_str());
   d->kind = (int)op.type * 10 + (op.type == OP_IGEMM ? op.mode : 0);
@@ -1008,9 +1047,9 @@ int cp_plan_op_desc(const cp_plan* P, int32_t i, cp_op_desc* d) {
   d->parent = -1;
   switch (op.type) {
     case OP_IGEMM: {
-      d->w = P->wts + op.w_off;
+      d->w = wts + op.w_off;
       d->w_ld = op.w_ld;
-      d->bias = P->wts + op.b_off;
+      d->bias = wts + op.b_off;
       d->family = op.kernel.family;
       d->x3 = op.kernel.x3;
       break;
@@ -1018,14 +1057,14 @@ int cp_plan_op_desc(const cp_plan* P, int32_t i, cp_op_desc* d) {
     case OP_MAXPOOL: d->family = CP_FAM_MAXPOOL; break;
     case OP_UPADD:
       d->family = CP_FAM_UPADD;
-      d->up_w = P->wts + op.upw_off;
+      d->up_w = wts + op.upw_off;
       d->f = op.f;
       d->has_skip = op.has_skip;
       break;
     case OP_GN_RELU:
       d->family = CP_FAM_GN_RELU;
-      d->gamma = P->wts + op.gamma_off;
-      d->beta = P->wts + op.beta_off;
+      d->gamma = wts + op.gamma_off;
+      d->beta = wts + op.beta_off;
       d->groups = op.groups;
       break;
     case OP_GRU:
@@ -1070,12 +1109,43 @@ int cp_plan_run_ops(cp_plan* P, int32_t batch, int32_t first, int32_t last, cons
   return CP_OK;
 }
 
+static int infer_models(cp_plan* P, int32_t batch, const float* images, const float* pre_img, const float* pre_hm,
+                        const float* pre_hm_hp, const cp_decode_params* prm, const double* meta, float* const* heads_out,
+                        float* dets, float* poses, int32_t* n_valid, void* stream);
+
 int cp_infer(cp_plan* P, int32_t batch, const float* images, const float* pre_img, const float* pre_hm,
              const float* pre_hm_hp, const cp_decode_params* prm, const double* meta, float* const* heads_out,
              float* dets, float* poses, int32_t* n_valid, void* stream) {
   if (!P || !images || !prm || !meta || !poses || !n_valid) return fail(CP_ERR_INVALID, "cp_infer: null argument");
   if (!P->loaded) return fail(CP_ERR_NOT_LOADED, "cp_infer: call cp_plan_load_weights first");
   if (batch <= 0 || batch > P->B) return fail(CP_ERR_INVALID, "cp_infer: batch exceeds the plan's max_batch");
+  if (P->models > 1) return fail(CP_ERR_INVALID, "cp_infer: a multi-model plan runs through cp_infer_multi");
+  return infer_models(P, batch, images, pre_img, pre_hm, pre_hm_hp, prm, meta, heads_out, dets, poses, n_valid, stream);
+}
+
+int cp_infer_multi(cp_plan* P, int32_t batch, const float* images, const cp_decode_params* prms, const double* meta,
+                   float* const* heads_out, float* dets, float* poses, int32_t* n_valid, void* stream) {
+  if (!P || !images || !prms || !meta || !poses || !n_valid) return fail(CP_ERR_INVALID, "cp_infer_multi: null argument");
+  if (!P->loaded) return fail(CP_ERR_NOT_LOADED, "cp_infer_multi: call cp_plan_load_weights_model for every model first");
+  if (batch <= 0 || batch > P->B) return fail(CP_ERR_INVALID, "cp_infer_multi: batch exceeds the plan's max_batch");
+  if (P->cfg.tracking) return fail(CP_ERR_INVALID, "cp_infer_multi: tracking plans run through cp_infer");
+  for (int m = 1; m < P->models; ++m) {
+    cp_decode_params a = prms[0], b = prms[m];
+    a.visible_thresh = b.visible_thresh = 0;      // the per-category constants (cuboid_pnp_shell.py:59-66, balance)
+    a.balance = b.balance = 0.f;
+    a.batch = b.batch = a.out_h = b.out_h = a.out_w = b.out_w = 0;      // set by the call
+    if (memcmp(&a, &b, sizeof(a)))
+      return fail(CP_ERR_INVALID, "cp_infer_multi: the models' decode parameters may differ in visible_thresh and balance only");
+  }
+  return infer_models(P, batch, images, nullptr, nullptr, nullptr, prms, meta, heads_out, dets, poses, n_valid, stream);
+}
+
+}  // extern "C"
+
+// forward + one decode over every model's heads; prm[0 .. P->models)
+static int infer_models(cp_plan* P, int32_t batch, const float* images, const float* pre_img, const float* pre_hm,
+                        const float* pre_hm_hp, const cp_decode_params* prm, const double* meta, float* const* heads_out,
+                        float* dets, float* poses, int32_t* n_valid, void* stream) {
   float* hp[CP_MAX_HEADS];
   for (int h = 0; h < P->cfg.num_heads; ++h)
     hp[h] = (heads_out && heads_out[h]) ? heads_out[h] : P->act + P->head_bufs[h].off;
@@ -1099,8 +1169,9 @@ int cp_infer(cp_plan* P, int32_t batch, const float* images, const float* pre_im
     else if (n == "tracking") hd.tracking = hp[h];
     else if (n == "tracking_hp") hd.tracking_hp = hp[h];
   }
-  cp_decode_params q = *prm;
-  q.batch = batch;
+  std::vector<cp_decode_params> qs(prm, prm + P->models);
+  cp_decode_params& q = qs[0];
+  q.batch = batch * P->models;
   q.out_h = P->H / 4;
   q.out_w = P->W / 4;
   q.apply_sigmoid = prm->apply_sigmoid == 2 ? 2 : 1;     // the plan's heads are logits; 2 = opt.mse_loss (raw hm_hp)
@@ -1109,12 +1180,11 @@ int cp_infer(cp_plan* P, int32_t batch, const float* images, const float* pre_im
     // grows only on the first call for a given K / batch (not steady state)
     if (P->decode_ws) cudaFree(P->decode_ws);
     cp_decode_params qmax = q;
-    qmax.batch = P->B;
+    qmax.batch = P->B * P->models;
     size_t cap = cp_decode_workspace_bytes(&qmax);
     CP_CUDA_CHECK(cudaMalloc(&P->decode_ws, cap));
     P->decode_ws_bytes = cap;
   }
-  return cp_decode_pnp(&q, &hd, meta, dets, poses, n_valid, P->decode_ws, P->decode_ws_bytes, stream);
+  return decode_pnp_models(qs.data(), P->models, &hd, meta, dets, poses, n_valid, P->decode_ws, P->decode_ws_bytes,
+                           stream);
 }
-
-}  // extern "C"

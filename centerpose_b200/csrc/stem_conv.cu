@@ -16,7 +16,7 @@ constexpr int ST_HALO_W = ST_W + 6, ST_HALO_H = ST_TY + 6;
 __global__ void __launch_bounds__(ST_TX* ST_TY)
     stem_conv7_kernel(const float* __restrict__ in, const float* __restrict__ wgt, const float* __restrict__ bias,
                       const float* __restrict__ residual, float* __restrict__ out, int B, int Cin, int H, int W,
-                      int relu) {
+                      int relu, int ipm, long long wstride) {
   extern __shared__ __align__(16) float sm[];
   float* ws = sm;                                        // [(ky*7+kx)*Cin + c][16]   (16-byte aligned)
   float* tile = sm + 49 * Cin * 16;                      // [Cin][ST_HALO_H][ST_HALO_W]
@@ -24,6 +24,10 @@ __global__ void __launch_bounds__(ST_TX* ST_TY)
   const int n = blockIdx.z;
   const int x0 = blockIdx.x * ST_W, y0 = blockIdx.y * ST_TY;
   const int nw = 49 * Cin * 16;
+  // image n runs model n / ipm (IgemmParams::ipm) on input frame n % ipm, which every model reads
+  wgt += (size_t)(n / ipm) * wstride;
+  bias += (size_t)(n / ipm) * wstride;
+  const int n_in = n % ipm;
   if (tid == 0) griddep_launch_dependents();      // PDL (common.cuh): weights are constants, the image is not
   for (int i = tid; i < nw; i += ST_TX * ST_TY) ws[i] = __ldg(wgt + i);
   griddep_wait();
@@ -35,7 +39,7 @@ __global__ void __launch_bounds__(ST_TX* ST_TY)
     int c = t / ST_HALO_H;
     int gy = y0 + yy - 3, gx = x0 + xx - 3;
     float v = 0.f;
-    if (gy >= 0 && gy < H && gx >= 0 && gx < W) v = __ldg(in + (((size_t)n * Cin + c) * H + gy) * W + gx);
+    if (gy >= 0 && gy < H && gx >= 0 && gx < W) v = __ldg(in + (((size_t)n_in * Cin + c) * H + gy) * W + gx);
     tile[i] = v;
   }
   __syncthreads();
@@ -122,13 +126,15 @@ constexpr int C3_PLANE = C3_HH * C3_HW + 1;                       // odd plane p
 
 __global__ void __launch_bounds__(C3_TX* C3_TY, 2)
     conv3_c16_kernel(const float* __restrict__ in, int inStride, const float* __restrict__ wgt, const float* __restrict__ bias,
-                     float* __restrict__ out, int outStride, int B, int H, int W, int relu) {
+                     float* __restrict__ out, int outStride, int B, int H, int W, int relu, int ipm, long long wstride) {
   extern __shared__ __align__(16) float sm[];
   float* ws = sm;                                  // [(ky*3+kx)*16 + c][16]
   float* tile = sm + 9 * 16 * 16;                  // [16 planes][C3_PLANE]
   const int tid = threadIdx.y * C3_TX + threadIdx.x;
   const int n = blockIdx.z;
   const int x0 = blockIdx.x * C3_W, y0 = blockIdx.y * C3_TY;
+  wgt += (size_t)(n / ipm) * wstride;      // model n / ipm (IgemmParams::ipm)
+  bias += (size_t)(n / ipm) * wstride;
   if (tid == 0) griddep_launch_dependents();      // PDL (common.cuh)
   for (int i = tid; i < 9 * 16 * 16; i += C3_TX * C3_TY) ws[i] = __ldg(wgt + i);
   griddep_wait();
@@ -230,7 +236,7 @@ int launch_conv3_c16(const IgemmParams& p, cudaStream_t s) {
   dim3 grid((p.Win + C3_W - 1) / C3_W, (p.Hin + C3_TY - 1) / C3_TY, p.B);
   dim3 block(C3_TX, C3_TY);
   CP_CUDA_CHECK(launch_kernel(conv3_c16_kernel, grid, block, smem, s, p.src[0], p.srcStride[0], p.wgt, p.bias, p.out, p.outStride,
-                              p.B, p.Hin, p.Win, p.relu));
+                              p.B, p.Hin, p.Win, p.relu, model_ipm(p), p.wstride));
   CP_LAUNCH_CHECK("conv3_c16_kernel");
   return CP_OK;
 }
@@ -252,7 +258,7 @@ int launch_stem_conv(const IgemmParams& p, cudaStream_t s) {
   dim3 grid((p.Win + ST_W - 1) / ST_W, (p.Hin + ST_TY - 1) / ST_TY, p.B);
   dim3 block(ST_TX, ST_TY);
   CP_CUDA_CHECK(launch_kernel(stem_conv7_kernel, grid, block, smem, s, p.src[0], p.wgt, p.bias, p.residual, p.out, p.B, p.Cin,
-                              p.Hin, p.Win, p.relu));
+                              p.Hin, p.Win, p.relu, model_ipm(p), p.wstride));
   CP_LAUNCH_CHECK("stem_conv7_kernel");
   return CP_OK;
 }

@@ -366,8 +366,9 @@ __device__ __forceinline__ void epilogue_row(const EpiParams& e, float (&vv)[NV]
 
 // Split-K, second half (conv_tma_splitk_finish, dcn_tma_splitk_finish): one thread per (tile row i, 4 columns) of an
 // (m, n) tile adds the ksplit partial sums ([mn tile][split][BN / 4][rows] float4, row-fastest: coalesced) in split
-// order and runs the epilogue.  row_at(mn, i, &n, &oy, &ox) maps the row to its output position (false: none).
-template <class Params, class RowAt>
+// order and runs the epilogue.  row_at(mn, i, &n, &oy, &ox) maps the row to its output position (false: none).  MULTI
+// (several models in the launch): image n takes the bias of model n / p.ipm.
+template <bool MULTI, class Params, class RowAt>
 __device__ __forceinline__ void splitk_finish(const Params& p, int rows, long long mn_tiles, RowAt row_at) {
   griddep_launch_dependents();
   griddep_wait();
@@ -389,7 +390,7 @@ __device__ __forceinline__ void splitk_finish(const Params& p, int rows, long lo
   int n, oy, ox;
   if (!row_at(mn, i, &n, &oy, &ox)) return;
   const int n_tile = (int)(mn % (p.CoutPad / p.BN));
-  const EpiParams e{p.bias, p.residual, p.resStride, p.relu, p.res_after_relu, p.round_tf32, p.out, p.outStride, p.out_nchw,
+  const EpiParams e{MULTI ? p.bias + (size_t)(n / p.ipm) * p.wstride : p.bias, p.residual, p.resStride, p.relu, p.res_after_relu, p.round_tf32, p.out, p.outStride, p.out_nchw,
                     p.Cout, p.CoutPad, p.H, p.W};
   float v[4] = {a.x, a.y, a.z, a.w};
   epilogue_row<4>(e, v, true, (n * p.H + oy) * p.W + ox, n, oy, ox, n_tile * p.BN + c4 * 4, min(p.Cout, (n_tile + 1) * p.BN));

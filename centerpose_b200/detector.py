@@ -9,6 +9,7 @@ rebuilding the reference's Python result structures from the fixed-shape pose
 records (`records_to_results`).  `run_batch()` is the batched entry point the
 reference does not have (B = 32 / 256 configurations of BASELINE.json).
 """
+import copy
 import json
 import os
 import time
@@ -17,8 +18,8 @@ import numpy as np
 import torch
 
 from . import _lib
-from .engine import decode_params, decode_pnp, make_meta, preprocess, preprocess_ragged
-from .model import create_model, load_model
+from .engine import Engine, decode_params, decode_pnp, make_meta, preprocess, preprocess_ragged
+from .model import _load_checkpoint, create_model, load_model
 from .tracker import Tracker, tracks_to_results
 
 
@@ -576,24 +577,8 @@ class ObjectPoseDetector(object):
         else:
             if new_video is not None:
                 raise ValueError("run_batch: new_video needs a list of slot frames")
-            dev = self.opt.device
-            if isinstance(frames, np.ndarray):
-                frames = torch.from_numpy(frames)
-            if frames.dtype == torch.uint8:
-                B, sh, sw, _ = frames.shape
-                fr = frames.to(dev, non_blocking=True)
-                x = preprocess(fr, self.opt.input_h, self.opt.input_w, self.opt.mean, self.opt.std)
-                c, s = np.array([sw / 2., sh / 2.], np.float32), float(max(sh, sw))
-                iw, ih = sw, sh
-            else:
-                x = frames.to(dev)
-                B, _, ih, iw = x.shape
-                c, s = np.array([iw / 2., ih / 2.], np.float32), float(max(ih, iw))
-            meta = make_meta(B, c, s, iw, ih, camera_matrix).numpy()
-            # the batched path pre-processes at scale 1 (what every shipped configuration uses); results of a multi-scale
-            # opt are those of test_scales[0] (object_pose.py:188), which run() reproduces frame by frame
-            if float(self.scales[0]) != 1.0:
-                raise NotImplementedError("run_batch pre-processes at scale 1; use run() for test_scales[0] != 1")
+            x, meta, c, s = self._array_input(frames, camera_matrix)
+            B = x.shape[0]
             if track:
                 if pre_dets is not None and len(pre_dets) != B:
                     raise ValueError("run_batch: %d pre_dets lists for %d streams" % (len(pre_dets), B))
@@ -605,6 +590,29 @@ class ObjectPoseDetector(object):
                                       pre_hms, pre_hm_hp, poses=out[0] if out is not None else None,
                                       n_valid=out[1] if out is not None else None)
         return _returned((poses, n_valid), to_host)
+
+    def _array_input(self, frames, camera_matrix):
+        """run_batch's array form: uint8 [B,H,W,3] frames (or pre-processed fp32 [B,3,h,w]) -> (x [B,3,h,w] fp32 CUDA,
+        meta rows [B,16] float64 host, c, s) with the fix_res affine of the frame size."""
+        dev = self.opt.device
+        if isinstance(frames, np.ndarray):
+            frames = torch.from_numpy(frames)
+        if frames.dtype == torch.uint8:
+            B, sh, sw, _ = frames.shape
+            fr = frames.to(dev, non_blocking=True)
+            x = preprocess(fr, self.opt.input_h, self.opt.input_w, self.opt.mean, self.opt.std)
+            c, s = np.array([sw / 2., sh / 2.], np.float32), float(max(sh, sw))
+            iw, ih = sw, sh
+        else:
+            x = frames.to(dev)
+            B, _, ih, iw = x.shape
+            c, s = np.array([iw / 2., ih / 2.], np.float32), float(max(ih, iw))
+        meta = make_meta(B, c, s, iw, ih, camera_matrix).numpy()
+        # the batched path pre-processes at scale 1 (what every shipped configuration uses); results of a multi-scale
+        # opt are those of test_scales[0] (object_pose.py:188), which run() reproduces frame by frame
+        if float(self.scales[0]) != 1.0:
+            raise NotImplementedError("run_batch pre-processes at scale 1; use run() for test_scales[0] != 1")
+        return x, meta, c, s
 
     # ------------------------------------------------------------------ ragged batches (lists of frames)
     def _ragged_input(self, frames, camera_matrix):
@@ -744,3 +752,105 @@ class ObjectPoseDetector(object):
 
 
 detector_factory = {"object_pose": ObjectPoseDetector}
+
+
+# ----------------------------------------------------------------------------- several categories at once
+class MultiCategoryDetector(ObjectPoseDetector):
+    """One checkpoint per object category (upstream publishes one per category), all run over the same frames by one
+    multi-model plan: every layer is one launch for all categories, followed by one decode.
+
+    checkpoints: ordered mapping category -> checkpoint path, loaded with load_model (and its weights_only rule).  All
+    checkpoints must have opt's architecture, heads and head_conv.  Category c decodes with decode_params(opt, c=c)
+    (its visible_thresh and balance coefficient).  Only run_batch is offered: tracking, run(), process() and the result
+    writers are single-category and raise here.  The checkpoints' weights stay on the host; on the device they exist
+    only in the plan."""
+
+    def __init__(self, opt, checkpoints):
+        if getattr(opt, "tracking_task", False):
+            raise ValueError("MultiCategoryDetector: tracking with several categories is not supported")
+        cats = list(checkpoints.keys())
+        if not 1 <= len(cats) <= _lib.CP_MAX_MODELS:
+            raise ValueError("MultiCategoryDetector: 1..%d categories, got %d" % (_lib.CP_MAX_MODELS, len(cats)))
+        for c in cats:
+            decode_params(opt, c=c)                  # raises on an unknown category
+        weights = []
+        for c in cats:
+            m = create_model(opt.arch, opt.heads, opt.head_conv, opt)
+            _check_checkpoint(m, checkpoints[c], c)
+            m = load_model(m, checkpoints[c])
+            weights.append({k: v.detach().cpu() for k, v in m.state_dict().items()})
+        self._plan_cfg = dict(arch=m._arch(), heads=m.heads, head_conv=m.head_conv,
+                              tracking_task_gru=m.use_convGRU and m.tracking_task, precision=m.precision)
+        base = copy.copy(opt)
+        base.load_model = ""
+        super().__init__(base, model=m)
+        self.model = None                            # the plan holds the weights; only the host copies are kept
+        self.categories = cats
+        self._weights = weights
+        self._prms = [decode_params(opt, c=c, test_scale=1.0) for c in cats]
+        self._eng = None
+
+    def engine(self, batch, height, width):
+        """The multi-model plan for this input shape (created on first use, rebuilt for a larger batch)."""
+        eng = self._eng
+        if eng is None or eng.max_batch < batch or (eng.height, eng.width) != (height, width):
+            if eng is not None:
+                eng.close()
+            dev = torch.device(self.opt.device)
+            c = self._plan_cfg
+            eng = Engine(c["arch"], c["heads"], c["head_conv"], max(batch, 1), height, width,
+                         dev.index if dev.index is not None else torch.cuda.current_device(),
+                         tracking_task_gru=c["tracking_task_gru"], precision=c["precision"], models=len(self._weights))
+            for i, sd in enumerate(self._weights):
+                eng.load_state_dict(sd, model=i)
+            self._eng = eng
+        return eng
+
+    def run_batch(self, frames, camera_matrix, to_host=True, out=None):
+        """run_batch of ObjectPoseDetector (a uint8 [B,H,W,3] array, or a list of mixed-size frames with one camera or
+        one per frame) for every category: the frames are pre-processed once.  Returns (poses [M,B,K,192],
+        n_valid [M,B]) in `categories` order, also for M = 1; out: optional (poses, n_valid) CUDA tensors of those
+        shapes to write into."""
+        if isinstance(frames, (list, tuple)):
+            check_frames(frames, allow_idle=False)
+            x, meta, _ = self._ragged_input(frames, camera_matrix)
+        else:
+            x, meta, _, _ = self._array_input(frames, camera_matrix)
+        eng = self.engine(x.shape[0], x.shape[2], x.shape[3])
+        if len(self._prms) > 1:
+            _, poses, n_valid = eng.infer(x, self._meta_rows(meta), self._prms,
+                                          poses=out[0] if out is not None else None,
+                                          n_valid=out[1] if out is not None else None)
+        else:             # a one-model plan: cp_infer, outputs [B, ...] -> [1, B, ...]
+            _, poses, n_valid = eng.infer(x, self._meta_rows(meta), self._prms[0],
+                                          poses=out[0][0] if out is not None else None,
+                                          n_valid=out[1][0] if out is not None else None)
+            poses, n_valid = out if out is not None else (poses.unsqueeze(0), n_valid.unsqueeze(0))
+        return _returned((poses, n_valid), to_host)
+
+
+def _single_category(name):
+    def refuse(self, *a, **k):
+        raise NotImplementedError("MultiCategoryDetector.%s: only run_batch runs several categories; use an "
+                                  "ObjectPoseDetector per category" % name)
+    refuse.__name__ = name
+    return refuse
+
+
+for _name in ("run", "process", "pre_process", "build_dict_out", "show_results", "save_results", "save_results_eval",
+              "reset_tracking"):
+    setattr(MultiCategoryDetector, _name, _single_category(_name))
+del _name
+
+
+def _check_checkpoint(model, path, category):
+    """The checkpoint must hold exactly the tensors of `model` (same architecture, heads and head_conv): one plan runs
+    every category's weights through the same schedule."""
+    sd = _load_checkpoint(path)["state_dict"]
+    got = {(k[7:] if k.startswith("module") and not k.startswith("module_list") else k): tuple(v.shape)
+           for k, v in sd.items()}
+    want = {k: tuple(v.shape) for k, v in model.state_dict().items()}
+    if got != want:
+        diff = sorted(set(got.items()) ^ set(want.items()))[:4]
+        raise ValueError("MultiCategoryDetector: the checkpoint of '%s' (%s) does not match the architecture, heads and "
+                         "head_conv of opt (first differences: %s)" % (category, path, diff))

@@ -134,9 +134,14 @@ def _device_view(ptr, n, device):
 
 
 class Engine(object):
+    """One native plan.  models > 1 (cp_plan_create_multi): `models` checkpoints of the same architecture run over the
+    same frames, every layer one launch for all of them; load each with load_state_dict(sd, model=m).  forward / infer
+    outputs then carry a leading [models] axis."""
+
     def __init__(self, arch, heads, head_conv, max_batch, height, width, device_index, tracking=False,
-                 tracking_task_gru=False, precision="fp32"):
+                 tracking_task_gru=False, precision="fp32", models=1):
         self.L = _lib.load()
+        self.models = int(models)
         self.heads = dict(heads)
         self.head_names = list(heads.keys())
         self.max_batch, self.height, self.width = int(max_batch), int(height), int(width)
@@ -158,7 +163,7 @@ class Engine(object):
         self._cfg = cfg
         plan = ctypes.c_void_p()
         with torch.cuda.device(self.device):
-            _lib.check(self.L.cp_plan_create(ctypes.byref(cfg), ctypes.byref(plan)), "cp_plan_create")
+            _lib.check(self.L.cp_plan_create_multi(ctypes.byref(cfg), self.models, ctypes.byref(plan)), "cp_plan_create")
         self.plan = plan
         self.weights_sig = None
         self.forward_launches = int(self.L.cp_plan_forward_launches(plan))
@@ -175,7 +180,7 @@ class Engine(object):
         except Exception:
             pass
 
-    def load_state_dict(self, sd):
+    def load_state_dict(self, sd, model=0):
         names, ptrs, numel, keep = [], [], [], []
         for k, v in sd.items():
             if not torch.is_tensor(v) or not v.dtype.is_floating_point:
@@ -190,7 +195,7 @@ class Engine(object):
         a_ptrs = (ctypes.c_void_p * n)(*ptrs)
         a_numel = (ctypes.c_int64 * n)(*numel)
         with torch.cuda.device(self.device):
-            rc = self.L.cp_plan_load_weights(self.plan, a_names, a_ptrs, a_numel, n, _stream())
+            rc = self.L.cp_plan_load_weights_model(self.plan, int(model), a_names, a_ptrs, a_numel, n, _stream())
             _lib.check(rc, "cp_plan_load_weights")
             torch.cuda.current_stream().synchronize()   # borrowed tensors may be freed after this
 
@@ -227,15 +232,22 @@ class Engine(object):
             raise ValueError("%s must be a contiguous %s tensor of shape %s on %s" % (name, dtype, tuple(shape), self.device))
         return t
 
+    def _lead(self, B):
+        """Leading axes of every output: (B,) or, on a multi-model plan, (models, B)."""
+        return (self.models, B) if self.models > 1 else (B,)
+
+    def _head_shape(self, B, c):
+        return self._lead(B) + (c, self.height // 4, self.width // 4)
+
     def forward(self, x, pre_img=None, pre_hm=None, pre_hm_hp=None, out=None):
-        """Head logits {name: [B,C,H/4,W/4] fp32 CUDA}."""
+        """Head logits {name: [B,C,H/4,W/4] fp32 CUDA} ([models,B,C,H/4,W/4] on a multi-model plan)."""
         B, xs = self._check_inputs(x, pre_img, pre_hm, pre_hm_hp)
         if out is None:
-            out = {n: torch.empty((B, c, self.height // 4, self.width // 4), dtype=torch.float32, device=self.device)
+            out = {n: torch.empty(self._head_shape(B, c), dtype=torch.float32, device=self.device)
                    for n, c in self.heads.items()}
         else:
             for n, c in self.heads.items():
-                self._out_tensor(out[n], "out[%s]" % n, (B, c, self.height // 4, self.width // 4), torch.float32)
+                self._out_tensor(out[n], "out[%s]" % n, self._head_shape(B, c), torch.float32)
         hp = (ctypes.c_void_p * len(self.head_names))(*[out[n].data_ptr() for n in self.head_names])
         with torch.cuda.device(self.device):
             rc = self.L.cp_forward(self.plan, B, _ptr(xs[0]), _ptr(xs[1]), _ptr(xs[2]), _ptr(xs[3]), hp, _stream())
@@ -245,7 +257,7 @@ class Engine(object):
     def profile(self, x, pre_img=None, pre_hm=None, pre_hm_hp=None):
         """One forward with CUDA events between the ops: list of dicts(name, kind, ms, flops, bytes)."""
         B, xs = self._check_inputs(x, pre_img, pre_hm, pre_hm_hp)
-        out = {n: torch.empty((B, c, self.height // 4, self.width // 4), dtype=torch.float32, device=self.device)
+        out = {n: torch.empty(self._head_shape(B, c), dtype=torch.float32, device=self.device)
                for n, c in self.heads.items()}
         hp = (ctypes.c_void_p * len(self.head_names))(*[out[n].data_ptr() for n in self.head_names])
         n_ops = int(self.L.cp_plan_num_ops(self.plan))
@@ -263,12 +275,13 @@ class Engine(object):
     def _act(a):
         return dict(off=int(a.off), ext=int(a.ext), C=int(a.C), H=int(a.H), W=int(a.W), stride=int(a.stride))
 
-    def op_descs(self):
-        """cp_plan_op_desc of every op: list of dicts (device pointers as ints, activations as dicts of cp_act_desc)."""
+    def op_descs(self, model=0):
+        """cp_plan_op_desc_model of every op: list of dicts (device pointers as ints, activations as dicts of
+        cp_act_desc), as model `model` sees them at max_batch."""
         out = []
         for i in range(int(self.L.cp_plan_num_ops(self.plan))):
             d = _lib.CpOpDesc()
-            _lib.check(self.L.cp_plan_op_desc(self.plan, i, ctypes.byref(d)), "cp_plan_op_desc")
+            _lib.check(self.L.cp_plan_op_desc_model(self.plan, int(model), i, ctypes.byref(d)), "cp_plan_op_desc")
             r = {}
             for name, _ in _lib.CpOpDesc._fields_:
                 v = getattr(d, name)
@@ -298,7 +311,7 @@ class Engine(object):
         Returns one dict(family, BN, ksplit, grid) per op."""
         B, xs = self._check_inputs(x, pre_img, pre_hm, pre_hm_hp)
         for n, c in self.heads.items():
-            self._out_tensor(out[n], "out[%s]" % n, (B, c, self.height // 4, self.width // 4), torch.float32)
+            self._out_tensor(out[n], "out[%s]" % n, self._head_shape(B, c), torch.float32)
         hp = (ctypes.c_void_p * len(self.head_names))(*[out[n].data_ptr() for n in self.head_names])
         n = max(0, last - first)
         info = (_lib.CpOpLaunch * max(1, n))()
@@ -311,33 +324,48 @@ class Engine(object):
 
     def infer(self, x, meta, prm, pre_img=None, pre_hm=None, pre_hm_hp=None, heads_out=None, want_dets=False,
               poses=None, n_valid=None, dets=None):
-        """forward + decode + PnP in one native call.  Returns (dets|None, poses, n_valid)."""
+        """forward + decode + PnP in one native call.  Returns (dets|None, poses, n_valid).  On a multi-model plan `prm`
+        is one cp_decode_params per model (cp_infer_multi) and the outputs are [models, B, ...]."""
         B, xs = self._check_inputs(x, pre_img, pre_hm, pre_hm_hp)
+        lead = self._lead(B)
         if not torch.is_tensor(meta) or tuple(meta.shape) != (B, _lib.CP_META_DOUBLES):
             raise ValueError("meta must be a [%d,%d] tensor (make_meta)" % (B, _lib.CP_META_DOUBLES))
         if meta.device != self.device or meta.dtype != torch.float64 or not meta.is_contiguous():
             meta = meta.to(self.device, torch.float64).contiguous()
+        if self.models > 1:
+            prms = list(prm)
+            if len(prms) != self.models:
+                raise ValueError("a plan of %d models needs %d decode parameter sets, got %d" % (self.models, self.models,
+                                                                                                len(prms)))
+            K = prms[0].K
+        else:
+            K = prm.K
         if poses is None:
-            poses = torch.empty((B, prm.K, _lib.CP_POSE_RECORD), dtype=torch.float32, device=self.device)
+            poses = torch.empty(lead + (K, _lib.CP_POSE_RECORD), dtype=torch.float32, device=self.device)
         else:
-            self._out_tensor(poses, "poses", (B, prm.K, _lib.CP_POSE_RECORD), torch.float32)
+            self._out_tensor(poses, "poses", lead + (K, _lib.CP_POSE_RECORD), torch.float32)
         if n_valid is None:
-            n_valid = torch.empty((B,), dtype=torch.int32, device=self.device)
+            n_valid = torch.empty(lead, dtype=torch.int32, device=self.device)
         else:
-            self._out_tensor(n_valid, "n_valid", (B,), torch.int32)
+            self._out_tensor(n_valid, "n_valid", lead, torch.int32)
         if want_dets and dets is None:
-            dets = torch.empty((B, prm.K, _lib.CP_DETS_RECORD), dtype=torch.float32, device=self.device)
+            dets = torch.empty(lead + (K, _lib.CP_DETS_RECORD), dtype=torch.float32, device=self.device)
         elif dets is not None:
-            self._out_tensor(dets, "dets", (B, prm.K, _lib.CP_DETS_RECORD), torch.float32)
+            self._out_tensor(dets, "dets", lead + (K, _lib.CP_DETS_RECORD), torch.float32)
         hp = None
         if heads_out is not None:
             for n, c in self.heads.items():
-                self._out_tensor(heads_out[n], "heads_out[%s]" % n, (B, c, self.height // 4, self.width // 4), torch.float32)
+                self._out_tensor(heads_out[n], "heads_out[%s]" % n, self._head_shape(B, c), torch.float32)
             hp = (ctypes.c_void_p * len(self.head_names))(*[heads_out[n].data_ptr() for n in self.head_names])
         with torch.cuda.device(self.device):
-            rc = self.L.cp_infer(self.plan, B, _ptr(xs[0]), _ptr(xs[1]), _ptr(xs[2]), _ptr(xs[3]), ctypes.byref(prm),
-                                 _ptr(meta), hp, _ptr(dets), _ptr(poses), _ptr(n_valid), _stream())
-        _lib.check(rc, "cp_infer")
+            if self.models > 1:
+                arr = (_lib.CpDecodeParams * self.models)(*prms)
+                rc = self.L.cp_infer_multi(self.plan, B, _ptr(xs[0]), arr, _ptr(meta), hp, _ptr(dets), _ptr(poses),
+                                           _ptr(n_valid), _stream())
+            else:
+                rc = self.L.cp_infer(self.plan, B, _ptr(xs[0]), _ptr(xs[1]), _ptr(xs[2]), _ptr(xs[3]), ctypes.byref(prm),
+                                     _ptr(meta), hp, _ptr(dets), _ptr(poses), _ptr(n_valid), _stream())
+        _lib.check(rc, "cp_infer_multi" if self.models > 1 else "cp_infer")
         return dets, poses, n_valid
 
 

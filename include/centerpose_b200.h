@@ -80,6 +80,7 @@ enum cp_precision {
 #define CP_META_DOUBLES 16  /* doubles per image in `meta`           */
 #define CP_MAX_K 128
 #define CP_MAX_CLASSES 80   /* hm channels the decode stage merges (decode.py:52-68 _topk) */
+#define CP_MAX_MODELS 16    /* checkpoints one multi-model plan holds (cp_plan_create_multi) */
 
 typedef struct cp_plan cp_plan;
 
@@ -101,6 +102,21 @@ typedef struct cp_config {
  * activation arena + packed-weight storage on cfg->device.  Synchronous. */
 int cp_plan_create(const cp_config* cfg, cp_plan** out);
 int cp_plan_destroy(cp_plan* plan);
+
+/* ---- multi-model plans: several checkpoints of one architecture (one per object category) over the same frames ----
+ * cp_plan_create_multi builds one schedule for `num_models` models (1..CP_MAX_MODELS; cp_plan_create is this call with
+ * 1).  Every op is ONE launch for all models: model m's weights are the m-th copy of the weight storage, and image b of
+ * model m is image m * batch + b of each launch, where batch is the number of frames of the call.  So the activations
+ * of a call at `batch` frames are [num_models * batch, ...] and model m's are a contiguous slice of them.
+ *   - images (and pre_img ...) and meta rows are [batch, ...]: every model reads the same frames, nothing is copied.
+ *   - head_out[i] of cp_forward / cp_plan_profile / cp_plan_run_ops is [num_models, batch, C, H/4, W/4].
+ *   - tracking configs take num_models == 1 only.
+ * cp_plan_load_weights_model fills model `model` (cp_plan_load_weights fills model 0); running before every model is
+ * loaded returns CP_ERR_NOT_LOADED. */
+int cp_plan_create_multi(const cp_config* cfg, int32_t num_models, cp_plan** out);
+int cp_plan_load_weights_model(cp_plan* plan, int32_t model, const char* const* names, const void* const* dev_ptrs,
+                               const int64_t* numel, int32_t n, void* stream);
+int32_t cp_plan_num_models(const cp_plan* plan);
 
 /* Ingest a reference state_dict (Appendix A of SURVEY.md).  names[i] is the
  * reference key (an optional leading "module." is ignored, model.py:43-47),
@@ -197,6 +213,10 @@ typedef struct cp_op_launch {
   int32_t grid;             /* CTAs of the main kernel (tensor-core families; 0 otherwise)                         */
 } cp_op_launch;
 int cp_plan_op_desc(const cp_plan* plan, int32_t i, cp_op_desc* out);
+/* op i as model `model` of a multi-model plan sees it: its weight, bias, up-sample and GroupNorm pointers, and
+ * activation offsets moved to its images for a call at the plan's max_batch (model m's images start at image
+ * m * max_batch; at a smaller batch they start at m * batch).  cp_plan_op_desc is this call with model 0. */
+int cp_plan_op_desc_model(const cp_plan* plan, int32_t model, int32_t i, cp_op_desc* out);
 int cp_plan_arena(const cp_plan* plan, float** act, int64_t* floats);
 /* `info` (may be NULL) receives last - first records. */
 int cp_plan_run_ops(cp_plan* plan, int32_t batch, int32_t first, int32_t last, const float* images, const float* pre_img,
@@ -274,6 +294,13 @@ int cp_infer(cp_plan* plan, int32_t batch, const float* images, const float* pre
              const float* pre_hm, const float* pre_hm_hp, const cp_decode_params* prm,
              const double* meta, float* const* heads_out, float* dets, float* poses,
              int32_t* n_valid, void* stream);
+
+/* cp_infer for every model of a multi-model plan: one forward and one decode for all of them.  prms[num_models]: the
+ * decode parameters of each model; they may differ in visible_thresh and balance only (else CP_ERR_INVALID).  meta is
+ * [batch] (the frames); heads_out[i] (optional) is [num_models, batch, C, H/4, W/4]; dets (optional)
+ * [num_models, batch, K, CP_DETS_RECORD]; poses [num_models, batch, K, CP_POSE_RECORD]; n_valid [num_models, batch]. */
+int cp_infer_multi(cp_plan* plan, int32_t batch, const float* images, const cp_decode_params* prms, const double* meta,
+                   float* const* heads_out, float* dets, float* poses, int32_t* n_valid, void* stream);
 
 /* Offsets (in floats) inside one CP_POSE_RECORD slot. */
 enum cp_pose_field {
