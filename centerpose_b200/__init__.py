@@ -4,13 +4,14 @@ Public surface (mirrors the reference's, see INTEGRATION.md):
     create_model, load_model, save_model      <- lib.models.model
     ObjectPoseDetector, detector_factory      <- lib.detectors.*
     MultiCategoryDetector                     <- one checkpoint per category, all in one plan
+    MultiCategoryTracker                      <- the same for CenterPoseTrack checkpoints, one tracker for all
     decode_pnp, decode_params, make_meta      <- fused decode / grouping / PnP stage
     dcn_v2_forward / dcn_v2_backward          <- `_ext.dcn_v2_forward` / `_ext.dcn_v2_backward`
 The hot path lives in libcenterpose_b200.so (include/centerpose_b200.h); there is
 no PyTorch or CPU fallback.
 """
 from .model import create_model, load_model, save_model, DLASegB200          # noqa: F401
-from .detector import MultiCategoryDetector, ObjectPoseDetector, detector_factory  # noqa: F401
+from .detector import MultiCategoryDetector, MultiCategoryTracker, ObjectPoseDetector, detector_factory  # noqa: F401
 from .engine import Engine, InferGraph, decode_pnp, decode_params, make_meta, dcn_v2_forward, dcn_v2_backward, preprocess, preprocess_ragged, conv2d_nhwc  # noqa: F401
 from .opts import default_opt                                                # noqa: F401
 from .tracker import Tracker, track_to_dict, tracks_to_results               # noqa: F401

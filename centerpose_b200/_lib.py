@@ -55,6 +55,7 @@ EXPORTS = [
     "cp_tracker_render_ex", "cp_tracker_seed", "cp_plan_op_desc", "cp_plan_arena", "cp_plan_run_ops",
     "cp_preprocess_ragged", "cp_tracker_step_ex", "cp_tracker_render_ex2", "cp_tracker_seed_ex",
     "cp_plan_create_multi", "cp_plan_load_weights_model", "cp_plan_num_models", "cp_plan_op_desc_model", "cp_infer_multi",
+    "cp_plan_create_multi_track", "cp_infer_multi_track", "cp_tracker_create_multi",
 ]
 
 # cp_op_family
@@ -199,6 +200,10 @@ def load():
     L.cp_plan_num_models.argtypes = [vp]
     L.cp_plan_op_desc_model.argtypes = [vp, i32, i32, ctypes.POINTER(CpOpDesc)]
     L.cp_infer_multi.argtypes = [vp, i32, vp, ctypes.POINTER(CpDecodeParams), vp, ctypes.POINTER(vp), vp, vp, vp, vp]
+    L.cp_plan_create_multi_track.argtypes = [ctypes.POINTER(CpConfig), i32, ctypes.POINTER(vp)]
+    L.cp_infer_multi_track.argtypes = [vp, i32, vp, vp, vp, vp, ctypes.POINTER(CpDecodeParams), vp, ctypes.POINTER(vp), vp,
+                                       vp, vp, vp]
+    L.cp_tracker_create_multi.argtypes = [ctypes.POINTER(CpTrackerConfig), i32, ctypes.POINTER(vp)]
     for name in EXPORTS:
         fn = getattr(L, name)
         if name not in ("cp_version", "cp_last_error", "cp_plan_bytes", "cp_plan_forward_launches",

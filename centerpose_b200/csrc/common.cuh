@@ -82,6 +82,10 @@ struct IgemmParams {
   // the models: image n reads source image n % ipm.  ipm == 0: one model.
   int ipm;
   long long wstride, tstride;
+  // Bit i set: NCHW source src[i] holds one image per launch image (multi-category tracking plans: every model's own
+  // previous-frame heat maps), so image n reads its source image n, not n % ipm.  Honoured by the kernels that read NCHW
+  // sources (stem_conv7_kernel, the NCHW mode of igemm_fp32).
+  unsigned nchw_per_model;
 };
 // images per model of a launch (model_ipm > 0 everywhere in the kernels)
 inline int model_ipm(const IgemmParams& p) { return p.ipm > 0 ? p.ipm : p.B; }

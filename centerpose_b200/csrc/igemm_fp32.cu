@@ -58,7 +58,8 @@ __global__ void __launch_bounds__(NT, 2) igemm_fp32_kernel(const IgemmParams p) 
   const int m0 = MULTI ? model * Mm + (blockIdx.x - model * bpm) * BM : blockIdx.x * BM;
   const int n0 = blockIdx.y * BN;
   const float* const wgt = MULTI ? p.wgt + (size_t)model * p.wstride : p.wgt;
-  const int n_shared = MULTI ? model * p.ipm : 0;      // NCHW sources are the models' shared input frames
+  // NCHW sources are the models' shared input frames, unless each model has its own (IgemmParams::nchw_per_model)
+  const int n_shared = (MULTI && !(p.nchw_per_model & 1u)) ? model * p.ipm : 0;
 
   // ---- A-load assignment: this thread fills k-quad `kq` of rows r0 and r0+64
   const int kq = tid & 3;

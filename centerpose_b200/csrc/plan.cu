@@ -123,6 +123,9 @@ struct cp_plan {
   // umma_wts + m * umma_bytes; the arena holds models * B images, model m's at [m * batch, (m + 1) * batch)
   int models = 1;
   std::vector<char> model_loaded;
+  // bit e set: external input e holds one image per model and frame ([models, batch, ...]) rather than one per frame
+  // (cp_plan_create_multi_track: pre_hm and pre_hm_hp, which each category draws from its own tracks)
+  unsigned ext_per_model = 0;
 };
 
 namespace cp {
@@ -566,6 +569,7 @@ void igemm_params(const cp_plan* P, const Op& op, int batch, const float* const 
   for (int i = 0; i < op.nsrc; ++i) {
     const Act& a = op.src[i];
     p.src[i] = a.ext >= 0 ? ext[a.ext] : P->act + a.off;
+    if (a.ext >= 0 && ((P->ext_per_model >> a.ext) & 1u)) p.nchw_per_model |= 1u << i;
     p.srcC[i] = a.C;
     p.srcStride[i] = a.stride;
   }
@@ -664,12 +668,27 @@ const char* cp_last_error(void) { return cp::g_last_error.c_str(); }
 
 int cp_plan_create(const cp_config* cfg, cp_plan** out) { return cp_plan_create_multi(cfg, 1, out); }
 
+static int create_plan(const cp_config* cfg, int32_t num_models, unsigned ext_per_model, cp_plan** out);
+
 int cp_plan_create_multi(const cp_config* cfg, int32_t num_models, cp_plan** out) {
   if (!cfg || !out) return fail(CP_ERR_INVALID, "cp_plan_create: null argument");
   if (num_models < 1 || num_models > CP_MAX_MODELS)
     return fail(CP_ERR_INVALID, "cp_plan_create_multi: num_models must be in 1..CP_MAX_MODELS");
   if (cfg->tracking && num_models > 1)
-    return fail(CP_ERR_INVALID, "cp_plan_create_multi: a tracking plan holds one model (multi-category tracking is not supported)");
+    return fail(CP_ERR_INVALID, "cp_plan_create_multi: a tracking plan made here holds one model; several tracking "
+                                "models run through cp_plan_create_multi_track");
+  return create_plan(cfg, num_models, 0u, out);
+}
+
+int cp_plan_create_multi_track(const cp_config* cfg, int32_t num_models, cp_plan** out) {
+  if (!cfg || !out) return fail(CP_ERR_INVALID, "cp_plan_create_multi_track: null argument");
+  if (cfg->tracking != 1) return fail(CP_ERR_INVALID, "cp_plan_create_multi_track: needs a tracking config (tracking = 1)");
+  if (num_models < 1 || num_models > CP_MAX_MODELS)
+    return fail(CP_ERR_INVALID, "cp_plan_create_multi_track: num_models must be in 1..CP_MAX_MODELS");
+  return create_plan(cfg, num_models, (1u << 2) | (1u << 3), out);      // pre_hm, pre_hm_hp: one per model and frame
+}
+
+static int create_plan(const cp_config* cfg, int32_t num_models, unsigned ext_per_model, cp_plan** out) {
   if (cfg->arch != CP_ARCH_DLA34 && cfg->arch != CP_ARCH_DLAV1_34)
     return fail(CP_ERR_INVALID, "cp_plan_create: unknown arch");
   if (!known_precision(cfg->precision))
@@ -692,6 +711,7 @@ int cp_plan_create_multi(const cp_config* cfg, int32_t num_models, cp_plan** out
   for (int i = 0; i < cfg->num_heads; ++i) P->cfg.head_names[i] = P->head_names[i].c_str();
   P->B = cfg->max_batch;
   P->models = num_models;
+  P->ext_per_model = ext_per_model;
   P->model_loaded.assign(num_models, 0);
   P->H = cfg->height;
   P->W = cfg->width;
@@ -1119,8 +1139,23 @@ int cp_infer(cp_plan* P, int32_t batch, const float* images, const float* pre_im
   if (!P || !images || !prm || !meta || !poses || !n_valid) return fail(CP_ERR_INVALID, "cp_infer: null argument");
   if (!P->loaded) return fail(CP_ERR_NOT_LOADED, "cp_infer: call cp_plan_load_weights first");
   if (batch <= 0 || batch > P->B) return fail(CP_ERR_INVALID, "cp_infer: batch exceeds the plan's max_batch");
-  if (P->models > 1) return fail(CP_ERR_INVALID, "cp_infer: a multi-model plan runs through cp_infer_multi");
+  if (P->models > 1)
+    return fail(CP_ERR_INVALID, P->cfg.tracking ? "cp_infer: a multi-model tracking plan runs through cp_infer_multi_track"
+                                                : "cp_infer: a multi-model plan runs through cp_infer_multi");
   return infer_models(P, batch, images, pre_img, pre_hm, pre_hm_hp, prm, meta, heads_out, dets, poses, n_valid, stream);
+}
+
+// the decode parameters of a multi-model call: the models may differ in their per-category constants only
+static int check_model_prms(const cp_plan* P, const cp_decode_params* prms, const char* fn) {
+  for (int m = 1; m < P->models; ++m) {
+    cp_decode_params a = prms[0], b = prms[m];
+    a.visible_thresh = b.visible_thresh = 0;      // the per-category constants (cuboid_pnp_shell.py:59-66, balance)
+    a.balance = b.balance = 0.f;
+    a.batch = b.batch = a.out_h = b.out_h = a.out_w = b.out_w = 0;      // set by the call
+    if (memcmp(&a, &b, sizeof(a)))
+      return fail(CP_ERR_INVALID, std::string(fn) + ": the models' decode parameters may differ in visible_thresh and balance only");
+  }
+  return CP_OK;
 }
 
 int cp_infer_multi(cp_plan* P, int32_t batch, const float* images, const cp_decode_params* prms, const double* meta,
@@ -1128,16 +1163,23 @@ int cp_infer_multi(cp_plan* P, int32_t batch, const float* images, const cp_deco
   if (!P || !images || !prms || !meta || !poses || !n_valid) return fail(CP_ERR_INVALID, "cp_infer_multi: null argument");
   if (!P->loaded) return fail(CP_ERR_NOT_LOADED, "cp_infer_multi: call cp_plan_load_weights_model for every model first");
   if (batch <= 0 || batch > P->B) return fail(CP_ERR_INVALID, "cp_infer_multi: batch exceeds the plan's max_batch");
-  if (P->cfg.tracking) return fail(CP_ERR_INVALID, "cp_infer_multi: tracking plans run through cp_infer");
-  for (int m = 1; m < P->models; ++m) {
-    cp_decode_params a = prms[0], b = prms[m];
-    a.visible_thresh = b.visible_thresh = 0;      // the per-category constants (cuboid_pnp_shell.py:59-66, balance)
-    a.balance = b.balance = 0.f;
-    a.batch = b.batch = a.out_h = b.out_h = a.out_w = b.out_w = 0;      // set by the call
-    if (memcmp(&a, &b, sizeof(a)))
-      return fail(CP_ERR_INVALID, "cp_infer_multi: the models' decode parameters may differ in visible_thresh and balance only");
-  }
+  if (P->cfg.tracking)
+    return fail(CP_ERR_INVALID, "cp_infer_multi: tracking plans run through cp_infer or cp_infer_multi_track");
+  if (int rc = check_model_prms(P, prms, "cp_infer_multi")) return rc;
   return infer_models(P, batch, images, nullptr, nullptr, nullptr, prms, meta, heads_out, dets, poses, n_valid, stream);
+}
+
+int cp_infer_multi_track(cp_plan* P, int32_t batch, const float* images, const float* pre_img, const float* pre_hm,
+                         const float* pre_hm_hp, const cp_decode_params* prms, const double* meta, float* const* heads_out,
+                         float* dets, float* poses, int32_t* n_valid, void* stream) {
+  if (!P || !images || !pre_img || !pre_hm || !pre_hm_hp || !prms || !meta || !poses || !n_valid)
+    return fail(CP_ERR_INVALID, "cp_infer_multi_track: null argument");
+  if (!P->cfg.tracking || P->ext_per_model != ((1u << 2) | (1u << 3)))
+    return fail(CP_ERR_INVALID, "cp_infer_multi_track: the plan was not made by cp_plan_create_multi_track");
+  if (!P->loaded) return fail(CP_ERR_NOT_LOADED, "cp_infer_multi_track: call cp_plan_load_weights_model for every model first");
+  if (batch <= 0 || batch > P->B) return fail(CP_ERR_INVALID, "cp_infer_multi_track: batch exceeds the plan's max_batch");
+  if (int rc = check_model_prms(P, prms, "cp_infer_multi_track")) return rc;
+  return infer_models(P, batch, images, pre_img, pre_hm, pre_hm_hp, prms, meta, heads_out, dets, poses, n_valid, stream);
 }
 
 }  // extern "C"

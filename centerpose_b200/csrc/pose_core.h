@@ -725,6 +725,18 @@ CP_HDN int pnp_collect(const double* pts, int n_in, const float* obj_scale, doub
   return n;
 }
 
+// The visibility gate of cuboid_pnp_shell.py:59-79: at least visible_thresh of the nine projected points (kps_pnp,
+// normalised) outside the image makes a pose invisible; visible_thresh <= 0 turns the gate off.
+CP_HD bool pnp_gate_invisible(const double* kpspnp, int visible_thresh) {
+  if (visible_thresh <= 0) return false;
+  int nv = 0;
+  for (int i = 0; i < 9; ++i) {
+    double a = kpspnp[2 * i], b = kpspnp[2 * i + 1];
+    if (a < 0 || a > 1 || b < 0 || b > 1) ++nv;
+  }
+  return nv >= visible_thresh;
+}
+
 // pnp_finish: everything after the solver (cuboid_pnp_solver.py:190-239, cuboid_pnp_shell.py:24-93)
 CP_HDN void pnp_finish(const double* V, const double* R, const double* t, double cost, int n, const double* Kc,
                        double width, double height, int visible_thresh, int opencv_return, PnPOut* o) {
@@ -791,14 +803,7 @@ CP_HDN void pnp_finish(const double* V, const double* R, const double* t, double
     o->kpspnp[2 * (i + 1) + 1] = o->proj[2 * i + 1] / height;
   }
   o->status = 1;
-  if (visible_thresh > 0) {
-    int nv = 0;
-    for (int i = 0; i < 9; ++i) {
-      double a = o->kpspnp[2 * i], b = o->kpspnp[2 * i + 1];
-      if (a < 0 || a > 1 || b < 0 || b > 1) ++nv;
-    }
-    if (nv >= visible_thresh) o->status = 2;
-  }
+  if (pnp_gate_invisible(o->kpspnp, visible_thresh)) o->status = 2;
   if (!(o->kpspnp[0] > 0 && o->kpspnp[0] < 1 && o->kpspnp[1] > 0 && o->kpspnp[1] < 1)) o->status = 2;
 }
 

@@ -16,7 +16,7 @@ constexpr int ST_HALO_W = ST_W + 6, ST_HALO_H = ST_TY + 6;
 __global__ void __launch_bounds__(ST_TX* ST_TY)
     stem_conv7_kernel(const float* __restrict__ in, const float* __restrict__ wgt, const float* __restrict__ bias,
                       const float* __restrict__ residual, float* __restrict__ out, int B, int Cin, int H, int W,
-                      int relu, int ipm, long long wstride) {
+                      int relu, int ipm, long long wstride, int in_ipm) {
   extern __shared__ __align__(16) float sm[];
   float* ws = sm;                                        // [(ky*7+kx)*Cin + c][16]   (16-byte aligned)
   float* tile = sm + 49 * Cin * 16;                      // [Cin][ST_HALO_H][ST_HALO_W]
@@ -24,10 +24,11 @@ __global__ void __launch_bounds__(ST_TX* ST_TY)
   const int n = blockIdx.z;
   const int x0 = blockIdx.x * ST_W, y0 = blockIdx.y * ST_TY;
   const int nw = 49 * Cin * 16;
-  // image n runs model n / ipm (IgemmParams::ipm) on input frame n % ipm, which every model reads
+  // image n runs model n / ipm (IgemmParams::ipm) on input image n % in_ipm: in_ipm = ipm when every model reads the same
+  // frames, the launch's whole batch when each model has its own input (IgemmParams::nchw_per_model)
   wgt += (size_t)(n / ipm) * wstride;
   bias += (size_t)(n / ipm) * wstride;
-  const int n_in = n % ipm;
+  const int n_in = n % in_ipm;
   if (tid == 0) griddep_launch_dependents();      // PDL (common.cuh): weights are constants, the image is not
   for (int i = tid; i < nw; i += ST_TX * ST_TY) ws[i] = __ldg(wgt + i);
   griddep_wait();
@@ -258,7 +259,8 @@ int launch_stem_conv(const IgemmParams& p, cudaStream_t s) {
   dim3 grid((p.Win + ST_W - 1) / ST_W, (p.Hin + ST_TY - 1) / ST_TY, p.B);
   dim3 block(ST_TX, ST_TY);
   CP_CUDA_CHECK(launch_kernel(stem_conv7_kernel, grid, block, smem, s, p.src[0], p.wgt, p.bias, p.residual, p.out, p.B, p.Cin,
-                              p.Hin, p.Win, p.relu, model_ipm(p), p.wstride));
+                              p.Hin, p.Win, p.relu, model_ipm(p), p.wstride,
+                              (p.nchw_per_model & 1u) ? p.B : model_ipm(p)));
   CP_LAUNCH_CHECK("stem_conv7_kernel");
   return CP_OK;
 }

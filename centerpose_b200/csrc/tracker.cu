@@ -5,6 +5,8 @@
 //
 // Reference (relative to /root/reference/src/lib): utils/tracker.py:15-302, detectors/base_detector.py:150-388
 // (_get_additional_inputs), :502-544 (gaussian_fusion), :660-665 (tracker.step in run()).
+#include <string.h>
+
 #include <new>
 
 #include "common.cuh"
@@ -14,8 +16,22 @@
 using namespace cp;
 using namespace cp::track;
 
+namespace cp {
+namespace {
+// The per-category settings of a tracker of several categories (cp_tracker_create_multi): stream s belongs to category
+// s / S and uses its visible_thresh (second PnP) and conf_border (keypoint-confidence gain).  Passed by value to the
+// step and render kernels; a one-category tracker has one row.
+struct CatCfg {
+  int S;                                   // streams per category
+  int visible_thresh[CP_MAX_MODELS];
+  double conf_lo[CP_MAX_MODELS], conf_hi[CP_MAX_MODELS];
+};
+}  // namespace
+}  // namespace cp
+
 struct cp_tracker {
-  cp_tracker_config cfg;
+  cp_tracker_config cfg;                    // cfg.streams: every category's streams (models x streams per category)
+  CatCfg cat;
   Slot* slots[2] = {nullptr, nullptr};      // [streams][max_tracks], ping-pong: slots[cur[s]] = current tracks of s
   int* n_tracks[2] = {nullptr, nullptr};    // [streams]
   int* cur = nullptr;                       // [streams] current buffer of each stream, flipped by the step kernel
@@ -34,7 +50,8 @@ constexpr int TRK_MAXK = CP_MAX_K;
 
 struct StepArgs {
   Cfg cfg;
-  int visible_thresh, opencv_return, T, K;
+  CatCfg cat;
+  int opencv_return, T, K;
   const float* poses;       // [B, K, 192]
   const int* n_valid;       // [B]
   const double* meta;       // [B, 16]
@@ -212,7 +229,8 @@ __global__ void __launch_bounds__(TRK_THREADS, 1) tracker_step_kernel(const Step
   __shared__ float fbuf[3 * 2 * TRK_MAXK];
   __shared__ int ibuf[4 * TRK_MAXK];
   __shared__ unsigned char taken[TRK_MAXK];
-  __shared__ int s_n;
+  __shared__ int s_n, s_vis;
+  __shared__ double s_conf[2];
   __shared__ double pnp_sm[(TRK_THREADS / 32) * PNP_SCRATCH];
 
   const float* poses = a.poses + (size_t)b * a.K * CP_POSE_RECORD;
@@ -225,6 +243,12 @@ __global__ void __launch_bounds__(TRK_THREADS, 1) tracker_step_kernel(const Step
   if (nv > a.K) nv = a.K;
   if (nv < 0) nv = 0;
 
+  if (tid == 0) {      // this stream's category settings (CatCfg), read back from shared memory where they are used
+    const int cat = st.s / a.cat.S;
+    s_vis = a.cat.visible_thresh[cat];
+    s_conf[0] = a.cat.conf_lo[cat];
+    s_conf[1] = a.cat.conf_hi[cat];
+  }
   if (a.plan) {
     const int n = a.plan_n[b];
     for (int e = tid; e < n; e += TRK_THREADS) entries[e] = a.plan[(size_t)b * a.T + e];
@@ -253,7 +277,10 @@ __global__ void __launch_bounds__(TRK_THREADS, 1) tracker_step_kernel(const Step
   double* sm = pnp_sm + warp * PNP_SCRATCH;
   for (int e = warp; e < n; e += NW) {
     double mean[16], sd[16], conf_avg, sc[3], su[3];
-    entry_readout(a.cfg, &nxt[e], mean, sd, &conf_avg, sc, su);
+    Cfg ccfg = a.cfg;
+    ccfg.conf_lo = s_conf[0];
+    ccfg.conf_hi = s_conf[1];
+    entry_readout(ccfg, &nxt[e], mean, sd, &conf_avg, sc, su);
     pose::PnPOut po;
     po.status = CP_PNP_NOT_RUN;
     po.n_pts = 0;
@@ -265,7 +292,10 @@ __global__ void __launch_bounds__(TRK_THREADS, 1) tracker_step_kernel(const Step
       else
         pose::cuboid_vertices(nxt[e].rec + CP_P_OBJ_SCALE, V);
       __syncwarp();
-      solve_and_shell_warp_v(mean, 8, V, meta + 5, meta[3], meta[4], a.visible_thresh, a.opencv_return, &po, sm, lane);
+      // the category's visibility gate is applied after the solve rather than inside it: the same status, and the
+      // shared solve keeps the register allocation of a one-category step
+      solve_and_shell_warp_v(mean, 8, V, meta + 5, meta[3], meta[4], 0, a.opencv_return, &po, sm, lane);
+      if (po.status == CP_PNP_OK && pose::pnp_gate_invisible(po.kpspnp, s_vis)) po.status = CP_PNP_INVISIBLE;
       in_boxes = (po.status == CP_PNP_OK && conf_avg > 0.25) ? 1 : 0;
     } else {
       in_boxes = ((int)nxt[e].rec[CP_P_STATUS] == CP_PNP_OK && nxt[e].age == 1) ? 1 : 0;
@@ -329,6 +359,7 @@ __global__ void __launch_bounds__(128) tracker_seed_kernel(const Cfg cfg, int T,
 // ---- previous-frame heat maps ----------------------------------------------------------------------------------------
 struct RenderArgs {
   Cfg cfg;
+  CatCfg cat;
   int T, inp_h, inp_w, render_hm_mode, render_hmhp_mode;
   double pre_thresh;
   const Slot* slots0;      // [streams, T]
@@ -362,6 +393,7 @@ __global__ void __launch_bounds__(256) tracker_render_kernel(const RenderArgs a)
   const int sid = a.ids ? a.ids[b] : b, c = a.cur[sid];
   if (t >= (c ? a.n1 : a.n0)[sid] || rmode == CP_RENDER_EMPTY) return;
   const bool gt = rmode == CP_RENDER_GT;
+  const double conf_lo = a.cat.conf_lo[sid / a.cat.S], conf_hi = a.cat.conf_hi[sid / a.cat.S];      // CatCfg
   __shared__ Patch pt[9];
   if (tid == 0) {
     for (int i = 0; i < 9; ++i) pt[i].live = 0;
@@ -450,11 +482,11 @@ __global__ void __launch_bounds__(256) tracker_render_kernel(const RenderArgs a)
                 if (!((int)rd > 0)) continue;                   // radius_detector[j, 0] > 0 (int32 truncation)
                 if (a.cfg.kalman && s.has_kf) {
                   const double std_c = sqrt(s.f.P[j][0] + s.f.P[j][5]);
-                  k = 1.0 - pow(exp(log(0.15) / (a.cfg.conf_lo - a.cfg.conf_hi)), std_c - a.cfg.conf_hi);
+                  k = 1.0 - pow(exp(log(0.15) / (conf_lo - conf_hi)), std_c - conf_hi);
                   if (k < 0.0) k = 0.0;
                 } else if (a.cfg.hps_uncertainty) {
                   const double std_c = sqrt(s.fus_std[2 * j] + s.fus_std[2 * j + 1]);
-                  k = 1.0 - pow(exp(log(0.15) / (a.cfg.conf_lo - a.cfg.conf_hi)), std_c - a.cfg.conf_hi);
+                  k = 1.0 - pow(exp(log(0.15) / (conf_lo - conf_hi)), std_c - conf_hi);
                   if (k < 0.0) k = 0.0;
                 } else {
                   k = (double)r[CP_P_KPS_HM_HEIGHT + j];
@@ -513,14 +545,38 @@ Cfg make_cfg(const cp_tracker_config& c) {
 
 extern "C" {
 
-int cp_tracker_create(const cp_tracker_config* cfg, cp_tracker** out) {
-  if (!cfg || !out) return fail(CP_ERR_INVALID, "cp_tracker_create: null argument");
+int cp_tracker_create(const cp_tracker_config* cfg, cp_tracker** out) { return cp_tracker_create_multi(cfg, 1, out); }
+
+int cp_tracker_create_multi(const cp_tracker_config* cfgs, int32_t models, cp_tracker** out) {
+  if (!cfgs || !out) return fail(CP_ERR_INVALID, "cp_tracker_create: null argument");
+  if (models < 1 || models > CP_MAX_MODELS)
+    return fail(CP_ERR_INVALID, "cp_tracker_create_multi: models must be in 1..CP_MAX_MODELS");
+  const cp_tracker_config* cfg = cfgs;
   if (cfg->streams <= 0 || cfg->max_tracks <= 0 || cfg->max_tracks > CP_MAX_K)
     return fail(CP_ERR_INVALID, "cp_tracker_create: streams must be > 0 and max_tracks in 1..128");
-  if (cfg->conf_lo == cfg->conf_hi) return fail(CP_ERR_INVALID, "cp_tracker_create: conf_border needs two distinct values");
+  if ((long long)cfg->streams * models > (1 << 30))
+    return fail(CP_ERR_INVALID, "cp_tracker_create_multi: too many streams");
+  for (int m = 0; m < models; ++m) {
+    if (cfgs[m].conf_lo == cfgs[m].conf_hi)
+      return fail(CP_ERR_INVALID, "cp_tracker_create: conf_border needs two distinct values");
+    cp_tracker_config a = cfgs[0], b = cfgs[m];
+    a.visible_thresh = b.visible_thresh = 0;      // the per-category settings (opt.c)
+    a.conf_lo = b.conf_lo = a.conf_hi = b.conf_hi = 0.f;
+    if (memcmp(&a, &b, sizeof(a)))
+      return fail(CP_ERR_INVALID, "cp_tracker_create_multi: the configs of category " + std::to_string(m) +
+                                      " and category 0 differ in more than visible_thresh, conf_lo and conf_hi");
+  }
   cp_tracker* t = new (std::nothrow) cp_tracker();
   if (!t) return fail(CP_ERR_INVALID, "cp_tracker_create: out of host memory");
   t->cfg = *cfg;
+  t->cfg.streams = cfg->streams * models;
+  t->cat.S = cfg->streams;
+  for (int m = 0; m < models; ++m) {
+    t->cat.visible_thresh[m] = cfgs[m].visible_thresh;
+    t->cat.conf_lo[m] = (double)cfgs[m].conf_lo;
+    t->cat.conf_hi[m] = (double)cfgs[m].conf_hi;
+  }
+  cfg = &t->cfg;
   struct DeviceGuard {
     int prev = -1;
     ~DeviceGuard() {
@@ -625,7 +681,7 @@ int cp_tracker_step_ex(cp_tracker* t, int32_t batch, const int32_t* stream_ids, 
   StepArgs a;
   if (int rc = upload_stream_ids(t, batch, stream_ids, s, &a.ids)) return rc;
   a.cfg = make_cfg(t->cfg);
-  a.visible_thresh = t->cfg.visible_thresh;
+  a.cat = t->cat;
   a.opencv_return = t->cfg.opencv_return;
   a.T = t->cfg.max_tracks;
   a.K = K;
@@ -681,6 +737,7 @@ int cp_tracker_render_ex2(cp_tracker* t, int32_t batch, const int32_t* stream_id
   CP_CUDA_CHECK(cudaMemsetAsync(pre_hm_hp, 0, sizeof(float) * plane * 8 * batch, s));
   if (any_mode) CP_CUDA_CHECK(cudaMemcpyAsync(t->modes, modes, sizeof(int32_t) * batch, cudaMemcpyHostToDevice, s));
   a.cfg = make_cfg(t->cfg);
+  a.cat = t->cat;
   a.T = t->cfg.max_tracks;
   a.inp_h = inp_h;
   a.inp_w = inp_w;

@@ -155,13 +155,14 @@ def _returned(pair, to_host):
 
 
 class _SlotState(object):
-    """run_batch(track=True): the tracker of S slot streams, each slot's previous network input (`pre`, [S,3,h,w], None
-    before the first step; never written in place, so it may be the network input of the previous step itself) and
+    """run_batch(track=True): the tracker of S slot streams (of every category, with `categories`: stream m * S + s is
+    slot s of category m), each slot's previous network input (`pre`, [S,3,h,w], None before the first step; never
+    written in place, so it may be the network input of the previous step itself; shared by the categories) and
     whether each slot has had a frame since the state was made."""
 
-    def __init__(self, opt, S, device):
+    def __init__(self, opt, S, device, categories=None):
         self.streams = S
-        self.tracker = Tracker(opt, streams=S, device=device)
+        self.tracker = Tracker(opt, streams=S, device=device, categories=categories)
         self.pre = None
         self.started = [False] * S
 
@@ -580,8 +581,7 @@ class ObjectPoseDetector(object):
             x, meta, c, s = self._array_input(frames, camera_matrix)
             B = x.shape[0]
             if track:
-                if pre_dets is not None and len(pre_dets) != B:
-                    raise ValueError("run_batch: %d pre_dets lists for %d streams" % (len(pre_dets), B))
+                pre_dets = self._slot_pre_dets(pre_dets, B)
                 trans = affine_from_center_scale(c, s, x.shape[3], x.shape[2])
                 return self._track_step(B, list(range(B)), x, self._meta_rows(meta), trans, None, pre_dets, frame_ids,
                                         to_host, None)
@@ -672,15 +672,9 @@ class ObjectPoseDetector(object):
         check_frames(frames, allow_idle=True)
         cams = camera_per_frame(camera_matrix, S)
         new_video = check_slot_list(new_video, S, "new_video", bool)
-        pre_dets = check_slot_list(pre_dets, S, "pre_dets")
+        pre_dets = self._slot_pre_dets(pre_dets, S)
         frame_ids = check_slot_list(frame_ids, S, "frame_ids")
-        dev, T = self.opt.device, _lib.CP_MAX_K
-        if out is None:
-            out = (torch.empty((S, T, _lib.CP_TRACK_RECORD), dtype=torch.float32, device=dev),
-                   torch.empty((S,), dtype=torch.int32, device=dev))
-        elif (tuple(out[0].shape) != (S, T, _lib.CP_TRACK_RECORD) or tuple(out[1].shape) != (S,)
-              or out[0].dtype != torch.float32 or out[1].dtype != torch.int32):
-            raise ValueError("run_batch: out must be (tracks [%d,%d,%d] fp32, n_tracks [%d] int32)" % (S, T, _lib.CP_TRACK_RECORD, S))
+        out = self._track_out(out, S)
         live = [i for i in range(S) if frames[i] is not None]
         if not live:
             out[0].zero_()
@@ -689,19 +683,53 @@ class ObjectPoseDetector(object):
         x, meta, trans = self._ragged_input([frames[i] for i in live], np.stack([cams[i] for i in live]))
         return self._track_step(S, live, x, self._meta_rows(meta), trans, new_video, pre_dets, frame_ids, to_host, out)
 
+    # ---- what a tracking step does per category: one category here; MultiCategoryTracker runs several through the
+    # same step (_track_step) by overriding these
+    def _track_categories(self):
+        """None: one category, opt.c (outputs [S, ...]); else the categories of the step (outputs [M, S, ...])."""
+        return None
+
+    def _track_engine(self, S, x):
+        """(the plan, its decode parameters) of a tracking step of S slots at the network input size of x."""
+        return self.model.engine(S, x.shape[2], x.shape[3], x.device), decode_params(self.opt, test_scale=1.0)
+
+    def _slot_pre_dets(self, pre_dets, S):
+        """run_batch's pre_dets, checked: None or, per slot, a list of pre_dets dicts (or None)."""
+        return check_slot_list(pre_dets, S, "pre_dets")
+
+    def _cat_pre_dets(self, pre_dets):
+        """Checked pre_dets -> one per-slot list (or None) per category."""
+        return [pre_dets]
+
+    def _track_out(self, out, S):
+        """The (tracks, n_tracks) CUDA tensors a step of S slots writes: `out` when given (checked), else new ones."""
+        lead = (S,) if self._track_categories() is None else (len(self._track_categories()), S)
+        dev, T = self.opt.device, _lib.CP_MAX_K
+        if out is None:
+            return (torch.empty(lead + (T, _lib.CP_TRACK_RECORD), dtype=torch.float32, device=dev),
+                    torch.empty(lead, dtype=torch.int32, device=dev))
+        if (tuple(out[0].shape) != lead + (T, _lib.CP_TRACK_RECORD) or tuple(out[1].shape) != lead
+                or out[0].dtype != torch.float32 or out[1].dtype != torch.int32):
+            raise ValueError("run_batch: out must be (tracks %s fp32, n_tracks %s int32)"
+                             % (list(lead + (T, _lib.CP_TRACK_RECORD)), list(lead)))
+        return out
+
     def _track_step(self, S, live, x, metat, trans, new_video, pre_dets, frame_ids, to_host, out):
         """One tracking step of S slots, both forms of run_batch(track=True).  Row k of x (network input [n,3,h,w]),
         metat (device meta rows [n,16]) and trans (trans_input, [n,2,3] or one [2,3] for all) is the next frame of slot
-        live[k]; new_video / pre_dets / frame_ids: None or per slot.  Writes (tracks [S,T,320], n_tracks [S]) into out
-        (None: new tensors; only when every slot is live), slots not in `live` with n_tracks 0 and zero rows."""
+        live[k]; new_video / pre_dets / frame_ids: None or per slot (pre_dets as _slot_pre_dets returns it).  Writes
+        (tracks [S,T,320], n_tracks [S]) into out (None: new tensors; only when every slot is live), slots not in
+        `live` with n_tracks 0 and zero rows.  With several categories (_track_categories) every category steps the same
+        slots: tracker stream m * S + s, outputs [M, S, ...], one render, one network call and one tracker step for all."""
+        cats = self._track_categories()
+        M = 1 if cats is None else len(cats)
         if self._slots is None or self._slots.streams != S:
-            self._slots = _SlotState(self.opt, S, self.opt.device)
+            self._slots = _SlotState(self.opt, S, self.opt.device, categories=cats)
         st = self._slots
         trk = st.tracker
         # looked up before the render, whose trans_input upload waits for the device: host work between that upload and
         # the network launch would leave the GPU idle
-        eng = self.model.engine(S, x.shape[2], x.shape[3], x.device)
-        prm = decode_params(self.opt, test_scale=1.0)
+        eng, prm = self._track_engine(S, x)
         # previous frames of another size (an fp32 array input that changed size): every slot takes this frame as its
         # previous frame and is seeded as at a start, but keeps its tracks
         resized = st.pre is not None and st.pre.shape[1:] != x.shape[1:]
@@ -710,14 +738,16 @@ class ObjectPoseDetector(object):
                              % (tuple(st.pre.shape[2:]), tuple(x.shape[2:])))
         new = [not st.started[i] or (new_video is not None and new_video[i]) for i in live]
         starts = [n or resized for n in new]
-        seeds, modes = [None] * S, []
-        for k, i in enumerate(live):
-            seeds[i], mode = self._track_policy(starts[k], frame_ids[i] if frame_ids is not None else None,
-                                                pre_dets[i] if pre_dets is not None else None)
-            modes.append(mode)
+        seeds, modes = [None] * (M * S), []
+        for m, pd in enumerate(self._cat_pre_dets(pre_dets)):
+            for k, i in enumerate(live):
+                seeds[m * S + i], mode = self._track_policy(starts[k], frame_ids[i] if frame_ids is not None else None,
+                                                            pd[i] if pd is not None else None)
+                modes.append(mode)
         for k, i in enumerate(live):
             if new[k]:                                        # base_detector.py:444-449: a fresh stream
-                trk.reset(i)
+                for m in range(M):
+                    trk.reset(m * S + i)
                 st.started[i] = True
         trk.seed(seeds)
         all_live = len(live) == S                             # every slot, in order: stream map NULL (the identity)
@@ -727,11 +757,26 @@ class ObjectPoseDetector(object):
             pre = st.pre
         else:
             pre = torch.stack([x[k] if starts[k] else st.pre[i] for k, i in enumerate(live)])
-        ids = None if all_live else live
+        n = len(live)
+        ids = None if all_live else [m * S + i for m in range(M) for i in live]
+        if M > 1:            # one render of every category's images (category m's are rows m * n ...), one meta row each
+            metat = metat.repeat(M, 1)
+            if np.asarray(trans).ndim == 3:
+                trans = np.tile(trans, (M, 1, 1))
         pre_hms, pre_hm_hp = trk.render(metat, trans, x.shape[2], x.shape[3], modes=modes, stream_ids=ids)
-        _, poses, n_valid = eng.infer(x, metat, prm, pre, pre_hms, pre_hm_hp)
-        if all_live:
+        if M > 1:
+            pre_hms, pre_hm_hp = pre_hms.view((M, n) + pre_hms.shape[1:]), pre_hm_hp.view((M, n) + pre_hm_hp.shape[1:])
+        _, poses, n_valid = eng.infer(x, metat[:n], prm, pre, pre_hms, pre_hm_hp)
+        poses, n_valid = poses.reshape((M * n,) + poses.shape[-2:]), n_valid.reshape(M * n)
+        if cats is not None:
+            out = self._track_out(out, S) if out is not None or not all_live else out
+        if all_live and cats is None:
             out = trk.step_records(poses, n_valid, metat, out=out)
+            st.pre = x
+        elif all_live:                                        # [M, S, ...] is the tracker's stream order
+            flat = None if out is None else (out[0].view((M * S,) + out[0].shape[-2:]), out[1].view(M * S))
+            flat = trk.step_records(poses, n_valid, metat, out=flat)
+            out = out if out is not None else (flat[0].view((M, S) + flat[0].shape[1:]), flat[1].view(M, S))
             st.pre = x
         else:
             tr, nt = trk.step_records(poses, n_valid, metat, stream_ids=ids)
@@ -739,8 +784,10 @@ class ObjectPoseDetector(object):
             old = st.pre if st.pre is not None else x.new_zeros((S,) + tuple(x.shape[1:]))
             st.pre = torch.stack([x[row[i]] if i in row else old[i] for i in range(S)])
             zt, zn = tr.new_zeros(tr.shape[1:]), nt.new_zeros(())
-            torch.stack([tr[row[i]] if i in row else zt for i in range(S)], out=out[0])
-            torch.stack([nt[row[i]] if i in row else zn for i in range(S)], out=out[1])
+            outs = [out] if cats is None else [(out[0][m], out[1][m]) for m in range(M)]
+            for m, (o_tr, o_nt) in enumerate(outs):
+                torch.stack([tr[m * n + row[i]] if i in row else zt for i in range(S)], out=o_tr)
+                torch.stack([nt[m * n + row[i]] if i in row else zn for i in range(S)], out=o_nt)
         return _returned(out, to_host)
 
     def reset_tracking(self):
@@ -767,28 +814,8 @@ class MultiCategoryDetector(ObjectPoseDetector):
 
     def __init__(self, opt, checkpoints):
         if getattr(opt, "tracking_task", False):
-            raise ValueError("MultiCategoryDetector: tracking with several categories is not supported")
-        cats = list(checkpoints.keys())
-        if not 1 <= len(cats) <= _lib.CP_MAX_MODELS:
-            raise ValueError("MultiCategoryDetector: 1..%d categories, got %d" % (_lib.CP_MAX_MODELS, len(cats)))
-        for c in cats:
-            decode_params(opt, c=c)                  # raises on an unknown category
-        weights = []
-        for c in cats:
-            m = create_model(opt.arch, opt.heads, opt.head_conv, opt)
-            _check_checkpoint(m, checkpoints[c], c)
-            m = load_model(m, checkpoints[c])
-            weights.append({k: v.detach().cpu() for k, v in m.state_dict().items()})
-        self._plan_cfg = dict(arch=m._arch(), heads=m.heads, head_conv=m.head_conv,
-                              tracking_task_gru=m.use_convGRU and m.tracking_task, precision=m.precision)
-        base = copy.copy(opt)
-        base.load_model = ""
-        super().__init__(base, model=m)
-        self.model = None                            # the plan holds the weights; only the host copies are kept
-        self.categories = cats
-        self._weights = weights
-        self._prms = [decode_params(opt, c=c, test_scale=1.0) for c in cats]
-        self._eng = None
+            raise ValueError("MultiCategoryDetector: tracking several categories runs through MultiCategoryTracker")
+        _load_categories(self, opt, checkpoints, "MultiCategoryDetector")
 
     def engine(self, batch, height, width):
         """The multi-model plan for this input shape (created on first use, rebuilt for a larger batch)."""
@@ -799,7 +826,7 @@ class MultiCategoryDetector(ObjectPoseDetector):
             dev = torch.device(self.opt.device)
             c = self._plan_cfg
             eng = Engine(c["arch"], c["heads"], c["head_conv"], max(batch, 1), height, width,
-                         dev.index if dev.index is not None else torch.cuda.current_device(),
+                         dev.index if dev.index is not None else torch.cuda.current_device(), tracking=c["tracking"],
                          tracking_task_gru=c["tracking_task_gru"], precision=c["precision"], models=len(self._weights))
             for i, sd in enumerate(self._weights):
                 eng.load_state_dict(sd, model=i)
@@ -829,21 +856,119 @@ class MultiCategoryDetector(ObjectPoseDetector):
         return _returned((poses, n_valid), to_host)
 
 
+class MultiCategoryTracker(MultiCategoryDetector):
+    """The tracking counterpart of MultiCategoryDetector: M CenterPoseTrack checkpoints (one per category, loaded and
+    checked the same way) track their objects in the same S video slots.  One step is one pre-process, one render of
+    every category's previous-frame heat maps, one multi-model network + decode call (cp_infer_multi_track) and one
+    tracker step over the M x S streams (cp_tracker_create_multi); the previous frames are shared by the categories.
+    Category c tracks with its visible_thresh, balance coefficient and opt.conf_border[c] (when conf_border is a dict).
+    The slot policy (starts, seeding, render modes, previous frames) is that of ObjectPoseDetector.run_batch(track=True),
+    run per category.  Not supported: opt.refined_Kalman and test_scales other than [1]."""
+
+    def __init__(self, opt, checkpoints):
+        if not getattr(opt, "tracking_task", False):
+            raise ValueError("MultiCategoryTracker needs a tracking opt (opt.tracking_task); detection of several "
+                             "categories runs through MultiCategoryDetector")
+        if getattr(opt, "refined_Kalman", False):
+            raise NotImplementedError("opt.refined_Kalman (utils/tracker_baseline.py, CenterPose + Kalman baseline) is not "
+                                      "on the accelerated path; use --tracking_task (CenterPoseTrack)")
+        if [float(v) for v in getattr(opt, "test_scales", [1.0])] != [1.0]:
+            raise NotImplementedError("CenterPoseTrack runs at test_scales=[1] (the reference re-initialises the tracker "
+                                      "state once per scale, base_detector.py:440-449)")
+        _load_categories(self, opt, checkpoints, "MultiCategoryTracker")
+        if not self._plan_cfg["tracking"]:
+            raise ValueError("MultiCategoryTracker: the tracking model needs the pre_img / pre_hm / pre_hm_hp inputs")
+        if self.tracker is not None:                # ObjectPoseDetector's one-stream tracker: the slots have their own
+            self.tracker.close()
+            self.tracker = None
+
+    def run_batch(self, frames, camera_matrix, new_video=None, pre_dets=None, frame_ids=None, to_host=True, out=None):
+        """The next frame of every slot, for every category.  frames: uint8 [S,H,W,3] (every slot steps), or a list of S
+        uint8 [H_s,W_s,3] frames of mixed sizes where None idles a slot this step, with camera_matrix [3,3] or one per
+        slot.  new_video[i]: slot i starts a new video (every category).  pre_dets: None, or a mapping category -> per
+        slot list of meta['pre_dets'] lists (None = that slot is not seeded); frame_ids: per slot meta['id'].
+        Returns (tracks [M,S,T,320], n_tracks [M,S]) in `categories` order (idle slots: n_tracks 0, zero rows), on the
+        host when `to_host`; out: optional (tracks, n_tracks) CUDA tensors of those shapes to write into."""
+        if isinstance(frames, (list, tuple)):
+            return self._run_slots(frames, camera_matrix, to_host, out, pre_dets, frame_ids, new_video)
+        if new_video is not None:
+            raise ValueError("run_batch: new_video needs a list of slot frames")
+        x, meta, c, s = self._array_input(frames, camera_matrix)
+        S = x.shape[0]
+        pre_dets = self._slot_pre_dets(pre_dets, S)
+        frame_ids = check_slot_list(frame_ids, S, "frame_ids")
+        trans = affine_from_center_scale(c, s, x.shape[3], x.shape[2])
+        return self._track_step(S, list(range(S)), x, self._meta_rows(meta), trans, None, pre_dets, frame_ids, to_host,
+                                self._track_out(out, S) if out is not None else None)
+
+    def _track_categories(self):
+        return self.categories
+
+    def _track_engine(self, S, x):
+        return self.engine(S, x.shape[2], x.shape[3]), (self._prms if len(self._prms) > 1 else self._prms[0])
+
+    def _slot_pre_dets(self, pre_dets, S):
+        if pre_dets is None:
+            return None
+        if not hasattr(pre_dets, "items"):
+            raise ValueError("run_batch: pre_dets maps a category to its per-slot pre_dets lists")
+        for c, v in pre_dets.items():
+            if c not in self.categories:
+                raise ValueError("run_batch: pre_dets for unknown category '%s' (categories: %s)" % (c, self.categories))
+            if v is not None and len(list(v)) != S:
+                raise ValueError("run_batch: pre_dets['%s'] has %d entries for %d slots" % (c, len(list(v)), S))
+        return {c: (list(v) if v is not None else None) for c, v in pre_dets.items()}
+
+    def _cat_pre_dets(self, pre_dets):
+        return [(pre_dets or {}).get(c) for c in self.categories]
+
+    def reset_tracking(self):
+        """Forget every slot's tracks and previous frames (the next step starts every slot)."""
+        self._slots = None
+
+
 def _single_category(name):
     def refuse(self, *a, **k):
-        raise NotImplementedError("MultiCategoryDetector.%s: only run_batch runs several categories; use an "
-                                  "ObjectPoseDetector per category" % name)
+        raise NotImplementedError("%s.%s: only run_batch runs several categories; use an ObjectPoseDetector per "
+                                  "category" % (type(self).__name__, name))
     refuse.__name__ = name
     return refuse
 
 
-for _name in ("run", "process", "pre_process", "build_dict_out", "show_results", "save_results", "save_results_eval",
-              "reset_tracking"):
+for _name in ("run", "process", "pre_process", "build_dict_out", "show_results", "save_results", "save_results_eval"):
     setattr(MultiCategoryDetector, _name, _single_category(_name))
+setattr(MultiCategoryDetector, "reset_tracking", _single_category("reset_tracking"))
 del _name
 
 
-def _check_checkpoint(model, path, category):
+def _load_categories(det, opt, checkpoints, who):
+    """The shared set-up of MultiCategoryDetector / MultiCategoryTracker: checks the categories and checkpoints, loads
+    every checkpoint to the host and makes `det` an ObjectPoseDetector of opt without a device model (the multi-model
+    plan, created by det.engine, holds the weights)."""
+    cats = list(checkpoints.keys())
+    if not 1 <= len(cats) <= _lib.CP_MAX_MODELS:
+        raise ValueError("%s: 1..%d categories, got %d" % (who, _lib.CP_MAX_MODELS, len(cats)))
+    for c in cats:
+        decode_params(opt, c=c)                  # raises on an unknown category
+    weights = []
+    for c in cats:
+        m = create_model(opt.arch, opt.heads, opt.head_conv, opt)
+        _check_checkpoint(m, checkpoints[c], c, who)
+        m = load_model(m, checkpoints[c])
+        weights.append({k: v.detach().cpu() for k, v in m.state_dict().items()})
+    det._plan_cfg = dict(arch=m._arch(), heads=m.heads, head_conv=m.head_conv, tracking=m.tracking_inputs,
+                         tracking_task_gru=m.use_convGRU and m.tracking_task, precision=m.precision)
+    base = copy.copy(opt)
+    base.load_model = ""
+    ObjectPoseDetector.__init__(det, base, model=m)
+    det.model = None                             # the plan holds the weights; only the host copies are kept
+    det.categories = cats
+    det._weights = weights
+    det._prms = [decode_params(opt, c=c, test_scale=1.0) for c in cats]
+    det._eng = None
+
+
+def _check_checkpoint(model, path, category, who="MultiCategoryDetector"):
     """The checkpoint must hold exactly the tensors of `model` (same architecture, heads and head_conv): one plan runs
     every category's weights through the same schedule."""
     sd = _load_checkpoint(path)["state_dict"]
@@ -852,5 +977,5 @@ def _check_checkpoint(model, path, category):
     want = {k: tuple(v.shape) for k, v in model.state_dict().items()}
     if got != want:
         diff = sorted(set(got.items()) ^ set(want.items()))[:4]
-        raise ValueError("MultiCategoryDetector: the checkpoint of '%s' (%s) does not match the architecture, heads and "
-                         "head_conv of opt (first differences: %s)" % (category, path, diff))
+        raise ValueError("%s: the checkpoint of '%s' (%s) does not match the architecture, heads and "
+                         "head_conv of opt (first differences: %s)" % (who, category, path, diff))

@@ -136,7 +136,9 @@ def _device_view(ptr, n, device):
 class Engine(object):
     """One native plan.  models > 1 (cp_plan_create_multi): `models` checkpoints of the same architecture run over the
     same frames, every layer one launch for all of them; load each with load_state_dict(sd, model=m).  forward / infer
-    outputs then carry a leading [models] axis."""
+    outputs then carry a leading [models] axis.  With tracking=True and models > 1 (cp_plan_create_multi_track) every
+    model also takes its own previous-frame heat maps: pre_hm [models,B,1,H,W] and pre_hm_hp [models,B,8,H,W], while
+    the frames and pre_img stay [B,...]."""
 
     def __init__(self, arch, heads, head_conv, max_batch, height, width, device_index, tracking=False,
                  tracking_task_gru=False, precision="fp32", models=1):
@@ -162,8 +164,9 @@ class Engine(object):
             cfg.head_channels[i] = int(self.heads[self.head_names[i]])
         self._cfg = cfg
         plan = ctypes.c_void_p()
+        create = self.L.cp_plan_create_multi_track if self.tracking and self.models > 1 else self.L.cp_plan_create_multi
         with torch.cuda.device(self.device):
-            _lib.check(self.L.cp_plan_create_multi(ctypes.byref(cfg), self.models, ctypes.byref(plan)), "cp_plan_create")
+            _lib.check(create(ctypes.byref(cfg), self.models, ctypes.byref(plan)), "cp_plan_create")
         self.plan = plan
         self.weights_sig = None
         self.forward_launches = int(self.L.cp_plan_forward_launches(plan))
@@ -220,9 +223,10 @@ class Engine(object):
         if self.tracking:
             if pre_img is None or pre_hm is None or pre_hm_hp is None:
                 raise ValueError("a tracking plan needs pre_img, pre_hm and pre_hm_hp")
+            lead = self._lead(B)          # the heat maps are per model on a multi-model plan
             xs += [self._dev(pre_img, "pre_img", (B, 3, self.height, self.width)),
-                   self._dev(pre_hm, "pre_hm", (B, 1, self.height, self.width)),
-                   self._dev(pre_hm_hp, "pre_hm_hp", (B, 8, self.height, self.width))]
+                   self._dev(pre_hm, "pre_hm", lead + (1, self.height, self.width)),
+                   self._dev(pre_hm_hp, "pre_hm_hp", lead + (8, self.height, self.width))]
         else:
             xs += [None, None, None]
         return B, xs
@@ -358,14 +362,18 @@ class Engine(object):
                 self._out_tensor(heads_out[n], "heads_out[%s]" % n, self._head_shape(B, c), torch.float32)
             hp = (ctypes.c_void_p * len(self.head_names))(*[heads_out[n].data_ptr() for n in self.head_names])
         with torch.cuda.device(self.device):
-            if self.models > 1:
+            if self.models > 1 and self.tracking:
+                arr = (_lib.CpDecodeParams * self.models)(*prms)
+                rc = self.L.cp_infer_multi_track(self.plan, B, _ptr(xs[0]), _ptr(xs[1]), _ptr(xs[2]), _ptr(xs[3]), arr,
+                                                 _ptr(meta), hp, _ptr(dets), _ptr(poses), _ptr(n_valid), _stream())
+            elif self.models > 1:
                 arr = (_lib.CpDecodeParams * self.models)(*prms)
                 rc = self.L.cp_infer_multi(self.plan, B, _ptr(xs[0]), arr, _ptr(meta), hp, _ptr(dets), _ptr(poses),
                                            _ptr(n_valid), _stream())
             else:
                 rc = self.L.cp_infer(self.plan, B, _ptr(xs[0]), _ptr(xs[1]), _ptr(xs[2]), _ptr(xs[3]), ctypes.byref(prm),
                                      _ptr(meta), hp, _ptr(dets), _ptr(poses), _ptr(n_valid), _stream())
-        _lib.check(rc, "cp_infer_multi" if self.models > 1 else "cp_infer")
+        _lib.check(rc, ("cp_infer_multi_track" if self.tracking else "cp_infer_multi") if self.models > 1 else "cp_infer")
         return dets, poses, n_valid
 
 

@@ -131,39 +131,60 @@ def seed_records(dets, opt):
     return out
 
 
+def _tracker_config(opt, cat, streams, max_tracks, device_index):
+    """cp_tracker_config of category `cat` (its visible_thresh and opt.conf_border[cat])."""
+    border = _opt(opt, "conf_border", {cat: [3, 9]})
+    border = border[cat] if isinstance(border, dict) else border
+    cfg = _lib.CpTrackerConfig()
+    cfg.streams, cfg.max_tracks = streams, max_tracks
+    cfg.kalman = int(bool(_opt(opt, "kalman", True)))
+    cfg.scale_pool = int(bool(_opt(opt, "scale_pool", True)))
+    cfg.use_pnp = int(bool(_opt(opt, "use_pnp", True)))
+    cfg.hps_uncertainty = int(bool(_opt(opt, "hps_uncertainty", True)))
+    cfg.max_age = int(_opt(opt, "max_age", 5))
+    cfg.visible_thresh = _VISIBLE[cat]
+    cfg.opencv_return = int(bool(_opt(opt, "show_axes", False)))
+    cfg.render_hm_mode = int(_opt(opt, "render_hm_mode", 1))
+    cfg.render_hmhp_mode = int(_opt(opt, "render_hmhp_mode", 2))
+    cfg.device = device_index
+    cfg.new_thresh = float(_opt(opt, "new_thresh", 0.3))
+    cfg.pre_thresh = float(_opt(opt, "pre_thresh", -1))
+    cfg.R = float(_opt(opt, "R", 20))
+    cfg.conf_lo, cfg.conf_hi = float(border[0]), float(border[1])
+    cfg.hungarian = int(bool(_opt(opt, "hungarian", False)))
+    return cfg
+
+
 class Tracker(object):
-    def __init__(self, opt, streams=1, device=None, max_tracks=_lib.CP_MAX_K):
+    """`streams` video streams of opt.c, or, with `categories` (a list of category names), `streams` slots of every
+    category in one tracker (cp_tracker_create_multi): tracker stream m * streams + s is slot s of categories[m], with
+    that category's visible_thresh and opt.conf_border[category] (when conf_border is a dict).  The device entry points
+    then address all len(categories) * streams streams (self.streams), one step advancing every one of them."""
+
+    def __init__(self, opt, streams=1, device=None, max_tracks=_lib.CP_MAX_K, categories=None):
         self.L = _lib.load()
         self.opt = opt
-        self.streams = int(streams)
         self.max_tracks = int(max_tracks)
         self.device = torch.device(device if device is not None else "cuda")
         if self.device.index is None:
             self.device = torch.device("cuda", torch.cuda.current_device())
-        cat = _opt(opt, "c", "chair")
-        border = _opt(opt, "conf_border", {cat: [3, 9]})
-        border = border[cat] if isinstance(border, dict) else border
-        cfg = _lib.CpTrackerConfig()
-        cfg.streams, cfg.max_tracks = self.streams, self.max_tracks
-        cfg.kalman = int(bool(_opt(opt, "kalman", True)))
-        cfg.scale_pool = int(bool(_opt(opt, "scale_pool", True)))
-        cfg.use_pnp = int(bool(_opt(opt, "use_pnp", True)))
-        cfg.hps_uncertainty = int(bool(_opt(opt, "hps_uncertainty", True)))
-        cfg.max_age = int(_opt(opt, "max_age", 5))
-        cfg.visible_thresh = _VISIBLE[cat]
-        cfg.opencv_return = int(bool(_opt(opt, "show_axes", False)))
-        cfg.render_hm_mode = int(_opt(opt, "render_hm_mode", 1))
-        cfg.render_hmhp_mode = int(_opt(opt, "render_hmhp_mode", 2))
-        cfg.device = self.device.index
-        cfg.new_thresh = float(_opt(opt, "new_thresh", 0.3))
-        cfg.pre_thresh = float(_opt(opt, "pre_thresh", -1))
-        cfg.R = float(_opt(opt, "R", 20))
-        cfg.conf_lo, cfg.conf_hi = float(border[0]), float(border[1])
-        cfg.hungarian = int(bool(_opt(opt, "hungarian", False)))
-        self._cfg = cfg
+        self.categories = list(categories) if categories is not None else [_opt(opt, "c", "chair")]
+        if not 1 <= len(self.categories) <= _lib.CP_MAX_MODELS:
+            raise ValueError("Tracker: 1..%d categories, got %d" % (_lib.CP_MAX_MODELS, len(self.categories)))
+        for c in self.categories if categories is not None else ():
+            if c not in _VISIBLE:
+                raise ValueError("Tracker: unknown category '%s' (cuboid_pnp_shell.py:59-66)" % c)
+        self.slots = int(streams)                        # streams per category
+        self.streams = self.slots * len(self.categories)
+        cfgs = [_tracker_config(opt, c, self.slots, self.max_tracks, self.device.index) for c in self.categories]
+        self._cfg = cfgs[0]
         h = ctypes.c_void_p()
         with torch.cuda.device(self.device):
-            _lib.check(self.L.cp_tracker_create(ctypes.byref(cfg), ctypes.byref(h)), "cp_tracker_create")
+            if categories is None:
+                rc = self.L.cp_tracker_create(ctypes.byref(cfgs[0]), ctypes.byref(h))
+            else:
+                rc = self.L.cp_tracker_create_multi((_lib.CpTrackerConfig * len(cfgs))(*cfgs), len(cfgs), ctypes.byref(h))
+            _lib.check(rc, "cp_tracker_create")
         self._h = h
         self.meta = None
         self._rows = None          # host copy of the latest step: (rows [B,T,320], n [B])

@@ -110,10 +110,17 @@ int cp_plan_destroy(cp_plan* plan);
  * of a call at `batch` frames are [num_models * batch, ...] and model m's are a contiguous slice of them.
  *   - images (and pre_img ...) and meta rows are [batch, ...]: every model reads the same frames, nothing is copied.
  *   - head_out[i] of cp_forward / cp_plan_profile / cp_plan_run_ops is [num_models, batch, C, H/4, W/4].
- *   - tracking configs take num_models == 1 only.
+ *   - tracking configs take num_models == 1 only here; several tracking models go through cp_plan_create_multi_track.
  * cp_plan_load_weights_model fills model `model` (cp_plan_load_weights fills model 0); running before every model is
  * loaded returns CP_ERR_NOT_LOADED. */
 int cp_plan_create_multi(const cp_config* cfg, int32_t num_models, cp_plan** out);
+/* A multi-model plan of `num_models` TRACKING models (cfg->tracking must be 1, else CP_ERR_INVALID; 1..CP_MAX_MODELS
+ * models, both archs).  Every category tracks its own objects, so its previous-frame heat maps are its own:
+ *   - images and pre_img are [batch, 3, H, W], shared by every model, as in cp_plan_create_multi;
+ *   - pre_hm is [num_models, batch, 1, H, W] and pre_hm_hp [num_models, batch, 8, H, W]: model m reads slice m.
+ * This layout holds for cp_forward, cp_plan_profile, cp_plan_run_ops and cp_infer_multi_track; outputs are
+ * [num_models, batch, ...] as in cp_plan_create_multi, and the schedule has the launches of a one-model tracking plan. */
+int cp_plan_create_multi_track(const cp_config* cfg, int32_t num_models, cp_plan** out);
 int cp_plan_load_weights_model(cp_plan* plan, int32_t model, const char* const* names, const void* const* dev_ptrs,
                                const int64_t* numel, int32_t n, void* stream);
 int32_t cp_plan_num_models(const cp_plan* plan);
@@ -301,6 +308,13 @@ int cp_infer(cp_plan* plan, int32_t batch, const float* images, const float* pre
  * [num_models, batch, K, CP_DETS_RECORD]; poses [num_models, batch, K, CP_POSE_RECORD]; n_valid [num_models, batch]. */
 int cp_infer_multi(cp_plan* plan, int32_t batch, const float* images, const cp_decode_params* prms, const double* meta,
                    float* const* heads_out, float* dets, float* poses, int32_t* n_valid, void* stream);
+/* cp_infer_multi for a plan of cp_plan_create_multi_track, with its four tracking inputs (images / pre_img [batch, ...],
+ * pre_hm / pre_hm_hp [num_models, batch, ...]).  prms, meta [batch] and the outputs as in cp_infer_multi: the pose records
+ * are [num_models, batch, K, CP_POSE_RECORD], which is the stream order of a cp_tracker_create_multi tracker of
+ * num_models categories x batch streams.  cp_infer_multi refuses tracking plans. */
+int cp_infer_multi_track(cp_plan* plan, int32_t batch, const float* images, const float* pre_img, const float* pre_hm,
+                         const float* pre_hm_hp, const cp_decode_params* prms, const double* meta, float* const* heads_out,
+                         float* dets, float* poses, int32_t* n_valid, void* stream);
 
 /* Offsets (in floats) inside one CP_POSE_RECORD slot. */
 enum cp_pose_field {
@@ -393,6 +407,13 @@ typedef struct cp_tracker_config {
 } cp_tracker_config;
 
 int cp_tracker_create(const cp_tracker_config* cfg, cp_tracker** out);
+/* One tracker for `models` object categories (1..CP_MAX_MODELS) of cfgs[0].streams streams each: tracker stream m * S + s
+ * (S = cfgs[0].streams) is stream s of category m and uses cfgs[m].visible_thresh, conf_lo and conf_hi; the configs may
+ * differ in those three fields only (else CP_ERR_INVALID, before anything is allocated).  Every other call sees a tracker
+ * of models * S streams: cp_tracker_step advances all of them in one launch (two with hungarian), the stream maps of the
+ * _ex calls address them as m * S + s, and the meta rows stay one per batch row (a frame's row repeated per category).
+ * cp_tracker_create is this call with models = 1. */
+int cp_tracker_create_multi(const cp_tracker_config* cfgs, int32_t models, cp_tracker** out);
 int cp_tracker_destroy(cp_tracker* trk);
 /* Tracker.reset(): forget every track of stream `index` (or of all streams when index < 0). */
 int cp_tracker_reset(cp_tracker* trk, int32_t index, void* stream);
