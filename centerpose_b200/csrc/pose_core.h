@@ -912,7 +912,10 @@ CP_HDN int soft_nms(double* bbox, double* score, int* perm, int n, double thresh
 }
 
 // ---- gpfit.moments on a (nr x nc) window of doubles (row-major, ld = nc) ----------------
-// returns false when the reference would raise (empty window / NaN centroid)
+// returns false when the reference would raise: an empty window, a NaN centroid, a centroid row / column index outside
+// the window, or a start point that fitgaussian's least_squares(bounds=(0, [inf, nr, nc, inf, inf])) rejects as
+// infeasible (a negative height, a centroid outside [0, nr] x [0, nc], a NaN or negative width).  Raw (opt.mse_loss)
+// windows with a non-positive total or a non-positive centroid row / column sum end here.
 CP_HDN bool moments(const double* w, int nr, int nc, double* height, double* x, double* y, double* wx, double* wy) {
   if (nr <= 0 || nc <= 0) return false;
   double total = 0, sx = 0, sy = 0, mx = w[0];
@@ -936,7 +939,7 @@ CP_HDN bool moments(const double* w, int nr, int nc, double* height, double* x, 
     num += fabs((r - yc) * (r - yc) * v);
     den += v;
   }
-  *wx = sqrt(num / den);  // abs() is applied to the summed numerator in the reference; all terms share the sign of v
+  const double wxv = sqrt(num / den);  // np.abs(...).sum(): abs per term (raw windows mix signs), then the sum
   num = 0;
   den = 0;
   for (int c = 0; c < nc; ++c) {
@@ -944,7 +947,12 @@ CP_HDN bool moments(const double* w, int nr, int nc, double* height, double* x, 
     num += fabs((c - xc) * (c - xc) * v);
     den += v;
   }
-  *wy = sqrt(num / den);
+  const double wyv = sqrt(num / den);
+  // the bounds test of least_squares, in_bounds(x0, lb, ub); every comparison with NaN is false
+  if (!(mx >= 0.0 && xc >= 0.0 && xc <= (double)nr && yc >= 0.0 && yc <= (double)nc && wxv >= 0.0 && wyv >= 0.0))
+    return false;
+  *wx = wxv;
+  *wy = wyv;
   *height = mx;
   *x = xc;
   *y = yc;

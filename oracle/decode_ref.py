@@ -16,7 +16,7 @@ Reference lines followed (relative to /root/reference/src/lib):
   models/decode.py:40-68             _topk_channel / _topk       -> topk_channel / topk_classes
   models/utils.py:43-47              _transpose_and_gather_feat  -> gather
   models/decode.py:72-375            object_pose_decode(Inference=True) -> decode
-  utils/gpfit.py:13-41               moments / fitgaussian(max_nfev=1) -> moments
+  utils/gpfit.py:13-41               moments / fitgaussian(max_nfev=1) -> moments / fit_start
   utils/image.py:23-74               transform_preds / get_affine_transform -> map_to_image
   utils/post_process.py:12-68        object_pose_post_process    -> post_process
   detectors/object_pose.py:27-124    soft_nms_nvidia(method=2)   -> soft_nms
@@ -126,11 +126,35 @@ def moments(data):
     return height, x, y, width_x, width_y
 
 
-def process_heads(heads):
-    """object_pose.py:136-138 -- returns a copy with sigmoid applied to hm, hm_hp."""
+def fit_start(data):
+    """What `fitgaussian` (gpfit.py:29-41) returns for a window, or None where the reference raises.  Raises are:
+    `moments` indexing a row / column that does not exist (int(NaN), a centroid of exactly rows or cols), and
+    least_squares rejecting the start point, because it is outside bounds=(0, [inf, rows, cols, inf, inf]) or NaN.
+    Otherwise max_nfev=1 returns the start point; a zero width is made strictly feasible."""
+    rows, cols = np.asarray(data).shape
+    with np.errstate(divide="ignore", invalid="ignore"):
+        try:
+            height, x, y, width_x, width_y = moments(data)
+        except (ValueError, IndexError, OverflowError):
+            return None
+    if not (height >= 0 and 0 <= x <= rows and 0 <= y <= cols and width_x >= 0 and width_y >= 0):
+        return None
+    # least_squares(max_nfev=1) only makes x0 strictly feasible
+    width_x = max(width_x, 1e-10) if width_x == 0 else width_x
+    width_y = max(width_y, 1e-10) if width_y == 0 else width_y
+    return height, x, y, width_x, width_y
+
+
+def process_heads(heads, apply_sigmoid=1):
+    """object_pose.py:136-138 -- returns a copy with sigmoid applied as `cp_decode_params.apply_sigmoid` says:
+    0 = hm and hm_hp are probabilities already (neither is touched), 1 = both are logits, 2 = only hm is a logit
+    (opt.mse_loss: hm_hp is decoded raw, and the moment window and the height read see the raw values)."""
+    if apply_sigmoid not in (0, 1, 2):
+        raise ValueError("apply_sigmoid must be 0, 1 or 2")
     out = {k: np.ascontiguousarray(v, dtype=F32) for k, v in heads.items()}
-    out["hm"] = sigmoid_f32(out["hm"])
-    if "hm_hp" in out:
+    if apply_sigmoid != 0:
+        out["hm"] = sigmoid_f32(out["hm"])
+    if "hm_hp" in out and apply_sigmoid == 1:
         out["hm_hp"] = sigmoid_f32(out["hm_hp"])
     return out
 
@@ -222,10 +246,10 @@ def decode(heads, prm):
                     big = np.zeros((H + 2 * ran, W + 2 * ran))
                     big[ran:H + ran, ran:W + ran] = data
                     win = big[int(fy):int(fy + 2 * ran + 1), int(fx):int(fx + 2 * ran + 1)]
-                    height, mu_x, mu_y, std_x, std_y = moments(win)
-                    # least_squares(max_nfev=1) only makes x0 strictly feasible
-                    std_x = max(std_x, 1e-10) if std_x == 0 else std_x
-                    std_y = max(std_y, 1e-10) if std_y == 0 else std_y
+                    fit = fit_start(win)
+                    if fit is None:         # the reference raises here; the -10000 sentinels stay (DESIGN.md 5)
+                        continue
+                    height, mu_x, mu_y, std_x, std_y = fit
                 else:
                     mu_x = ran
                     mu_y = ran

@@ -171,6 +171,41 @@ def test_moments_matches_oracle(pose_host):
         assert ok and np.allclose(out5, ref, rtol=1e-12, atol=1e-14)
 
 
+def test_moments_rejects_what_fitgaussian_rejects(pose_host):
+    """Raw (opt.mse_loss) windows mix signs: a non-positive total or centroid row / column sum, a centroid outside the
+    window, a NaN or negative width.  pose::moments accepts exactly the windows whose start point
+    scipy.optimize.least_squares takes with fitgaussian's bounds (decode_ref.fit_start), with the same values."""
+    opt = pytest.importorskip("scipy.optimize")
+    rng = np.random.default_rng(14)
+    seen = {True: 0, False: 0}
+    for trial in range(400):
+        nr, nc = int(rng.integers(1, 12)), int(rng.integers(1, 12))
+        w = rng.uniform(-0.3, 1.0, size=(nr, nc)) * (rng.uniform(size=(nr, nc)) > 0.3)
+        w[rng.uniform(size=(nr, nc)) < 0.2] = -rng.uniform(0.0, 0.5)
+        w = np.ascontiguousarray(w)
+        out5 = np.zeros(5)
+        ok = bool(pose_host.host_moments(w.ctypes.data_as(dp), nr, nc, out5.ctypes.data_as(dp)))
+        fit = decode_ref.fit_start(w)
+        assert ok == (fit is not None), (trial, w)
+        seen[ok] += 1
+        with np.errstate(all="ignore"):
+            try:
+                ref = decode_ref.moments(w)
+            except (ValueError, IndexError, OverflowError):
+                assert not ok
+                continue
+        x0 = np.array(ref, np.float64)
+        fitgaussian = lambda: opt.least_squares(lambda p: np.zeros(1), x0, bounds=(0, [np.inf, nr, nc, np.inf, np.inf]),
+                                                max_nfev=1)
+        if not ok:
+            with pytest.raises(ValueError):
+                fitgaussian()
+            continue
+        assert np.allclose(out5, ref, rtol=1e-12, atol=1e-14)
+        fitgaussian()
+    assert seen[True] > 20 and seen[False] > 20, seen
+
+
 def test_cuboid_vertices_order(pose_host):
     scale = np.array([0.4, 0.8, 1.2], np.float32)
     V = np.zeros(24)

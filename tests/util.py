@@ -145,13 +145,13 @@ def decode_case_geometry(g):
     return np.array([256., 256.], np.float32), 512.0, [1.0], True
 
 
-def oracle_records(heads_b, prm, cam, width, height, c, s, L, scale=1):
-    """Full oracle pipeline for one image -> (dets dict, [n,192] records)."""
+def oracle_records(heads_b, prm, cam, width, height, c, s, L, scale=1, apply_sigmoid=1):
+    """Full oracle pipeline for one image -> (dets dict, [n,192] records).  apply_sigmoid: as in cp_decode_params."""
     from oracle import decode_ref, pnp_ref
     import sys
     sys.path.insert(0, ROOT)
     from oracle.make_golden import result_to_record
-    dets = decode_ref.decode(decode_ref.process_heads(heads_b), prm)
+    dets = decode_ref.decode(decode_ref.process_heads(heads_b, apply_sigmoid), prm)
     pp = decode_ref.post_process(dets, c, s, heads_b["hm"].shape[1], heads_b["hm"].shape[2], scale=scale)
     for i, d in enumerate(pp):
         d["_k"] = i
