@@ -56,7 +56,12 @@ EXPORTS = [
     "cp_preprocess_ragged", "cp_tracker_step_ex", "cp_tracker_render_ex2", "cp_tracker_seed_ex",
     "cp_plan_create_multi", "cp_plan_load_weights_model", "cp_plan_num_models", "cp_plan_op_desc_model", "cp_infer_multi",
     "cp_plan_create_multi_track", "cp_infer_multi_track", "cp_tracker_create_multi",
+    "cp_plan_create_ex", "cp_plan_memory", "cp_plan_allocations",
 ]
+
+# cp_plan_create_ex / cp_plan_memory flags
+CP_PLAN_REUSE_ACTIVATIONS = 1
+CP_PLAN_MULTI_TRACK = 2
 
 # cp_op_family
 FAM_NONE, FAM_IGEMM_FP32, FAM_STEM, FAM_CONV3_C16, FAM_IGEMM_UMMA, FAM_CONV_TMA, FAM_DCN_TMA = 0, 1, 2, 3, 4, 5, 6
@@ -93,6 +98,14 @@ class CpOpDesc(ctypes.Structure):
 
 class CpOpLaunch(ctypes.Structure):
     _fields_ = [(n, ctypes.c_int32) for n in ("family", "BN", "ksplit", "grid")]
+
+
+class CpMemoryInfo(ctypes.Structure):
+    _fields_ = [(n, ctypes.c_int64) for n in ("activation_bytes", "weight_bytes", "tile_bytes", "workspace_bytes")]
+
+
+class CpActAlloc(ctypes.Structure):
+    _fields_ = [("floats", ctypes.c_int64), ("off", ctypes.c_int64), ("first", ctypes.c_int32), ("last", ctypes.c_int32)]
 
 
 class CpConfig(ctypes.Structure):
@@ -204,6 +217,10 @@ def load():
     L.cp_infer_multi_track.argtypes = [vp, i32, vp, vp, vp, vp, ctypes.POINTER(CpDecodeParams), vp, ctypes.POINTER(vp), vp,
                                        vp, vp, vp]
     L.cp_tracker_create_multi.argtypes = [ctypes.POINTER(CpTrackerConfig), i32, ctypes.POINTER(vp)]
+    L.cp_plan_create_ex.argtypes = [ctypes.POINTER(CpConfig), i32, ctypes.c_uint32, ctypes.POINTER(vp)]
+    L.cp_plan_memory.argtypes = [ctypes.POINTER(CpConfig), i32, ctypes.c_uint32, ctypes.POINTER(CpMemoryInfo)]
+    L.cp_plan_allocations.argtypes = [ctypes.POINTER(CpConfig), i32, ctypes.c_uint32, ctypes.POINTER(CpActAlloc), i32,
+                                      ctypes.POINTER(i32)]
     for name in EXPORTS:
         fn = getattr(L, name)
         if name not in ("cp_version", "cp_last_error", "cp_plan_bytes", "cp_plan_forward_launches",

@@ -213,7 +213,8 @@ inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
 // Every kernel of the forward schedule therefore (a) signals `launch_dependents` at its very start, so the NEXT kernel's
 // CTAs are placed on an SM the moment a CTA of this one retires, and (b) executes `griddep_wait()` before its first
 // read of an activation / first global write.  What runs before the wait touches only per-plan constants (weights,
-// biases) and the CTA's own shared memory.  Kernels launched without the attribute see both instructions as no-ops.
+// biases) and the CTA's own shared memory.  A plan that reuses arena memory (CP_PLAN_REUSE_ACTIVATIONS) relies on this: the
+// next launch may overwrite what this one reads (DESIGN §4).  Kernels launched without the attribute see both instructions as no-ops.
 // g_pdl is set by run_forward (plan.cu) around the op loop; stand-alone ops (cp_conv2d ...) pack their weights on the
 // stream right before the launch and therefore never use it.  CP_NO_PDL=1 disables it (A/B runs).
 extern thread_local int g_pdl;

@@ -17,6 +17,7 @@
 #include <string>
 #include <vector>
 
+#include "arena_pack.h"
 #include "common.cuh"
 
 namespace cp {
@@ -38,6 +39,7 @@ struct Act {
   int C = 0, H = 0, W = 0;
   int stride = 0;  // pixel stride in floats
   int ext = -1;    // >= 0: external NCHW input index (0 images, 1 pre_img, 2 pre_hm, 3 pre_hm_hp)
+  int buf = -1;    // >= 0: the arena allocation it is a view of (cp_plan::bufs)
 };
 
 enum OpType { OP_IGEMM, OP_MAXPOOL, OP_UPADD, OP_GN_RELU, OP_GRU };
@@ -56,9 +58,9 @@ struct Op {
   int kh = 1, kw = 1, stride = 1, pad = 0, Cin = 0, Cout = 0, CoutPad = 0, Kpad = 0;
   size_t w_off = 0, b_off = 0;
   int w_ld = 0;            // leading dimension of the fp32 packed weight matrix
-  ConvKernel kernel;       // chosen once the arena exists (choose_kernels)
+  ConvKernel kernel;       // chosen before the arena exists (select_kernels)
   size_t tile_off = 0;     // bytes into the plan's tensor-core weight-tile buffer
-  TmaMaps maps;            // conv_tma / dcn_tma: encoded once the arena exists
+  TmaMaps maps;            // conv_tma / dcn_tma: encoded once the arena exists (encode_maps)
   std::vector<int> head_children;   // merged heads 3x3 conv: indices of the per-head 1x1 ops that read its slices
   bool fuse_heads = false;          // ... which run inside its epilogue (conv_tma.cu), never touching HBM
   bool fused_away = false;          // this 1x1 op is computed by its parent's epilogue
@@ -126,6 +128,12 @@ struct cp_plan {
   // bit e set: external input e holds one image per model and frame ([models, batch, ...]) rather than one per frame
   // (cp_plan_create_multi_track: pre_hm and pre_hm_hp, which each category draws from its own tracks)
   unsigned ext_per_model = 0;
+  // Every arena allocation of the schedule (Builder::new_act) with the ops over which it is live, and its offset in
+  // floats.  Without CP_PLAN_REUSE_ACTIVATIONS the offsets are the bump allocation's: every allocation has its own
+  // memory.  With it they come from arena_pack(), and an allocation no op touches has none.
+  bool reuse = false;
+  std::vector<ArenaAlloc> bufs;
+  std::vector<size_t> buf_off;
 };
 
 namespace cp {
@@ -148,7 +156,12 @@ struct Builder {
     a.H = H;
     a.W = W;
     a.stride = C;
-    act_cur += ((size_t)B * H * W * C + 63) / 64 * 64;
+    a.buf = (int)P->bufs.size();
+    ArenaAlloc al;
+    al.floats = arena_align((size_t)B * H * W * C);
+    P->bufs.push_back(al);
+    P->buf_off.push_back(act_cur);
+    act_cur += al.floats;
     return a;
   }
 
@@ -372,6 +385,8 @@ int build_graph(cp_plan* P) {
   b.B = P->B * P->models;
   P->ops.clear();
   P->jobs.clear();
+  P->bufs.clear();
+  P->buf_off.clear();
   const int H = P->H, W = P->W;
 
   auto ext = [&](int idx, int C) {
@@ -619,22 +634,24 @@ void igemm_params(const cp_plan* P, const Op& op, int batch, const float* const 
   }
 }
 
-// The kernel of every conv op (needs the arena: the choice reads the op's residual), its weight-tile offset, its tensor
-// maps, and which per-head 1x1 convs run inside the epilogue of their merged heads conv.
-int choose_kernels(cp_plan* P) {
+// The kernel of every conv op, its weight-tile offset, and which per-head 1x1 convs run inside the epilogue of their
+// merged heads conv.  Runs before the arena exists (cp_plan_memory has no device at all): the choice reads shapes,
+// strides and whether a residual is added, never an address.
+void select_kernels(cp_plan* P) {
   // 16-channel layers (level0 / level1): 133 K single-tile CTAs of almost no MMA work are dominated by the fixed per-CTA
   // cost of a tensor-core kernel -> keep them, and the NCHW stems, on CUDA cores
   const ConvPolicy pol{true, !P->no_dcn_tma, true, true};
   const float* const no_ext[4] = {nullptr, nullptr, nullptr, nullptr};
+  static const float residual_present = 0.f;      // a residual at arena offset 0 of a null arena would read as none
   P->umma_bytes = 0;
   for (auto& op : P->ops) {
     if (op.type != OP_IGEMM) continue;
     IgemmParams p;
     igemm_params(P, op, P->B, no_ext, nullptr, &p);
+    if (op.has_res) p.residual = &residual_present;
     op.kernel = select_conv_kernel(p, P->cfg.precision, pol);
     op.tile_off = P->umma_bytes;
     P->umma_bytes += (op.kernel.wbytes + 1023) / 1024 * 1024;
-    if (int rc = conv_encode(op.kernel, p, P->B * P->models, &op.maps)) return rc;
   }
   // The per-head 1x1 convs move into the epilogue of the merged heads conv when that one runs on conv_tma: hidden =
   // relu(conv3x3) never reaches HBM (3.7 GB of writes + 3.7 GB of reads and seven launches at batch 32).  In both
@@ -654,6 +671,82 @@ int choose_kernels(cp_plan* P) {
     op.fuse_heads = true;
     for (int ci : op.head_children) P->ops[ci].fused_away = true;
   }
+}
+
+// The op range over which each arena allocation is live, from the ops that run (a fused-away 1x1 does not, and a
+// fused heads conv never stores its hidden tile), then, with CP_PLAN_REUSE_ACTIVATIONS, the packed offsets.  The head
+// buffers stay live to the end of the call: cp_infer decodes them after the last op.
+void layout_arena(cp_plan* P) {
+  for (auto& b : P->bufs) b.first = b.last = -1;
+  auto touch = [P](const Act& a, int i) {
+    if (a.buf < 0) return;
+    ArenaAlloc& b = P->bufs[a.buf];
+    if (b.first < 0) b.first = i;
+    b.last = std::max(b.last, i);
+  };
+  const int end = (int)P->ops.size();
+  for (int i = 0; i < end; ++i) {
+    const Op& op = P->ops[i];
+    if (op.fused_away) continue;
+    switch (op.type) {
+      case OP_IGEMM:
+        for (int s = 0; s < op.nsrc; ++s) touch(op.src[s], i);
+        if (op.has_res) touch(op.res, i);
+        if (op.mode == IGEMM_DCN) touch(op.om, i);
+        if (op.out_head >= 0) touch(P->head_bufs[op.out_head], i);
+        else if (!op.fuse_heads) touch(op.out, i);
+        if (op.fuse_heads)
+          for (int c : op.head_children) touch(P->head_bufs[P->ops[c].out_head], i);
+        break;
+      case OP_MAXPOOL:
+        touch(op.src[0], i);
+        touch(op.out, i);
+        break;
+      case OP_UPADD:
+        touch(op.src[0], i);
+        if (op.has_skip) touch(op.skip, i);
+        touch(op.out, i);
+        break;
+      case OP_GN_RELU:
+        touch(op.out, i);
+        break;
+      case OP_GRU:
+        touch(op.gx, i);
+        if (!op.first_step) {
+          touch(op.gh, i);
+          touch(op.gprev, i);
+        }
+        touch(op.out, i);
+        break;
+    }
+  }
+  for (const Act& h : P->head_bufs) touch(h, end);
+  if (!P->reuse) return;
+  std::vector<size_t> off;
+  P->act_floats = arena_pack(P->bufs, &off);
+  auto move = [&](Act& a) {
+    if (a.buf >= 0) a.off = a.off - P->buf_off[a.buf] + off[a.buf];
+  };
+  for (auto& op : P->ops) {
+    for (Act& a : op.src) move(a);
+    for (Act* a : {&op.out, &op.res, &op.om, &op.skip, &op.gx, &op.gh, &op.gprev}) move(*a);
+  }
+  for (Act& h : P->head_bufs) move(h);
+  P->buf_off = off;
+}
+
+// False for an allocation that got no memory (a reuse plan's merged heads hidden tile when the 1x1s are fused).
+bool has_memory(const cp_plan* P, const Act& a) { return a.buf < 0 || !P->reuse || P->bufs[a.buf].first >= 0; }
+
+// The tensor maps of the TMA convolutions: they hold the arena addresses.
+int encode_maps(cp_plan* P) {
+  const float* const no_ext[4] = {nullptr, nullptr, nullptr, nullptr};
+  for (auto& op : P->ops) {
+    if (op.type != OP_IGEMM) continue;
+    IgemmParams p;
+    igemm_params(P, op, P->B, no_ext, nullptr, &p);
+    if (int rc = conv_encode(op.kernel, p, P->B * P->models, &op.maps)) return rc;
+  }
   return CP_OK;
 }
 
@@ -668,7 +761,7 @@ const char* cp_last_error(void) { return cp::g_last_error.c_str(); }
 
 int cp_plan_create(const cp_config* cfg, cp_plan** out) { return cp_plan_create_multi(cfg, 1, out); }
 
-static int create_plan(const cp_config* cfg, int32_t num_models, unsigned ext_per_model, cp_plan** out);
+static int create_plan(const cp_config* cfg, int32_t num_models, uint32_t flags, cp_plan** out);
 
 int cp_plan_create_multi(const cp_config* cfg, int32_t num_models, cp_plan** out) {
   if (!cfg || !out) return fail(CP_ERR_INVALID, "cp_plan_create: null argument");
@@ -685,10 +778,31 @@ int cp_plan_create_multi_track(const cp_config* cfg, int32_t num_models, cp_plan
   if (cfg->tracking != 1) return fail(CP_ERR_INVALID, "cp_plan_create_multi_track: needs a tracking config (tracking = 1)");
   if (num_models < 1 || num_models > CP_MAX_MODELS)
     return fail(CP_ERR_INVALID, "cp_plan_create_multi_track: num_models must be in 1..CP_MAX_MODELS");
-  return create_plan(cfg, num_models, (1u << 2) | (1u << 3), out);      // pre_hm, pre_hm_hp: one per model and frame
+  return create_plan(cfg, num_models, CP_PLAN_MULTI_TRACK, out);
 }
 
-static int create_plan(const cp_config* cfg, int32_t num_models, unsigned ext_per_model, cp_plan** out) {
+// the arguments cp_plan_create_ex and cp_plan_memory share (the config itself is checked by plan_layout)
+static int check_ex_args(const cp_config* cfg, int32_t num_models, uint32_t flags, const char* fn) {
+  const std::string f(fn);
+  if (!cfg) return fail(CP_ERR_INVALID, f + ": null argument");
+  if (flags & ~(uint32_t)(CP_PLAN_REUSE_ACTIVATIONS | CP_PLAN_MULTI_TRACK)) return fail(CP_ERR_INVALID, f + ": unknown flags");
+  if (num_models < 1 || num_models > CP_MAX_MODELS) return fail(CP_ERR_INVALID, f + ": num_models must be in 1..CP_MAX_MODELS");
+  if ((flags & CP_PLAN_MULTI_TRACK) && cfg->tracking != 1)
+    return fail(CP_ERR_INVALID, f + ": CP_PLAN_MULTI_TRACK needs a tracking config (tracking = 1)");
+  if (cfg->tracking && num_models > 1 && !(flags & CP_PLAN_MULTI_TRACK))
+    return fail(CP_ERR_INVALID, f + ": several tracking models need CP_PLAN_MULTI_TRACK");
+  return CP_OK;
+}
+
+int cp_plan_create_ex(const cp_config* cfg, int32_t num_models, uint32_t flags, cp_plan** out) {
+  if (!out) return fail(CP_ERR_INVALID, "cp_plan_create_ex: null argument");
+  if (int rc = check_ex_args(cfg, num_models, flags, "cp_plan_create_ex")) return rc;
+  return create_plan(cfg, num_models, flags, out);
+}
+
+// Everything about a plan that needs no device: the checked config, the schedule, the kernel of every op, the weight
+// and tile sizes and the arena layout.
+static int plan_layout(cp_plan* P, const cp_config* cfg, int32_t num_models, uint32_t flags) {
   if (cfg->arch != CP_ARCH_DLA34 && cfg->arch != CP_ARCH_DLAV1_34)
     return fail(CP_ERR_INVALID, "cp_plan_create: unknown arch");
   if (!known_precision(cfg->precision))
@@ -701,7 +815,6 @@ static int create_plan(const cp_config* cfg, int32_t num_models, unsigned ext_pe
     return fail(CP_ERR_INVALID, "cp_plan_create: head_conv must be a positive multiple of 64");
   if (cfg->arch == CP_ARCH_DLAV1_34 && cfg->head_conv != 256)
     return fail(CP_ERR_INVALID, "cp_plan_create: dlav1 GroupNorm path needs head_conv == 256");
-  std::unique_ptr<cp_plan> P(new cp_plan());
   P->cfg = *cfg;
   for (int i = 0; i < cfg->num_heads; ++i) {
     if (!cfg->head_names[i] || cfg->head_channels[i] <= 0 || cfg->head_channels[i] > 16)
@@ -711,11 +824,30 @@ static int create_plan(const cp_config* cfg, int32_t num_models, unsigned ext_pe
   for (int i = 0; i < cfg->num_heads; ++i) P->cfg.head_names[i] = P->head_names[i].c_str();
   P->B = cfg->max_batch;
   P->models = num_models;
-  P->ext_per_model = ext_per_model;
+  P->ext_per_model = (flags & CP_PLAN_MULTI_TRACK) ? (1u << 2) | (1u << 3) : 0u;   // pre_hm, pre_hm_hp: one per model and frame
+  P->reuse = (flags & CP_PLAN_REUSE_ACTIVATIONS) != 0;
   P->model_loaded.assign(num_models, 0);
   P->H = cfg->height;
   P->W = cfg->width;
   if (const char* e = getenv("CP_NO_DCN_TMA")) P->no_dcn_tma = atoi(e) != 0;
+  if (int rc = build_graph(P)) return rc;
+  select_kernels(P);
+  layout_arena(P);
+  return CP_OK;
+}
+
+static void plan_memory(const cp_plan* P, cp_memory_info* m) {
+  const bool splitk = P->cfg.precision == CP_PREC_TF32X3 || P->cfg.precision == CP_PREC_TF32;
+  m->activation_bytes = (int64_t)(P->act_floats * sizeof(float));
+  m->weight_bytes = (int64_t)(P->w_floats * P->models * sizeof(float));
+  m->tile_bytes = (int64_t)(P->umma_bytes * P->models);
+  m->workspace_bytes = (int64_t)(sizeof(double) * gn_workspace_doubles(P->B * P->models) +
+                                 (splitk ? kSplitkWsFloats * sizeof(float) : 0));
+}
+
+static int create_plan(const cp_config* cfg, int32_t num_models, uint32_t flags, cp_plan** out) {
+  std::unique_ptr<cp_plan> P(new cp_plan());
+  if (int rc = plan_layout(P.get(), cfg, num_models, flags)) return rc;
   // the plan lives on cfg->device; the caller's current device is restored on every exit path
   struct DeviceGuard {
     int prev = -1;
@@ -725,13 +857,11 @@ static int create_plan(const cp_config* cfg, int32_t num_models, unsigned ext_pe
   } guard;
   CP_CUDA_CHECK(cudaGetDevice(&guard.prev));
   CP_CUDA_CHECK(cudaSetDevice(cfg->device));
-  int rc = build_graph(P.get());
-  if (rc) return rc;
   CP_CUDA_CHECK(cudaMalloc(&P->act, P->act_floats * sizeof(float)));
   CP_CUDA_CHECK(cudaMalloc(&P->wts, P->w_floats * num_models * sizeof(float)));
   CP_CUDA_CHECK(cudaMemset(P->wts, 0, P->w_floats * num_models * sizeof(float)));
   CP_CUDA_CHECK(cudaMalloc(&P->gn_stats, sizeof(double) * gn_workspace_doubles(P->B * num_models)));
-  if ((rc = choose_kernels(P.get()))) return rc;
+  if (int rc = encode_maps(P.get())) return rc;
   if (P->umma_bytes) CP_CUDA_CHECK(cudaMalloc(&P->umma_wts, P->umma_bytes * num_models));
   if (cfg->precision == CP_PREC_TF32X3 || cfg->precision == CP_PREC_TF32) {
     CP_CUDA_CHECK(cudaMalloc(&P->splitk_ws, kSplitkWsFloats * sizeof(float)));
@@ -740,6 +870,34 @@ static int create_plan(const cp_config* cfg, int32_t num_models, unsigned ext_pe
   for (auto& op : P->ops) n += op.fused_away ? 0 : ((op.type == OP_GN_RELU) ? 3 : 1);
   P->launches = n;
   *out = P.release();
+  return CP_OK;
+}
+
+int cp_plan_memory(const cp_config* cfg, int32_t num_models, uint32_t flags, cp_memory_info* out) {
+  if (!out) return fail(CP_ERR_INVALID, "cp_plan_memory: null argument");
+  if (int rc = check_ex_args(cfg, num_models, flags, "cp_plan_memory")) return rc;
+  cp_plan P;      // host side only: nothing is allocated on a device
+  if (int rc = plan_layout(&P, cfg, num_models, flags)) return rc;
+  plan_memory(&P, out);
+  return CP_OK;
+}
+
+int cp_plan_allocations(const cp_config* cfg, int32_t num_models, uint32_t flags, cp_act_alloc* out, int32_t max_allocs,
+                        int32_t* n_allocs) {
+  if (!out || !n_allocs) return fail(CP_ERR_INVALID, "cp_plan_allocations: null argument");
+  if (int rc = check_ex_args(cfg, num_models, flags, "cp_plan_allocations")) return rc;
+  cp_plan P;
+  if (int rc = plan_layout(&P, cfg, num_models, flags)) return rc;
+  const int n = (int)std::min(P.bufs.size(), (size_t)std::max(max_allocs, 0));
+  for (int i = 0; i < n; ++i) {
+    const ArenaAlloc& b = P.bufs[i];
+    const bool mem = !P.reuse || b.first >= 0;
+    out[i].floats = mem ? (int64_t)b.floats : 0;
+    out[i].off = mem ? (int64_t)P.buf_off[i] : -1;
+    out[i].first = b.first;
+    out[i].last = b.last;
+  }
+  *n_allocs = (int32_t)P.bufs.size();
   return CP_OK;
 }
 
@@ -1038,7 +1196,10 @@ int cp_plan_op_desc_model(const cp_plan* P, int32_t model, int32_t i, cp_op_desc
   const Op& op = P->ops[i];
   const float* const wts = P->wts + (size_t)model * P->w_floats;
   const size_t first = (size_t)model * P->B;
-  auto act_desc = [first](const Act& a, cp_act_desc* ad) { ::act_desc(a, ad, first); };
+  auto act_desc = [P, first](const Act& a, cp_act_desc* ad) {
+    ::act_desc(a, ad, first);
+    if (!has_memory(P, a)) ad->off = -1;
+  };
   memset(d, 0, sizeof(*d));
   snprintf(d->name, sizeof(d->name), "%s", op.name.c_str());
   d->kind = (int)op.type * 10 + (op.type == OP_IGEMM ? op.mode : 0);

@@ -818,7 +818,8 @@ class MultiCategoryDetector(ObjectPoseDetector):
         _load_categories(self, opt, checkpoints, "MultiCategoryDetector")
 
     def engine(self, batch, height, width):
-        """The multi-model plan for this input shape (created on first use, rebuilt for a larger batch)."""
+        """The multi-model plan for this input shape (created on first use, rebuilt for a larger batch), its activation
+        arena packed by liveness (Engine reuse_activations)."""
         eng = self._eng
         if eng is None or eng.max_batch < batch or (eng.height, eng.width) != (height, width):
             if eng is not None:
@@ -827,7 +828,8 @@ class MultiCategoryDetector(ObjectPoseDetector):
             c = self._plan_cfg
             eng = Engine(c["arch"], c["heads"], c["head_conv"], max(batch, 1), height, width,
                          dev.index if dev.index is not None else torch.cuda.current_device(), tracking=c["tracking"],
-                         tracking_task_gru=c["tracking_task_gru"], precision=c["precision"], models=len(self._weights))
+                         tracking_task_gru=c["tracking_task_gru"], precision=c["precision"], models=len(self._weights),
+                         reuse_activations=True)
             for i, sd in enumerate(self._weights):
                 eng.load_state_dict(sd, model=i)
             self._eng = eng

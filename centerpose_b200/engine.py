@@ -133,15 +133,59 @@ def _device_view(ptr, n, device):
         return torch.as_tensor(_CudaArray(ptr, n), device=device)
 
 
+def _config(arch, heads, head_conv, max_batch, height, width, device_index=0, tracking=False, tracking_task_gru=False,
+            precision="fp32"):
+    """(cp_config, the encoded head names it points to: keep them alive while the config is used)."""
+    cfg = _lib.CpConfig()
+    cfg.arch = {"dla_34": _lib.CP_ARCH_DLA34, "dlav1_34": _lib.CP_ARCH_DLAV1_34}[arch]
+    cfg.tracking = int(tracking)
+    cfg.tracking_task_gru = int(tracking_task_gru)
+    cfg.max_batch, cfg.height, cfg.width = int(max_batch), int(height), int(width)
+    cfg.precision = _lib.PRECISIONS[precision]
+    cfg.device = device_index
+    cfg.head_conv = int(head_conv)
+    names = [n.encode() for n in heads]
+    cfg.num_heads = len(names)
+    for i, (n, c) in enumerate(zip(names, heads.values())):
+        cfg.head_names[i] = n
+        cfg.head_channels[i] = int(c)
+    return cfg, names
+
+
+def _plan_flags(tracking, models, reuse_activations):
+    return ((_lib.CP_PLAN_MULTI_TRACK if tracking and models > 1 else 0) |
+            (_lib.CP_PLAN_REUSE_ACTIVATIONS if reuse_activations else 0))
+
+
+def plan_memory(arch, heads, head_conv, max_batch, height, width, tracking=False, tracking_task_gru=False,
+                precision="fp32", models=1, reuse_activations=False):
+    """cp_plan_memory: the device bytes an Engine of these arguments owns, computed on the host without a GPU.
+    dict(activation, weights, tiles, workspace, total)."""
+    L = _lib.load()
+    cfg, keep = _config(arch, dict(heads), head_conv, max_batch, height, width, 0, tracking, tracking_task_gru, precision)
+    m = _lib.CpMemoryInfo()
+    _lib.check(L.cp_plan_memory(ctypes.byref(cfg), int(models), _plan_flags(tracking, int(models), reuse_activations),
+                                ctypes.byref(m)), "cp_plan_memory")
+    out = dict(activation=int(m.activation_bytes), weights=int(m.weight_bytes), tiles=int(m.tile_bytes),
+               workspace=int(m.workspace_bytes))
+    out["total"] = sum(out.values())
+    return out
+
+
 class Engine(object):
     """One native plan.  models > 1 (cp_plan_create_multi): `models` checkpoints of the same architecture run over the
     same frames, every layer one launch for all of them; load each with load_state_dict(sd, model=m).  forward / infer
     outputs then carry a leading [models] axis.  With tracking=True and models > 1 (cp_plan_create_multi_track) every
     model also takes its own previous-frame heat maps: pre_hm [models,B,1,H,W] and pre_hm_hp [models,B,8,H,W], while
-    the frames and pre_img stay [B,...]."""
+    the frames and pre_img stay [B,...].
+
+    reuse_activations=True (CP_PLAN_REUSE_ACTIVATIONS) packs the activation arena by liveness: the results are the same
+    bits in a fraction of the memory, but the arena no longer holds every layer's output after a call, which the
+    per-layer diagnostics (op_descs, arena, run_ops from the middle of the schedule) read.  `memory` is the byte
+    breakdown of the plan (plan_memory)."""
 
     def __init__(self, arch, heads, head_conv, max_batch, height, width, device_index, tracking=False,
-                 tracking_task_gru=False, precision="fp32", models=1):
+                 tracking_task_gru=False, precision="fp32", models=1, reuse_activations=False):
         self.L = _lib.load()
         self.models = int(models)
         self.heads = dict(heads)
@@ -149,28 +193,20 @@ class Engine(object):
         self.max_batch, self.height, self.width = int(max_batch), int(height), int(width)
         self.device = torch.device("cuda", device_index)
         self.tracking = bool(tracking)
-        cfg = _lib.CpConfig()
-        cfg.arch = {"dla_34": _lib.CP_ARCH_DLA34, "dlav1_34": _lib.CP_ARCH_DLAV1_34}[arch]
-        cfg.tracking = int(tracking)
-        cfg.tracking_task_gru = int(tracking_task_gru)
-        cfg.max_batch, cfg.height, cfg.width = self.max_batch, self.height, self.width
-        cfg.precision = _lib.PRECISIONS[precision]
-        cfg.device = device_index
-        cfg.head_conv = int(head_conv)
-        cfg.num_heads = len(self.head_names)
-        self._names = [n.encode() for n in self.head_names]
-        for i, n in enumerate(self._names):
-            cfg.head_names[i] = n
-            cfg.head_channels[i] = int(self.heads[self.head_names[i]])
+        self.reuse_activations = bool(reuse_activations)
+        cfg, self._names = _config(arch, self.heads, head_conv, max_batch, height, width, device_index, tracking,
+                                   tracking_task_gru, precision)
         self._cfg = cfg
         plan = ctypes.c_void_p()
-        create = self.L.cp_plan_create_multi_track if self.tracking and self.models > 1 else self.L.cp_plan_create_multi
+        flags = _plan_flags(self.tracking, self.models, self.reuse_activations)
         with torch.cuda.device(self.device):
-            _lib.check(create(ctypes.byref(cfg), self.models, ctypes.byref(plan)), "cp_plan_create")
+            _lib.check(self.L.cp_plan_create_ex(ctypes.byref(cfg), self.models, flags, ctypes.byref(plan)), "cp_plan_create")
         self.plan = plan
         self.weights_sig = None
         self.forward_launches = int(self.L.cp_plan_forward_launches(plan))
         self.plan_bytes = int(self.L.cp_plan_bytes(plan))
+        self.memory = plan_memory(arch, heads, head_conv, max_batch, height, width, tracking, tracking_task_gru, precision,
+                                  self.models, self.reuse_activations)
 
     def close(self):
         if getattr(self, "plan", None):

@@ -121,6 +121,43 @@ int cp_plan_create_multi(const cp_config* cfg, int32_t num_models, cp_plan** out
  * This layout holds for cp_forward, cp_plan_profile, cp_plan_run_ops and cp_infer_multi_track; outputs are
  * [num_models, batch, ...] as in cp_plan_create_multi, and the schedule has the launches of a one-model tracking plan. */
 int cp_plan_create_multi_track(const cp_config* cfg, int32_t num_models, cp_plan** out);
+
+/* ---- plan flags: cp_plan_create_ex / cp_plan_memory ----------------------------------------------------------------
+ * CP_PLAN_REUSE_ACTIVATIONS: activations whose lifetimes do not overlap share arena memory.  An allocation is live from
+ *   the op that first writes it to the op that last reads it; the head buffers cp_infer decodes stay live to the end of
+ *   the call.  The plan computes bit for bit what a plan without the flag computes, in a fraction of the arena (README).
+ *   Consequences for the diagnostics: the cp_act_desc offsets of different ops may coincide, an allocation no op touches
+ *   (the merged heads' hidden tile when the 1x1s are fused into its epilogue) reports off = -1, and cp_plan_run_ops is
+ *   valid for op ranges whose inputs are still live, for example when stepping from op 0 in order.
+ * CP_PLAN_MULTI_TRACK: the per-model pre_hm / pre_hm_hp layout of cp_plan_create_multi_track (needs cfg->tracking = 1;
+ *   a tracking config of several models needs it). */
+#define CP_PLAN_REUSE_ACTIVATIONS 1u
+#define CP_PLAN_MULTI_TRACK 2u
+/* cp_plan_create_multi (flags 0) or cp_plan_create_multi_track (CP_PLAN_MULTI_TRACK) with flags; unknown flag bits return
+ * CP_ERR_INVALID.  The three creators above are this call with those flags. */
+int cp_plan_create_ex(const cp_config* cfg, int32_t num_models, uint32_t flags, cp_plan** out);
+/* Device memory a plan of these arguments owns, in bytes, computed on the host without a device (to size a deployment
+ * before creating the plan).  cp_plan_bytes of the created plan is activation_bytes + weight_bytes.  The decode workspace
+ * cp_infer sizes on its first call is not included (cp_decode_workspace_bytes). */
+typedef struct cp_memory_info {
+  int64_t activation_bytes;  /* the activation arena                                                               */
+  int64_t weight_bytes;      /* packed fp32 weights of every model                                                 */
+  int64_t tile_bytes;        /* pre-swizzled tensor-core weight tiles of every model                               */
+  int64_t workspace_bytes;   /* GroupNorm statistics and split-K partial sums                                      */
+} cp_memory_info;
+int cp_plan_memory(const cp_config* cfg, int32_t num_models, uint32_t flags, cp_memory_info* out);
+/* The arena allocations of such a plan (host only, like cp_plan_memory): allocation i takes `floats` floats at `off`
+ * floats into the arena and is live over ops [first, last] of the schedule (last = cp_plan_num_ops: to the end of the
+ * call; first = -1 when no op touches it); floats = 0 and off = -1 when it gets no memory.  Fills the first max_allocs
+ * records at most; *n_allocs receives the number of allocations. */
+typedef struct cp_act_alloc {
+  int64_t floats;
+  int64_t off;
+  int32_t first, last;
+} cp_act_alloc;
+int cp_plan_allocations(const cp_config* cfg, int32_t num_models, uint32_t flags, cp_act_alloc* out, int32_t max_allocs,
+                        int32_t* n_allocs);
+
 int cp_plan_load_weights_model(cp_plan* plan, int32_t model, const char* const* names, const void* const* dev_ptrs,
                                const int64_t* numel, int32_t n, void* stream);
 int32_t cp_plan_num_models(const cp_plan* plan);
@@ -230,7 +267,7 @@ int cp_plan_run_ops(cp_plan* plan, int32_t batch, int32_t first, int32_t last, c
                     const float* pre_hm, const float* pre_hm_hp, float* const* head_out, void* stream,
                     cp_op_launch* info);
 
-/* Arena / weight bytes owned by the plan (for logging). */
+/* Arena / weight bytes owned by the plan (for logging): activation_bytes + weight_bytes of cp_plan_memory. */
 int64_t cp_plan_bytes(const cp_plan* plan);
 /* Number of kernel launches one cp_forward enqueues (for bench gpu_launches). */
 int32_t cp_plan_forward_launches(const cp_plan* plan);
