@@ -10,7 +10,7 @@ Public surface (mirrors the reference's, see INTEGRATION.md):
 The hot path lives in libcenterpose_b200.so (include/centerpose_b200.h); there is
 no PyTorch or CPU fallback.
 """
-from .model import create_model, load_model, save_model, DLASegB200          # noqa: F401
+from .model import create_model, load_model, save_model, DLASegB200, PoseResNetB200          # noqa: F401
 from .detector import MultiCategoryDetector, MultiCategoryTracker, ObjectPoseDetector, detector_factory  # noqa: F401
 from .engine import Engine, InferGraph, decode_pnp, decode_params, make_meta, dcn_v2_forward, dcn_v2_backward, preprocess, preprocess_ragged, conv2d_nhwc  # noqa: F401
 from .opts import default_opt                                                # noqa: F401

@@ -19,6 +19,7 @@ CP_MAX_MODELS = 16
 
 CP_ARCH_DLA34 = 0
 CP_ARCH_DLAV1_34 = 1
+CP_ARCH_RES_18, CP_ARCH_RES_34, CP_ARCH_RES_50, CP_ARCH_RES_101, CP_ARCH_RES_152 = 2, 3, 4, 5, 6
 CP_PREC_FP32 = 0
 CP_PREC_TF32X3 = 1
 CP_PREC_BF16 = 2

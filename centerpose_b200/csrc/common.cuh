@@ -39,8 +39,18 @@ extern thread_local long long g_launch_counter;      // kernels launched by this
 enum IgemmMode {
   IGEMM_NCHW_SCALAR = 0,  // generic k -> (tap, c) decode, NCHW input (7x7 stems, Cin = 1/3/8)
   IGEMM_NHWC_VEC = 1,     // Cin of every source % 16 == 0, float4 gathers
-  IGEMM_DCN = 2           // 3x3 s1 p1 modulated deformable sampling, single NHWC source
+  IGEMM_DCN = 2,          // 3x3 s1 p1 modulated deformable sampling, single NHWC source
+  // Dense ConvTranspose2d(k 4, stride 2, pad 1) over one NHWC source (msra_resnet.py:208-233), by sub-pixel phases:
+  // output pixel (2y + py, 2x + px) only sees input rows y + dy(py, a) and columns x + dx(px, b), a, b in {0, 1}, with
+  // dy(0, a) = -a (ky = 1 + 2a) and dy(1, a) = 1 - a (ky = 2a), the same for columns.  Each phase (py, px) is an
+  // implicit GEMM over the INPUT grid with kh = kw = 2 taps, K = 4 Cin (row (2a + b) Cin + ci); the weight matrix is
+  // the four phases' [Kpad][CoutPad] blocks in the order py * 2 + px (launch_pack_deconv_weight), and Hout / Wout are
+  // the output's 2 Hin / 2 Win.  The phase is a grid coordinate.
+  IGEMM_DECONV = 3
 };
+// deconv phases: input offset and kernel row of tap a of phase p (the same for columns)
+__host__ __device__ __forceinline__ int deconv_dy(int p, int a) { return p ? 1 - a : -a; }
+__host__ __device__ __forceinline__ int deconv_ky(int p, int a) { return p ? 2 * a : 1 + 2 * a; }
 
 struct IgemmParams {
   const float* src[4];
@@ -157,6 +167,11 @@ int launch_igemm_umma(const IgemmParams& p, int prec, cudaStream_t stream, Launc
 
 // elementwise / data-movement kernels (elementwise.cu)
 int launch_maxpool2(const float* in, float* out, int B, int H, int W, int C, cudaStream_t s);
+// MaxPool2d(3, 2, 1) over NHWC (msra_resnet.py:120), out = [residual +] maxpool(in); H, W even, C % 4 == 0
+int launch_maxpool3s2(const float* in, const float* residual, float* out, int B, int H, int W, int C, cudaStream_t s);
+// ConvTranspose2d weight [Cin][Cout][4][4] -> the four phase blocks of IGEMM_DECONV, [4][Kpad][CoutPad], times scale
+int launch_pack_deconv_weight(const float* w_io44, const float* scale, float* out, int Cin, int Cout, int CoutPad, int Kpad,
+                              cudaStream_t s);
 // upsample_add / group_norm_relu: image n uses the weights at (n / ipm) * wstride floats (multi-model plans; ipm = B:
 // one model)
 int launch_upsample_add(const float* in, const float* wgt_kkc, const float* skip, float* out, int B,

@@ -20,9 +20,10 @@ ConvKernel select_conv_kernel(const IgemmParams& p, int32_t precision, const Con
       return {CP_FAM_CONV_TMA, x3, pol.round_out && !x3, tma_tile_n(p.CoutPad, x3), tma_cslab(p, x3),
               tma_weight_bytes(p.Cin, p.kh * p.kw, p.CoutPad, x3)};
     const bool gx3 = gather_x3(precision);
+    const int phases = p.mode == IGEMM_DECONV ? 4 : 1;      // a transposed conv has one tile set per phase
     if (umma_supported(p, gx3))
       return {CP_FAM_IGEMM_UMMA, gx3, false, umma_tile_n(p.CoutPad, gx3), 0,
-              umma_weight_bytes(p.kh * p.kw * p.Cin, p.CoutPad, gx3)};
+              phases * umma_weight_bytes(p.kh * p.kw * p.Cin, p.CoutPad, gx3)};
     if (!pol.cuda_core_fallback) return {CP_FAM_NONE};
   }
   return {stem_supported(p) ? CP_FAM_STEM : (conv3_c16_supported(p) ? CP_FAM_CONV3_C16 : CP_FAM_IGEMM_FP32)};
@@ -40,8 +41,16 @@ int conv_pack(const ConvKernel& k, const IgemmParams& p, int ld, void* tiles, cu
     case CP_FAM_DCN_TMA:
     case CP_FAM_CONV_TMA:
       return launch_pack_tma_weight(p.wgt, ld, p.Cin, p.kh * p.kw, p.Cout, p.CoutPad, k.x3, k.cslab, k.BN, tiles, s);
-    case CP_FAM_IGEMM_UMMA:
-      return launch_pack_umma_weight(p.wgt, ld, p.kh * p.kw * p.Cin, p.Cout, p.CoutPad, k.x3, tiles, s);
+    case CP_FAM_IGEMM_UMMA: {
+      // IGEMM_DECONV: the phases' [Kpad][ld] blocks follow each other, and so do their tile sets
+      const int phases = p.mode == IGEMM_DECONV ? 4 : 1;
+      const size_t phase_bytes = k.wbytes / phases;
+      for (int ph = 0; ph < phases; ++ph)
+        if (int rc = launch_pack_umma_weight(p.wgt + (size_t)ph * p.Kpad * ld, ld, p.kh * p.kw * p.Cin, p.Cout, p.CoutPad,
+                                             k.x3, (unsigned char*)tiles + ph * phase_bytes, s))
+          return rc;
+      return CP_OK;
+    }
     default:
       return CP_OK;
   }

@@ -39,6 +39,47 @@ __global__ void maxpool2_kernel(const float4* __restrict__ in, float4* __restric
   }
 }
 
+// ---- MaxPool2d(3, 2, 1) (msra_resnet.py:120, 132, 139, 147) [+ residual: the tracking stems' sum, :242-247] ----
+// The -inf padding never wins: every window holds its centre (2 oy, 2 ox).  The sum is residual + pool, the order of
+// `x = x + self.pre_img_layer(pre_img)`.
+__global__ void maxpool3s2_kernel(const float4* __restrict__ in, const float4* __restrict__ res, float4* __restrict__ out,
+                                  int B, int H, int W, int C4) {
+  griddep_launch_dependents();      // PDL (common.cuh)
+  griddep_wait();
+  const int Ho = H / 2, Wo = W / 2;
+  const size_t total = (size_t)B * Ho * Wo * C4;
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int c = i % C4;
+    size_t t = i / C4;
+    const int ox = t % Wo;
+    t /= Wo;
+    const int oy = t % Ho;
+    const int n = t / Ho;
+    float4 r = __ldg(in + ((size_t)(n * H + 2 * oy) * W + 2 * ox) * C4 + c);
+    for (int dy = -1; dy <= 1; ++dy) {
+      const int iy = 2 * oy + dy;
+      if (iy < 0 || iy >= H) continue;
+      for (int dx = -1; dx <= 1; ++dx) {
+        const int ix = 2 * ox + dx;
+        if (ix < 0 || ix >= W) continue;
+        const float4 v = __ldg(in + ((size_t)(n * H + iy) * W + ix) * C4 + c);
+        r.x = fmaxf(r.x, v.x);
+        r.y = fmaxf(r.y, v.y);
+        r.z = fmaxf(r.z, v.z);
+        r.w = fmaxf(r.w, v.w);
+      }
+    }
+    if (res) {
+      const float4 a = __ldg(res + i);
+      r.x = a.x + r.x;
+      r.y = a.y + r.y;
+      r.z = a.z + r.z;
+      r.w = a.w + r.w;
+    }
+    out[i] = r;
+  }
+}
+
 // ---- depthwise ConvTranspose2d(C, C, 2f, stride f, pad f/2, groups C) + skip add
 //      (pose_dla_dcn.py:402-405, :415-417).  Every output pixel receives exactly
 //      2 x 2 taps; weights are packed [ky][kx][C].
@@ -105,6 +146,26 @@ __global__ void pack_conv_weight_kernel(const float* __restrict__ w, const float
       }
     }
     out[(size_t)k * ld + colOff + co] = v;
+  }
+}
+
+// ConvTranspose2d [Cin][Cout][4][4] -> phase p = py * 2 + px: [k = (2a + b) * Cin + ci][CoutPad] holds
+// w[ci][co][ky(py, a)][kx(px, b)] * scale[co] (IGEMM_DECONV, common.cuh); rows K..Kpad and columns Cout.. are zero.
+__global__ void pack_deconv_weight_kernel(const float* __restrict__ w, const float* __restrict__ scale, float* __restrict__ out,
+                                          int Cin, int Cout, int CoutPad, int Kpad) {
+  const size_t total = (size_t)4 * Kpad * CoutPad;
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int co = i % CoutPad;
+    const size_t r = i / CoutPad;
+    const int k = r % Kpad, ph = r / Kpad;
+    float v = 0.f;
+    if (co < Cout && k < 4 * Cin) {
+      const int ci = k % Cin, tap = k / Cin;
+      const int ky = deconv_ky(ph >> 1, tap >> 1), kx = deconv_ky(ph & 1, tap & 1);
+      v = w[(((size_t)ci * Cout + co) * 4 + ky) * 4 + kx];
+      if (scale) v *= scale[co];
+    }
+    out[i] = v;
   }
 }
 
@@ -273,6 +334,23 @@ int launch_maxpool2(const float* in, float* out, int B, int H, int W, int C, cud
   CP_CUDA_CHECK(launch_kernel(maxpool2_kernel, dim3(blocks_for(total)), dim3(TPB), 0, s, (const float4*)in, (float4*)out, B, H, W,
                               C / 4));
   CP_LAUNCH_CHECK("maxpool2_kernel");
+  return CP_OK;
+}
+
+int launch_maxpool3s2(const float* in, const float* res, float* out, int B, int H, int W, int C, cudaStream_t s) {
+  if (C % 4 || H % 2 || W % 2) return fail(CP_ERR_INVALID, "maxpool3s2: C%4, H%2, W%2");
+  size_t total = (size_t)B * (H / 2) * (W / 2) * (C / 4);
+  CP_CUDA_CHECK(launch_kernel(maxpool3s2_kernel, dim3(blocks_for(total)), dim3(TPB), 0, s, (const float4*)in,
+                              (const float4*)res, (float4*)out, B, H, W, C / 4));
+  CP_LAUNCH_CHECK("maxpool3s2_kernel");
+  return CP_OK;
+}
+
+int launch_pack_deconv_weight(const float* w, const float* scale, float* out, int Cin, int Cout, int CoutPad, int Kpad,
+                              cudaStream_t s) {
+  const size_t total = (size_t)4 * Kpad * CoutPad;
+  pack_deconv_weight_kernel<<<blocks_for(total), TPB, 0, s>>>(w, scale, out, Cin, Cout, CoutPad, Kpad);
+  CP_LAUNCH_CHECK("pack_deconv_weight_kernel");
   return CP_OK;
 }
 

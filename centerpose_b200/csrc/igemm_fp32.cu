@@ -5,6 +5,8 @@
 //     of up to four sources (DLA Root nodes, pose_dla_dcn.py:160-168),
 //   * the 7x7 stems reading the user's NCHW input directly
 //     (pose_dla_dcn.py:234-238, 253-271),
+//   * the dense 4x4 stride-2 transposed convolutions of the ResNet up-sampling (msra_resnet.py:208-233), as four
+//     sub-pixel phase GEMMs over the input (IGEMM_DECONV, common.cuh; the phase is blockIdx.z),
 //   * the DCNv2 modulated deformable 3x3 convolution: the A tile is produced by
 //     bilinear sampling at offset positions and multiplied by the mask, exactly
 //     the arithmetic of dcn_v2_im2col_cuda.cu:25-54,125-195, but the
@@ -50,14 +52,18 @@ __global__ void __launch_bounds__(NT, 2) igemm_fp32_kernel(const IgemmParams p) 
   const int tid = threadIdx.x;
   const int tx = tid & 15;
   const int ty = tid >> 4;
+  // the GEMM rows: output pixels, or for IGEMM_DECONV the input pixels of phase blockIdx.z = py * 2 + px
+  constexpr bool DECONV = MODE == IGEMM_DECONV;
+  const int Hg = DECONV ? p.Hin : p.Hout, Wg = DECONV ? p.Win : p.Wout;
+  const int py = blockIdx.z >> 1, px = blockIdx.z & 1;
   // row blocks are cut per model (IgemmParams::ipm); rows from M on belong to the next model
-  const int Mm = MULTI ? p.ipm * p.Hout * p.Wout : 0;
+  const int Mm = MULTI ? p.ipm * Hg * Wg : 0;
   const int bpm = MULTI ? (Mm + BM - 1) / BM : 1;
   const int model = MULTI ? blockIdx.x / bpm : 0;
-  const int M = MULTI ? (model + 1) * Mm : p.B * p.Hout * p.Wout;
+  const int M = MULTI ? (model + 1) * Mm : p.B * Hg * Wg;
   const int m0 = MULTI ? model * Mm + (blockIdx.x - model * bpm) * BM : blockIdx.x * BM;
   const int n0 = blockIdx.y * BN;
-  const float* const wgt = MULTI ? p.wgt + (size_t)model * p.wstride : p.wgt;
+  const float* const wgt = (MULTI ? p.wgt + (size_t)model * p.wstride : p.wgt) + (size_t)blockIdx.z * p.Kpad * p.CoutPad;
   // NCHW sources are the models' shared input frames, unless each model has its own (IgemmParams::nchw_per_model)
   const int n_shared = (MULTI && !(p.nchw_per_model & 1u)) ? model * p.ipm : 0;
 
@@ -70,10 +76,10 @@ __global__ void __launch_bounds__(NT, 2) igemm_fp32_kernel(const IgemmParams p) 
     int m = m0 + r0 + i * 64;
     row[i].valid = m < M;
     int mm = row[i].valid ? m : 0;
-    row[i].ox = mm % p.Wout;
-    int t = mm / p.Wout;
-    row[i].oy = t % p.Hout;
-    row[i].n = t / p.Hout;
+    row[i].ox = mm % Wg;
+    int t = mm / Wg;
+    row[i].oy = t % Hg;
+    row[i].n = t / Hg;
   }
 
   const int ktiles = p.Kpad / BK;
@@ -112,6 +118,18 @@ __global__ void __launch_bounds__(NT, 2) igemm_fp32_kernel(const IgemmParams p) 
           v[j] = x;
         }
         a_reg[i] = make_float4(v[0], v[1], v[2], v[3]);
+      }
+    } else if (DECONV) {
+      const int tap = kt / chunks_per_tap;
+      const int c0 = (kt - tap * chunks_per_tap) * BK;
+      const int dy = deconv_dy(py, tap >> 1), dx = deconv_dy(px, tap & 1);
+#pragma unroll
+      for (int i = 0; i < 2; ++i) {
+        const int iy = row[i].oy + dy, ix = row[i].ox + dx;
+        const bool ok = row[i].valid && iy >= 0 && iy < p.Hin && ix >= 0 && ix < p.Win;
+        a_reg[i] = ok ? __ldg(reinterpret_cast<const float4*>(
+                            p.src[0] + ((size_t)(row[i].n * p.Hin + iy) * p.Win + ix) * p.srcStride[0] + c0 + kq * 4))
+                      : make_float4(0.f, 0.f, 0.f, 0.f);
       }
     } else if (MODE == IGEMM_NHWC_VEC) {
       int tap = kt / chunks_per_tap;
@@ -260,6 +278,10 @@ __global__ void __launch_bounds__(NT, 2) igemm_fp32_kernel(const IgemmParams p) 
   for (int i = 0; i < 8; ++i) {
     int m = m0 + ty * 8 + i;
     if (m >= M) continue;
+    if (DECONV) {      // input pixel (n, y, x) of phase (py, px) -> output pixel (n, 2y + py, 2x + px)
+      const int x = m % Wg, t = m / Wg;
+      m = ((t / Hg) * p.Hout + 2 * (t % Hg) + py) * p.Wout + 2 * x + px;
+    }
     float v[TN];
 #pragma unroll
     for (int j = 0; j < TN; ++j) v[j] = acc[i][j] + bias[j];
@@ -306,6 +328,7 @@ int launch_bn_models(const IgemmParams& p, dim3 grid, cudaStream_t stream) {
     case IGEMM_NCHW_SCALAR: CP_CUDA_CHECK(launch_kernel(igemm_fp32_kernel<BN, IGEMM_NCHW_SCALAR, MULTI>, grid, dim3(NT), 0, stream, p)); break;
     case IGEMM_NHWC_VEC: CP_CUDA_CHECK(launch_kernel(igemm_fp32_kernel<BN, IGEMM_NHWC_VEC, MULTI>, grid, dim3(NT), 0, stream, p)); break;
     case IGEMM_DCN: CP_CUDA_CHECK(launch_kernel(igemm_fp32_kernel<BN, IGEMM_DCN, MULTI>, grid, dim3(NT), 0, stream, p)); break;
+    case IGEMM_DECONV: CP_CUDA_CHECK(launch_kernel(igemm_fp32_kernel<BN, IGEMM_DECONV, MULTI>, grid, dim3(NT), 0, stream, p)); break;
     default: return fail(CP_ERR_INVALID, "igemm: bad mode");
   }
   CP_LAUNCH_CHECK("igemm_fp32_kernel");
@@ -316,8 +339,9 @@ template <int BN>
 int launch_bn(const IgemmParams& p0, cudaStream_t stream) {
   IgemmParams p = p0;
   p.ipm = model_ipm(p0);
-  const int Mm = p.ipm * p.Hout * p.Wout;
-  dim3 grid((Mm + BM - 1) / BM * (p.B / p.ipm), p.CoutPad / BN);
+  const bool deconv = p.mode == IGEMM_DECONV;
+  const int Mm = p.ipm * (deconv ? p.Hin * p.Win : p.Hout * p.Wout);
+  dim3 grid((Mm + BM - 1) / BM * (p.B / p.ipm), p.CoutPad / BN, deconv ? 4 : 1);
   // several models in the launch: the model-indexed instantiations; one model runs the one-model code unchanged
   return p.B > p.ipm ? launch_bn_models<BN, true>(p, grid, stream) : launch_bn_models<BN, false>(p, grid, stream);
 }
@@ -336,6 +360,9 @@ int launch_igemm_fp32(const IgemmParams& p, cudaStream_t stream) {
   }
   if (p.mode == IGEMM_DCN && (p.kh != 3 || p.kw != 3 || p.stride != 1 || p.pad != 1 || p.nsrc != 1))
     return fail(CP_ERR_INVALID, "igemm: DCN supports 3x3 stride 1 pad 1 only");
+  if (p.mode == IGEMM_DECONV &&
+      (p.kh != 2 || p.kw != 2 || p.nsrc != 1 || p.out_nchw || p.Hout != 2 * p.Hin || p.Wout != 2 * p.Win))
+    return fail(CP_ERR_INVALID, "igemm: transposed conv needs one NHWC source, 2x2 phase taps and an NHWC 2x output");
   if (!p.out_nchw && (p.outStride % 4 != 0)) return fail(CP_ERR_INVALID, "igemm: outStride % 4");
   if (p.CoutPad % 64 == 0) return launch_bn<64>(p, stream);
   if (p.CoutPad % 32 == 0) return launch_bn<32>(p, stream);

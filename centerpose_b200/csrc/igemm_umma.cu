@@ -3,7 +3,8 @@
 //   D[m, n] = sum_k A[m, k] * W[n, k]      m = output pixel, n = output channel, k = (tap, ci)
 //
 // Same contract as igemm_fp32.cu (IgemmParams: NHWC fp32 activations, channel-concatenated
-// sources, DCNv2 deformable gather, fused bias / residual / ReLU epilogue) but the contraction
+// sources, DCNv2 deformable gather, the sub-pixel phases of the 4x4 stride-2 transposed conv with the phase in
+// blockIdx.y, fused bias / residual / ReLU epilogue) but the contraction
 // runs on the tensor cores:
 //   * warps 0-7 (two threads per tile row) GATHER the A tile -- plain im2col rows or the
 //     bilinear deformable samples of dcn_v2_im2col_cuda.cu:125-195 -- convert it and write it
@@ -63,13 +64,18 @@ __global__ void __launch_bounds__(UM_THREADS, 1) igemm_umma_kernel(const IgemmPa
   // 1-D grid, n tile fastest: the CTAs that share an A row block run back to back and hit it in L2
   // (gridDim.y would overflow at 65535 row blocks: B = 32 at 512 x 512 has 65536).  Row blocks are cut per model
   // (IgemmParams::ipm) so that a block never mixes two models' weights; rows from M on belong to the next model.
+  // The GEMM rows are output pixels, or for IGEMM_DECONV the input pixels of phase blockIdx.y = py * 2 + px, whose
+  // weight tiles follow the previous phases' (common.cuh).
+  constexpr bool DECONV = MODE == IGEMM_DECONV;
+  const int Hg = DECONV ? p.Hin : p.Hout, Wg = DECONV ? p.Win : p.Wout;
+  const int py = blockIdx.y >> 1, px = blockIdx.y & 1;
   const int n_tiles = p.CoutPad / BN;
   const int n_tile = blockIdx.x % n_tiles;
-  const int Mm = MULTI ? p.ipm * p.Hout * p.Wout : 0;
+  const int Mm = MULTI ? p.ipm * Hg * Wg : 0;
   const int bpm = MULTI ? (Mm + UM_BM - 1) / UM_BM : 1;
   const int model = MULTI ? (blockIdx.x / n_tiles) / bpm : 0;
   const int m0 = MULTI ? model * Mm + ((blockIdx.x / n_tiles) - model * bpm) * UM_BM : (blockIdx.x / n_tiles) * UM_BM;
-  const int M = MULTI ? (model + 1) * Mm : p.B * p.Hout * p.Wout;
+  const int M = MULTI ? (model + 1) * Mm : p.B * Hg * Wg;
   const int K = p.kh * p.kw * p.Cin;
   const int KB = (K + T::kElems - 1) / T::kElems;
 
@@ -87,17 +93,18 @@ __global__ void __launch_bounds__(UM_THREADS, 1) igemm_umma_kernel(const IgemmPa
     // =========================== A producers: two threads per tile row, four 16-byte chunks each ===============
     {
       const unsigned char* wsrc =
-          reinterpret_cast<const unsigned char*>(p.wgt_umma) + (size_t)model * p.tstride + (size_t)n_tile * KB * b_tile_bytes;
+          reinterpret_cast<const unsigned char*>(p.wgt_umma) + (size_t)model * p.tstride +
+          ((size_t)blockIdx.y * n_tiles + n_tile) * KB * b_tile_bytes;
       const int r = tid >> 1;
       const int qbase = (tid & 1) * 4;
       const int m = m0 + r;
       const bool valid = m < M;
       int ox = 0, oy = 0, n = 0;
       if (valid) {
-        ox = m % p.Wout;
-        int t = m / p.Wout;
-        oy = t % p.Hout;
-        n = t / p.Hout;
+        ox = m % Wg;
+        int t = m / Wg;
+        oy = t % Hg;
+        n = t / Hg;
       }
       const uint32_t row_off = (uint32_t)(r >> 3) * 1024u + (uint32_t)(r & 7) * 128u;
       const uint32_t sw = (uint32_t)(r & 7);
@@ -166,7 +173,8 @@ __global__ void __launch_bounds__(UM_THREADS, 1) igemm_umma_kernel(const IgemmPa
               }
             } else {
               const int ky = tap / p.kw, kx = tap - ky * p.kw;
-              const int iy = oy * p.stride - p.pad + ky, ix = ox * p.stride - p.pad + kx;
+              const int iy = DECONV ? oy + deconv_dy(py, ky) : oy * p.stride - p.pad + ky;
+              const int ix = DECONV ? ox + deconv_dy(px, kx) : ox * p.stride - p.pad + kx;
               if (iy >= 0 && iy < p.Hin && ix >= 0 && ix < p.Win) {
                 int s = 0, cb = 0;
                 while (s + 1 < p.nsrc && c >= cb + p.srcC[s]) {
@@ -287,14 +295,19 @@ __global__ void __launch_bounds__(UM_THREADS, 1) igemm_umma_kernel(const IgemmPa
     float* dstage = reinterpret_cast<float*>(smem + (tiles0 - smem_u32(smem)) + (size_t)STAGES * stage_bytes) +
                     (size_t)c * (DRAIN_STAGE_BYTES / 4);
     auto fn = [&](int r, int cb, float (&v)[16]) {
-      const int m = m0 + c * 64 + r;
+      int m = m0 + c * 64 + r;
       const bool valid = m < M;
       int ox = 0, oy = 0, n = 0;
       if (valid) {
-        ox = m % p.Wout;
-        const int t = m / p.Wout;
-        oy = t % p.Hout;
-        n = t / p.Hout;
+        ox = m % Wg;
+        const int t = m / Wg;
+        oy = t % Hg;
+        n = t / Hg;
+        if (DECONV) {      // input pixel (n, y, x) of phase (py, px) -> output pixel (n, 2y + py, 2x + px)
+          oy = 2 * oy + py;
+          ox = 2 * ox + px;
+          m = (n * p.Hout + oy) * p.Wout + ox;
+        }
       }
       if (cb < BN) epilogue_row<16>(ep, v, valid, m, n, oy, ox, n_tile * BN + cb, col_end);
     };
@@ -357,7 +370,10 @@ __global__ void pack_umma_weight_kernel(const float* __restrict__ src, int ld, i
 int umma_tile_n(int CoutPad, int prec) { return wgmma_tile_n(CoutPad, prec == 1 ? 64 : 128); }
 
 bool umma_supported(const IgemmParams& p, int prec) {
-  if (p.mode != IGEMM_NHWC_VEC && p.mode != IGEMM_DCN) return false;
+  if (p.mode != IGEMM_NHWC_VEC && p.mode != IGEMM_DCN && p.mode != IGEMM_DECONV) return false;
+  if (p.mode == IGEMM_DECONV &&
+      (p.kh != 2 || p.kw != 2 || p.nsrc != 1 || p.out_nchw || p.Hout != 2 * p.Hin || p.Wout != 2 * p.Win))
+    return false;
   const int ch = prec == 0 ? 8 : 4;
   if (p.Cin % ch) return false;
   for (int s = 0; s < p.nsrc; ++s)
@@ -393,23 +409,26 @@ template <int PREC, int BN, bool MULTI>
 static int launch_igemm_umma_bn(const IgemmParams& p, int stages, size_t smem, int nacc, cudaStream_t stream,
                                 LaunchInfo* info) {
   void (*kern)(const IgemmParams, const int, const int) =
-      (p.mode == IGEMM_DCN) ? igemm_umma_kernel<PREC, IGEMM_DCN, BN, MULTI> : igemm_umma_kernel<PREC, IGEMM_NHWC_VEC, BN, MULTI>;
-  static PerDevice<bool, 2> configured;
-  const int slot = p.mode == IGEMM_DCN ? 1 : 0;
+      (p.mode == IGEMM_DCN)      ? igemm_umma_kernel<PREC, IGEMM_DCN, BN, MULTI>
+      : (p.mode == IGEMM_DECONV) ? igemm_umma_kernel<PREC, IGEMM_DECONV, BN, MULTI>
+                                 : igemm_umma_kernel<PREC, IGEMM_NHWC_VEC, BN, MULTI>;
+  static PerDevice<bool, 3> configured;
+  const int slot = p.mode == IGEMM_DCN ? 1 : (p.mode == IGEMM_DECONV ? 2 : 0);
   if (!configured.here(slot)) {
     CP_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     configured.here(slot) = true;
   }
   IgemmParams q = p;
   q.ipm = model_ipm(p);
-  const int Mm = q.ipm * p.Hout * p.Wout;
-  dim3 grid((unsigned)((size_t)(p.CoutPad / BN) * ((Mm + UM_BM - 1) / UM_BM) * (p.B / q.ipm)));
+  const bool deconv = p.mode == IGEMM_DECONV;
+  const int Mm = q.ipm * (deconv ? p.Hin * p.Win : p.Hout * p.Wout);
+  dim3 grid((unsigned)((size_t)(p.CoutPad / BN) * ((Mm + UM_BM - 1) / UM_BM) * (p.B / q.ipm)), deconv ? 4 : 1);
   CP_CUDA_CHECK(launch_kernel(kern, grid, dim3(UM_THREADS), smem, stream, q, stages, nacc));
   CP_LAUNCH_CHECK("igemm_umma_kernel");
   if (info) {
     info->BN = BN;
     info->ksplit = 1;
-    info->grid = grid.x;
+    info->grid = (long long)grid.x * grid.y;
   }
   return CP_OK;
 }

@@ -9,6 +9,11 @@
 //   pose_dla_dcn.py:457-570  DLASeg: ida_up, heads (3x3 -> [GN] -> ReLU -> 1x1), convGRU routing
 //   DCNv2/dcn_v2.py:97-128   DCN = 3x3 conv -> 27 ch (18 offsets + 9 mask logits) + deformable 3x3
 //   convGRU.py:20-94, GN.py:4-9
+// and the ResNet family (resnet() below, msra_resnet.py):
+//   msra_resnet.py:116-124, 235-252  stem (7x7/2 conv, BN, ReLU, 3x3/2 max-pool), pre_* stems :126-147, layer1..4
+//   msra_resnet.py:35-105, 178-193   BasicBlock / Bottleneck, downsample; resnet_spec :300-304
+//   msra_resnet.py:150-154, 208-233  deconv_layers: 3 x (ConvTranspose2d 4x4/2/1, BN, ReLU)
+//   msra_resnet.py:157-174, 256-257  heads (3x3 -> ReLU -> 1x1)
 #include <stdlib.h>
 #include <string.h>
 
@@ -42,12 +47,13 @@ struct Act {
   int buf = -1;    // >= 0: the arena allocation it is a view of (cp_plan::bufs)
 };
 
-enum OpType { OP_IGEMM, OP_MAXPOOL, OP_UPADD, OP_GN_RELU, OP_GRU };
+enum OpType { OP_IGEMM, OP_MAXPOOL, OP_UPADD, OP_GN_RELU, OP_GRU, OP_MAXPOOL3 };
 
 struct Op {
   OpType type = OP_IGEMM;
   std::string name;
-  // igemm
+  // igemm (IGEMM_DECONV: kh = kw = 4, stride 2, pad 1 as the layer is declared; igemm_params maps it to its phases)
+  // and OP_MAXPOOL3 (src[0], out, optional res)
   Act src[4];
   int nsrc = 0;
   int mode = IGEMM_NHWC_VEC;
@@ -78,7 +84,7 @@ struct Op {
   bool first_step = false;
 };
 
-enum PackType { PACK_CONV, PACK_BIAS, PACK_UP, PACK_VEC };
+enum PackType { PACK_CONV, PACK_BIAS, PACK_UP, PACK_VEC, PACK_DECONV };
 
 struct PackJob {
   PackType type;
@@ -269,6 +275,80 @@ struct Builder {
     return op.out;
   }
 
+  // MaxPool2d(3, 2, 1) [+ residual] (msra_resnet.py:120, 242-247)
+  Act maxpool3(const Act& x, const Act* res, const std::string& name) {
+    Op op;
+    op.type = OP_MAXPOOL3;
+    op.src[0] = x;
+    if (res) {
+      op.has_res = true;
+      op.res = *res;
+    }
+    op.out = new_act(x.C, x.H / 2, x.W / 2);
+    op.name = name;
+    P->ops.push_back(op);
+    return op.out;
+  }
+
+  // ConvTranspose2d(Cin, Cout, 4, stride 2, pad 1, bias=False) + folded BN + ReLU (msra_resnet.py:219-230)
+  Act deconv_bn(const Act& x, const std::string& wkey, const std::string& bn, int Cout) {
+    Op op;
+    op.type = OP_IGEMM;
+    op.nsrc = 1;
+    op.src[0] = x;
+    op.mode = IGEMM_DECONV;
+    op.kh = op.kw = 4;
+    op.stride = 2;
+    op.pad = 1;
+    op.Cin = x.C;
+    op.Cout = Cout;
+    op.CoutPad = round_up(Cout, 64);
+    op.Kpad = 4 * x.C;
+    op.relu = true;
+    op.out = new_act(Cout, 2 * x.H, 2 * x.W);
+    op.w_ld = op.CoutPad;
+    op.w_off = walloc((size_t)4 * op.Kpad * op.CoutPad);
+    op.b_off = walloc(op.CoutPad);
+    PackJob jb;
+    jb.type = PACK_BIAS;
+    jb.bn = bn;
+    jb.Cout = Cout;
+    jb.CoutPad = op.CoutPad;
+    jb.dst = op.b_off;
+    jb.scale = walloc(op.CoutPad);
+    P->jobs.push_back(jb);
+    PackJob jw;
+    jw.type = PACK_DECONV;
+    jw.key = wkey;
+    jw.Cout = Cout;
+    jw.Cin = x.C;
+    jw.CoutPad = op.CoutPad;
+    jw.Kpad = op.Kpad;
+    jw.dst = op.w_off;
+    jw.scale = jb.scale;
+    jw.use_scale = true;
+    P->jobs.push_back(jw);
+    op.name = wkey.substr(0, wkey.rfind('.'));
+    P->ops.push_back(op);
+    return op.out;
+  }
+
+  // BasicBlock (msra_resnet.py:35-64) and Bottleneck (:67-105): out = relu(bn(conv) + residual), the stride on conv1 of
+  // a BasicBlock and on the 3x3 conv2 of a Bottleneck; `downsample` (1x1 at that stride + BN) when the shape changes
+  Act res_block(const Act& x, const std::string& p, int planes, int stride, bool bottleneck) {
+    const int Cout = bottleneck ? 4 * planes : planes;
+    Act residual = x;
+    if (stride != 1 || x.C != Cout)
+      residual = conv_bn(x, p + ".downsample.0", p + ".downsample.1", Cout, 1, stride, 0, false);
+    if (!bottleneck) {
+      Act y = conv_bn(x, p + ".conv1", p + ".bn1", planes, 3, stride, 1, true);
+      return conv_bn(y, p + ".conv2", p + ".bn2", planes, 3, 1, 1, true, &residual, false);
+    }
+    Act y = conv_bn(x, p + ".conv1", p + ".bn1", planes, 1, 1, 0, true);
+    y = conv_bn(y, p + ".conv2", p + ".bn2", planes, 3, stride, 1, true);
+    return conv_bn(y, p + ".conv3", p + ".bn3", Cout, 1, 1, 0, true, &residual, false);
+  }
+
   Act basic_block(const Act& x, const std::string& p, int Cout, int stride, const Act& residual) {
     Act y = conv_bn(x, p + ".conv1", p + ".bn1", Cout, 3, stride, 1, true);
     return conv_bn(y, p + ".conv2", p + ".bn2", Cout, 3, 1, 1, true, &residual, false);
@@ -378,6 +458,35 @@ struct Builder {
   }
 };
 
+bool is_res_arch(int arch) { return arch >= CP_ARCH_RES_18 && arch <= CP_ARCH_RES_152; }
+
+// PoseResNet up to the heads (msra_resnet.py:235-254): stem, layer1..4 (resnet_spec :300-304), deconv_layers.
+template <class Ext>
+Act resnet(Builder& b, const cp_config& c, Ext ext) {
+  static const int kBlocks[5][4] = {{2, 2, 2, 2}, {3, 4, 6, 3}, {3, 4, 6, 3}, {3, 4, 23, 3}, {3, 8, 36, 3}};
+  const int d = c.arch - CP_ARCH_RES_18;
+  const bool bottleneck = c.arch >= CP_ARCH_RES_50;
+  Act x = b.conv(std::vector<Act>{ext(0, 3)}, "conv1.weight", "", "bn1", 64, 7, 2, 3, true);
+  x = b.maxpool3(x, nullptr, "maxpool");
+  if (c.tracking) {      // x = x + pre_img_layer(pre_img) + pre_hm_layer(pre_hm) + pre_hm_hp_layer(pre_hm_hp), in this order
+    const char* keys[3] = {"pre_img_layer", "pre_hm_layer", "pre_hm_hp_layer"};
+    const int cin[3] = {3, 1, 8};
+    for (int e = 0; e < 3; ++e) {
+      const std::string k = keys[e];
+      Act t = b.conv(std::vector<Act>{ext(e + 1, cin[e])}, k + ".0.weight", "", k + ".1", 64, 7, 2, 3, true);
+      x = b.maxpool3(t, &x, k + ".3");
+    }
+  }
+  for (int l = 0; l < 4; ++l)
+    for (int j = 0; j < kBlocks[d][l]; ++j)
+      x = b.res_block(x, "layer" + std::to_string(l + 1) + "." + std::to_string(j), 64 << l, (l > 0 && j == 0) ? 2 : 1,
+                      bottleneck);
+  for (int i = 0; i < 3; ++i)
+    x = b.deconv_bn(x, "deconv_layers." + std::to_string(3 * i) + ".weight", "deconv_layers." + std::to_string(3 * i + 1),
+                    256);
+  return x;
+}
+
 int build_graph(cp_plan* P) {
   const cp_config& c = P->cfg;
   Builder b;
@@ -397,55 +506,61 @@ int build_graph(cp_plan* P) {
     a.W = W;
     return a;
   };
-  // ---- DLA-34 base (pose_dla_dcn.py:310-322)
-  Act x = b.conv({ext(0, 3)}, "base.base_layer.0.weight", "", "base.base_layer.1", 16, 7, 1, 3, true);
-  if (c.tracking) {
-    x = b.conv({ext(1, 3)}, "base.pre_img_layer.0.weight", "", "base.pre_img_layer.1", 16, 7, 1, 3, true, &x, true);
-    x = b.conv({ext(2, 1)}, "base.pre_hm_layer.0.weight", "", "base.pre_hm_layer.1", 16, 7, 1, 3, true, &x, true);
-    x = b.conv({ext(3, 8)}, "base.pre_hm_hp_layer.0.weight", "", "base.pre_hm_hp_layer.1", 16, 7, 1, 3, true, &x,
-               true);
-  }
-  std::vector<Act> lv(6);
-  lv[0] = b.conv_bn(x, "base.level0.0", "base.level0.1", 16, 3, 1, 1, true);
-  lv[1] = b.conv_bn(lv[0], "base.level1.0", "base.level1.1", 32, 3, 2, 1, true);
-  lv[2] = b.tree1(lv[1], "base.level2", 32, 64, 2, false, {});
-  lv[3] = b.tree2(lv[2], "base.level3", 64, 128, 2);
-  lv[4] = b.tree2(lv[3], "base.level4", 128, 256, 2);
-  lv[5] = b.tree1(lv[4], "base.level5", 256, 512, 2, true, {});
-
-  // ---- DLAUp (pose_dla_dcn.py:420-443), first_level = 2
-  const int first = 2;
-  std::vector<int> channels = {64, 128, 256, 512};
-  std::vector<int> in_channels = channels;
-  std::vector<int> scales = {1, 2, 4, 8};
-  struct Ida {
-    int o;
-    std::vector<int> up_f;
-  };
-  std::vector<Ida> idas;
-  const int nch = (int)channels.size();
-  for (int i = 0; i < nch - 1; ++i) {
-    int j = nch - i - 2;
-    Ida d;
-    d.o = channels[j];
-    for (int t = j; t < nch; ++t) d.up_f.push_back(scales[t] / scales[j]);
-    idas.push_back(d);
-    for (int t = j + 1; t < nch; ++t) {
-      scales[t] = scales[j];
-      in_channels[t] = channels[j];
+  Act F;      // the stride-4 feature the heads read
+  if (is_res_arch(c.arch)) {
+    F = resnet(b, c, ext);
+  } else {
+    // ---- DLA-34 base (pose_dla_dcn.py:310-322)
+    Act x = b.conv({ext(0, 3)}, "base.base_layer.0.weight", "", "base.base_layer.1", 16, 7, 1, 3, true);
+    if (c.tracking) {
+      x = b.conv({ext(1, 3)}, "base.pre_img_layer.0.weight", "", "base.pre_img_layer.1", 16, 7, 1, 3, true, &x, true);
+      x = b.conv({ext(2, 1)}, "base.pre_hm_layer.0.weight", "", "base.pre_hm_layer.1", 16, 7, 1, 3, true, &x, true);
+      x = b.conv({ext(3, 8)}, "base.pre_hm_hp_layer.0.weight", "", "base.pre_hm_hp_layer.1", 16, 7, 1, 3, true, &x,
+                 true);
     }
+    std::vector<Act> lv(6);
+    lv[0] = b.conv_bn(x, "base.level0.0", "base.level0.1", 16, 3, 1, 1, true);
+    lv[1] = b.conv_bn(lv[0], "base.level1.0", "base.level1.1", 32, 3, 2, 1, true);
+    lv[2] = b.tree1(lv[1], "base.level2", 32, 64, 2, false, {});
+    lv[3] = b.tree2(lv[2], "base.level3", 64, 128, 2);
+    lv[4] = b.tree2(lv[3], "base.level4", 128, 256, 2);
+    lv[5] = b.tree1(lv[4], "base.level5", 256, 512, 2, true, {});
+
+    // ---- DLAUp (pose_dla_dcn.py:420-443), first_level = 2
+    const int first = 2;
+    std::vector<int> channels = {64, 128, 256, 512};
+    std::vector<int> in_channels = channels;
+    std::vector<int> scales = {1, 2, 4, 8};
+    struct Ida {
+      int o;
+      std::vector<int> up_f;
+    };
+    std::vector<Ida> idas;
+    const int nch = (int)channels.size();
+    for (int i = 0; i < nch - 1; ++i) {
+      int j = nch - i - 2;
+      Ida d;
+      d.o = channels[j];
+      for (int t = j; t < nch; ++t) d.up_f.push_back(scales[t] / scales[j]);
+      idas.push_back(d);
+      for (int t = j + 1; t < nch; ++t) {
+        scales[t] = scales[j];
+        in_channels[t] = channels[j];
+      }
+    }
+    std::vector<Act> layers = lv;
+    std::vector<Act> out = {layers.back()};
+    for (int i = 0; i < (int)layers.size() - first - 1; ++i) {
+      b.ida_up(layers, "dla_up.ida_" + std::to_string(i), (int)layers.size() - i - 2, (int)layers.size(), idas[i].o,
+               idas[i].up_f);
+      out.insert(out.begin(), layers.back());
+    }
+    // ---- ida_up over out[0:3] (pose_dla_dcn.py:487-488, 533-536), last_level = 5
+    std::vector<Act> y(out.begin(), out.begin() + 3);
+    b.ida_up(y, "ida_up", 0, 3, 64, {1, 2, 4});
+    F = y.back();
+
   }
-  std::vector<Act> layers = lv;
-  std::vector<Act> out = {layers.back()};
-  for (int i = 0; i < (int)layers.size() - first - 1; ++i) {
-    b.ida_up(layers, "dla_up.ida_" + std::to_string(i), (int)layers.size() - i - 2, (int)layers.size(), idas[i].o,
-             idas[i].up_f);
-    out.insert(out.begin(), layers.back());
-  }
-  // ---- ida_up over out[0:3] (pose_dla_dcn.py:487-488, 533-536), last_level = 5
-  std::vector<Act> y(out.begin(), out.begin() + 3);
-  b.ida_up(y, "ida_up", 0, 3, 64, {1, 2, 4});
-  Act F = y.back();
 
   // ---- optional convGRU (convGRU.py:72-94): the three input convs see the same x at every step -> hoisted
   std::vector<Act> feat_for_head(c.num_heads, F);
@@ -598,6 +713,13 @@ void igemm_params(const cp_plan* P, const Op& op, int batch, const float* const 
   p.pad = op.pad;
   p.Hout = (p.Hin + 2 * op.pad - op.kh) / op.stride + 1;
   p.Wout = (p.Win + 2 * op.pad - op.kw) / op.stride + 1;
+  if (op.mode == IGEMM_DECONV) {      // the 4x4/2/1 transposed conv as four 2x2-tap phase GEMMs (common.cuh)
+    p.kh = p.kw = 2;
+    p.stride = 1;
+    p.pad = 0;
+    p.Hout = 2 * p.Hin;
+    p.Wout = 2 * p.Win;
+  }
   p.Cout = op.Cout;
   p.CoutPad = op.CoutPad;
   p.Kpad = op.Kpad;
@@ -702,6 +824,11 @@ void layout_arena(cp_plan* P) {
         touch(op.src[0], i);
         touch(op.out, i);
         break;
+      case OP_MAXPOOL3:
+        touch(op.src[0], i);
+        if (op.has_res) touch(op.res, i);
+        touch(op.out, i);
+        break;
       case OP_UPADD:
         touch(op.src[0], i);
         if (op.has_skip) touch(op.skip, i);
@@ -803,8 +930,10 @@ int cp_plan_create_ex(const cp_config* cfg, int32_t num_models, uint32_t flags, 
 // Everything about a plan that needs no device: the checked config, the schedule, the kernel of every op, the weight
 // and tile sizes and the arena layout.
 static int plan_layout(cp_plan* P, const cp_config* cfg, int32_t num_models, uint32_t flags) {
-  if (cfg->arch != CP_ARCH_DLA34 && cfg->arch != CP_ARCH_DLAV1_34)
+  if (cfg->arch != CP_ARCH_DLA34 && cfg->arch != CP_ARCH_DLAV1_34 && !is_res_arch(cfg->arch))
     return fail(CP_ERR_INVALID, "cp_plan_create: unknown arch");
+  if (is_res_arch(cfg->arch) && cfg->tracking_task_gru)
+    return fail(CP_ERR_INVALID, "cp_plan_create: tracking_task_gru needs the dlav1 convGRU; ResNets have none");
   if (!known_precision(cfg->precision))
     return fail(CP_ERR_INVALID, "cp_plan_create: unknown precision");
   if (cfg->height % 32 || cfg->width % 32 || cfg->height <= 0 || cfg->width <= 0)
@@ -975,6 +1104,12 @@ int cp_plan_load_weights_model(cp_plan* P, int32_t model, const char* const* nam
         if ((rc = launch_pack_up_weight(w, wts + j.dst, j.Cout, j.kh, s))) return rc;
         break;
       }
+      case PACK_DECONV: {
+        const float* w = nullptr;
+        if ((rc = get(j.key, (int64_t)j.Cin * j.Cout * 16, &w))) return rc;
+        if ((rc = launch_pack_deconv_weight(w, wts + j.scale, wts + j.dst, j.Cin, j.Cout, j.CoutPad, j.Kpad, s))) return rc;
+        break;
+      }
       case PACK_VEC: {
         const float* w = nullptr;
         if ((rc = get(j.key, j.Cout, &w))) return rc;
@@ -1048,6 +1183,12 @@ static int run_op(cp_plan* P, size_t idx, int batch, const float* const ext[4], 
                                 op.src[0].C, s)))
         return rc;
       break;
+    case OP_MAXPOOL3:
+      li.family = CP_FAM_MAXPOOL;
+      if ((rc = launch_maxpool3s2(P->act + op.src[0].off, op.has_res ? P->act + op.res.off : nullptr, P->act + op.out.off,
+                                  images, op.src[0].H, op.src[0].W, op.src[0].C, s)))
+        return rc;
+      break;
     case OP_UPADD:
       li.family = CP_FAM_UPADD;
       if ((rc = launch_upsample_add(P->act + op.src[0].off, P->wts + op.upw_off,
@@ -1102,6 +1243,12 @@ static int run_forward(cp_plan* P, int batch, const float* const ext[4], float* 
   return CP_OK;
 }
 
+// cp_op_stat.kind / cp_op_desc.kind: op type * 10 + igemm mode; the 3x3/2 max-pool is 11 (10 is the 2x2 DLA pool)
+static int op_kind(const Op& op) {
+  if (op.type == OP_MAXPOOL3) return 11;
+  return (int)op.type * 10 + (op.type == OP_IGEMM ? op.mode : 0);
+}
+
 // Algorithmic work of one op at batch `batch` (2*MAC; fp32 bytes of the tensors it must touch once).
 static void op_work(const Op& op, int batch, double* flops, double* bytes) {
   *flops = 0;
@@ -1113,6 +1260,10 @@ static void op_work(const Op& op, int batch, double* flops, double* bytes) {
       int Ho = (Hin + 2 * op.pad - op.kh) / op.stride + 1, Wo = (Win + 2 * op.pad - op.kw) / op.stride + 1;
       double M = B * Ho * Wo;
       *flops = 2.0 * M * op.kh * op.kw * op.Cin * op.Cout;
+      if (op.mode == IGEMM_DECONV) {      // 16 taps per input pixel: 4 per output pixel
+        M = B * op.out.H * op.out.W;
+        *flops = 2.0 * M * 4 * op.Cin * op.Cout;
+      }
       *bytes = 4.0 * (B * Hin * Win * op.Cin + (double)op.kh * op.kw * op.Cin * op.Cout + (op.fuse_heads ? 0.0 : M * op.Cout) +
                       (op.has_res ? M * op.Cout : 0.0) + (op.mode == IGEMM_DCN ? M * 27 : 0.0));
       if (op.fused_away) {      // accounted to the parent below
@@ -1123,6 +1274,9 @@ static void op_work(const Op& op, int batch, double* flops, double* bytes) {
     }
     case OP_MAXPOOL:
       *bytes = 4.0 * B * op.src[0].H * op.src[0].W * op.src[0].C * 1.25;
+      break;
+    case OP_MAXPOOL3:
+      *bytes = 4.0 * B * op.src[0].H * op.src[0].W * op.src[0].C * (op.has_res ? 1.5 : 1.25);
       break;
     case OP_UPADD: {
       double o = B * op.out.H * op.out.W * op.out.C;
@@ -1167,7 +1321,7 @@ int cp_plan_profile(cp_plan* P, int32_t batch, const float* images, const float*
       cp_op_stat& st = stats[n];
       memset(&st, 0, sizeof(st));
       snprintf(st.name, sizeof(st.name), "%s", op.name.c_str());
-      st.kind = (int)op.type * 10 + (op.type == OP_IGEMM ? op.mode : 0);
+      st.kind = op_kind(op);
       cudaEventElapsedTime(&st.ms, ctx.ev[i], ctx.ev[i + 1]);
       op_work(op, batch * P->models, &st.flops, &st.bytes);
     }
@@ -1202,7 +1356,7 @@ int cp_plan_op_desc_model(const cp_plan* P, int32_t model, int32_t i, cp_op_desc
   };
   memset(d, 0, sizeof(*d));
   snprintf(d->name, sizeof(d->name), "%s", op.name.c_str());
-  d->kind = (int)op.type * 10 + (op.type == OP_IGEMM ? op.mode : 0);
+  d->kind = op_kind(op);
   d->nsrc = op.nsrc;
   for (int k = 0; k < 4; ++k) act_desc(op.src[k], &d->src[k]);
   if (op.type != OP_IGEMM) act_desc(op.src[0], &d->src[0]);
@@ -1236,6 +1390,7 @@ int cp_plan_op_desc_model(const cp_plan* P, int32_t model, int32_t i, cp_op_desc
       break;
     }
     case OP_MAXPOOL: d->family = CP_FAM_MAXPOOL; break;
+    case OP_MAXPOOL3: d->family = CP_FAM_MAXPOOL; break;
     case OP_UPADD:
       d->family = CP_FAM_UPADD;
       d->up_w = wts + op.upw_off;

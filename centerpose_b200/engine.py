@@ -133,11 +133,16 @@ def _device_view(ptr, n, device):
         return torch.as_tensor(_CudaArray(ptr, n), device=device)
 
 
+ARCHS = {"dla_34": _lib.CP_ARCH_DLA34, "dlav1_34": _lib.CP_ARCH_DLAV1_34, "res_18": _lib.CP_ARCH_RES_18,
+         "res_34": _lib.CP_ARCH_RES_34, "res_50": _lib.CP_ARCH_RES_50, "res_101": _lib.CP_ARCH_RES_101,
+         "res_152": _lib.CP_ARCH_RES_152}      # cp_arch
+
+
 def _config(arch, heads, head_conv, max_batch, height, width, device_index=0, tracking=False, tracking_task_gru=False,
             precision="fp32"):
     """(cp_config, the encoded head names it points to: keep them alive while the config is used)."""
     cfg = _lib.CpConfig()
-    cfg.arch = {"dla_34": _lib.CP_ARCH_DLA34, "dlav1_34": _lib.CP_ARCH_DLAV1_34}[arch]
+    cfg.arch = ARCHS[arch]
     cfg.tracking = int(tracking)
     cfg.tracking_task_gru = int(tracking_task_gru)
     cfg.max_batch, cfg.height, cfg.width = int(max_batch), int(height), int(width)

@@ -3,10 +3,11 @@ network -- the drop-in for /root/reference/src/lib/models/model.py:26-105.
 
 `create_model(arch, heads, head_conv, opt)` returns an `nn.Module` whose
 `state_dict()` has exactly the reference's keys and shapes (SURVEY.md
-Appendix A: 416 / 439 / 450 keys for dla_34 / dlav1_34 / dla_34-tracking), so
-reference checkpoints load unchanged, and whose
+Appendix A: 416 / 439 / 450 keys for dla_34 / dlav1_34 / dla_34-tracking; the
+ResNets res_18 .. res_152 of msra_resnet.py likewise), so reference checkpoints
+load unchanged, and whose
 `forward(x, pre_img=None, pre_hm=None, pre_hm_hp=None) -> [ {head: logits} ]`
-(pose_dla_dcn.py:523-570) runs the hand-written sm_90a plan in
+(pose_dla_dcn.py:523-570, msra_resnet.py:235-258) runs the hand-written sm_90a plan in
 libcenterpose_b200.so.  The sub-modules below only HOLD parameters under the
 reference's names; no PyTorch operator ever runs on the hot path and there is
 no CPU fallback -- calling forward without CUDA raises.
@@ -116,7 +117,60 @@ def _flag(opt, name):
     return bool(getattr(opt, name, False)) if opt is not None else False
 
 
-class DLASegB200(nn.Module):
+class _NativeNet(nn.Module):
+    """What every network of this package shares: the parameters are held under the reference's names, and forward
+    runs the native plan of `_arch()` (include/centerpose_b200.h cp_arch) for the input's shape."""
+
+    # ------------------------------------------------------------------ native plan management
+    def _signature(self):
+        sig = []
+        for t in list(self.parameters()) + list(self.buffers()):
+            sig.append((t.data_ptr(), t._version))
+        return hash(tuple(sig))
+
+    def engine(self, batch, height, width, device=None):
+        """The native engine for this input shape (created on first use).  Its activation arena is packed by liveness
+        (Engine reuse_activations): the results are the same bits as a full arena's in a fraction of the memory."""
+        from .engine import Engine
+        device = device if device is not None else next(self.parameters()).device
+        if device.type != "cuda":
+            raise RuntimeError("centerpose_b200: the network only runs on CUDA (sm_90a); "
+                               "there is no CPU fallback -- move the model with .to('cuda')")
+        key = (height, width, device.index if device.index is not None else torch.cuda.current_device(), self.precision)
+        eng = self._engines.get(key)
+        if eng is None or eng.max_batch < batch:
+            if eng is not None:
+                eng.close()
+            eng = Engine(self._arch(), self.heads, self.head_conv, max(batch, 1), height, width, key[2],
+                         tracking=self.tracking_inputs, tracking_task_gru=self.use_convGRU and self.tracking_task,
+                         precision=self.precision, reuse_activations=True)
+            eng.weights_sig = None
+            self._engines[key] = eng
+        sig = self._signature()
+        if eng.weights_sig != sig:
+            eng.load_state_dict(self.state_dict())
+            eng.weights_sig = sig
+        return eng
+
+    def forward(self, x, pre_img=None, pre_hm=None, pre_hm_hp=None):
+        if x.dim() != 4 or x.shape[1] != 3:
+            raise ValueError("expected NCHW input with 3 channels")
+        if not x.is_cuda:
+            raise RuntimeError("centerpose_b200: forward needs a CUDA tensor (no CPU fallback)")
+        B, _, H, W = x.shape
+        eng = self.engine(B, H, W, x.device)
+        with torch.no_grad():
+            out = eng.forward(x, pre_img, pre_hm, pre_hm_hp)
+        return [out]
+
+    def _apply(self, fn, *a, **k):
+        r = super()._apply(fn, *a, **k)
+        for e in self._engines.values():
+            e.weights_sig = None
+        return r
+
+
+class DLASegB200(_NativeNet):
     """H100-native DLASeg (pose_dla_dcn.py:457-570).
 
     `precision` selects the kernels of the plan (include/centerpose_b200.h cp_precision): "tf32x3" (default: wgmma
@@ -185,56 +239,8 @@ class DLASegB200(nn.Module):
         self._engines = {}
         self._weights_sig = None
 
-    # ------------------------------------------------------------------ native plan management
-    def _signature(self):
-        sig = []
-        for t in list(self.parameters()) + list(self.buffers()):
-            sig.append((t.data_ptr(), t._version))
-        return hash(tuple(sig))
-
-    def engine(self, batch, height, width, device=None):
-        """The native engine for this input shape (created on first use).  Its activation arena is packed by liveness
-        (Engine reuse_activations): the results are the same bits as a full arena's in a fraction of the memory."""
-        from .engine import Engine
-        device = device if device is not None else next(self.parameters()).device
-        if device.type != "cuda":
-            raise RuntimeError("centerpose_b200: the network only runs on CUDA (sm_90a); "
-                               "there is no CPU fallback -- move the model with .to('cuda')")
-        key = (height, width, device.index if device.index is not None else torch.cuda.current_device(), self.precision)
-        eng = self._engines.get(key)
-        if eng is None or eng.max_batch < batch:
-            if eng is not None:
-                eng.close()
-            eng = Engine(self._arch(), self.heads, self.head_conv, max(batch, 1), height, width, key[2],
-                         tracking=self.tracking_inputs, tracking_task_gru=self.use_convGRU and self.tracking_task,
-                         precision=self.precision, reuse_activations=True)
-            eng.weights_sig = None
-            self._engines[key] = eng
-        sig = self._signature()
-        if eng.weights_sig != sig:
-            eng.load_state_dict(self.state_dict())
-            eng.weights_sig = sig
-        return eng
-
     def _arch(self):
         return "dlav1_34" if self.use_convGRU else "dla_34"
-
-    def forward(self, x, pre_img=None, pre_hm=None, pre_hm_hp=None):
-        if x.dim() != 4 or x.shape[1] != 3:
-            raise ValueError("expected NCHW input with 3 channels")
-        if not x.is_cuda:
-            raise RuntimeError("centerpose_b200: forward needs a CUDA tensor (no CPU fallback)")
-        B, _, H, W = x.shape
-        eng = self.engine(B, H, W, x.device)
-        with torch.no_grad():
-            out = eng.forward(x, pre_img, pre_hm, pre_hm_hp)
-        return [out]
-
-    def _apply(self, fn, *a, **k):
-        r = super()._apply(fn, *a, **k)
-        for e in self._engines.values():
-            e.weights_sig = None
-        return r
 
 
 def get_pose_net(num_layers, heads, head_conv=256, down_ratio=4, opt=None):
@@ -251,7 +257,102 @@ def get_dla_dcn_convGRU(num_layers, heads, head_conv=256, down_ratio=4, opt=None
     return DLASegB200(heads, head_conv, use_convGRU=True, opt=opt)
 
 
-_model_factory = {"dla": get_pose_net, "dlav1": get_dla_dcn_convGRU}
+# resnet_spec (msra_resnet.py:300-304): (bottleneck, blocks of layer1..4)
+_RESNET_SPEC = {18: (False, [2, 2, 2, 2]), 34: (False, [3, 4, 6, 3]), 50: (True, [3, 4, 6, 3]),
+                101: (True, [3, 4, 23, 3]), 152: (True, [3, 8, 36, 3])}
+
+
+def _res_block(cin, planes, stride, bottleneck):
+    """BasicBlock (msra_resnet.py:35-64) / Bottleneck (:67-105) parameters, with `downsample` (:180-185)."""
+    m = _Holder()
+    cout = planes * (4 if bottleneck else 1)
+    if bottleneck:
+        m.conv1, m.bn1 = _conv(cin, planes, 1), nn.BatchNorm2d(planes)
+        m.conv2, m.bn2 = nn.Conv2d(planes, planes, 3, stride, 1, bias=False), nn.BatchNorm2d(planes)
+        m.conv3, m.bn3 = _conv(planes, cout, 1), nn.BatchNorm2d(cout)
+    else:
+        m.conv1, m.bn1 = nn.Conv2d(cin, planes, 3, stride, 1, bias=False), nn.BatchNorm2d(planes)
+        m.conv2, m.bn2 = _conv(planes, planes, 3), nn.BatchNorm2d(planes)
+    if stride != 1 or cin != cout:
+        m.downsample = nn.Sequential(nn.Conv2d(cin, cout, 1, stride, bias=False), nn.BatchNorm2d(cout))
+    return m
+
+
+def _res_stem(cin):
+    return nn.Sequential(nn.Conv2d(cin, 64, 7, 2, 3, bias=False), nn.BatchNorm2d(64), nn.ReLU(inplace=True),
+                         nn.MaxPool2d(3, 2, 1))
+
+
+class PoseResNetB200(_NativeNet):
+    """H100-native PoseResNet (msra_resnet.py:108-258) of depth 18, 34, 50, 101 or 152: the 7x7/2 stem and 3x3/2
+    max-pool, layer1..4, three 4x4/2 transposed convs to 256 channels and the heads (3x3 -> ReLU -> 1x1; the reference's
+    default head_conv for a ResNet is 64, opts.py:344-345).  The tracking stems pre_img / pre_hm / pre_hm_hp (:126-147)
+    come with opt.tracking_task as for DLA.  There is no ImageNet download (init_weights, :260-297): the weights come
+    from a checkpoint.  `precision` as for DLASegB200."""
+
+    def __init__(self, num_layers, heads, head_conv=64, opt=None, precision="tf32x3"):
+        super().__init__()
+        if num_layers not in _RESNET_SPEC:
+            raise ValueError("centerpose_b200 implements res_18, res_34, res_50, res_101 and res_152 (resnet_spec, "
+                             "msra_resnet.py:300-304); got depth %r" % (num_layers,))
+        if head_conv <= 0:
+            raise ValueError("head_conv must be > 0: the bare 1x1 heads of msra_resnet.py:166-173 are not implemented "
+                             "(the reference's ResNet default is 64, opts.py:344-345)")
+        self.opt = opt
+        self.num_layers = num_layers
+        self.heads = dict(heads)
+        self.head_conv = head_conv
+        self.use_convGRU = False
+        self.tracking_inputs = _flag(opt, "pre_img") or _flag(opt, "pre_hm") or _flag(opt, "pre_hm_hp")
+        if self.tracking_inputs and not (_flag(opt, "pre_img") and _flag(opt, "pre_hm") and _flag(opt, "pre_hm_hp")):
+            raise ValueError("centerpose_b200 supports the tracking stems only as the full "
+                             "pre_img + pre_hm + pre_hm_hp set (demo.py:117-123)")
+        self.tracking_task = _flag(opt, "tracking_task")
+        self.precision = precision
+
+        bottleneck, blocks = _RESNET_SPEC[num_layers]
+        self.conv1 = nn.Conv2d(3, 64, 7, 2, 3, bias=False)
+        self.bn1 = nn.BatchNorm2d(64)
+        cin = 64
+        for i, n in enumerate(blocks):
+            planes = 64 << i
+            layer = nn.Sequential()
+            for j in range(n):
+                layer.add_module(str(j), _res_block(cin, planes, 2 if (i > 0 and j == 0) else 1, bottleneck))
+                cin = planes * (4 if bottleneck else 1)
+            setattr(self, "layer%d" % (i + 1), layer)
+        if self.tracking_inputs:
+            self.pre_img_layer = _res_stem(3)
+            self.pre_hm_layer = _res_stem(1)
+            self.pre_hm_hp_layer = _res_stem(8)
+        deconv = []
+        for _ in range(3):
+            deconv += [nn.ConvTranspose2d(cin, 256, 4, stride=2, padding=1, output_padding=0, bias=False),
+                       nn.BatchNorm2d(256), nn.ReLU(inplace=True)]
+            cin = 256
+        self.deconv_layers = nn.Sequential(*deconv)
+        for head in sorted(self.heads):       # registration order of msra_resnet.py:157-174 (the state_dict order)
+            fc = nn.Sequential(nn.Conv2d(256, head_conv, 3, padding=1, bias=True), nn.ReLU(inplace=True),
+                               nn.Conv2d(head_conv, self.heads[head], 1, bias=True))
+            with torch.no_grad():
+                fc[0].bias.zero_()
+                fc[2].bias.fill_(-2.19 if "hm" in head else 0.0)
+            setattr(self, head, fc)
+        self._engines = {}
+        self._weights_sig = None
+
+    def _arch(self):
+        return "res_%d" % self.num_layers
+
+
+def get_pose_resnet(num_layers, heads, head_conv=64, down_ratio=4, opt=None):
+    """'res' factory (msra_resnet.py:307-312)."""
+    if down_ratio != 4:
+        raise ValueError("centerpose_b200 implements the ResNets at down_ratio 4")
+    return PoseResNetB200(num_layers, heads, head_conv, opt=opt)
+
+
+_model_factory = {"dla": get_pose_net, "dlav1": get_dla_dcn_convGRU, "res": get_pose_resnet}
 
 
 def create_model(arch, heads, head_conv, opt=None):
@@ -259,7 +360,7 @@ def create_model(arch, heads, head_conv, opt=None):
     num_layers = int(arch[arch.find("_") + 1:]) if "_" in arch else 0
     name = arch[:arch.find("_")] if "_" in arch else arch
     if name not in _model_factory:
-        raise KeyError("centerpose_b200 implements the 'dla' and 'dlav1' backbones; got '%s'" % arch)
+        raise KeyError("centerpose_b200 implements the 'dla', 'dlav1' and 'res' backbones; got '%s'" % arch)
     return _model_factory[name](num_layers=num_layers, heads=heads, head_conv=head_conv, opt=opt)
 
 

@@ -15,7 +15,7 @@ def default_opt(arch="dla_34", tracking_task=False, rep_mode=1, c="chair", gpus=
     o.task = "object_pose"                 # opts.py:19
     o.dataset = "objectron"
     o.arch = arch                          # opts.py:77
-    o.head_conv = 256                      # opts.py:344-345 ('dla' in arch)
+    o.head_conv = 256 if "dla" in arch else 64      # opts.py:344-345
     o.down_ratio = 4                       # opts.py:85
     o.K = K                                # opts.py:120
     o.rep_mode = rep_mode                  # opts.py:211-220

@@ -61,7 +61,18 @@ enum cp_status {
 /* ---- architecture / precision -------------------------------------------- */
 enum cp_arch {
   CP_ARCH_DLA34 = 0,        /* 'dla_34'   : DLA-34 + DCNv2            (model.py:19) */
-  CP_ARCH_DLAV1_34 = 1      /* 'dlav1_34' : + convGRU + GroupNorm heads (model.py:20) */
+  CP_ARCH_DLAV1_34 = 1,     /* 'dlav1_34' : + convGRU + GroupNorm heads (model.py:20) */
+  /* 'res_N' (model.py:17, networks/msra_resnet.py; opts.py:77-79 lists res_101 as tested): 7x7/2 stem + 3x3/2 max-pool
+   * (:116-120), layer1..4 of BasicBlocks (18, 34) or Bottlenecks (50, 101, 152) per resnet_spec (:300-304), three
+   * ConvTranspose2d 4x4/2/1 + BN + ReLU to 256 channels (:208-233), heads 3x3 -> ReLU -> 1x1 (:157-174).  Tracking
+   * configs add the pre_img / pre_hm / pre_hm_hp stems, each summed after its own max-pool (:126-147, 242-247).
+   * tracking_task_gru is CP_ERR_INVALID (no convGRU); head_conv as for DLA (the reference's default for res is 64,
+   * opts.py:344-345). */
+  CP_ARCH_RES_18 = 2,
+  CP_ARCH_RES_34 = 3,
+  CP_ARCH_RES_50 = 4,
+  CP_ARCH_RES_101 = 5,
+  CP_ARCH_RES_152 = 6
 };
 
 enum cp_precision {
@@ -186,7 +197,8 @@ int cp_forward(cp_plan* plan, int32_t batch, const float* images, const float* p
  * schedule; the call synchronises on the last event.  `flops` / `bytes` are the ALGORITHMIC
  * work of the op (2*MAC; fp32 tensors touched once), used for the roofline in bench.py.
  * kind = op_type*10 + igemm_mode  (0: NCHW stem conv, 1: NHWC conv, 2: deformable conv,
- * 10: max-pool, 20: up-sample+add, 30: GroupNorm+ReLU, 40: GRU gate). */
+ * 3: dense ConvTranspose2d 4x4 stride 2 pad 1 (ResNet up-sampling), 10: 2x2 max-pool, 11: 3x3 stride-2 pad-1
+ * max-pool [+ residual] (ResNet stems), 20: up-sample+add, 30: GroupNorm+ReLU, 40: GRU gate). */
 typedef struct cp_op_stat {
   char name[96];
   int32_t kind;
@@ -230,7 +242,10 @@ typedef struct cp_op_desc {
   cp_act_desc out;          /* output (GroupNorm: the channel slice it normalises in place)                         */
   int32_t out_head;         /* >= 0: the conv writes head out_head as NCHW instead of `out`                        */
   int32_t kh, stride, pad, Cin, Cout, CoutPad, Kpad;
-  const float* w;           /* device fp32 [Kpad][w_ld], row k = (ky*kh + kx)*Cin + ci, BN folded               */
+  const float* w;           /* device fp32 [Kpad][w_ld], row k = (ky*kh + kx)*Cin + ci, BN folded.  kind 3: four phase
+                             * blocks [4][Kpad][w_ld], Kpad = 4 Cin; phase py*2+px, row (2a+b)*Cin + ci holds
+                             * weight[ci][co][ky][kx] with ky = 1+2a (py 0) or 2a (py 1) and kx likewise; it feeds output
+                             * (2y+py, 2x+px) from input (y+dy, x+dx), dy = -a (py 0) or 1-a (py 1)                   */
   int32_t w_ld;
   const float* bias;        /* device fp32 [Cout]                                                                  */
   int32_t relu, has_res, res_after_relu;   /* out = relu(acc + bias [+ res]) or relu(acc + bias) + res           */
