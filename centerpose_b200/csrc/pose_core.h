@@ -741,9 +741,10 @@ CP_HD bool pnp_gate_invisible(const double* kpspnp, int visible_thresh) {
 CP_HDN void pnp_finish(const double* V, const double* R, const double* t, double cost, int n, const double* Kc,
                        double width, double height, int visible_thresh, int opencv_return, PnPOut* o) {
   const double fx = Kc[0], fy = Kc[4], cx = Kc[2], cy = Kc[5];
+  // a NaN or +-inf pose is a solver failure (pnp_ref.solve_pnp: np.isfinite); `fabs(x) <= DBL_MAX` is false for both
   bool finite = (cost == cost) && fabs(cost) < 1e300;
-  for (int i = 0; i < 9; ++i) finite = finite && (R[i] == R[i]);
-  for (int i = 0; i < 3; ++i) finite = finite && (t[i] == t[i]);
+  for (int i = 0; i < 9; ++i) finite = finite && (fabs(R[i]) <= 1.7976931348623157e308);
+  for (int i = 0; i < 3; ++i) finite = finite && (fabs(t[i]) <= 1.7976931348623157e308);
   if (!finite) {
     o->status = 5;
     return;

@@ -313,6 +313,11 @@ def solve_pnp(points2d, vertices, Kc, opencv_return=False):
         return out          # cuboid_pnp_solver.py:157-160
     o2 = np.array(o2)
     o3 = np.array(o3)
+    if not (np.isfinite(o2).all() and np.isfinite(o3).all()):
+        # a NaN / inf point or cuboid vertex (scale[1] = 0, denormal or inf, an overflowing width): cv2 asserts on
+        # such input, the device solvers end in SOLVER_FAIL -- the rule of DESIGN.md section 5
+        out["status"] = ST_SOLVER_FAIL
+        return out
     if len(o2) < 6:         # :162-163 SOLVEPNP_EPNP
         sol = epnp(o3, o2, np.asarray(Kc, np.float64))
         if sol is None:

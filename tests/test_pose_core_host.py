@@ -78,6 +78,28 @@ def test_pnp_failure_paths(pose_host):
     assert st3 == 2
 
 
+def test_nonfinite_input_is_solver_failure(pose_host):
+    """A NaN / inf image point or cuboid vertex (scale[1] = 0, denormal or inf; a width that overflows fp32) is
+    SOLVER_FAIL in pose_core.h and in the oracle -- on the DLT + LM path (8 points) and on the EPnP path (5 points)."""
+    cam = synth.default_camera(512, 512)
+    V = pnp_ref.cuboid_vertices(np.ones(3, np.float32))
+    uv = pnp_ref.project(V, synth._rand_rot(np.random.default_rng(5)), np.array([0.1, -0.2, 4.0]), cam)
+    cases = [(uv, s) for s in ((1, 0, 1), (1, 1e-40, 1), (1, np.inf, 1), (3e38, 1e-3, 1), (1, -0.0, 1))]
+    for bad in (np.inf, np.nan):
+        p = uv.copy()
+        p[2, 1] = bad
+        cases.append((p, (1, 1, 1)))
+    for pts, sc in cases:
+        for keep in (8, 5):
+            p = pts.copy()
+            p[keep:] = -10000.0
+            scale = np.array(sc, np.float32)
+            st, npt, out = _solve(pose_host, p, scale, cam, 512, 512, 6, 0)
+            assert (st, npt) == (pnp_ref.ST_SOLVER_FAIL, keep), (sc, keep, st)
+            with np.errstate(all="ignore"):
+                assert pnp_ref.pnp_shell({"obj_scale": scale, "kps": p.reshape(-1)}, p, cam, 512, 512)[0] == st
+
+
 def _epnp_case(rng, n, noise):
     import cv2
     K = np.array([[663.0, 0, 300.3], [0, 663.0, 395.0], [0, 0, 1.0]])
