@@ -12,7 +12,7 @@ no PyTorch or CPU fallback.
 """
 from .model import create_model, load_model, save_model, DLASegB200, PoseResNetB200          # noqa: F401
 from .detector import MultiCategoryDetector, MultiCategoryTracker, ObjectPoseDetector, detector_factory  # noqa: F401
-from .engine import Engine, InferGraph, decode_pnp, decode_params, make_meta, dcn_v2_forward, dcn_v2_backward, preprocess, preprocess_ragged, conv2d_nhwc  # noqa: F401
+from .engine import Engine, InferGraph, decode_pnp, decode_params, make_meta, dcn_v2_forward, dcn_v2_backward, preprocess, preprocess_ragged, preprocess_yuv420, conv2d_nhwc  # noqa: F401
 from .opts import default_opt                                                # noqa: F401
 from .tracker import Tracker, track_to_dict, tracks_to_results               # noqa: F401
 from .pipeline import BatchPipeline, TrackPipeline                           # noqa: F401

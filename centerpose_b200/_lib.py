@@ -57,8 +57,12 @@ EXPORTS = [
     "cp_preprocess_ragged", "cp_tracker_step_ex", "cp_tracker_render_ex2", "cp_tracker_seed_ex",
     "cp_plan_create_multi", "cp_plan_load_weights_model", "cp_plan_num_models", "cp_plan_op_desc_model", "cp_infer_multi",
     "cp_plan_create_multi_track", "cp_infer_multi_track", "cp_tracker_create_multi",
-    "cp_plan_create_ex", "cp_plan_memory", "cp_plan_allocations",
+    "cp_plan_create_ex", "cp_plan_memory", "cp_plan_allocations", "cp_preprocess_yuv420",
 ]
+
+# cp_pixel_format; "bgr" is the interleaved uint8 [H,W,3] input of every other pre-process entry point
+CP_PIX_NV12, CP_PIX_I420 = 0, 1
+PIXEL_FORMATS = ("bgr", "nv12", "i420")
 
 # cp_plan_create_ex / cp_plan_memory flags
 CP_PLAN_REUSE_ACTIVATIONS = 1
@@ -196,6 +200,9 @@ def load():
     L.cp_preprocess_affine.argtypes = [vp, vp, i32, i32, i32, i32, i32, ctypes.POINTER(ctypes.c_double),
                                        ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_float), vp]
     L.cp_preprocess_ragged.argtypes = [vp, i64, ctypes.POINTER(i64), ctypes.POINTER(i32), vp, i32, i32, i32,
+                                       ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_float),
+                                       ctypes.POINTER(ctypes.c_float), vp]
+    L.cp_preprocess_yuv420.argtypes = [vp, i64, ctypes.POINTER(i64), ctypes.POINTER(i32), i32, vp, i32, i32, i32,
                                        ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_float),
                                        ctypes.POINTER(ctypes.c_float), vp]
     L.cp_tracker_create.argtypes = [ctypes.POINTER(CpTrackerConfig), ctypes.POINTER(vp)]

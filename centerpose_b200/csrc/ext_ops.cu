@@ -4,7 +4,8 @@
 //                        (reference: DCNv2/src/cuda/dcn_v2_cuda.cu:42-172).
 //   cp_preprocess     -- batched uint8 HWC frames -> normalised fp32 NCHW network input
 //                        (reference: detectors/base_detector.py:91-148, fix_res branch); cp_preprocess_ragged does
-//                        the same for frames of different sizes in one launch.
+//                        the same for frames of different sizes in one launch, and cp_preprocess_yuv420 for NV12 / I420
+//                        frames (the colour conversion of cv2.cvtColor fused into the warp's tap fetch).
 #include <vector>
 
 #include "common.cuh"
@@ -26,9 +27,13 @@ struct WarpM {
   double m[6];
 };
 
-// one output pixel (x, y) of frame `img` [sh, sw, 3] under the inverted matrix W, all three channels
-__device__ __forceinline__ void warp_pixel(const uint8_t* __restrict__ img, float* __restrict__ out, size_t plane, int sh,
-                                           int sw, int x, int y, const WarpM& W, const float* mean, const float* stdv) {
+// one output pixel (x, y) of a [sh, sw] frame under the inverted matrix W, all three channels.  The source pixels come
+// from `px`: px.taps(iy, ix, in-frame flags) sees the 2 x 2 taps (iy, ix) .. (iy + 1, ix + 1) once, then px(k, yy, xx, c)
+// is channel c (B, G, R) of in-frame tap k = 2 (yy - iy) + (xx - ix) as an integer 0..255.  Taps outside the frame are
+// the border value 0 and are never fetched.
+template <class Fetch>
+__device__ __forceinline__ void warp_walk(Fetch px, float* __restrict__ out, size_t plane, int sh, int sw, int x,
+                                          int y, const WarpM& W, const float* mean, const float* stdv) {
   // unfused double arithmetic (the host code OpenCV runs here has no FMA contraction)
   const int X0 = __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(W.m[1], (double)y), W.m[2]), 1024.0)) + 16;
   const int Y0 = __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(W.m[4], (double)y), W.m[5]), 1024.0)) + 16;
@@ -43,15 +48,16 @@ __device__ __forceinline__ void warp_pixel(const uint8_t* __restrict__ img, floa
   const int w00 = (32 - fy) * (32 - fx) * 32, w01 = (32 - fy) * fx * 32, w10 = fy * (32 - fx) * 32, w11 = fy * fx * 32;
   const bool y0 = iy >= 0 && iy < sh, y1 = iy + 1 >= 0 && iy + 1 < sh;
   const bool x0 = ix >= 0 && ix < sw, x1 = ix + 1 >= 0 && ix + 1 < sw;
+  px.taps(iy, ix, y0 && x0, y0 && x1, y1 && x0, y1 && x1);
   for (int c = 0; c < 3; ++c) {
     int v00 = 0, v01 = 0, v10 = 0, v11 = 0;
     if (y0) {
-      if (x0) v00 = img[((size_t)iy * sw + ix) * 3 + c];
-      if (x1) v01 = img[((size_t)iy * sw + ix + 1) * 3 + c];
+      if (x0) v00 = px(0, iy, ix, c);
+      if (x1) v01 = px(1, iy, ix + 1, c);
     }
     if (y1) {
-      if (x0) v10 = img[((size_t)(iy + 1) * sw + ix) * 3 + c];
-      if (x1) v11 = img[((size_t)(iy + 1) * sw + ix + 1) * 3 + c];
+      if (x0) v10 = px(2, iy + 1, ix, c);
+      if (x1) v11 = px(3, iy + 1, ix + 1, c);
     }
     int u8 = (v00 * w00 + v01 * w01 + v10 * w10 + v11 * w11 + (1 << 14)) >> 15;
     u8 = max(0, min(255, u8));
@@ -59,6 +65,64 @@ __device__ __forceinline__ void warp_pixel(const uint8_t* __restrict__ img, floa
     out[c * plane] = (float)r;
   }
 }
+
+// interleaved 8-bit BGR [sh, sw, 3]: every channel is read where it is used
+struct BgrFetch {
+  const uint8_t* __restrict__ img;
+  int sw;
+  __device__ __forceinline__ void taps(int, int, bool, bool, bool, bool) {}
+  __device__ __forceinline__ int operator()(int, int yy, int xx, int c) const {
+    return img[((size_t)yy * sw + xx) * 3 + c];
+  }
+};
+
+__device__ __forceinline__ void warp_pixel(const uint8_t* __restrict__ img, float* __restrict__ out, size_t plane, int sh,
+                                           int sw, int x, int y, const WarpM& W, const float* mean, const float* stdv) {
+  warp_walk(BgrFetch{img, sw}, out, plane, sh, sw, x, y, W, mean, stdv);
+}
+
+// YUV 4:2:0 [3 sh / 2, sw] (sh, sw even) converted per tap to the BGR that cv2.cvtColor(COLOR_YUV2BGR_NV12 / _I420)
+// gives, restated bit for bit (OpenCV color_yuv.simd.hpp, yuv42x_to_rgb8 for 8-bit: BT.601 limited range in 20-bit
+// fixed point, no chroma interpolation; tests/yuv_ref.py yuv420_to_bgr, pinned against cv2 on every (Y, U, V)):
+//   y = max(Y - 16, 0) * 1220542 + 2^19, u = U - 128, v = V - 128
+//   B = sat((y + 2116026 u) >> 20), G = sat((y - 852492 v - 409993 u) >> 20), R = sat((y + 1673527 v) >> 20)
+// The Y plane [sh, sw] comes first; then NV12: U, V interleaved, row yy / 2, bytes (xx & ~1) and (xx | 1); I420: the U
+// plane [sh/2, sw/2], then the V plane [sh/2, sw/2].  Only in-frame taps are converted: warpAffine's border 0 is BGR 0.
+template <int kFormat>
+struct Yuv420Fetch {
+  const uint8_t* __restrict__ img;
+  int sh, sw;
+  int yv[4], u[4], v[4];      // per tap: max(Y - 16, 0) * 1220542 + 2^19, U - 128, V - 128
+  // every in-frame tap is read and converted once, before the first channel is written
+  __device__ __forceinline__ void taps(int iy, int ix, bool in00, bool in01, bool in10, bool in11) {
+    const bool in[4] = {in00, in01, in10, in11};
+    const uint8_t* __restrict__ chroma = img + (size_t)sh * sw;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      yv[k] = u[k] = v[k] = 0;
+      if (!in[k]) continue;
+      const int yy = iy + (k >> 1), xx = ix + (k & 1);
+      int U, V;
+      if (kFormat == CP_PIX_NV12) {
+        const size_t o = (size_t)(yy >> 1) * sw + (xx & ~1);
+        U = chroma[o];
+        V = chroma[o + 1];
+      } else {
+        const size_t o = (size_t)(yy >> 1) * (sw >> 1) + (xx >> 1);
+        U = chroma[o];
+        V = chroma[(size_t)(sh >> 1) * (sw >> 1) + o];
+      }
+      yv[k] = max((int)img[(size_t)yy * sw + xx] - 16, 0) * 1220542 + (1 << 19);
+      u[k] = U - 128;
+      v[k] = V - 128;
+    }
+  }
+  __device__ __forceinline__ int operator()(int k, int, int, int c) const {
+    const int t = c == 0 ? yv[k] + 2116026 * u[k]
+                         : (c == 1 ? yv[k] - 852492 * v[k] - 409993 * u[k] : yv[k] + 1673527 * v[k]);
+    return max(0, min(255, t >> 20));
+  }
+};
 
 __global__ void preprocess_kernel(const uint8_t* __restrict__ frames, float* __restrict__ out, int B, int sh,
                                   int sw, int dh, int dw, const WarpM W, float m0, float m1, float m2, float s0, float s1,
@@ -97,6 +161,25 @@ __global__ void preprocess_ragged_kernel(const uint8_t* __restrict__ frames, con
     const RaggedFrame f = fr[n];
     warp_pixel(frames + f.offset, out + (((size_t)n * 3) * dh + y) * dw + x, (size_t)dh * dw, f.sh, f.sw, x, y, f.W, mean,
                stdv);
+  }
+}
+
+// the ragged launch on YUV 4:2:0 frames (kFormat: cp_pixel_format): the same walk with the tap fetch converting to BGR
+template <int kFormat>
+__global__ void preprocess_yuv420_kernel(const uint8_t* __restrict__ frames, const RaggedFrame* __restrict__ fr,
+                                         float* __restrict__ out, int B, int dh, int dw, float m0, float m1, float m2,
+                                         float s0, float s1, float s2) {
+  size_t total = (size_t)B * dh * dw;
+  const float mean[3] = {m0, m1, m2};
+  const float stdv[3] = {s0, s1, s2};
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int x = (int)(i % dw);
+    const size_t t = i / dw;
+    const int y = (int)(t % dh);
+    const int n = (int)(t / dh);
+    const RaggedFrame f = fr[n];
+    warp_walk(Yuv420Fetch<kFormat>{frames + f.offset, f.sh, f.sw}, out + (((size_t)n * 3) * dh + y) * dw + x,
+              (size_t)dh * dw, f.sh, f.sw, x, y, f.W, mean, stdv);
   }
 }
 
@@ -142,6 +225,59 @@ int preprocess_blocks(size_t total) {
   int blocks = (int)((total + 255) / 256);
   if (blocks > 132 * 16) blocks = 132 * 16;
   return blocks;
+}
+
+// The per-frame parameters of a ragged batch, checked against the packed buffer before any work is enqueued.  `yuv`:
+// the frames are YUV 4:2:0 (even sizes, h * w * 3 / 2 bytes each), else BGR (h * w * 3 bytes).
+int ragged_frames(const char* who, int64_t frames_bytes, const int64_t* offsets, const int32_t* src_hw, int B, int dst_h,
+                  int dst_w, const double* trans_input, bool yuv, std::vector<RaggedFrame>& fr) {
+  const std::string w0 = who;
+  fr.resize(B);
+  for (int b = 0; b < B; ++b) {
+    const int h = src_hw[2 * b], w = src_hw[2 * b + 1];
+    if (h <= 0 || w <= 0 || (yuv && (h % 2 || w % 2)))
+      return fail(CP_ERR_INVALID, w0 + ": frame " + std::to_string(b) + " has size " + std::to_string(h) + " x " +
+                                      std::to_string(w) + (yuv ? " (YUV 4:2:0 needs even sizes)" : ""));
+    const int64_t bytes = yuv ? (int64_t)h * w * 3 / 2 : (int64_t)h * w * 3;
+    if (offsets[b] < 0 || offsets[b] > frames_bytes || bytes > frames_bytes - offsets[b])
+      return fail(CP_ERR_INVALID, w0 + ": frame " + std::to_string(b) + " (" + std::to_string(h) + " x " +
+                                      std::to_string(w) + " at byte " + std::to_string(offsets[b]) +
+                                      ") lies outside the " + std::to_string(frames_bytes) + "-byte buffer");
+    double T[6];
+    if (trans_input) {
+      for (int i = 0; i < 6; ++i) T[i] = trans_input[6 * b + i];
+    } else {
+      fix_res_affine(h, w, dst_h, dst_w, T);
+    }
+    fr[b].W = invert_affine(T);
+    fr[b].offset = offsets[b];
+    fr[b].sh = h;
+    fr[b].sw = w;
+  }
+  return CP_OK;
+}
+
+// uploads the per-frame parameters (stream-ordered) and enqueues launch(device parameters)
+template <class Launch>
+int launch_ragged(const char* who, const char* kernel, const std::vector<RaggedFrame>& fr, cudaStream_t s,
+                  Launch launch) {
+  const int B = (int)fr.size();
+  RaggedFrame* dfr = nullptr;
+  CP_CUDA_CHECK(cudaMallocAsync(&dfr, sizeof(RaggedFrame) * B, s));
+  int rc = CP_OK;
+  // a pageable source: the bytes are staged before cudaMemcpyAsync returns, so `fr` may go out of scope
+  if (cudaMemcpyAsync(dfr, fr.data(), sizeof(RaggedFrame) * B, cudaMemcpyHostToDevice, s) != cudaSuccess) {
+    rc = fail(CP_ERR_CUDA, std::string(who) + ": parameter upload");
+  } else {
+    launch(dfr);
+    const cudaError_t e = cudaGetLastError();
+    if (e != cudaSuccess)
+      rc = fail(CP_ERR_CUDA, std::string(kernel) + ": " + cudaGetErrorString(e));
+    else
+      ++g_launch_counter;
+  }
+  cudaFreeAsync(dfr, s);
+  return rc;
 }
 
 }  // namespace
@@ -312,45 +448,36 @@ int cp_preprocess_ragged(const uint8_t* frames, int64_t frames_bytes, const int6
                          const float mean[3], const float stdv[3], void* stream_) {
   if (!frames || !offsets || !src_hw || !out || !mean || !stdv) return fail(CP_ERR_INVALID, "cp_preprocess_ragged: null argument");
   if (B <= 0 || dst_h <= 0 || dst_w <= 0 || frames_bytes <= 0) return fail(CP_ERR_INVALID, "cp_preprocess_ragged: bad shape");
-  std::vector<RaggedFrame> fr(B);
-  for (int b = 0; b < B; ++b) {
-    const int h = src_hw[2 * b], w = src_hw[2 * b + 1];
-    if (h <= 0 || w <= 0)
-      return fail(CP_ERR_INVALID, "cp_preprocess_ragged: frame " + std::to_string(b) + " has size " + std::to_string(h) +
-                                      " x " + std::to_string(w));
-    if (offsets[b] < 0 || offsets[b] > frames_bytes || (int64_t)h * w * 3 > frames_bytes - offsets[b])
-      return fail(CP_ERR_INVALID, "cp_preprocess_ragged: frame " + std::to_string(b) + " (" + std::to_string(h) + " x " +
-                                      std::to_string(w) + " at byte " + std::to_string(offsets[b]) +
-                                      ") lies outside the " + std::to_string(frames_bytes) + "-byte buffer");
-    double T[6];
-    if (trans_input) {
-      for (int i = 0; i < 6; ++i) T[i] = trans_input[6 * b + i];
-    } else {
-      fix_res_affine(h, w, dst_h, dst_w, T);
-    }
-    fr[b].W = invert_affine(T);
-    fr[b].offset = offsets[b];
-    fr[b].sh = h;
-    fr[b].sw = w;
-  }
+  std::vector<RaggedFrame> fr;
+  int rc = ragged_frames("cp_preprocess_ragged", frames_bytes, offsets, src_hw, B, dst_h, dst_w, trans_input, false, fr);
+  if (rc) return rc;
   cudaStream_t s = (cudaStream_t)stream_;
-  RaggedFrame* dfr = nullptr;
-  CP_CUDA_CHECK(cudaMallocAsync(&dfr, sizeof(RaggedFrame) * B, s));
-  int rc = CP_OK;
-  // a pageable source: the bytes are staged before cudaMemcpyAsync returns, so `fr` may go out of scope
-  if (cudaMemcpyAsync(dfr, fr.data(), sizeof(RaggedFrame) * B, cudaMemcpyHostToDevice, s) != cudaSuccess) {
-    rc = fail(CP_ERR_CUDA, "cp_preprocess_ragged: parameter upload");
-  } else {
+  return launch_ragged("cp_preprocess_ragged", "preprocess_ragged_kernel", fr, s, [&](const RaggedFrame* dfr) {
     preprocess_ragged_kernel<<<preprocess_blocks((size_t)B * dst_h * dst_w), 256, 0, s>>>(
         frames, dfr, out, B, dst_h, dst_w, mean[0], mean[1], mean[2], stdv[0], stdv[1], stdv[2]);
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess)
-      rc = fail(CP_ERR_CUDA, std::string("preprocess_ragged_kernel: ") + cudaGetErrorString(e));
+  });
+}
+
+int cp_preprocess_yuv420(const uint8_t* frames, int64_t frames_bytes, const int64_t* offsets, const int32_t* src_hw,
+                         int32_t format, float* out, int32_t B, int32_t dst_h, int32_t dst_w, const double* trans_input,
+                         const float mean[3], const float stdv[3], void* stream_) {
+  if (!frames || !offsets || !src_hw || !out || !mean || !stdv) return fail(CP_ERR_INVALID, "cp_preprocess_yuv420: null argument");
+  if (B <= 0 || dst_h <= 0 || dst_w <= 0 || frames_bytes <= 0) return fail(CP_ERR_INVALID, "cp_preprocess_yuv420: bad shape");
+  if (format != CP_PIX_NV12 && format != CP_PIX_I420)
+    return fail(CP_ERR_INVALID, "cp_preprocess_yuv420: unknown pixel format " + std::to_string(format));
+  std::vector<RaggedFrame> fr;
+  int rc = ragged_frames("cp_preprocess_yuv420", frames_bytes, offsets, src_hw, B, dst_h, dst_w, trans_input, true, fr);
+  if (rc) return rc;
+  cudaStream_t s = (cudaStream_t)stream_;
+  return launch_ragged("cp_preprocess_yuv420", "preprocess_yuv420_kernel", fr, s, [&](const RaggedFrame* dfr) {
+    const int blocks = preprocess_blocks((size_t)B * dst_h * dst_w);
+    if (format == CP_PIX_NV12)
+      preprocess_yuv420_kernel<CP_PIX_NV12><<<blocks, 256, 0, s>>>(frames, dfr, out, B, dst_h, dst_w, mean[0], mean[1],
+                                                                    mean[2], stdv[0], stdv[1], stdv[2]);
     else
-      ++g_launch_counter;
-  }
-  cudaFreeAsync(dfr, s);
-  return rc;
+      preprocess_yuv420_kernel<CP_PIX_I420><<<blocks, 256, 0, s>>>(frames, dfr, out, B, dst_h, dst_w, mean[0], mean[1],
+                                                                    mean[2], stdv[0], stdv[1], stdv[2]);
+  });
 }
 
 }  // extern "C"

@@ -18,7 +18,8 @@ import numpy as np
 import torch
 
 from . import _lib
-from .engine import Engine, decode_params, decode_pnp, make_meta, preprocess, preprocess_ragged
+from .engine import (Engine, check_pixel_format, decode_params, decode_pnp, image_size, make_meta, preprocess,
+                     preprocess_ragged, preprocess_yuv420)
 from .model import _load_checkpoint, create_model, load_model
 from .tracker import Tracker, tracks_to_results
 
@@ -122,8 +123,10 @@ def camera_per_frame(camera_matrix, B):
     return list(cam)
 
 
-def check_frames(frames, allow_idle):
-    """The frames of a ragged batch: uint8 [H,W,3] numpy arrays or tensors (None = an idle slot when allowed)."""
+def check_frames(frames, allow_idle, pixel_format="bgr"):
+    """The frames of a ragged batch: uint8 [H,W,3] numpy arrays or tensors, or uint8 [3H/2,W] with an "nv12" / "i420"
+    pixel_format (None = an idle slot when allowed)."""
+    check_pixel_format(pixel_format)
     if len(frames) == 0:
         raise ValueError("run_batch: an empty list of frames")
     for b, f in enumerate(frames):
@@ -135,9 +138,9 @@ def check_frames(frames, allow_idle):
             raise TypeError("run_batch: frame %d is a %s, not a numpy array or tensor" % (b, type(f).__name__))
         dt = f.dtype
         if dt not in (np.uint8, torch.uint8):
-            raise TypeError("run_batch: frame %d is %s; the ragged path takes uint8 [H,W,3] frames" % (b, dt))
-        if f.ndim != 3 or f.shape[2] != 3 or f.shape[0] < 1 or f.shape[1] < 1:
-            raise ValueError("run_batch: frame %d has shape %s, expected [H,W,3]" % (b, tuple(f.shape)))
+            raise TypeError("run_batch: frame %d is %s; the ragged path takes uint8 %s frames"
+                            % (b, dt, "[H,W,3]" if pixel_format == "bgr" else "[3H/2,W]"))
+        image_size(f.shape, pixel_format, "run_batch: frame %d" % b)
 
 
 def check_slot_list(values, S, name, kind=None):
@@ -541,7 +544,7 @@ class ObjectPoseDetector(object):
 
     # ------------------------------------------------------------------ batched API (not in the reference)
     def run_batch(self, frames, camera_matrix, pre_images=None, pre_hms=None, pre_hm_hp=None, to_host=True, track=False,
-                  out=None, pre_dets=None, frame_ids=None, new_video=None):
+                  out=None, pre_dets=None, frame_ids=None, new_video=None, pixel_format="bgr"):
         """frames: uint8 [B,H,W,3] (numpy / pinned CPU tensor / CUDA tensor) or a
         pre-processed fp32 [B,3,h,w] CUDA tensor.  One native cp_infer call for the
         whole batch.  Returns (poses [B,K,192], n_valid [B]) -- on the host when
@@ -563,22 +566,27 @@ class ObjectPoseDetector(object):
         video starts on its first frame after the state is made (first call, a new number of slots, reset_tracking()).
         Both forms go through one tracking step (`_track_step`); the array form is the case where every slot steps.
         With a list, a None frame idles its slot this call, new_video[i] starts a new video in slot i, and `out` (see
-        `_run_slots`) is honoured; the array form ignores `out`."""
+        `_run_slots`) is honoured; the array form ignores `out`.
+
+        pixel_format="nv12" / "i420": the uint8 frames are YUV 4:2:0 as video decoders give them, uint8 [B,3H/2,W] (array
+        form) or a list of uint8 [3H_b/2,W_b] (H and W even), converted on the device inside the pre-process: every
+        result equals, bit for bit, that of the same call on cv2.cvtColor(frame, COLOR_YUV2BGR_NV12 / _I420).  c, s and
+        the meta rows come from the image size (H, W)."""
         if track and not getattr(self.opt, "tracking_task", False):
             raise ValueError("run_batch(track=True) needs a tracking model (opt.tracking_task)")
         if isinstance(frames, (list, tuple)):
             if pre_images is not None or pre_hms is not None or pre_hm_hp is not None:
                 raise ValueError("run_batch(list): the previous frames and heat maps are kept per slot (track=True)")
             if track:
-                return self._run_slots(frames, camera_matrix, to_host, out, pre_dets, frame_ids, new_video)
+                return self._run_slots(frames, camera_matrix, to_host, out, pre_dets, frame_ids, new_video, pixel_format)
             if new_video is not None or pre_dets is not None or frame_ids is not None:
                 raise ValueError("run_batch(list): new_video / pre_dets / frame_ids need track=True")
-            check_frames(frames, allow_idle=False)
-            x, meta, _ = self._ragged_input(frames, camera_matrix)
+            check_frames(frames, allow_idle=False, pixel_format=pixel_format)
+            x, meta, _ = self._ragged_input(frames, camera_matrix, pixel_format)
         else:
             if new_video is not None:
                 raise ValueError("run_batch: new_video needs a list of slot frames")
-            x, meta, c, s = self._array_input(frames, camera_matrix)
+            x, meta, c, s = self._array_input(frames, camera_matrix, pixel_format)
             B = x.shape[0]
             if track:
                 pre_dets = self._slot_pre_dets(pre_dets, B)
@@ -591,13 +599,26 @@ class ObjectPoseDetector(object):
                                       n_valid=out[1] if out is not None else None)
         return _returned((poses, n_valid), to_host)
 
-    def _array_input(self, frames, camera_matrix):
-        """run_batch's array form: uint8 [B,H,W,3] frames (or pre-processed fp32 [B,3,h,w]) -> (x [B,3,h,w] fp32 CUDA,
-        meta rows [B,16] float64 host, c, s) with the fix_res affine of the frame size."""
+    def _array_input(self, frames, camera_matrix, pixel_format="bgr"):
+        """run_batch's array form: uint8 [B,H,W,3] frames, uint8 [B,3H/2,W] YUV 4:2:0 frames of pixel_format (or
+        pre-processed fp32 [B,3,h,w]) -> (x [B,3,h,w] fp32 CUDA, meta rows [B,16] float64 host, c, s) with the fix_res
+        affine of the image size."""
         dev = self.opt.device
         if isinstance(frames, np.ndarray):
             frames = torch.from_numpy(frames)
-        if frames.dtype == torch.uint8:
+        if check_pixel_format(pixel_format) != "bgr":
+            if frames.dtype != torch.uint8 or frames.dim() != 3:
+                raise ValueError("run_batch: %s frames are uint8 [B,3H/2,W], got %s %s"
+                                 % (pixel_format, frames.dtype, tuple(frames.shape)))
+            B = frames.shape[0]
+            sh, sw = image_size(frames.shape[1:], pixel_format, "run_batch: each frame")
+            fr = frames.to(dev, non_blocking=True).contiguous().reshape(-1)
+            n = sh * sw * 3 // 2
+            x = preprocess_yuv420(fr, np.arange(B, dtype=np.int64) * n, [(sh, sw)] * B, pixel_format, self.opt.input_h,
+                                  self.opt.input_w, self.opt.mean, self.opt.std)
+            c, s = np.array([sw / 2., sh / 2.], np.float32), float(max(sh, sw))
+            iw, ih = sw, sh
+        elif frames.dtype == torch.uint8:
             B, sh, sw, _ = frames.shape
             fr = frames.to(dev, non_blocking=True)
             x = preprocess(fr, self.opt.input_h, self.opt.input_w, self.opt.mean, self.opt.std)
@@ -615,10 +636,11 @@ class ObjectPoseDetector(object):
         return x, meta, c, s
 
     # ------------------------------------------------------------------ ragged batches (lists of frames)
-    def _ragged_input(self, frames, camera_matrix):
-        """Validated list of uint8 HWC frames -> (x [B,3,h,w] fp32 CUDA, meta rows [B,16] float64 host, trans_input
-        [B,2,3] host).  The frames are copied into one device buffer and pre-processed by one cp_preprocess_ragged
-        launch with the same fix_res affine (c = frame centre, s = max side) and meta row that pre_process / run() use."""
+    def _ragged_input(self, frames, camera_matrix, pixel_format="bgr"):
+        """Validated list of uint8 HWC frames (or YUV 4:2:0 [3H/2,W] frames of pixel_format) -> (x [B,3,h,w] fp32 CUDA,
+        meta rows [B,16] float64 host, trans_input [B,2,3] host).  The frames are copied into one device buffer and
+        pre-processed by one cp_preprocess_ragged (cp_preprocess_yuv420) launch with the same fix_res affine (c = image
+        centre, s = max side) and meta row that pre_process / run() use."""
         if getattr(self.opt, "fix_short", 0) > 0 or not getattr(self.opt, "fix_res", True):
             raise NotImplementedError("run_batch(list) pre-processes in the fix_res mode only")
         if float(self.scales[0]) != 1.0:
@@ -631,7 +653,7 @@ class ObjectPoseDetector(object):
         for b, f in enumerate(frames):
             t = torch.from_numpy(f) if isinstance(f, np.ndarray) else f
             ts.append(t)
-            hw[b] = t.shape[:2]
+            hw[b] = image_size(t.shape, pixel_format)
             offs[b] = off
             off += t.numel()
         if self._packed is None or self._packed.numel() < off or self._packed.device != torch.device(dev):
@@ -647,7 +669,11 @@ class ObjectPoseDetector(object):
                 self._affines[(h, w)] = affine_from_center_scale(c, sc, iw, ih)
             trans[b] = self._affines[(h, w)]
             meta[b] = make_meta(1, c, sc, w, h, cams[b]).numpy()[0]
-        x = preprocess_ragged(self._packed, offs, hw, ih, iw, self.opt.mean, self.opt.std, trans_input=trans)
+        if pixel_format == "bgr":
+            x = preprocess_ragged(self._packed, offs, hw, ih, iw, self.opt.mean, self.opt.std, trans_input=trans)
+        else:
+            x = preprocess_yuv420(self._packed, offs, hw, pixel_format, ih, iw, self.opt.mean, self.opt.std,
+                                  trans_input=trans)
         return x, meta, trans
 
     def _meta_rows(self, meta):
@@ -659,7 +685,7 @@ class ObjectPoseDetector(object):
             self._meta_key = key
         return self._meta_dev
 
-    def _run_slots(self, frames, camera_matrix, to_host, out, pre_dets, frame_ids, new_video):
+    def _run_slots(self, frames, camera_matrix, to_host, out, pre_dets, frame_ids, new_video, pixel_format="bgr"):
         """run_batch(list, track=True): frames[i] is the next frame of the video in slot i, or None when slot i is idle
         this step (its tracker stream is not stepped and keeps its state).  new_video[i] marks the first frame of a
         video in slot i, which then behaves exactly like the first run() call of a fresh detector: the stream is reset,
@@ -669,7 +695,7 @@ class ObjectPoseDetector(object):
         Returns (tracks [S,T,320], n_tracks [S]) for the S slots, idle slots with n_tracks 0 and zero rows; out:
         optional (tracks, n_tracks) CUDA tensors of those shapes to write into."""
         S = len(frames)
-        check_frames(frames, allow_idle=True)
+        check_frames(frames, allow_idle=True, pixel_format=pixel_format)
         cams = camera_per_frame(camera_matrix, S)
         new_video = check_slot_list(new_video, S, "new_video", bool)
         pre_dets = self._slot_pre_dets(pre_dets, S)
@@ -680,7 +706,7 @@ class ObjectPoseDetector(object):
             out[0].zero_()
             out[1].zero_()
             return _returned(out, to_host)
-        x, meta, trans = self._ragged_input([frames[i] for i in live], np.stack([cams[i] for i in live]))
+        x, meta, trans = self._ragged_input([frames[i] for i in live], np.stack([cams[i] for i in live]), pixel_format)
         return self._track_step(S, live, x, self._meta_rows(meta), trans, new_video, pre_dets, frame_ids, to_host, out)
 
     # ---- what a tracking step does per category: one category here; MultiCategoryTracker runs several through the
@@ -835,16 +861,16 @@ class MultiCategoryDetector(ObjectPoseDetector):
             self._eng = eng
         return eng
 
-    def run_batch(self, frames, camera_matrix, to_host=True, out=None):
+    def run_batch(self, frames, camera_matrix, to_host=True, out=None, pixel_format="bgr"):
         """run_batch of ObjectPoseDetector (a uint8 [B,H,W,3] array, or a list of mixed-size frames with one camera or
-        one per frame) for every category: the frames are pre-processed once.  Returns (poses [M,B,K,192],
-        n_valid [M,B]) in `categories` order, also for M = 1; out: optional (poses, n_valid) CUDA tensors of those
-        shapes to write into."""
+        one per frame; YUV 4:2:0 frames with pixel_format "nv12" / "i420") for every category: the frames are
+        pre-processed once.  Returns (poses [M,B,K,192], n_valid [M,B]) in `categories` order, also for M = 1; out:
+        optional (poses, n_valid) CUDA tensors of those shapes to write into."""
         if isinstance(frames, (list, tuple)):
-            check_frames(frames, allow_idle=False)
-            x, meta, _ = self._ragged_input(frames, camera_matrix)
+            check_frames(frames, allow_idle=False, pixel_format=pixel_format)
+            x, meta, _ = self._ragged_input(frames, camera_matrix, pixel_format)
         else:
-            x, meta, _, _ = self._array_input(frames, camera_matrix)
+            x, meta, _, _ = self._array_input(frames, camera_matrix, pixel_format)
         eng = self.engine(x.shape[0], x.shape[2], x.shape[3])
         if len(self._prms) > 1:
             _, poses, n_valid = eng.infer(x, self._meta_rows(meta), self._prms,
@@ -884,18 +910,20 @@ class MultiCategoryTracker(MultiCategoryDetector):
             self.tracker.close()
             self.tracker = None
 
-    def run_batch(self, frames, camera_matrix, new_video=None, pre_dets=None, frame_ids=None, to_host=True, out=None):
+    def run_batch(self, frames, camera_matrix, new_video=None, pre_dets=None, frame_ids=None, to_host=True, out=None,
+                  pixel_format="bgr"):
         """The next frame of every slot, for every category.  frames: uint8 [S,H,W,3] (every slot steps), or a list of S
         uint8 [H_s,W_s,3] frames of mixed sizes where None idles a slot this step, with camera_matrix [3,3] or one per
         slot.  new_video[i]: slot i starts a new video (every category).  pre_dets: None, or a mapping category -> per
         slot list of meta['pre_dets'] lists (None = that slot is not seeded); frame_ids: per slot meta['id'].
         Returns (tracks [M,S,T,320], n_tracks [M,S]) in `categories` order (idle slots: n_tracks 0, zero rows), on the
-        host when `to_host`; out: optional (tracks, n_tracks) CUDA tensors of those shapes to write into."""
+        host when `to_host`; out: optional (tracks, n_tracks) CUDA tensors of those shapes to write into.
+        pixel_format "nv12" / "i420": YUV 4:2:0 frames, uint8 [S,3H/2,W] or [3H_s/2,W_s] (as ObjectPoseDetector.run_batch)."""
         if isinstance(frames, (list, tuple)):
-            return self._run_slots(frames, camera_matrix, to_host, out, pre_dets, frame_ids, new_video)
+            return self._run_slots(frames, camera_matrix, to_host, out, pre_dets, frame_ids, new_video, pixel_format)
         if new_video is not None:
             raise ValueError("run_batch: new_video needs a list of slot frames")
-        x, meta, c, s = self._array_input(frames, camera_matrix)
+        x, meta, c, s = self._array_input(frames, camera_matrix, pixel_format)
         S = x.shape[0]
         pre_dets = self._slot_pre_dets(pre_dets, S)
         frame_ids = check_slot_list(frame_ids, S, "frame_ids")

@@ -511,6 +511,74 @@ def preprocess_ragged(packed_u8, offsets, src_hw, dst_h, dst_w, mean, std, out=N
     return out
 
 
+_YUV420 = {"nv12": _lib.CP_PIX_NV12, "i420": _lib.CP_PIX_I420}
+
+
+def check_pixel_format(pixel_format):
+    """pixel_format: "bgr" (uint8 [H,W,3]), "nv12" or "i420" (uint8 [3H/2,W], cp_pixel_format)."""
+    if pixel_format not in _lib.PIXEL_FORMATS:
+        raise ValueError("pixel_format must be one of %s, got %r" % (", ".join(_lib.PIXEL_FORMATS), pixel_format))
+    return pixel_format
+
+
+def frame_shape(h, w, pixel_format):
+    """The buffer shape of one h x w image in pixel_format: [h,w,3] for "bgr", [3h/2,w] for "nv12" / "i420" (h and w
+    even, else ValueError)."""
+    if check_pixel_format(pixel_format) == "bgr":
+        return (int(h), int(w), 3)
+    if h % 2 or w % 2 or h < 2 or w < 2:
+        raise ValueError("%s frames need an even, positive image size; got %d x %d" % (pixel_format, h, w))
+    return (int(h) * 3 // 2, int(w))
+
+
+def image_size(shape, pixel_format, what="frame"):
+    """(H, W) of the image a buffer of `shape` holds in pixel_format; ValueError (naming the expected shape) when the
+    shape is not one of that format."""
+    shape = tuple(int(v) for v in shape)
+    if check_pixel_format(pixel_format) == "bgr":
+        if len(shape) != 3 or shape[2] != 3 or shape[0] < 1 or shape[1] < 1:
+            raise ValueError("%s has shape %s, expected [H,W,3]" % (what, shape))
+        return shape[0], shape[1]
+    if len(shape) == 2 and shape[0] % 3 == 0:
+        h, w = shape[0] * 2 // 3, shape[1]
+        if h >= 2 and w >= 2 and h % 2 == 0 and w % 2 == 0:
+            return h, w
+    raise ValueError("%s has shape %s, expected a %s frame [3H/2,W] with H and W even" % (what, shape, pixel_format))
+
+
+def preprocess_yuv420(packed_u8, offsets, src_hw, pixel_format, dst_h, dst_w, mean, std, out=None, trans_input=None):
+    """cp_preprocess_yuv420: preprocess_ragged for YUV 4:2:0 frames.  packed_u8: flat uint8 CUDA buffer holding frame b
+    (uint8 [3H/2,W] in pixel_format "nv12" or "i420", (H, W) = src_hw[b], both even) at byte offsets[b] -> fp32
+    [B,3,dst_h,dst_w] CUDA, frame b bit for bit what preprocess_ragged gives for cv2.cvtColor(frame, COLOR_YUV2BGR_*).
+    trans_input: optional [B,2,3] forward affines; default = each frame's fix_res affine (that of `preprocess`)."""
+    L = _lib.load()
+    if pixel_format not in _YUV420:
+        raise ValueError("preprocess_yuv420: pixel_format must be 'nv12' or 'i420', got %r" % (pixel_format,))
+    if not packed_u8.is_cuda or packed_u8.dtype != torch.uint8 or not packed_u8.is_contiguous():
+        raise RuntimeError("preprocess_yuv420 needs a contiguous uint8 CUDA buffer")
+    offs = np.ascontiguousarray(offsets, np.int64).reshape(-1)
+    hw = np.ascontiguousarray(src_hw, np.int32).reshape(-1, 2)
+    B = offs.shape[0]
+    if hw.shape[0] != B:
+        raise ValueError("preprocess_yuv420: %d offsets for %d frame sizes" % (B, hw.shape[0]))
+    if out is None:
+        out = torch.empty((B, 3, dst_h, dst_w), dtype=torch.float32, device=packed_u8.device)
+    tm = None
+    if trans_input is not None:
+        tr = np.ascontiguousarray(trans_input, np.float64).reshape(-1)
+        if tr.shape[0] != 6 * B:
+            raise ValueError("preprocess_yuv420: trans_input must hold %d 2x3 matrices" % B)
+        tm = tr.ctypes.data_as(ctypes.POINTER(ctypes.c_double))
+    m = (ctypes.c_float * 3)(*[float(v) for v in mean])
+    s = (ctypes.c_float * 3)(*[float(v) for v in std])
+    with torch.cuda.device(packed_u8.device):
+        rc = L.cp_preprocess_yuv420(_ptr(packed_u8), packed_u8.numel(), offs.ctypes.data_as(ctypes.POINTER(ctypes.c_int64)),
+                                    hw.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), _YUV420[pixel_format], _ptr(out), B,
+                                    dst_h, dst_w, tm, m, s, _stream())
+    _lib.check(rc, "cp_preprocess_yuv420")
+    return out
+
+
 def conv2d_nhwc(x, weight, bias=None, residual=None, stride=1, pad=0, relu=False, precision="fp32"):
     """cp_conv2d: x [B,H,W,Cin] NHWC fp32 CUDA, weight OIHW -> [B,Ho,Wo,Cout] NHWC."""
     L = _lib.load()

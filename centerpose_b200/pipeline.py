@@ -25,6 +25,10 @@ per-rank records are all-gathered (one NCCL call per batch, `dist.PoseBuffer`) b
         pipe.submit(frames, new_video=starts)
         if pipe.in_flight == pipe.depth:
             tracks, n_tracks = pipe.collect()   # [S,T,320], [S] of the OLDEST submitted frame
+
+Both take `pixel_format="nv12"` or `"i420"` for YUV 4:2:0 frames as video decoders give them (uint8 [3H/2,W] per
+frame, H and W even): they are uploaded as they are, half the bytes of BGR, and converted inside the pre-process
+kernel; the results equal those of the same frames converted by cv2.cvtColor and submitted as BGR.
 """
 import collections
 
@@ -33,12 +37,13 @@ import torch
 
 from . import _lib
 from .dist import PoseBuffer, shard_range, slot_layout
+from .engine import check_pixel_format, frame_shape
 
 
 class _Slot(object):
-    def __init__(self, batch, height, width, K, device, world):
-        self.u8 = torch.empty((batch, height, width, 3), dtype=torch.uint8, device=device)
-        self.staging = torch.empty((batch, height, width, 3), dtype=torch.uint8).pin_memory()
+    def __init__(self, batch, shape, K, device, world):
+        self.u8 = torch.empty((batch,) + shape, dtype=torch.uint8, device=device)
+        self.staging = torch.empty((batch,) + shape, dtype=torch.uint8).pin_memory()
         self.pbuf = PoseBuffer(batch, K, device, world=world)
         self.h2d_done = torch.cuda.Event()
         self.compute_done = torch.cuda.Event()           # the pre-process kernel has consumed `u8`
@@ -47,7 +52,13 @@ class _Slot(object):
 
 
 class BatchPipeline(object):
-    def __init__(self, det, batch, height, width, camera_matrix, world=1, depth=2, to_host=True, group=None):
+    """height, width: the image size of every frame; pixel_format "bgr" (frames uint8 [B,H,W,3]), "nv12" or "i420"
+    (uint8 [B,3H/2,W])."""
+
+    def __init__(self, det, batch, height, width, camera_matrix, world=1, depth=2, to_host=True, group=None,
+                 pixel_format="bgr"):
+        self.pixel_format = check_pixel_format(pixel_format)
+        shape = frame_shape(int(height), int(width), pixel_format)
         self.det, self.cam, self.depth, self.to_host, self.group = det, camera_matrix, int(depth), to_host, group
         self.device = torch.device(det.opt.device)
         if self.device.type != "cuda":
@@ -56,7 +67,7 @@ class BatchPipeline(object):
         with torch.cuda.device(self.device):
             self.copy_stream = torch.cuda.Stream()
             self.side_stream = torch.cuda.Stream()
-            self.slots = [_Slot(batch, height, width, det.opt.K, self.device, world) for _ in range(self.depth)]
+            self.slots = [_Slot(batch, shape, det.opt.K, self.device, world) for _ in range(self.depth)]
         self._queue = collections.deque()
         self._next = 0
 
@@ -65,7 +76,8 @@ class BatchPipeline(object):
         return len(self._queue)
 
     def submit(self, frames):
-        """frames: uint8 [B,H,W,3] numpy array or CPU tensor (pinned memory makes the upload asynchronous)."""
+        """frames: uint8 [B,H,W,3] (or [B,3H/2,W] in a YUV pixel_format) numpy array or CPU tensor (pinned memory makes
+        the upload asynchronous)."""
         if len(self._queue) >= self.depth:
             raise RuntimeError("BatchPipeline: collect() the oldest batch before submitting batch %d" % (self.depth + 1))
         if isinstance(frames, np.ndarray):
@@ -89,7 +101,8 @@ class BatchPipeline(object):
         compute.wait_event(slot.h2d_done)
         if slot.used:
             compute.wait_event(slot.side_done)           # the slot's previous gather / download have read its records
-        self.det.run_batch(slot.u8, self.cam, to_host=False, out=(slot.pbuf.poses, slot.pbuf.n_valid))
+        self.det.run_batch(slot.u8, self.cam, to_host=False, out=(slot.pbuf.poses, slot.pbuf.n_valid),
+                           pixel_format=self.pixel_format)
         slot.compute_done.record(compute)
         slot.used = True
         # the all-gather and the download run on a side stream: the next batch's kernels neither queue behind the copy nor
@@ -143,9 +156,11 @@ class TrackPipeline(object):
     """Double-buffered `run_batch(list, track=True)` over `slots` video slots: the frames of step i+1 are uploaded
     (through pinned staging) on a copy stream while step i computes, and the track records of step i are read back one
     submit later.  With world > 1 (under torchrun) rank `rank` runs the slots shard_range(slots, rank, world) and one
-    all-gather per step collects everyone's records (`dist.slot_layout`)."""
+    all-gather per step collects everyone's records (`dist.slot_layout`).  pixel_format "nv12" / "i420": every frame is
+    YUV 4:2:0, uint8 [3H/2,W]."""
 
-    def __init__(self, det, slots, camera_matrix, world=1, rank=0, depth=2, to_host=True, group=None):
+    def __init__(self, det, slots, camera_matrix, world=1, rank=0, depth=2, to_host=True, group=None, pixel_format="bgr"):
+        self.pixel_format = check_pixel_format(pixel_format)
         self.det, self.depth, self.to_host, self.group = det, int(depth), to_host, group
         self.device = torch.device(det.opt.device)
         if self.device.type != "cuda":
@@ -173,8 +188,9 @@ class TrackPipeline(object):
         return None if values is None else values[self.lo:self.hi]
 
     def submit(self, frames, new_video=None, pre_dets=None, frame_ids=None, camera_matrix=None):
-        """frames: one entry per slot (all `slots`, on every rank): uint8 [H,W,3] numpy array or CPU tensor (pinned
-        memory makes the upload asynchronous), or None for an idle slot.  new_video / pre_dets / frame_ids as in
+        """frames: one entry per slot (all `slots`, on every rank): uint8 [H,W,3] (or [3H/2,W] in a YUV pixel_format)
+        numpy array or CPU tensor (pinned memory makes the upload asynchronous), or None for an idle slot.  new_video /
+        pre_dets / frame_ids as in
         run_batch(list, track=True); camera_matrix: [3,3] or [slots,3,3] from this step on (e.g. when a slot starts
         a video from another camera)."""
         if len(self._queue) >= self.depth:
@@ -183,7 +199,7 @@ class TrackPipeline(object):
         if camera_matrix is not None:
             self.cams = np.stack(camera_per_frame(camera_matrix, self.slots))
         frames = self._local(frames, "frame")
-        check_frames(frames, allow_idle=True)
+        check_frames(frames, allow_idle=True, pixel_format=self.pixel_format)
         st = self.sets[self._next]
         self._next = (self._next + 1) % self.depth
         compute = torch.cuda.current_stream(self.device)
@@ -219,7 +235,8 @@ class TrackPipeline(object):
         if n > 0:
             self.det.run_batch(dev_frames, self.cams[self.lo:self.hi], to_host=False, track=True,
                                out=(st.buf.poses[:n], st.buf.n_valid[:n]), new_video=self._local(new_video, "new_video"),
-                               pre_dets=self._local(pre_dets, "pre_dets"), frame_ids=self._local(frame_ids, "frame_ids"))
+                               pre_dets=self._local(pre_dets, "pre_dets"), frame_ids=self._local(frame_ids, "frame_ids"),
+                               pixel_format=self.pixel_format)
         st.compute_done.record(compute)
         st.used = True
         with torch.cuda.stream(self.side_stream):

@@ -33,7 +33,7 @@
  *       utils/pnp/cuboid_pnp_shell.py:11-93, utils/pnp/cuboid_pnp_solver.py:91-239
  *   cp_infer
  *       detectors/base_detector.py:473-654 (process -> post_process -> merge -> PnP)
- *   cp_preprocess / cp_preprocess_affine / cp_preprocess_ragged
+ *   cp_preprocess / cp_preprocess_affine / cp_preprocess_ragged / cp_preprocess_yuv420
  *       detectors/base_detector.py:91-148 pre_process (resize + affine warp + normalise)
  */
 #ifndef CENTERPOSE_B200_H_
@@ -599,6 +599,26 @@ int cp_preprocess_affine(const uint8_t* frames, float* out, int32_t B, int32_t s
  * hundred bytes of per-frame parameters come from the stream-ordered allocator. */
 int cp_preprocess_ragged(const uint8_t* frames, int64_t frames_bytes, const int64_t* offsets, const int32_t* src_hw,
                          float* out, int32_t B, int32_t dst_h, int32_t dst_w, const double* trans_input,
+                         const float mean[3], const float std[3], void* stream);
+
+/* YUV 4:2:0 frames as video decoders and cameras produce them, in cv2's layouts: one uint8 [3H/2, W] buffer per frame,
+ * the Y plane [H, W] first, then
+ *   CP_PIX_NV12: interleaved chroma rows [H/2, W], U at even and V at odd bytes (NVDEC's and most cameras' output);
+ *   CP_PIX_I420: the U plane [H/2, W/2], then the V plane [H/2, W/2] (ffmpeg's yuv420p). */
+enum cp_pixel_format {
+  CP_PIX_NV12 = 0,
+  CP_PIX_I420 = 1
+};
+/* cp_preprocess_ragged on YUV 4:2:0 frames: frame b is [src_hw[b][0] * 3 / 2, src_hw[b][1]] uint8 in `format`, i.e.
+ * src_hw[b][0] * src_hw[b][1] * 3 / 2 bytes starting `offsets[b]` bytes into `frames`; src_hw holds the IMAGE sizes
+ * (H, W), which must be even.  Frame b's output equals, bit for bit, cp_preprocess_ragged on
+ * cv2.cvtColor(frame, COLOR_YUV2BGR_NV12 / COLOR_YUV2BGR_I420) with the same trans_input (NULL: each frame's fix_res
+ * affine).  The conversion (BT.601 limited range, 20-bit fixed point, one U, V per 2x2 block, as cv2) runs inside the
+ * warp on the four taps of every output pixel; taps outside the frame are BGR 0, like warpAffine's border.  An odd size,
+ * an unknown format or a frame that does not fit inside frames_bytes returns CP_ERR_INVALID before any work is enqueued.
+ * A uniform batch is the case of equal sizes. */
+int cp_preprocess_yuv420(const uint8_t* frames, int64_t frames_bytes, const int64_t* offsets, const int32_t* src_hw,
+                         int32_t format, float* out, int32_t B, int32_t dst_h, int32_t dst_w, const double* trans_input,
                          const float mean[3], const float std[3], void* stream);
 
 /* ---- misc ------------------------------------------------------------------ */
