@@ -221,6 +221,8 @@ int dcn_tma_encode(const IgemmParams& p, int Bmax, void* map_out /* 128 bytes, 6
 int launch_dcn_tma(const IgemmParams& p, const void* map, const ConvKernel& k, cudaStream_t stream, LaunchInfo* info);
 
 inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
+// Output columns of a convolution's packed weight matrix: 16, 32, then multiples of 64 (27 offset/mask channels -> 32)
+inline int conv_cout_pad(int Cout) { return round_up(Cout, Cout > 32 ? 64 : (Cout > 16 ? 32 : 16)); }
 
 // ---------------------------------------------------------------------------
 // Programmatic dependent launch (PDL).  The forward is ~90 dependent launches; at batch 1 a launch is ~25 us of which the

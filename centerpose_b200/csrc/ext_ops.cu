@@ -305,7 +305,7 @@ int cp_conv2d(const float* x, const float* weight, const float* bias, const floa
   if (!known_precision(precision)) return fail(CP_ERR_INVALID, "unknown precision");
   int rc;
   cudaStream_t s = (cudaStream_t)stream_;
-  const int CoPad = round_up(Cout, Cout > 32 ? 64 : (Cout > 16 ? 32 : 16));
+  const int CoPad = conv_cout_pad(Cout);
   const int K = k * k * Cin;
   float* scratch = nullptr;
   CP_CUDA_CHECK(cudaMallocAsync(&scratch, ((size_t)K * CoPad + CoPad) * sizeof(float), s));
@@ -373,7 +373,7 @@ int cp_dcn_v2_forward_ex(const float* input, const float* weight, const float* b
   if (B <= 0 || C <= 0 || H <= 0 || W <= 0 || Co <= 0) return fail(CP_ERR_INVALID, "cp_dcn_v2_forward: bad shape");
   cudaStream_t s = (cudaStream_t)stream_;
   const int Cp = round_up(C, 16);
-  const int CoPad = round_up(Co, Co > 32 ? 64 : (Co > 16 ? 32 : 16));
+  const int CoPad = conv_cout_pad(Co);
   const size_t npix = (size_t)B * H * W;
   const size_t n_x = npix * Cp, n_om = npix * 32, n_w = (size_t)9 * Cp * CoPad, n_b = CoPad;
   float* scratch = nullptr;

@@ -19,6 +19,7 @@
 
 #include <map>
 #include <memory>
+#include <set>
 #include <string>
 #include <vector>
 
@@ -46,6 +47,9 @@ struct Act {
   int ext = -1;    // >= 0: external NCHW input index (0 images, 1 pre_img, 2 pre_hm, 3 pre_hm_hp)
   int buf = -1;    // >= 0: the arena allocation it is a view of (cp_plan::bufs)
 };
+
+// the external inputs a multi-track plan takes once per model and frame: pre_hm and pre_hm_hp
+constexpr unsigned kMultiTrackInputs = (1u << 2) | (1u << 3);
 
 enum OpType { OP_IGEMM, OP_MAXPOOL, OP_UPADD, OP_GN_RELU, OP_GRU, OP_MAXPOOL3 };
 
@@ -100,6 +104,21 @@ struct PackJob {
 struct WRef {
   const float* p;
   int64_t n;
+};
+
+// One OP_IGEMM op as the builder declares it (Builder::conv).
+struct ConvSpec {
+  std::vector<Act> src;             // concatenated along channels; an external NCHW source makes it an IGEMM_NCHW_SCALAR stem
+  int k = 1, stride = 1, pad = 0;   // IGEMM_DECONV: 4, 2, 1, as the ConvTranspose2d is declared
+  int Cout = 0;
+  bool relu = false;
+  const Act* res = nullptr;         // added before the ReLU, or after it with res_after_relu
+  bool res_after_relu = false;
+  int head = -1;                    // >= 0: the output is head `head`'s NCHW tensor, else a new allocation
+  int mode = IGEMM_NHWC_VEC;        // or IGEMM_DCN, reading its offsets / mask logits from `om`, or IGEMM_DECONV
+  Act om;
+  std::string wkey, bias_key, bn;   // the state-dict weight, bias and BatchNorm prefix packed for this op ("": none) ...
+  size_t w_off = 0, b_off = 0;      // ... or, with wkey empty, where Builder::merged_weights packed them
 };
 
 }  // namespace
@@ -171,70 +190,69 @@ struct Builder {
     return a;
   }
 
-  // generic conv (+ folded BN) op
-  Act conv(const std::vector<Act>& srcs, const std::string& wkey, const std::string& bias_key,
-           const std::string& bn, int Cout, int k, int stride, int pad, bool relu, const Act* res = nullptr,
-           bool res_after = false, const Act* out_slice = nullptr, int colOff = 0, int ld = 0,
-           size_t shared_w = (size_t)-1, size_t shared_b = (size_t)-1, int out_head = -1) {
+  // The OP_IGEMM op of `s`: its padded GEMM shape, its output allocation, its weight storage and their pack jobs.
+  Act conv(const ConvSpec& s) {
+    const bool deconv = s.mode == IGEMM_DECONV;      // four 2x2-tap phase GEMMs, one [Kpad][CoutPad] block each
     Op op;
-    op.type = OP_IGEMM;
-    op.nsrc = (int)srcs.size();
-    int Cin = 0;
+    op.nsrc = (int)s.src.size();
     for (int i = 0; i < op.nsrc; ++i) {
-      op.src[i] = srcs[i];
-      Cin += srcs[i].C;
+      op.src[i] = s.src[i];
+      op.Cin += s.src[i].C;
     }
-    op.mode = srcs[0].ext >= 0 ? IGEMM_NCHW_SCALAR : IGEMM_NHWC_VEC;
-    op.kh = op.kw = k;
-    op.stride = stride;
-    op.pad = pad;
-    op.Cin = Cin;
-    op.Cout = Cout;
-    op.CoutPad = round_up(Cout, 16);
-    if (op.CoutPad > 16 && op.CoutPad % 32) op.CoutPad = round_up(Cout, 32);
-    if (op.CoutPad > 32 && op.CoutPad % 64) op.CoutPad = round_up(Cout, 64);
-    op.Kpad = round_up(k * k * Cin, 16);
-    op.relu = relu;
-    if (res) {
+    op.mode = s.src[0].ext >= 0 ? IGEMM_NCHW_SCALAR : s.mode;
+    op.kh = op.kw = s.k;
+    op.stride = s.stride;
+    op.pad = s.pad;
+    op.Cout = s.Cout;
+    op.CoutPad = op.w_ld = conv_cout_pad(s.Cout);
+    op.Kpad = round_up((deconv ? 4 : s.k * s.k) * op.Cin, 16);
+    op.relu = s.relu;
+    if (s.res) {
       op.has_res = true;
-      op.res = *res;
-      op.res_after_relu = res_after;
+      op.res = *s.res;
+      op.res_after_relu = s.res_after_relu;
     }
-    int Hin = srcs[0].H, Win = srcs[0].W;
-    int Ho = (Hin + 2 * pad - k) / stride + 1, Wo = (Win + 2 * pad - k) / stride + 1;
-    op.out_head = out_head;
-    if (out_slice) {
-      op.out = *out_slice;
-    } else if (out_head < 0) {
-      op.out = new_act(Cout, Ho, Wo);
-      if (op.CoutPad != Cout) {
-        // padded channels are never stored (the kernel masks n >= Cout); the
-        // pixel stride is widened for the 27 -> 32 offset/mask tensor only
-      }
+    op.om = s.om;
+    const int Hin = s.src[0].H, Win = s.src[0].W;
+    const int Ho = deconv ? 2 * Hin : (Hin + 2 * s.pad - s.k) / s.stride + 1;
+    const int Wo = deconv ? 2 * Win : (Win + 2 * s.pad - s.k) / s.stride + 1;
+    op.out_head = s.head;
+    // padded channels are never stored (the kernels mask n >= Cout), but a new allocation's pixel stride spans them:
+    // the 27-channel offset / mask tensor is read in rows of 32
+    if (s.head < 0) op.out = new_act(op.CoutPad, Ho, Wo);
+    op.out.C = s.Cout;
+    op.out.H = Ho;
+    op.out.W = Wo;
+    if (s.wkey.empty()) {
+      op.w_off = s.w_off;
+      op.b_off = s.b_off;
     } else {
-      op.out.C = Cout;
-      op.out.H = Ho;
-      op.out.W = Wo;
+      op.w_off = walloc((size_t)(deconv ? 4 : 1) * op.Kpad * op.CoutPad);
+      op.b_off = walloc(op.CoutPad);
+      add_pack(deconv ? PACK_DECONV : PACK_CONV, s.wkey, s.bias_key, s.bn, s.Cout, op.Cin, s.k, op.CoutPad, op.Kpad,
+               op.CoutPad, 0, op.w_off, op.b_off);
     }
-    // weights
-    op.w_ld = op.CoutPad;
-    if (shared_w != (size_t)-1) {
-      op.w_off = shared_w;
-      op.b_off = shared_b;
-    } else {
-      int ldw = ld ? ld : op.CoutPad;
-      op.w_off = walloc((size_t)op.Kpad * ldw);
-      op.b_off = walloc(ldw);
-      add_pack(wkey, bias_key, bn, Cout, Cin, k, op.CoutPad, op.Kpad, ldw, colOff, op.w_off, op.b_off);
-    }
-    op.name = wkey.empty() ? std::string("conv") + std::to_string(k) + "x" + std::to_string(k) + "_merged_" + std::to_string(Cout)
-                           : wkey.substr(0, wkey.rfind('.'));
+    op.name = s.wkey.empty() ? "conv" + std::to_string(s.k) + "x" + std::to_string(s.k) + "_merged_" + std::to_string(s.Cout)
+                             : s.wkey.substr(0, s.wkey.rfind('.'));
+    if (op.mode == IGEMM_DCN) op.name += "(dcn)";
     P->ops.push_back(op);
     return op.out;
   }
 
-  void add_pack(const std::string& wkey, const std::string& bias_key, const std::string& bn, int Cout, int Cin,
-                int k, int CoutPad, int Kpad, int ld, int colOff, size_t w_off, size_t b_off) {
+  // Several convs over one input, side by side in one [Kpad][keys.size() * Cout] weight matrix and bias, for one
+  // N-wide conv (ConvSpec w_off / b_off): the merged heads 3x3s and the convGRU gate convs.  Returns (w_off, b_off).
+  std::pair<size_t, size_t> merged_weights(const std::vector<std::string>& keys, bool bias, int Cin, int k, int Cout) {
+    const int N = (int)keys.size() * Cout, Kpad = round_up(k * k * Cin, 16);
+    const size_t w = walloc((size_t)Kpad * N), b = walloc(N);
+    for (size_t i = 0; i < keys.size(); ++i)
+      add_pack(PACK_CONV, keys[i] + ".weight", bias ? keys[i] + ".bias" : "", "", Cout, Cin, k, Cout, Kpad, N,
+               (int)i * Cout, w, b);
+    return {w, b};
+  }
+
+  // The bias (+ folded BN) job and the weight job of a [Kpad][CoutPad] block at column `colOff` of a matrix `ld` wide
+  void add_pack(PackType type, const std::string& wkey, const std::string& bias_key, const std::string& bn, int Cout,
+                int Cin, int k, int CoutPad, int Kpad, int ld, int colOff, size_t w_off, size_t b_off) {
     PackJob jb;
     jb.type = PACK_BIAS;
     jb.key = bias_key;
@@ -245,7 +263,7 @@ struct Builder {
     jb.scale = walloc(CoutPad);
     P->jobs.push_back(jb);
     PackJob jw;
-    jw.type = PACK_CONV;
+    jw.type = type;
     jw.key = wkey;
     jw.Cout = Cout;
     jw.Cin = Cin;
@@ -261,8 +279,9 @@ struct Builder {
   }
 
   Act conv_bn(const Act& x, const std::string& convkey, const std::string& bnkey, int Cout, int k, int stride,
-              int pad, bool relu, const Act* res = nullptr, bool res_after = false) {
-    return conv({x}, convkey + ".weight", "", bnkey, Cout, k, stride, pad, relu, res, res_after);
+              int pad, bool relu, const Act* res = nullptr) {
+    return conv({.src = {x}, .k = k, .stride = stride, .pad = pad, .Cout = Cout, .relu = relu, .res = res,
+                 .wkey = convkey + ".weight", .bn = bnkey});
   }
 
   Act maxpool(const Act& x) {
@@ -292,45 +311,8 @@ struct Builder {
 
   // ConvTranspose2d(Cin, Cout, 4, stride 2, pad 1, bias=False) + folded BN + ReLU (msra_resnet.py:219-230)
   Act deconv_bn(const Act& x, const std::string& wkey, const std::string& bn, int Cout) {
-    Op op;
-    op.type = OP_IGEMM;
-    op.nsrc = 1;
-    op.src[0] = x;
-    op.mode = IGEMM_DECONV;
-    op.kh = op.kw = 4;
-    op.stride = 2;
-    op.pad = 1;
-    op.Cin = x.C;
-    op.Cout = Cout;
-    op.CoutPad = round_up(Cout, 64);
-    op.Kpad = 4 * x.C;
-    op.relu = true;
-    op.out = new_act(Cout, 2 * x.H, 2 * x.W);
-    op.w_ld = op.CoutPad;
-    op.w_off = walloc((size_t)4 * op.Kpad * op.CoutPad);
-    op.b_off = walloc(op.CoutPad);
-    PackJob jb;
-    jb.type = PACK_BIAS;
-    jb.bn = bn;
-    jb.Cout = Cout;
-    jb.CoutPad = op.CoutPad;
-    jb.dst = op.b_off;
-    jb.scale = walloc(op.CoutPad);
-    P->jobs.push_back(jb);
-    PackJob jw;
-    jw.type = PACK_DECONV;
-    jw.key = wkey;
-    jw.Cout = Cout;
-    jw.Cin = x.C;
-    jw.CoutPad = op.CoutPad;
-    jw.Kpad = op.Kpad;
-    jw.dst = op.w_off;
-    jw.scale = jb.scale;
-    jw.use_scale = true;
-    P->jobs.push_back(jw);
-    op.name = wkey.substr(0, wkey.rfind('.'));
-    P->ops.push_back(op);
-    return op.out;
+    return conv({.src = {x}, .k = 4, .stride = 2, .pad = 1, .Cout = Cout, .relu = true, .mode = IGEMM_DECONV, .wkey = wkey,
+                 .bn = bn});
   }
 
   // BasicBlock (msra_resnet.py:35-64) and Bottleneck (:67-105): out = relu(bn(conv) + residual), the stride on conv1 of
@@ -342,16 +324,16 @@ struct Builder {
       residual = conv_bn(x, p + ".downsample.0", p + ".downsample.1", Cout, 1, stride, 0, false);
     if (!bottleneck) {
       Act y = conv_bn(x, p + ".conv1", p + ".bn1", planes, 3, stride, 1, true);
-      return conv_bn(y, p + ".conv2", p + ".bn2", planes, 3, 1, 1, true, &residual, false);
+      return conv_bn(y, p + ".conv2", p + ".bn2", planes, 3, 1, 1, true, &residual);
     }
     Act y = conv_bn(x, p + ".conv1", p + ".bn1", planes, 1, 1, 0, true);
     y = conv_bn(y, p + ".conv2", p + ".bn2", planes, 3, stride, 1, true);
-    return conv_bn(y, p + ".conv3", p + ".bn3", Cout, 1, 1, 0, true, &residual, false);
+    return conv_bn(y, p + ".conv3", p + ".bn3", Cout, 1, 1, 0, true, &residual);
   }
 
   Act basic_block(const Act& x, const std::string& p, int Cout, int stride, const Act& residual) {
     Act y = conv_bn(x, p + ".conv1", p + ".bn1", Cout, 3, stride, 1, true);
-    return conv_bn(y, p + ".conv2", p + ".bn2", Cout, 3, 1, 1, true, &residual, false);
+    return conv_bn(y, p + ".conv2", p + ".bn2", Cout, 3, 1, 1, true, &residual);
   }
 
   // levels == 1 Tree
@@ -366,7 +348,7 @@ struct Builder {
     Act x2 = basic_block(x1, p + ".tree2", Cout, 1, x1);
     std::vector<Act> cat = {x2, x1};
     for (auto& c : children) cat.push_back(c);
-    return conv(cat, p + ".root.conv.weight", "", p + ".root.bn", Cout, 1, 1, 0, true);
+    return conv({.src = cat, .Cout = Cout, .relu = true, .wkey = p + ".root.conv.weight", .bn = p + ".root.bn"});
   }
 
   // levels == 2 Tree with level_root (level3 / level4); the outer `project` is dead compute
@@ -376,53 +358,12 @@ struct Builder {
     return tree1(x1, p + ".tree2", Cout, Cout, 1, false, {bottom, x1});
   }
 
+  // DCN (DCNv2/dcn_v2.py:97-128): the 3x3 offset / mask conv (18 offsets + 9 mask logits), then the deformable 3x3
   Act deform_conv(const Act& x, const std::string& p, int Cout) {
-    // offset / mask conv: 3x3 -> 27 channels stored with pixel stride 32
-    Op om;
-    om.type = OP_IGEMM;
-    om.nsrc = 1;
-    om.src[0] = x;
-    om.mode = IGEMM_NHWC_VEC;
-    om.kh = om.kw = 3;
-    om.stride = 1;
-    om.pad = 1;
-    om.Cin = x.C;
-    om.Cout = 27;
-    om.CoutPad = 32;
-    om.Kpad = 9 * x.C;
-    om.out = new_act(32, x.H, x.W);
-    om.out.C = 27;
-    om.w_ld = 32;
-    om.w_off = walloc((size_t)om.Kpad * 32);
-    om.b_off = walloc(32);
-    add_pack(p + ".conv.conv_offset_mask.weight", p + ".conv.conv_offset_mask.bias", "", 27, x.C, 3, 32,
-             om.Kpad, 32, 0, om.w_off, om.b_off);
-    om.name = p + ".conv.conv_offset_mask";
-    P->ops.push_back(om);
-
-    Op op;
-    op.type = OP_IGEMM;
-    op.nsrc = 1;
-    op.src[0] = x;
-    op.mode = IGEMM_DCN;
-    op.kh = op.kw = 3;
-    op.stride = 1;
-    op.pad = 1;
-    op.Cin = x.C;
-    op.Cout = Cout;
-    op.CoutPad = round_up(Cout, 64);
-    op.Kpad = 9 * x.C;
-    op.relu = true;
-    op.om = om.out;
-    op.out = new_act(Cout, x.H, x.W);
-    op.w_ld = op.CoutPad;
-    op.w_off = walloc((size_t)op.Kpad * op.CoutPad);
-    op.b_off = walloc(op.CoutPad);
-    add_pack(p + ".conv.weight", p + ".conv.bias", p + ".actf.0", Cout, x.C, 3, op.CoutPad, op.Kpad,
-             op.CoutPad, 0, op.w_off, op.b_off);
-    op.name = p + ".conv(dcn)";
-    P->ops.push_back(op);
-    return op.out;
+    const Act om = conv({.src = {x}, .k = 3, .pad = 1, .Cout = 27, .wkey = p + ".conv.conv_offset_mask.weight",
+                         .bias_key = p + ".conv.conv_offset_mask.bias"});
+    return conv({.src = {x}, .k = 3, .pad = 1, .Cout = Cout, .relu = true, .mode = IGEMM_DCN, .om = om,
+                 .wkey = p + ".conv.weight", .bias_key = p + ".conv.bias", .bn = p + ".actf.0"});
   }
 
   Act up_add(const Act& x, const std::string& key, int f, const Act& skip) {
@@ -466,14 +407,16 @@ Act resnet(Builder& b, const cp_config& c, Ext ext) {
   static const int kBlocks[5][4] = {{2, 2, 2, 2}, {3, 4, 6, 3}, {3, 4, 6, 3}, {3, 4, 23, 3}, {3, 8, 36, 3}};
   const int d = c.arch - CP_ARCH_RES_18;
   const bool bottleneck = c.arch >= CP_ARCH_RES_50;
-  Act x = b.conv(std::vector<Act>{ext(0, 3)}, "conv1.weight", "", "bn1", 64, 7, 2, 3, true);
+  Act x = b.conv({.src = {ext(0, 3)}, .k = 7, .stride = 2, .pad = 3, .Cout = 64, .relu = true, .wkey = "conv1.weight",
+                  .bn = "bn1"});
   x = b.maxpool3(x, nullptr, "maxpool");
   if (c.tracking) {      // x = x + pre_img_layer(pre_img) + pre_hm_layer(pre_hm) + pre_hm_hp_layer(pre_hm_hp), in this order
     const char* keys[3] = {"pre_img_layer", "pre_hm_layer", "pre_hm_hp_layer"};
     const int cin[3] = {3, 1, 8};
     for (int e = 0; e < 3; ++e) {
       const std::string k = keys[e];
-      Act t = b.conv(std::vector<Act>{ext(e + 1, cin[e])}, k + ".0.weight", "", k + ".1", 64, 7, 2, 3, true);
+      Act t = b.conv({.src = {ext(e + 1, cin[e])}, .k = 7, .stride = 2, .pad = 3, .Cout = 64, .relu = true,
+                      .wkey = k + ".0.weight", .bn = k + ".1"});
       x = b.maxpool3(t, &x, k + ".3");
     }
   }
@@ -511,12 +454,14 @@ int build_graph(cp_plan* P) {
     F = resnet(b, c, ext);
   } else {
     // ---- DLA-34 base (pose_dla_dcn.py:310-322)
-    Act x = b.conv({ext(0, 3)}, "base.base_layer.0.weight", "", "base.base_layer.1", 16, 7, 1, 3, true);
-    if (c.tracking) {
-      x = b.conv({ext(1, 3)}, "base.pre_img_layer.0.weight", "", "base.pre_img_layer.1", 16, 7, 1, 3, true, &x, true);
-      x = b.conv({ext(2, 1)}, "base.pre_hm_layer.0.weight", "", "base.pre_hm_layer.1", 16, 7, 1, 3, true, &x, true);
-      x = b.conv({ext(3, 8)}, "base.pre_hm_hp_layer.0.weight", "", "base.pre_hm_hp_layer.1", 16, 7, 1, 3, true, &x,
-                 true);
+    Act x = b.conv({.src = {ext(0, 3)}, .k = 7, .pad = 3, .Cout = 16, .relu = true, .wkey = "base.base_layer.0.weight",
+                    .bn = "base.base_layer.1"});
+    if (c.tracking) {      // x = x + relu(bn(conv(pre_*))) for pre_img, pre_hm, pre_hm_hp, in this order
+      const char* keys[3] = {"base.pre_img_layer", "base.pre_hm_layer", "base.pre_hm_hp_layer"};
+      const int cin[3] = {3, 1, 8};
+      for (int e = 0; e < 3; ++e)
+        x = b.conv({.src = {ext(e + 1, cin[e])}, .k = 7, .pad = 3, .Cout = 16, .relu = true, .res = &x,
+                    .res_after_relu = true, .wkey = std::string(keys[e]) + ".0.weight", .bn = std::string(keys[e]) + ".1"});
     }
     std::vector<Act> lv(6);
     lv[0] = b.conv_bn(x, "base.level0.0", "base.level0.1", 16, 3, 1, 1, true);
@@ -568,27 +513,16 @@ int build_graph(cp_plan* P) {
   if (gru) {
     const int steps = c.tracking_task_gru ? 4 : 3;
     const int HC = 64;
-    // xi = [Wir x + b | Wiz x + b | Win x + b]
-    Act xi = b.new_act(3 * HC, F.H, F.W);
-    size_t wx = b.walloc((size_t)9 * 64 * 3 * HC), bx = b.walloc(3 * HC);
-    const char* xin[3] = {"Wir", "Wiz", "Win"};
-    const char* hin[3] = {"Whr", "Whz", "Whn"};
-    for (int g = 0; g < 3; ++g)
-      b.add_pack(std::string("convGRU.cell0.") + xin[g] + ".weight", std::string("convGRU.cell0.") + xin[g] + ".bias",
-                 "", HC, 64, 3, HC, 9 * 64, 3 * HC, g * HC, wx, bx);
-    b.conv({F}, "", "", "", 3 * HC, 3, 1, 1, false, nullptr, false, &xi, 0, 0, wx, bx);
-    size_t wh = b.walloc((size_t)9 * HC * 3 * HC), bh = b.walloc(3 * HC);
-    for (int g = 0; g < 3; ++g)
-      b.add_pack(std::string("convGRU.cell0.") + hin[g] + ".weight", "", "", HC, HC, 3, HC, 9 * HC, 3 * HC, g * HC, wh,
-                 bh);
+    // xi = [Wir x + b | Wiz x + b | Win x + b], hh = [Whr h | Whz h | Whn h]
+    const std::string cell = "convGRU.cell0.";
+    const auto [wx, bx] = b.merged_weights({cell + "Wir", cell + "Wiz", cell + "Win"}, true, F.C, 3, HC);
+    const Act xi = b.conv({.src = {F}, .k = 3, .pad = 1, .Cout = 3 * HC, .w_off = wx, .b_off = bx});
+    const auto [wh, bh] = b.merged_weights({cell + "Whr", cell + "Whz", cell + "Whn"}, false, HC, 3, HC);
     std::vector<Act> hs;
     Act hprev;
     for (int s = 0; s < steps; ++s) {
       Act hh;
-      if (s > 0) {
-        hh = b.new_act(3 * HC, F.H, F.W);
-        b.conv({hprev}, "", "", "", 3 * HC, 3, 1, 1, false, nullptr, false, &hh, 0, 0, wh, bh);
-      }
+      if (s > 0) hh = b.conv({.src = {hprev}, .k = 3, .pad = 1, .Cout = 3 * HC, .w_off = wh, .b_off = bh});
       Op op;
       op.type = OP_GRU;
       op.gx = xi;
@@ -629,13 +563,10 @@ int build_graph(cp_plan* P) {
       if (!done[h] && feat_for_head[h].off == feat_for_head[h0].off) grp.push_back(h);
     const Act& f = feat_for_head[h0];
     const int N = (int)grp.size() * HCV;
-    Act mid = b.new_act(N, f.H, f.W);
-    size_t wm = b.walloc((size_t)9 * f.C * N), bm = b.walloc(N);
-    for (size_t gi = 0; gi < grp.size(); ++gi) {
-      const std::string& n = P->head_names[grp[gi]];
-      b.add_pack(n + ".0.weight", n + ".0.bias", "", HCV, f.C, 3, HCV, 9 * f.C, N, (int)gi * HCV, wm, bm);
-    }
-    b.conv({f}, "", "", "", N, 3, 1, 1, !gru, nullptr, false, &mid, 0, 0, wm, bm);
+    std::vector<std::string> keys;
+    for (int h : grp) keys.push_back(P->head_names[h] + ".0");
+    const auto [wm, bm] = b.merged_weights(keys, true, f.C, 3, HCV);
+    const Act mid = b.conv({.src = {f}, .k = 3, .pad = 1, .Cout = N, .relu = !gru, .w_off = wm, .b_off = bm});
     const size_t merged_idx = P->ops.size() - 1;
     std::vector<int> children;
     for (size_t gi = 0; gi < grp.size(); ++gi) {
@@ -668,8 +599,7 @@ int build_graph(cp_plan* P) {
         P->ops.push_back(g);
         last = n + ".3";
       }
-      b.conv({slice}, last + ".weight", last + ".bias", "", c.head_channels[h], 1, 1, 0, false, nullptr, false,
-             nullptr, 0, 0, (size_t)-1, (size_t)-1, h);
+      b.conv({.src = {slice}, .Cout = c.head_channels[h], .head = h, .wkey = last + ".weight", .bias_key = last + ".bias"});
       children.push_back((int)P->ops.size() - 1);
     }
     if (!gru) P->ops[merged_idx].head_children = children;     // GroupNorm sits between the two convs in dlav1
@@ -756,6 +686,12 @@ void igemm_params(const cp_plan* P, const Op& op, int batch, const float* const 
   }
 }
 
+// igemm_params at the plan's batch with no inputs bound: what kernel selection, tensor maps and weight tiles read
+void plan_params(const cp_plan* P, const Op& op, IgemmParams* p) {
+  static const float* const no_ext[4] = {};
+  igemm_params(P, op, P->B, no_ext, nullptr, p);
+}
+
 // The kernel of every conv op, its weight-tile offset, and which per-head 1x1 convs run inside the epilogue of their
 // merged heads conv.  Runs before the arena exists (cp_plan_memory has no device at all): the choice reads shapes,
 // strides and whether a residual is added, never an address.
@@ -763,13 +699,12 @@ void select_kernels(cp_plan* P) {
   // 16-channel layers (level0 / level1): 133 K single-tile CTAs of almost no MMA work are dominated by the fixed per-CTA
   // cost of a tensor-core kernel -> keep them, and the NCHW stems, on CUDA cores
   const ConvPolicy pol{true, !P->no_dcn_tma, true, true};
-  const float* const no_ext[4] = {nullptr, nullptr, nullptr, nullptr};
   static const float residual_present = 0.f;      // a residual at arena offset 0 of a null arena would read as none
   P->umma_bytes = 0;
   for (auto& op : P->ops) {
     if (op.type != OP_IGEMM) continue;
     IgemmParams p;
-    igemm_params(P, op, P->B, no_ext, nullptr, &p);
+    plan_params(P, op, &p);
     if (op.has_res) p.residual = &residual_present;
     op.kernel = select_conv_kernel(p, P->cfg.precision, pol);
     op.tile_off = P->umma_bytes;
@@ -795,83 +730,74 @@ void select_kernels(cp_plan* P) {
   }
 }
 
-// The op range over which each arena allocation is live, from the ops that run (a fused-away 1x1 does not, and a
-// fused heads conv never stores its hidden tile), then, with CP_PLAN_REUSE_ACTIVATIONS, the packed offsets.  The head
+// Every arena tensor op `op` reads or writes when it runs, passed to f as an Act&: none for a fused-away 1x1, the plan's
+// head buffer for a head output, and no hidden tile for a fused heads conv (its children's head buffers instead).
+template <class F>
+void for_each_act(cp_plan* P, Op& op, F f) {
+  if (op.fused_away) return;
+  switch (op.type) {
+    case OP_IGEMM:
+      for (int s = 0; s < op.nsrc; ++s) f(op.src[s]);
+      if (op.has_res) f(op.res);
+      if (op.mode == IGEMM_DCN) f(op.om);
+      if (op.out_head >= 0) f(P->head_bufs[op.out_head]);
+      else if (!op.fuse_heads) f(op.out);
+      if (op.fuse_heads)
+        for (int c : op.head_children) f(P->head_bufs[P->ops[c].out_head]);
+      return;
+    case OP_MAXPOOL:
+    case OP_MAXPOOL3:
+    case OP_UPADD:
+      f(op.src[0]);
+      if (op.has_res) f(op.res);
+      if (op.has_skip) f(op.skip);
+      break;
+    case OP_GN_RELU:
+      break;
+    case OP_GRU:
+      f(op.gx);
+      if (!op.first_step) {
+        f(op.gh);
+        f(op.gprev);
+      }
+      break;
+  }
+  f(op.out);
+}
+
+// The op range over which each arena allocation is live, then, with CP_PLAN_REUSE_ACTIVATIONS, the packed offsets.  Both
+// come from one list of uses, so no view can be moved without being live or live without being moved.  The head
 // buffers stay live to the end of the call: cp_infer decodes them after the last op.
 void layout_arena(cp_plan* P) {
+  std::vector<std::pair<int, Act*>> uses;      // (op index, view)
+  const int end = (int)P->ops.size();
+  for (int i = 0; i < end; ++i) for_each_act(P, P->ops[i], [&](Act& a) { uses.push_back({i, &a}); });
+  for (Act& h : P->head_bufs) uses.push_back({end, &h});
   for (auto& b : P->bufs) b.first = b.last = -1;
-  auto touch = [P](const Act& a, int i) {
-    if (a.buf < 0) return;
-    ArenaAlloc& b = P->bufs[a.buf];
+  for (const auto& [i, a] : uses) {
+    if (a->buf < 0) continue;
+    ArenaAlloc& b = P->bufs[a->buf];
     if (b.first < 0) b.first = i;
     b.last = std::max(b.last, i);
-  };
-  const int end = (int)P->ops.size();
-  for (int i = 0; i < end; ++i) {
-    const Op& op = P->ops[i];
-    if (op.fused_away) continue;
-    switch (op.type) {
-      case OP_IGEMM:
-        for (int s = 0; s < op.nsrc; ++s) touch(op.src[s], i);
-        if (op.has_res) touch(op.res, i);
-        if (op.mode == IGEMM_DCN) touch(op.om, i);
-        if (op.out_head >= 0) touch(P->head_bufs[op.out_head], i);
-        else if (!op.fuse_heads) touch(op.out, i);
-        if (op.fuse_heads)
-          for (int c : op.head_children) touch(P->head_bufs[P->ops[c].out_head], i);
-        break;
-      case OP_MAXPOOL:
-        touch(op.src[0], i);
-        touch(op.out, i);
-        break;
-      case OP_MAXPOOL3:
-        touch(op.src[0], i);
-        if (op.has_res) touch(op.res, i);
-        touch(op.out, i);
-        break;
-      case OP_UPADD:
-        touch(op.src[0], i);
-        if (op.has_skip) touch(op.skip, i);
-        touch(op.out, i);
-        break;
-      case OP_GN_RELU:
-        touch(op.out, i);
-        break;
-      case OP_GRU:
-        touch(op.gx, i);
-        if (!op.first_step) {
-          touch(op.gh, i);
-          touch(op.gprev, i);
-        }
-        touch(op.out, i);
-        break;
-    }
   }
-  for (const Act& h : P->head_bufs) touch(h, end);
   if (!P->reuse) return;
   std::vector<size_t> off;
   P->act_floats = arena_pack(P->bufs, &off);
-  auto move = [&](Act& a) {
-    if (a.buf >= 0) a.off = a.off - P->buf_off[a.buf] + off[a.buf];
-  };
-  for (auto& op : P->ops) {
-    for (Act& a : op.src) move(a);
-    for (Act* a : {&op.out, &op.res, &op.om, &op.skip, &op.gx, &op.gh, &op.gprev}) move(*a);
-  }
-  for (Act& h : P->head_bufs) move(h);
+  std::set<Act*> moved;      // a head buffer is listed by the op that writes it and again at the end
+  for (const auto& [i, a] : uses)
+    if (a->buf >= 0 && moved.insert(a).second) a->off = a->off - P->buf_off[a->buf] + off[a->buf];
   P->buf_off = off;
 }
 
 // False for an allocation that got no memory (a reuse plan's merged heads hidden tile when the 1x1s are fused).
 bool has_memory(const cp_plan* P, const Act& a) { return a.buf < 0 || !P->reuse || P->bufs[a.buf].first >= 0; }
 
-// The tensor maps of the TMA convolutions: they hold the arena addresses.
+// The tensor maps of the TMA convolutions that launch: they hold the arena addresses.
 int encode_maps(cp_plan* P) {
-  const float* const no_ext[4] = {nullptr, nullptr, nullptr, nullptr};
   for (auto& op : P->ops) {
-    if (op.type != OP_IGEMM) continue;
+    if (op.type != OP_IGEMM || op.fused_away) continue;
     IgemmParams p;
-    igemm_params(P, op, P->B, no_ext, nullptr, &p);
+    plan_params(P, op, &p);
     if (int rc = conv_encode(op.kernel, p, P->B * P->models, &op.maps)) return rc;
   }
   return CP_OK;
@@ -953,7 +879,7 @@ static int plan_layout(cp_plan* P, const cp_config* cfg, int32_t num_models, uin
   for (int i = 0; i < cfg->num_heads; ++i) P->cfg.head_names[i] = P->head_names[i].c_str();
   P->B = cfg->max_batch;
   P->models = num_models;
-  P->ext_per_model = (flags & CP_PLAN_MULTI_TRACK) ? (1u << 2) | (1u << 3) : 0u;   // pre_hm, pre_hm_hp: one per model and frame
+  P->ext_per_model = (flags & CP_PLAN_MULTI_TRACK) ? kMultiTrackInputs : 0u;
   P->reuse = (flags & CP_PLAN_REUSE_ACTIVATIONS) != 0;
   P->model_loaded.assign(num_models, 0);
   P->H = cfg->height;
@@ -1119,11 +1045,10 @@ int cp_plan_load_weights_model(cp_plan* P, int32_t model, const char* const* nam
     }
   }
   // second pass: tensor-core weight tiles are cut from the finished fp32 matrices (merged matrices are complete now)
-  const float* const no_ext[4] = {nullptr, nullptr, nullptr, nullptr};
   for (auto& op : P->ops) {
     if (op.type != OP_IGEMM || !op.kernel.wbytes) continue;
     IgemmParams p;
-    igemm_params(P, op, P->B, no_ext, nullptr, &p);
+    plan_params(P, op, &p);
     p.wgt += (size_t)model * P->w_floats;
     if ((rc = conv_pack(op.kernel, p, op.w_ld, P->umma_wts + (size_t)model * P->umma_bytes + op.tile_off, s))) return rc;
   }
@@ -1293,11 +1218,19 @@ static void op_work(const Op& op, int batch, double* flops, double* bytes) {
   }
 }
 
+// The checks every call that runs the schedule starts with: `given` is false when a pointer `fn` needs is null, `load`
+// names the call that loads the weights.
+static int check_run(const cp_plan* P, bool given, int32_t batch, const char* fn, const char* load = "cp_plan_load_weights") {
+  if (!P || !given) return fail(CP_ERR_INVALID, std::string(fn) + ": null argument");
+  if (!P->loaded) return fail(CP_ERR_NOT_LOADED, std::string(fn) + ": call " + load + " first");
+  if (batch <= 0 || batch > P->B) return fail(CP_ERR_INVALID, std::string(fn) + ": batch exceeds the plan's max_batch");
+  return CP_OK;
+}
+static const char* const kLoadEveryModel = "cp_plan_load_weights_model for every model";
+
 int cp_forward(cp_plan* P, int32_t batch, const float* images, const float* pre_img, const float* pre_hm,
                const float* pre_hm_hp, float* const* head_out, void* stream) {
-  if (!P || !images || !head_out) return fail(CP_ERR_INVALID, "cp_forward: null argument");
-  if (!P->loaded) return fail(CP_ERR_NOT_LOADED, "cp_forward: call cp_plan_load_weights first");
-  if (batch <= 0 || batch > P->B) return fail(CP_ERR_INVALID, "cp_forward: batch exceeds the plan's max_batch");
+  if (int rc = check_run(P, images && head_out, batch, "cp_forward")) return rc;
   const float* ext[4] = {images, pre_img, pre_hm, pre_hm_hp};
   return run_forward(P, batch, ext, head_out, (cudaStream_t)stream);
 }
@@ -1307,9 +1240,7 @@ int cp_plan_num_ops(const cp_plan* P) { return P ? (int)P->ops.size() : 0; }
 int cp_plan_profile(cp_plan* P, int32_t batch, const float* images, const float* pre_img, const float* pre_hm,
                     const float* pre_hm_hp, float* const* head_out, void* stream, cp_op_stat* stats, int32_t max_stats,
                     int32_t* n_stats) {
-  if (!P || !images || !head_out || !stats || !n_stats) return fail(CP_ERR_INVALID, "cp_plan_profile: null argument");
-  if (!P->loaded) return fail(CP_ERR_NOT_LOADED, "cp_plan_profile: call cp_plan_load_weights first");
-  if (batch <= 0 || batch > P->B) return fail(CP_ERR_INVALID, "cp_plan_profile: batch exceeds the plan's max_batch");
+  if (int rc = check_run(P, images && head_out && stats && n_stats, batch, "cp_plan_profile")) return rc;
   const float* ext[4] = {images, pre_img, pre_hm, pre_hm_hp};
   ProfCtx ctx;
   int rc = run_forward(P, batch, ext, head_out, (cudaStream_t)stream, &ctx);
@@ -1431,9 +1362,7 @@ int cp_plan_arena(const cp_plan* P, float** act, int64_t* floats) {
 int cp_plan_run_ops(cp_plan* P, int32_t batch, int32_t first, int32_t last, const float* images, const float* pre_img,
                     const float* pre_hm, const float* pre_hm_hp, float* const* head_out, void* stream,
                     cp_op_launch* info) {
-  if (!P || !images || !head_out) return fail(CP_ERR_INVALID, "cp_plan_run_ops: null argument");
-  if (!P->loaded) return fail(CP_ERR_NOT_LOADED, "cp_plan_run_ops: call cp_plan_load_weights first");
-  if (batch <= 0 || batch > P->B) return fail(CP_ERR_INVALID, "cp_plan_run_ops: batch exceeds the plan's max_batch");
+  if (int rc = check_run(P, images && head_out, batch, "cp_plan_run_ops")) return rc;
   if (first < 0 || last < first || last > (int)P->ops.size())
     return fail(CP_ERR_INVALID, "cp_plan_run_ops: op range outside the schedule");
   const float* ext[4] = {images, pre_img, pre_hm, pre_hm_hp};
@@ -1452,9 +1381,7 @@ static int infer_models(cp_plan* P, int32_t batch, const float* images, const fl
 int cp_infer(cp_plan* P, int32_t batch, const float* images, const float* pre_img, const float* pre_hm,
              const float* pre_hm_hp, const cp_decode_params* prm, const double* meta, float* const* heads_out,
              float* dets, float* poses, int32_t* n_valid, void* stream) {
-  if (!P || !images || !prm || !meta || !poses || !n_valid) return fail(CP_ERR_INVALID, "cp_infer: null argument");
-  if (!P->loaded) return fail(CP_ERR_NOT_LOADED, "cp_infer: call cp_plan_load_weights first");
-  if (batch <= 0 || batch > P->B) return fail(CP_ERR_INVALID, "cp_infer: batch exceeds the plan's max_batch");
+  if (int rc = check_run(P, images && prm && meta && poses && n_valid, batch, "cp_infer")) return rc;
   if (P->models > 1)
     return fail(CP_ERR_INVALID, P->cfg.tracking ? "cp_infer: a multi-model tracking plan runs through cp_infer_multi_track"
                                                 : "cp_infer: a multi-model plan runs through cp_infer_multi");
@@ -1476,9 +1403,8 @@ static int check_model_prms(const cp_plan* P, const cp_decode_params* prms, cons
 
 int cp_infer_multi(cp_plan* P, int32_t batch, const float* images, const cp_decode_params* prms, const double* meta,
                    float* const* heads_out, float* dets, float* poses, int32_t* n_valid, void* stream) {
-  if (!P || !images || !prms || !meta || !poses || !n_valid) return fail(CP_ERR_INVALID, "cp_infer_multi: null argument");
-  if (!P->loaded) return fail(CP_ERR_NOT_LOADED, "cp_infer_multi: call cp_plan_load_weights_model for every model first");
-  if (batch <= 0 || batch > P->B) return fail(CP_ERR_INVALID, "cp_infer_multi: batch exceeds the plan's max_batch");
+  if (int rc = check_run(P, images && prms && meta && poses && n_valid, batch, "cp_infer_multi", kLoadEveryModel))
+    return rc;
   if (P->cfg.tracking)
     return fail(CP_ERR_INVALID, "cp_infer_multi: tracking plans run through cp_infer or cp_infer_multi_track");
   if (int rc = check_model_prms(P, prms, "cp_infer_multi")) return rc;
@@ -1488,12 +1414,10 @@ int cp_infer_multi(cp_plan* P, int32_t batch, const float* images, const cp_deco
 int cp_infer_multi_track(cp_plan* P, int32_t batch, const float* images, const float* pre_img, const float* pre_hm,
                          const float* pre_hm_hp, const cp_decode_params* prms, const double* meta, float* const* heads_out,
                          float* dets, float* poses, int32_t* n_valid, void* stream) {
-  if (!P || !images || !pre_img || !pre_hm || !pre_hm_hp || !prms || !meta || !poses || !n_valid)
-    return fail(CP_ERR_INVALID, "cp_infer_multi_track: null argument");
-  if (!P->cfg.tracking || P->ext_per_model != ((1u << 2) | (1u << 3)))
+  const bool given = images && pre_img && pre_hm && pre_hm_hp && prms && meta && poses && n_valid;
+  if (P && given && (!P->cfg.tracking || P->ext_per_model != kMultiTrackInputs))
     return fail(CP_ERR_INVALID, "cp_infer_multi_track: the plan was not made by cp_plan_create_multi_track");
-  if (!P->loaded) return fail(CP_ERR_NOT_LOADED, "cp_infer_multi_track: call cp_plan_load_weights_model for every model first");
-  if (batch <= 0 || batch > P->B) return fail(CP_ERR_INVALID, "cp_infer_multi_track: batch exceeds the plan's max_batch");
+  if (int rc = check_run(P, given, batch, "cp_infer_multi_track", kLoadEveryModel)) return rc;
   if (int rc = check_model_prms(P, prms, "cp_infer_multi_track")) return rc;
   return infer_models(P, batch, images, pre_img, pre_hm, pre_hm_hp, prms, meta, heads_out, dets, poses, n_valid, stream);
 }
