@@ -58,10 +58,11 @@ EXPORTS = [
     "cp_plan_create_multi", "cp_plan_load_weights_model", "cp_plan_num_models", "cp_plan_op_desc_model", "cp_infer_multi",
     "cp_plan_create_multi_track", "cp_infer_multi_track", "cp_tracker_create_multi",
     "cp_plan_create_ex", "cp_plan_memory", "cp_plan_allocations", "cp_preprocess_yuv420",
+    "cp_preprocess_slots_dev", "cp_tracker_reset_dev", "cp_tracker_render_dev",
 ]
 
 # cp_pixel_format; "bgr" is the interleaved uint8 [H,W,3] input of every other pre-process entry point
-CP_PIX_NV12, CP_PIX_I420 = 0, 1
+CP_PIX_NV12, CP_PIX_I420, CP_PIX_BGR = 0, 1, 2
 PIXEL_FORMATS = ("bgr", "nv12", "i420")
 
 # cp_plan_create_ex / cp_plan_memory flags
@@ -205,6 +206,8 @@ def load():
     L.cp_preprocess_yuv420.argtypes = [vp, i64, ctypes.POINTER(i64), ctypes.POINTER(i32), i32, vp, i32, i32, i32,
                                        ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_float),
                                        ctypes.POINTER(ctypes.c_float), vp]
+    L.cp_preprocess_slots_dev.argtypes = [vp, i32, i32, i32, i32, i32, i32, ctypes.POINTER(ctypes.c_double),
+                                          ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_float), vp, vp, vp, vp]
     L.cp_tracker_create.argtypes = [ctypes.POINTER(CpTrackerConfig), ctypes.POINTER(vp)]
     L.cp_tracker_destroy.argtypes = [vp]
     L.cp_tracker_reset.argtypes = [vp, i32, vp]
@@ -215,6 +218,8 @@ def load():
     L.cp_tracker_step_ex.argtypes = [vp, i32, ctypes.POINTER(i32), vp, vp, i32, vp, vp, vp, vp]
     L.cp_tracker_render_ex2.argtypes = [vp, i32, ctypes.POINTER(i32), vp, vp, i32, i32, ctypes.POINTER(i32), vp, vp, vp]
     L.cp_tracker_seed_ex.argtypes = [vp, i32, ctypes.POINTER(i32), vp, vp, i32, vp]
+    L.cp_tracker_reset_dev.argtypes = [vp, i32, vp, vp]
+    L.cp_tracker_render_dev.argtypes = [vp, i32, vp, vp, i32, i32, vp, vp, vp, vp]
     L.cp_plan_create_multi.argtypes = [ctypes.POINTER(CpConfig), i32, ctypes.POINTER(vp)]
     L.cp_plan_load_weights_model.argtypes = [vp, i32, ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(vp),
                                              ctypes.POINTER(i64), i32, vp]

@@ -5,7 +5,8 @@
 //   cp_preprocess     -- batched uint8 HWC frames -> normalised fp32 NCHW network input
 //                        (reference: detectors/base_detector.py:91-148, fix_res branch); cp_preprocess_ragged does
 //                        the same for frames of different sizes in one launch, and cp_preprocess_yuv420 for NV12 / I420
-//                        frames (the colour conversion of cv2.cvtColor fused into the warp's tap fetch).
+//                        frames (the colour conversion of cv2.cvtColor fused into the warp's tap fetch);
+//                        cp_preprocess_slots_dev is the graph-safe form for one tracking step of a uniform batch.
 #include <vector>
 
 #include "common.cuh"
@@ -30,10 +31,12 @@ struct WarpM {
 // one output pixel (x, y) of a [sh, sw] frame under the inverted matrix W, all three channels.  The source pixels come
 // from `px`: px.taps(iy, ix, in-frame flags) sees the 2 x 2 taps (iy, ix) .. (iy + 1, ix + 1) once, then px(k, yy, xx, c)
 // is channel c (B, G, R) of in-frame tap k = 2 (yy - iy) + (xx - ix) as an integer 0..255.  Taps outside the frame are
-// the border value 0 and are never fetched.
-template <class Fetch>
+// the border value 0 and are never fetched.  kTwin: the same values also go to `twin` when it is not null (a tracking
+// slot's previous-frame input at the start of its video); without it the walk compiles as it always has.
+template <class Fetch, bool kTwin = false>
 __device__ __forceinline__ void warp_walk(Fetch px, float* __restrict__ out, size_t plane, int sh, int sw, int x,
-                                          int y, const WarpM& W, const float* mean, const float* stdv) {
+                                          int y, const WarpM& W, const float* mean, const float* stdv,
+                                          float* __restrict__ twin = nullptr) {
   // unfused double arithmetic (the host code OpenCV runs here has no FMA contraction)
   const int X0 = __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(W.m[1], (double)y), W.m[2]), 1024.0)) + 16;
   const int Y0 = __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(W.m[4], (double)y), W.m[5]), 1024.0)) + 16;
@@ -63,6 +66,7 @@ __device__ __forceinline__ void warp_walk(Fetch px, float* __restrict__ out, siz
     u8 = max(0, min(255, u8));
     const double r = ((double)u8 / 255.0 - (double)mean[c]) / (double)stdv[c];
     out[c * plane] = (float)r;
+    if (kTwin && twin) twin[c * plane] = (float)r;
   }
 }
 
@@ -180,6 +184,34 @@ __global__ void preprocess_yuv420_kernel(const uint8_t* __restrict__ frames, con
     const RaggedFrame f = fr[n];
     warp_walk(Yuv420Fetch<kFormat>{frames + f.offset, f.sh, f.sw}, out + (((size_t)n * 3) * dh + y) * dw + x,
               (size_t)dh * dw, f.sh, f.sw, x, y, f.W, mean, stdv);
+  }
+}
+
+// The frames of one tracking step: B slots of one size, format (cp_pixel_format) and affine, frame n at byte n * bytes.
+// Every parameter is a kernel argument or device memory, so a captured launch replays unchanged.  A slot whose start[n]
+// is set begins a video with this frame, which is then also its previous frame: the walk writes it to prev[n] as well.
+template <int kFormat>
+__global__ void preprocess_slots_kernel(const uint8_t* __restrict__ frames, float* __restrict__ out,
+                                        float* __restrict__ prev, const int* __restrict__ start, int B, int sh, int sw,
+                                        int dh, int dw, const WarpM W, float m0, float m1, float m2, float s0, float s1,
+                                        float s2) {
+  const size_t total = (size_t)B * dh * dw, plane = (size_t)dh * dw;
+  const size_t bytes = kFormat == CP_PIX_BGR ? (size_t)sh * sw * 3 : (size_t)sh * sw * 3 / 2;
+  const float mean[3] = {m0, m1, m2};
+  const float stdv[3] = {s0, s1, s2};
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int x = (int)(i % dw);
+    const size_t t = i / dw;
+    const int y = (int)(t % dh);
+    const int n = (int)(t / dh);
+    const size_t o = (((size_t)n * 3) * dh + y) * dw + x;
+    float* twin = start && start[n] ? prev + o : nullptr;
+    const uint8_t* img = frames + n * bytes;
+    if constexpr (kFormat == CP_PIX_BGR)
+      warp_walk<BgrFetch, true>(BgrFetch{img, sw}, out + o, plane, sh, sw, x, y, W, mean, stdv, twin);
+    else
+      warp_walk<Yuv420Fetch<kFormat>, true>(Yuv420Fetch<kFormat>{img, sh, sw}, out + o, plane, sh, sw, x, y, W, mean,
+                                            stdv, twin);
   }
 }
 
@@ -478,6 +510,40 @@ int cp_preprocess_yuv420(const uint8_t* frames, int64_t frames_bytes, const int6
       preprocess_yuv420_kernel<CP_PIX_I420><<<blocks, 256, 0, s>>>(frames, dfr, out, B, dst_h, dst_w, mean[0], mean[1],
                                                                     mean[2], stdv[0], stdv[1], stdv[2]);
   });
+}
+
+int cp_preprocess_slots_dev(const uint8_t* frames, int32_t format, int32_t B, int32_t src_h, int32_t src_w,
+                            int32_t dst_h, int32_t dst_w, const double* trans_input, const float mean[3],
+                            const float stdv[3], const int32_t* start, float* out, float* prev, void* stream_) {
+  if (!frames || !out || !mean || !stdv) return fail(CP_ERR_INVALID, "cp_preprocess_slots_dev: null argument");
+  if (!start != !prev) return fail(CP_ERR_INVALID, "cp_preprocess_slots_dev: start and prev go together");
+  if (format != CP_PIX_BGR && format != CP_PIX_NV12 && format != CP_PIX_I420)
+    return fail(CP_ERR_INVALID, "cp_preprocess_slots_dev: unknown pixel format " + std::to_string(format));
+  if (B <= 0 || src_h <= 0 || src_w <= 0 || dst_h <= 0 || dst_w <= 0)
+    return fail(CP_ERR_INVALID, "cp_preprocess_slots_dev: bad shape");
+  if (format != CP_PIX_BGR && (src_h % 2 || src_w % 2))
+    return fail(CP_ERR_INVALID, "cp_preprocess_slots_dev: YUV 4:2:0 frames need an even size, got " +
+                                    std::to_string(src_h) + " x " + std::to_string(src_w));
+  double T[6];
+  if (trans_input)
+    for (int i = 0; i < 6; ++i) T[i] = trans_input[i];
+  else
+    fix_res_affine(src_h, src_w, dst_h, dst_w, T);
+  const WarpM W = invert_affine(T);
+  const int blocks = preprocess_blocks((size_t)B * dst_h * dst_w);
+  cudaStream_t s = (cudaStream_t)stream_;
+  auto launch = [&](auto kernel) {
+    kernel<<<blocks, 256, 0, s>>>(frames, out, prev, start, B, src_h, src_w, dst_h, dst_w, W, mean[0], mean[1], mean[2],
+                                  stdv[0], stdv[1], stdv[2]);
+  };
+  if (format == CP_PIX_BGR)
+    launch(preprocess_slots_kernel<CP_PIX_BGR>);
+  else if (format == CP_PIX_NV12)
+    launch(preprocess_slots_kernel<CP_PIX_NV12>);
+  else
+    launch(preprocess_slots_kernel<CP_PIX_I420>);
+  CP_LAUNCH_CHECK("preprocess_slots_kernel");
+  return CP_OK;
 }
 
 }  // extern "C"

@@ -319,9 +319,11 @@ __global__ void __launch_bounds__(TRK_THREADS, 1) tracker_step_kernel(const Step
   }
 }
 
-__global__ void tracker_reset_kernel(int* n0, int* n1, int* id_count, int streams, int index) {
+// streams i < n: all of them (index < 0) or stream `index`; with `flags` (device [n]) the streams whose flag is set
+__global__ void tracker_reset_kernel(int* n0, int* n1, int* id_count, int streams, int index,
+                                     const int* flags = nullptr) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < streams && (index < 0 || i == index)) {
+  if (i < streams && (flags ? flags[i] != 0 : (index < 0 || i == index))) {
     n0[i] = 0;
     n1[i] = 0;
     id_count[i] = 0;
@@ -632,6 +634,18 @@ int cp_tracker_reset(cp_tracker* t, int32_t index, void* stream) {
   return CP_OK;
 }
 
+int cp_tracker_reset_dev(cp_tracker* t, int32_t batch, const int32_t* flags, void* stream) {
+  if (batch <= 0) return fail(CP_ERR_INVALID, "cp_tracker_reset_dev: batch must be > 0");
+  if (!t || !flags) return fail(CP_ERR_INVALID, "cp_tracker_reset_dev: null argument");
+  if (batch > t->cfg.streams)
+    return fail(CP_ERR_INVALID, "cp_tracker_reset_dev: batch " + std::to_string(batch) + " exceeds the tracker's " +
+                                    std::to_string(t->cfg.streams) + " streams");
+  tracker_reset_kernel<<<(batch + 127) / 128, 128, 0, (cudaStream_t)stream>>>(t->n_tracks[0], t->n_tracks[1],
+                                                                             t->id_count, batch, -1, flags);
+  CP_LAUNCH_CHECK("tracker_reset_kernel");
+  return CP_OK;
+}
+
 }  // extern "C"
 
 namespace {
@@ -659,6 +673,45 @@ int upload_stream_ids(cp_tracker* t, int32_t batch, const int32_t* ids, cudaStre
   if (!ids) return CP_OK;
   CP_CUDA_CHECK(cudaMemcpyAsync(t->ids, ids, sizeof(int32_t) * batch, cudaMemcpyHostToDevice, s));
   *dev = t->ids;
+  return CP_OK;
+}
+
+int check_render(const cp_tracker* t, int32_t batch, const double* meta, const double* trans_input, int32_t inp_h,
+                 int32_t inp_w, const float* pre_hm, const float* pre_hm_hp) {
+  if (!t || !meta || !trans_input || !pre_hm || !pre_hm_hp) return fail(CP_ERR_INVALID, "cp_tracker_render: null argument");
+  if (batch <= 0 || batch > t->cfg.streams || inp_h <= 0 || inp_w <= 0) return fail(CP_ERR_INVALID, "cp_tracker_render: bad shape");
+  return CP_OK;
+}
+
+// the render of a checked call; ids and modes (device [batch] or nullptr) are read by the kernel
+int launch_render(cp_tracker* t, int32_t batch, const int* ids, const double* meta, const double* trans_input, int32_t inp_h,
+                  int32_t inp_w, const int* modes, float* pre_hm, float* pre_hm_hp, cudaStream_t s) {
+  const size_t plane = (size_t)inp_h * inp_w;
+  RenderArgs a;
+  a.ids = ids;
+  CP_CUDA_CHECK(cudaMemsetAsync(pre_hm, 0, sizeof(float) * plane * batch, s));
+  CP_CUDA_CHECK(cudaMemsetAsync(pre_hm_hp, 0, sizeof(float) * plane * 8 * batch, s));
+  a.cfg = make_cfg(t->cfg);
+  a.cat = t->cat;
+  a.T = t->cfg.max_tracks;
+  a.inp_h = inp_h;
+  a.inp_w = inp_w;
+  a.render_hm_mode = t->cfg.render_hm_mode;
+  a.render_hmhp_mode = t->cfg.render_hmhp_mode;
+  a.pre_thresh = (double)t->cfg.pre_thresh;
+  a.slots0 = t->slots[0];
+  a.slots1 = t->slots[1];
+  a.n0 = t->n_tracks[0];
+  a.n1 = t->n_tracks[1];
+  a.cur = t->cur;
+  a.meta = meta;
+  a.trans = trans_input;
+  a.pre_hm = pre_hm;
+  a.pre_hm_hp = pre_hm_hp;
+  a.modes = modes;
+  dim3 grid(t->cfg.max_tracks, batch);
+  tracker_render_kernel<<<grid, 256, 0, s>>>(a);
+  CP_LAUNCH_CHECK("tracker_render_kernel");
   return CP_OK;
 }
 
@@ -727,37 +780,18 @@ int cp_tracker_render_ex2(cp_tracker* t, int32_t batch, const int32_t* stream_id
     any_mode = any_mode || modes[b] != CP_RENDER_TRACKS;
   }
   if (int rc = check_stream_ids(t, batch, stream_ids, "cp_tracker_render")) return rc;
-  if (!t || !meta || !trans_input || !pre_hm || !pre_hm_hp) return fail(CP_ERR_INVALID, "cp_tracker_render: null argument");
-  if (batch <= 0 || batch > t->cfg.streams || inp_h <= 0 || inp_w <= 0) return fail(CP_ERR_INVALID, "cp_tracker_render: bad shape");
+  if (int rc = check_render(t, batch, meta, trans_input, inp_h, inp_w, pre_hm, pre_hm_hp)) return rc;
   cudaStream_t s = (cudaStream_t)stream;
-  const size_t plane = (size_t)inp_h * inp_w;
-  RenderArgs a;
-  if (int rc = upload_stream_ids(t, batch, stream_ids, s, &a.ids)) return rc;
-  CP_CUDA_CHECK(cudaMemsetAsync(pre_hm, 0, sizeof(float) * plane * batch, s));
-  CP_CUDA_CHECK(cudaMemsetAsync(pre_hm_hp, 0, sizeof(float) * plane * 8 * batch, s));
+  const int* ids = nullptr;
+  if (int rc = upload_stream_ids(t, batch, stream_ids, s, &ids)) return rc;
   if (any_mode) CP_CUDA_CHECK(cudaMemcpyAsync(t->modes, modes, sizeof(int32_t) * batch, cudaMemcpyHostToDevice, s));
-  a.cfg = make_cfg(t->cfg);
-  a.cat = t->cat;
-  a.T = t->cfg.max_tracks;
-  a.inp_h = inp_h;
-  a.inp_w = inp_w;
-  a.render_hm_mode = t->cfg.render_hm_mode;
-  a.render_hmhp_mode = t->cfg.render_hmhp_mode;
-  a.pre_thresh = (double)t->cfg.pre_thresh;
-  a.slots0 = t->slots[0];
-  a.slots1 = t->slots[1];
-  a.n0 = t->n_tracks[0];
-  a.n1 = t->n_tracks[1];
-  a.cur = t->cur;
-  a.meta = meta;
-  a.trans = trans_input;
-  a.pre_hm = pre_hm;
-  a.pre_hm_hp = pre_hm_hp;
-  a.modes = any_mode ? t->modes : nullptr;
-  dim3 grid(t->cfg.max_tracks, batch);
-  tracker_render_kernel<<<grid, 256, 0, s>>>(a);
-  CP_LAUNCH_CHECK("tracker_render_kernel");
-  return CP_OK;
+  return launch_render(t, batch, ids, meta, trans_input, inp_h, inp_w, any_mode ? t->modes : nullptr, pre_hm, pre_hm_hp, s);
+}
+
+int cp_tracker_render_dev(cp_tracker* t, int32_t batch, const double* meta, const double* trans_input, int32_t inp_h,
+                          int32_t inp_w, const int32_t* modes, float* pre_hm, float* pre_hm_hp, void* stream) {
+  if (int rc = check_render(t, batch, meta, trans_input, inp_h, inp_w, pre_hm, pre_hm_hp)) return rc;
+  return launch_render(t, batch, nullptr, meta, trans_input, inp_h, inp_w, modes, pre_hm, pre_hm_hp, (cudaStream_t)stream);
 }
 
 int cp_tracker_seed(cp_tracker* t, int32_t batch, const float* seeds, const int32_t* n_seeds, int32_t S, void* stream) {

@@ -344,3 +344,141 @@ class Tracker(object):
         _lib.check(rc, "cp_tracker_render_ex")
         out[0]._cp_keep = (meta, tr)
         return out
+
+
+class TrackGraph(object):
+    """The array form of ObjectPoseDetector.run_batch(track=True) replayed from CUDA graphs: `slots` video slots of one
+    frame size (frame_hw = (H, W)), pixel format and camera each, every slot stepping on every call.  A step is the
+    pre-process, the reset of the slots whose video starts, the previous-frame render, the network + decode + PnP and the
+    tracker step, captured once; a call is one copy of the frames, one copy of the start flags and one graph launch, and
+    the host does not wait for the device.  Every step's (tracks [S,T,320], n_tracks [S]) are bit for bit those of
+    run_batch(track=True) on a fresh detector fed the same frames (with new_video as run_batch(list) takes it).
+
+    The previous network input needs no copy: the step alternates between two input buffers, and the graph of odd steps
+    is that of even steps with the two swapped.  A slot that starts a video (on the first call, after reset(), or with
+    new_video[i]) has its network input written to the previous-frame buffer too, by the pre-process itself.
+
+    det: an ObjectPoseDetector of a tracking opt (opt.tracking_task).  The graph holds its own copy of the plan and the
+    model's weights (taken now), its own tracker and buffers: building it leaves det._slots untouched, and det.run_batch
+    (track=True) and this graph may be called in any order, each keeping its own slot state.  Greedy or opt.hungarian
+    association, opt.empty_pre_hm and the heat maps drawn from the tracks follow opt as in run_batch.  Refused (ValueError
+    or NotImplementedError; they stay on run_batch): several categories, test_scales other than [1], the ground-truth
+    heat maps (opt.gt_pre_hm_hmhp / gt_pre_hm_hmhp_first), pre_dets seeding, idle slots and mixed frame sizes.
+
+    camera_matrix: [3,3] for every slot or [S,3,3].  pixel_format "bgr": frames are uint8 [S,H,W,3]; "nv12" / "i420":
+    uint8 [S,3H/2,W] (H, W even).  Frames may be on the host (pinned memory keeps the copy asynchronous; the caller must
+    not overwrite them until the step's outputs are read) or on the device."""
+
+    def __init__(self, det, slots, frame_hw, camera_matrix, pixel_format="bgr"):
+        from .detector import ObjectPoseDetector, affine_from_center_scale, camera_per_frame
+        from .engine import Engine, check_pixel_format, decode_params, frame_shape, make_meta
+        if not isinstance(det, ObjectPoseDetector) or det._track_categories() is not None:
+            raise NotImplementedError("TrackGraph tracks one category; several run through MultiCategoryTracker.run_batch")
+        opt = det.opt
+        if not getattr(opt, "tracking_task", False):
+            raise ValueError("TrackGraph needs a tracking model (opt.tracking_task)")
+        if [float(v) for v in getattr(opt, "test_scales", [1.0])] != [1.0]:
+            raise NotImplementedError("TrackGraph runs at test_scales=[1]; multi-scale tracking runs through run()")
+        if getattr(opt, "gt_pre_hm_hmhp", False) or getattr(opt, "gt_pre_hm_hmhp_first", False):
+            raise NotImplementedError("TrackGraph draws the previous-frame heat maps from the tracks; the ground-truth "
+                                      "heat maps (opt.gt_pre_hm_hmhp / gt_pre_hm_hmhp_first) run through run_batch")
+        S = int(slots)
+        if S < 1:
+            raise ValueError("TrackGraph: slots must be >= 1, got %d" % S)
+        if len(frame_hw) != 2 or int(frame_hw[0]) < 1 or int(frame_hw[1]) < 1:
+            raise ValueError("TrackGraph: frame_hw is one (H, W) for every slot, got %r" % (frame_hw,))
+        H, W = self.frame_hw = int(frame_hw[0]), int(frame_hw[1])
+        self.pixel_format = check_pixel_format(pixel_format)
+        self.frame_shape = (S,) + frame_shape(H, W, pixel_format)
+        cams = np.stack(camera_per_frame(camera_matrix, S))
+        self.L = L = _lib.load()
+        self.slots, self.device = S, torch.device("cuda", torch.cuda.current_device())
+        dev, m = self.device, det.model
+        ih, iw = opt.input_h, opt.input_w
+        self.eng = Engine(m._arch(), m.heads, m.head_conv, S, ih, iw, dev.index, tracking=m.tracking_inputs,
+                          tracking_task_gru=m.use_convGRU and m.tracking_task, precision=m.precision,
+                          reuse_activations=True)
+        self.eng.load_state_dict(m.state_dict())
+        self.prm = decode_params(opt, test_scale=1.0)
+        self.tracker = Tracker(opt, streams=S, device=dev)
+        # the per-slot rows run_batch's array form builds for this frame size (its fix_res c, s and affine)
+        c, s = np.array([W / 2., H / 2.], np.float32), float(max(H, W))
+        self.meta = make_meta(S, c, s, W, H, cams).to(dev)
+        trans = affine_from_center_scale(c, s, iw, ih).reshape(1, 6)
+        self.trans = torch.from_numpy(np.tile(trans, (S, 1))).to(dev)
+        mode = _lib.RENDER_EMPTY if getattr(opt, "empty_pre_hm", False) else _lib.RENDER_TRACKS
+        self.modes = torch.full((S,), mode, dtype=torch.int32, device=dev)
+        self._mean = (ctypes.c_float * 3)(*[float(v) for v in opt.mean])
+        self._std = (ctypes.c_float * 3)(*[float(v) for v in opt.std])
+        self.frames = torch.zeros(self.frame_shape, dtype=torch.uint8, device=dev)
+        self.start = torch.ones((S,), dtype=torch.int32, device=dev)
+        self.x = [torch.zeros((S, 3, ih, iw), dtype=torch.float32, device=dev) for _ in range(2)]
+        self.pre_hm = torch.zeros((S, 1, ih, iw), dtype=torch.float32, device=dev)
+        self.pre_hm_hp = torch.zeros((S, 8, ih, iw), dtype=torch.float32, device=dev)
+        self.poses = torch.zeros((S, self.prm.K, _lib.CP_POSE_RECORD), dtype=torch.float32, device=dev)
+        self.n_valid = torch.zeros((S,), dtype=torch.int32, device=dev)
+        self.tracks = torch.zeros((S, self.tracker.max_tracks, _lib.CP_TRACK_RECORD), dtype=torch.float32, device=dev)
+        self.n_tracks = torch.zeros((S,), dtype=torch.int32, device=dev)
+        side = torch.cuda.Stream(device=dev)
+        side.wait_stream(torch.cuda.current_stream(dev))
+        with torch.cuda.stream(side):            # warm-up outside the capture; the first call resets every slot
+            for p in (0, 1):
+                self._step(p)
+        torch.cuda.current_stream(dev).wait_stream(side)
+        torch.cuda.synchronize(dev)
+        self.graphs = []
+        for p in (0, 1):
+            g = torch.cuda.CUDAGraph(keep_graph=True)
+            with torch.cuda.graph(g):
+                self._step(p)
+            g.instantiate()
+            self.graphs.append(g)
+        self._parity = 0
+        self._fresh = True
+
+    def _step(self, p):
+        """The launches of one step: network input in x[p], previous frames in x[1 - p]."""
+        L, st, h = self.L, _stream(), self.tracker._h
+        S, (H, W), (ih, iw), cur, prev = self.slots, self.frame_hw, self.x[p].shape[2:], self.x[p], self.x[1 - p]
+        fmt = {"bgr": _lib.CP_PIX_BGR, "nv12": _lib.CP_PIX_NV12, "i420": _lib.CP_PIX_I420}[self.pixel_format]
+        with torch.cuda.device(self.device):
+            _lib.check(L.cp_tracker_reset_dev(h, S, _ptr(self.start), st), "cp_tracker_reset_dev")
+            _lib.check(L.cp_preprocess_slots_dev(_ptr(self.frames), fmt, S, H, W, ih, iw, None, self._mean, self._std,
+                                                 _ptr(self.start), _ptr(cur), _ptr(prev), st), "cp_preprocess_slots_dev")
+            _lib.check(L.cp_tracker_render_dev(h, S, _ptr(self.meta), _ptr(self.trans), ih, iw, _ptr(self.modes),
+                                               _ptr(self.pre_hm), _ptr(self.pre_hm_hp), st), "cp_tracker_render_dev")
+            self.eng.infer(cur, self.meta, self.prm, prev, self.pre_hm, self.pre_hm_hp, poses=self.poses,
+                           n_valid=self.n_valid)
+            _lib.check(L.cp_tracker_step(h, S, _ptr(self.poses), _ptr(self.n_valid), self.prm.K, _ptr(self.meta),
+                                         _ptr(self.tracks), _ptr(self.n_tracks), st), "cp_tracker_step")
+
+    def reset(self):
+        """Forget every slot's tracks and previous frame: the next call starts a video in every slot."""
+        self._fresh = True
+
+    def __call__(self, frames, new_video=None, pre_dets=None):
+        """The next frame of every slot -> (tracks [S,T,320], n_tracks [S]): views of the graph's own buffers,
+        overwritten by the next call.  new_video: None or one bool per slot (slot i starts a new video with this frame)."""
+        if pre_dets is not None:
+            raise NotImplementedError("TrackGraph does not seed tracks; pre_dets seeding runs through run_batch(track=True)")
+        if isinstance(frames, np.ndarray):
+            frames = torch.from_numpy(frames)
+        if not torch.is_tensor(frames) or frames.dtype != torch.uint8 or tuple(frames.shape) != self.frame_shape:
+            what = ("%s %s" % (frames.dtype, tuple(frames.shape))) if torch.is_tensor(frames) else type(frames).__name__
+            raise ValueError("TrackGraph steps every slot at one frame size: frames must be uint8 %s (%s), got %s; idle "
+                             "slots and mixed sizes run through run_batch(list, track=True)"
+                             % (list(self.frame_shape), self.pixel_format, what))
+        start = np.full(self.slots, int(self._fresh), np.int32)
+        if new_video is not None:
+            new_video = [bool(v) for v in new_video]
+            if len(new_video) != self.slots:
+                raise ValueError("TrackGraph: %d new_video entries for %d slots" % (len(new_video), self.slots))
+            start |= np.array(new_video, np.int32)
+        with torch.cuda.device(self.device):
+            self.frames.copy_(frames, non_blocking=True)
+            # a pageable source: staged before copy_ returns, without waiting for the device
+            self.start.copy_(torch.from_numpy(start), non_blocking=True)
+            self.graphs[self._parity].replay()
+        self._parity ^= 1
+        self._fresh = False
+        return self.tracks, self.n_tracks

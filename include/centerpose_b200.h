@@ -502,6 +502,21 @@ int cp_tracker_render_ex2(cp_tracker* trk, int32_t batch, const int32_t* stream_
                           const double* trans_input, int32_t inp_h, int32_t inp_w, const int32_t* modes, float* pre_hm,
                           float* pre_hm_hp, void* stream);
 
+/* Graph-safe forms: every per-step input is in device memory and read when the kernels run, nothing is allocated and
+ * no host memory is read after the call returns, so a CUDA graph that captured the call replays it as issued.  Bad
+ * arguments return CP_ERR_INVALID before any work is enqueued; a failure inside a capture (a cudaErrorStreamCapture*
+ * status) returns CP_ERR_CUDA with its text in cp_last_error.  cp_tracker_step (greedy or Hungarian) is graph-safe as
+ * it is.
+ *
+ * cp_tracker_reset_dev: flags is a DEVICE int32 [batch] (batch in 1..streams); every stream b with flags[b] != 0 is
+ * reset exactly as cp_tracker_reset(trk, b) does (tracks, ids, ages, filters and scale pool forgotten). */
+int cp_tracker_reset_dev(cp_tracker* trk, int32_t batch, const int32_t* flags, void* stream);
+/* cp_tracker_render_ex without a stream map and with `modes` a DEVICE int32 [batch] of cp_render_mode values (or NULL
+ * for all CP_RENDER_TRACKS); the kernel reads them, so they are not checked: a value other than CP_RENDER_GT or
+ * CP_RENDER_EMPTY draws the tracks. */
+int cp_tracker_render_dev(cp_tracker* trk, int32_t batch, const double* meta, const double* trans_input, int32_t inp_h,
+                          int32_t inp_w, const int32_t* modes, float* pre_hm, float* pre_hm_hp, void* stream);
+
 /* Offsets (in floats) inside one CP_SEED_RECORD: one dict of meta['pre_dets'] (eval_video_official.py:422-450). */
 #define CP_SEED_RECORD 264
 enum cp_seed_field {
@@ -607,7 +622,8 @@ int cp_preprocess_ragged(const uint8_t* frames, int64_t frames_bytes, const int6
  *   CP_PIX_I420: the U plane [H/2, W/2], then the V plane [H/2, W/2] (ffmpeg's yuv420p). */
 enum cp_pixel_format {
   CP_PIX_NV12 = 0,
-  CP_PIX_I420 = 1
+  CP_PIX_I420 = 1,
+  CP_PIX_BGR = 2   /* interleaved uint8 [H, W, 3]; taken by cp_preprocess_slots_dev (cp_preprocess_yuv420 refuses it) */
 };
 /* cp_preprocess_ragged on YUV 4:2:0 frames: frame b is [src_hw[b][0] * 3 / 2, src_hw[b][1]] uint8 in `format`, i.e.
  * src_hw[b][0] * src_hw[b][1] * 3 / 2 bytes starting `offsets[b]` bytes into `frames`; src_hw holds the IMAGE sizes
@@ -620,6 +636,19 @@ enum cp_pixel_format {
 int cp_preprocess_yuv420(const uint8_t* frames, int64_t frames_bytes, const int64_t* offsets, const int32_t* src_hw,
                          int32_t format, float* out, int32_t B, int32_t dst_h, int32_t dst_w, const double* trans_input,
                          const float mean[3], const float std[3], void* stream);
+
+/* The pre-process of one tracking step of B video slots, safe to capture in a CUDA graph: it reads no host memory and
+ * allocates nothing once enqueued, so a replay runs it with the arguments it was captured with.  frames: device uint8,
+ * B frames of one image size (src_h, src_w) in `format` (cp_pixel_format; YUV 4:2:0 needs an even size), frame b at byte
+ * b * (bytes of one frame).  trans_input: HOST row-major 2x3 forward affine for every frame, read before the call
+ * returns (NULL: the fix_res affine of the size, as cp_preprocess).  out: device fp32 [B,3,dst_h,dst_w], frame b bit for
+ * bit what cp_preprocess_affine (BGR) or cp_preprocess_yuv420 (NV12 / I420) gives for it.  start: device int32 [B] read
+ * when the kernel runs, or NULL; where start[b] != 0 frame b's output is written to prev[b] (device fp32
+ * [B,3,dst_h,dst_w]) as well: a slot whose video starts with this frame takes it as its previous frame.  start and prev
+ * are both given or both NULL.  Bad arguments return CP_ERR_INVALID before any work is enqueued. */
+int cp_preprocess_slots_dev(const uint8_t* frames, int32_t format, int32_t B, int32_t src_h, int32_t src_w,
+                            int32_t dst_h, int32_t dst_w, const double* trans_input, const float mean[3],
+                            const float std[3], const int32_t* start, float* out, float* prev, void* stream);
 
 /* ---- misc ------------------------------------------------------------------ */
 int cp_version(void);
