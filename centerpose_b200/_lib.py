@@ -59,6 +59,7 @@ EXPORTS = [
     "cp_plan_create_multi_track", "cp_infer_multi_track", "cp_tracker_create_multi",
     "cp_plan_create_ex", "cp_plan_memory", "cp_plan_allocations", "cp_preprocess_yuv420",
     "cp_preprocess_slots_dev", "cp_tracker_reset_dev", "cp_tracker_render_dev",
+    "cp_preprocess_frame_table_bytes", "cp_preprocess_frame_table", "cp_preprocess_slots_ragged_dev",
 ]
 
 # cp_pixel_format; "bgr" is the interleaved uint8 [H,W,3] input of every other pre-process entry point
@@ -208,6 +209,12 @@ def load():
                                        ctypes.POINTER(ctypes.c_float), vp]
     L.cp_preprocess_slots_dev.argtypes = [vp, i32, i32, i32, i32, i32, i32, ctypes.POINTER(ctypes.c_double),
                                           ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_float), vp, vp, vp, vp]
+    L.cp_preprocess_frame_table_bytes.argtypes = [i32]
+    L.cp_preprocess_frame_table_bytes.restype = i64
+    L.cp_preprocess_frame_table.argtypes = [i64, ctypes.POINTER(i64), ctypes.POINTER(i32), i32, i32, i32, i32,
+                                            ctypes.POINTER(ctypes.c_double), vp, vp]
+    L.cp_preprocess_slots_ragged_dev.argtypes = [vp, vp, i32, i32, i32, i32, ctypes.POINTER(ctypes.c_float),
+                                                 ctypes.POINTER(ctypes.c_float), vp, vp, vp, vp]
     L.cp_tracker_create.argtypes = [ctypes.POINTER(CpTrackerConfig), ctypes.POINTER(vp)]
     L.cp_tracker_destroy.argtypes = [vp]
     L.cp_tracker_reset.argtypes = [vp, i32, vp]
@@ -237,7 +244,7 @@ def load():
     for name in EXPORTS:
         fn = getattr(L, name)
         if name not in ("cp_version", "cp_last_error", "cp_plan_bytes", "cp_plan_forward_launches",
-                        "cp_decode_workspace_bytes"):
+                        "cp_decode_workspace_bytes", "cp_preprocess_frame_table_bytes"):
             fn.restype = ctypes.c_int
     _lib = L
     return L

@@ -6,7 +6,8 @@
 //                        (reference: detectors/base_detector.py:91-148, fix_res branch); cp_preprocess_ragged does
 //                        the same for frames of different sizes in one launch, and cp_preprocess_yuv420 for NV12 / I420
 //                        frames (the colour conversion of cv2.cvtColor fused into the warp's tap fetch);
-//                        cp_preprocess_slots_dev is the graph-safe form for one tracking step of a uniform batch.
+//                        cp_preprocess_slots_dev is the graph-safe form for one tracking step of a uniform batch, and
+//                        cp_preprocess_slots_ragged_dev (over a cp_preprocess_frame_table) that of slots of mixed sizes.
 #include <vector>
 
 #include "common.cuh"
@@ -212,6 +213,34 @@ __global__ void preprocess_slots_kernel(const uint8_t* __restrict__ frames, floa
     else
       warp_walk<Yuv420Fetch<kFormat>, true>(Yuv420Fetch<kFormat>{img, sh, sw}, out + o, plane, sh, sw, x, y, W, mean,
                                             stdv, twin);
+  }
+}
+
+// The frames of one tracking step when the slots differ in size: the ragged walk of preprocess_ragged_kernel /
+// preprocess_yuv420_kernel over a frame table `fr` in device memory (built once, cp_preprocess_frame_table), with the
+// start-flag twin write of preprocess_slots_kernel.  Nothing is read from the host, so a captured launch replays unchanged.
+template <int kFormat>
+__global__ void preprocess_slots_ragged_kernel(const uint8_t* __restrict__ frames, const RaggedFrame* __restrict__ fr,
+                                               float* __restrict__ out, float* __restrict__ prev,
+                                               const int* __restrict__ start, int B, int dh, int dw, float m0, float m1,
+                                               float m2, float s0, float s1, float s2) {
+  const size_t total = (size_t)B * dh * dw, plane = (size_t)dh * dw;
+  const float mean[3] = {m0, m1, m2};
+  const float stdv[3] = {s0, s1, s2};
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int x = (int)(i % dw);
+    const size_t t = i / dw;
+    const int y = (int)(t % dh);
+    const int n = (int)(t / dh);
+    const size_t o = (((size_t)n * 3) * dh + y) * dw + x;
+    float* twin = start && start[n] ? prev + o : nullptr;
+    const RaggedFrame f = fr[n];
+    if constexpr (kFormat == CP_PIX_BGR)
+      warp_walk<BgrFetch, true>(BgrFetch{frames + f.offset, f.sw}, out + o, plane, f.sh, f.sw, x, y, f.W, mean, stdv,
+                                twin);
+    else
+      warp_walk<Yuv420Fetch<kFormat>, true>(Yuv420Fetch<kFormat>{frames + f.offset, f.sh, f.sw}, out + o, plane, f.sh,
+                                            f.sw, x, y, f.W, mean, stdv, twin);
   }
 }
 
@@ -543,6 +572,58 @@ int cp_preprocess_slots_dev(const uint8_t* frames, int32_t format, int32_t B, in
   else
     launch(preprocess_slots_kernel<CP_PIX_I420>);
   CP_LAUNCH_CHECK("preprocess_slots_kernel");
+  return CP_OK;
+}
+
+int64_t cp_preprocess_frame_table_bytes(int32_t B) {
+  if (B <= 0) return fail(CP_ERR_INVALID, "cp_preprocess_frame_table_bytes: B must be > 0, got " + std::to_string(B));
+  return (int64_t)sizeof(RaggedFrame) * B;
+}
+
+int cp_preprocess_frame_table(int64_t frames_bytes, const int64_t* offsets, const int32_t* src_hw, int32_t format,
+                              int32_t B, int32_t dst_h, int32_t dst_w, const double* trans_input, void* table,
+                              void* stream_) {
+  if (!offsets || !src_hw || !table) return fail(CP_ERR_INVALID, "cp_preprocess_frame_table: null argument");
+  if (B <= 0 || dst_h <= 0 || dst_w <= 0 || frames_bytes <= 0)
+    return fail(CP_ERR_INVALID, "cp_preprocess_frame_table: bad shape");
+  if (format != CP_PIX_BGR && format != CP_PIX_NV12 && format != CP_PIX_I420)
+    return fail(CP_ERR_INVALID, "cp_preprocess_frame_table: unknown pixel format " + std::to_string(format));
+  std::vector<RaggedFrame> fr;
+  int rc = ragged_frames("cp_preprocess_frame_table", frames_bytes, offsets, src_hw, B, dst_h, dst_w, trans_input,
+                         format != CP_PIX_BGR, fr);
+  if (rc) return rc;
+  // a build-time call: the copy is complete when it returns, so `fr` may go out of scope
+  cudaStream_t s = (cudaStream_t)stream_;
+  cudaError_t e = cudaMemcpyAsync(table, fr.data(), sizeof(RaggedFrame) * B, cudaMemcpyHostToDevice, s);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+  if (e != cudaSuccess)
+    return fail(CP_ERR_CUDA, std::string("cp_preprocess_frame_table: table upload: ") + cudaGetErrorString(e));
+  return CP_OK;
+}
+
+int cp_preprocess_slots_ragged_dev(const uint8_t* frames, const void* table, int32_t format, int32_t B, int32_t dst_h,
+                                   int32_t dst_w, const float mean[3], const float stdv[3], const int32_t* start,
+                                   float* out, float* prev, void* stream_) {
+  if (!frames || !table || !out || !mean || !stdv)
+    return fail(CP_ERR_INVALID, "cp_preprocess_slots_ragged_dev: null argument");
+  if (!start != !prev) return fail(CP_ERR_INVALID, "cp_preprocess_slots_ragged_dev: start and prev go together");
+  if (format != CP_PIX_BGR && format != CP_PIX_NV12 && format != CP_PIX_I420)
+    return fail(CP_ERR_INVALID, "cp_preprocess_slots_ragged_dev: unknown pixel format " + std::to_string(format));
+  if (B <= 0 || dst_h <= 0 || dst_w <= 0) return fail(CP_ERR_INVALID, "cp_preprocess_slots_ragged_dev: bad shape");
+  const RaggedFrame* fr = (const RaggedFrame*)table;
+  const int blocks = preprocess_blocks((size_t)B * dst_h * dst_w);
+  cudaStream_t s = (cudaStream_t)stream_;
+  auto launch = [&](auto kernel) {
+    kernel<<<blocks, 256, 0, s>>>(frames, fr, out, prev, start, B, dst_h, dst_w, mean[0], mean[1], mean[2], stdv[0],
+                                  stdv[1], stdv[2]);
+  };
+  if (format == CP_PIX_BGR)
+    launch(preprocess_slots_ragged_kernel<CP_PIX_BGR>);
+  else if (format == CP_PIX_NV12)
+    launch(preprocess_slots_ragged_kernel<CP_PIX_NV12>);
+  else
+    launch(preprocess_slots_ragged_kernel<CP_PIX_I420>);
+  CP_LAUNCH_CHECK("preprocess_slots_ragged_kernel");
   return CP_OK;
 }
 

@@ -346,13 +346,28 @@ class Tracker(object):
         return out
 
 
+def _frame_sizes(frame_hw, S, who):
+    """frame_hw of a graph of S slots -> ([(H, W)], per_slot): one size for every slot, or one per slot."""
+    per_slot = (isinstance(frame_hw, (list, tuple, np.ndarray)) and len(frame_hw) > 0
+                and all(isinstance(v, (list, tuple, np.ndarray)) for v in frame_hw))
+    if per_slot and len(frame_hw) != S:
+        raise ValueError("%s: frame_hw is one (H, W) for every slot or one per slot, got %d for %d slots"
+                         % (who, len(frame_hw), S))
+    sizes = []
+    for hw in (frame_hw if per_slot else [frame_hw]):
+        if len(hw) != 2 or int(hw[0]) < 1 or int(hw[1]) < 1:
+            raise ValueError("%s: frame_hw is one (H, W) for every slot or one per slot, got %r" % (who, frame_hw))
+        sizes.append((int(hw[0]), int(hw[1])))
+    return sizes, per_slot
+
+
 class TrackGraph(object):
-    """The array form of ObjectPoseDetector.run_batch(track=True) replayed from CUDA graphs: `slots` video slots of one
-    frame size (frame_hw = (H, W)), pixel format and camera each, every slot stepping on every call.  A step is the
-    pre-process, the reset of the slots whose video starts, the previous-frame render, the network + decode + PnP and the
-    tracker step, captured once; a call is one copy of the frames, one copy of the start flags and one graph launch, and
-    the host does not wait for the device.  Every step's (tracks [S,T,320], n_tracks [S]) are bit for bit those of
-    run_batch(track=True) on a fresh detector fed the same frames (with new_video as run_batch(list) takes it).
+    """The array form of ObjectPoseDetector.run_batch(track=True) replayed from CUDA graphs: `slots` video slots with a
+    pixel format and a camera each, every slot stepping on every call.  A step is the pre-process, the reset of the slots
+    whose video starts, the previous-frame render, the network + decode + PnP and the tracker step, captured once; a call
+    is one copy per frame buffer, one copy of the start flags and one graph launch, and the host does not wait for the
+    device.  Every step's (tracks [S,T,320], n_tracks [S]) are bit for bit those of run_batch(track=True) on a fresh
+    detector fed the same frames (with new_video as run_batch(list) takes it).
 
     The previous network input needs no copy: the step alternates between two input buffers, and the graph of odd steps
     is that of even steps with the two swapped.  A slot that starts a video (on the first call, after reset(), or with
@@ -362,63 +377,109 @@ class TrackGraph(object):
     model's weights (taken now), its own tracker and buffers: building it leaves det._slots untouched, and det.run_batch
     (track=True) and this graph may be called in any order, each keeping its own slot state.  Greedy or opt.hungarian
     association, opt.empty_pre_hm and the heat maps drawn from the tracks follow opt as in run_batch.  Refused (ValueError
-    or NotImplementedError; they stay on run_batch): several categories, test_scales other than [1], the ground-truth
-    heat maps (opt.gt_pre_hm_hmhp / gt_pre_hm_hmhp_first), pre_dets seeding, idle slots and mixed frame sizes.
+    or NotImplementedError; they stay on run_batch): test_scales other than [1], the ground-truth heat maps
+    (opt.gt_pre_hm_hmhp / gt_pre_hm_hmhp_first), pre_dets seeding and idle slots.  Several categories go through
+    MultiCategoryTrackGraph.
 
-    camera_matrix: [3,3] for every slot or [S,3,3].  pixel_format "bgr": frames are uint8 [S,H,W,3]; "nv12" / "i420":
-    uint8 [S,3H/2,W] (H, W even).  Frames may be on the host (pinned memory keeps the copy asynchronous; the caller must
-    not overwrite them until the step's outputs are read) or on the device."""
+    frame_hw: one (H, W) for every slot, or a list of S (H_s, W_s).  camera_matrix: [3,3] for every slot or [S,3,3].
+      - One size: a call takes the frames as one array, uint8 [S,H,W,3] for pixel_format "bgr", [S,3H/2,W] for "nv12" /
+        "i420" (H, W even); one copy and the uniform pre-process (cp_preprocess_slots_dev).
+      - One size per slot: a call takes a list of S frames, uint8 [H_s,W_s,3] or [3H_s/2,W_s], each copied into its own
+        region of one packed device buffer; the step is that of run_batch(list, track=True) with every slot present, the
+        pre-process reading a frame table built once now (cp_preprocess_slots_ragged_dev).
+    Frames may be on the host (pinned memory keeps the copy asynchronous; the caller must not overwrite them until the
+    step's outputs are read) or on the device."""
+
+    _host_step = "run_batch(track=True)"              # where what the graph refuses runs
+    _host_list = "run_batch(list, track=True)"
 
     def __init__(self, det, slots, frame_hw, camera_matrix, pixel_format="bgr"):
-        from .detector import ObjectPoseDetector, affine_from_center_scale, camera_per_frame
-        from .engine import Engine, check_pixel_format, decode_params, frame_shape, make_meta
+        from .detector import ObjectPoseDetector
         if not isinstance(det, ObjectPoseDetector) or det._track_categories() is not None:
-            raise NotImplementedError("TrackGraph tracks one category; several run through MultiCategoryTracker.run_batch")
-        opt = det.opt
+            raise NotImplementedError("TrackGraph tracks one category; several run through MultiCategoryTracker.run_batch "
+                                      "or a MultiCategoryTrackGraph")
+        self._build(det, slots, frame_hw, camera_matrix, pixel_format)
+
+    def _plan(self, det, S, ih, iw):
+        """(plan, decode parameters, tracker, categories or None) of the graph: a copy of det's plan and weights."""
+        from .engine import Engine, decode_params
+        m = det.model
+        eng = Engine(m._arch(), m.heads, m.head_conv, S, ih, iw, self.device.index, tracking=m.tracking_inputs,
+                     tracking_task_gru=m.use_convGRU and m.tracking_task, precision=m.precision, reuse_activations=True)
+        eng.load_state_dict(m.state_dict())
+        return eng, decode_params(det.opt, test_scale=1.0), Tracker(det.opt, streams=S, device=self.device), None
+
+    def _build(self, det, slots, frame_hw, camera_matrix, pixel_format):
+        """Checks, buffers and the two captured steps; everything that refuses comes before any device work."""
+        from .detector import affine_from_center_scale, camera_per_frame
+        from .engine import check_pixel_format, frame_shape, make_meta
+        who, opt = type(self).__name__, det.opt
         if not getattr(opt, "tracking_task", False):
-            raise ValueError("TrackGraph needs a tracking model (opt.tracking_task)")
+            raise ValueError("%s needs a tracking model (opt.tracking_task)" % who)
         if [float(v) for v in getattr(opt, "test_scales", [1.0])] != [1.0]:
-            raise NotImplementedError("TrackGraph runs at test_scales=[1]; multi-scale tracking runs through run()")
+            raise NotImplementedError("%s runs at test_scales=[1]; multi-scale tracking runs through run()" % who)
         if getattr(opt, "gt_pre_hm_hmhp", False) or getattr(opt, "gt_pre_hm_hmhp_first", False):
-            raise NotImplementedError("TrackGraph draws the previous-frame heat maps from the tracks; the ground-truth "
-                                      "heat maps (opt.gt_pre_hm_hmhp / gt_pre_hm_hmhp_first) run through run_batch")
+            raise NotImplementedError("%s draws the previous-frame heat maps from the tracks; the ground-truth heat maps "
+                                      "(opt.gt_pre_hm_hmhp / gt_pre_hm_hmhp_first) run through %s" % (who, self._host_step))
         S = int(slots)
         if S < 1:
-            raise ValueError("TrackGraph: slots must be >= 1, got %d" % S)
-        if len(frame_hw) != 2 or int(frame_hw[0]) < 1 or int(frame_hw[1]) < 1:
-            raise ValueError("TrackGraph: frame_hw is one (H, W) for every slot, got %r" % (frame_hw,))
-        H, W = self.frame_hw = int(frame_hw[0]), int(frame_hw[1])
+            raise ValueError("%s: slots must be >= 1, got %d" % (who, S))
+        sizes, self.per_slot = _frame_sizes(frame_hw, S, who)
         self.pixel_format = check_pixel_format(pixel_format)
-        self.frame_shape = (S,) + frame_shape(H, W, pixel_format)
+        shapes = [frame_shape(h, w, pixel_format) for h, w in sizes]
         cams = np.stack(camera_per_frame(camera_matrix, S))
+        if self.per_slot:
+            self.frame_hw, self.frame_shape = sizes, shapes
+        else:
+            self.frame_hw, self.frame_shape = sizes[0], (S,) + shapes[0]
+            sizes = sizes * S
         self.L = L = _lib.load()
         self.slots, self.device = S, torch.device("cuda", torch.cuda.current_device())
-        dev, m = self.device, det.model
+        dev = self.device
         ih, iw = opt.input_h, opt.input_w
-        self.eng = Engine(m._arch(), m.heads, m.head_conv, S, ih, iw, dev.index, tracking=m.tracking_inputs,
-                          tracking_task_gru=m.use_convGRU and m.tracking_task, precision=m.precision,
-                          reuse_activations=True)
-        self.eng.load_state_dict(m.state_dict())
-        self.prm = decode_params(opt, test_scale=1.0)
-        self.tracker = Tracker(opt, streams=S, device=dev)
-        # the per-slot rows run_batch's array form builds for this frame size (its fix_res c, s and affine)
-        c, s = np.array([W / 2., H / 2.], np.float32), float(max(H, W))
-        self.meta = make_meta(S, c, s, W, H, cams).to(dev)
-        trans = affine_from_center_scale(c, s, iw, ih).reshape(1, 6)
-        self.trans = torch.from_numpy(np.tile(trans, (S, 1))).to(dev)
+        self.eng, self.prm, self.tracker, self.categories = self._plan(det, S, ih, iw)
+        M = 1 if self.categories is None else len(self.categories)
+        MS = self.streams = M * S                        # tracker stream m * S + s: slot s of category m
+        # every slot's row of run_batch: its fix_res c, s and meta row and the affine of its size, repeated per category
+        meta, trans = np.zeros((S, _lib.CP_META_DOUBLES), np.float64), np.zeros((S, 6), np.float64)
+        for b, (h, w) in enumerate(sizes):
+            c, sc = np.array([w / 2., h / 2.], np.float32), float(max(h, w))
+            meta[b] = make_meta(1, c, sc, w, h, cams[b]).numpy()[0]
+            trans[b] = affine_from_center_scale(c, sc, iw, ih).reshape(6)
+        self.meta = torch.from_numpy(meta).to(dev)                   # the network's rows, one per frame
+        self.meta_all = self.meta if M == 1 else torch.from_numpy(np.tile(meta, (M, 1))).to(dev)
+        self.trans = torch.from_numpy(np.tile(trans, (M, 1))).to(dev)
         mode = _lib.RENDER_EMPTY if getattr(opt, "empty_pre_hm", False) else _lib.RENDER_TRACKS
-        self.modes = torch.full((S,), mode, dtype=torch.int32, device=dev)
+        self.modes = torch.full((MS,), mode, dtype=torch.int32, device=dev)
         self._mean = (ctypes.c_float * 3)(*[float(v) for v in opt.mean])
         self._std = (ctypes.c_float * 3)(*[float(v) for v in opt.std])
-        self.frames = torch.zeros(self.frame_shape, dtype=torch.uint8, device=dev)
-        self.start = torch.ones((S,), dtype=torch.int32, device=dev)
+        self._fmt = {"bgr": _lib.CP_PIX_BGR, "nv12": _lib.CP_PIX_NV12, "i420": _lib.CP_PIX_I420}[self.pixel_format]
+        if self.per_slot:
+            n = [int(np.prod(s)) for s in shapes]
+            offs = np.concatenate([[0], np.cumsum(n)[:-1]]).astype(np.int64)
+            self.frames = torch.zeros((int(sum(n)),), dtype=torch.uint8, device=dev)
+            self._slot_frames = [self.frames[o:o + k].view(s) for o, k, s in zip(offs, n, shapes)]
+            self.table = torch.zeros((int(L.cp_preprocess_frame_table_bytes(S)),), dtype=torch.uint8, device=dev)
+            hw = np.ascontiguousarray(sizes, np.int32)
+            with torch.cuda.device(dev):
+                _lib.check(L.cp_preprocess_frame_table(self.frames.numel(), offs.ctypes.data_as(ctypes.POINTER(ctypes.c_int64)),
+                                                       hw.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), self._fmt, S, ih,
+                                                       iw, trans.ctypes.data_as(ctypes.POINTER(ctypes.c_double)),
+                                                       _ptr(self.table), _stream()), "cp_preprocess_frame_table")
+        else:
+            self.frames = torch.zeros(self.frame_shape, dtype=torch.uint8, device=dev)
+        self.start = torch.ones((MS,), dtype=torch.int32, device=dev)
         self.x = [torch.zeros((S, 3, ih, iw), dtype=torch.float32, device=dev) for _ in range(2)]
-        self.pre_hm = torch.zeros((S, 1, ih, iw), dtype=torch.float32, device=dev)
-        self.pre_hm_hp = torch.zeros((S, 8, ih, iw), dtype=torch.float32, device=dev)
-        self.poses = torch.zeros((S, self.prm.K, _lib.CP_POSE_RECORD), dtype=torch.float32, device=dev)
-        self.n_valid = torch.zeros((S,), dtype=torch.int32, device=dev)
-        self.tracks = torch.zeros((S, self.tracker.max_tracks, _lib.CP_TRACK_RECORD), dtype=torch.float32, device=dev)
-        self.n_tracks = torch.zeros((S,), dtype=torch.int32, device=dev)
+        lead = self.eng._lead(S)                         # the plan's per-model axes: (S,) or (M, S)
+        self.pre_hm = torch.zeros(lead + (1, ih, iw), dtype=torch.float32, device=dev)
+        self.pre_hm_hp = torch.zeros(lead + (8, ih, iw), dtype=torch.float32, device=dev)
+        K = (self.prm[0] if isinstance(self.prm, list) else self.prm).K
+        self.poses = torch.zeros(lead + (K, _lib.CP_POSE_RECORD), dtype=torch.float32, device=dev)
+        self.n_valid = torch.zeros(lead, dtype=torch.int32, device=dev)
+        self.tracks = torch.zeros((MS, self.tracker.max_tracks, _lib.CP_TRACK_RECORD), dtype=torch.float32, device=dev)
+        self.n_tracks = torch.zeros((MS,), dtype=torch.int32, device=dev)
+        out_lead = (S,) if self.categories is None else (M, S)
+        self._out = (self.tracks.view(out_lead + self.tracks.shape[1:]), self.n_tracks.view(out_lead))
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(side):            # warm-up outside the capture; the first call resets every slot
@@ -439,46 +500,119 @@ class TrackGraph(object):
     def _step(self, p):
         """The launches of one step: network input in x[p], previous frames in x[1 - p]."""
         L, st, h = self.L, _stream(), self.tracker._h
-        S, (H, W), (ih, iw), cur, prev = self.slots, self.frame_hw, self.x[p].shape[2:], self.x[p], self.x[1 - p]
-        fmt = {"bgr": _lib.CP_PIX_BGR, "nv12": _lib.CP_PIX_NV12, "i420": _lib.CP_PIX_I420}[self.pixel_format]
+        S, MS, (ih, iw), cur, prev = self.slots, self.streams, self.x[p].shape[2:], self.x[p], self.x[1 - p]
         with torch.cuda.device(self.device):
-            _lib.check(L.cp_tracker_reset_dev(h, S, _ptr(self.start), st), "cp_tracker_reset_dev")
-            _lib.check(L.cp_preprocess_slots_dev(_ptr(self.frames), fmt, S, H, W, ih, iw, None, self._mean, self._std,
-                                                 _ptr(self.start), _ptr(cur), _ptr(prev), st), "cp_preprocess_slots_dev")
-            _lib.check(L.cp_tracker_render_dev(h, S, _ptr(self.meta), _ptr(self.trans), ih, iw, _ptr(self.modes),
+            _lib.check(L.cp_tracker_reset_dev(h, MS, _ptr(self.start), st), "cp_tracker_reset_dev")
+            if self.per_slot:
+                _lib.check(L.cp_preprocess_slots_ragged_dev(_ptr(self.frames), _ptr(self.table), self._fmt, S, ih, iw,
+                                                            self._mean, self._std, _ptr(self.start), _ptr(cur),
+                                                            _ptr(prev), st), "cp_preprocess_slots_ragged_dev")
+            else:
+                H, W = self.frame_hw
+                _lib.check(L.cp_preprocess_slots_dev(_ptr(self.frames), self._fmt, S, H, W, ih, iw, None, self._mean,
+                                                     self._std, _ptr(self.start), _ptr(cur), _ptr(prev), st),
+                           "cp_preprocess_slots_dev")
+            _lib.check(L.cp_tracker_render_dev(h, MS, _ptr(self.meta_all), _ptr(self.trans), ih, iw, _ptr(self.modes),
                                                _ptr(self.pre_hm), _ptr(self.pre_hm_hp), st), "cp_tracker_render_dev")
             self.eng.infer(cur, self.meta, self.prm, prev, self.pre_hm, self.pre_hm_hp, poses=self.poses,
                            n_valid=self.n_valid)
-            _lib.check(L.cp_tracker_step(h, S, _ptr(self.poses), _ptr(self.n_valid), self.prm.K, _ptr(self.meta),
-                                         _ptr(self.tracks), _ptr(self.n_tracks), st), "cp_tracker_step")
+            _lib.check(L.cp_tracker_step(h, MS, _ptr(self.poses), _ptr(self.n_valid), self.poses.shape[-2],
+                                         _ptr(self.meta_all), _ptr(self.tracks), _ptr(self.n_tracks), st), "cp_tracker_step")
 
     def reset(self):
         """Forget every slot's tracks and previous frame: the next call starts a video in every slot."""
         self._fresh = True
 
+    def _frames(self, frames):
+        """The frames of one call, checked against the slots' shapes: one tensor, or one per slot."""
+        who = type(self).__name__
+        if not self.per_slot:
+            if isinstance(frames, np.ndarray):
+                frames = torch.from_numpy(frames)
+            if not torch.is_tensor(frames) or frames.dtype != torch.uint8 or tuple(frames.shape) != self.frame_shape:
+                what = ("%s %s" % (frames.dtype, tuple(frames.shape))) if torch.is_tensor(frames) else type(frames).__name__
+                raise ValueError("%s steps every slot at one frame size: frames must be uint8 %s (%s), got %s; idle "
+                                 "slots and mixed sizes run through %s or a %s built with one frame_hw per slot"
+                                 % (who, list(self.frame_shape), self.pixel_format, what, self._host_list, who))
+            return [frames]
+        if not isinstance(frames, (list, tuple)) or len(frames) != self.slots:
+            what = "%d frames" % len(frames) if isinstance(frames, (list, tuple)) else type(frames).__name__
+            raise ValueError("%s was built with one frame_hw per slot: frames is a list of %d frames, got %s"
+                             % (who, self.slots, what))
+        out = []
+        for b, f in enumerate(frames):
+            if f is None:
+                raise ValueError("%s steps every slot: slot %d is idle; idle slots run through %s"
+                                 % (who, b, self._host_list))
+            if isinstance(f, np.ndarray):
+                f = torch.from_numpy(f)
+            if not torch.is_tensor(f) or f.dtype != torch.uint8 or tuple(f.shape) != self.frame_shape[b]:
+                what = ("%s %s" % (f.dtype, tuple(f.shape))) if torch.is_tensor(f) else type(f).__name__
+                raise ValueError("%s: slot %d takes uint8 %s frames (%s, frame_hw %s), got %s"
+                                 % (who, b, list(self.frame_shape[b]), self.pixel_format, self.frame_hw[b], what))
+            out.append(f)
+        return out
+
     def __call__(self, frames, new_video=None, pre_dets=None):
-        """The next frame of every slot -> (tracks [S,T,320], n_tracks [S]): views of the graph's own buffers,
-        overwritten by the next call.  new_video: None or one bool per slot (slot i starts a new video with this frame)."""
+        """The next frame of every slot -> (tracks [S,T,320], n_tracks [S]) ([M,S,...] in MultiCategoryTrackGraph):
+        views of the graph's own buffers, overwritten by the next call.  frames: one array (one frame_hw) or a list of
+        one frame per slot (one frame_hw per slot).  new_video: None or one bool per slot (slot i starts a new video
+        with this frame)."""
+        who = type(self).__name__
         if pre_dets is not None:
-            raise NotImplementedError("TrackGraph does not seed tracks; pre_dets seeding runs through run_batch(track=True)")
-        if isinstance(frames, np.ndarray):
-            frames = torch.from_numpy(frames)
-        if not torch.is_tensor(frames) or frames.dtype != torch.uint8 or tuple(frames.shape) != self.frame_shape:
-            what = ("%s %s" % (frames.dtype, tuple(frames.shape))) if torch.is_tensor(frames) else type(frames).__name__
-            raise ValueError("TrackGraph steps every slot at one frame size: frames must be uint8 %s (%s), got %s; idle "
-                             "slots and mixed sizes run through run_batch(list, track=True)"
-                             % (list(self.frame_shape), self.pixel_format, what))
+            raise NotImplementedError("%s does not seed tracks; pre_dets seeding runs through %s" % (who, self._host_step))
+        frames = self._frames(frames)
         start = np.full(self.slots, int(self._fresh), np.int32)
         if new_video is not None:
             new_video = [bool(v) for v in new_video]
             if len(new_video) != self.slots:
-                raise ValueError("TrackGraph: %d new_video entries for %d slots" % (len(new_video), self.slots))
+                raise ValueError("%s: %d new_video entries for %d slots" % (who, len(new_video), self.slots))
             start |= np.array(new_video, np.int32)
+        start = np.tile(start, self.streams // self.slots)       # one flag per tracker stream, the same in every category
         with torch.cuda.device(self.device):
-            self.frames.copy_(frames, non_blocking=True)
+            for dst, f in zip(self._slot_frames if self.per_slot else [self.frames], frames):
+                dst.copy_(f, non_blocking=True)
             # a pageable source: staged before copy_ returns, without waiting for the device
             self.start.copy_(torch.from_numpy(start), non_blocking=True)
             self.graphs[self._parity].replay()
         self._parity ^= 1
         self._fresh = False
-        return self.tracks, self.n_tracks
+        return self._out
+
+
+class MultiCategoryTrackGraph(TrackGraph):
+    """TrackGraph over a MultiCategoryTracker: its M categories track in the same `slots` video slots, and every step's
+    (tracks [M,S,T,320], n_tracks [M,S]), in trk.categories order, are bit for bit those of trk.run_batch on the same
+    frames (its array form with one frame_hw, its list form with every slot present with one frame_hw per slot).  The
+    step is TrackGraph's: one pre-process of the shared frames, the reset of the M x S tracker streams of the slots that
+    start a video, one render of every category's previous-frame heat maps, one multi-model network + decode call
+    (cp_infer_multi_track) and one tracker step over the M x S streams, each category with its own visible_thresh, balance
+    coefficient and opt.conf_border.
+
+    The graph owns its plan (every category's weights, copied from trk now), its tracker and buffers: trk._slots is left
+    untouched, and trk.run_batch and this graph may be called in any order.  Refused as in TrackGraph; several categories
+    of one graph need a MultiCategoryTracker (a MultiCategoryDetector is not a tracking model)."""
+
+    _host_step = "MultiCategoryTracker.run_batch"
+    _host_list = "MultiCategoryTracker.run_batch(list)"
+
+    def __init__(self, trk, slots, frame_hw, camera_matrix, pixel_format="bgr"):
+        from .detector import MultiCategoryDetector, MultiCategoryTracker
+        if not isinstance(trk, MultiCategoryTracker):
+            if isinstance(trk, MultiCategoryDetector):
+                raise ValueError("MultiCategoryTrackGraph needs a MultiCategoryTracker; a MultiCategoryDetector is not a "
+                                 "tracking model")
+            raise NotImplementedError("MultiCategoryTrackGraph takes a MultiCategoryTracker; one category's "
+                                      "ObjectPoseDetector goes to TrackGraph")
+        self._build(trk, slots, frame_hw, camera_matrix, pixel_format)
+
+    def _plan(self, trk, S, ih, iw):
+        from .engine import Engine
+        c, M = trk._plan_cfg, len(trk.categories)
+        eng = Engine(c["arch"], c["heads"], c["head_conv"], S, ih, iw, self.device.index, tracking=c["tracking"],
+                     tracking_task_gru=c["tracking_task_gru"], precision=c["precision"], models=M,
+                     reuse_activations=True)
+        for m, sd in enumerate(trk._weights):
+            eng.load_state_dict(sd, model=m)
+        prm = list(trk._prms) if M > 1 else trk._prms[0]
+        return eng, prm, Tracker(trk.opt, streams=S, device=self.device, categories=trk.categories), list(trk.categories)

@@ -623,7 +623,8 @@ int cp_preprocess_ragged(const uint8_t* frames, int64_t frames_bytes, const int6
 enum cp_pixel_format {
   CP_PIX_NV12 = 0,
   CP_PIX_I420 = 1,
-  CP_PIX_BGR = 2   /* interleaved uint8 [H, W, 3]; taken by cp_preprocess_slots_dev (cp_preprocess_yuv420 refuses it) */
+  CP_PIX_BGR = 2   /* interleaved uint8 [H, W, 3]; taken by cp_preprocess_slots_dev and cp_preprocess_slots_ragged_dev
+                    * (cp_preprocess_yuv420 refuses it) */
 };
 /* cp_preprocess_ragged on YUV 4:2:0 frames: frame b is [src_hw[b][0] * 3 / 2, src_hw[b][1]] uint8 in `format`, i.e.
  * src_hw[b][0] * src_hw[b][1] * 3 / 2 bytes starting `offsets[b]` bytes into `frames`; src_hw holds the IMAGE sizes
@@ -649,6 +650,31 @@ int cp_preprocess_yuv420(const uint8_t* frames, int64_t frames_bytes, const int6
 int cp_preprocess_slots_dev(const uint8_t* frames, int32_t format, int32_t B, int32_t src_h, int32_t src_w,
                             int32_t dst_h, int32_t dst_w, const double* trans_input, const float mean[3],
                             const float std[3], const int32_t* start, float* out, float* prev, void* stream);
+
+/* The pre-process of one tracking step of B video slots whose frames differ in size, safe to capture in a CUDA graph.
+ * It takes two calls:
+ *   - cp_preprocess_frame_table, once, when the graph is built: the per-frame parameters (byte offset, size and
+ *     inverted affine of every frame) are checked on the host and written to `table`, caller-owned DEVICE memory of
+ *     cp_preprocess_frame_table_bytes(B) bytes (8-byte aligned).  offsets (int64 [B]), src_hw (int32 [B,2], image sizes
+ *     (H, W)) and trans_input (double [B,6] row-major 2x3 forward affines, or NULL for each frame's fix_res affine) are
+ *     HOST arrays read before the call returns.  It runs the checks of cp_preprocess_ragged / cp_preprocess_yuv420: a
+ *     null pointer, B <= 0, a frame that does not fit inside frames_bytes, an odd size in a YUV 4:2:0 format or an
+ *     unknown format return CP_ERR_INVALID before any work.  The table is uploaded on `stream` and the call waits for
+ *     the copy, so it must not be called inside a capture.
+ *   - cp_preprocess_slots_ragged_dev, the captured call: frames (a device buffer of at least frames_bytes bytes, laid out
+ *     as the table says), the table and start are device memory read when the kernel runs, nothing is allocated and no
+ *     host memory is read after the call returns.  `format` must be the one the table was built for.  out: device fp32
+ *     [B,3,dst_h,dst_w], frame b bit for bit what cp_preprocess_ragged (CP_PIX_BGR) or cp_preprocess_yuv420 (NV12 /
+ *     I420) gives for it with the same offsets, sizes and affines.  start / prev as in cp_preprocess_slots_dev: where
+ *     start[b] != 0 frame b's output is written to prev[b] as well, other rows of prev are not touched; both given or
+ *     both NULL.  Bad arguments return CP_ERR_INVALID before any work is enqueued. */
+int64_t cp_preprocess_frame_table_bytes(int32_t B);
+int cp_preprocess_frame_table(int64_t frames_bytes, const int64_t* offsets, const int32_t* src_hw, int32_t format,
+                              int32_t B, int32_t dst_h, int32_t dst_w, const double* trans_input, void* table,
+                              void* stream);
+int cp_preprocess_slots_ragged_dev(const uint8_t* frames, const void* table, int32_t format, int32_t B, int32_t dst_h,
+                                   int32_t dst_w, const float mean[3], const float std[3], const int32_t* start,
+                                   float* out, float* prev, void* stream);
 
 /* ---- misc ------------------------------------------------------------------ */
 int cp_version(void);

@@ -75,12 +75,18 @@ def measure(S, fmt, steps, warmup, runs, prof_dir):
     tg = cpb.TrackGraph(det, slots=S, frame_hw=(H, W), camera_matrix=cam, pixel_format=fmt)
     arms = {"graph": lambda f: tg(f),
             "run_batch": lambda f: det.run_batch(f, cam, track=True, pixel_format=fmt, to_host=False)}
-    frames = video(S, fmt, warmup + steps)
+    return time_arms(arms, [tg.reset, det.reset_tracking], video(S, fmt, warmup + steps), warmup, runs,
+                     "S=%d %s" % (S, fmt), prof_dir and os.path.join(prof_dir, "track_graph_%%s_S%d_%s.json" % (S, fmt)))
+
+
+def time_arms(arms, resets, frames, warmup, runs, label, trace=None):
+    """Both arms over the same frames, alternating step by step, after calling every reset; their outputs are checked
+    identical at every step.  trace: a path pattern with one %s (the arm) for the profiler traces, or None."""
     res = {a: {"step_ms": [], "gpu_ms": []} for a in arms}
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     for _ in range(runs):
-        tg.reset()
-        det.reset_tracking()
+        for r in resets:
+            r()
         for k, f in enumerate(frames):
             outs = {}
             for a, fn in arms.items():
@@ -97,7 +103,7 @@ def measure(S, fmt, steps, warmup, runs, prof_dir):
                     res[a]["gpu_ms"].append(ev0.elapsed_time(ev1))
             g, r = outs["graph"], outs["run_batch"]
             if not (np.array_equal(g[0], r[0]) and np.array_equal(g[1], r[1])):
-                raise SystemExit("S=%d %s step %d: TrackGraph and run_batch disagree" % (S, fmt, k))
+                raise SystemExit("%s step %d: the graph and run_batch disagree" % (label, k))
     # kernel and copy sums per step, profiled in a run of their own
     from torch.autograd import DeviceType
     n_prof = 5
@@ -119,8 +125,8 @@ def measure(S, fmt, steps, warmup, runs, prof_dir):
             end = max(end, s1)
         res[a]["busy_ms"] = busy / 1e3 / n_prof
         res[a]["kernels_per_step"] = len(kern) / n_prof
-        if prof_dir:
-            prof.export_chrome_trace(os.path.join(prof_dir, "track_graph_%s_S%d_%s.json" % (a, S, fmt)))
+        if trace:
+            prof.export_chrome_trace(trace % a)
     for a in arms:
         for k in ("step_ms", "gpu_ms"):
             v = np.array(res[a][k])
