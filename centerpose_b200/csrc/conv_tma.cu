@@ -318,45 +318,67 @@ __global__ void __launch_bounds__(X3 ? TM_THREADS_X3 : TM_THREADS, 1) conv_tma_k
       const uint32_t row0 = (p.k == 3 ? (uint32_t)(g.g0 - 1 - g.r_lo * p.Wt) : 0u) + (uint32_t)c * 64u;
 #pragma unroll
       for (int j = 0; j < (X3 ? BN / 2 : 1); ++j) sums[j] = 0.f;
-      int kbi = 0, gk = 0;
-      for (int s = 0; s < sps; ++s) {
-        mbar_wait(bar_a + 8u * (uint32_t)sa, pa);
-        const uint32_t a_slab = slabs0 + (uint32_t)sa * a_stage;
-        for (int tap = 0; tap < taps; ++tap, ++kbi) {
+      // x3: the K blocks of an accumulation group chain on one accumulator, so each stays in flight until the next one of
+      // its group is queued behind it, and the group's last is waited for before the promotion; the wgmmas and their
+      // order are those of a wait after every K block.  With one slab stage the next slab's TMA needs the stage back at
+      // once, so there (and in tf32, where there is no group) every K block is waited for.
+      const int group = X3 ? p.group : 1;
+      const bool overlap = X3 && p.SA > 1;
+      int tap = 0;
+      // retire the K block before position (sb, sa, tap): its weight stage, and its slab stage when it was a slab's last tap
+      auto release_prev = [&]() {
+        if (wt == 0) {
+          mbar_arrive(bar_b_empty + 8u * (uint32_t)(sb == 0 ? p.SB - 1 : sb - 1));
+          if (tap == 0) mbar_arrive(bar_a_empty + 8u * (uint32_t)(sa == 0 ? p.SA - 1 : sa - 1));
+        }
+      };
+      for (int kb0 = 0; kb0 < KB; kb0 += group) {
+        const int n_kb = min(group, KB - kb0);
+        for (int i = 0; i < n_kb; ++i) {
+          if (tap == 0) mbar_wait(bar_a + 8u * (uint32_t)sa, pa);
           const int ky = tap / 3, kx = tap - ky * 3;
           const uint32_t arow = row0 + (p.k == 3 ? (uint32_t)(ky * p.Wt + kx) : 0u);
           mbar_wait(bar_b_full + 8u * (uint32_t)sb, pb);
-          const uint64_t da = make_desc(a_slab + arow * rowb, p.cslab);
+          const uint64_t da = make_desc(slabs0 + (uint32_t)sa * a_stage + arow * rowb, p.cslab);
           const uint64_t db = make_desc(btiles0 + (uint32_t)sb * btile_bytes, p.cslab);
-          const bool fresh = X3 ? gk == 0 : kbi == 0;
+          const bool fresh = X3 ? i == 0 : kb0 == 0;
           if (p.cslab == 32)
-            mma_kblock<BN, X3, false, 4>(acc, da, db, a_lo_u, b_lo_u, fresh);
+            mma_kblock_issue<BN, X3, false, 4>(acc, da, db, a_lo_u, b_lo_u, fresh);
           else
-            mma_kblock<BN, X3, false, 2>(acc, da, db, a_lo_u, b_lo_u, fresh);
-          if (wt == 0) {
-            mbar_arrive(bar_b_empty + 8u * (uint32_t)sb);
-            if (tap == taps - 1) mbar_arrive(bar_a_empty + 8u * (uint32_t)sa);
+            mma_kblock_issue<BN, X3, false, 2>(acc, da, db, a_lo_u, b_lo_u, fresh);
+          if (overlap && i > 0) {
+            wg_wait<1>();
+            release_prev();
           }
           if (++sb == p.SB) {
             sb = 0;
             pb ^= 1u;
           }
-          if (X3) {
-            // two-level accumulation: the tensor core sums `group` K blocks, every finished group is added into fp32
-            // registers with round-to-nearest
-            if (gk == p.group - 1 || kbi == KB - 1) {
-#pragma unroll
-              for (int j = 0; j < (X3 ? BN / 2 : 1); ++j) sums[j] += acc[X3 ? j : 0];
-              gk = 0;
-            } else {
-              ++gk;
+          if (++tap == taps) {
+            tap = 0;
+            if (++sa == p.SA) {
+              sa = 0;
+              pa ^= 1u;
             }
           }
+          if (!overlap) {
+            wg_wait<0>();
+            release_prev();
+          }
         }
-        if (++sa == p.SA) {
-          sa = 0;
-          pa ^= 1u;
-        }
+        wg_wait<0>();
+        if (overlap) release_prev();
+        // two-level accumulation: the tensor core sums `group` K blocks, every finished group is added into fp32
+        // registers with round-to-nearest
+#pragma unroll
+        for (int j = 0; j < (X3 ? BN / 2 : 1); ++j)
+          if (X3) sums[j] += acc[X3 ? j : 0];
+      }
+      // x3: the next tile's first wgmma overwrites the accumulator, so it is dead through the epilogue; saying so frees
+      // its registers there for the drain and the fused 1x1 (ptxas then spills less, DESIGN §4)
+      if (X3) {
+#pragma unroll
+        for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
       }
       // ---- epilogue: rows of this warpgroup, 32 columns at a time through shared memory (drain_rows)
       const int r_me = wt >> 1;
@@ -401,6 +423,72 @@ __global__ void __launch_bounds__(X3 ? TM_THREADS_X3 : TM_THREADS, 1) conv_tma_k
           epilogue_row<16>(ep, v, valid, m, n, oy, ox, g.n_tile * BN + cb, col_end);
         }
       };
+      if constexpr (X3 && FUSE) {
+        // x3 fused 1x1 (BN = 128): thread (rg, hh, og) accumulates rows rg + 16 i (i < 4) x outputs 4 og .. 4 og + 3 over
+        // hidden channels c0 + 16 hh .. + 15 of every 32-column chunk, in increasing order: each (row, output) sees the
+        // products and order of a thread per row and half, but a weight float4 feeds 16 FMAs instead of 4.  The chunk
+        // passes through the stage as relu(conv + bias), 64 rows x 32 columns, 16-byte groups XOR-swizzled by row & 7
+        // (conflict-free float4 reads).
+        const int rg = wt >> 3, hh = (wt >> 2) & 1, og = wt & 3;
+        const int fr0 = (wt >> 5) * 16 + ((wt & 31) >> 2), fcq = (wt & 3) * 2;     // accumulator fragment (drain_rows)
+        const float* b1 = p.bias + wofs + (size_t)g.n_tile * BN;
+        const float4* w2 = reinterpret_cast<const float4*>(p.fuse_w[head] + wofs) + (size_t)part * BN * 4 + og;
+        auto at = [&](int r, int col) { return r * 32 + ((((col >> 2) ^ r) & 7) << 2) + (col & 3); };
+#pragma unroll
+        for (int c0 = 0; c0 < BN; c0 += 32) {
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            if (j * 8 >= c0 && j * 8 < c0 + 32) {
+              const int col = j * 8 - c0 + fcq;
+              const float bx = __ldg(b1 + c0 + col), by = __ldg(b1 + c0 + col + 1);
+              dstage[at(fr0, col)] = fmaxf(sums[X3 ? 4 * j : 0] + bx, 0.f);
+              dstage[at(fr0, col + 1)] = fmaxf(sums[X3 ? 4 * j + 1 : 0] + by, 0.f);
+              dstage[at(fr0 + 8, col)] = fmaxf(sums[X3 ? 4 * j + 2 : 0] + bx, 0.f);
+              dstage[at(fr0 + 8, col + 1)] = fmaxf(sums[X3 ? 4 * j + 3 : 0] + by, 0.f);
+            }
+          }
+          wg_bar_sync(1 + c);
+#pragma unroll
+          for (int m4 = 0; m4 < 4; ++m4) {
+            const int k0 = 16 * hh + 4 * m4;          // hidden channels c0 + k0 .. + 3
+            float4 hv[4];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) hv[i] = *reinterpret_cast<const float4*>(dstage + at(rg + 16 * i, k0));
+#pragma unroll
+            for (int kk = 0; kk < 4; ++kk) {
+              const float4 w = __ldg(w2 + (size_t)(c0 + k0 + kk) * 4);
+#pragma unroll
+              for (int i = 0; i < 4; ++i) {
+                const float h = kk == 0 ? hv[i].x : kk == 1 ? hv[i].y : kk == 2 ? hv[i].z : hv[i].w;
+                acc2[FUSE ? 4 * i + 0 : 0] = fmaf(h, w.x, acc2[FUSE ? 4 * i + 0 : 0]);
+                acc2[FUSE ? 4 * i + 1 : 0] = fmaf(h, w.y, acc2[FUSE ? 4 * i + 1 : 0]);
+                acc2[FUSE ? 4 * i + 2 : 0] = fmaf(h, w.z, acc2[FUSE ? 4 * i + 2 : 0]);
+                acc2[FUSE ? 4 * i + 3 : 0] = fmaf(h, w.w, acc2[FUSE ? 4 * i + 3 : 0]);
+              }
+            }
+          }
+          wg_bar_sync(1 + c);
+        }
+        if (part == p.tph - 1) {
+          // the two hidden halves of a (row, output) are in lanes that differ in bit 2
+#pragma unroll
+          for (int j = 0; j < 16; ++j) acc2[FUSE ? j : 0] += __shfl_xor_sync(0xffffffffu, acc2[FUSE ? j : 0], 4);
+          if (hh == 0) {
+            const int co = p.fuse_cout[head];
+            const size_t plane = (size_t)p.H * p.W;
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+              int n1, oy1, ox1, m1;
+              if (!tile_position<MULTI>(p, g, c * 64 + rg + 16 * i, &n1, &oy1, &ox1, &m1)) continue;
+              float* o = p.fuse_out[head] + ((size_t)n1 * co * p.H + oy1) * p.W + ox1;
+#pragma unroll
+              for (int u = 0; u < 4; ++u)
+                if (4 * og + u < co) o[(4 * og + u) * plane] = acc2[FUSE ? 4 * i + u : 0] + __ldg(p.fuse_b[head] + wofs + 4 * og + u);
+            }
+          }
+        }
+        continue;
+      }
       if constexpr (X3)
         drain_rows<BN>(sums, dstage, wt, 1 + c, fn);
       else

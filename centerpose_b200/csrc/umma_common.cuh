@@ -172,11 +172,11 @@ template <> __device__ __forceinline__ void wgmma_tf32_rs<128>(float (&d)[64], c
 
 // One K block on the tensor cores: KS slices of 32 bytes (8 tf32 / 16 bf16 elements) of a 64-row A tile and a BN-row B
 // tile.  X3: 3-term split a_lo b_hi + a_hi b_lo + a_hi b_hi (lo tiles at a_lo / b_lo descriptor units past the hi tiles),
-// cross terms first.  fresh: the first product overwrites the accumulator.  Returns when the products are in `acc` and
-// the operand tiles may be reused.
+// cross terms first.  fresh: the first product overwrites the accumulator.  mma_kblock_issue commits the products as one
+// wgmma group and returns at once; mma_kblock returns when they are in `acc` and the operand tiles may be reused.
 template <int BN, bool X3, bool BF16, int KS>
-__device__ __forceinline__ void mma_kblock(float (&acc)[BN / 2], uint64_t da, uint64_t db, uint32_t a_lo, uint32_t b_lo,
-                                           bool fresh) {
+__device__ __forceinline__ void mma_kblock_issue(float (&acc)[BN / 2], uint64_t da, uint64_t db, uint32_t a_lo, uint32_t b_lo,
+                                                 bool fresh) {
   wg_fence();
 #pragma unroll
   for (int ks = 0; ks < KS; ++ks) {
@@ -195,6 +195,11 @@ __device__ __forceinline__ void mma_kblock(float (&acc)[BN / 2], uint64_t da, ui
     for (int ks = 0; ks < KS; ++ks) wgmma_tf32<BN>(acc, da + 2u * ks, db + 2u * ks, 1u);
   }
   wg_commit();
+}
+template <int BN, bool X3, bool BF16, int KS>
+__device__ __forceinline__ void mma_kblock(float (&acc)[BN / 2], uint64_t da, uint64_t db, uint32_t a_lo, uint32_t b_lo,
+                                           bool fresh) {
+  mma_kblock_issue<BN, X3, BF16, KS>(acc, da, db, a_lo, b_lo, fresh);
   wg_wait<0>();
 }
 
