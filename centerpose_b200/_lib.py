@@ -60,6 +60,7 @@ EXPORTS = [
     "cp_plan_create_ex", "cp_plan_memory", "cp_plan_allocations", "cp_preprocess_yuv420",
     "cp_preprocess_slots_dev", "cp_tracker_reset_dev", "cp_tracker_render_dev",
     "cp_preprocess_frame_table_bytes", "cp_preprocess_frame_table", "cp_preprocess_slots_ragged_dev",
+    "cp_preprocess_slots_rows_dev", "cp_gather_rows_dev", "cp_tracker_render_dev2", "cp_tracker_step_dev",
 ]
 
 # cp_pixel_format; "bgr" is the interleaved uint8 [H,W,3] input of every other pre-process entry point
@@ -215,6 +216,9 @@ def load():
                                             ctypes.POINTER(ctypes.c_double), vp, vp]
     L.cp_preprocess_slots_ragged_dev.argtypes = [vp, vp, i32, i32, i32, i32, ctypes.POINTER(ctypes.c_float),
                                                  ctypes.POINTER(ctypes.c_float), vp, vp, vp, vp]
+    L.cp_preprocess_slots_rows_dev.argtypes = [vp, vp, i32, vp, i32, i32, i32, ctypes.POINTER(ctypes.c_float),
+                                               ctypes.POINTER(ctypes.c_float), vp, vp, vp, vp, vp]
+    L.cp_gather_rows_dev.argtypes = [vp, vp, i64, i32, vp, vp]
     L.cp_tracker_create.argtypes = [ctypes.POINTER(CpTrackerConfig), ctypes.POINTER(vp)]
     L.cp_tracker_destroy.argtypes = [vp]
     L.cp_tracker_reset.argtypes = [vp, i32, vp]
@@ -227,6 +231,8 @@ def load():
     L.cp_tracker_seed_ex.argtypes = [vp, i32, ctypes.POINTER(i32), vp, vp, i32, vp]
     L.cp_tracker_reset_dev.argtypes = [vp, i32, vp, vp]
     L.cp_tracker_render_dev.argtypes = [vp, i32, vp, vp, i32, i32, vp, vp, vp, vp]
+    L.cp_tracker_render_dev2.argtypes = [vp, i32, vp, vp, vp, i32, i32, vp, vp, vp, vp]
+    L.cp_tracker_step_dev.argtypes = [vp, i32, vp, vp, vp, i32, vp, vp, vp, vp]
     L.cp_plan_create_multi.argtypes = [ctypes.POINTER(CpConfig), i32, ctypes.POINTER(vp)]
     L.cp_plan_load_weights_model.argtypes = [vp, i32, ctypes.POINTER(ctypes.c_char_p), ctypes.POINTER(vp),
                                              ctypes.POINTER(i64), i32, vp]

@@ -7,7 +7,9 @@
 //                        the same for frames of different sizes in one launch, and cp_preprocess_yuv420 for NV12 / I420
 //                        frames (the colour conversion of cv2.cvtColor fused into the warp's tap fetch);
 //                        cp_preprocess_slots_dev is the graph-safe form for one tracking step of a uniform batch, and
-//                        cp_preprocess_slots_ragged_dev (over a cp_preprocess_frame_table) that of slots of mixed sizes.
+//                        cp_preprocess_slots_ragged_dev (over a cp_preprocess_frame_table) that of slots of mixed sizes,
+//                        cp_preprocess_slots_rows_dev that of the live slots of a step with idle slots;
+//   cp_gather_rows_dev -- a row gather through a device map, the graph-safe reordering of per-slot rows.
 #include <vector>
 
 #include "common.cuh"
@@ -33,11 +35,14 @@ struct WarpM {
 // from `px`: px.taps(iy, ix, in-frame flags) sees the 2 x 2 taps (iy, ix) .. (iy + 1, ix + 1) once, then px(k, yy, xx, c)
 // is channel c (B, G, R) of in-frame tap k = 2 (yy - iy) + (xx - ix) as an integer 0..255.  Taps outside the frame are
 // the border value 0 and are never fetched.  kTwin: the same values also go to `twin` when it is not null (a tracking
-// slot's previous-frame input at the start of its video); without it the walk compiles as it always has.
-template <class Fetch, bool kTwin = false>
+// slot's previous-frame input at the start of its video).  kExchange: a slot's previous frame is kept in `store`; when
+// twin is not null, twin takes the value (`start`) or the stored one, and the value then replaces the stored one.  Each
+// thread reads and writes only its own elements.  Without either flag the walk compiles as it always has.
+template <class Fetch, bool kTwin = false, bool kExchange = false>
 __device__ __forceinline__ void warp_walk(Fetch px, float* __restrict__ out, size_t plane, int sh, int sw, int x,
                                           int y, const WarpM& W, const float* mean, const float* stdv,
-                                          float* __restrict__ twin = nullptr) {
+                                          float* __restrict__ twin = nullptr, float* __restrict__ store = nullptr,
+                                          bool start = false) {
   // unfused double arithmetic (the host code OpenCV runs here has no FMA contraction)
   const int X0 = __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(W.m[1], (double)y), W.m[2]), 1024.0)) + 16;
   const int Y0 = __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(W.m[4], (double)y), W.m[5]), 1024.0)) + 16;
@@ -67,7 +72,14 @@ __device__ __forceinline__ void warp_walk(Fetch px, float* __restrict__ out, siz
     u8 = max(0, min(255, u8));
     const double r = ((double)u8 / 255.0 - (double)mean[c]) / (double)stdv[c];
     out[c * plane] = (float)r;
-    if (kTwin && twin) twin[c * plane] = (float)r;
+    if constexpr (kExchange) {
+      if (twin) {
+        twin[c * plane] = start ? (float)r : store[c * plane];
+        store[c * plane] = (float)r;
+      }
+    } else if (kTwin && twin) {
+      twin[c * plane] = (float)r;
+    }
   }
 }
 
@@ -241,6 +253,50 @@ __global__ void preprocess_slots_ragged_kernel(const uint8_t* __restrict__ frame
     else
       warp_walk<Yuv420Fetch<kFormat>, true>(Yuv420Fetch<kFormat>{frames + f.offset, f.sh, f.sw}, out + o, plane, f.sh,
                                             f.sw, x, y, f.W, mean, stdv, twin);
+  }
+}
+
+// The frames of one tracking step when some slots are idle: row n of the B live rows is slot rows[n]'s frame, warped
+// through that slot's entry of the frame table into out[n].  With prev (and store), the slot's previous frame moves
+// through a per-slot store in the same walk: prev[n] = start[slot] ? value : store[slot], then store[slot] = value.  The
+// live rows name distinct slots, so no two threads touch the same store element.  rows and start are device memory
+// read when the kernel runs, so a captured launch replays whatever map the last copy left there.
+template <int kFormat>
+__global__ void preprocess_slots_rows_kernel(const uint8_t* __restrict__ frames, const RaggedFrame* __restrict__ fr,
+                                             const int* __restrict__ rows, const int* __restrict__ start,
+                                             float* __restrict__ store, float* __restrict__ out,
+                                             float* __restrict__ prev, int B, int dh, int dw, float m0, float m1,
+                                             float m2, float s0, float s1, float s2) {
+  const size_t total = (size_t)B * dh * dw, plane = (size_t)dh * dw;
+  const float mean[3] = {m0, m1, m2};
+  const float stdv[3] = {s0, s1, s2};
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int x = (int)(i % dw);
+    const size_t t = i / dw;
+    const int y = (int)(t % dh);
+    const int n = (int)(t / dh);
+    const int slot = rows[n];
+    const size_t px = (size_t)y * dw + x, o = (size_t)n * 3 * plane + px;
+    const bool st = start && start[slot];
+    float* twin = prev ? prev + o : nullptr;
+    float* keep = prev ? store + (size_t)slot * 3 * plane + px : nullptr;
+    const RaggedFrame f = fr[slot];
+    if constexpr (kFormat == CP_PIX_BGR)
+      warp_walk<BgrFetch, true, true>(BgrFetch{frames + f.offset, f.sw}, out + o, plane, f.sh, f.sw, x, y, f.W, mean,
+                                      stdv, twin, keep, st);
+    else
+      warp_walk<Yuv420Fetch<kFormat>, true, true>(Yuv420Fetch<kFormat>{frames + f.offset, f.sh, f.sw}, out + o, plane,
+                                                  f.sh, f.sw, x, y, f.W, mean, stdv, twin, keep, st);
+  }
+}
+
+// dst row i = src row map[i], or zeros where map[i] < 0; rows of `words` 32-bit words
+__global__ void gather_rows_kernel(const uint32_t* __restrict__ src, uint32_t* __restrict__ dst, size_t words, int n,
+                                  const int* __restrict__ map) {
+  const size_t total = (size_t)n * words;
+  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+    const int r = map[i / words];
+    dst[i] = r >= 0 ? src[(size_t)r * words + i % words] : 0u;
   }
 }
 
@@ -624,6 +680,44 @@ int cp_preprocess_slots_ragged_dev(const uint8_t* frames, const void* table, int
   else
     launch(preprocess_slots_ragged_kernel<CP_PIX_I420>);
   CP_LAUNCH_CHECK("preprocess_slots_ragged_kernel");
+  return CP_OK;
+}
+
+int cp_preprocess_slots_rows_dev(const uint8_t* frames, const void* table, int32_t format, const int32_t* rows, int32_t B,
+                                 int32_t dst_h, int32_t dst_w, const float mean[3], const float stdv[3],
+                                 const int32_t* start, float* store, float* out, float* prev, void* stream_) {
+  if (!frames || !table || !rows || !out || !mean || !stdv)
+    return fail(CP_ERR_INVALID, "cp_preprocess_slots_rows_dev: null argument");
+  if (!store != !prev) return fail(CP_ERR_INVALID, "cp_preprocess_slots_rows_dev: store and prev go together");
+  if (format != CP_PIX_BGR && format != CP_PIX_NV12 && format != CP_PIX_I420)
+    return fail(CP_ERR_INVALID, "cp_preprocess_slots_rows_dev: unknown pixel format " + std::to_string(format));
+  if (B <= 0 || dst_h <= 0 || dst_w <= 0) return fail(CP_ERR_INVALID, "cp_preprocess_slots_rows_dev: bad shape");
+  const RaggedFrame* fr = (const RaggedFrame*)table;
+  const int blocks = preprocess_blocks((size_t)B * dst_h * dst_w);
+  cudaStream_t s = (cudaStream_t)stream_;
+  auto launch = [&](auto kernel) {
+    kernel<<<blocks, 256, 0, s>>>(frames, fr, rows, start, store, out, prev, B, dst_h, dst_w, mean[0], mean[1], mean[2],
+                                  stdv[0], stdv[1], stdv[2]);
+  };
+  if (format == CP_PIX_BGR)
+    launch(preprocess_slots_rows_kernel<CP_PIX_BGR>);
+  else if (format == CP_PIX_NV12)
+    launch(preprocess_slots_rows_kernel<CP_PIX_NV12>);
+  else
+    launch(preprocess_slots_rows_kernel<CP_PIX_I420>);
+  CP_LAUNCH_CHECK("preprocess_slots_rows_kernel");
+  return CP_OK;
+}
+
+int cp_gather_rows_dev(const void* src, void* dst, int64_t row_bytes, int32_t n, const int32_t* map, void* stream_) {
+  if (!src || !dst || !map) return fail(CP_ERR_INVALID, "cp_gather_rows_dev: null argument");
+  if (n <= 0 || row_bytes <= 0 || row_bytes % 4)
+    return fail(CP_ERR_INVALID, "cp_gather_rows_dev: bad shape (n " + std::to_string(n) + ", row_bytes " +
+                                    std::to_string(row_bytes) + ": rows are a positive multiple of 4 bytes)");
+  const size_t words = (size_t)row_bytes / 4;
+  gather_rows_kernel<<<preprocess_blocks(words * n), 256, 0, (cudaStream_t)stream_>>>(
+      (const uint32_t*)src, (uint32_t*)dst, words, n, map);
+  CP_LAUNCH_CHECK("gather_rows_kernel");
   return CP_OK;
 }
 

@@ -715,24 +715,19 @@ int launch_render(cp_tracker* t, int32_t batch, const int* ids, const double* me
   return CP_OK;
 }
 
-}  // namespace
-
-extern "C" {
-
-int cp_tracker_step(cp_tracker* t, int32_t batch, const float* poses, const int32_t* n_valid, int32_t K, const double* meta,
-                    float* tracks_out, int32_t* n_tracks, void* stream) {
-  return cp_tracker_step_ex(t, batch, nullptr, poses, n_valid, K, meta, tracks_out, n_tracks, stream);
-}
-
-int cp_tracker_step_ex(cp_tracker* t, int32_t batch, const int32_t* stream_ids, const float* poses, const int32_t* n_valid,
-                       int32_t K, const double* meta, float* tracks_out, int32_t* n_tracks, void* stream) {
-  if (int rc = check_stream_ids(t, batch, stream_ids, "cp_tracker_step")) return rc;
+int check_step(const cp_tracker* t, int32_t batch, const float* poses, const int32_t* n_valid, int32_t K,
+               const double* meta, const float* tracks_out, const int32_t* n_tracks) {
   if (!t || !poses || !n_valid || !meta || !tracks_out || !n_tracks) return fail(CP_ERR_INVALID, "cp_tracker_step: null argument");
   if (batch <= 0 || batch > t->cfg.streams) return fail(CP_ERR_INVALID, "cp_tracker_step: batch exceeds the tracker's streams");
   if (K <= 0 || K > CP_MAX_K) return fail(CP_ERR_INVALID, "cp_tracker_step: K must be in 1..128");
-  cudaStream_t s = (cudaStream_t)stream;
+  return CP_OK;
+}
+
+// the step of a checked call; ids (device [batch] or nullptr) is read by the kernels
+int launch_step(cp_tracker* t, int32_t batch, const int* ids, const float* poses, const int32_t* n_valid, int32_t K,
+                const double* meta, float* tracks_out, int32_t* n_tracks, cudaStream_t s) {
   StepArgs a;
-  if (int rc = upload_stream_ids(t, batch, stream_ids, s, &a.ids)) return rc;
+  a.ids = ids;
   a.cfg = make_cfg(t->cfg);
   a.cat = t->cat;
   a.opencv_return = t->cfg.opencv_return;
@@ -758,6 +753,32 @@ int cp_tracker_step_ex(cp_tracker* t, int32_t batch, const int32_t* stream_ids, 
   tracker_step_kernel<<<batch, TRK_THREADS, 0, s>>>(a);     // flips cur[] of the streams it steps, and only those
   CP_LAUNCH_CHECK("tracker_step_kernel");
   return CP_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
+int cp_tracker_step(cp_tracker* t, int32_t batch, const float* poses, const int32_t* n_valid, int32_t K, const double* meta,
+                    float* tracks_out, int32_t* n_tracks, void* stream) {
+  return cp_tracker_step_ex(t, batch, nullptr, poses, n_valid, K, meta, tracks_out, n_tracks, stream);
+}
+
+int cp_tracker_step_ex(cp_tracker* t, int32_t batch, const int32_t* stream_ids, const float* poses, const int32_t* n_valid,
+                       int32_t K, const double* meta, float* tracks_out, int32_t* n_tracks, void* stream) {
+  if (int rc = check_stream_ids(t, batch, stream_ids, "cp_tracker_step")) return rc;
+  if (int rc = check_step(t, batch, poses, n_valid, K, meta, tracks_out, n_tracks)) return rc;
+  cudaStream_t s = (cudaStream_t)stream;
+  const int* ids = nullptr;
+  if (int rc = upload_stream_ids(t, batch, stream_ids, s, &ids)) return rc;
+  return launch_step(t, batch, ids, poses, n_valid, K, meta, tracks_out, n_tracks, s);
+}
+
+int cp_tracker_step_dev(cp_tracker* t, int32_t batch, const int32_t* stream_ids, const float* poses,
+                        const int32_t* n_valid, int32_t K, const double* meta, float* tracks_out, int32_t* n_tracks,
+                        void* stream) {
+  if (int rc = check_step(t, batch, poses, n_valid, K, meta, tracks_out, n_tracks)) return rc;
+  return launch_step(t, batch, stream_ids, poses, n_valid, K, meta, tracks_out, n_tracks, (cudaStream_t)stream);
 }
 
 int cp_tracker_render(cp_tracker* t, int32_t batch, const double* meta, const double* trans_input, int32_t inp_h,
@@ -792,6 +813,14 @@ int cp_tracker_render_dev(cp_tracker* t, int32_t batch, const double* meta, cons
                           int32_t inp_w, const int32_t* modes, float* pre_hm, float* pre_hm_hp, void* stream) {
   if (int rc = check_render(t, batch, meta, trans_input, inp_h, inp_w, pre_hm, pre_hm_hp)) return rc;
   return launch_render(t, batch, nullptr, meta, trans_input, inp_h, inp_w, modes, pre_hm, pre_hm_hp, (cudaStream_t)stream);
+}
+
+int cp_tracker_render_dev2(cp_tracker* t, int32_t batch, const int32_t* stream_ids, const double* meta,
+                           const double* trans_input, int32_t inp_h, int32_t inp_w, const int32_t* modes, float* pre_hm,
+                           float* pre_hm_hp, void* stream) {
+  if (int rc = check_render(t, batch, meta, trans_input, inp_h, inp_w, pre_hm, pre_hm_hp)) return rc;
+  return launch_render(t, batch, stream_ids, meta, trans_input, inp_h, inp_w, modes, pre_hm, pre_hm_hp,
+                       (cudaStream_t)stream);
 }
 
 int cp_tracker_seed(cp_tracker* t, int32_t batch, const float* seeds, const int32_t* n_seeds, int32_t S, void* stream) {

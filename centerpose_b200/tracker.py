@@ -378,8 +378,8 @@ class TrackGraph(object):
     (track=True) and this graph may be called in any order, each keeping its own slot state.  Greedy or opt.hungarian
     association, opt.empty_pre_hm and the heat maps drawn from the tracks follow opt as in run_batch.  Refused (ValueError
     or NotImplementedError; they stay on run_batch): test_scales other than [1], the ground-truth heat maps
-    (opt.gt_pre_hm_hmhp / gt_pre_hm_hmhp_first), pre_dets seeding and idle slots.  Several categories go through
-    MultiCategoryTrackGraph.
+    (opt.gt_pre_hm_hmhp / gt_pre_hm_hmhp_first), pre_dets seeding, and idle slots unless idle_slots=True.  Several
+    categories go through MultiCategoryTrackGraph.
 
     frame_hw: one (H, W) for every slot, or a list of S (H_s, W_s).  camera_matrix: [3,3] for every slot or [S,3,3].
       - One size: a call takes the frames as one array, uint8 [S,H,W,3] for pixel_format "bgr", [S,3H/2,W] for "nv12" /
@@ -388,17 +388,27 @@ class TrackGraph(object):
         region of one packed device buffer; the step is that of run_batch(list, track=True) with every slot present, the
         pre-process reading a frame table built once now (cp_preprocess_slots_ragged_dev).
     Frames may be on the host (pinned memory keeps the copy asynchronous; the caller must not overwrite them until the
-    step's outputs are read) or on the device."""
+    step's outputs are read) or on the device.
+
+    idle_slots=True: a call takes a list of S entries, a frame of that slot's size and format or None for an idle slot
+    (with one frame_hw, a uint8 [S, ...] array still means every slot live).  Every step is bit for bit
+    run_batch(list, track=True) of a fresh detector on the same list: an idle slot comes back with n_tracks 0 and zero
+    rows, and its stream, tracks and previous frame are left as they were; a slot's first live frame (after building or
+    reset()) starts its video, and new_video[i] restarts a live slot and is ignored on an idle one; an all-idle call
+    returns zeros and launches nothing.  One step is captured per live count L = 1..S (the network runs at batch L, as
+    in run_batch), so building costs S warm-up steps and S captures; a call is one copy per live frame, one copy of an
+    int32 control block (start flags and the row / stream maps) and one graph launch.  Each slot's previous frame is
+    kept in a per-slot store that the pre-process exchanges in place."""
 
     _host_step = "run_batch(track=True)"              # where what the graph refuses runs
     _host_list = "run_batch(list, track=True)"
 
-    def __init__(self, det, slots, frame_hw, camera_matrix, pixel_format="bgr"):
+    def __init__(self, det, slots, frame_hw, camera_matrix, pixel_format="bgr", idle_slots=False):
         from .detector import ObjectPoseDetector
         if not isinstance(det, ObjectPoseDetector) or det._track_categories() is not None:
             raise NotImplementedError("TrackGraph tracks one category; several run through MultiCategoryTracker.run_batch "
                                       "or a MultiCategoryTrackGraph")
-        self._build(det, slots, frame_hw, camera_matrix, pixel_format)
+        self._build(det, slots, frame_hw, camera_matrix, pixel_format, idle_slots)
 
     def _plan(self, det, S, ih, iw):
         """(plan, decode parameters, tracker, categories or None) of the graph: a copy of det's plan and weights."""
@@ -409,8 +419,9 @@ class TrackGraph(object):
         eng.load_state_dict(m.state_dict())
         return eng, decode_params(det.opt, test_scale=1.0), Tracker(det.opt, streams=S, device=self.device), None
 
-    def _build(self, det, slots, frame_hw, camera_matrix, pixel_format):
-        """Checks, buffers and the two captured steps; everything that refuses comes before any device work."""
+    def _build(self, det, slots, frame_hw, camera_matrix, pixel_format, idle_slots=False):
+        """Checks, buffers and the captured steps (two, or one per live count with idle_slots); everything that refuses
+        comes before any device work."""
         from .detector import affine_from_center_scale, camera_per_frame
         from .engine import check_pixel_format, frame_shape, make_meta
         who, opt = type(self).__name__, det.opt
@@ -425,6 +436,7 @@ class TrackGraph(object):
         if S < 1:
             raise ValueError("%s: slots must be >= 1, got %d" % (who, S))
         sizes, self.per_slot = _frame_sizes(frame_hw, S, who)
+        self.idle_slots = bool(idle_slots)
         self.pixel_format = check_pixel_format(pixel_format)
         shapes = [frame_shape(h, w, pixel_format) for h, w in sizes]
         cams = np.stack(camera_per_frame(camera_matrix, S))
@@ -433,6 +445,7 @@ class TrackGraph(object):
         else:
             self.frame_hw, self.frame_shape = sizes[0], (S,) + shapes[0]
             sizes = sizes * S
+        self._slot_hw, self._slot_shapes = sizes, shapes if self.per_slot else shapes * S
         self.L = L = _lib.load()
         self.slots, self.device = S, torch.device("cuda", torch.cuda.current_device())
         dev = self.device
@@ -454,11 +467,11 @@ class TrackGraph(object):
         self._mean = (ctypes.c_float * 3)(*[float(v) for v in opt.mean])
         self._std = (ctypes.c_float * 3)(*[float(v) for v in opt.std])
         self._fmt = {"bgr": _lib.CP_PIX_BGR, "nv12": _lib.CP_PIX_NV12, "i420": _lib.CP_PIX_I420}[self.pixel_format]
-        if self.per_slot:
-            n = [int(np.prod(s)) for s in shapes]
+        if self.per_slot or self.idle_slots:                # a frame table (with idle slots: of S equal sizes too)
+            n = [int(np.prod(s)) for s in self._slot_shapes]
             offs = np.concatenate([[0], np.cumsum(n)[:-1]]).astype(np.int64)
             self.frames = torch.zeros((int(sum(n)),), dtype=torch.uint8, device=dev)
-            self._slot_frames = [self.frames[o:o + k].view(s) for o, k, s in zip(offs, n, shapes)]
+            self._slot_frames = [self.frames[o:o + k].view(s) for o, k, s in zip(offs, n, self._slot_shapes)]
             self.table = torch.zeros((int(L.cp_preprocess_frame_table_bytes(S)),), dtype=torch.uint8, device=dev)
             hw = np.ascontiguousarray(sizes, np.int32)
             with torch.cuda.device(dev):
@@ -468,7 +481,20 @@ class TrackGraph(object):
                                                        _ptr(self.table), _stream()), "cp_preprocess_frame_table")
         else:
             self.frames = torch.zeros(self.frame_shape, dtype=torch.uint8, device=dev)
-        self.start = torch.ones((MS,), dtype=torch.int32, device=dev)
+        if self.idle_slots:
+            # one int32 control block per call: start flags [M*S] (per tracker stream), rows [S] (the slot of each live
+            # row), ids [M*S] (the tracker stream of each live row of each category) and inv [M*S] (the row of each
+            # stream, or -1); a step at live count n reads the first n rows and M * n ids
+            self.ctrl = torch.zeros((3 * MS + S,), dtype=torch.int32, device=dev)
+            self.start, self.rows = self.ctrl[:MS], self.ctrl[MS:MS + S]
+            self.ids, self.inv = self.ctrl[MS + S:2 * MS + S], self.ctrl[2 * MS + S:]
+            self.store = torch.zeros((S, 3, ih, iw), dtype=torch.float32, device=dev)   # every slot's previous frame
+            # the live rows' meta rows and affines, gathered from the per-slot rows above
+            self.meta_rows = torch.zeros((S, _lib.CP_META_DOUBLES), dtype=torch.float64, device=dev)
+            self.meta_trk = torch.zeros((MS, _lib.CP_META_DOUBLES), dtype=torch.float64, device=dev)
+            self.trans_trk = torch.zeros((MS, 6), dtype=torch.float64, device=dev)
+        else:
+            self.start = torch.ones((MS,), dtype=torch.int32, device=dev)
         self.x = [torch.zeros((S, 3, ih, iw), dtype=torch.float32, device=dev) for _ in range(2)]
         lead = self.eng._lead(S)                         # the plan's per-model axes: (S,) or (M, S)
         self.pre_hm = torch.zeros(lead + (1, ih, iw), dtype=torch.float32, device=dev)
@@ -478,27 +504,42 @@ class TrackGraph(object):
         self.n_valid = torch.zeros(lead, dtype=torch.int32, device=dev)
         self.tracks = torch.zeros((MS, self.tracker.max_tracks, _lib.CP_TRACK_RECORD), dtype=torch.float32, device=dev)
         self.n_tracks = torch.zeros((MS,), dtype=torch.int32, device=dev)
+        if self.idle_slots:                              # the step's compact rows, before the scatter to the slots
+            self.tracks_rows, self.n_tracks_rows = torch.zeros_like(self.tracks), torch.zeros_like(self.n_tracks)
         out_lead = (S,) if self.categories is None else (M, S)
         self._out = (self.tracks.view(out_lead + self.tracks.shape[1:]), self.n_tracks.view(out_lead))
+        # the captured steps: p = 0, 1 (the input buffers swapped), or with idle slots p = every live count 1..S
+        steps = range(1, S + 1) if self.idle_slots else (0, 1)
         side = torch.cuda.Stream(device=dev)
         side.wait_stream(torch.cuda.current_stream(dev))
         with torch.cuda.stream(side):            # warm-up outside the capture; the first call resets every slot
-            for p in (0, 1):
+            for p in steps:
+                if self.idle_slots:
+                    self.ctrl.copy_(torch.from_numpy(self._control(list(range(p)), np.ones(S, np.int32))))
                 self._step(p)
         torch.cuda.current_stream(dev).wait_stream(side)
         torch.cuda.synchronize(dev)
-        self.graphs = []
-        for p in (0, 1):
+        if self.idle_slots:                      # the warm-ups stepped every stream: start from nothing
+            self.tracker.reset()
+            torch.cuda.synchronize(dev)
+        self.graphs, pool = [], None
+        for p in steps:
             g = torch.cuda.CUDAGraph(keep_graph=True)
-            with torch.cuda.graph(g):
+            with torch.cuda.graph(g, pool=pool):
                 self._step(p)
             g.instantiate()
             self.graphs.append(g)
+            if self.idle_slots:                  # the S graphs replay in turn on one stream: one memory pool
+                pool = g.pool()
         self._parity = 0
         self._fresh = True
+        self._started = [False] * S
 
     def _step(self, p):
-        """The launches of one step: network input in x[p], previous frames in x[1 - p]."""
+        """The launches of one step: network input in x[p], previous frames in x[1 - p]; with idle slots, the step of p
+        live slots (_step_rows)."""
+        if self.idle_slots:
+            return self._step_rows(p)
         L, st, h = self.L, _stream(), self.tracker._h
         S, MS, (ih, iw), cur, prev = self.slots, self.streams, self.x[p].shape[2:], self.x[p], self.x[1 - p]
         with torch.cuda.device(self.device):
@@ -519,14 +560,76 @@ class TrackGraph(object):
             _lib.check(L.cp_tracker_step(h, MS, _ptr(self.poses), _ptr(self.n_valid), self.poses.shape[-2],
                                          _ptr(self.meta_all), _ptr(self.tracks), _ptr(self.n_tracks), st), "cp_tracker_step")
 
+    def _step_rows(self, n):
+        """The launches of a step of n live slots: the reset of the starting streams, the row-mapped pre-process with
+        the previous-frame exchange, the gathers of the live rows' meta rows and affines, the render, the network at
+        batch n, the tracker step over the live streams and the scatter of their tracks to the slots (zeros for idle
+        slots).  Which slots are live is data in the control block; n fixes the shapes."""
+        L, st, h, S, MS = self.L, _stream(), self.tracker._h, self.slots, self.streams
+        M, cur, prev = MS // S, self.x[0], self.x[1]
+        (ih, iw), Mn, lead = cur.shape[2:], M * n, self.eng._lead(n)
+
+        def view(t):                          # the first rows of a buffer of the plan's lead axes, as lead(n) + inner
+            inner = tuple(t.shape[len(lead):])
+            return t.view(-1)[:int(np.prod(lead + inner))].view(lead + inner)
+
+        def gather(src, dst, rows, m):
+            _lib.check(L.cp_gather_rows_dev(_ptr(src), _ptr(dst), src[0].numel() * src.element_size(), rows, _ptr(m),
+                                            st), "cp_gather_rows_dev")
+        pre_hm, pre_hm_hp, poses, n_valid = view(self.pre_hm), view(self.pre_hm_hp), view(self.poses), view(self.n_valid)
+        with torch.cuda.device(self.device):
+            _lib.check(L.cp_tracker_reset_dev(h, MS, _ptr(self.start), st), "cp_tracker_reset_dev")
+            _lib.check(L.cp_preprocess_slots_rows_dev(_ptr(self.frames), _ptr(self.table), self._fmt, _ptr(self.rows), n,
+                                                      ih, iw, self._mean, self._std, _ptr(self.start), _ptr(self.store),
+                                                      _ptr(cur), _ptr(prev), st), "cp_preprocess_slots_rows_dev")
+            gather(self.meta, self.meta_rows, n, self.rows)
+            gather(self.meta_all, self.meta_trk, Mn, self.ids)
+            gather(self.trans, self.trans_trk, Mn, self.ids)
+            _lib.check(L.cp_tracker_render_dev2(h, Mn, _ptr(self.ids), _ptr(self.meta_trk), _ptr(self.trans_trk), ih, iw,
+                                                _ptr(self.modes), _ptr(pre_hm), _ptr(pre_hm_hp), st),
+                       "cp_tracker_render_dev2")
+            self.eng.infer(cur[:n], self.meta_rows[:n], self.prm, prev[:n], pre_hm, pre_hm_hp, poses=poses,
+                           n_valid=n_valid)
+            _lib.check(L.cp_tracker_step_dev(h, Mn, _ptr(self.ids), _ptr(poses), _ptr(n_valid), poses.shape[-2],
+                                             _ptr(self.meta_trk), _ptr(self.tracks_rows), _ptr(self.n_tracks_rows), st),
+                       "cp_tracker_step_dev")
+            gather(self.tracks_rows, self.tracks, MS, self.inv)
+            gather(self.n_tracks_rows.view(MS, 1), self.n_tracks.view(MS, 1), MS, self.inv)
+
+    def _control(self, live, start):
+        """The control block of a step over the slots `live` (in row order), start: int32 [S] (slots that start)."""
+        S, MS = self.slots, self.streams
+        M, n = MS // S, len(live)
+        rows = np.zeros(S, np.int32)
+        rows[:n] = live
+        ids = np.zeros(MS, np.int32)
+        ids[:M * n] = [m * S + i for m in range(M) for i in live]
+        inv = np.full(MS, -1, np.int32)
+        inv[ids[:M * n]] = np.arange(M * n, dtype=np.int32)
+        return np.concatenate([np.tile(start, M), rows, ids, inv]).astype(np.int32)
+
     def reset(self):
-        """Forget every slot's tracks and previous frame: the next call starts a video in every slot."""
+        """Forget every slot's tracks and previous frame: the next call starts a video in every slot (with idle slots:
+        each slot's next live frame starts its video)."""
         self._fresh = True
+        self._started = [False] * self.slots
 
     def _frames(self, frames):
-        """The frames of one call, checked against the slots' shapes: one tensor, or one per slot."""
+        """The frames of one call, checked against the slots' shapes: one tensor, or one per slot (with idle slots: one
+        per slot, None for an idle one)."""
         who = type(self).__name__
-        if not self.per_slot:
+        if self.idle_slots and not isinstance(frames, (list, tuple)):
+            if self.per_slot or not (torch.is_tensor(frames) or isinstance(frames, np.ndarray)):
+                raise ValueError("%s was built with idle slots: frames is a list of %d frames (None for an idle slot)%s, "
+                                 "got %s" % (who, self.slots, "" if self.per_slot else " or one uint8 %s array"
+                                             % list(self.frame_shape), type(frames).__name__))
+            frames = torch.from_numpy(frames) if isinstance(frames, np.ndarray) else frames
+            if frames.dtype != torch.uint8 or tuple(frames.shape) != self.frame_shape:
+                raise ValueError("%s: frames must be uint8 %s (%s), got %s %s" % (who, list(self.frame_shape),
+                                                                                 self.pixel_format, frames.dtype,
+                                                                                 tuple(frames.shape)))
+            return list(frames)                         # every slot live
+        if not self.per_slot and not self.idle_slots:
             if isinstance(frames, np.ndarray):
                 frames = torch.from_numpy(frames)
             if not torch.is_tensor(frames) or frames.dtype != torch.uint8 or tuple(frames.shape) != self.frame_shape:
@@ -537,19 +640,22 @@ class TrackGraph(object):
             return [frames]
         if not isinstance(frames, (list, tuple)) or len(frames) != self.slots:
             what = "%d frames" % len(frames) if isinstance(frames, (list, tuple)) else type(frames).__name__
-            raise ValueError("%s was built with one frame_hw per slot: frames is a list of %d frames, got %s"
-                             % (who, self.slots, what))
+            raise ValueError("%s was built with %s: frames is a list of %d frames, got %s"
+                             % (who, "idle slots" if self.idle_slots else "one frame_hw per slot", self.slots, what))
         out = []
         for b, f in enumerate(frames):
             if f is None:
+                if self.idle_slots:
+                    out.append(None)
+                    continue
                 raise ValueError("%s steps every slot: slot %d is idle; idle slots run through %s"
                                  % (who, b, self._host_list))
             if isinstance(f, np.ndarray):
                 f = torch.from_numpy(f)
-            if not torch.is_tensor(f) or f.dtype != torch.uint8 or tuple(f.shape) != self.frame_shape[b]:
+            if not torch.is_tensor(f) or f.dtype != torch.uint8 or tuple(f.shape) != self._slot_shapes[b]:
                 what = ("%s %s" % (f.dtype, tuple(f.shape))) if torch.is_tensor(f) else type(f).__name__
                 raise ValueError("%s: slot %d takes uint8 %s frames (%s, frame_hw %s), got %s"
-                                 % (who, b, list(self.frame_shape[b]), self.pixel_format, self.frame_hw[b], what))
+                                 % (who, b, list(self._slot_shapes[b]), self.pixel_format, self._slot_hw[b], what))
             out.append(f)
         return out
 
@@ -568,6 +674,8 @@ class TrackGraph(object):
             if len(new_video) != self.slots:
                 raise ValueError("%s: %d new_video entries for %d slots" % (who, len(new_video), self.slots))
             start |= np.array(new_video, np.int32)
+        if self.idle_slots:
+            return self._call_rows(frames, start)
         start = np.tile(start, self.streams // self.slots)       # one flag per tracker stream, the same in every category
         with torch.cuda.device(self.device):
             for dst, f in zip(self._slot_frames if self.per_slot else [self.frames], frames):
@@ -576,6 +684,28 @@ class TrackGraph(object):
             self.start.copy_(torch.from_numpy(start), non_blocking=True)
             self.graphs[self._parity].replay()
         self._parity ^= 1
+        self._fresh = False
+        return self._out
+
+    def _call_rows(self, frames, start):
+        """A call with idle slots: frames[i] None idles slot i.  A live slot starts its video when it has not started
+        since the graph was built or reset, or when start[i] (new_video); an idle slot is not stepped and keeps its
+        tracks and previous frame.  Copies the live frames and the control block, then replays the graph of the live
+        count; with no live slot, zeros the outputs and launches no graph."""
+        live = [i for i, f in enumerate(frames) if f is not None]
+        with torch.cuda.device(self.device):
+            if not live:
+                self.tracks.zero_()
+                self.n_tracks.zero_()
+                return self._out
+            start = np.array([i in live and (bool(start[i]) or not self._started[i]) for i in range(self.slots)], np.int32)
+            for i in live:
+                self._slot_frames[i].copy_(frames[i], non_blocking=True)
+            # a pageable source: staged before copy_ returns, without waiting for the device
+            self.ctrl.copy_(torch.from_numpy(self._control(live, start)), non_blocking=True)
+            self.graphs[len(live) - 1].replay()
+        for i in live:
+            self._started[i] = True
         self._fresh = False
         return self._out
 
@@ -591,12 +721,13 @@ class MultiCategoryTrackGraph(TrackGraph):
 
     The graph owns its plan (every category's weights, copied from trk now), its tracker and buffers: trk._slots is left
     untouched, and trk.run_batch and this graph may be called in any order.  Refused as in TrackGraph; several categories
-    of one graph need a MultiCategoryTracker (a MultiCategoryDetector is not a tracking model)."""
+    of one graph need a MultiCategoryTracker (a MultiCategoryDetector is not a tracking model).  idle_slots=True as in
+    TrackGraph, bit for bit trk.run_batch(list) with None for the idle slots."""
 
     _host_step = "MultiCategoryTracker.run_batch"
     _host_list = "MultiCategoryTracker.run_batch(list)"
 
-    def __init__(self, trk, slots, frame_hw, camera_matrix, pixel_format="bgr"):
+    def __init__(self, trk, slots, frame_hw, camera_matrix, pixel_format="bgr", idle_slots=False):
         from .detector import MultiCategoryDetector, MultiCategoryTracker
         if not isinstance(trk, MultiCategoryTracker):
             if isinstance(trk, MultiCategoryDetector):
@@ -604,7 +735,7 @@ class MultiCategoryTrackGraph(TrackGraph):
                                  "tracking model")
             raise NotImplementedError("MultiCategoryTrackGraph takes a MultiCategoryTracker; one category's "
                                       "ObjectPoseDetector goes to TrackGraph")
-        self._build(trk, slots, frame_hw, camera_matrix, pixel_format)
+        self._build(trk, slots, frame_hw, camera_matrix, pixel_format, idle_slots)
 
     def _plan(self, trk, S, ih, iw):
         from .engine import Engine

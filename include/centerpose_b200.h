@@ -516,6 +516,20 @@ int cp_tracker_reset_dev(cp_tracker* trk, int32_t batch, const int32_t* flags, v
  * CP_RENDER_EMPTY draws the tracks. */
 int cp_tracker_render_dev(cp_tracker* trk, int32_t batch, const double* meta, const double* trans_input, int32_t inp_h,
                           int32_t inp_w, const int32_t* modes, float* pre_hm, float* pre_hm_hp, void* stream);
+/* cp_tracker_render_dev with a stream map: image i draws the tracks of tracker stream stream_ids[i].  stream_ids is a
+ * DEVICE int32 [batch] (or NULL: the identity) that the kernel reads WITHOUT checking: the caller guarantees every id is
+ * in 0..streams-1 and none appears twice (cp_tracker_render_ex2 checks a host map; this one cannot). */
+int cp_tracker_render_dev2(cp_tracker* trk, int32_t batch, const int32_t* stream_ids, const double* meta,
+                           const double* trans_input, int32_t inp_h, int32_t inp_w, const int32_t* modes, float* pre_hm,
+                           float* pre_hm_hp, void* stream);
+/* cp_tracker_step_ex with the stream map in device memory: row i (poses[i], n_valid[i], meta[i], tracks_out[i],
+ * n_tracks[i]) steps tracker stream stream_ids[i]; streams the map does not list keep their state.  stream_ids is a
+ * DEVICE int32 [batch] (or NULL: the identity) that the kernels read WITHOUT checking: the caller guarantees every id is
+ * in 0..streams-1 and none appears twice.  Greedy or Hungarian association as configured; the kernels are those of
+ * cp_tracker_step_ex. */
+int cp_tracker_step_dev(cp_tracker* trk, int32_t batch, const int32_t* stream_ids, const float* poses,
+                        const int32_t* n_valid, int32_t K, const double* meta, float* tracks_out, int32_t* n_tracks,
+                        void* stream);
 
 /* Offsets (in floats) inside one CP_SEED_RECORD: one dict of meta['pre_dets'] (eval_video_official.py:422-450). */
 #define CP_SEED_RECORD 264
@@ -675,6 +689,23 @@ int cp_preprocess_frame_table(int64_t frames_bytes, const int64_t* offsets, cons
 int cp_preprocess_slots_ragged_dev(const uint8_t* frames, const void* table, int32_t format, int32_t B, int32_t dst_h,
                                    int32_t dst_w, const float mean[3], const float std[3], const int32_t* start,
                                    float* out, float* prev, void* stream);
+/* The pre-process of one tracking step in which only some of the S slots of a cp_preprocess_frame_table have a frame,
+ * safe to capture in a CUDA graph.  Row n of the B live rows is slot rows[n]: out[n] (device fp32 [B,3,dst_h,dst_w]) is
+ * bit for bit what cp_preprocess_slots_ragged_dev gives for that slot's frame.  rows (int32 [B]), start (int32 [S], per
+ * SLOT) and the table are DEVICE memory read when the kernel runs, WITHOUT checking: the caller guarantees every
+ * rows[n] is in 0..S-1 and none appears twice.  store (device fp32 [S,3,dst_h,dst_w], the previous frame of every slot)
+ * and prev (device fp32 [B,3,dst_h,dst_w]) are both given or both NULL; with them the walk also sets
+ *   prev[n] = start[rows[n]] ? out[n] : store[rows[n]],  then  store[rows[n]] = out[n],
+ * so a slot that starts its video takes this frame as its previous frame, and an idle slot's stored frame is not
+ * touched.  start NULL: no slot starts.  Bad arguments return CP_ERR_INVALID before any work is enqueued. */
+int cp_preprocess_slots_rows_dev(const uint8_t* frames, const void* table, int32_t format, const int32_t* rows, int32_t B,
+                                 int32_t dst_h, int32_t dst_w, const float mean[3], const float std[3],
+                                 const int32_t* start, float* store, float* out, float* prev, void* stream);
+/* A row gather, safe to capture in a CUDA graph: dst row i = src row map[i], or zeros where map[i] < 0, for i in 0..n-1,
+ * rows of row_bytes bytes (a positive multiple of 4; src and dst 4-byte aligned).  map is a DEVICE int32 [n] read when
+ * the kernel runs, WITHOUT checking: the caller guarantees every map[i] is below the rows of src.  Bad arguments return
+ * CP_ERR_INVALID before any work is enqueued. */
+int cp_gather_rows_dev(const void* src, void* dst, int64_t row_bytes, int32_t n, const int32_t* map, void* stream);
 
 /* ---- misc ------------------------------------------------------------------ */
 int cp_version(void);

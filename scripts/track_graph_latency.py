@@ -81,7 +81,8 @@ def measure(S, fmt, steps, warmup, runs, prof_dir):
 
 def time_arms(arms, resets, frames, warmup, runs, label, trace=None):
     """Both arms over the same frames, alternating step by step, after calling every reset; their outputs are checked
-    identical at every step.  trace: a path pattern with one %s (the arm) for the profiler traces, or None."""
+    identical at every step (the first two arms').  trace: a path pattern with one %s (the arm) for the profiler traces,
+    or None."""
     res = {a: {"step_ms": [], "gpu_ms": []} for a in arms}
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     for _ in range(runs):
@@ -101,9 +102,9 @@ def time_arms(arms, resets, frames, warmup, runs, label, trace=None):
                 if k >= warmup:
                     res[a]["step_ms"].append((t1 - t0) * 1e3)
                     res[a]["gpu_ms"].append(ev0.elapsed_time(ev1))
-            g, r = outs["graph"], outs["run_batch"]
+            (ga, g), (ra, r) = list(outs.items())[:2]
             if not (np.array_equal(g[0], r[0]) and np.array_equal(g[1], r[1])):
-                raise SystemExit("%s step %d: the graph and run_batch disagree" % (label, k))
+                raise SystemExit("%s step %d: %s and %s disagree" % (label, k, ga, ra))
     # kernel and copy sums per step, profiled in a run of their own
     from torch.autograd import DeviceType
     n_prof = 5
