@@ -14,6 +14,8 @@
 //   warp 1 : weight-tile producer, cp.async.bulk          (ring of SB stages, tiles pre-swizzled at load time)
 //   warpgroups 1, 2 : consumers, rows [0, 64) / [64, 128) of the tile: wgmma into registers + epilogue
 //   warpgroup 3 (x3 only) : hi / lo splitters of the activation slabs
+//   warpgroup 4 (x3 with the fused per-head 1x1 only) : the 1x1, from a ring of relu(conv + bias) chunks the
+//                           consumers fill, so it runs under the next tile's MMAs
 // Reference semantics: nn.Conv2d(k, stride 1, padding k//2) + folded BatchNorm + residual + ReLU
 // (pose_dla_dcn.py:37-62, 153-168, 496-505).
 #include <cuda.h>
@@ -27,6 +29,11 @@ namespace {
 constexpr int TM_BM = 128;
 constexpr int TM_THREADS = 384;       // control warpgroup + two consumer warpgroups
 constexpr int TM_THREADS_X3 = 512;    // + the splitter warpgroup
+constexpr int TM_THREADS_X3F = 640;   // + the fused 1x1 warpgroup
+// x3 fused 1x1: a hidden-ring slot holds relu(conv + bias) of one tile's 128 rows x 32 columns; the 1x1 weights of
+// one N tile (BN = 128 hidden channels x 16 outputs) are staged next to the ring
+constexpr uint32_t TM_HSLOT_BYTES = 128u * 32u * 4u;
+constexpr uint32_t TM_W1_BYTES = 128u * 16u * 4u;
 
 struct TmaConvParams {
   CUtensorMap amap[4];
@@ -66,6 +73,7 @@ struct TmaConvParams {
   // of them over its ipm images) so that no tile mixes two models' weights.
   int ipm;
   long long wstride, tstride, tiles_per_model;
+  int RS;             // x3 fused 1x1: slots of the hidden ring (1 or 2)
 };
 
 using namespace umma;
@@ -73,6 +81,7 @@ using namespace umma;
 struct TmaCtl {
   unsigned long long a_full[4], a_empty[4], a_split[4];
   unsigned long long b_full[8], b_empty[8];
+  unsigned long long h_full[2], h_empty[2];     // x3 fused 1x1: hidden ring
 };
 static_assert(sizeof(TmaCtl) <= 512, "control block");
 
@@ -136,7 +145,13 @@ __device__ __forceinline__ bool tile_position(const TmaConvParams& p, const Tile
 // pipeline state across tiles, so the TMA / split of tile i+1 overlap the epilogue of tile i and the fixed cost of a CTA
 // (barrier init, descriptor fetch, pipeline fill) is paid once per SM instead of per tile.
 template <bool X3, bool FUSE, int BN, bool MULTI>
-__global__ void __launch_bounds__(X3 ? TM_THREADS_X3 : TM_THREADS, 1) conv_tma_kernel(const __grid_constant__ TmaConvParams p) {
+__global__ void __launch_bounds__(X3 ? (FUSE ? TM_THREADS_X3F : TM_THREADS_X3) : TM_THREADS, 1)
+    conv_tma_kernel(const __grid_constant__ TmaConvParams p) {
+  // x3 fused: the per-head 1x1 runs in its own warpgroup (warps 16 - 19) behind the hidden ring
+  constexpr bool EPI = X3 && FUSE;
+  // setmaxnreg per role; the counts of the five (x3 fused) or four (x3) warpgroups add up to at most what the launch
+  // gives 640 (96 each) or 512 (128 each) threads.  Counts above the launch's are taken with .inc, below it with .dec.
+  constexpr int REG_CTL = EPI ? 32 : 40, REG_SPLIT = EPI ? 40 : 48, REG_EPI = 104, REG_CONS = EPI ? 152 : 208;
   extern __shared__ __align__(1024) unsigned char smem[];
   TmaCtl* ctl = reinterpret_cast<TmaCtl*>(smem);
   if (threadIdx.x == 0) griddep_launch_dependents();      // PDL (common.cuh): the next launch may take this SM when we retire
@@ -170,6 +185,12 @@ __global__ void __launch_bounds__(X3 ? TM_THREADS_X3 : TM_THREADS, 1) conv_tma_k
       mbar_init(smem_u32(&ctl->b_full[s]), 1);
       mbar_init(smem_u32(&ctl->b_empty[s]), 2);
     }
+    if constexpr (EPI) {
+      for (int s = 0; s < p.RS; ++s) {
+        mbar_init(smem_u32(&ctl->h_full[s]), 256);     // every consumer thread
+        mbar_init(smem_u32(&ctl->h_empty[s]), 128);    // every 1x1 thread
+      }
+    }
     fence_mbar_init();
   }
   __syncthreads();
@@ -182,7 +203,7 @@ __global__ void __launch_bounds__(X3 ? TM_THREADS_X3 : TM_THREADS, 1) conv_tma_k
   // sums.  The control and splitter warpgroups hand registers to the consumers with setmaxnreg; the role code sits
   // inside the branch that executed it so that ptxas allocates per branch.
   if (warp < 4) {
-    if (X3) asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (X3) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(REG_CTL));
     if (warp == 0) {
       // ===================== activation slabs via TMA =====================
       if (lane == 0) {
@@ -242,8 +263,103 @@ __global__ void __launch_bounds__(X3 ? TM_THREADS_X3 : TM_THREADS, 1) conv_tma_k
       }
       __syncwarp();
     }
+  } else if (EPI && warp >= 16) {
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(REG_EPI));
+    // ===================== fused per-head 1x1 (x3): hidden ring -> head outputs =====================
+    // Thread (rg, hh, og) accumulates rows rg + 32 i (i < 4) x outputs 8 og .. 8 og + 7 over hidden channels
+    // c0 + 16 hh .. + 15 of every 32-column chunk, in increasing order and across the head's tph N tiles: each
+    // (row, output) sees the products and order of a thread per row and half.
+    const int wt = tid - 512, rg = wt >> 2, hh = (wt >> 1) & 1, og = wt & 1;
+    // the hidden ring, then the staged 1x1 weights, take the place of the consumers' staging buffers
+    const float* hring = reinterpret_cast<const float*>(smem + (drain0 - smem_u32(smem)));
+    float4* w1 = reinterpret_cast<float4*>(smem + (drain0 - smem_u32(smem)) + (size_t)p.RS * TM_HSLOT_BYTES);
+    const uint32_t bar_h_full = smem_u32(&ctl->h_full[0]), bar_h_empty = smem_u32(&ctl->h_empty[0]);
+    auto at = [&](int r, int col) { return r * 32 + ((((col >> 2) ^ r) & 7) << 2) + (col & 3); };
+    // the tile's 1x1 weights as float4 (hidden k, outputs 4 q .. 4 q + 3) at (4 k + q) ^ (k & 16 ? 4 : 0): rows k and
+    // k ^ 1 trade places in the upper half of every 32, so the two hidden halves of a warp read different banks
+    auto stage_w1 = [&](long long tile) {
+      const TileGeo g = decode_tile<MULTI>(p, tile, n_tiles);
+      const int head = g.n_tile / p.tph, part = g.n_tile - head * p.tph;
+      const float4* src = reinterpret_cast<const float4*>(p.fuse_w[head] + (MULTI ? (size_t)g.model * p.wstride : 0)) +
+                          (size_t)part * BN * 4;
+      for (int i = wt; i < BN * 4; i += 128) w1[i ^ (((i >> 2) & 16) ? 4 : 0)] = __ldg(src + i);
+    };
+    int rs = 0;
+    uint32_t rp = 0;
+    float acc2[32];
+    long long it = 0, tile = tile_at(0);
+    if (tile < total_tiles) stage_w1(tile);
+    wg_bar_sync(3);
+    while (tile < total_tiles) {
+      const TileGeo g = decode_tile<MULTI>(p, tile, n_tiles);
+      const int head = g.n_tile / p.tph, part = g.n_tile - head * p.tph;
+      if (part == 0) {
+#pragma unroll
+        for (int j = 0; j < 32; ++j) acc2[j] = 0.f;
+      }
+#pragma unroll 1
+      for (int c0 = 0; c0 < BN; c0 += 32) {
+        mbar_wait(bar_h_full + 8u * (uint32_t)rs, rp);
+        const float* hs = hring + (size_t)rs * (TM_HSLOT_BYTES / 4);
+#pragma unroll
+        for (int m4 = 0; m4 < 4; ++m4) {
+          const int k0 = 16 * hh + 4 * m4;          // hidden channels c0 + k0 .. + 3
+          float4 hv[4];
+#pragma unroll
+          for (int i = 0; i < 4; ++i) hv[i] = *reinterpret_cast<const float4*>(hs + at(rg + 32 * i, k0));
+#pragma unroll
+          for (int kk = 0; kk < 4; ++kk) {
+            const int wi = (((c0 + k0 + kk) << 2) + 2 * og) ^ (hh << 2);
+            const float4 wa = w1[wi], wb = w1[wi + 1];
+#pragma unroll
+            for (int i = 0; i < 4; ++i) {
+              const float h = kk == 0 ? hv[i].x : kk == 1 ? hv[i].y : kk == 2 ? hv[i].z : hv[i].w;
+              acc2[8 * i + 0] = fmaf(h, wa.x, acc2[8 * i + 0]);
+              acc2[8 * i + 1] = fmaf(h, wa.y, acc2[8 * i + 1]);
+              acc2[8 * i + 2] = fmaf(h, wa.z, acc2[8 * i + 2]);
+              acc2[8 * i + 3] = fmaf(h, wa.w, acc2[8 * i + 3]);
+              acc2[8 * i + 4] = fmaf(h, wb.x, acc2[8 * i + 4]);
+              acc2[8 * i + 5] = fmaf(h, wb.y, acc2[8 * i + 5]);
+              acc2[8 * i + 6] = fmaf(h, wb.z, acc2[8 * i + 6]);
+              acc2[8 * i + 7] = fmaf(h, wb.w, acc2[8 * i + 7]);
+            }
+          }
+        }
+        mbar_arrive(bar_h_empty + 8u * (uint32_t)rs);
+        if (++rs == p.RS) {
+          rs = 0;
+          rp ^= 1u;
+        }
+      }
+      if (part == p.tph - 1) {
+        // the two hidden halves of a (row, output) are in lanes that differ in bit 1
+#pragma unroll
+        for (int j = 0; j < 32; ++j) acc2[j] += __shfl_xor_sync(0xffffffffu, acc2[j], 2);
+        if (hh == 0) {
+          const int co = p.fuse_cout[head] - 8 * og;          // outputs of this thread: min(8, co)
+          const float* b2 = p.fuse_b[head] + (MULTI ? (size_t)g.model * p.wstride : 0) + 8 * og;
+          float bo[8];
+#pragma unroll
+          for (int u = 0; u < 8; ++u) bo[u] = u < co ? __ldg(b2 + u) : 0.f;
+          const size_t plane = (size_t)p.H * p.W;
+#pragma unroll
+          for (int i = 0; i < 4; ++i) {
+            int n1, oy1, ox1, m1;
+            if (!tile_position<MULTI>(p, g, rg + 32 * i, &n1, &oy1, &ox1, &m1)) continue;
+            float* o = p.fuse_out[head] + ((size_t)n1 * p.fuse_cout[head] * p.H + oy1) * p.W + ox1 + 8 * og * plane;
+#pragma unroll
+            for (int u = 0; u < 8; ++u)
+              if (u < co) o[u * plane] = acc2[8 * i + u] + bo[u];
+          }
+        }
+      }
+      tile = tile_at(++it);
+      wg_bar_sync(3);              // every thread is done with this tile's weights
+      if (tile < total_tiles) stage_w1(tile);
+      wg_bar_sync(3);
+    }
   } else if (X3 && warp >= 12) {
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 48;");
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(REG_SPLIT));
     // ===================== hi / lo splitters (x3): slab -> tf32-exact hi (in place) + lo slab =====================
     const int st = tid - 384;
     int stage = 0;
@@ -281,7 +397,7 @@ __global__ void __launch_bounds__(X3 ? TM_THREADS_X3 : TM_THREADS, 1) conv_tma_k
       }
     }
   } else {
-    if (X3) asm volatile("setmaxnreg.inc.sync.aligned.u32 208;");
+    if (X3) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(REG_CONS));
     // ===================== consumers: warpgroup c multiplies rows [64 c, 64 c + 64) of every tile =====================
     const int c = (warp - 4) >> 2, wt = tid & 127;
     float* dstage = reinterpret_cast<float*>(smem + (drain0 - smem_u32(smem))) + (size_t)c * (DRAIN_STAGE_BYTES / 4);
@@ -380,6 +496,35 @@ __global__ void __launch_bounds__(X3 ? TM_THREADS_X3 : TM_THREADS, 1) conv_tma_k
 #pragma unroll
         for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
       }
+      if constexpr (EPI) {
+        // relu(conv + bias) of this warpgroup's 64 rows goes to the hidden ring, 32 columns per slot, 16-byte groups
+        // XOR-swizzled by row & 7 (conflict-free float4 reads); the 1x1 warpgroup takes it from there
+        const int fr0 = (wt >> 5) * 16 + ((wt & 31) >> 2), fcq = (wt & 3) * 2;     // accumulator fragment (drain_rows)
+        const float* b1 = p.bias + (MULTI ? (size_t)g.model * p.wstride : 0) + (size_t)g.n_tile * BN;
+        float* hring = reinterpret_cast<float*>(smem + (drain0 - smem_u32(smem)));        // hidden ring
+        const uint32_t bar_h_full = smem_u32(&ctl->h_full[0]), bar_h_empty = smem_u32(&ctl->h_empty[0]);
+        auto at = [&](int r, int col) { return r * 32 + ((((col >> 2) ^ r) & 7) << 2) + (col & 3); };
+#pragma unroll
+        for (int c0 = 0; c0 < BN; c0 += 32) {
+          const uint32_t chunk = (uint32_t)it * (BN / 32) + c0 / 32;       // chunks so far: ring slot and phase
+          const uint32_t rs = chunk % p.RS, rp = (chunk / p.RS) & 1u;
+          mbar_wait(bar_h_empty + 8u * rs, rp ^ 1u);
+          float* hs = hring + (size_t)rs * (TM_HSLOT_BYTES / 4) + c * 64 * 32;
+#pragma unroll
+          for (int j = 0; j < BN / 8; ++j) {
+            if (j * 8 >= c0 && j * 8 < c0 + 32) {
+              const int col = j * 8 - c0 + fcq;
+              const float bx = __ldg(b1 + c0 + col), by = __ldg(b1 + c0 + col + 1);
+              hs[at(fr0, col)] = fmaxf(sums[X3 ? 4 * j : 0] + bx, 0.f);
+              hs[at(fr0, col + 1)] = fmaxf(sums[X3 ? 4 * j + 1 : 0] + by, 0.f);
+              hs[at(fr0 + 8, col)] = fmaxf(sums[X3 ? 4 * j + 2 : 0] + bx, 0.f);
+              hs[at(fr0 + 8, col + 1)] = fmaxf(sums[X3 ? 4 * j + 3 : 0] + by, 0.f);
+            }
+          }
+          mbar_arrive(bar_h_full + 8u * rs);
+        }
+        continue;
+      }
       // ---- epilogue: rows of this warpgroup, 32 columns at a time through shared memory (drain_rows)
       const int r_me = wt >> 1;
       int n, oy, ox, m;
@@ -423,72 +568,6 @@ __global__ void __launch_bounds__(X3 ? TM_THREADS_X3 : TM_THREADS, 1) conv_tma_k
           epilogue_row<16>(ep, v, valid, m, n, oy, ox, g.n_tile * BN + cb, col_end);
         }
       };
-      if constexpr (X3 && FUSE) {
-        // x3 fused 1x1 (BN = 128): thread (rg, hh, og) accumulates rows rg + 16 i (i < 4) x outputs 4 og .. 4 og + 3 over
-        // hidden channels c0 + 16 hh .. + 15 of every 32-column chunk, in increasing order: each (row, output) sees the
-        // products and order of a thread per row and half, but a weight float4 feeds 16 FMAs instead of 4.  The chunk
-        // passes through the stage as relu(conv + bias), 64 rows x 32 columns, 16-byte groups XOR-swizzled by row & 7
-        // (conflict-free float4 reads).
-        const int rg = wt >> 3, hh = (wt >> 2) & 1, og = wt & 3;
-        const int fr0 = (wt >> 5) * 16 + ((wt & 31) >> 2), fcq = (wt & 3) * 2;     // accumulator fragment (drain_rows)
-        const float* b1 = p.bias + wofs + (size_t)g.n_tile * BN;
-        const float4* w2 = reinterpret_cast<const float4*>(p.fuse_w[head] + wofs) + (size_t)part * BN * 4 + og;
-        auto at = [&](int r, int col) { return r * 32 + ((((col >> 2) ^ r) & 7) << 2) + (col & 3); };
-#pragma unroll
-        for (int c0 = 0; c0 < BN; c0 += 32) {
-#pragma unroll
-          for (int j = 0; j < BN / 8; ++j) {
-            if (j * 8 >= c0 && j * 8 < c0 + 32) {
-              const int col = j * 8 - c0 + fcq;
-              const float bx = __ldg(b1 + c0 + col), by = __ldg(b1 + c0 + col + 1);
-              dstage[at(fr0, col)] = fmaxf(sums[X3 ? 4 * j : 0] + bx, 0.f);
-              dstage[at(fr0, col + 1)] = fmaxf(sums[X3 ? 4 * j + 1 : 0] + by, 0.f);
-              dstage[at(fr0 + 8, col)] = fmaxf(sums[X3 ? 4 * j + 2 : 0] + bx, 0.f);
-              dstage[at(fr0 + 8, col + 1)] = fmaxf(sums[X3 ? 4 * j + 3 : 0] + by, 0.f);
-            }
-          }
-          wg_bar_sync(1 + c);
-#pragma unroll
-          for (int m4 = 0; m4 < 4; ++m4) {
-            const int k0 = 16 * hh + 4 * m4;          // hidden channels c0 + k0 .. + 3
-            float4 hv[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) hv[i] = *reinterpret_cast<const float4*>(dstage + at(rg + 16 * i, k0));
-#pragma unroll
-            for (int kk = 0; kk < 4; ++kk) {
-              const float4 w = __ldg(w2 + (size_t)(c0 + k0 + kk) * 4);
-#pragma unroll
-              for (int i = 0; i < 4; ++i) {
-                const float h = kk == 0 ? hv[i].x : kk == 1 ? hv[i].y : kk == 2 ? hv[i].z : hv[i].w;
-                acc2[FUSE ? 4 * i + 0 : 0] = fmaf(h, w.x, acc2[FUSE ? 4 * i + 0 : 0]);
-                acc2[FUSE ? 4 * i + 1 : 0] = fmaf(h, w.y, acc2[FUSE ? 4 * i + 1 : 0]);
-                acc2[FUSE ? 4 * i + 2 : 0] = fmaf(h, w.z, acc2[FUSE ? 4 * i + 2 : 0]);
-                acc2[FUSE ? 4 * i + 3 : 0] = fmaf(h, w.w, acc2[FUSE ? 4 * i + 3 : 0]);
-              }
-            }
-          }
-          wg_bar_sync(1 + c);
-        }
-        if (part == p.tph - 1) {
-          // the two hidden halves of a (row, output) are in lanes that differ in bit 2
-#pragma unroll
-          for (int j = 0; j < 16; ++j) acc2[FUSE ? j : 0] += __shfl_xor_sync(0xffffffffu, acc2[FUSE ? j : 0], 4);
-          if (hh == 0) {
-            const int co = p.fuse_cout[head];
-            const size_t plane = (size_t)p.H * p.W;
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              int n1, oy1, ox1, m1;
-              if (!tile_position<MULTI>(p, g, c * 64 + rg + 16 * i, &n1, &oy1, &ox1, &m1)) continue;
-              float* o = p.fuse_out[head] + ((size_t)n1 * co * p.H + oy1) * p.W + ox1;
-#pragma unroll
-              for (int u = 0; u < 4; ++u)
-                if (4 * og + u < co) o[(4 * og + u) * plane] = acc2[FUSE ? 4 * i + u : 0] + __ldg(p.fuse_b[head] + wofs + 4 * og + u);
-            }
-          }
-        }
-        continue;
-      }
       if constexpr (X3)
         drain_rows<BN>(sums, dstage, wt, 1 + c, fn);
       else
@@ -586,10 +665,19 @@ static int tma_boxh(int Wt) { return (TM_BM + 1 + 2 * Wt + Wt - 1) / Wt + 1; }
 // Shared memory for the slab and weight-tile rings: 227 KB less the control block, alignment, slack and the two
 // epilogue staging buffers.
 constexpr size_t TM_BUDGET = 222 * 1024 - 2 * (size_t)DRAIN_STAGE_BYTES;
+// x3 fused 1x1: the hidden ring and the staged 1x1 weights take the place of the two staging buffers
+static size_t tma_epi_bytes(int rs) { return (size_t)rs * TM_HSLOT_BYTES + TM_W1_BYTES; }
 
-// Stage counts of the slab ring (SA) and the weight-tile ring (SB).
-static int tma_smem_layout(uint32_t a_stage, uint32_t btile, int k, int* SA, int* SB, size_t* smem) {
-  const size_t budget = TM_BUDGET;
+// Stage counts of the slab ring (SA), the weight-tile ring (SB) and, x3 with the fused 1x1 (epi), the hidden ring (RS).
+// Two hidden slots where two slab stages and three weight stages still fit next to them, else one.
+static int tma_smem_layout(uint32_t a_stage, uint32_t btile, int k, bool epi, int* SA, int* SB, int* RS, size_t* smem) {
+  size_t fixed = 2 * (size_t)DRAIN_STAGE_BYTES;
+  *RS = 0;
+  if (epi) {
+    *RS = 2 * (size_t)a_stage + 3 * (size_t)btile <= 222 * 1024 - tma_epi_bytes(2) ? 2 : 1;
+    fixed = tma_epi_bytes(*RS);
+  }
+  const size_t budget = 222 * 1024 - fixed;
   int sa = 2;
   if ((size_t)sa * a_stage + 2 * (size_t)btile > budget) sa = 1;
   if ((size_t)sa * a_stage + 2 * (size_t)btile > budget) return fail(CP_ERR_INVALID, "conv_tma: slab does not fit shared memory");
@@ -604,7 +692,7 @@ static int tma_smem_layout(uint32_t a_stage, uint32_t btile, int k, int* SA, int
   }
   *SA = sa;
   *SB = sb;
-  *smem = 512 + 2048 + (size_t)sa * a_stage + (size_t)sb * btile + 2 * (size_t)DRAIN_STAGE_BYTES;
+  *smem = 512 + 2048 + (size_t)sa * a_stage + (size_t)sb * btile + fixed;
   return CP_OK;
 }
 
@@ -776,7 +864,7 @@ int launch_conv_tma(const IgemmParams& p, const void* maps, const ConvKernel& k,
   const uint32_t btile = (uint32_t)q.BN * (uint32_t)q.cslab * 4u * (x3 ? 2u : 1u);
   const uint32_t a_stage = q.slab_stride * (x3 ? 2u : 1u);
   size_t smem = 0;
-  if (int rc = tma_smem_layout(a_stage, btile, q.k, &q.SA, &q.SB, &smem)) return rc;
+  if (int rc = tma_smem_layout(a_stage, btile, q.k, x3 && p.fuse_n > 0, &q.SA, &q.SB, &q.RS, &smem)) return rc;
   q.bias = p.bias;
   q.residual = p.residual;
   q.resStride = p.resStride;
@@ -813,7 +901,7 @@ int launch_conv_tma(const IgemmParams& p, const void* maps, const ConvKernel& k,
   if (q.total_tiles >= (1ll << 31)) return fail(CP_ERR_INVALID, "conv_tma: too many tiles");
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3((unsigned)(q.total_tiles < num_sms ? q.total_tiles : num_sms));
-  cfg.blockDim = dim3(x3 ? TM_THREADS_X3 : TM_THREADS);
+  cfg.blockDim = dim3(x3 ? (q.fuse ? TM_THREADS_X3F : TM_THREADS_X3) : TM_THREADS);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = stream;
   // several models in the launch: the model-indexed instantiations; one model runs the one-model code unchanged
