@@ -17,6 +17,7 @@ import torch
 
 from . import _lib
 from .engine import _VISIBLE, _ptr, _stream
+from .graph import _SlotGraph
 
 
 def _opt(opt, name, default):
@@ -346,22 +347,7 @@ class Tracker(object):
         return out
 
 
-def _frame_sizes(frame_hw, S, who):
-    """frame_hw of a graph of S slots -> ([(H, W)], per_slot): one size for every slot, or one per slot."""
-    per_slot = (isinstance(frame_hw, (list, tuple, np.ndarray)) and len(frame_hw) > 0
-                and all(isinstance(v, (list, tuple, np.ndarray)) for v in frame_hw))
-    if per_slot and len(frame_hw) != S:
-        raise ValueError("%s: frame_hw is one (H, W) for every slot or one per slot, got %d for %d slots"
-                         % (who, len(frame_hw), S))
-    sizes = []
-    for hw in (frame_hw if per_slot else [frame_hw]):
-        if len(hw) != 2 or int(hw[0]) < 1 or int(hw[1]) < 1:
-            raise ValueError("%s: frame_hw is one (H, W) for every slot or one per slot, got %r" % (who, frame_hw))
-        sizes.append((int(hw[0]), int(hw[1])))
-    return sizes, per_slot
-
-
-class TrackGraph(object):
+class TrackGraph(_SlotGraph):
     """The array form of ObjectPoseDetector.run_batch(track=True) replayed from CUDA graphs: `slots` video slots with a
     pixel format and a camera each, every slot stepping on every call.  A step is the pre-process, the reset of the slots
     whose video starts, the previous-frame render, the network + decode + PnP and the tracker step, captured once; a call
@@ -379,7 +365,8 @@ class TrackGraph(object):
     association, opt.empty_pre_hm and the heat maps drawn from the tracks follow opt as in run_batch.  Refused (ValueError
     or NotImplementedError; they stay on run_batch): test_scales other than [1], the ground-truth heat maps
     (opt.gt_pre_hm_hmhp / gt_pre_hm_hmhp_first), pre_dets seeding, and idle slots unless idle_slots=True.  Several
-    categories go through MultiCategoryTrackGraph.
+    categories go through MultiCategoryTrackGraph; a detection model through DetectGraph (graph.py), which shares this
+    graph's frame handling, capture and call.
 
     frame_hw: one (H, W) for every slot, or a list of S (H_s, W_s).  camera_matrix: [3,3] for every slot or [S,3,3].
       - One size: a call takes the frames as one array, uint8 [S,H,W,3] for pixel_format "bgr", [S,3H/2,W] for "nv12" /
@@ -410,21 +397,7 @@ class TrackGraph(object):
                                       "or a MultiCategoryTrackGraph")
         self._build(det, slots, frame_hw, camera_matrix, pixel_format, idle_slots)
 
-    def _plan(self, det, S, ih, iw):
-        """(plan, decode parameters, tracker, categories or None) of the graph: a copy of det's plan and weights."""
-        from .engine import Engine, decode_params
-        m = det.model
-        eng = Engine(m._arch(), m.heads, m.head_conv, S, ih, iw, self.device.index, tracking=m.tracking_inputs,
-                     tracking_task_gru=m.use_convGRU and m.tracking_task, precision=m.precision, reuse_activations=True)
-        eng.load_state_dict(m.state_dict())
-        return eng, decode_params(det.opt, test_scale=1.0), Tracker(det.opt, streams=S, device=self.device), None
-
-    def _build(self, det, slots, frame_hw, camera_matrix, pixel_format, idle_slots=False):
-        """Checks, buffers and the captured steps (two, or one per live count with idle_slots); everything that refuses
-        comes before any device work."""
-        from .detector import affine_from_center_scale, camera_per_frame
-        from .engine import check_pixel_format, frame_shape, make_meta
-        who, opt = type(self).__name__, det.opt
+    def _refuse(self, opt, who):
         if not getattr(opt, "tracking_task", False):
             raise ValueError("%s needs a tracking model (opt.tracking_task)" % who)
         if [float(v) for v in getattr(opt, "test_scales", [1.0])] != [1.0]:
@@ -432,65 +405,23 @@ class TrackGraph(object):
         if getattr(opt, "gt_pre_hm_hmhp", False) or getattr(opt, "gt_pre_hm_hmhp_first", False):
             raise NotImplementedError("%s draws the previous-frame heat maps from the tracks; the ground-truth heat maps "
                                       "(opt.gt_pre_hm_hmhp / gt_pre_hm_hmhp_first) run through %s" % (who, self._host_step))
-        S = int(slots)
-        if S < 1:
-            raise ValueError("%s: slots must be >= 1, got %d" % (who, S))
-        sizes, self.per_slot = _frame_sizes(frame_hw, S, who)
-        self.idle_slots = bool(idle_slots)
-        self.pixel_format = check_pixel_format(pixel_format)
-        shapes = [frame_shape(h, w, pixel_format) for h, w in sizes]
-        cams = np.stack(camera_per_frame(camera_matrix, S))
-        if self.per_slot:
-            self.frame_hw, self.frame_shape = sizes, shapes
-        else:
-            self.frame_hw, self.frame_shape = sizes[0], (S,) + shapes[0]
-            sizes = sizes * S
-        self._slot_hw, self._slot_shapes = sizes, shapes if self.per_slot else shapes * S
-        self.L = L = _lib.load()
-        self.slots, self.device = S, torch.device("cuda", torch.cuda.current_device())
-        dev = self.device
-        ih, iw = opt.input_h, opt.input_w
-        self.eng, self.prm, self.tracker, self.categories = self._plan(det, S, ih, iw)
-        M = 1 if self.categories is None else len(self.categories)
-        MS = self.streams = M * S                        # tracker stream m * S + s: slot s of category m
-        # every slot's row of run_batch: its fix_res c, s and meta row and the affine of its size, repeated per category
-        meta, trans = np.zeros((S, _lib.CP_META_DOUBLES), np.float64), np.zeros((S, 6), np.float64)
-        for b, (h, w) in enumerate(sizes):
-            c, sc = np.array([w / 2., h / 2.], np.float32), float(max(h, w))
-            meta[b] = make_meta(1, c, sc, w, h, cams[b]).numpy()[0]
-            trans[b] = affine_from_center_scale(c, sc, iw, ih).reshape(6)
-        self.meta = torch.from_numpy(meta).to(dev)                   # the network's rows, one per frame
+
+    def _steps(self):
+        return (0, 1)                            # the input buffers swapped on odd steps
+
+    def _buffers(self, opt, meta, trans):
+        """The tracker of M x S streams (stream m * S + s: slot s of category m), the previous frames, the rendered heat
+        maps and the outputs; every slot's meta row and affine repeated per category."""
+        S, MS, dev = self.slots, self.streams, self.device
+        M, ih, iw = MS // S, opt.input_h, opt.input_w
+        self.tracker = Tracker(opt, streams=S, device=dev, categories=self.categories)
         self.meta_all = self.meta if M == 1 else torch.from_numpy(np.tile(meta, (M, 1))).to(dev)
         self.trans = torch.from_numpy(np.tile(trans, (M, 1))).to(dev)
         mode = _lib.RENDER_EMPTY if getattr(opt, "empty_pre_hm", False) else _lib.RENDER_TRACKS
         self.modes = torch.full((MS,), mode, dtype=torch.int32, device=dev)
-        self._mean = (ctypes.c_float * 3)(*[float(v) for v in opt.mean])
-        self._std = (ctypes.c_float * 3)(*[float(v) for v in opt.std])
-        self._fmt = {"bgr": _lib.CP_PIX_BGR, "nv12": _lib.CP_PIX_NV12, "i420": _lib.CP_PIX_I420}[self.pixel_format]
-        if self.per_slot or self.idle_slots:                # a frame table (with idle slots: of S equal sizes too)
-            n = [int(np.prod(s)) for s in self._slot_shapes]
-            offs = np.concatenate([[0], np.cumsum(n)[:-1]]).astype(np.int64)
-            self.frames = torch.zeros((int(sum(n)),), dtype=torch.uint8, device=dev)
-            self._slot_frames = [self.frames[o:o + k].view(s) for o, k, s in zip(offs, n, self._slot_shapes)]
-            self.table = torch.zeros((int(L.cp_preprocess_frame_table_bytes(S)),), dtype=torch.uint8, device=dev)
-            hw = np.ascontiguousarray(sizes, np.int32)
-            with torch.cuda.device(dev):
-                _lib.check(L.cp_preprocess_frame_table(self.frames.numel(), offs.ctypes.data_as(ctypes.POINTER(ctypes.c_int64)),
-                                                       hw.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), self._fmt, S, ih,
-                                                       iw, trans.ctypes.data_as(ctypes.POINTER(ctypes.c_double)),
-                                                       _ptr(self.table), _stream()), "cp_preprocess_frame_table")
-        else:
-            self.frames = torch.zeros(self.frame_shape, dtype=torch.uint8, device=dev)
         if self.idle_slots:
-            # one int32 control block per call: start flags [M*S] (per tracker stream), rows [S] (the slot of each live
-            # row), ids [M*S] (the tracker stream of each live row of each category) and inv [M*S] (the row of each
-            # stream, or -1); a step at live count n reads the first n rows and M * n ids
-            self.ctrl = torch.zeros((3 * MS + S,), dtype=torch.int32, device=dev)
-            self.start, self.rows = self.ctrl[:MS], self.ctrl[MS:MS + S]
-            self.ids, self.inv = self.ctrl[MS + S:2 * MS + S], self.ctrl[2 * MS + S:]
             self.store = torch.zeros((S, 3, ih, iw), dtype=torch.float32, device=dev)   # every slot's previous frame
-            # the live rows' meta rows and affines, gathered from the per-slot rows above
-            self.meta_rows = torch.zeros((S, _lib.CP_META_DOUBLES), dtype=torch.float64, device=dev)
+            # the live rows' meta rows and affines of every category, gathered from the per-slot rows above
             self.meta_trk = torch.zeros((MS, _lib.CP_META_DOUBLES), dtype=torch.float64, device=dev)
             self.trans_trk = torch.zeros((MS, 6), dtype=torch.float64, device=dev)
         else:
@@ -508,32 +439,11 @@ class TrackGraph(object):
             self.tracks_rows, self.n_tracks_rows = torch.zeros_like(self.tracks), torch.zeros_like(self.n_tracks)
         out_lead = (S,) if self.categories is None else (M, S)
         self._out = (self.tracks.view(out_lead + self.tracks.shape[1:]), self.n_tracks.view(out_lead))
-        # the captured steps: p = 0, 1 (the input buffers swapped), or with idle slots p = every live count 1..S
-        steps = range(1, S + 1) if self.idle_slots else (0, 1)
-        side = torch.cuda.Stream(device=dev)
-        side.wait_stream(torch.cuda.current_stream(dev))
-        with torch.cuda.stream(side):            # warm-up outside the capture; the first call resets every slot
-            for p in steps:
-                if self.idle_slots:
-                    self.ctrl.copy_(torch.from_numpy(self._control(list(range(p)), np.ones(S, np.int32))))
-                self._step(p)
-        torch.cuda.current_stream(dev).wait_stream(side)
-        torch.cuda.synchronize(dev)
+
+    def _warmed(self):
         if self.idle_slots:                      # the warm-ups stepped every stream: start from nothing
             self.tracker.reset()
-            torch.cuda.synchronize(dev)
-        self.graphs, pool = [], None
-        for p in steps:
-            g = torch.cuda.CUDAGraph(keep_graph=True)
-            with torch.cuda.graph(g, pool=pool):
-                self._step(p)
-            g.instantiate()
-            self.graphs.append(g)
-            if self.idle_slots:                  # the S graphs replay in turn on one stream: one memory pool
-                pool = g.pool()
-        self._parity = 0
-        self._fresh = True
-        self._started = [False] * S
+            torch.cuda.synchronize(self.device)
 
     def _step(self, p):
         """The launches of one step: network input in x[p], previous frames in x[1 - p]; with idle slots, the step of p
@@ -541,18 +451,10 @@ class TrackGraph(object):
         if self.idle_slots:
             return self._step_rows(p)
         L, st, h = self.L, _stream(), self.tracker._h
-        S, MS, (ih, iw), cur, prev = self.slots, self.streams, self.x[p].shape[2:], self.x[p], self.x[1 - p]
+        MS, (ih, iw), cur, prev = self.streams, self.x[p].shape[2:], self.x[p], self.x[1 - p]
         with torch.cuda.device(self.device):
             _lib.check(L.cp_tracker_reset_dev(h, MS, _ptr(self.start), st), "cp_tracker_reset_dev")
-            if self.per_slot:
-                _lib.check(L.cp_preprocess_slots_ragged_dev(_ptr(self.frames), _ptr(self.table), self._fmt, S, ih, iw,
-                                                            self._mean, self._std, _ptr(self.start), _ptr(cur),
-                                                            _ptr(prev), st), "cp_preprocess_slots_ragged_dev")
-            else:
-                H, W = self.frame_hw
-                _lib.check(L.cp_preprocess_slots_dev(_ptr(self.frames), self._fmt, S, H, W, ih, iw, None, self._mean,
-                                                     self._std, _ptr(self.start), _ptr(cur), _ptr(prev), st),
-                           "cp_preprocess_slots_dev")
+            self._preprocess(cur, self.start, prev)
             _lib.check(L.cp_tracker_render_dev(h, MS, _ptr(self.meta_all), _ptr(self.trans), ih, iw, _ptr(self.modes),
                                                _ptr(self.pre_hm), _ptr(self.pre_hm_hp), st), "cp_tracker_render_dev")
             self.eng.infer(cur, self.meta, self.prm, prev, self.pre_hm, self.pre_hm_hp, poses=self.poses,
@@ -565,26 +467,17 @@ class TrackGraph(object):
         the previous-frame exchange, the gathers of the live rows' meta rows and affines, the render, the network at
         batch n, the tracker step over the live streams and the scatter of their tracks to the slots (zeros for idle
         slots).  Which slots are live is data in the control block; n fixes the shapes."""
-        L, st, h, S, MS = self.L, _stream(), self.tracker._h, self.slots, self.streams
-        M, cur, prev = MS // S, self.x[0], self.x[1]
-        (ih, iw), Mn, lead = cur.shape[2:], M * n, self.eng._lead(n)
-
-        def view(t):                          # the first rows of a buffer of the plan's lead axes, as lead(n) + inner
-            inner = tuple(t.shape[len(lead):])
-            return t.view(-1)[:int(np.prod(lead + inner))].view(lead + inner)
-
-        def gather(src, dst, rows, m):
-            _lib.check(L.cp_gather_rows_dev(_ptr(src), _ptr(dst), src[0].numel() * src.element_size(), rows, _ptr(m),
-                                            st), "cp_gather_rows_dev")
-        pre_hm, pre_hm_hp, poses, n_valid = view(self.pre_hm), view(self.pre_hm_hp), view(self.poses), view(self.n_valid)
+        L, st, h, MS = self.L, _stream(), self.tracker._h, self.streams
+        M, cur, prev = MS // self.slots, self.x[0], self.x[1]
+        (ih, iw), Mn = cur.shape[2:], M * n
+        pre_hm, pre_hm_hp = self._rows_view(self.pre_hm, n), self._rows_view(self.pre_hm_hp, n)
+        poses, n_valid = self._rows_view(self.poses, n), self._rows_view(self.n_valid, n)
         with torch.cuda.device(self.device):
             _lib.check(L.cp_tracker_reset_dev(h, MS, _ptr(self.start), st), "cp_tracker_reset_dev")
-            _lib.check(L.cp_preprocess_slots_rows_dev(_ptr(self.frames), _ptr(self.table), self._fmt, _ptr(self.rows), n,
-                                                      ih, iw, self._mean, self._std, _ptr(self.start), _ptr(self.store),
-                                                      _ptr(cur), _ptr(prev), st), "cp_preprocess_slots_rows_dev")
-            gather(self.meta, self.meta_rows, n, self.rows)
-            gather(self.meta_all, self.meta_trk, Mn, self.ids)
-            gather(self.trans, self.trans_trk, Mn, self.ids)
+            self._preprocess_rows(n, cur, self.start, self.store, prev)
+            self._gather(self.meta, self.meta_rows, n, self.rows)
+            self._gather(self.meta_all, self.meta_trk, Mn, self.ids)
+            self._gather(self.trans, self.trans_trk, Mn, self.ids)
             _lib.check(L.cp_tracker_render_dev2(h, Mn, _ptr(self.ids), _ptr(self.meta_trk), _ptr(self.trans_trk), ih, iw,
                                                 _ptr(self.modes), _ptr(pre_hm), _ptr(pre_hm_hp), st),
                        "cp_tracker_render_dev2")
@@ -593,71 +486,8 @@ class TrackGraph(object):
             _lib.check(L.cp_tracker_step_dev(h, Mn, _ptr(self.ids), _ptr(poses), _ptr(n_valid), poses.shape[-2],
                                              _ptr(self.meta_trk), _ptr(self.tracks_rows), _ptr(self.n_tracks_rows), st),
                        "cp_tracker_step_dev")
-            gather(self.tracks_rows, self.tracks, MS, self.inv)
-            gather(self.n_tracks_rows.view(MS, 1), self.n_tracks.view(MS, 1), MS, self.inv)
-
-    def _control(self, live, start):
-        """The control block of a step over the slots `live` (in row order), start: int32 [S] (slots that start)."""
-        S, MS = self.slots, self.streams
-        M, n = MS // S, len(live)
-        rows = np.zeros(S, np.int32)
-        rows[:n] = live
-        ids = np.zeros(MS, np.int32)
-        ids[:M * n] = [m * S + i for m in range(M) for i in live]
-        inv = np.full(MS, -1, np.int32)
-        inv[ids[:M * n]] = np.arange(M * n, dtype=np.int32)
-        return np.concatenate([np.tile(start, M), rows, ids, inv]).astype(np.int32)
-
-    def reset(self):
-        """Forget every slot's tracks and previous frame: the next call starts a video in every slot (with idle slots:
-        each slot's next live frame starts its video)."""
-        self._fresh = True
-        self._started = [False] * self.slots
-
-    def _frames(self, frames):
-        """The frames of one call, checked against the slots' shapes: one tensor, or one per slot (with idle slots: one
-        per slot, None for an idle one)."""
-        who = type(self).__name__
-        if self.idle_slots and not isinstance(frames, (list, tuple)):
-            if self.per_slot or not (torch.is_tensor(frames) or isinstance(frames, np.ndarray)):
-                raise ValueError("%s was built with idle slots: frames is a list of %d frames (None for an idle slot)%s, "
-                                 "got %s" % (who, self.slots, "" if self.per_slot else " or one uint8 %s array"
-                                             % list(self.frame_shape), type(frames).__name__))
-            frames = torch.from_numpy(frames) if isinstance(frames, np.ndarray) else frames
-            if frames.dtype != torch.uint8 or tuple(frames.shape) != self.frame_shape:
-                raise ValueError("%s: frames must be uint8 %s (%s), got %s %s" % (who, list(self.frame_shape),
-                                                                                 self.pixel_format, frames.dtype,
-                                                                                 tuple(frames.shape)))
-            return list(frames)                         # every slot live
-        if not self.per_slot and not self.idle_slots:
-            if isinstance(frames, np.ndarray):
-                frames = torch.from_numpy(frames)
-            if not torch.is_tensor(frames) or frames.dtype != torch.uint8 or tuple(frames.shape) != self.frame_shape:
-                what = ("%s %s" % (frames.dtype, tuple(frames.shape))) if torch.is_tensor(frames) else type(frames).__name__
-                raise ValueError("%s steps every slot at one frame size: frames must be uint8 %s (%s), got %s; idle "
-                                 "slots and mixed sizes run through %s or a %s built with one frame_hw per slot"
-                                 % (who, list(self.frame_shape), self.pixel_format, what, self._host_list, who))
-            return [frames]
-        if not isinstance(frames, (list, tuple)) or len(frames) != self.slots:
-            what = "%d frames" % len(frames) if isinstance(frames, (list, tuple)) else type(frames).__name__
-            raise ValueError("%s was built with %s: frames is a list of %d frames, got %s"
-                             % (who, "idle slots" if self.idle_slots else "one frame_hw per slot", self.slots, what))
-        out = []
-        for b, f in enumerate(frames):
-            if f is None:
-                if self.idle_slots:
-                    out.append(None)
-                    continue
-                raise ValueError("%s steps every slot: slot %d is idle; idle slots run through %s"
-                                 % (who, b, self._host_list))
-            if isinstance(f, np.ndarray):
-                f = torch.from_numpy(f)
-            if not torch.is_tensor(f) or f.dtype != torch.uint8 or tuple(f.shape) != self._slot_shapes[b]:
-                what = ("%s %s" % (f.dtype, tuple(f.shape))) if torch.is_tensor(f) else type(f).__name__
-                raise ValueError("%s: slot %d takes uint8 %s frames (%s, frame_hw %s), got %s"
-                                 % (who, b, list(self._slot_shapes[b]), self.pixel_format, self._slot_hw[b], what))
-            out.append(f)
-        return out
+            self._gather(self.tracks_rows, self.tracks, MS, self.inv)
+            self._gather(self.n_tracks_rows.view(MS, 1), self.n_tracks.view(MS, 1), MS, self.inv)
 
     def __call__(self, frames, new_video=None, pre_dets=None):
         """The next frame of every slot -> (tracks [S,T,320], n_tracks [S]) ([M,S,...] in MultiCategoryTrackGraph):
@@ -674,40 +504,7 @@ class TrackGraph(object):
             if len(new_video) != self.slots:
                 raise ValueError("%s: %d new_video entries for %d slots" % (who, len(new_video), self.slots))
             start |= np.array(new_video, np.int32)
-        if self.idle_slots:
-            return self._call_rows(frames, start)
-        start = np.tile(start, self.streams // self.slots)       # one flag per tracker stream, the same in every category
-        with torch.cuda.device(self.device):
-            for dst, f in zip(self._slot_frames if self.per_slot else [self.frames], frames):
-                dst.copy_(f, non_blocking=True)
-            # a pageable source: staged before copy_ returns, without waiting for the device
-            self.start.copy_(torch.from_numpy(start), non_blocking=True)
-            self.graphs[self._parity].replay()
-        self._parity ^= 1
-        self._fresh = False
-        return self._out
-
-    def _call_rows(self, frames, start):
-        """A call with idle slots: frames[i] None idles slot i.  A live slot starts its video when it has not started
-        since the graph was built or reset, or when start[i] (new_video); an idle slot is not stepped and keeps its
-        tracks and previous frame.  Copies the live frames and the control block, then replays the graph of the live
-        count; with no live slot, zeros the outputs and launches no graph."""
-        live = [i for i, f in enumerate(frames) if f is not None]
-        with torch.cuda.device(self.device):
-            if not live:
-                self.tracks.zero_()
-                self.n_tracks.zero_()
-                return self._out
-            start = np.array([i in live and (bool(start[i]) or not self._started[i]) for i in range(self.slots)], np.int32)
-            for i in live:
-                self._slot_frames[i].copy_(frames[i], non_blocking=True)
-            # a pageable source: staged before copy_ returns, without waiting for the device
-            self.ctrl.copy_(torch.from_numpy(self._control(live, start)), non_blocking=True)
-            self.graphs[len(live) - 1].replay()
-        for i in live:
-            self._started[i] = True
-        self._fresh = False
-        return self._out
+        return self._replay(frames, start)
 
 
 class MultiCategoryTrackGraph(TrackGraph):
@@ -736,14 +533,3 @@ class MultiCategoryTrackGraph(TrackGraph):
             raise NotImplementedError("MultiCategoryTrackGraph takes a MultiCategoryTracker; one category's "
                                       "ObjectPoseDetector goes to TrackGraph")
         self._build(trk, slots, frame_hw, camera_matrix, pixel_format, idle_slots)
-
-    def _plan(self, trk, S, ih, iw):
-        from .engine import Engine
-        c, M = trk._plan_cfg, len(trk.categories)
-        eng = Engine(c["arch"], c["heads"], c["head_conv"], S, ih, iw, self.device.index, tracking=c["tracking"],
-                     tracking_task_gru=c["tracking_task_gru"], precision=c["precision"], models=M,
-                     reuse_activations=True)
-        for m, sd in enumerate(trk._weights):
-            eng.load_state_dict(sd, model=m)
-        prm = list(trk._prms) if M > 1 else trk._prms[0]
-        return eng, prm, Tracker(trk.opt, streams=S, device=self.device, categories=trk.categories), list(trk.categories)
