@@ -5,11 +5,14 @@
 //   cp_preprocess     -- batched uint8 HWC frames -> normalised fp32 NCHW network input
 //                        (reference: detectors/base_detector.py:91-148, fix_res branch); cp_preprocess_ragged does
 //                        the same for frames of different sizes in one launch, and cp_preprocess_yuv420 for NV12 / I420
-//                        frames (the colour conversion of cv2.cvtColor fused into the warp's tap fetch);
+//                        frames (the colour conversion of cv2.cvtColor fused into the warp's tap fetch), and
+//                        cp_preprocess_formats for the camera formats (RGB24, RGBA, BGRA, YUYV, UYVY), one per frame;
 //                        cp_preprocess_slots_dev is the graph-safe form for one tracking step of a uniform batch, and
 //                        cp_preprocess_slots_ragged_dev (over a cp_preprocess_frame_table) that of slots of mixed sizes,
-//                        cp_preprocess_slots_rows_dev that of the live slots of a step with idle slots;
+//                        cp_preprocess_slots_rows_dev that of the live slots of a step with idle slots (a table may hold
+//                        one format per frame: cp_preprocess_frame_table_formats, launched as CP_PIX_PER_FRAME);
 //   cp_gather_rows_dev -- a row gather through a device map, the graph-safe reordering of per-slot rows.
+#include <type_traits>
 #include <vector>
 
 #include "common.cuh"
@@ -98,6 +101,19 @@ __device__ __forceinline__ void warp_pixel(const uint8_t* __restrict__ img, floa
   warp_walk(BgrFetch{img, sw}, out, plane, sh, sw, x, y, W, mean, stdv);
 }
 
+// interleaved 8-bit pixels of kBytes (3 or 4) bytes with B, G and R at bytes kB, kG and kR: RGB24 <2, 1, 0>, RGBA
+// <2, 1, 0> and BGRA <0, 1, 2> (cv2.cvtColor COLOR_RGB2BGR / COLOR_RGBA2BGR / COLOR_BGRA2BGR are these channel
+// selects; alpha is never read).  Every channel is read where it is used, as in BgrFetch.
+template <int kBytes, int kB, int kG, int kR>
+struct PackedFetch {
+  const uint8_t* __restrict__ img;
+  int sw;
+  __device__ __forceinline__ void taps(int, int, bool, bool, bool, bool) {}
+  __device__ __forceinline__ int operator()(int, int yy, int xx, int c) const {
+    return img[((size_t)yy * sw + xx) * kBytes + (c == 0 ? kB : (c == 1 ? kG : kR))];
+  }
+};
+
 // YUV 4:2:0 [3 sh / 2, sw] (sh, sw even) converted per tap to the BGR that cv2.cvtColor(COLOR_YUV2BGR_NV12 / _I420)
 // gives, restated bit for bit (OpenCV color_yuv.simd.hpp, yuv42x_to_rgb8 for 8-bit: BT.601 limited range in 20-bit
 // fixed point, no chroma interpolation; tests/yuv_ref.py yuv420_to_bgr, pinned against cv2 on every (Y, U, V)):
@@ -141,6 +157,63 @@ struct Yuv420Fetch {
   }
 };
 
+// packed YUV 4:2:2 [sh, sw, 2] (sw even): the pixel pair (xx & ~1, xx | 1) of a row is 4 bytes, Y0 U Y1 V (YUYV) or
+// U Y0 V Y1 (UYVY), one U, V for both pixels.  cv2.cvtColor(COLOR_YUV2BGR_YUYV / _UYVY) converts each pixel with the
+// arithmetic of Yuv420Fetch and no chroma interpolation (tests/yuv422_ref.py, pinned against cv2 on every (Y, U, V)).
+// Every in-frame tap is read and converted once, before the first channel is written; taps outside stay BGR 0.
+template <int kFormat>
+struct Yuv422Fetch {
+  const uint8_t* __restrict__ img;
+  int sw;
+  int yv[4], u[4], v[4];
+  __device__ __forceinline__ void taps(int iy, int ix, bool in00, bool in01, bool in10, bool in11) {
+    const bool in[4] = {in00, in01, in10, in11};
+    constexpr int kY = kFormat == CP_PIX_YUYV422 ? 0 : 1, kU = 1 - kY;    // byte of Y0 and of U in a pair
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      yv[k] = u[k] = v[k] = 0;
+      if (!in[k]) continue;
+      const int yy = iy + (k >> 1), xx = ix + (k & 1);
+      const uint8_t* __restrict__ pair = img + ((size_t)yy * sw + (xx & ~1)) * 2;
+      yv[k] = max((int)pair[kY + 2 * (xx & 1)] - 16, 0) * 1220542 + (1 << 19);
+      u[k] = pair[kU] - 128;
+      v[k] = pair[kU + 2] - 128;
+    }
+  }
+  // the conversion of Yuv420Fetch (written out again there, so that its instances compile as they did before 4:2:2)
+  __device__ __forceinline__ int operator()(int k, int, int, int c) const {
+    const int t = c == 0 ? yv[k] + 2116026 * u[k]
+                         : (c == 1 ? yv[k] - 852492 * v[k] - 409993 * u[k] : yv[k] + 1673527 * v[k]);
+    return max(0, min(255, t >> 20));
+  }
+};
+
+// The bytes of one sh x sw frame in a cp_pixel_format (0 for CP_PIX_PER_FRAME or an unknown value).
+__host__ __device__ constexpr size_t frame_bytes(int format, size_t sh, size_t sw) {
+  return format == CP_PIX_NV12 || format == CP_PIX_I420     ? sh * sw * 3 / 2
+         : format == CP_PIX_BGR || format == CP_PIX_RGB24    ? sh * sw * 3
+         : format == CP_PIX_RGBA || format == CP_PIX_BGRA    ? sh * sw * 4
+         : format == CP_PIX_YUYV422 || format == CP_PIX_UYVY422 ? sh * sw * 2
+                                                             : 0;
+}
+
+// the tap fetch of a frame at img in format kFormat
+template <int kFormat>
+__device__ __forceinline__ auto make_fetch(const uint8_t* __restrict__ img, int sh, int sw) {
+  if constexpr (kFormat == CP_PIX_BGR)
+    return BgrFetch{img, sw};
+  else if constexpr (kFormat == CP_PIX_NV12 || kFormat == CP_PIX_I420)
+    return Yuv420Fetch<kFormat>{img, sh, sw};
+  else if constexpr (kFormat == CP_PIX_RGB24)
+    return PackedFetch<3, 2, 1, 0>{img, sw};
+  else if constexpr (kFormat == CP_PIX_RGBA)
+    return PackedFetch<4, 2, 1, 0>{img, sw};
+  else if constexpr (kFormat == CP_PIX_BGRA)
+    return PackedFetch<4, 0, 1, 2>{img, sw};
+  else
+    return Yuv422Fetch<kFormat>{img, sw};
+}
+
 __global__ void preprocess_kernel(const uint8_t* __restrict__ frames, float* __restrict__ out, int B, int sh,
                                   int sw, int dh, int dw, const WarpM W, float m0, float m1, float m2, float s0, float s1,
                                   float s2) {
@@ -163,6 +236,32 @@ struct RaggedFrame {
   long long offset;     // bytes into the packed frame buffer
   int sh, sw;
 };
+
+// A table of per-frame formats (launched as CP_PIX_PER_FRAME) keeps frame b's cp_pixel_format in the top byte of its
+// offset, so its entries are RaggedFrames of the same 64 bytes and a walk still reads one entry per output pixel.
+constexpr int kFormatShift = 56;
+constexpr long long kOffsetMask = (1ll << kFormatShift) - 1;
+
+// walk(fetch) with the tap fetch of frame f in format kFormat; CP_PIX_PER_FRAME: in the format its entry holds.  The
+// format is uniform across a frame, so the branch costs a frame's threads nothing but the switch.
+template <int kFormat, class Walk>
+__device__ __forceinline__ void frame_walk(const uint8_t* __restrict__ frames, const RaggedFrame& f, Walk walk) {
+  if constexpr (kFormat != CP_PIX_PER_FRAME) {
+    walk(make_fetch<kFormat>(frames + f.offset, f.sh, f.sw));
+  } else {
+    const uint8_t* img = frames + (f.offset & kOffsetMask);
+    switch ((int)(f.offset >> kFormatShift)) {
+      case CP_PIX_NV12: walk(make_fetch<CP_PIX_NV12>(img, f.sh, f.sw)); break;
+      case CP_PIX_I420: walk(make_fetch<CP_PIX_I420>(img, f.sh, f.sw)); break;
+      case CP_PIX_BGR: walk(make_fetch<CP_PIX_BGR>(img, f.sh, f.sw)); break;
+      case CP_PIX_RGB24: walk(make_fetch<CP_PIX_RGB24>(img, f.sh, f.sw)); break;
+      case CP_PIX_RGBA: walk(make_fetch<CP_PIX_RGBA>(img, f.sh, f.sw)); break;
+      case CP_PIX_BGRA: walk(make_fetch<CP_PIX_BGRA>(img, f.sh, f.sw)); break;
+      case CP_PIX_YUYV422: walk(make_fetch<CP_PIX_YUYV422>(img, f.sh, f.sw)); break;
+      default: walk(make_fetch<CP_PIX_UYVY422>(img, f.sh, f.sw)); break;
+    }
+  }
+}
 
 __global__ void preprocess_ragged_kernel(const uint8_t* __restrict__ frames, const RaggedFrame* __restrict__ fr,
                                          float* __restrict__ out, int B, int dh, int dw, float m0, float m1, float m2,
@@ -209,7 +308,9 @@ __global__ void preprocess_slots_kernel(const uint8_t* __restrict__ frames, floa
                                         int dh, int dw, const WarpM W, float m0, float m1, float m2, float s0, float s1,
                                         float s2) {
   const size_t total = (size_t)B * dh * dw, plane = (size_t)dh * dw;
-  const size_t bytes = kFormat == CP_PIX_BGR ? (size_t)sh * sw * 3 : (size_t)sh * sw * 3 / 2;
+  const size_t bytes = kFormat == CP_PIX_BGR                                 ? (size_t)sh * sw * 3
+                       : kFormat == CP_PIX_NV12 || kFormat == CP_PIX_I420 ? (size_t)sh * sw * 3 / 2
+                                                                          : frame_bytes(kFormat, sh, sw);
   const float mean[3] = {m0, m1, m2};
   const float stdv[3] = {s0, s1, s2};
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
@@ -220,17 +321,23 @@ __global__ void preprocess_slots_kernel(const uint8_t* __restrict__ frames, floa
     const size_t o = (((size_t)n * 3) * dh + y) * dw + x;
     float* twin = start && start[n] ? prev + o : nullptr;
     const uint8_t* img = frames + n * bytes;
-    if constexpr (kFormat == CP_PIX_BGR)
+    if constexpr (kFormat == CP_PIX_BGR) {
       warp_walk<BgrFetch, true>(BgrFetch{img, sw}, out + o, plane, sh, sw, x, y, W, mean, stdv, twin);
-    else
+    } else if constexpr (kFormat == CP_PIX_NV12 || kFormat == CP_PIX_I420) {
       warp_walk<Yuv420Fetch<kFormat>, true>(Yuv420Fetch<kFormat>{img, sh, sw}, out + o, plane, sh, sw, x, y, W, mean,
                                             stdv, twin);
+    } else {
+      auto px = make_fetch<kFormat>(img, sh, sw);
+      warp_walk<decltype(px), true>(px, out + o, plane, sh, sw, x, y, W, mean, stdv, twin);
+    }
   }
 }
 
 // The frames of one tracking step when the slots differ in size: the ragged walk of preprocess_ragged_kernel /
 // preprocess_yuv420_kernel over a frame table `fr` in device memory (built once, cp_preprocess_frame_table), with the
 // start-flag twin write of preprocess_slots_kernel.  Nothing is read from the host, so a captured launch replays unchanged.
+// Without start flags it is also the ragged launch of the formats preprocess_ragged_kernel / _yuv420_kernel do not read,
+// and of a batch of per-frame formats (kFormat CP_PIX_PER_FRAME).
 template <int kFormat>
 __global__ void preprocess_slots_ragged_kernel(const uint8_t* __restrict__ frames, const RaggedFrame* __restrict__ fr,
                                                float* __restrict__ out, float* __restrict__ prev,
@@ -250,9 +357,13 @@ __global__ void preprocess_slots_ragged_kernel(const uint8_t* __restrict__ frame
     if constexpr (kFormat == CP_PIX_BGR)
       warp_walk<BgrFetch, true>(BgrFetch{frames + f.offset, f.sw}, out + o, plane, f.sh, f.sw, x, y, f.W, mean, stdv,
                                 twin);
-    else
+    else if constexpr (kFormat == CP_PIX_NV12 || kFormat == CP_PIX_I420)
       warp_walk<Yuv420Fetch<kFormat>, true>(Yuv420Fetch<kFormat>{frames + f.offset, f.sh, f.sw}, out + o, plane, f.sh,
                                             f.sw, x, y, f.W, mean, stdv, twin);
+    else
+      frame_walk<kFormat>(frames, f, [&](auto px) {
+        warp_walk<decltype(px), true>(px, out + o, plane, f.sh, f.sw, x, y, f.W, mean, stdv, twin);
+      });
   }
 }
 
@@ -284,9 +395,13 @@ __global__ void preprocess_slots_rows_kernel(const uint8_t* __restrict__ frames,
     if constexpr (kFormat == CP_PIX_BGR)
       warp_walk<BgrFetch, true, true>(BgrFetch{frames + f.offset, f.sw}, out + o, plane, f.sh, f.sw, x, y, f.W, mean,
                                       stdv, twin, keep, st);
-    else
+    else if constexpr (kFormat == CP_PIX_NV12 || kFormat == CP_PIX_I420)
       warp_walk<Yuv420Fetch<kFormat>, true, true>(Yuv420Fetch<kFormat>{frames + f.offset, f.sh, f.sw}, out + o, plane,
                                                   f.sh, f.sw, x, y, f.W, mean, stdv, twin, keep, st);
+    else
+      frame_walk<kFormat>(frames, f, [&](auto px) {
+        warp_walk<decltype(px), true, true>(px, out + o, plane, f.sh, f.sw, x, y, f.W, mean, stdv, twin, keep, st);
+      });
   }
 }
 
@@ -344,18 +459,53 @@ int preprocess_blocks(size_t total) {
   return blocks;
 }
 
-// The per-frame parameters of a ragged batch, checked against the packed buffer before any work is enqueued.  `yuv`:
-// the frames are YUV 4:2:0 (even sizes, h * w * 3 / 2 bytes each), else BGR (h * w * 3 bytes).
+bool is_yuv420(int format) { return format == CP_PIX_NV12 || format == CP_PIX_I420; }
+bool is_yuv422(int format) { return format == CP_PIX_YUYV422 || format == CP_PIX_UYVY422; }
+bool known_format(int format) {
+  return format == CP_PIX_BGR || is_yuv420(format) || format == CP_PIX_RGB24 || format == CP_PIX_RGBA ||
+         format == CP_PIX_BGRA || is_yuv422(format);
+}
+
+// f(std::integral_constant<int, format>) for a format chosen at run time (one of cp_pixel_format; with kPerFrame also
+// CP_PIX_PER_FRAME), already checked
+template <bool kPerFrame, class F>
+void with_format(int format, F f) {
+  switch (format) {
+    case CP_PIX_NV12: f(std::integral_constant<int, CP_PIX_NV12>{}); break;
+    case CP_PIX_I420: f(std::integral_constant<int, CP_PIX_I420>{}); break;
+    case CP_PIX_BGR: f(std::integral_constant<int, CP_PIX_BGR>{}); break;
+    case CP_PIX_RGB24: f(std::integral_constant<int, CP_PIX_RGB24>{}); break;
+    case CP_PIX_RGBA: f(std::integral_constant<int, CP_PIX_RGBA>{}); break;
+    case CP_PIX_BGRA: f(std::integral_constant<int, CP_PIX_BGRA>{}); break;
+    case CP_PIX_YUYV422: f(std::integral_constant<int, CP_PIX_YUYV422>{}); break;
+    case CP_PIX_UYVY422: f(std::integral_constant<int, CP_PIX_UYVY422>{}); break;
+    default:
+      if constexpr (kPerFrame) f(std::integral_constant<int, CP_PIX_PER_FRAME>{});
+  }
+}
+
+// The per-frame parameters of a ragged batch, checked against the packed buffer before any work is enqueued.  Frame b
+// is in `format` (a cp_pixel_format), or in formats[b] when `formats` (host int32 [B]) is given; then each entry's
+// offset also carries the frame's format (kFormatShift), for a CP_PIX_PER_FRAME launch.
 int ragged_frames(const char* who, int64_t frames_bytes, const int64_t* offsets, const int32_t* src_hw, int B, int dst_h,
-                  int dst_w, const double* trans_input, bool yuv, std::vector<RaggedFrame>& fr) {
+                  int dst_w, const double* trans_input, int format, const int32_t* formats, std::vector<RaggedFrame>& fr) {
   const std::string w0 = who;
+  if (formats && frames_bytes > kOffsetMask)
+    return fail(CP_ERR_INVALID, w0 + ": a " + std::to_string(frames_bytes) + "-byte buffer is too large for per-frame "
+                                "formats");
   fr.resize(B);
   for (int b = 0; b < B; ++b) {
     const int h = src_hw[2 * b], w = src_hw[2 * b + 1];
-    if (h <= 0 || w <= 0 || (yuv && (h % 2 || w % 2)))
+    const int fmt = formats ? formats[b] : format;
+    if (!known_format(fmt))
+      return fail(CP_ERR_INVALID, w0 + ": frame " + std::to_string(b) + " has unknown pixel format " +
+                                      std::to_string(fmt));
+    const bool yuv = is_yuv420(fmt);
+    if (h <= 0 || w <= 0 || (yuv && (h % 2 || w % 2)) || (is_yuv422(fmt) && w % 2))
       return fail(CP_ERR_INVALID, w0 + ": frame " + std::to_string(b) + " has size " + std::to_string(h) + " x " +
-                                      std::to_string(w) + (yuv ? " (YUV 4:2:0 needs even sizes)" : ""));
-    const int64_t bytes = yuv ? (int64_t)h * w * 3 / 2 : (int64_t)h * w * 3;
+                                      std::to_string(w) + (yuv ? " (YUV 4:2:0 needs even sizes)"
+                                                               : is_yuv422(fmt) ? " (YUV 4:2:2 needs an even width)" : ""));
+    const int64_t bytes = (int64_t)frame_bytes(fmt, h, w);
     if (offsets[b] < 0 || offsets[b] > frames_bytes || bytes > frames_bytes - offsets[b])
       return fail(CP_ERR_INVALID, w0 + ": frame " + std::to_string(b) + " (" + std::to_string(h) + " x " +
                                       std::to_string(w) + " at byte " + std::to_string(offsets[b]) +
@@ -367,7 +517,7 @@ int ragged_frames(const char* who, int64_t frames_bytes, const int64_t* offsets,
       fix_res_affine(h, w, dst_h, dst_w, T);
     }
     fr[b].W = invert_affine(T);
-    fr[b].offset = offsets[b];
+    fr[b].offset = formats ? offsets[b] | (long long)fmt << kFormatShift : offsets[b];
     fr[b].sh = h;
     fr[b].sw = w;
   }
@@ -395,6 +545,21 @@ int launch_ragged(const char* who, const char* kernel, const std::vector<RaggedF
   }
   cudaFreeAsync(dfr, s);
   return rc;
+}
+
+// checks a frame table's frames (ragged_frames) and writes it to `table`
+int upload_frame_table(const char* who, int64_t frames_bytes, const int64_t* offsets, const int32_t* src_hw, int format,
+                       const int32_t* formats, int B, int dst_h, int dst_w, const double* trans_input, void* table,
+                       void* stream_) {
+  std::vector<RaggedFrame> fr;
+  int rc = ragged_frames(who, frames_bytes, offsets, src_hw, B, dst_h, dst_w, trans_input, format, formats, fr);
+  if (rc) return rc;
+  // a build-time call: the copy is complete when it returns, so `fr` may go out of scope
+  cudaStream_t s = (cudaStream_t)stream_;
+  cudaError_t e = cudaMemcpyAsync(table, fr.data(), sizeof(RaggedFrame) * B, cudaMemcpyHostToDevice, s);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+  if (e != cudaSuccess) return fail(CP_ERR_CUDA, std::string(who) + ": table upload: " + cudaGetErrorString(e));
+  return CP_OK;
 }
 
 }  // namespace
@@ -566,7 +731,8 @@ int cp_preprocess_ragged(const uint8_t* frames, int64_t frames_bytes, const int6
   if (!frames || !offsets || !src_hw || !out || !mean || !stdv) return fail(CP_ERR_INVALID, "cp_preprocess_ragged: null argument");
   if (B <= 0 || dst_h <= 0 || dst_w <= 0 || frames_bytes <= 0) return fail(CP_ERR_INVALID, "cp_preprocess_ragged: bad shape");
   std::vector<RaggedFrame> fr;
-  int rc = ragged_frames("cp_preprocess_ragged", frames_bytes, offsets, src_hw, B, dst_h, dst_w, trans_input, false, fr);
+  int rc = ragged_frames("cp_preprocess_ragged", frames_bytes, offsets, src_hw, B, dst_h, dst_w, trans_input, CP_PIX_BGR,
+                         nullptr, fr);
   if (rc) return rc;
   cudaStream_t s = (cudaStream_t)stream_;
   return launch_ragged("cp_preprocess_ragged", "preprocess_ragged_kernel", fr, s, [&](const RaggedFrame* dfr) {
@@ -583,7 +749,8 @@ int cp_preprocess_yuv420(const uint8_t* frames, int64_t frames_bytes, const int6
   if (format != CP_PIX_NV12 && format != CP_PIX_I420)
     return fail(CP_ERR_INVALID, "cp_preprocess_yuv420: unknown pixel format " + std::to_string(format));
   std::vector<RaggedFrame> fr;
-  int rc = ragged_frames("cp_preprocess_yuv420", frames_bytes, offsets, src_hw, B, dst_h, dst_w, trans_input, true, fr);
+  int rc = ragged_frames("cp_preprocess_yuv420", frames_bytes, offsets, src_hw, B, dst_h, dst_w, trans_input, format,
+                         nullptr, fr);
   if (rc) return rc;
   cudaStream_t s = (cudaStream_t)stream_;
   return launch_ragged("cp_preprocess_yuv420", "preprocess_yuv420_kernel", fr, s, [&](const RaggedFrame* dfr) {
@@ -597,17 +764,43 @@ int cp_preprocess_yuv420(const uint8_t* frames, int64_t frames_bytes, const int6
   });
 }
 
+int cp_preprocess_formats(const uint8_t* frames, int64_t frames_bytes, const int64_t* offsets, const int32_t* src_hw,
+                          const int32_t* formats, float* out, int32_t B, int32_t dst_h, int32_t dst_w,
+                          const double* trans_input, const float mean[3], const float stdv[3], void* stream_) {
+  if (!frames || !offsets || !src_hw || !formats || !out || !mean || !stdv)
+    return fail(CP_ERR_INVALID, "cp_preprocess_formats: null argument");
+  if (B <= 0 || dst_h <= 0 || dst_w <= 0 || frames_bytes <= 0) return fail(CP_ERR_INVALID, "cp_preprocess_formats: bad shape");
+  int format = formats[0];
+  for (int b = 1; b < B; ++b)
+    if (formats[b] != format) format = CP_PIX_PER_FRAME;
+  std::vector<RaggedFrame> fr;
+  int rc = ragged_frames("cp_preprocess_formats", frames_bytes, offsets, src_hw, B, dst_h, dst_w, trans_input, format,
+                         format == CP_PIX_PER_FRAME ? formats : nullptr, fr);
+  if (rc) return rc;
+  cudaStream_t s = (cudaStream_t)stream_;
+  // the walk of the graph-safe ragged launch without start flags: one instance per format, or the per-frame one
+  return launch_ragged("cp_preprocess_formats", "preprocess_slots_ragged_kernel", fr, s, [&](const RaggedFrame* dfr) {
+    with_format<true>(format, [&](auto k) {
+      preprocess_slots_ragged_kernel<decltype(k)::value><<<preprocess_blocks((size_t)B * dst_h * dst_w), 256, 0, s>>>(
+          frames, dfr, out, nullptr, nullptr, B, dst_h, dst_w, mean[0], mean[1], mean[2], stdv[0], stdv[1], stdv[2]);
+    });
+  });
+}
+
 int cp_preprocess_slots_dev(const uint8_t* frames, int32_t format, int32_t B, int32_t src_h, int32_t src_w,
                             int32_t dst_h, int32_t dst_w, const double* trans_input, const float mean[3],
                             const float stdv[3], const int32_t* start, float* out, float* prev, void* stream_) {
   if (!frames || !out || !mean || !stdv) return fail(CP_ERR_INVALID, "cp_preprocess_slots_dev: null argument");
   if (!start != !prev) return fail(CP_ERR_INVALID, "cp_preprocess_slots_dev: start and prev go together");
-  if (format != CP_PIX_BGR && format != CP_PIX_NV12 && format != CP_PIX_I420)
+  if (!known_format(format))
     return fail(CP_ERR_INVALID, "cp_preprocess_slots_dev: unknown pixel format " + std::to_string(format));
   if (B <= 0 || src_h <= 0 || src_w <= 0 || dst_h <= 0 || dst_w <= 0)
     return fail(CP_ERR_INVALID, "cp_preprocess_slots_dev: bad shape");
-  if (format != CP_PIX_BGR && (src_h % 2 || src_w % 2))
+  if (is_yuv420(format) && (src_h % 2 || src_w % 2))
     return fail(CP_ERR_INVALID, "cp_preprocess_slots_dev: YUV 4:2:0 frames need an even size, got " +
+                                    std::to_string(src_h) + " x " + std::to_string(src_w));
+  if (is_yuv422(format) && src_w % 2)
+    return fail(CP_ERR_INVALID, "cp_preprocess_slots_dev: YUV 4:2:2 frames need an even width, got " +
                                     std::to_string(src_h) + " x " + std::to_string(src_w));
   double T[6];
   if (trans_input)
@@ -621,12 +814,7 @@ int cp_preprocess_slots_dev(const uint8_t* frames, int32_t format, int32_t B, in
     kernel<<<blocks, 256, 0, s>>>(frames, out, prev, start, B, src_h, src_w, dst_h, dst_w, W, mean[0], mean[1], mean[2],
                                   stdv[0], stdv[1], stdv[2]);
   };
-  if (format == CP_PIX_BGR)
-    launch(preprocess_slots_kernel<CP_PIX_BGR>);
-  else if (format == CP_PIX_NV12)
-    launch(preprocess_slots_kernel<CP_PIX_NV12>);
-  else
-    launch(preprocess_slots_kernel<CP_PIX_I420>);
+  with_format<false>(format, [&](auto k) { launch(preprocess_slots_kernel<decltype(k)::value>); });
   CP_LAUNCH_CHECK("preprocess_slots_kernel");
   return CP_OK;
 }
@@ -642,19 +830,20 @@ int cp_preprocess_frame_table(int64_t frames_bytes, const int64_t* offsets, cons
   if (!offsets || !src_hw || !table) return fail(CP_ERR_INVALID, "cp_preprocess_frame_table: null argument");
   if (B <= 0 || dst_h <= 0 || dst_w <= 0 || frames_bytes <= 0)
     return fail(CP_ERR_INVALID, "cp_preprocess_frame_table: bad shape");
-  if (format != CP_PIX_BGR && format != CP_PIX_NV12 && format != CP_PIX_I420)
+  if (!known_format(format))
     return fail(CP_ERR_INVALID, "cp_preprocess_frame_table: unknown pixel format " + std::to_string(format));
-  std::vector<RaggedFrame> fr;
-  int rc = ragged_frames("cp_preprocess_frame_table", frames_bytes, offsets, src_hw, B, dst_h, dst_w, trans_input,
-                         format != CP_PIX_BGR, fr);
-  if (rc) return rc;
-  // a build-time call: the copy is complete when it returns, so `fr` may go out of scope
-  cudaStream_t s = (cudaStream_t)stream_;
-  cudaError_t e = cudaMemcpyAsync(table, fr.data(), sizeof(RaggedFrame) * B, cudaMemcpyHostToDevice, s);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(s);
-  if (e != cudaSuccess)
-    return fail(CP_ERR_CUDA, std::string("cp_preprocess_frame_table: table upload: ") + cudaGetErrorString(e));
-  return CP_OK;
+  return upload_frame_table("cp_preprocess_frame_table", frames_bytes, offsets, src_hw, format, nullptr, B, dst_h, dst_w,
+                            trans_input, table, stream_);
+}
+
+int cp_preprocess_frame_table_formats(int64_t frames_bytes, const int64_t* offsets, const int32_t* src_hw,
+                                      const int32_t* formats, int32_t B, int32_t dst_h, int32_t dst_w,
+                                      const double* trans_input, void* table, void* stream_) {
+  if (!offsets || !src_hw || !formats || !table) return fail(CP_ERR_INVALID, "cp_preprocess_frame_table_formats: null argument");
+  if (B <= 0 || dst_h <= 0 || dst_w <= 0 || frames_bytes <= 0)
+    return fail(CP_ERR_INVALID, "cp_preprocess_frame_table_formats: bad shape");
+  return upload_frame_table("cp_preprocess_frame_table_formats", frames_bytes, offsets, src_hw, CP_PIX_PER_FRAME, formats,
+                            B, dst_h, dst_w, trans_input, table, stream_);
 }
 
 int cp_preprocess_slots_ragged_dev(const uint8_t* frames, const void* table, int32_t format, int32_t B, int32_t dst_h,
@@ -663,7 +852,7 @@ int cp_preprocess_slots_ragged_dev(const uint8_t* frames, const void* table, int
   if (!frames || !table || !out || !mean || !stdv)
     return fail(CP_ERR_INVALID, "cp_preprocess_slots_ragged_dev: null argument");
   if (!start != !prev) return fail(CP_ERR_INVALID, "cp_preprocess_slots_ragged_dev: start and prev go together");
-  if (format != CP_PIX_BGR && format != CP_PIX_NV12 && format != CP_PIX_I420)
+  if (!known_format(format) && format != CP_PIX_PER_FRAME)
     return fail(CP_ERR_INVALID, "cp_preprocess_slots_ragged_dev: unknown pixel format " + std::to_string(format));
   if (B <= 0 || dst_h <= 0 || dst_w <= 0) return fail(CP_ERR_INVALID, "cp_preprocess_slots_ragged_dev: bad shape");
   const RaggedFrame* fr = (const RaggedFrame*)table;
@@ -673,12 +862,7 @@ int cp_preprocess_slots_ragged_dev(const uint8_t* frames, const void* table, int
     kernel<<<blocks, 256, 0, s>>>(frames, fr, out, prev, start, B, dst_h, dst_w, mean[0], mean[1], mean[2], stdv[0],
                                   stdv[1], stdv[2]);
   };
-  if (format == CP_PIX_BGR)
-    launch(preprocess_slots_ragged_kernel<CP_PIX_BGR>);
-  else if (format == CP_PIX_NV12)
-    launch(preprocess_slots_ragged_kernel<CP_PIX_NV12>);
-  else
-    launch(preprocess_slots_ragged_kernel<CP_PIX_I420>);
+  with_format<true>(format, [&](auto k) { launch(preprocess_slots_ragged_kernel<decltype(k)::value>); });
   CP_LAUNCH_CHECK("preprocess_slots_ragged_kernel");
   return CP_OK;
 }
@@ -689,7 +873,7 @@ int cp_preprocess_slots_rows_dev(const uint8_t* frames, const void* table, int32
   if (!frames || !table || !rows || !out || !mean || !stdv)
     return fail(CP_ERR_INVALID, "cp_preprocess_slots_rows_dev: null argument");
   if (!store != !prev) return fail(CP_ERR_INVALID, "cp_preprocess_slots_rows_dev: store and prev go together");
-  if (format != CP_PIX_BGR && format != CP_PIX_NV12 && format != CP_PIX_I420)
+  if (!known_format(format) && format != CP_PIX_PER_FRAME)
     return fail(CP_ERR_INVALID, "cp_preprocess_slots_rows_dev: unknown pixel format " + std::to_string(format));
   if (B <= 0 || dst_h <= 0 || dst_w <= 0) return fail(CP_ERR_INVALID, "cp_preprocess_slots_rows_dev: bad shape");
   const RaggedFrame* fr = (const RaggedFrame*)table;
@@ -699,12 +883,7 @@ int cp_preprocess_slots_rows_dev(const uint8_t* frames, const void* table, int32
     kernel<<<blocks, 256, 0, s>>>(frames, fr, rows, start, store, out, prev, B, dst_h, dst_w, mean[0], mean[1], mean[2],
                                   stdv[0], stdv[1], stdv[2]);
   };
-  if (format == CP_PIX_BGR)
-    launch(preprocess_slots_rows_kernel<CP_PIX_BGR>);
-  else if (format == CP_PIX_NV12)
-    launch(preprocess_slots_rows_kernel<CP_PIX_NV12>);
-  else
-    launch(preprocess_slots_rows_kernel<CP_PIX_I420>);
+  with_format<true>(format, [&](auto k) { launch(preprocess_slots_rows_kernel<decltype(k)::value>); });
   CP_LAUNCH_CHECK("preprocess_slots_rows_kernel");
   return CP_OK;
 }

@@ -18,8 +18,8 @@ import numpy as np
 import torch
 
 from . import _lib
-from .engine import (Engine, check_pixel_format, decode_params, decode_pnp, image_size, make_meta, preprocess,
-                     preprocess_ragged, preprocess_yuv420)
+from .engine import (_YUV420, Engine, check_pixel_format, decode_params, decode_pnp, frame_layout, image_size, make_meta,
+                     preprocess, preprocess_formats, preprocess_ragged, preprocess_yuv420, slot_formats)
 from .model import _load_checkpoint, create_model, load_model
 from .tracker import Tracker, tracks_to_results
 
@@ -124,11 +124,14 @@ def camera_per_frame(camera_matrix, B):
 
 
 def check_frames(frames, allow_idle, pixel_format="bgr"):
-    """The frames of a ragged batch: uint8 [H,W,3] numpy arrays or tensors, or uint8 [3H/2,W] with an "nv12" / "i420"
-    pixel_format (None = an idle slot when allowed)."""
-    check_pixel_format(pixel_format)
+    """The frames of a ragged batch: uint8 [H,W,3] numpy arrays or tensors, or the buffers of another pixel_format
+    (engine.check_pixel_format), one name for every frame or a list with one per frame (None = an idle slot when
+    allowed)."""
+    if not isinstance(pixel_format, (list, tuple)):
+        check_pixel_format(pixel_format)
     if len(frames) == 0:
         raise ValueError("run_batch: an empty list of frames")
+    fmts = slot_formats(pixel_format, len(frames))
     for b, f in enumerate(frames):
         if f is None:
             if not allow_idle:
@@ -139,8 +142,8 @@ def check_frames(frames, allow_idle, pixel_format="bgr"):
         dt = f.dtype
         if dt not in (np.uint8, torch.uint8):
             raise TypeError("run_batch: frame %d is %s; the ragged path takes uint8 %s frames"
-                            % (b, dt, "[H,W,3]" if pixel_format == "bgr" else "[3H/2,W]"))
-        image_size(f.shape, pixel_format, "run_batch: frame %d" % b)
+                            % (b, dt, frame_layout(fmts[b])))
+        image_size(f.shape, fmts[b], "run_batch: frame %d" % b)
 
 
 def check_slot_list(values, S, name, kind=None):
@@ -571,7 +574,11 @@ class ObjectPoseDetector(object):
         pixel_format="nv12" / "i420": the uint8 frames are YUV 4:2:0 as video decoders give them, uint8 [B,3H/2,W] (array
         form) or a list of uint8 [3H_b/2,W_b] (H and W even), converted on the device inside the pre-process: every
         result equals, bit for bit, that of the same call on cv2.cvtColor(frame, COLOR_YUV2BGR_NV12 / _I420).  c, s and
-        the meta rows come from the image size (H, W)."""
+        the meta rows come from the image size (H, W).  The camera formats "rgb24" (uint8 [B,H,W,3]), "rgba" / "bgra"
+        ([B,H,W,4]) and "yuyv422" / "uyvy422" ([B,H,W,2], W even) are converted the same way, each bit for bit its
+        cv2.cvtColor to BGR (COLOR_RGB2BGR, _RGBA2BGR, _BGRA2BGR, COLOR_YUV2BGR_YUYV, _UYVY).  With a list of frames,
+        pixel_format may also be a list of one name per frame or slot (cameras of different kinds); a list of one name
+        repeated is that name."""
         if track and not getattr(self.opt, "tracking_task", False):
             raise ValueError("run_batch(track=True) needs a tracking model (opt.tracking_task)")
         if isinstance(frames, (list, tuple)):
@@ -600,22 +607,24 @@ class ObjectPoseDetector(object):
         return _returned((poses, n_valid), to_host)
 
     def _array_input(self, frames, camera_matrix, pixel_format="bgr"):
-        """run_batch's array form: uint8 [B,H,W,3] frames, uint8 [B,3H/2,W] YUV 4:2:0 frames of pixel_format (or
+        """run_batch's array form: uint8 [B,H,W,3] frames, frames of another pixel_format (uint8 [B,3H/2,W], [B,H,W,C]) (or
         pre-processed fp32 [B,3,h,w]) -> (x [B,3,h,w] fp32 CUDA, meta rows [B,16] float64 host, c, s) with the fix_res
         affine of the image size."""
         dev = self.opt.device
         if isinstance(frames, np.ndarray):
             frames = torch.from_numpy(frames)
         if check_pixel_format(pixel_format) != "bgr":
-            if frames.dtype != torch.uint8 or frames.dim() != 3:
-                raise ValueError("run_batch: %s frames are uint8 [B,3H/2,W], got %s %s"
-                                 % (pixel_format, frames.dtype, tuple(frames.shape)))
+            layout = frame_layout(pixel_format)
+            if frames.dtype != torch.uint8 or frames.dim() != layout.count(",") + 2:
+                raise ValueError("run_batch: %s frames are uint8 [B,%s, got %s %s"
+                                 % (pixel_format, layout[1:], frames.dtype, tuple(frames.shape)))
             B = frames.shape[0]
             sh, sw = image_size(frames.shape[1:], pixel_format, "run_batch: each frame")
             fr = frames.to(dev, non_blocking=True).contiguous().reshape(-1)
-            n = sh * sw * 3 // 2
-            x = preprocess_yuv420(fr, np.arange(B, dtype=np.int64) * n, [(sh, sw)] * B, pixel_format, self.opt.input_h,
-                                  self.opt.input_w, self.opt.mean, self.opt.std)
+            n = fr.numel() // max(B, 1)
+            run = preprocess_yuv420 if pixel_format in _YUV420 else preprocess_formats
+            x = run(fr, np.arange(B, dtype=np.int64) * n, [(sh, sw)] * B, pixel_format, self.opt.input_h,
+                    self.opt.input_w, self.opt.mean, self.opt.std)
             c, s = np.array([sw / 2., sh / 2.], np.float32), float(max(sh, sw))
             iw, ih = sw, sh
         elif frames.dtype == torch.uint8:
@@ -637,23 +646,25 @@ class ObjectPoseDetector(object):
 
     # ------------------------------------------------------------------ ragged batches (lists of frames)
     def _ragged_input(self, frames, camera_matrix, pixel_format="bgr"):
-        """Validated list of uint8 HWC frames (or YUV 4:2:0 [3H/2,W] frames of pixel_format) -> (x [B,3,h,w] fp32 CUDA,
-        meta rows [B,16] float64 host, trans_input [B,2,3] host).  The frames are copied into one device buffer and
-        pre-processed by one cp_preprocess_ragged (cp_preprocess_yuv420) launch with the same fix_res affine (c = image
-        centre, s = max side) and meta row that pre_process / run() use."""
+        """Validated list of uint8 HWC frames (or frames of pixel_format: one name, or one per frame) -> (x [B,3,h,w]
+        fp32 CUDA, meta rows [B,16] float64 host, trans_input [B,2,3] host).  The frames are copied into one device
+        buffer and pre-processed by one cp_preprocess_ragged (cp_preprocess_yuv420, cp_preprocess_formats for the camera
+        formats and for mixed formats) launch with the same fix_res affine (c = image centre, s = max side) and meta row
+        that pre_process / run() use."""
         if getattr(self.opt, "fix_short", 0) > 0 or not getattr(self.opt, "fix_res", True):
             raise NotImplementedError("run_batch(list) pre-processes in the fix_res mode only")
         if float(self.scales[0]) != 1.0:
             raise NotImplementedError("run_batch pre-processes at scale 1; use run() for test_scales[0] != 1")
         B = len(frames)
         cams = camera_per_frame(camera_matrix, B)
+        fmts = slot_formats(pixel_format, B)
         dev = self.opt.device
         ih, iw = self.opt.input_h, self.opt.input_w
         ts, hw, offs, off = [], np.zeros((B, 2), np.int32), np.zeros(B, np.int64), 0
         for b, f in enumerate(frames):
             t = torch.from_numpy(f) if isinstance(f, np.ndarray) else f
             ts.append(t)
-            hw[b] = image_size(t.shape, pixel_format)
+            hw[b] = image_size(t.shape, fmts[b])
             offs[b] = off
             off += t.numel()
         if self._packed is None or self._packed.numel() < off or self._packed.device != torch.device(dev):
@@ -669,11 +680,14 @@ class ObjectPoseDetector(object):
                 self._affines[(h, w)] = affine_from_center_scale(c, sc, iw, ih)
             trans[b] = self._affines[(h, w)]
             meta[b] = make_meta(1, c, sc, w, h, cams[b]).numpy()[0]
-        if pixel_format == "bgr":
+        one = fmts[0] if len(set(fmts)) == 1 else None        # one format: its launch, whatever form named it
+        if one == "bgr":
             x = preprocess_ragged(self._packed, offs, hw, ih, iw, self.opt.mean, self.opt.std, trans_input=trans)
+        elif one in _YUV420:
+            x = preprocess_yuv420(self._packed, offs, hw, one, ih, iw, self.opt.mean, self.opt.std, trans_input=trans)
         else:
-            x = preprocess_yuv420(self._packed, offs, hw, pixel_format, ih, iw, self.opt.mean, self.opt.std,
-                                  trans_input=trans)
+            x = preprocess_formats(self._packed, offs, hw, one or fmts, ih, iw, self.opt.mean, self.opt.std,
+                                   trans_input=trans)
         return x, meta, trans
 
     def _meta_rows(self, meta):
@@ -706,7 +720,9 @@ class ObjectPoseDetector(object):
             out[0].zero_()
             out[1].zero_()
             return _returned(out, to_host)
-        x, meta, trans = self._ragged_input([frames[i] for i in live], np.stack([cams[i] for i in live]), pixel_format)
+        fmts = slot_formats(pixel_format, S)
+        x, meta, trans = self._ragged_input([frames[i] for i in live], np.stack([cams[i] for i in live]),
+                                            [fmts[i] for i in live])
         return self._track_step(S, live, x, self._meta_rows(meta), trans, new_video, pre_dets, frame_ids, to_host, out)
 
     # ---- what a tracking step does per category: one category here; MultiCategoryTracker runs several through the
@@ -863,7 +879,8 @@ class MultiCategoryDetector(ObjectPoseDetector):
 
     def run_batch(self, frames, camera_matrix, to_host=True, out=None, pixel_format="bgr"):
         """run_batch of ObjectPoseDetector (a uint8 [B,H,W,3] array, or a list of mixed-size frames with one camera or
-        one per frame; YUV 4:2:0 frames with pixel_format "nv12" / "i420") for every category: the frames are
+        one per frame; YUV 4:2:0 and camera formats with pixel_format, a list of names with a list of frames, as there)
+        for every category: the frames are
         pre-processed once.  Returns (poses [M,B,K,192], n_valid [M,B]) in `categories` order, also for M = 1; out:
         optional (poses, n_valid) CUDA tensors of those shapes to write into."""
         if isinstance(frames, (list, tuple)):
@@ -918,7 +935,8 @@ class MultiCategoryTracker(MultiCategoryDetector):
         slot list of meta['pre_dets'] lists (None = that slot is not seeded); frame_ids: per slot meta['id'].
         Returns (tracks [M,S,T,320], n_tracks [M,S]) in `categories` order (idle slots: n_tracks 0, zero rows), on the
         host when `to_host`; out: optional (tracks, n_tracks) CUDA tensors of those shapes to write into.
-        pixel_format "nv12" / "i420": YUV 4:2:0 frames, uint8 [S,3H/2,W] or [3H_s/2,W_s] (as ObjectPoseDetector.run_batch)."""
+        pixel_format "nv12" / "i420": YUV 4:2:0 frames, uint8 [S,3H/2,W] or [3H_s/2,W_s]; the camera formats and one name
+        per slot with a list of frames as in ObjectPoseDetector.run_batch."""
         if isinstance(frames, (list, tuple)):
             return self._run_slots(frames, camera_matrix, to_host, out, pre_dets, frame_ids, new_video, pixel_format)
         if new_video is not None:

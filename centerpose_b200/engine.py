@@ -512,20 +512,52 @@ def preprocess_ragged(packed_u8, offsets, src_hw, dst_h, dst_w, mean, std, out=N
 
 
 _YUV420 = {"nv12": _lib.CP_PIX_NV12, "i420": _lib.CP_PIX_I420}
+# the buffer of one H x W image in each pixel_format: [3H/2,W] for YUV 4:2:0, else [H,W,C]
+_LAYOUT = {"bgr": "[H,W,3]", "nv12": "[3H/2,W]", "i420": "[3H/2,W]", "rgb24": "[H,W,3]", "rgba": "[H,W,4]",
+           "bgra": "[H,W,4]", "yuyv422": "[H,W,2]", "uyvy422": "[H,W,2]"}
+_CHANNELS = {"bgr": 3, "rgb24": 3, "rgba": 4, "bgra": 4, "yuyv422": 2, "uyvy422": 2}
 
 
 def check_pixel_format(pixel_format):
-    """pixel_format: "bgr" (uint8 [H,W,3]), "nv12" or "i420" (uint8 [3H/2,W], cp_pixel_format)."""
+    """pixel_format (cp_pixel_format): "bgr" (uint8 [H,W,3], cv2.imread's), "nv12" or "i420" (uint8 [3H/2,W], H and W
+    even), or a camera format named as ffmpeg's pix_fmt: "rgb24" ([H,W,3]), "rgba" / "bgra" ([H,W,4], alpha ignored),
+    "yuyv422" / "uyvy422" ([H,W,2] packed YUV 4:2:2, W even).  One name; a list (one per camera) goes through
+    slot_formats where frames come as a list."""
+    if isinstance(pixel_format, (list, tuple)):
+        raise ValueError("pixel_format must be one name here, got a list %r; one name per camera goes with a list of "
+                         "frames (run_batch(list), a graph built with one frame_hw per slot)" % (list(pixel_format),))
     if pixel_format not in _lib.PIXEL_FORMATS:
         raise ValueError("pixel_format must be one of %s, got %r" % (", ".join(_lib.PIXEL_FORMATS), pixel_format))
     return pixel_format
 
 
+def slot_formats(pixel_format, n, who="run_batch"):
+    """The pixel formats of n frames or slots: one name for all of them, or a list of n names (one per camera)."""
+    if not isinstance(pixel_format, (list, tuple)):
+        return [check_pixel_format(pixel_format)] * n
+    if len(pixel_format) != n:
+        raise ValueError("%s: pixel_format is one name or one per frame, got %d names for %d frames"
+                         % (who, len(pixel_format), n))
+    for f in pixel_format:
+        if isinstance(f, (list, tuple)) or f not in _lib.PIXEL_FORMATS:
+            raise ValueError("pixel_format must be one of %s, got %r in %r"
+                             % (", ".join(_lib.PIXEL_FORMATS), f, list(pixel_format)))
+    return list(pixel_format)
+
+
+def frame_layout(pixel_format):
+    """"[H,W,3]", "[3H/2,W]", ...: the buffer of one image in pixel_format, for messages."""
+    return _LAYOUT[check_pixel_format(pixel_format)]
+
+
 def frame_shape(h, w, pixel_format):
-    """The buffer shape of one h x w image in pixel_format: [h,w,3] for "bgr", [3h/2,w] for "nv12" / "i420" (h and w
-    even, else ValueError)."""
-    if check_pixel_format(pixel_format) == "bgr":
-        return (int(h), int(w), 3)
+    """The buffer shape of one h x w image in pixel_format: [h,w,3] for "bgr" / "rgb24", [h,w,4] for "rgba" / "bgra",
+    [h,w,2] for "yuyv422" / "uyvy422" (w even), [3h/2,w] for "nv12" / "i420" (h and w even); else ValueError."""
+    c = _CHANNELS.get(check_pixel_format(pixel_format))
+    if c is not None:
+        if c == 2 and (w % 2 or h < 1 or w < 2):
+            raise ValueError("%s frames need an even, positive width; got %d x %d" % (pixel_format, h, w))
+        return (int(h), int(w), c)
     if h % 2 or w % 2 or h < 2 or w < 2:
         raise ValueError("%s frames need an even, positive image size; got %d x %d" % (pixel_format, h, w))
     return (int(h) * 3 // 2, int(w))
@@ -535,15 +567,51 @@ def image_size(shape, pixel_format, what="frame"):
     """(H, W) of the image a buffer of `shape` holds in pixel_format; ValueError (naming the expected shape) when the
     shape is not one of that format."""
     shape = tuple(int(v) for v in shape)
-    if check_pixel_format(pixel_format) == "bgr":
-        if len(shape) != 3 or shape[2] != 3 or shape[0] < 1 or shape[1] < 1:
-            raise ValueError("%s has shape %s, expected [H,W,3]" % (what, shape))
+    c = _CHANNELS.get(check_pixel_format(pixel_format))
+    if c is not None:
+        if len(shape) != 3 or shape[2] != c or shape[0] < 1 or shape[1] < 1 or (c == 2 and shape[1] % 2):
+            raise ValueError("%s has shape %s, expected %s[H,W,%d]%s" % (what, shape, "" if c == 3 else "a %s frame "
+                                                                        % pixel_format, c, " with W even" if c == 2 else ""))
         return shape[0], shape[1]
     if len(shape) == 2 and shape[0] % 3 == 0:
         h, w = shape[0] * 2 // 3, shape[1]
         if h >= 2 and w >= 2 and h % 2 == 0 and w % 2 == 0:
             return h, w
     raise ValueError("%s has shape %s, expected a %s frame [3H/2,W] with H and W even" % (what, shape, pixel_format))
+
+
+def preprocess_formats(packed_u8, offsets, src_hw, pixel_format, dst_h, dst_w, mean, std, out=None, trans_input=None):
+    """cp_preprocess_formats: preprocess_ragged for frames in any pixel_format, one name for every frame or a list of B
+    names (one per frame).  packed_u8: flat uint8 CUDA buffer holding frame b (its pixel format's buffer of image size
+    src_hw[b]) at byte offsets[b] -> fp32 [B,3,dst_h,dst_w] CUDA, frame b bit for bit what preprocess_ragged gives for
+    cv2.cvtColor(frame) to BGR.  trans_input: optional [B,2,3] forward affines; default = each frame's fix_res affine."""
+    L = _lib.load()
+    offs = np.ascontiguousarray(offsets, np.int64).reshape(-1)
+    hw = np.ascontiguousarray(src_hw, np.int32).reshape(-1, 2)
+    B = offs.shape[0]
+    codes = np.array([_lib.PIXEL_FORMAT_CODES[f] for f in slot_formats(pixel_format, B, "preprocess_formats")],
+                     np.int32)
+    if not packed_u8.is_cuda or packed_u8.dtype != torch.uint8 or not packed_u8.is_contiguous():
+        raise RuntimeError("preprocess_formats needs a contiguous uint8 CUDA buffer")
+    if hw.shape[0] != B:
+        raise ValueError("preprocess_formats: %d offsets for %d frame sizes" % (B, hw.shape[0]))
+    if out is None:
+        out = torch.empty((B, 3, dst_h, dst_w), dtype=torch.float32, device=packed_u8.device)
+    tm = None
+    if trans_input is not None:
+        tr = np.ascontiguousarray(trans_input, np.float64).reshape(-1)
+        if tr.shape[0] != 6 * B:
+            raise ValueError("preprocess_formats: trans_input must hold %d 2x3 matrices" % B)
+        tm = tr.ctypes.data_as(ctypes.POINTER(ctypes.c_double))
+    m = (ctypes.c_float * 3)(*[float(v) for v in mean])
+    s = (ctypes.c_float * 3)(*[float(v) for v in std])
+    with torch.cuda.device(packed_u8.device):
+        rc = L.cp_preprocess_formats(_ptr(packed_u8), packed_u8.numel(), offs.ctypes.data_as(ctypes.POINTER(ctypes.c_int64)),
+                                     hw.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)),
+                                     codes.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), _ptr(out), B, dst_h, dst_w, tm,
+                                     m, s, _stream())
+    _lib.check(rc, "cp_preprocess_formats")
+    return out
 
 
 def preprocess_yuv420(packed_u8, offsets, src_hw, pixel_format, dst_h, dst_w, mean, std, out=None, trans_input=None):

@@ -61,7 +61,7 @@ class _SlotGraph(object):
     def _build(self, det, slots, frame_hw, camera_matrix, pixel_format, idle_slots=False):
         """Checks, buffers and the captured steps; everything that refuses comes before any device work."""
         from .detector import affine_from_center_scale, camera_per_frame
-        from .engine import check_pixel_format, frame_shape, make_meta
+        from .engine import check_pixel_format, frame_shape, make_meta, slot_formats
         who, opt = type(self).__name__, det.opt
         self._refuse(opt, who)
         S = int(slots)
@@ -69,8 +69,13 @@ class _SlotGraph(object):
             raise ValueError("%s: slots must be >= 1, got %d" % (who, S))
         sizes, self.per_slot = _frame_sizes(frame_hw, S, who)
         self.idle_slots = bool(idle_slots)
-        self.pixel_format = check_pixel_format(pixel_format)
-        shapes = [frame_shape(h, w, pixel_format) for h, w in sizes]
+        if isinstance(pixel_format, (list, tuple)) and not self.per_slot:
+            raise ValueError("%s: one pixel_format per slot goes with one frame_hw per slot; with one frame_hw every "
+                             "slot takes one name, got %r" % (who, list(pixel_format)))
+        fmts = slot_formats(pixel_format, S, who) if self.per_slot else [check_pixel_format(pixel_format)]
+        # one name repeated is that name: the same table, launches and bits
+        self.pixel_format = fmts[0] if len(set(fmts)) == 1 else fmts
+        shapes = [frame_shape(h, w, f) for (h, w), f in zip(sizes, fmts)]
         cams = np.stack(camera_per_frame(camera_matrix, S))
         if self.per_slot:
             self.frame_hw, self.frame_shape = sizes, shapes
@@ -94,7 +99,8 @@ class _SlotGraph(object):
         self.meta = torch.from_numpy(meta).to(dev)                   # the network's rows, one per frame
         self._mean = (ctypes.c_float * 3)(*[float(v) for v in opt.mean])
         self._std = (ctypes.c_float * 3)(*[float(v) for v in opt.std])
-        self._fmt = {"bgr": _lib.CP_PIX_BGR, "nv12": _lib.CP_PIX_NV12, "i420": _lib.CP_PIX_I420}[self.pixel_format]
+        mixed = isinstance(self.pixel_format, list)       # per-slot formats: a table of them, one per-frame launch
+        self._fmt = _lib.CP_PIX_PER_FRAME if mixed else _lib.PIXEL_FORMAT_CODES[self.pixel_format]
         if self.per_slot or self.idle_slots:                # a frame table (with idle slots: of S equal sizes too)
             n = [int(np.prod(s)) for s in self._slot_shapes]
             offs = np.concatenate([[0], np.cumsum(n)[:-1]]).astype(np.int64)
@@ -102,11 +108,18 @@ class _SlotGraph(object):
             self._slot_frames = [self.frames[o:o + k].view(s) for o, k, s in zip(offs, n, self._slot_shapes)]
             self.table = torch.zeros((int(L.cp_preprocess_frame_table_bytes(S)),), dtype=torch.uint8, device=dev)
             hw = np.ascontiguousarray(sizes, np.int32)
+            p64, p32 = offs.ctypes.data_as(ctypes.POINTER(ctypes.c_int64)), hw.ctypes.data_as(ctypes.POINTER(ctypes.c_int32))
+            ptr = trans.ctypes.data_as(ctypes.POINTER(ctypes.c_double))
             with torch.cuda.device(dev):
-                _lib.check(L.cp_preprocess_frame_table(self.frames.numel(), offs.ctypes.data_as(ctypes.POINTER(ctypes.c_int64)),
-                                                       hw.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), self._fmt, S, ih,
-                                                       iw, trans.ctypes.data_as(ctypes.POINTER(ctypes.c_double)),
-                                                       _ptr(self.table), _stream()), "cp_preprocess_frame_table")
+                if mixed:
+                    codes = np.array([_lib.PIXEL_FORMAT_CODES[f] for f in fmts], np.int32)
+                    _lib.check(L.cp_preprocess_frame_table_formats(self.frames.numel(), p64, p32,
+                                                                   codes.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)),
+                                                                   S, ih, iw, ptr, _ptr(self.table), _stream()),
+                               "cp_preprocess_frame_table_formats")
+                else:
+                    _lib.check(L.cp_preprocess_frame_table(self.frames.numel(), p64, p32, self._fmt, S, ih, iw, ptr,
+                                                           _ptr(self.table), _stream()), "cp_preprocess_frame_table")
         else:
             self.frames = torch.zeros(self.frame_shape, dtype=torch.uint8, device=dev)
         if self.idle_slots:
@@ -241,7 +254,8 @@ class _SlotGraph(object):
             if not torch.is_tensor(f) or f.dtype != torch.uint8 or tuple(f.shape) != self._slot_shapes[b]:
                 what = ("%s %s" % (f.dtype, tuple(f.shape))) if torch.is_tensor(f) else type(f).__name__
                 raise ValueError("%s: slot %d takes uint8 %s frames (%s, frame_hw %s), got %s"
-                                 % (who, b, list(self._slot_shapes[b]), self.pixel_format, self._slot_hw[b], what))
+                                 % (who, b, list(self._slot_shapes[b]), self.pixel_format[b] if isinstance(
+                                     self.pixel_format, list) else self.pixel_format, self._slot_hw[b], what))
             out.append(f)
         return out
 
@@ -307,9 +321,10 @@ class DetectGraph(_SlotGraph):
     MultiCategoryDetectGraph.
 
     frame_hw, camera_matrix, pixel_format and the frames of a call are those of TrackGraph: one (H, W) for every slot
-    (frames uint8 [S,H,W,3], or [S,3H/2,W] for "nv12" / "i420") or a list of S sizes (a list of S frames, packed into
-    one device buffer and pre-processed through a frame table built now); [3,3] or [S,3,3] cameras.  Frames may be in
-    pinned host memory (keep them unchanged until the step's outputs are read) or on the device.
+    (frames uint8 [S,H,W,3], or [S,3H/2,W] for "nv12" / "i420", [S,H,W,C] for a camera format) or a list of S sizes (a
+    list of S frames, packed into one device buffer and pre-processed through a frame table built now; pixel_format may
+    then be a list of one name per slot); [3,3] or [S,3,3] cameras.  Frames may be in pinned host memory (keep them
+    unchanged until the step's outputs are read) or on the device.
 
     idle_slots=True: a call takes a list of S entries, None for an idle camera (with one frame_hw, a uint8 [S, ...]
     array still means every slot live).  Every step is bit for bit run_batch(list) of the live frames with their

@@ -33,7 +33,7 @@
  *       utils/pnp/cuboid_pnp_shell.py:11-93, utils/pnp/cuboid_pnp_solver.py:91-239
  *   cp_infer
  *       detectors/base_detector.py:473-654 (process -> post_process -> merge -> PnP)
- *   cp_preprocess / cp_preprocess_affine / cp_preprocess_ragged / cp_preprocess_yuv420
+ *   cp_preprocess / cp_preprocess_affine / cp_preprocess_ragged / cp_preprocess_yuv420 / cp_preprocess_formats
  *       detectors/base_detector.py:91-148 pre_process (resize + affine warp + normalise)
  */
 #ifndef CENTERPOSE_B200_H_
@@ -637,8 +637,19 @@ int cp_preprocess_ragged(const uint8_t* frames, int64_t frames_bytes, const int6
 enum cp_pixel_format {
   CP_PIX_NV12 = 0,
   CP_PIX_I420 = 1,
-  CP_PIX_BGR = 2   /* interleaved uint8 [H, W, 3]; taken by cp_preprocess_slots_dev and cp_preprocess_slots_ragged_dev
+  CP_PIX_BGR = 2,  /* interleaved uint8 [H, W, 3]; taken by cp_preprocess_slots_dev and cp_preprocess_slots_ragged_dev
                     * (cp_preprocess_yuv420 refuses it) */
+  /* Camera formats, ffmpeg's pix_fmt names; one uint8 [H, W, C] buffer per frame.  Each is converted to BGR inside the
+   * warp, per tap, bit for bit what cv2.cvtColor gives with the code named (taps outside the frame are BGR 0).  Taken by
+   * cp_preprocess_formats, cp_preprocess_slots_dev, the frame tables and their launches; cp_preprocess_yuv420 refuses
+   * them.  The values are grouped by family; those in between are not formats. */
+  CP_PIX_RGB24 = 16,     /* [H, W, 3] R G B (ROS 2 / PIL / PyAV "rgb24"): COLOR_RGB2BGR */
+  CP_PIX_RGBA = 17,      /* [H, W, 4] R G B A, alpha ignored: COLOR_RGBA2BGR */
+  CP_PIX_BGRA = 18,      /* [H, W, 4] B G R A, alpha ignored: COLOR_BGRA2BGR */
+  CP_PIX_YUYV422 = 32,   /* [H, W, 2], W even, Y0 U Y1 V per pixel pair (V4L2 YUYV, GStreamer YUY2): COLOR_YUV2BGR_YUYV */
+  CP_PIX_UYVY422 = 33,   /* [H, W, 2], W even, U Y0 V Y1 per pixel pair (V4L2 / GStreamer UYVY): COLOR_YUV2BGR_UYVY */
+  /* not a frame format: a launch over a table of per-frame formats (cp_preprocess_frame_table_formats) */
+  CP_PIX_PER_FRAME = 64
 };
 /* cp_preprocess_ragged on YUV 4:2:0 frames: frame b is [src_hw[b][0] * 3 / 2, src_hw[b][1]] uint8 in `format`, i.e.
  * src_hw[b][0] * src_hw[b][1] * 3 / 2 bytes starting `offsets[b]` bytes into `frames`; src_hw holds the IMAGE sizes
@@ -651,13 +662,23 @@ enum cp_pixel_format {
 int cp_preprocess_yuv420(const uint8_t* frames, int64_t frames_bytes, const int64_t* offsets, const int32_t* src_hw,
                          int32_t format, float* out, int32_t B, int32_t dst_h, int32_t dst_w, const double* trans_input,
                          const float mean[3], const float std[3], void* stream);
+/* cp_preprocess_ragged with one pixel format per frame: frame b is in formats[b] (HOST int32 [B], any cp_pixel_format
+ * but CP_PIX_PER_FRAME), its buffer shape given by that format and the image size src_hw[b] = (H, W) (4:2:0: both even;
+ * 4:2:2: W even).  Frame b's output equals, bit for bit, cp_preprocess_ragged on cv2.cvtColor(frame) to BGR with the
+ * same trans_input (NULL: each frame's fix_res affine).  One launch: one format's walk when every frame has it, else a
+ * walk that reads each frame's format from the per-frame parameters.  An unknown format, a size its format cannot have
+ * or a frame that does not fit inside frames_bytes at its format's size returns CP_ERR_INVALID before any work is
+ * enqueued. */
+int cp_preprocess_formats(const uint8_t* frames, int64_t frames_bytes, const int64_t* offsets, const int32_t* src_hw,
+                          const int32_t* formats, float* out, int32_t B, int32_t dst_h, int32_t dst_w,
+                          const double* trans_input, const float mean[3], const float std[3], void* stream);
 
 /* The pre-process of one tracking step of B video slots, safe to capture in a CUDA graph: it reads no host memory and
  * allocates nothing once enqueued, so a replay runs it with the arguments it was captured with.  frames: device uint8,
  * B frames of one image size (src_h, src_w) in `format` (cp_pixel_format; YUV 4:2:0 needs an even size), frame b at byte
  * b * (bytes of one frame).  trans_input: HOST row-major 2x3 forward affine for every frame, read before the call
  * returns (NULL: the fix_res affine of the size, as cp_preprocess).  out: device fp32 [B,3,dst_h,dst_w], frame b bit for
- * bit what cp_preprocess_affine (BGR) or cp_preprocess_yuv420 (NV12 / I420) gives for it.  start: device int32 [B] read
+ * bit what cp_preprocess_affine (BGR), cp_preprocess_yuv420 (NV12 / I420) or cp_preprocess_formats gives for it.  start: device int32 [B] read
  * when the kernel runs, or NULL; where start[b] != 0 frame b's output is written to prev[b] (device fp32
  * [B,3,dst_h,dst_w]) as well: a slot whose video starts with this frame takes it as its previous frame.  start and prev
  * are both given or both NULL.  Bad arguments return CP_ERR_INVALID before any work is enqueued. */
@@ -689,6 +710,15 @@ int cp_preprocess_frame_table(int64_t frames_bytes, const int64_t* offsets, cons
 int cp_preprocess_slots_ragged_dev(const uint8_t* frames, const void* table, int32_t format, int32_t B, int32_t dst_h,
                                    int32_t dst_w, const float mean[3], const float std[3], const int32_t* start,
                                    float* out, float* prev, void* stream);
+/* A frame table with one pixel format per frame (cameras of different kinds in one step): cp_preprocess_frame_table
+ * with formats[b] (HOST int32 [B], any cp_pixel_format but CP_PIX_PER_FRAME) for frame b, checked the same way (an
+ * unknown format, an odd width in 4:2:2 or odd size in 4:2:0, a frame overrunning frames_bytes at its format's size
+ * return CP_ERR_INVALID before any work).  The table has cp_preprocess_frame_table_bytes(B) bytes and is launched by
+ * cp_preprocess_slots_ragged_dev and cp_preprocess_slots_rows_dev with format CP_PIX_PER_FRAME (and only so): frame b's
+ * output is then bit for bit what the launch of a one-format table gives for it. */
+int cp_preprocess_frame_table_formats(int64_t frames_bytes, const int64_t* offsets, const int32_t* src_hw,
+                                      const int32_t* formats, int32_t B, int32_t dst_h, int32_t dst_w,
+                                      const double* trans_input, void* table, void* stream);
 /* The pre-process of one tracking step in which only some of the S slots of a cp_preprocess_frame_table have a frame,
  * safe to capture in a CUDA graph.  Row n of the B live rows is slot rows[n]: out[n] (device fp32 [B,3,dst_h,dst_w]) is
  * bit for bit what cp_preprocess_slots_ragged_dev gives for that slot's frame.  rows (int32 [B]), start (int32 [S], per
