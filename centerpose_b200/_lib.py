@@ -61,7 +61,7 @@ EXPORTS = [
     "cp_preprocess_slots_dev", "cp_tracker_reset_dev", "cp_tracker_render_dev",
     "cp_preprocess_frame_table_bytes", "cp_preprocess_frame_table", "cp_preprocess_slots_ragged_dev",
     "cp_preprocess_slots_rows_dev", "cp_gather_rows_dev", "cp_tracker_render_dev2", "cp_tracker_step_dev",
-    "cp_preprocess_formats", "cp_preprocess_frame_table_formats",
+    "cp_preprocess_formats", "cp_preprocess_frame_table_formats", "cp_plan_op_ksegments", "cp_plan_ksegments",
 ]
 
 # cp_pixel_format; "bgr" is the interleaved uint8 [H,W,3] input of every other pre-process entry point.  The camera
@@ -76,6 +76,10 @@ PIXEL_FORMAT_CODES = {"bgr": CP_PIX_BGR, "nv12": CP_PIX_NV12, "i420": CP_PIX_I42
 # cp_plan_create_ex / cp_plan_memory flags
 CP_PLAN_REUSE_ACTIVATIONS = 1
 CP_PLAN_MULTI_TRACK = 2
+CP_PLAN_BATCH_INVARIANT = 32
+
+# cp_kpath: how a conv_tma / dcn_tma launch summed its K segments (cp_plan_op_ksegments)
+KPATH_NONE, KPATH_ONE, KPATH_SPLIT, KPATH_FOLD = 0, 1, 2, 3
 
 # cp_op_family
 FAM_NONE, FAM_IGEMM_FP32, FAM_STEM, FAM_CONV3_C16, FAM_IGEMM_UMMA, FAM_CONV_TMA, FAM_DCN_TMA = 0, 1, 2, 3, 4, 5, 6
@@ -258,6 +262,9 @@ def load():
     L.cp_plan_memory.argtypes = [ctypes.POINTER(CpConfig), i32, ctypes.c_uint32, ctypes.POINTER(CpMemoryInfo)]
     L.cp_plan_allocations.argtypes = [ctypes.POINTER(CpConfig), i32, ctypes.c_uint32, ctypes.POINTER(CpActAlloc), i32,
                                       ctypes.POINTER(i32)]
+    L.cp_plan_op_ksegments.argtypes = [vp, i32, ctypes.POINTER(i32), ctypes.POINTER(i32), ctypes.POINTER(i32)]
+    L.cp_plan_ksegments.argtypes = [ctypes.POINTER(CpConfig), i32, ctypes.c_uint32, ctypes.POINTER(i32), i32,
+                                    ctypes.POINTER(i32)]
     for name in EXPORTS:
         fn = getattr(L, name)
         if name not in ("cp_version", "cp_last_error", "cp_plan_bytes", "cp_plan_forward_launches",

@@ -6,6 +6,7 @@
 #include <string>
 
 #include "../../include/centerpose_b200.h"
+#include "ksegments.h"        // fixed_ksegments: the K segments of batch-invariant plans
 
 namespace cp {
 
@@ -112,6 +113,7 @@ struct LaunchInfo {
   int BN = 0;           // N tile
   int ksplit = 1;       // split-K factor (1 = off)
   long long grid = 0;   // CTAs of the main kernel
+  int path = 0;         // cp_kpath: how the K segments were summed
 };
 
 // dedicated 7x7 stem kernel (stem_conv.cu); consumes the same packed fp32 weights as the generic kernel
@@ -129,6 +131,9 @@ struct ConvKernel {
   int BN = 0;                       // N tile (tensor-core families)
   int cslab = 0;                    // channels per activation slab (conv_tma / dcn_tma)
   size_t wbytes = 0;                // bytes of the pre-swizzled weight tiles (0: the kernel reads the fp32 matrix)
+  // conv_tma / dcn_tma K segments of a batch-invariant plan (fixed_ksegments, set at plan time); 0: the launcher picks
+  // split-K from the launch's tiles and the SM count (splitk_factor)
+  int ksegments = 0;
 };
 // Where the callers of select_conv_kernel differ.
 struct ConvPolicy {
@@ -212,6 +217,7 @@ int tma_encode_nhwc_box(const float* base, int C, int W, int H, int B, int strid
                         int swizzle64, void* map_out /* 128 bytes, 64-byte aligned */);
 int tma_conv_encode(const IgemmParams& p, int Bmax, int cslab, void* maps_out /* 4 x 128 bytes */);
 int launch_conv_tma(const IgemmParams& p, const void* maps, const ConvKernel& k, cudaStream_t stream, LaunchInfo* info);
+long long conv_tma_image_tiles(const IgemmParams& p, int BN);     // (m, n) tiles of one image of one model
 
 // TMA-staged deformable convolution (dcn_tma.cu): DCNv2 3x3 stride 1 pad 1 over one NHWC fp32 source, kind::tf32.
 // x3 = 1: 3-term split + promoted accumulation (fp32-equivalent);  x3 = 0: single pass.
@@ -219,6 +225,7 @@ bool dcn_tma_supported(const IgemmParams& p, int x3);
 int dcn_tma_tile_n(int CoutPad, int x3);
 int dcn_tma_encode(const IgemmParams& p, int Bmax, void* map_out /* 128 bytes, 64-byte aligned */);
 int launch_dcn_tma(const IgemmParams& p, const void* map, const ConvKernel& k, cudaStream_t stream, LaunchInfo* info);
+long long dcn_tma_image_tiles(const IgemmParams& p, int BN);      // (m, n) tiles of one image of one model
 
 inline int round_up(int x, int m) { return (x + m - 1) / m * m; }
 // Output columns of a convolution's packed weight matrix: 16, 32, then multiples of 64 (27 offset/mask channels -> 32)

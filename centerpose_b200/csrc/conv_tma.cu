@@ -144,7 +144,12 @@ __device__ __forceinline__ bool tile_position(const TmaConvParams& p, const Tile
 // PERSISTENT kernel: gridDim.x = min(#tiles, #SMs); CTA c processes tiles c, c + gridDim.x, ...  Every role keeps its
 // pipeline state across tiles, so the TMA / split of tile i+1 overlap the epilogue of tile i and the fixed cost of a CTA
 // (barrier init, descriptor fetch, pipeline fill) is paid once per SM instead of per tile.
-template <bool X3, bool FUSE, int BN, bool MULTI>
+//
+// FOLD (x3, not fused; batch-invariant plans): one CTA per (m, n) tile sums the ksplit K segments of `sps` slabs back to
+// back, each exactly as a split-K CTA of that segment does (its accumulation groups start at the segment's first K
+// block), and adds them in segment order into a running total, ((0 + seg 0) + seg 1) + ..., which is what
+// splitk_finish computes from the parked partial sums: a tile's outputs are the same bits on either path.
+template <bool X3, bool FUSE, int BN, bool MULTI, bool FOLD>
 __global__ void __launch_bounds__(X3 ? (FUSE ? TM_THREADS_X3F : TM_THREADS_X3) : TM_THREADS, 1)
     conv_tma_kernel(const __grid_constant__ TmaConvParams p) {
   // x3 fused: the per-head 1x1 runs in its own warpgroup (warps 16 - 19) behind the hidden ring
@@ -165,8 +170,8 @@ __global__ void __launch_bounds__(X3 ? (FUSE ? TM_THREADS_X3F : TM_THREADS_X3) :
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int n_tiles = p.CoutPad / BN;
   const int taps = p.k * p.k;
-  const int KS_SPLIT = p.ksplit;                   // split-K factor (1 = off)
-  const int sps = p.sps;                           // slabs per split
+  const int KS_SPLIT = FOLD ? 1 : p.ksplit;        // split-K factor (1 = off)
+  const int sps = FOLD ? p.sps * p.ksplit : p.sps; // slabs per split (fold: every slab of the tile)
   const int KB = sps * taps;                       // K blocks THIS CTA runs per tile
   const int KB_all = (p.Cin / p.cslab) * taps;     // K blocks of the whole contraction (weight-tile addressing)
   const long long total_tiles = p.total_tiles;
@@ -423,6 +428,7 @@ __global__ void __launch_bounds__(X3 ? (FUSE ? TM_THREADS_X3F : TM_THREADS_X3) :
     uint32_t pa = 0, pb = 0;
     float acc[BN / 2];
     float sums[X3 ? BN / 2 : 1];
+    float tot[FOLD ? BN / 2 : 1];        // fold: the running total of the finished K segments
     float acc2[FUSE ? 16 : 1];           // fused 1x1: partial outputs (this thread's half of the hidden channels) of its row
 #pragma unroll
     for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
@@ -434,6 +440,10 @@ __global__ void __launch_bounds__(X3 ? (FUSE ? TM_THREADS_X3F : TM_THREADS_X3) :
       const uint32_t row0 = (p.k == 3 ? (uint32_t)(g.g0 - 1 - g.r_lo * p.Wt) : 0u) + (uint32_t)c * 64u;
 #pragma unroll
       for (int j = 0; j < (X3 ? BN / 2 : 1); ++j) sums[j] = 0.f;
+      if constexpr (FOLD) {
+#pragma unroll
+        for (int j = 0; j < BN / 2; ++j) tot[j] = 0.f;
+      }
       // x3: the K blocks of an accumulation group chain on one accumulator, so each stays in flight until the next one of
       // its group is queued behind it, and the group's last is waited for before the promotion; the wgmmas and their
       // order are those of a wait after every K block.  With one slab stage the next slab's TMA needs the stage back at
@@ -448,47 +458,58 @@ __global__ void __launch_bounds__(X3 ? (FUSE ? TM_THREADS_X3F : TM_THREADS_X3) :
           if (tap == 0) mbar_arrive(bar_a_empty + 8u * (uint32_t)(sa == 0 ? p.SA - 1 : sa - 1));
         }
       };
-      for (int kb0 = 0; kb0 < KB; kb0 += group) {
-        const int n_kb = min(group, KB - kb0);
-        for (int i = 0; i < n_kb; ++i) {
-          if (tap == 0) mbar_wait(bar_a + 8u * (uint32_t)sa, pa);
-          const int ky = tap / 3, kx = tap - ky * 3;
-          const uint32_t arow = row0 + (p.k == 3 ? (uint32_t)(ky * p.Wt + kx) : 0u);
-          mbar_wait(bar_b_full + 8u * (uint32_t)sb, pb);
-          const uint64_t da = make_desc(slabs0 + (uint32_t)sa * a_stage + arow * rowb, p.cslab);
-          const uint64_t db = make_desc(btiles0 + (uint32_t)sb * btile_bytes, p.cslab);
-          const bool fresh = X3 ? i == 0 : kb0 == 0;
-          if (p.cslab == 32)
-            mma_kblock_issue<BN, X3, false, 4>(acc, da, db, a_lo_u, b_lo_u, fresh);
-          else
-            mma_kblock_issue<BN, X3, false, 2>(acc, da, db, a_lo_u, b_lo_u, fresh);
-          if (overlap && i > 0) {
-            wg_wait<1>();
-            release_prev();
-          }
-          if (++sb == p.SB) {
-            sb = 0;
-            pb ^= 1u;
-          }
-          if (++tap == taps) {
-            tap = 0;
-            if (++sa == p.SA) {
-              sa = 0;
-              pa ^= 1u;
+      const int KB_seg = FOLD ? p.sps * taps : KB;       // K blocks of one segment
+      for (int seg = 0; seg < (FOLD ? p.ksplit : 1); ++seg) {
+        for (int kb0 = 0; kb0 < KB_seg; kb0 += group) {
+          const int n_kb = min(group, KB_seg - kb0);
+          for (int i = 0; i < n_kb; ++i) {
+            if (tap == 0) mbar_wait(bar_a + 8u * (uint32_t)sa, pa);
+            const int ky = tap / 3, kx = tap - ky * 3;
+            const uint32_t arow = row0 + (p.k == 3 ? (uint32_t)(ky * p.Wt + kx) : 0u);
+            mbar_wait(bar_b_full + 8u * (uint32_t)sb, pb);
+            const uint64_t da = make_desc(slabs0 + (uint32_t)sa * a_stage + arow * rowb, p.cslab);
+            const uint64_t db = make_desc(btiles0 + (uint32_t)sb * btile_bytes, p.cslab);
+            const bool fresh = X3 ? i == 0 : kb0 == 0;
+            if (p.cslab == 32)
+              mma_kblock_issue<BN, X3, false, 4>(acc, da, db, a_lo_u, b_lo_u, fresh);
+            else
+              mma_kblock_issue<BN, X3, false, 2>(acc, da, db, a_lo_u, b_lo_u, fresh);
+            if (overlap && i > 0) {
+              wg_wait<1>();
+              release_prev();
+            }
+            if (++sb == p.SB) {
+              sb = 0;
+              pb ^= 1u;
+            }
+            if (++tap == taps) {
+              tap = 0;
+              if (++sa == p.SA) {
+                sa = 0;
+                pa ^= 1u;
+              }
+            }
+            if (!overlap) {
+              wg_wait<0>();
+              release_prev();
             }
           }
-          if (!overlap) {
-            wg_wait<0>();
-            release_prev();
+          wg_wait<0>();
+          if (overlap) release_prev();
+          // two-level accumulation: the tensor core sums `group` K blocks, every finished group is added into fp32
+          // registers with round-to-nearest
+#pragma unroll
+          for (int j = 0; j < (X3 ? BN / 2 : 1); ++j)
+            if (X3) sums[j] += acc[X3 ? j : 0];
+        }
+        if constexpr (FOLD) {
+          // the segment is done: add it to the total and start the next one from zero, as its split-K CTA would
+#pragma unroll
+          for (int j = 0; j < BN / 2; ++j) {
+            tot[j] += sums[j];
+            sums[j] = 0.f;
           }
         }
-        wg_wait<0>();
-        if (overlap) release_prev();
-        // two-level accumulation: the tensor core sums `group` K blocks, every finished group is added into fp32
-        // registers with round-to-nearest
-#pragma unroll
-        for (int j = 0; j < (X3 ? BN / 2 : 1); ++j)
-          if (X3) sums[j] += acc[X3 ? j : 0];
       }
       // x3: the next tile's first wgmma overwrites the accumulator, so it is dead through the epilogue; saying so frees
       // its registers there for the drain and the fused 1x1 (ptxas then spills less, DESIGN §4)
@@ -568,7 +589,9 @@ __global__ void __launch_bounds__(X3 ? (FUSE ? TM_THREADS_X3F : TM_THREADS_X3) :
           epilogue_row<16>(ep, v, valid, m, n, oy, ox, g.n_tile * BN + cb, col_end);
         }
       };
-      if constexpr (X3)
+      if constexpr (FOLD)
+        drain_rows<BN>(tot, dstage, wt, 1 + c, fn);
+      else if constexpr (X3)
         drain_rows<BN>(sums, dstage, wt, 1 + c, fn);
       else
         drain_rows<BN>(acc, dstage, wt, 1 + c, fn);
@@ -730,6 +753,11 @@ bool tma_conv_supported(const IgemmParams& p, int x3) {
   return a_stage + 2 * btile <= TM_BUDGET;
 }
 
+long long conv_tma_image_tiles(const IgemmParams& p, int BN) {
+  const long long positions = p.kh == 3 ? (long long)p.Hin * (p.Win + 2) : (long long)p.Hin * p.Win;
+  return (positions + TM_BM - 1) / TM_BM * (p.CoutPad / BN);
+}
+
 size_t tma_weight_bytes(int Cin, int taps, int CoutPad, int x3) {
   return (size_t)CoutPad * Cin * taps * 4 * (x3 ? 2 : 1);
 }
@@ -796,14 +824,15 @@ int tma_conv_encode(const IgemmParams& p, int Bmax, int cs, void* maps_out) {
   return CP_OK;
 }
 
-template <bool X3, bool FUSE, bool MULTI>
+// FOLD (x3, not fused only): the K segments folded in one CTA per tile (batch-invariant plans)
+template <bool X3, bool FUSE, bool MULTI, bool FOLD = false>
 static int launch_conv_tma_kernel(const TmaConvParams& q, const cudaLaunchConfig_t& cfg0) {
   void (*kern)(TmaConvParams) = nullptr;
   switch (q.BN) {
-    case 16: kern = conv_tma_kernel<X3, FUSE, 16, MULTI>; break;
-    case 32: kern = conv_tma_kernel<X3, FUSE, 32, MULTI>; break;
-    case 64: kern = conv_tma_kernel<X3, FUSE, 64, MULTI>; break;
-    case 128: kern = conv_tma_kernel<X3, FUSE, 128, MULTI>; break;
+    case 16: kern = conv_tma_kernel<X3, FUSE, 16, MULTI, FOLD>; break;
+    case 32: kern = conv_tma_kernel<X3, FUSE, 32, MULTI, FOLD>; break;
+    case 64: kern = conv_tma_kernel<X3, FUSE, 64, MULTI, FOLD>; break;
+    case 128: kern = conv_tma_kernel<X3, FUSE, 128, MULTI, FOLD>; break;
     default: return fail(CP_ERR_INVALID, "conv_tma: unsupported N tile");
   }
   static PerDevice<bool, 4> configured;
@@ -895,9 +924,20 @@ int launch_conv_tma(const IgemmParams& p, const void* maps, const ConvKernel& k,
   if (int rc = device_sm_count(&num_sms)) return rc;
   // split-K (tf32x3, plain epilogue): small feature maps give a persistent kernel fewer tiles than SMs while every tile
   // walks a long serial K loop (level5 at batch 1: 16 tiles x 144 K blocks).  Deal slab-aligned K ranges to more CTAs.
-  q.ksplit = x3 && !q.fuse ? splitk_factor(mn, nslab, num_sms, (size_t)q.tile_m * q.BN, p.splitk_ws_floats) : 1;
+  // Batch-invariant plans fix the segments by the layer's shape (k.ksegments) and split them only when their partial sums
+  // fit the workspace; otherwise one CTA per tile folds them (the FOLD instances of conv_tma_kernel), with the same bits.
+  const size_t tile_floats = (size_t)q.tile_m * q.BN;
+  bool fold = false;
+  if (k.ksegments > 0) {
+    if (nslab % k.ksegments || (k.ksegments > 1 && (!x3 || q.fuse)))
+      return fail(CP_ERR_INVALID, "conv_tma: K segments do not fit the launch");
+    q.ksplit = k.ksegments;
+    fold = q.ksplit > 1 && (size_t)mn * q.ksplit * tile_floats > p.splitk_ws_floats;
+  } else {
+    q.ksplit = x3 && !q.fuse ? splitk_factor(mn, nslab, num_sms, tile_floats, p.splitk_ws_floats) : 1;
+  }
   q.sps = nslab / q.ksplit;
-  q.total_tiles = mn * q.ksplit;
+  q.total_tiles = fold ? mn : mn * q.ksplit;
   if (q.total_tiles >= (1ll << 31)) return fail(CP_ERR_INVALID, "conv_tma: too many tiles");
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3((unsigned)(q.total_tiles < num_sms ? q.total_tiles : num_sms));
@@ -907,7 +947,9 @@ int launch_conv_tma(const IgemmParams& p, const void* maps, const ConvKernel& k,
   // several models in the launch: the model-indexed instantiations; one model runs the one-model code unchanged
   const bool multi = p.B > q.ipm;
   int rc;
-  if (multi)
+  if (fold)
+    rc = multi ? launch_conv_tma_kernel<true, false, true, true>(q, cfg) : launch_conv_tma_kernel<true, false, false, true>(q, cfg);
+  else if (multi)
     rc = x3 ? (q.fuse ? launch_conv_tma_kernel<true, true, true>(q, cfg) : launch_conv_tma_kernel<true, false, true>(q, cfg))
             : (q.fuse ? launch_conv_tma_kernel<false, true, true>(q, cfg) : launch_conv_tma_kernel<false, false, true>(q, cfg));
   else
@@ -918,8 +960,9 @@ int launch_conv_tma(const IgemmParams& p, const void* maps, const ConvKernel& k,
     info->BN = q.BN;
     info->ksplit = q.ksplit;
     info->grid = cfg.gridDim.x;
+    info->path = q.ksplit == 1 ? CP_KPATH_ONE : (fold ? CP_KPATH_FOLD : CP_KPATH_SPLIT);
   }
-  if (q.ksplit > 1) {
+  if (q.ksplit > 1 && !fold) {
     const long long threads = mn * (q.BN / 4) * q.tile_m;
     CP_CUDA_CHECK(launch_kernel(multi ? conv_tma_splitk_finish<true> : conv_tma_splitk_finish<false>,
                                 dim3((unsigned)((threads + 255) / 256)), dim3(256), 0, stream, q, mn));

@@ -120,8 +120,12 @@ __device__ __forceinline__ void coef_row(const DcnTmaParams& p, const float* __r
   }
 }
 
-// MULTI: the launch holds several models (DcnTmaParams::ipm); otherwise the code is that of one model
-template <bool X3, int BN, bool MULTI>
+// MULTI: the launch holds several models (DcnTmaParams::ipm); otherwise the code is that of one model.
+// FOLD (batch-invariant plans): one CTA per (m, n) tile sums the ksplit K segments of `sps` slabs back to back, each
+// exactly as a split-K CTA of that segment does (x3: accumulation groups start at the segment's first K block; tf32:
+// the segment's first wgmma starts a fresh accumulator), and adds them in segment order into a running total,
+// ((0 + seg 0) + seg 1) + ..., as splitk_finish adds the parked partial sums: the same bits on either path.
+template <bool X3, int BN, bool MULTI, bool FOLD>
 __global__ void __launch_bounds__(DT_THREADS, 1) dcn_tma_kernel(const __grid_constant__ DcnTmaParams p) {
   extern __shared__ __align__(1024) unsigned char smem[];
   DcnCtl* ctl = reinterpret_cast<DcnCtl*>(smem);
@@ -137,10 +141,10 @@ __global__ void __launch_bounds__(DT_THREADS, 1) dcn_tma_kernel(const __grid_con
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int n_tiles = p.CoutPad / BN;
-  const int nslab = p.sps;                           // slabs one tile walks (all of them unless split-K)
+  const int nslab = FOLD ? p.sps * p.ksplit : p.sps;  // slabs one tile walks (all of them unless split-K)
   const int KB = nslab * 9;
   const int KB_all = (p.Cin / DT_CS) * 9;
-  const int KS_SPLIT = p.ksplit;
+  const int KS_SPLIT = FOLD ? 1 : p.ksplit;
   const long long total_tiles = p.total_tiles;
 
   if (tid == 0) {
@@ -392,14 +396,22 @@ __global__ void __launch_bounds__(DT_THREADS, 1) dcn_tma_kernel(const __grid_con
     uint32_t pb = 0, cnt = 0;
     float acc[BN / 2];
     float sums[X3 ? BN / 2 : 1];
+    float tot[FOLD ? BN / 2 : 1];      // fold: the running total of the finished K segments
+    const int KB_seg = FOLD ? p.sps * 9 : KB;
 #pragma unroll
     for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
     for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       if (c == 0 && tile + gridDim.x < total_tiles) make_records(tile + gridDim.x);
 #pragma unroll
       for (int j = 0; j < (X3 ? BN / 2 : 1); ++j) sums[j] = 0.f;
+      if constexpr (FOLD) {
+#pragma unroll
+        for (int j = 0; j < BN / 2; ++j) tot[j] = 0.f;
+      }
       int gk = 0;
+      int kseg = 0;                    // fold: K blocks done in the current segment
       for (int kbi = 0; kbi < KB; ++kbi, ++cnt) {
+        const bool seg_end = FOLD ? kseg == KB_seg - 1 : kbi == KB - 1;
         const uint32_t sa = cnt & (uint32_t)(p.AH - 1);
         mbar_wait(bar_a_full + 8u * sa, (cnt >> (p.AH - 1)) & 1u);
         mbar_wait(bar_b_full + 8u * (uint32_t)sb, pb);
@@ -408,7 +420,7 @@ __global__ void __launch_bounds__(DT_THREADS, 1) dcn_tma_kernel(const __grid_con
         if (X3)
           mma_kblock_x3<BN, 2>(acc, a_tile, wt, db, ((uint32_t)BN * 64u) >> 4, gk == 0);
         else
-          mma_kblock<BN, false, false, 2>(acc, make_desc(a_tile, DT_CS), db, 0, 0, kbi == 0);
+          mma_kblock<BN, false, false, 2>(acc, make_desc(a_tile, DT_CS), db, 0, 0, FOLD ? kseg == 0 : kbi == 0);
         if (wt == 0) {
           mbar_arrive(bar_a_empty + 8u * sa);
           mbar_arrive(bar_b_empty + 8u * (uint32_t)sb);
@@ -419,13 +431,28 @@ __global__ void __launch_bounds__(DT_THREADS, 1) dcn_tma_kernel(const __grid_con
         }
         if (X3) {
           // two-level accumulation (see conv_tma.cu): every finished group is added, with round-to-nearest, into sums
-          if (gk == p.group - 1 || kbi == KB - 1) {
+          if (gk == p.group - 1 || seg_end) {
 #pragma unroll
             for (int j = 0; j < (X3 ? BN / 2 : 1); ++j) sums[j] += acc[X3 ? j : 0];
             gk = 0;
           } else {
             ++gk;
           }
+        }
+        if constexpr (FOLD) {
+          // the segment is done: add it to the total; the next one starts from zero, as its split-K CTA would
+          if (seg_end) {
+#pragma unroll
+            for (int j = 0; j < BN / 2; ++j) {
+              if (X3) {
+                tot[j] += sums[X3 ? j : 0];
+                sums[X3 ? j : 0] = 0.f;
+              } else {
+                tot[j] += acc[j];
+              }
+            }
+          }
+          kseg = seg_end ? 0 : kseg + 1;
         }
       }
       const int n_tile = (int)((tile / KS_SPLIT) % n_tiles);
@@ -448,7 +475,9 @@ __global__ void __launch_bounds__(DT_THREADS, 1) dcn_tma_kernel(const __grid_con
           epilogue_row<16>(ep, v, true, m, n, oy, ox, n_tile * BN + cb0, col_end);
         }
       };
-      if constexpr (X3)
+      if constexpr (FOLD)
+        drain_rows<BN>(tot, dstage, wt, 1 + c, fn);
+      else if constexpr (X3)
         drain_rows<BN>(sums, dstage, wt, 1 + c, fn);
       else
         drain_rows<BN>(acc, dstage, wt, 1 + c, fn);
@@ -483,8 +512,29 @@ bool dcn_tma_supported(const IgemmParams& p, int x3) {
   return dcn_tma_tile_n(p.CoutPad, x3) != 0;
 }
 
+long long dcn_tma_image_tiles(const IgemmParams& p, int BN) {
+  return (long long)(p.Win / DT_PW) * (p.Hin / DT_PH) * (p.CoutPad / BN);
+}
+
 int dcn_tma_encode(const IgemmParams& p, int Bmax, void* map_out) {
   return tma_encode_nhwc_box(p.src[0], p.srcC[0], p.Win, p.Hin, Bmax, p.srcStride[0], DT_CS, DT_SW, DT_SH, 1, map_out);
+}
+
+// The instance of one launch (null: no such N tile).  FOLD: the K segments folded in one CTA per tile.
+using DcnTmaKernel = void (*)(DcnTmaParams);
+template <bool FOLD>
+static DcnTmaKernel dcn_tma_kernel_for(int BN, bool x3, bool multi) {
+  switch (BN) {
+    case 16: return multi ? (x3 ? dcn_tma_kernel<true, 16, true, FOLD> : dcn_tma_kernel<false, 16, true, FOLD>)
+                          : (x3 ? dcn_tma_kernel<true, 16, false, FOLD> : dcn_tma_kernel<false, 16, false, FOLD>);
+    case 32: return multi ? (x3 ? dcn_tma_kernel<true, 32, true, FOLD> : dcn_tma_kernel<false, 32, true, FOLD>)
+                          : (x3 ? dcn_tma_kernel<true, 32, false, FOLD> : dcn_tma_kernel<false, 32, false, FOLD>);
+    case 64: return multi ? (x3 ? dcn_tma_kernel<true, 64, true, FOLD> : dcn_tma_kernel<false, 64, true, FOLD>)
+                          : (x3 ? dcn_tma_kernel<true, 64, false, FOLD> : dcn_tma_kernel<false, 64, false, FOLD>);
+    case 128: return multi ? (x3 ? dcn_tma_kernel<true, 128, true, FOLD> : dcn_tma_kernel<false, 128, true, FOLD>)
+                           : (x3 ? dcn_tma_kernel<true, 128, false, FOLD> : dcn_tma_kernel<false, 128, false, FOLD>);
+    default: return nullptr;
+  }
 }
 
 int launch_dcn_tma(const IgemmParams& p, const void* map, const ConvKernel& k, cudaStream_t stream, LaunchInfo* info) {
@@ -539,32 +589,32 @@ int launch_dcn_tma(const IgemmParams& p, const void* map, const ConvKernel& k, c
   q.tstride = p.tstride;
   const bool multi = p.B > q.ipm;      // several models: the model-indexed instantiations
   const size_t smem = fixed + (size_t)q.SB * btile;
-  void (*kern)(DcnTmaParams) = nullptr;
-  switch (q.BN) {
-    case 16: kern = multi ? (x3 ? dcn_tma_kernel<true, 16, true> : dcn_tma_kernel<false, 16, true>)
-                          : (x3 ? dcn_tma_kernel<true, 16, false> : dcn_tma_kernel<false, 16, false>); break;
-    case 32: kern = multi ? (x3 ? dcn_tma_kernel<true, 32, true> : dcn_tma_kernel<false, 32, true>)
-                          : (x3 ? dcn_tma_kernel<true, 32, false> : dcn_tma_kernel<false, 32, false>); break;
-    case 64: kern = multi ? (x3 ? dcn_tma_kernel<true, 64, true> : dcn_tma_kernel<false, 64, true>)
-                          : (x3 ? dcn_tma_kernel<true, 64, false> : dcn_tma_kernel<false, 64, false>); break;
-    case 128: kern = multi ? (x3 ? dcn_tma_kernel<true, 128, true> : dcn_tma_kernel<false, 128, true>)
-                           : (x3 ? dcn_tma_kernel<true, 128, false> : dcn_tma_kernel<false, 128, false>); break;
-    default: return fail(CP_ERR_INVALID, "dcn_tma: unsupported N tile");
+  int num_sms = 0;
+  if (int rc = device_sm_count(&num_sms)) return rc;
+  // split-K: at batch 1 the 512 -> 256 DCN at 16 x 16 is 4 tiles of 288 K blocks; deal slab ranges to idle SMs.
+  // Batch-invariant plans fix the segments by the layer's shape (k.ksegments) and split them only when their partial sums
+  // fit the workspace; otherwise one CTA per tile folds them (the FOLD instances of dcn_tma_kernel), with the same bits.
+  const int nslab = p.Cin / DT_CS;
+  const size_t tile_floats = (size_t)DT_BM * q.BN;
+  bool fold = false;
+  q.part = p.splitk_ws;
+  if (k.ksegments > 0) {
+    if (nslab % k.ksegments) return fail(CP_ERR_INVALID, "dcn_tma: K segments do not fit the launch");
+    q.ksplit = k.ksegments;
+    fold = q.ksplit > 1 && (size_t)mn * q.ksplit * tile_floats > p.splitk_ws_floats;
+  } else {
+    q.ksplit = splitk_factor(mn, nslab, num_sms, tile_floats, p.splitk_ws_floats);
   }
-  static PerDevice<bool, 16> configured;
-  const int slot = (multi ? 8 : 0) + (x3 ? 4 : 0) + (q.BN == 128 ? 3 : (q.BN == 64 ? 2 : (q.BN == 32 ? 1 : 0)));
+  q.sps = nslab / q.ksplit;
+  q.total_tiles = fold ? mn : mn * q.ksplit;
+  const DcnTmaKernel kern = fold ? dcn_tma_kernel_for<true>(q.BN, x3, multi) : dcn_tma_kernel_for<false>(q.BN, x3, multi);
+  if (!kern) return fail(CP_ERR_INVALID, "dcn_tma: unsupported N tile");
+  static PerDevice<bool, 32> configured;
+  const int slot = (fold ? 16 : 0) + (multi ? 8 : 0) + (x3 ? 4 : 0) + (q.BN == 128 ? 3 : (q.BN == 64 ? 2 : (q.BN == 32 ? 1 : 0)));
   if (!configured.here(slot)) {
     CP_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     configured.here(slot) = true;
   }
-  int num_sms = 0;
-  if (int rc = device_sm_count(&num_sms)) return rc;
-  // split-K: at batch 1 the 512 -> 256 DCN at 16 x 16 is 4 tiles of 288 K blocks; deal slab ranges to idle SMs
-  const int nslab = p.Cin / DT_CS;
-  q.part = p.splitk_ws;
-  q.ksplit = splitk_factor(mn, nslab, num_sms, (size_t)DT_BM * q.BN, p.splitk_ws_floats);
-  q.sps = nslab / q.ksplit;
-  q.total_tiles = mn * q.ksplit;
   const unsigned grid = (unsigned)(q.total_tiles < num_sms ? q.total_tiles : num_sms);
   CP_CUDA_CHECK(launch_kernel(kern, dim3(grid), dim3(DT_THREADS), smem, stream, q));
   CP_LAUNCH_CHECK("dcn_tma_kernel");
@@ -572,8 +622,9 @@ int launch_dcn_tma(const IgemmParams& p, const void* map, const ConvKernel& k, c
     info->BN = q.BN;
     info->ksplit = q.ksplit;
     info->grid = grid;
+    info->path = q.ksplit == 1 ? CP_KPATH_ONE : (fold ? CP_KPATH_FOLD : CP_KPATH_SPLIT);
   }
-  if (q.ksplit > 1) {
+  if (q.ksplit > 1 && !fold) {
     const long long threads = mn * (q.BN / 4) * DT_BM;
     CP_CUDA_CHECK(launch_kernel(multi ? dcn_tma_splitk_finish<true> : dcn_tma_splitk_finish<false>, dim3((unsigned)((threads + 255) / 256)), dim3(256), 0, stream, q, mn));
     CP_LAUNCH_CHECK("dcn_tma_splitk_finish");

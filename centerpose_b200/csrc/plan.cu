@@ -69,6 +69,7 @@ struct Op {
   size_t w_off = 0, b_off = 0;
   int w_ld = 0;            // leading dimension of the fp32 packed weight matrix
   ConvKernel kernel;       // chosen before the arena exists (select_kernels)
+  int last_ksplit = 0, last_path = CP_KPATH_NONE;     // what the op's latest launch did (cp_plan_op_ksegments)
   size_t tile_off = 0;     // bytes into the plan's tensor-core weight-tile buffer
   TmaMaps maps;            // conv_tma / dcn_tma: encoded once the arena exists (encode_maps)
   std::vector<int> head_children;   // merged heads 3x3 conv: indices of the per-head 1x1 ops that read its slices
@@ -157,6 +158,7 @@ struct cp_plan {
   // floats.  Without CP_PLAN_REUSE_ACTIVATIONS the offsets are the bump allocation's: every allocation has its own
   // memory.  With it they come from arena_pack(), and an allocation no op touches has none.
   bool reuse = false;
+  bool invariant = false;          // CP_PLAN_BATCH_INVARIANT: every split-capable launch has fixed K segments
   std::vector<ArenaAlloc> bufs;
   std::vector<size_t> buf_off;
 };
@@ -728,6 +730,23 @@ void select_kernels(cp_plan* P) {
     op.fuse_heads = true;
     for (int ci : op.head_children) P->ops[ci].fused_away = true;
   }
+  // CP_PLAN_BATCH_INVARIANT: the K segments of every launch that may split, from the layer's shape alone (fixed_ksegments:
+  // the tiles of one image of one model and the channel slabs).  The default's splits are the x3 conv_tma launches
+  // without the fused 1x1 and every dcn_tma launch; every other launch keeps one segment.
+  for (auto& op : P->ops) {
+    if (op.type != OP_IGEMM) continue;
+    ConvKernel& k = op.kernel;
+    k.ksegments = 0;
+    if (!P->invariant) continue;
+    k.ksegments = 1;
+    if (op.fused_away) continue;           // runs inside its parent's epilogue
+    IgemmParams p;
+    plan_params(P, op, &p);
+    if (k.family == CP_FAM_DCN_TMA)
+      k.ksegments = fixed_ksegments(dcn_tma_image_tiles(p, k.BN), p.Cin / k.cslab);
+    else if (k.family == CP_FAM_CONV_TMA && k.x3 && !op.fuse_heads)
+      k.ksegments = fixed_ksegments(conv_tma_image_tiles(p, k.BN), p.Cin / k.cslab);
+  }
 }
 
 // Every arena tensor op `op` reads or writes when it runs, passed to f as an Act&: none for a fused-away 1x1, the plan's
@@ -838,7 +857,8 @@ int cp_plan_create_multi_track(const cp_config* cfg, int32_t num_models, cp_plan
 static int check_ex_args(const cp_config* cfg, int32_t num_models, uint32_t flags, const char* fn) {
   const std::string f(fn);
   if (!cfg) return fail(CP_ERR_INVALID, f + ": null argument");
-  if (flags & ~(uint32_t)(CP_PLAN_REUSE_ACTIVATIONS | CP_PLAN_MULTI_TRACK)) return fail(CP_ERR_INVALID, f + ": unknown flags");
+  if (flags & ~(uint32_t)(CP_PLAN_REUSE_ACTIVATIONS | CP_PLAN_MULTI_TRACK | CP_PLAN_BATCH_INVARIANT))
+    return fail(CP_ERR_INVALID, f + ": unknown flags");
   if (num_models < 1 || num_models > CP_MAX_MODELS) return fail(CP_ERR_INVALID, f + ": num_models must be in 1..CP_MAX_MODELS");
   if ((flags & CP_PLAN_MULTI_TRACK) && cfg->tracking != 1)
     return fail(CP_ERR_INVALID, f + ": CP_PLAN_MULTI_TRACK needs a tracking config (tracking = 1)");
@@ -881,6 +901,7 @@ static int plan_layout(cp_plan* P, const cp_config* cfg, int32_t num_models, uin
   P->models = num_models;
   P->ext_per_model = (flags & CP_PLAN_MULTI_TRACK) ? kMultiTrackInputs : 0u;
   P->reuse = (flags & CP_PLAN_REUSE_ACTIVATIONS) != 0;
+  P->invariant = (flags & CP_PLAN_BATCH_INVARIANT) != 0;
   P->model_loaded.assign(num_models, 0);
   P->H = cfg->height;
   P->W = cfg->width;
@@ -953,6 +974,28 @@ int cp_plan_allocations(const cp_config* cfg, int32_t num_models, uint32_t flags
     out[i].last = b.last;
   }
   *n_allocs = (int32_t)P.bufs.size();
+  return CP_OK;
+}
+
+int cp_plan_ksegments(const cp_config* cfg, int32_t num_models, uint32_t flags, int32_t* segments, int32_t max_ops,
+                      int32_t* n_ops) {
+  if (!segments || !n_ops) return fail(CP_ERR_INVALID, "cp_plan_ksegments: null argument");
+  if (int rc = check_ex_args(cfg, num_models, flags, "cp_plan_ksegments")) return rc;
+  cp_plan P;
+  if (int rc = plan_layout(&P, cfg, num_models, flags)) return rc;
+  const int n = (int)std::min(P.ops.size(), (size_t)std::max(max_ops, 0));
+  for (int i = 0; i < n; ++i) segments[i] = P.ops[i].type == OP_IGEMM ? P.ops[i].kernel.ksegments : (P.invariant ? 1 : 0);
+  *n_ops = (int32_t)P.ops.size();
+  return CP_OK;
+}
+
+int cp_plan_op_ksegments(const cp_plan* P, int32_t i, int32_t* segments, int32_t* last_segments, int32_t* last_path) {
+  if (!P || !segments) return fail(CP_ERR_INVALID, "cp_plan_op_ksegments: null argument");
+  if (i < 0 || i >= (int)P->ops.size()) return fail(CP_ERR_INVALID, "cp_plan_op_ksegments: op index out of range");
+  const Op& op = P->ops[i];
+  *segments = op.type == OP_IGEMM ? op.kernel.ksegments : (P->invariant ? 1 : 0);
+  if (last_segments) *last_segments = op.last_ksplit;
+  if (last_path) *last_path = op.last_path;
   return CP_OK;
 }
 
@@ -1100,6 +1143,8 @@ static int run_op(cp_plan* P, size_t idx, int batch, const float* const ext[4], 
       li.BN = tc.BN;
       li.ksplit = tc.ksplit;
       li.grid = (int32_t)tc.grid;
+      P->ops[idx].last_ksplit = tc.ksplit;
+      P->ops[idx].last_path = tc.path;
       break;
     }
     case OP_MAXPOOL:

@@ -871,7 +871,7 @@ class MultiCategoryDetector(ObjectPoseDetector):
             eng = Engine(c["arch"], c["heads"], c["head_conv"], max(batch, 1), height, width,
                          dev.index if dev.index is not None else torch.cuda.current_device(), tracking=c["tracking"],
                          tracking_task_gru=c["tracking_task_gru"], precision=c["precision"], models=len(self._weights),
-                         reuse_activations=True)
+                         reuse_activations=True, batch_invariant=c["batch_invariant"])
             for i, sd in enumerate(self._weights):
                 eng.load_state_dict(sd, model=i)
             self._eng = eng
@@ -1005,7 +1005,8 @@ def _load_categories(det, opt, checkpoints, who):
         m = load_model(m, checkpoints[c])
         weights.append({k: v.detach().cpu() for k, v in m.state_dict().items()})
     det._plan_cfg = dict(arch=m._arch(), heads=m.heads, head_conv=m.head_conv, tracking=m.tracking_inputs,
-                         tracking_task_gru=m.use_convGRU and m.tracking_task, precision=m.precision)
+                         tracking_task_gru=m.use_convGRU and m.tracking_task, precision=m.precision,
+                         batch_invariant=m.batch_invariant)
     base = copy.copy(opt)
     base.load_model = ""
     ObjectPoseDetector.__init__(det, base, model=m)

@@ -157,24 +157,38 @@ def _config(arch, heads, head_conv, max_batch, height, width, device_index=0, tr
     return cfg, names
 
 
-def _plan_flags(tracking, models, reuse_activations):
+def _plan_flags(tracking, models, reuse_activations, batch_invariant=False):
     return ((_lib.CP_PLAN_MULTI_TRACK if tracking and models > 1 else 0) |
-            (_lib.CP_PLAN_REUSE_ACTIVATIONS if reuse_activations else 0))
+            (_lib.CP_PLAN_REUSE_ACTIVATIONS if reuse_activations else 0) |
+            (_lib.CP_PLAN_BATCH_INVARIANT if batch_invariant else 0))
 
 
 def plan_memory(arch, heads, head_conv, max_batch, height, width, tracking=False, tracking_task_gru=False,
-                precision="fp32", models=1, reuse_activations=False):
+                precision="fp32", models=1, reuse_activations=False, batch_invariant=False):
     """cp_plan_memory: the device bytes an Engine of these arguments owns, computed on the host without a GPU.
     dict(activation, weights, tiles, workspace, total)."""
     L = _lib.load()
     cfg, keep = _config(arch, dict(heads), head_conv, max_batch, height, width, 0, tracking, tracking_task_gru, precision)
     m = _lib.CpMemoryInfo()
-    _lib.check(L.cp_plan_memory(ctypes.byref(cfg), int(models), _plan_flags(tracking, int(models), reuse_activations),
-                                ctypes.byref(m)), "cp_plan_memory")
+    flags = _plan_flags(tracking, int(models), reuse_activations, batch_invariant)
+    _lib.check(L.cp_plan_memory(ctypes.byref(cfg), int(models), flags, ctypes.byref(m)), "cp_plan_memory")
     out = dict(activation=int(m.activation_bytes), weights=int(m.weight_bytes), tiles=int(m.tile_bytes),
                workspace=int(m.workspace_bytes))
     out["total"] = sum(out.values())
     return out
+
+
+def plan_ksegments(arch, heads, head_conv, max_batch, height, width, tracking=False, tracking_task_gru=False,
+                   precision="fp32", models=1, reuse_activations=False, batch_invariant=False):
+    """cp_plan_ksegments: the K segments of every op of an Engine of these arguments, on the host without a GPU.  With
+    batch_invariant the fixed G of each op (1 where it never splits); without it 0 for every op."""
+    L = _lib.load()
+    cfg, keep = _config(arch, dict(heads), head_conv, max_batch, height, width, 0, tracking, tracking_task_gru, precision)
+    flags = _plan_flags(tracking, int(models), reuse_activations, batch_invariant)
+    n = ctypes.c_int32(0)
+    buf = (ctypes.c_int32 * 1024)()
+    _lib.check(L.cp_plan_ksegments(ctypes.byref(cfg), int(models), flags, buf, 1024, ctypes.byref(n)), "cp_plan_ksegments")
+    return [int(buf[i]) for i in range(min(n.value, 1024))]
 
 
 class Engine(object):
@@ -187,10 +201,14 @@ class Engine(object):
     reuse_activations=True (CP_PLAN_REUSE_ACTIVATIONS) packs the activation arena by liveness: the results are the same
     bits in a fraction of the memory, but the arena no longer holds every layer's output after a call, which the
     per-layer diagnostics (op_descs, arena, run_ops from the middle of the schedule) read.  `memory` is the byte
-    breakdown of the plan (plan_memory)."""
+    breakdown of the plan (plan_memory).
+
+    batch_invariant=True (CP_PLAN_BATCH_INVARIANT) fixes every launch's K reduction by the layer's shape: each frame's
+    outputs are the same bits at any batch, in any row, with any number of models and on any SM count (README, "Batch
+    invariance").  It costs no memory; the default plan is unchanged."""
 
     def __init__(self, arch, heads, head_conv, max_batch, height, width, device_index, tracking=False,
-                 tracking_task_gru=False, precision="fp32", models=1, reuse_activations=False):
+                 tracking_task_gru=False, precision="fp32", models=1, reuse_activations=False, batch_invariant=False):
         self.L = _lib.load()
         self.models = int(models)
         self.heads = dict(heads)
@@ -199,11 +217,12 @@ class Engine(object):
         self.device = torch.device("cuda", device_index)
         self.tracking = bool(tracking)
         self.reuse_activations = bool(reuse_activations)
+        self.batch_invariant = bool(batch_invariant)
         cfg, self._names = _config(arch, self.heads, head_conv, max_batch, height, width, device_index, tracking,
                                    tracking_task_gru, precision)
         self._cfg = cfg
         plan = ctypes.c_void_p()
-        flags = _plan_flags(self.tracking, self.models, self.reuse_activations)
+        flags = _plan_flags(self.tracking, self.models, self.reuse_activations, self.batch_invariant)
         with torch.cuda.device(self.device):
             _lib.check(self.L.cp_plan_create_ex(ctypes.byref(cfg), self.models, flags, ctypes.byref(plan)), "cp_plan_create")
         self.plan = plan
@@ -211,7 +230,7 @@ class Engine(object):
         self.forward_launches = int(self.L.cp_plan_forward_launches(plan))
         self.plan_bytes = int(self.L.cp_plan_bytes(plan))
         self.memory = plan_memory(arch, heads, head_conv, max_batch, height, width, tracking, tracking_task_gru, precision,
-                                  self.models, self.reuse_activations)
+                                  self.models, self.reuse_activations, self.batch_invariant)
 
     def close(self):
         if getattr(self, "plan", None):
@@ -366,6 +385,14 @@ class Engine(object):
         _lib.check(rc, "cp_plan_run_ops")
         return [dict(family=int(info[i].family), BN=int(info[i].BN), ksplit=int(info[i].ksplit),
                      grid=int(info[i].grid)) for i in range(n)]
+
+    def op_ksegments(self, i):
+        """cp_plan_op_ksegments of op i: dict(segments = the fixed G of a batch-invariant plan, 0 in a default one;
+        last_segments, last_path = the split-K factor and cp_kpath (_lib.KPATH_*) of the op's latest launch)."""
+        g, ls, lp = ctypes.c_int32(), ctypes.c_int32(), ctypes.c_int32()
+        _lib.check(self.L.cp_plan_op_ksegments(self.plan, int(i), ctypes.byref(g), ctypes.byref(ls), ctypes.byref(lp)),
+                   "cp_plan_op_ksegments")
+        return dict(segments=int(g.value), last_segments=int(ls.value), last_path=int(lp.value))
 
     def infer(self, x, meta, prm, pre_img=None, pre_hm=None, pre_hm_hp=None, heads_out=None, want_dets=False,
               poses=None, n_valid=None, dets=None):

@@ -48,13 +48,14 @@ class _SlotGraph(object):
             c, M = det._plan_cfg, len(det.categories)
             eng = Engine(c["arch"], c["heads"], c["head_conv"], S, ih, iw, self.device.index, tracking=c["tracking"],
                          tracking_task_gru=c["tracking_task_gru"], precision=c["precision"], models=M,
-                         reuse_activations=True)
+                         reuse_activations=True, batch_invariant=c["batch_invariant"])
             for m, sd in enumerate(det._weights):
                 eng.load_state_dict(sd, model=m)
             return eng, (list(det._prms) if M > 1 else det._prms[0]), list(det.categories)
         m = det.model
         eng = Engine(m._arch(), m.heads, m.head_conv, S, ih, iw, self.device.index, tracking=m.tracking_inputs,
-                     tracking_task_gru=m.use_convGRU and m.tracking_task, precision=m.precision, reuse_activations=True)
+                     tracking_task_gru=m.use_convGRU and m.tracking_task, precision=m.precision, reuse_activations=True,
+                     batch_invariant=m.batch_invariant)
         eng.load_state_dict(m.state_dict())
         return eng, decode_params(det.opt, test_scale=1.0), None
 

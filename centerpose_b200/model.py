@@ -136,14 +136,15 @@ class _NativeNet(nn.Module):
         if device.type != "cuda":
             raise RuntimeError("centerpose_b200: the network only runs on CUDA (sm_90a); "
                                "there is no CPU fallback -- move the model with .to('cuda')")
-        key = (height, width, device.index if device.index is not None else torch.cuda.current_device(), self.precision)
+        key = (height, width, device.index if device.index is not None else torch.cuda.current_device(), self.precision,
+               self.batch_invariant)
         eng = self._engines.get(key)
         if eng is None or eng.max_batch < batch:
             if eng is not None:
                 eng.close()
             eng = Engine(self._arch(), self.heads, self.head_conv, max(batch, 1), height, width, key[2],
                          tracking=self.tracking_inputs, tracking_task_gru=self.use_convGRU and self.tracking_task,
-                         precision=self.precision, reuse_activations=True)
+                         precision=self.precision, reuse_activations=True, batch_invariant=self.batch_invariant)
             eng.weights_sig = None
             self._engines[key] = eng
         sig = self._signature()
@@ -175,7 +176,8 @@ class DLASegB200(_NativeNet):
 
     `precision` selects the kernels of the plan (include/centerpose_b200.h cp_precision): "tf32x3" (default: wgmma
     3-term split with promoted accumulation, fp32-equivalent - meets the same parity bar as "fp32"), "fp32" (CUDA-core
-    FFMA), "tf32" (wgmma single pass), "bf16"."""
+    FFMA), "tf32" (wgmma single pass), "bf16".  `batch_invariant` (from opt.batch_invariant, default False) makes every
+    plan of the network batch-invariant (Engine batch_invariant): a frame's outputs are the same bits at any batch."""
 
     def __init__(self, heads, head_conv=256, use_convGRU=False, opt=None, precision="tf32x3"):
         super().__init__()
@@ -189,6 +191,7 @@ class DLASegB200(_NativeNet):
                              "pre_img + pre_hm + pre_hm_hp set (demo.py:117-123)")
         self.tracking_task = _flag(opt, "tracking_task")
         self.precision = precision
+        self.batch_invariant = bool(getattr(opt, "batch_invariant", False))
         if head_conv <= 0:
             raise ValueError("head_conv must be > 0 (the reference's DLA default is 256, opts.py:344-345)")
 
@@ -309,6 +312,7 @@ class PoseResNetB200(_NativeNet):
                              "pre_img + pre_hm + pre_hm_hp set (demo.py:117-123)")
         self.tracking_task = _flag(opt, "tracking_task")
         self.precision = precision
+        self.batch_invariant = bool(getattr(opt, "batch_invariant", False))
 
         bottleneck, blocks = _RESNET_SPEC[num_layers]
         self.conv1 = nn.Conv2d(3, 64, 7, 2, 3, bias=False)

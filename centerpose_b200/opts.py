@@ -10,7 +10,7 @@ CATEGORIES = ("bike", "book", "bottle", "camera", "cereal_box", "chair", "cup", 
 
 
 def default_opt(arch="dla_34", tracking_task=False, rep_mode=1, c="chair", gpus="0", K=100,
-                vis_thresh=0.3, show_axes=False, load_model="", input_res=512, debug=0):
+                vis_thresh=0.3, show_axes=False, load_model="", input_res=512, debug=0, batch_invariant=False):
     o = SimpleNamespace()
     o.task = "object_pose"                 # opts.py:19
     o.dataset = "objectron"
@@ -24,6 +24,7 @@ def default_opt(arch="dla_34", tracking_task=False, rep_mode=1, c="chair", gpus=
     o.show_axes = show_axes
     o.load_model = load_model
     o.debug = debug
+    o.batch_invariant = bool(batch_invariant)     # CP_PLAN_BATCH_INVARIANT plans (README, "Batch invariance")
     o.gpus = [0] if not str(gpus).startswith("-") else [-1]
     o.test_scales = [1.0]                  # opts.py:116
     o.fix_res = True                       # not keep_res (opts.py:337)

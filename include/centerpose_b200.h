@@ -141,9 +141,20 @@ int cp_plan_create_multi_track(const cp_config* cfg, int32_t num_models, cp_plan
  *   (the merged heads' hidden tile when the 1x1s are fused into its epilogue) reports off = -1, and cp_plan_run_ops is
  *   valid for op ranges whose inputs are still live, for example when stepping from op 0 in order.
  * CP_PLAN_MULTI_TRACK: the per-model pre_hm / pre_hm_hp layout of cp_plan_create_multi_track (needs cfg->tracking = 1;
- *   a tracking config of several models needs it). */
+ *   a tracking config of several models needs it).
+ * CP_PLAN_BATCH_INVARIANT: every output element is the same bits whatever the batch of the call, the frame's row in it,
+ *   the number of models in the plan and the device's SM count.  By default the tf32x3 conv_tma launches (not fused) and
+ *   the dcn_tma launches split their K loop over a number of CTAs chosen from the launch's tiles and the SM count, so a
+ *   frame's sums depend on its batch.  With the flag every such launch cuts K into G segments fixed by the layer's shape
+ *   (G: the largest divisor of the launch's channel slabs with G x the (m, n) tiles of one image of one model <= 132; 1
+ *   wherever the default never splits), sums each segment as a split CTA of it does and adds the segments in order,
+ *   ((0 + seg 0) + seg 1) + ..., before the epilogue.  The segments run on separate CTAs when their partial sums fit the
+ *   plan's split-K workspace and back to back in one CTA per tile otherwise; the choice never changes a bit
+ *   (cp_plan_op_ksegments reports it).  G is what the default picks at batch 1 on a 132-SM H100, so there the flag gives
+ *   the bits of a batch-1 call of a default plan.  It adds no memory; fp32 and bf16 plans accept it and are unchanged. */
 #define CP_PLAN_REUSE_ACTIVATIONS 1u
 #define CP_PLAN_MULTI_TRACK 2u
+#define CP_PLAN_BATCH_INVARIANT 32u
 /* cp_plan_create_multi (flags 0) or cp_plan_create_multi_track (CP_PLAN_MULTI_TRACK) with flags; unknown flag bits return
  * CP_ERR_INVALID.  The three creators above are this call with those flags. */
 int cp_plan_create_ex(const cp_config* cfg, int32_t num_models, uint32_t flags, cp_plan** out);
@@ -271,6 +282,21 @@ typedef struct cp_op_launch {
   int32_t ksplit;           /* split-K factor (1 = off)                                                            */
   int32_t grid;             /* CTAs of the main kernel (tensor-core families; 0 otherwise)                         */
 } cp_op_launch;
+/* How a launch summed its K segments (cp_plan_op_ksegments). */
+enum cp_kpath {
+  CP_KPATH_NONE = 0,        /* not a conv_tma / dcn_tma launch, or not launched yet                                   */
+  CP_KPATH_ONE = 1,         /* one segment: each (m, n) tile on one CTA over the whole K                               */
+  CP_KPATH_SPLIT = 2,       /* split-K: one CTA per (tile, segment), partial sums added by the finish kernel           */
+  CP_KPATH_FOLD = 3         /* CP_PLAN_BATCH_INVARIANT: one CTA per tile runs the segments back to back                */
+};
+/* Op i's K segments: *segments receives the G of a CP_PLAN_BATCH_INVARIANT plan (1 where it never splits) and 0 for
+ * every op of a default plan, whose launches choose; *last_segments and *last_path (either may be NULL) what the op's
+ * latest launch (cp_forward, cp_infer*, cp_plan_run_ops ...) did: its split-K factor and a cp_kpath. */
+int cp_plan_op_ksegments(const cp_plan* plan, int32_t i, int32_t* segments, int32_t* last_segments, int32_t* last_path);
+/* The segments of every op of a plan of these arguments, as cp_plan_op_ksegments' *segments, computed on the host
+ * without a device (like cp_plan_memory).  Fills the first max_ops entries at most; *n_ops receives cp_plan_num_ops. */
+int cp_plan_ksegments(const cp_config* cfg, int32_t num_models, uint32_t flags, int32_t* segments, int32_t max_ops,
+                      int32_t* n_ops);
 int cp_plan_op_desc(const cp_plan* plan, int32_t i, cp_op_desc* out);
 /* op i as model `model` of a multi-model plan sees it: its weight, bias, up-sample and GroupNorm pointers, and
  * activation offsets moved to its images for a call at the plan's max_batch (model m's images start at image
