@@ -18,8 +18,8 @@
 //
 //   warp 0        : TMA producer for slabs
 //   warp 1        : weight-tile producer (cp.async.bulk, pre-swizzled tiles)
-//   warps 4-7     : consumer of tile rows [0, 64) (wgmma into registers + epilogue); thread i also writes the sampling
-//                   records (one 16-byte record per tap) of position i of the NEXT tile
+//   warps 2-3     : sampling records (one 16-byte record per tap and position) of each tile, a tile ahead of the gather
+//   warps 4-7     : consumer of tile rows [0, 64) (wgmma into registers + epilogue)
 //   warps 8-11    : gather, one thread per position: 4 corners x 16 channels from the slab -> bilinear blend * mask ->
 //                   A tile in the SWIZZLE_64B K-major layout (tf32-rounded; fp32 in x3, where the consumers split it
 //                   into hi / lo in registers), AH A stages
@@ -42,6 +42,8 @@ constexpr int DT_HALO = 8;           // slab margin around the patch, both direc
 constexpr int DT_SH = DT_PH + 2 * DT_HALO, DT_SW = DT_PW + 2 * DT_HALO;     // slab rows x columns (24 x 32)
 constexpr uint32_t DT_SLAB_BYTES = DT_SH * DT_SW * DT_CS * 4;               // 49152
 constexpr uint32_t DT_COEF_BYTES = DT_BM * 9 * 16;
+constexpr int DT_GROUP = kX3GroupBlocks * 2;     // x3: 16-channel K blocks per accumulation group (conv_tma.cu's MMA count)
+static_assert(DT_GROUP == 2, "the x3 consumer holds the A fragments of at most two K blocks");
 
 struct DcnTmaParams {
   CUtensorMap amap;
@@ -53,8 +55,7 @@ struct DcnTmaParams {
   int tiles_x, tiles_per_image;      // patches per image row / per image
   long long total_tiles;             // m tiles x n tiles (n fastest)
   int SB;
-  int group;                         // x3: K blocks (16 channels) per accumulation group
-  int AH;                            // A stages (1 or 2)
+  int AH;                            // A stages (1, 2 or 4)
   const float* bias;
   const float* residual;
   int resStride, relu, res_after_relu;
@@ -71,7 +72,7 @@ struct DcnTmaParams {
 
 struct DcnCtl {
   unsigned long long s_full[2], s_empty[2];
-  unsigned long long a_full[2], a_empty[2];
+  unsigned long long a_full[4], a_empty[4];
   unsigned long long c_full[2], c_empty[2];
   unsigned long long b_full[8], b_empty[8];
 };
@@ -82,19 +83,17 @@ struct DcnCtl {
 constexpr int RB_DX = 14, RB_DY = 15, RB_W = 16, RB_SLAB = 20, RB_LIVE = 21;
 
 // Sampling records of one output position (all 9 taps) -> shared memory.  dcn_v2_im2col_cuda.cu:160-195: the sample
-// (h_im, w_im) is used only when it lies in (-1, H) x (-1, W); every corner carries its own bounds test.
+// (h_im, w_im) is used only when it lies in (-1, H) x (-1, W); every corner carries its own bounds test.  The offsets
+// and the mask are loaded tap by tap: the record warps run with 48 registers.
 __device__ __forceinline__ void coef_row(const DcnTmaParams& p, const float* __restrict__ om, int oy, int ox, int ys,
                                          int xs, uint32_t dst) {
-  float o[27];
-#pragma unroll
-  for (int j = 0; j < 27; ++j) o[j] = __ldg(om + j);
   const int H = p.H, W = p.W;
 #pragma unroll
   for (int tap = 0; tap < 9; ++tap) {
     const int ky = tap / 3, kx = tap - ky * 3;
-    float mm = o[18 + tap];
+    float mm = __ldg(om + 18 + tap);
     if (p.mask_is_logit) mm = 1.0f / (1.0f + expf(-mm));
-    const float h_im = (float)(oy - 1 + ky) + o[2 * tap], w_im = (float)(ox - 1 + kx) + o[2 * tap + 1];
+    const float h_im = (float)(oy - 1 + ky) + __ldg(om + 2 * tap), w_im = (float)(ox - 1 + kx) + __ldg(om + 2 * tap + 1);
     float lh = 0.f, lw = 0.f, mk = 0.f;
     uint32_t pk = 0;
     if (h_im > -1.f && w_im > -1.f && h_im < (float)H && w_im < (float)W) {
@@ -146,17 +145,18 @@ __global__ void __launch_bounds__(DT_THREADS, 1) dcn_tma_kernel(const __grid_con
   const int KB_all = (p.Cin / DT_CS) * 9;
   const int KS_SPLIT = FOLD ? 1 : p.ksplit;
   const long long total_tiles = p.total_tiles;
+  const uint32_t ah_log = (uint32_t)(31 - __clz(p.AH));      // K block n uses A stage n % AH, in round n / AH
 
   if (tid == 0) {
     for (int s = 0; s < 2; ++s) {
       mbar_init(smem_u32(&ctl->s_full[s]), 1);
       mbar_init(smem_u32(&ctl->s_empty[s]), 4);             // one arrival per gather warp
-      mbar_init(smem_u32(&ctl->c_full[s]), 4);              // one arrival per record-writing warp (4-7)
+      mbar_init(smem_u32(&ctl->c_full[s]), 2);              // one arrival per record warp (2, 3)
       mbar_init(smem_u32(&ctl->c_empty[s]), 4);
     }
     for (int s = 0; s < p.AH; ++s) {
       mbar_init(smem_u32(&ctl->a_full[s]), 4);              // written by the four gather warps
-      mbar_init(smem_u32(&ctl->a_empty[s]), 2);             // released by both consumer warpgroups
+      mbar_init(smem_u32(&ctl->a_empty[s]), 8);             // released by every consumer warp
     }
     for (int s = 0; s < p.SB; ++s) {
       mbar_init(smem_u32(&ctl->b_full[s]), 1);
@@ -171,7 +171,7 @@ __global__ void __launch_bounds__(DT_THREADS, 1) dcn_tma_kernel(const __grid_con
 
   if (warp < 4) {
     // the control warpgroup hands registers to the consumers (a 64 x BN accumulator + the x3 running sums)
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 48;");
     if (warp == 0) {
       // ===================== slabs via TMA =====================
       if (lane == 0) {
@@ -197,6 +197,31 @@ __global__ void __launch_bounds__(DT_THREADS, 1) dcn_tma_kernel(const __grid_con
         }
       }
       __syncwarp();
+    } else if (warp >= 2) {
+      // ===================== sampling records: thread t writes positions t and t + 64 of every tile into the record
+      // buffer the gather freed last (double-buffered), while the gather and the consumers work on the tile before
+      const int rt = tid - 64;
+      int cb = 0;
+      uint32_t pc = 0;
+      for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+        const long long m_tile = (tile / KS_SPLIT) / n_tiles;
+        const int img = (int)(m_tile / p.tiles_per_image);
+        const int pt = (int)(m_tile - (long long)img * p.tiles_per_image);
+        const int y0 = (pt / p.tiles_x) * DT_PH, x0 = (pt % p.tiles_x) * DT_PW;
+        mbar_wait(smem_u32(&ctl->c_empty[cb]), pc ^ 1u);
+#pragma unroll 1
+        for (int i = rt; i < DT_BM; i += 64) {
+          const int oy = y0 + (i >> 4), ox = x0 + (i & 15);
+          coef_row(p, p.offmask + ((size_t)((size_t)img * p.H + oy) * p.W + ox) * p.omStride, oy, ox, y0 - DT_HALO,
+                   x0 - DT_HALO, coef0 + (uint32_t)cb * DT_COEF_BYTES + (uint32_t)i * 144u);
+        }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(smem_u32(&ctl->c_full[cb]));
+        if (++cb == 2) {
+          cb = 0;
+          pc ^= 1u;
+        }
+      }
     } else if (warp == 1) {
       // ===================== weight tiles =====================
       if (lane == 0) {
@@ -222,8 +247,8 @@ __global__ void __launch_bounds__(DT_THREADS, 1) dcn_tma_kernel(const __grid_con
       __syncwarp();
     }
   } else if (warp >= 8 && warp < 12) {
-    // 128 x 40 + 128 x 120 + 256 x 176 = 64 K registers: the consumers also hold the hi / lo A fragments of a K block
-    asm volatile("setmaxnreg.dec.sync.aligned.u32 120;");
+    // 128 x 48 + 128 x 112 + 256 x 176 = 64 K registers: the consumers also hold the hi / lo A fragments of two K blocks
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 112;");
     // ===================== gather: thread = one position of the tile; the record of a (position, tap) is decoded once
     // for all 16 channels and a stage is synchronised once per K block =====================
     const int gt = tid - 256;
@@ -232,7 +257,7 @@ __global__ void __launch_bounds__(DT_THREADS, 1) dcn_tma_kernel(const __grid_con
     const uint32_t asw = (uint32_t)(row >> 1) & 3u;
     int ss = 0, cb = 0;
     uint32_t ps = 0, pc = 0;
-    uint32_t cnt = 0;                      // K blocks produced; stage = cnt % AH
+    uint32_t cnt = 0;                      // K blocks produced
     for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       const long long m_tile = (tile / KS_SPLIT) / n_tiles;
       const int s0 = (int)(tile % KS_SPLIT) * nslab;
@@ -322,7 +347,7 @@ __global__ void __launch_bounds__(DT_THREADS, 1) dcn_tma_kernel(const __grid_con
         }
         const int sa = (int)(cnt & (uint32_t)(p.AH - 1));          // barrier index == tile slot
         const uint32_t a_dst = a_row + (uint32_t)sa * a_stage + (asw << 4);      // chunk c -> a_dst ^ (c << 4)
-        mbar_wait(smem_u32(&ctl->a_empty[sa]), ((cnt >> (p.AH - 1)) & 1u) ^ 1u);
+        mbar_wait(smem_u32(&ctl->a_empty[sa]), ((cnt >> ah_log) & 1u) ^ 1u);
 #pragma unroll
         for (int c = 0; c < 4; ++c) {
           const uint32_t off = (uint32_t)c << 4;
@@ -331,7 +356,7 @@ __global__ void __launch_bounds__(DT_THREADS, 1) dcn_tma_kernel(const __grid_con
           else
             st_shared_v4f(a_dst ^ off, tf32_round(v[c].x), tf32_round(v[c].y), tf32_round(v[c].z), tf32_round(v[c].w));
         }
-        fence_proxy_async_smem();
+        if (!X3) fence_proxy_async_smem();      // tf32: the wgmmas read A through the async proxy; x3 reads it with ldmatrix
         __syncwarp();
         if (lane == 0) mbar_arrive(smem_u32(&ctl->a_full[sa]));
         ++cnt;
@@ -369,31 +394,34 @@ __global__ void __launch_bounds__(DT_THREADS, 1) dcn_tma_kernel(const __grid_con
     ep.CoutPad = p.CoutPad;
     ep.H = p.H;
     ep.W = p.W;
-    // Warpgroup 0 is idle while the gather runs, and its thread i == position i: it also prepares the sampling records
-    // of the NEXT tile (double-buffered), so the gather warps never wait for them.
-    int cb = 0;
-    uint32_t pc = 0;
-    auto make_records = [&](long long t) {
-      const long long mt = (t / KS_SPLIT) / n_tiles;
-      const int im = (int)(mt / p.tiles_per_image);
-      const int pt = (int)(mt - (long long)im * p.tiles_per_image);
-      const int y0 = (pt / p.tiles_x) * DT_PH, x0 = (pt % p.tiles_x) * DT_PW;
-      const int oy = y0 + (wt >> 4), ox = x0 + (wt & 15);
-      mbar_wait(smem_u32(&ctl->c_empty[cb]), pc ^ 1u);
-      coef_row(p, p.offmask + ((size_t)((size_t)im * p.H + oy) * p.W + ox) * p.omStride, oy, ox, y0 - DT_HALO, x0 - DT_HALO,
-               coef0 + (uint32_t)cb * DT_COEF_BYTES + (uint32_t)wt * 144u);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(smem_u32(&ctl->c_full[cb]));
-      if (++cb == 2) {
-        cb = 0;
-        pc ^= 1u;
-      }
-    };
-    if (c == 0 && (long long)blockIdx.x < total_tiles) make_records(blockIdx.x);
     const uint32_t bar_a_full = smem_u32(&ctl->a_full[0]), bar_a_empty = smem_u32(&ctl->a_empty[0]);
     const uint32_t bar_b_full = smem_u32(&ctl->b_full[0]), bar_b_empty = smem_u32(&ctl->b_empty[0]);
+    const uint32_t b_lo = ((uint32_t)BN * 64u) >> 4;
     int sb = 0;
     uint32_t pb = 0, cnt = 0;
+    // K block n's A stage: this warpgroup's half once it is written; each warp releases it on its own
+    auto a_wait = [&](uint32_t n) {
+      const uint32_t sa = n & (uint32_t)(p.AH - 1);
+      mbar_wait(bar_a_full + 8u * sa, (n >> ah_log) & 1u);
+      return atiles0 + sa * a_stage + (uint32_t)c * 64u * 64u;
+    };
+    auto a_release = [&](uint32_t n) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_a_empty + 8u * (n & (uint32_t)(p.AH - 1)));
+    };
+    // the next weight stage: waits for it, returns its descriptor and its index (for the release)
+    auto b_wait = [&](int& st) {
+      mbar_wait(bar_b_full + 8u * (uint32_t)sb, pb);
+      st = sb;
+      if (++sb == p.SB) {
+        sb = 0;
+        pb ^= 1u;
+      }
+      return make_desc(btiles0 + (uint32_t)st * btile_bytes, DT_CS);
+    };
+    auto b_release = [&](int st) {
+      if (wt == 0) mbar_arrive(bar_b_empty + 8u * (uint32_t)st);
+    };
     float acc[BN / 2];
     float sums[X3 ? BN / 2 : 1];
     float tot[FOLD ? BN / 2 : 1];      // fold: the running total of the finished K segments
@@ -401,47 +429,68 @@ __global__ void __launch_bounds__(DT_THREADS, 1) dcn_tma_kernel(const __grid_con
 #pragma unroll
     for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
     for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
-      if (c == 0 && tile + gridDim.x < total_tiles) make_records(tile + gridDim.x);
 #pragma unroll
       for (int j = 0; j < (X3 ? BN / 2 : 1); ++j) sums[j] = 0.f;
       if constexpr (FOLD) {
 #pragma unroll
         for (int j = 0; j < BN / 2; ++j) tot[j] = 0.f;
       }
-      int gk = 0;
       int kseg = 0;                    // fold: K blocks done in the current segment
-      for (int kbi = 0; kbi < KB; ++kbi, ++cnt) {
-        const bool seg_end = FOLD ? kseg == KB_seg - 1 : kbi == KB - 1;
-        const uint32_t sa = cnt & (uint32_t)(p.AH - 1);
-        mbar_wait(bar_a_full + 8u * sa, (cnt >> (p.AH - 1)) & 1u);
-        mbar_wait(bar_b_full + 8u * (uint32_t)sb, pb);
-        const uint32_t a_tile = atiles0 + sa * a_stage + (uint32_t)c * 64u * 64u;
-        const uint64_t db = make_desc(btiles0 + (uint32_t)sb * btile_bytes, DT_CS);
-        if (X3)
-          mma_kblock_x3<BN, 2>(acc, a_tile, wt, db, ((uint32_t)BN * 64u) >> 4, gk == 0);
-        else
-          mma_kblock<BN, false, false, 2>(acc, make_desc(a_tile, DT_CS), db, 0, 0, FOLD ? kseg == 0 : kbi == 0);
-        if (wt == 0) {
-          mbar_arrive(bar_a_empty + 8u * sa);
-          mbar_arrive(bar_b_empty + 8u * (uint32_t)sb);
+      // one accumulation group per step (x3: DT_GROUP K blocks, fewer at the end of a K segment; tf32: one K block)
+      for (int kbi = 0; kbi < KB;) {
+        const int left = FOLD ? KB_seg - kseg : KB - kbi;
+        const int ng = X3 ? min(left, DT_GROUP) : 1;
+        if constexpr (X3 && BN <= 64) {
+          // the group's two K blocks are issued back to back on the accumulator and waited for once; each A stage is
+          // released as soon as its fragments are in registers
+          uint32_t hi0[2][4], lo0[2][4], hi1[2][4], lo1[2][4];
+          int st0, st1 = 0;
+          x3_load_a<2>(hi0, lo0, a_wait(cnt), wt);
+          a_release(cnt);
+          x3_issue<BN, 2>(acc, hi0, lo0, b_wait(st0), b_lo, true);
+          if (ng == 2) {
+            x3_load_a<2>(hi1, lo1, a_wait(cnt + 1), wt);
+            a_release(cnt + 1);
+            x3_issue<BN, 2>(acc, hi1, lo1, b_wait(st1), b_lo, false);
+          }
+          wg_wait<0>();
+          x3_keep<2>(hi0, lo0);
+          b_release(st0);
+          if (ng == 2) {
+            x3_keep<2>(hi1, lo1);
+            b_release(st1);
+          }
+        } else if constexpr (X3) {
+          // BN = 128: the fragments of a second K block do not fit beside the accumulator; each K block is waited for
+          for (int g = 0; g < ng; ++g) {
+            uint32_t hi[2][4], lo[2][4];
+            int st;
+            x3_load_a<2>(hi, lo, a_wait(cnt + g), wt);
+            a_release(cnt + g);
+            x3_issue<BN, 2>(acc, hi, lo, b_wait(st), b_lo, g == 0);
+            wg_wait<0>();
+            x3_keep<2>(hi, lo);
+            b_release(st);
+          }
+        } else {
+          // single pass: the wgmmas read A from shared memory, so its stage is released after the wait
+          int st;
+          const uint64_t da = make_desc(a_wait(cnt), DT_CS);
+          mma_kblock<BN, false, false, 2>(acc, da, b_wait(st), 0, 0, FOLD ? kseg == 0 : kbi == 0);
+          a_release(cnt);
+          b_release(st);
         }
-        if (++sb == p.SB) {
-          sb = 0;
-          pb ^= 1u;
-        }
+        cnt += (uint32_t)ng;
+        kbi += ng;
         if (X3) {
           // two-level accumulation (see conv_tma.cu): every finished group is added, with round-to-nearest, into sums
-          if (gk == p.group - 1 || seg_end) {
 #pragma unroll
-            for (int j = 0; j < (X3 ? BN / 2 : 1); ++j) sums[j] += acc[X3 ? j : 0];
-            gk = 0;
-          } else {
-            ++gk;
-          }
+          for (int j = 0; j < (X3 ? BN / 2 : 1); ++j) sums[j] += acc[X3 ? j : 0];
         }
         if constexpr (FOLD) {
           // the segment is done: add it to the total; the next one starts from zero, as its split-K CTA would
-          if (seg_end) {
+          kseg += ng;
+          if (kseg == KB_seg) {
 #pragma unroll
             for (int j = 0; j < BN / 2; ++j) {
               if (X3) {
@@ -451,8 +500,8 @@ __global__ void __launch_bounds__(DT_THREADS, 1) dcn_tma_kernel(const __grid_con
                 tot[j] += acc[j];
               }
             }
+            kseg = 0;
           }
-          kseg = seg_end ? 0 : kseg + 1;
         }
       }
       const int n_tile = (int)((tile / KS_SPLIT) % n_tiles);
@@ -560,16 +609,15 @@ int launch_dcn_tma(const IgemmParams& p, const void* map, const ConvKernel& k, c
   q.tiles_per_image = q.tiles_x * (p.Hin / DT_PH);
   const long long mn = (long long)q.tiles_per_image * p.B * (p.CoutPad / q.BN);
   const uint32_t a_stage = 8192u;
-  q.group = kX3GroupBlocks * 2;      // 16-channel K blocks: same MMA count per group as conv_tma.cu
   const uint32_t btile = (uint32_t)q.BN * 64u * (x3 ? 2u : 1u);
   const size_t budget = 226 * 1024;
-  // two A stages where >= 3 weight stages still fit, else one
-  q.AH = 2;
+  // the deepest A ring (4, 2 or 1 stages) beside which >= 3 weight stages still fit
+  q.AH = 4;
   size_t fixed = 1024 + 2 * (size_t)DT_COEF_BYTES + 1024 + 2 * (size_t)DT_SLAB_BYTES + (size_t)q.AH * a_stage +
                  2 * (size_t)DRAIN_STAGE_BYTES;
-  if (fixed + 3 * (size_t)btile > budget) {
-    q.AH = 1;
-    fixed -= a_stage;
+  while (q.AH > 1 && fixed + 3 * (size_t)btile > budget) {
+    q.AH >>= 1;
+    fixed -= (size_t)q.AH * a_stage;
   }
   if (fixed + 2 * (size_t)btile > budget) return fail(CP_ERR_INVALID, "dcn_tma: tile does not fit shared memory");
   q.SB = (int)((budget - fixed) / btile);

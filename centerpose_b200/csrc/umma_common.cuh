@@ -224,17 +224,19 @@ __device__ __forceinline__ void ldsm_x4(uint32_t (&r)[4], uint32_t addr) {
 // split there; B keeps its hi tile at `db` and its lo tile `b_lo` descriptor units further.  The A tile is K-major with
 // rows of 32 KS bytes (KS = 4: SWIZZLE_128B, KS = 2: SWIZZLE_64B), row 0 at `a_tile` (a multiple of the row size; the
 // XOR comes from the address bits, as in make_desc).  wt: thread in the warpgroup.  fresh: the first product
-// overwrites the accumulator.  Returns when the products are in `acc` and the operand tiles may be reused.
-template <int BN, int KS>
-__device__ __forceinline__ void mma_kblock_x3(float (&acc)[BN / 2], uint32_t a_tile, int wt, uint64_t db, uint32_t b_lo,
-                                              bool fresh) {
+// overwrites the accumulator.
+//
+// In three steps, so that a caller can release the A tile as soon as it is in registers and keep several K blocks in
+// flight: x3_load_a reads and splits this thread's fragments (the A tile is free once every warp has run it),
+// x3_issue issues and commits the K block's wgmmas, and x3_keep, after the wait, marks the end of the fragments' lives.
+template <int KS>
+__device__ __forceinline__ void x3_load_a(uint32_t (&hi)[KS][4], uint32_t (&lo)[KS][4], uint32_t a_tile, int wt) {
   const uint32_t lane = (uint32_t)wt & 31u;
   // ldmatrix matrices 0..3 = (rows 0-7, k 0-3), (rows 8-15, k 0-3), (rows 0-7, k 4-7), (rows 8-15, k 4-7) of the warp's
   // 16 rows: the wgmma A fragment a[0..3]
   const uint32_t row = (uint32_t)(wt >> 5) * 16u + (lane & 7u) + ((lane >> 3) & 1u) * 8u;
   const uint32_t a_row = a_tile + row * (32u * KS);
   const uint32_t x = ((lane >> 4) << 4) ^ ((a_row >> 3) & (KS == 4 ? 0x70u : 0x30u));
-  uint32_t hi[KS][4], lo[KS][4];
 #pragma unroll
   for (int ks = 0; ks < KS; ++ks) {
     ldsm_x4(hi[ks], a_row + (((uint32_t)ks << 5) ^ x));
@@ -246,6 +248,10 @@ __device__ __forceinline__ void mma_kblock_x3(float (&acc)[BN / 2], uint32_t a_t
       hi[ks][j] = __float_as_uint(h);
     }
   }
+}
+template <int BN, int KS>
+__device__ __forceinline__ void x3_issue(float (&acc)[BN / 2], const uint32_t (&hi)[KS][4], const uint32_t (&lo)[KS][4],
+                                         uint64_t db, uint32_t b_lo, bool fresh) {
   wg_fence();
 #pragma unroll
   for (int ks = 0; ks < KS; ++ks) {
@@ -255,12 +261,24 @@ __device__ __forceinline__ void mma_kblock_x3(float (&acc)[BN / 2], uint32_t a_t
 #pragma unroll
   for (int ks = 0; ks < KS; ++ks) wgmma_tf32_rs<BN>(acc, hi[ks], db + 2u * ks, 1u);
   wg_commit();
-  wg_wait<0>();
-  // the tensor cores read the A registers until the wait: keep them live (and unchanged) up to here
+}
+// the tensor cores read the A registers until the wait: keep them live (and unchanged) up to here
+template <int KS>
+__device__ __forceinline__ void x3_keep(uint32_t (&hi)[KS][4], uint32_t (&lo)[KS][4]) {
 #pragma unroll
   for (int ks = 0; ks < KS; ++ks)
 #pragma unroll
     for (int j = 0; j < 4; ++j) asm volatile("" : "+r"(hi[ks][j]), "+r"(lo[ks][j]));
+}
+// All three steps and the wait: returns when the products are in `acc` and the operand tiles may be reused.
+template <int BN, int KS>
+__device__ __forceinline__ void mma_kblock_x3(float (&acc)[BN / 2], uint32_t a_tile, int wt, uint64_t db, uint32_t b_lo,
+                                              bool fresh) {
+  uint32_t hi[KS][4], lo[KS][4];
+  x3_load_a<KS>(hi, lo, a_tile, wt);
+  x3_issue<BN, KS>(acc, hi, lo, db, b_lo, fresh);
+  wg_wait<0>();
+  x3_keep<KS>(hi, lo);
 }
 
 __device__ __forceinline__ uint32_t pack_bf16x2(float a, float b) {
