@@ -37,15 +37,11 @@ struct WarpM {
 // one output pixel (x, y) of a [sh, sw] frame under the inverted matrix W, all three channels.  The source pixels come
 // from `px`: px.taps(iy, ix, in-frame flags) sees the 2 x 2 taps (iy, ix) .. (iy + 1, ix + 1) once, then px(k, yy, xx, c)
 // is channel c (B, G, R) of in-frame tap k = 2 (yy - iy) + (xx - ix) as an integer 0..255.  Taps outside the frame are
-// the border value 0 and are never fetched.  kTwin: the same values also go to `twin` when it is not null (a tracking
-// slot's previous-frame input at the start of its video).  kExchange: a slot's previous frame is kept in `store`; when
-// twin is not null, twin takes the value (`start`) or the stored one, and the value then replaces the stored one.  Each
-// thread reads and writes only its own elements.  Without either flag the walk compiles as it always has.
-template <class Fetch, bool kTwin = false, bool kExchange = false>
+// the border value 0 and are never fetched.  Channel c's value goes to out[c * plane], then to prev(c, value), the
+// previous-frame write of the launch's mode (preprocess_kernel).
+template <class Fetch, class Prev>
 __device__ __forceinline__ void warp_walk(Fetch px, float* __restrict__ out, size_t plane, int sh, int sw, int x,
-                                          int y, const WarpM& W, const float* mean, const float* stdv,
-                                          float* __restrict__ twin = nullptr, float* __restrict__ store = nullptr,
-                                          bool start = false) {
+                                          int y, const WarpM& W, const float* mean, const float* stdv, Prev prev) {
   // unfused double arithmetic (the host code OpenCV runs here has no FMA contraction)
   const int X0 = __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(W.m[1], (double)y), W.m[2]), 1024.0)) + 16;
   const int Y0 = __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(W.m[4], (double)y), W.m[5]), 1024.0)) + 16;
@@ -75,35 +71,13 @@ __device__ __forceinline__ void warp_walk(Fetch px, float* __restrict__ out, siz
     u8 = max(0, min(255, u8));
     const double r = ((double)u8 / 255.0 - (double)mean[c]) / (double)stdv[c];
     out[c * plane] = (float)r;
-    if constexpr (kExchange) {
-      if (twin) {
-        twin[c * plane] = start ? (float)r : store[c * plane];
-        store[c * plane] = (float)r;
-      }
-    } else if (kTwin && twin) {
-      twin[c * plane] = (float)r;
-    }
+    prev(c, (float)r);
   }
 }
 
-// interleaved 8-bit BGR [sh, sw, 3]: every channel is read where it is used
-struct BgrFetch {
-  const uint8_t* __restrict__ img;
-  int sw;
-  __device__ __forceinline__ void taps(int, int, bool, bool, bool, bool) {}
-  __device__ __forceinline__ int operator()(int, int yy, int xx, int c) const {
-    return img[((size_t)yy * sw + xx) * 3 + c];
-  }
-};
-
-__device__ __forceinline__ void warp_pixel(const uint8_t* __restrict__ img, float* __restrict__ out, size_t plane, int sh,
-                                           int sw, int x, int y, const WarpM& W, const float* mean, const float* stdv) {
-  warp_walk(BgrFetch{img, sw}, out, plane, sh, sw, x, y, W, mean, stdv);
-}
-
-// interleaved 8-bit pixels of kBytes (3 or 4) bytes with B, G and R at bytes kB, kG and kR: RGB24 <2, 1, 0>, RGBA
-// <2, 1, 0> and BGRA <0, 1, 2> (cv2.cvtColor COLOR_RGB2BGR / COLOR_RGBA2BGR / COLOR_BGRA2BGR are these channel
-// selects; alpha is never read).  Every channel is read where it is used, as in BgrFetch.
+// interleaved 8-bit pixels of kBytes (3 or 4) bytes with B, G and R at bytes kB, kG and kR: BGR <0, 1, 2>, RGB24 and
+// RGBA <2, 1, 0>, BGRA <0, 1, 2> (cv2.cvtColor COLOR_RGB2BGR / COLOR_RGBA2BGR / COLOR_BGRA2BGR are these channel
+// selects; alpha is never read).  Every channel is read where it is used.
 template <int kBytes, int kB, int kG, int kR>
 struct PackedFetch {
   const uint8_t* __restrict__ img;
@@ -114,73 +88,53 @@ struct PackedFetch {
   }
 };
 
-// YUV 4:2:0 [3 sh / 2, sw] (sh, sw even) converted per tap to the BGR that cv2.cvtColor(COLOR_YUV2BGR_NV12 / _I420)
-// gives, restated bit for bit (OpenCV color_yuv.simd.hpp, yuv42x_to_rgb8 for 8-bit: BT.601 limited range in 20-bit
-// fixed point, no chroma interpolation; tests/yuv_ref.py yuv420_to_bgr, pinned against cv2 on every (Y, U, V)):
+// YUV frames converted per tap to the BGR that cv2.cvtColor gives, restated bit for bit (OpenCV color_yuv.simd.hpp,
+// 8-bit: BT.601 limited range in 20-bit fixed point, no chroma interpolation; tests/yuv_ref.py and tests/yuv422_ref.py,
+// pinned against cv2 on every (Y, U, V)):
 //   y = max(Y - 16, 0) * 1220542 + 2^19, u = U - 128, v = V - 128
 //   B = sat((y + 2116026 u) >> 20), G = sat((y - 852492 v - 409993 u) >> 20), R = sat((y + 1673527 v) >> 20)
-// The Y plane [sh, sw] comes first; then NV12: U, V interleaved, row yy / 2, bytes (xx & ~1) and (xx | 1); I420: the U
-// plane [sh/2, sw/2], then the V plane [sh/2, sw/2].  Only in-frame taps are converted: warpAffine's border 0 is BGR 0.
+// 4:2:0 (COLOR_YUV2BGR_NV12 / _I420) [3 sh / 2, sw] (sh, sw even): the Y plane [sh, sw] comes first; then NV12: U, V
+// interleaved, row yy / 2, bytes (xx & ~1) and (xx | 1); I420: the U plane [sh/2, sw/2], then the V plane [sh/2, sw/2].
+// Packed 4:2:2 (COLOR_YUV2BGR_YUYV / _UYVY) [sh, sw, 2] (sw even): the pixel pair (xx & ~1, xx | 1) of a row is 4 bytes,
+// Y0 U Y1 V (YUYV) or U Y0 V Y1 (UYVY), one U, V for both pixels.  Every in-frame tap is read and converted once, before
+// the first channel is written; taps outside stay BGR 0, warpAffine's border of the converted image.
 template <int kFormat>
-struct Yuv420Fetch {
+struct YuvFetch {
   const uint8_t* __restrict__ img;
   int sh, sw;
   int yv[4], u[4], v[4];      // per tap: max(Y - 16, 0) * 1220542 + 2^19, U - 128, V - 128
-  // every in-frame tap is read and converted once, before the first channel is written
   __device__ __forceinline__ void taps(int iy, int ix, bool in00, bool in01, bool in10, bool in11) {
     const bool in[4] = {in00, in01, in10, in11};
-    const uint8_t* __restrict__ chroma = img + (size_t)sh * sw;
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
       yv[k] = u[k] = v[k] = 0;
       if (!in[k]) continue;
       const int yy = iy + (k >> 1), xx = ix + (k & 1);
-      int U, V;
-      if (kFormat == CP_PIX_NV12) {
-        const size_t o = (size_t)(yy >> 1) * sw + (xx & ~1);
-        U = chroma[o];
-        V = chroma[o + 1];
+      int Y, U, V;
+      if constexpr (kFormat == CP_PIX_NV12 || kFormat == CP_PIX_I420) {
+        const uint8_t* __restrict__ chroma = img + (size_t)sh * sw;
+        if constexpr (kFormat == CP_PIX_NV12) {
+          const size_t o = (size_t)(yy >> 1) * sw + (xx & ~1);
+          U = chroma[o];
+          V = chroma[o + 1];
+        } else {
+          const size_t o = (size_t)(yy >> 1) * (sw >> 1) + (xx >> 1);
+          U = chroma[o];
+          V = chroma[(size_t)(sh >> 1) * (sw >> 1) + o];
+        }
+        Y = img[(size_t)yy * sw + xx];
       } else {
-        const size_t o = (size_t)(yy >> 1) * (sw >> 1) + (xx >> 1);
-        U = chroma[o];
-        V = chroma[(size_t)(sh >> 1) * (sw >> 1) + o];
+        constexpr int kY = kFormat == CP_PIX_YUYV422 ? 0 : 1, kU = 1 - kY;    // byte of Y0 and of U in a pair
+        const uint8_t* __restrict__ pair = img + ((size_t)yy * sw + (xx & ~1)) * 2;
+        Y = pair[kY + 2 * (xx & 1)];
+        U = pair[kU];
+        V = pair[kU + 2];
       }
-      yv[k] = max((int)img[(size_t)yy * sw + xx] - 16, 0) * 1220542 + (1 << 19);
+      yv[k] = max(Y - 16, 0) * 1220542 + (1 << 19);
       u[k] = U - 128;
       v[k] = V - 128;
     }
   }
-  __device__ __forceinline__ int operator()(int k, int, int, int c) const {
-    const int t = c == 0 ? yv[k] + 2116026 * u[k]
-                         : (c == 1 ? yv[k] - 852492 * v[k] - 409993 * u[k] : yv[k] + 1673527 * v[k]);
-    return max(0, min(255, t >> 20));
-  }
-};
-
-// packed YUV 4:2:2 [sh, sw, 2] (sw even): the pixel pair (xx & ~1, xx | 1) of a row is 4 bytes, Y0 U Y1 V (YUYV) or
-// U Y0 V Y1 (UYVY), one U, V for both pixels.  cv2.cvtColor(COLOR_YUV2BGR_YUYV / _UYVY) converts each pixel with the
-// arithmetic of Yuv420Fetch and no chroma interpolation (tests/yuv422_ref.py, pinned against cv2 on every (Y, U, V)).
-// Every in-frame tap is read and converted once, before the first channel is written; taps outside stay BGR 0.
-template <int kFormat>
-struct Yuv422Fetch {
-  const uint8_t* __restrict__ img;
-  int sw;
-  int yv[4], u[4], v[4];
-  __device__ __forceinline__ void taps(int iy, int ix, bool in00, bool in01, bool in10, bool in11) {
-    const bool in[4] = {in00, in01, in10, in11};
-    constexpr int kY = kFormat == CP_PIX_YUYV422 ? 0 : 1, kU = 1 - kY;    // byte of Y0 and of U in a pair
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      yv[k] = u[k] = v[k] = 0;
-      if (!in[k]) continue;
-      const int yy = iy + (k >> 1), xx = ix + (k & 1);
-      const uint8_t* __restrict__ pair = img + ((size_t)yy * sw + (xx & ~1)) * 2;
-      yv[k] = max((int)pair[kY + 2 * (xx & 1)] - 16, 0) * 1220542 + (1 << 19);
-      u[k] = pair[kU] - 128;
-      v[k] = pair[kU + 2] - 128;
-    }
-  }
-  // the conversion of Yuv420Fetch (written out again there, so that its instances compile as they did before 4:2:2)
   __device__ __forceinline__ int operator()(int k, int, int, int c) const {
     const int t = c == 0 ? yv[k] + 2116026 * u[k]
                          : (c == 1 ? yv[k] - 852492 * v[k] - 409993 * u[k] : yv[k] + 1673527 * v[k]);
@@ -200,37 +154,15 @@ __host__ __device__ constexpr size_t frame_bytes(int format, size_t sh, size_t s
 // the tap fetch of a frame at img in format kFormat
 template <int kFormat>
 __device__ __forceinline__ auto make_fetch(const uint8_t* __restrict__ img, int sh, int sw) {
-  if constexpr (kFormat == CP_PIX_BGR)
-    return BgrFetch{img, sw};
-  else if constexpr (kFormat == CP_PIX_NV12 || kFormat == CP_PIX_I420)
-    return Yuv420Fetch<kFormat>{img, sh, sw};
-  else if constexpr (kFormat == CP_PIX_RGB24)
-    return PackedFetch<3, 2, 1, 0>{img, sw};
-  else if constexpr (kFormat == CP_PIX_RGBA)
-    return PackedFetch<4, 2, 1, 0>{img, sw};
-  else if constexpr (kFormat == CP_PIX_BGRA)
-    return PackedFetch<4, 0, 1, 2>{img, sw};
+  if constexpr (kFormat == CP_PIX_BGR || kFormat == CP_PIX_BGRA)
+    return PackedFetch<kFormat == CP_PIX_BGR ? 3 : 4, 0, 1, 2>{img, sw};
+  else if constexpr (kFormat == CP_PIX_RGB24 || kFormat == CP_PIX_RGBA)
+    return PackedFetch<kFormat == CP_PIX_RGB24 ? 3 : 4, 2, 1, 0>{img, sw};
   else
-    return Yuv422Fetch<kFormat>{img, sw};
+    return YuvFetch<kFormat>{img, sh, sw};
 }
 
-__global__ void preprocess_kernel(const uint8_t* __restrict__ frames, float* __restrict__ out, int B, int sh,
-                                  int sw, int dh, int dw, const WarpM W, float m0, float m1, float m2, float s0, float s1,
-                                  float s2) {
-  size_t total = (size_t)B * dh * dw;
-  const float mean[3] = {m0, m1, m2};
-  const float stdv[3] = {s0, s1, s2};
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-    const int x = (int)(i % dw);
-    const size_t t = i / dw;
-    const int y = (int)(t % dh);
-    const int n = (int)(t / dh);
-    warp_pixel(frames + (size_t)n * sh * sw * 3, out + (((size_t)n * 3) * dh + y) * dw + x, (size_t)dh * dw, sh, sw, x, y,
-               W, mean, stdv);
-  }
-}
-
-// per-frame parameters of the ragged launch
+// per-frame parameters of a frame table
 struct RaggedFrame {
   WarpM W;
   long long offset;     // bytes into the packed frame buffer
@@ -263,145 +195,60 @@ __device__ __forceinline__ void frame_walk(const uint8_t* __restrict__ frames, c
   }
 }
 
-__global__ void preprocess_ragged_kernel(const uint8_t* __restrict__ frames, const RaggedFrame* __restrict__ fr,
-                                         float* __restrict__ out, int B, int dh, int dw, float m0, float m1, float m2,
-                                         float s0, float s1, float s2) {
-  size_t total = (size_t)B * dh * dw;
-  const float mean[3] = {m0, m1, m2};
-  const float stdv[3] = {s0, s1, s2};
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-    const int x = (int)(i % dw);
-    const size_t t = i / dw;
-    const int y = (int)(t % dh);
-    const int n = (int)(t / dh);
-    const RaggedFrame f = fr[n];
-    warp_pixel(frames + f.offset, out + (((size_t)n * 3) * dh + y) * dw + x, (size_t)dh * dw, f.sh, f.sw, x, y, f.W, mean,
-               stdv);
-  }
-}
+// The arguments of preprocess_kernel.  Every one is a kernel argument or device memory, so a captured launch replays
+// unchanged.
+struct PreprocessArgs {
+  const uint8_t* frames;
+  const RaggedFrame* fr;     // the table form: row n is slot s = rows ? rows[n] : n, its frame fr[s]
+  const int* rows;
+  WarpM W;                   // the uniform form: one sh x sw frame per row, frame n at byte n * frame_bytes
+  int sh, sw;
+  int B, dh, dw;
+  float mean[3], stdv[3];
+  const int* start;          // the previous frame (PrevMode): prev null: none; store null: the twin (start[s]: a slot
+  float* store;              // beginning a video); else the exchange (the live rows name distinct slots)
+  float* prev;
+  float* out;
+};
 
-// the ragged launch on YUV 4:2:0 frames (kFormat: cp_pixel_format): the same walk with the tap fetch converting to BGR
-template <int kFormat>
-__global__ void preprocess_yuv420_kernel(const uint8_t* __restrict__ frames, const RaggedFrame* __restrict__ fr,
-                                         float* __restrict__ out, int B, int dh, int dw, float m0, float m1, float m2,
-                                         float s0, float s1, float s2) {
-  size_t total = (size_t)B * dh * dw;
-  const float mean[3] = {m0, m1, m2};
-  const float stdv[3] = {s0, s1, s2};
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-    const int x = (int)(i % dw);
-    const size_t t = i / dw;
-    const int y = (int)(t % dh);
-    const int n = (int)(t / dh);
-    const RaggedFrame f = fr[n];
-    warp_walk(Yuv420Fetch<kFormat>{frames + f.offset, f.sh, f.sw}, out + (((size_t)n * 3) * dh + y) * dw + x,
-              (size_t)dh * dw, f.sh, f.sw, x, y, f.W, mean, stdv);
-  }
-}
+// The previous-frame writes of a launch (PreprocessArgs): none; the twin, prev[n] = the value where start[s] is set;
+// the exchange, prev[n] = start[s] ? value : store[s], then store[s] = value.  The mode is a template parameter, so a
+// launch without previous frames runs the walk alone and each mode keeps the registers it needs by itself.
+enum PrevMode { kNoPrev, kTwin, kExchange };
 
-// The frames of one tracking step: B slots of one size, format (cp_pixel_format) and affine, frame n at byte n * bytes.
-// Every parameter is a kernel argument or device memory, so a captured launch replays unchanged.  A slot whose start[n]
-// is set begins a video with this frame, which is then also its previous frame: the walk writes it to prev[n] as well.
-template <int kFormat>
-__global__ void preprocess_slots_kernel(const uint8_t* __restrict__ frames, float* __restrict__ out,
-                                        float* __restrict__ prev, const int* __restrict__ start, int B, int sh, int sw,
-                                        int dh, int dw, const WarpM W, float m0, float m1, float m2, float s0, float s1,
-                                        float s2) {
-  const size_t total = (size_t)B * dh * dw, plane = (size_t)dh * dw;
-  const size_t bytes = kFormat == CP_PIX_BGR                                 ? (size_t)sh * sw * 3
-                       : kFormat == CP_PIX_NV12 || kFormat == CP_PIX_I420 ? (size_t)sh * sw * 3 / 2
-                                                                          : frame_bytes(kFormat, sh, sw);
-  const float mean[3] = {m0, m1, m2};
-  const float stdv[3] = {s0, s1, s2};
+// B rows of [3, dh, dw]: row n is frame n (uniform) or the frame of slot s through the table (kTable), in format
+// kFormat (CP_PIX_PER_FRAME: each table entry's own).  Every thread is one output pixel of one row, grid-stride, and
+// reads and writes only its own elements.
+template <int kFormat, bool kTable, PrevMode kMode>
+__global__ void preprocess_kernel(const PreprocessArgs a) {
+  const size_t plane = (size_t)a.dh * a.dw, total = (size_t)a.B * plane;
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-    const int x = (int)(i % dw);
-    const size_t t = i / dw;
-    const int y = (int)(t % dh);
-    const int n = (int)(t / dh);
-    const size_t o = (((size_t)n * 3) * dh + y) * dw + x;
-    float* twin = start && start[n] ? prev + o : nullptr;
-    const uint8_t* img = frames + n * bytes;
-    if constexpr (kFormat == CP_PIX_BGR) {
-      warp_walk<BgrFetch, true>(BgrFetch{img, sw}, out + o, plane, sh, sw, x, y, W, mean, stdv, twin);
-    } else if constexpr (kFormat == CP_PIX_NV12 || kFormat == CP_PIX_I420) {
-      warp_walk<Yuv420Fetch<kFormat>, true>(Yuv420Fetch<kFormat>{img, sh, sw}, out + o, plane, sh, sw, x, y, W, mean,
-                                            stdv, twin);
+    const int x = (int)(i % a.dw);
+    const size_t t = i / a.dw;
+    const int y = (int)(t % a.dh);
+    const int n = (int)(t / a.dh);
+    int s = n;
+    RaggedFrame f;
+    if constexpr (kTable) {
+      if (kMode == kExchange || a.rows) s = a.rows[n];      // the exchange is the rows form's only
+      f = a.fr[s];
     } else {
-      auto px = make_fetch<kFormat>(img, sh, sw);
-      warp_walk<decltype(px), true>(px, out + o, plane, sh, sw, x, y, W, mean, stdv, twin);
+      f = RaggedFrame{a.W, (long long)(n * frame_bytes(kFormat, a.sh, a.sw)), a.sh, a.sw};
     }
-  }
-}
-
-// The frames of one tracking step when the slots differ in size: the ragged walk of preprocess_ragged_kernel /
-// preprocess_yuv420_kernel over a frame table `fr` in device memory (built once, cp_preprocess_frame_table), with the
-// start-flag twin write of preprocess_slots_kernel.  Nothing is read from the host, so a captured launch replays unchanged.
-// Without start flags it is also the ragged launch of the formats preprocess_ragged_kernel / _yuv420_kernel do not read,
-// and of a batch of per-frame formats (kFormat CP_PIX_PER_FRAME).
-template <int kFormat>
-__global__ void preprocess_slots_ragged_kernel(const uint8_t* __restrict__ frames, const RaggedFrame* __restrict__ fr,
-                                               float* __restrict__ out, float* __restrict__ prev,
-                                               const int* __restrict__ start, int B, int dh, int dw, float m0, float m1,
-                                               float m2, float s0, float s1, float s2) {
-  const size_t total = (size_t)B * dh * dw, plane = (size_t)dh * dw;
-  const float mean[3] = {m0, m1, m2};
-  const float stdv[3] = {s0, s1, s2};
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-    const int x = (int)(i % dw);
-    const size_t t = i / dw;
-    const int y = (int)(t % dh);
-    const int n = (int)(t / dh);
-    const size_t o = (((size_t)n * 3) * dh + y) * dw + x;
-    float* twin = start && start[n] ? prev + o : nullptr;
-    const RaggedFrame f = fr[n];
-    if constexpr (kFormat == CP_PIX_BGR)
-      warp_walk<BgrFetch, true>(BgrFetch{frames + f.offset, f.sw}, out + o, plane, f.sh, f.sw, x, y, f.W, mean, stdv,
-                                twin);
-    else if constexpr (kFormat == CP_PIX_NV12 || kFormat == CP_PIX_I420)
-      warp_walk<Yuv420Fetch<kFormat>, true>(Yuv420Fetch<kFormat>{frames + f.offset, f.sh, f.sw}, out + o, plane, f.sh,
-                                            f.sw, x, y, f.W, mean, stdv, twin);
-    else
-      frame_walk<kFormat>(frames, f, [&](auto px) {
-        warp_walk<decltype(px), true>(px, out + o, plane, f.sh, f.sw, x, y, f.W, mean, stdv, twin);
+    const size_t px = (size_t)y * a.dw + x, o = (size_t)n * 3 * plane + px;
+    const bool start = kMode != kNoPrev && a.start && a.start[s];
+    float* prev = a.prev + o;
+    float* store = a.store + (size_t)s * 3 * plane + px;
+    frame_walk<kFormat>(a.frames, f, [&](auto fetch) {
+      warp_walk(fetch, a.out + o, plane, f.sh, f.sw, x, y, f.W, a.mean, a.stdv, [&](int c, float v) {
+        if constexpr (kMode == kTwin) {
+          if (start) prev[c * plane] = v;
+        } else if constexpr (kMode == kExchange) {
+          prev[c * plane] = start ? v : store[c * plane];
+          store[c * plane] = v;
+        }
       });
-  }
-}
-
-// The frames of one tracking step when some slots are idle: row n of the B live rows is slot rows[n]'s frame, warped
-// through that slot's entry of the frame table into out[n].  With prev (and store), the slot's previous frame moves
-// through a per-slot store in the same walk: prev[n] = start[slot] ? value : store[slot], then store[slot] = value.  The
-// live rows name distinct slots, so no two threads touch the same store element.  rows and start are device memory
-// read when the kernel runs, so a captured launch replays whatever map the last copy left there.
-template <int kFormat>
-__global__ void preprocess_slots_rows_kernel(const uint8_t* __restrict__ frames, const RaggedFrame* __restrict__ fr,
-                                             const int* __restrict__ rows, const int* __restrict__ start,
-                                             float* __restrict__ store, float* __restrict__ out,
-                                             float* __restrict__ prev, int B, int dh, int dw, float m0, float m1,
-                                             float m2, float s0, float s1, float s2) {
-  const size_t total = (size_t)B * dh * dw, plane = (size_t)dh * dw;
-  const float mean[3] = {m0, m1, m2};
-  const float stdv[3] = {s0, s1, s2};
-  for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
-    const int x = (int)(i % dw);
-    const size_t t = i / dw;
-    const int y = (int)(t % dh);
-    const int n = (int)(t / dh);
-    const int slot = rows[n];
-    const size_t px = (size_t)y * dw + x, o = (size_t)n * 3 * plane + px;
-    const bool st = start && start[slot];
-    float* twin = prev ? prev + o : nullptr;
-    float* keep = prev ? store + (size_t)slot * 3 * plane + px : nullptr;
-    const RaggedFrame f = fr[slot];
-    if constexpr (kFormat == CP_PIX_BGR)
-      warp_walk<BgrFetch, true, true>(BgrFetch{frames + f.offset, f.sw}, out + o, plane, f.sh, f.sw, x, y, f.W, mean,
-                                      stdv, twin, keep, st);
-    else if constexpr (kFormat == CP_PIX_NV12 || kFormat == CP_PIX_I420)
-      warp_walk<Yuv420Fetch<kFormat>, true, true>(Yuv420Fetch<kFormat>{frames + f.offset, f.sh, f.sw}, out + o, plane,
-                                                  f.sh, f.sw, x, y, f.W, mean, stdv, twin, keep, st);
-    else
-      frame_walk<kFormat>(frames, f, [&](auto px) {
-        warp_walk<decltype(px), true, true>(px, out + o, plane, f.sh, f.sw, x, y, f.W, mean, stdv, twin, keep, st);
-      });
+    });
   }
 }
 
@@ -466,9 +313,9 @@ bool known_format(int format) {
          format == CP_PIX_BGRA || is_yuv422(format);
 }
 
-// f(std::integral_constant<int, format>) for a format chosen at run time (one of cp_pixel_format; with kPerFrame also
+// f(std::integral_constant<int, format>) for a format chosen at run time (one of cp_pixel_format or
 // CP_PIX_PER_FRAME), already checked
-template <bool kPerFrame, class F>
+template <class F>
 void with_format(int format, F f) {
   switch (format) {
     case CP_PIX_NV12: f(std::integral_constant<int, CP_PIX_NV12>{}); break;
@@ -479,9 +326,54 @@ void with_format(int format, F f) {
     case CP_PIX_BGRA: f(std::integral_constant<int, CP_PIX_BGRA>{}); break;
     case CP_PIX_YUYV422: f(std::integral_constant<int, CP_PIX_YUYV422>{}); break;
     case CP_PIX_UYVY422: f(std::integral_constant<int, CP_PIX_UYVY422>{}); break;
-    default:
-      if constexpr (kPerFrame) f(std::integral_constant<int, CP_PIX_PER_FRAME>{});
+    default: f(std::integral_constant<int, CP_PIX_PER_FRAME>{});
   }
+}
+
+// the arguments every form of preprocess_kernel takes; the entry points fill in the frame source and previous frame
+PreprocessArgs preprocess_args(const uint8_t* frames, float* out, int B, int dh, int dw, const float mean[3],
+                               const float stdv[3]) {
+  PreprocessArgs a{};
+  a.frames = frames;
+  a.out = out;
+  a.B = B;
+  a.dh = dh;
+  a.dw = dw;
+  for (int c = 0; c < 3; ++c) {
+    a.mean[c] = mean[c];
+    a.stdv[c] = stdv[c];
+  }
+  return a;
+}
+
+// enqueues preprocess_kernel in `format`: the table form when a.fr is set (which may also be CP_PIX_PER_FRAME and
+// take the store exchange, with rows), else the uniform form; the previous-frame mode is the one a's pointers select
+int launch_preprocess(int format, const PreprocessArgs& a, cudaStream_t s) {
+  if (a.fr ? !known_format(format) && format != CP_PIX_PER_FRAME || (a.store && !a.rows)
+           : !known_format(format) || a.store)
+    return fail(CP_ERR_INVALID, "preprocess_kernel: no instance for pixel format " + std::to_string(format) +
+                                    (a.fr ? " over a frame table" : " over a uniform batch") +
+                                    (a.store ? " with a store" : ""));
+  const int blocks = preprocess_blocks((size_t)a.B * a.dh * a.dw);
+  const PrevMode mode = !a.prev ? kNoPrev : !a.store ? kTwin : kExchange;
+  with_format(format, [&](auto k) {
+    constexpr int kFormat = decltype(k)::value;
+    if (a.fr) {
+      if (mode == kNoPrev)
+        preprocess_kernel<kFormat, true, kNoPrev><<<blocks, 256, 0, s>>>(a);
+      else if (mode == kTwin)
+        preprocess_kernel<kFormat, true, kTwin><<<blocks, 256, 0, s>>>(a);
+      else
+        preprocess_kernel<kFormat, true, kExchange><<<blocks, 256, 0, s>>>(a);
+    } else if constexpr (kFormat != CP_PIX_PER_FRAME) {
+      if (mode == kNoPrev)
+        preprocess_kernel<kFormat, false, kNoPrev><<<blocks, 256, 0, s>>>(a);
+      else
+        preprocess_kernel<kFormat, false, kTwin><<<blocks, 256, 0, s>>>(a);
+    }
+  });
+  CP_LAUNCH_CHECK("preprocess_kernel");
+  return CP_OK;
 }
 
 // The per-frame parameters of a ragged batch, checked against the packed buffer before any work is enqueued.  Frame b
@@ -524,24 +416,17 @@ int ragged_frames(const char* who, int64_t frames_bytes, const int64_t* offsets,
   return CP_OK;
 }
 
-// uploads the per-frame parameters (stream-ordered) and enqueues launch(device parameters)
-template <class Launch>
-int launch_ragged(const char* who, const char* kernel, const std::vector<RaggedFrame>& fr, cudaStream_t s,
-                  Launch launch) {
-  const int B = (int)fr.size();
+// uploads the frame table `fr` (stream-ordered) and enqueues the table form of preprocess_kernel over it
+int launch_ragged(const char* who, int format, const std::vector<RaggedFrame>& fr, PreprocessArgs a, cudaStream_t s) {
   RaggedFrame* dfr = nullptr;
-  CP_CUDA_CHECK(cudaMallocAsync(&dfr, sizeof(RaggedFrame) * B, s));
-  int rc = CP_OK;
+  CP_CUDA_CHECK(cudaMallocAsync(&dfr, sizeof(RaggedFrame) * fr.size(), s));
+  int rc;
   // a pageable source: the bytes are staged before cudaMemcpyAsync returns, so `fr` may go out of scope
-  if (cudaMemcpyAsync(dfr, fr.data(), sizeof(RaggedFrame) * B, cudaMemcpyHostToDevice, s) != cudaSuccess) {
+  if (cudaMemcpyAsync(dfr, fr.data(), sizeof(RaggedFrame) * fr.size(), cudaMemcpyHostToDevice, s) != cudaSuccess) {
     rc = fail(CP_ERR_CUDA, std::string(who) + ": parameter upload");
   } else {
-    launch(dfr);
-    const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess)
-      rc = fail(CP_ERR_CUDA, std::string(kernel) + ": " + cudaGetErrorString(e));
-    else
-      ++g_launch_counter;
+    a.fr = dfr;
+    rc = launch_preprocess(format, a, s);
   }
   cudaFreeAsync(dfr, s);
   return rc;
@@ -709,11 +594,11 @@ int cp_preprocess_affine(const uint8_t* frames, float* out, int32_t B, int32_t s
   if (!frames || !out || !mean || !stdv || !trans_input) return fail(CP_ERR_INVALID, "cp_preprocess: null argument");
   if (B <= 0 || src_h <= 0 || src_w <= 0 || dst_h <= 0 || dst_w <= 0)
     return fail(CP_ERR_INVALID, "cp_preprocess: bad shape");
-  const WarpM W = invert_affine(trans_input);
-  preprocess_kernel<<<preprocess_blocks((size_t)B * dst_h * dst_w), 256, 0, (cudaStream_t)stream_>>>(
-      frames, out, B, src_h, src_w, dst_h, dst_w, W, mean[0], mean[1], mean[2], stdv[0], stdv[1], stdv[2]);
-  CP_LAUNCH_CHECK("preprocess_kernel");
-  return CP_OK;
+  PreprocessArgs a = preprocess_args(frames, out, B, dst_h, dst_w, mean, stdv);
+  a.W = invert_affine(trans_input);
+  a.sh = src_h;
+  a.sw = src_w;
+  return launch_preprocess(CP_PIX_BGR, a, (cudaStream_t)stream_);
 }
 
 // the fix_res affine of the frame size (fix_res_affine above)
@@ -734,11 +619,8 @@ int cp_preprocess_ragged(const uint8_t* frames, int64_t frames_bytes, const int6
   int rc = ragged_frames("cp_preprocess_ragged", frames_bytes, offsets, src_hw, B, dst_h, dst_w, trans_input, CP_PIX_BGR,
                          nullptr, fr);
   if (rc) return rc;
-  cudaStream_t s = (cudaStream_t)stream_;
-  return launch_ragged("cp_preprocess_ragged", "preprocess_ragged_kernel", fr, s, [&](const RaggedFrame* dfr) {
-    preprocess_ragged_kernel<<<preprocess_blocks((size_t)B * dst_h * dst_w), 256, 0, s>>>(
-        frames, dfr, out, B, dst_h, dst_w, mean[0], mean[1], mean[2], stdv[0], stdv[1], stdv[2]);
-  });
+  return launch_ragged("cp_preprocess_ragged", CP_PIX_BGR, fr, preprocess_args(frames, out, B, dst_h, dst_w, mean, stdv),
+                       (cudaStream_t)stream_);
 }
 
 int cp_preprocess_yuv420(const uint8_t* frames, int64_t frames_bytes, const int64_t* offsets, const int32_t* src_hw,
@@ -752,16 +634,8 @@ int cp_preprocess_yuv420(const uint8_t* frames, int64_t frames_bytes, const int6
   int rc = ragged_frames("cp_preprocess_yuv420", frames_bytes, offsets, src_hw, B, dst_h, dst_w, trans_input, format,
                          nullptr, fr);
   if (rc) return rc;
-  cudaStream_t s = (cudaStream_t)stream_;
-  return launch_ragged("cp_preprocess_yuv420", "preprocess_yuv420_kernel", fr, s, [&](const RaggedFrame* dfr) {
-    const int blocks = preprocess_blocks((size_t)B * dst_h * dst_w);
-    if (format == CP_PIX_NV12)
-      preprocess_yuv420_kernel<CP_PIX_NV12><<<blocks, 256, 0, s>>>(frames, dfr, out, B, dst_h, dst_w, mean[0], mean[1],
-                                                                    mean[2], stdv[0], stdv[1], stdv[2]);
-    else
-      preprocess_yuv420_kernel<CP_PIX_I420><<<blocks, 256, 0, s>>>(frames, dfr, out, B, dst_h, dst_w, mean[0], mean[1],
-                                                                    mean[2], stdv[0], stdv[1], stdv[2]);
-  });
+  return launch_ragged("cp_preprocess_yuv420", format, fr, preprocess_args(frames, out, B, dst_h, dst_w, mean, stdv),
+                       (cudaStream_t)stream_);
 }
 
 int cp_preprocess_formats(const uint8_t* frames, int64_t frames_bytes, const int64_t* offsets, const int32_t* src_hw,
@@ -777,14 +651,8 @@ int cp_preprocess_formats(const uint8_t* frames, int64_t frames_bytes, const int
   int rc = ragged_frames("cp_preprocess_formats", frames_bytes, offsets, src_hw, B, dst_h, dst_w, trans_input, format,
                          format == CP_PIX_PER_FRAME ? formats : nullptr, fr);
   if (rc) return rc;
-  cudaStream_t s = (cudaStream_t)stream_;
-  // the walk of the graph-safe ragged launch without start flags: one instance per format, or the per-frame one
-  return launch_ragged("cp_preprocess_formats", "preprocess_slots_ragged_kernel", fr, s, [&](const RaggedFrame* dfr) {
-    with_format<true>(format, [&](auto k) {
-      preprocess_slots_ragged_kernel<decltype(k)::value><<<preprocess_blocks((size_t)B * dst_h * dst_w), 256, 0, s>>>(
-          frames, dfr, out, nullptr, nullptr, B, dst_h, dst_w, mean[0], mean[1], mean[2], stdv[0], stdv[1], stdv[2]);
-    });
-  });
+  return launch_ragged("cp_preprocess_formats", format, fr, preprocess_args(frames, out, B, dst_h, dst_w, mean, stdv),
+                       (cudaStream_t)stream_);
 }
 
 int cp_preprocess_slots_dev(const uint8_t* frames, int32_t format, int32_t B, int32_t src_h, int32_t src_w,
@@ -807,16 +675,13 @@ int cp_preprocess_slots_dev(const uint8_t* frames, int32_t format, int32_t B, in
     for (int i = 0; i < 6; ++i) T[i] = trans_input[i];
   else
     fix_res_affine(src_h, src_w, dst_h, dst_w, T);
-  const WarpM W = invert_affine(T);
-  const int blocks = preprocess_blocks((size_t)B * dst_h * dst_w);
-  cudaStream_t s = (cudaStream_t)stream_;
-  auto launch = [&](auto kernel) {
-    kernel<<<blocks, 256, 0, s>>>(frames, out, prev, start, B, src_h, src_w, dst_h, dst_w, W, mean[0], mean[1], mean[2],
-                                  stdv[0], stdv[1], stdv[2]);
-  };
-  with_format<false>(format, [&](auto k) { launch(preprocess_slots_kernel<decltype(k)::value>); });
-  CP_LAUNCH_CHECK("preprocess_slots_kernel");
-  return CP_OK;
+  PreprocessArgs a = preprocess_args(frames, out, B, dst_h, dst_w, mean, stdv);
+  a.W = invert_affine(T);
+  a.sh = src_h;
+  a.sw = src_w;
+  a.start = start;
+  a.prev = prev;
+  return launch_preprocess(format, a, (cudaStream_t)stream_);
 }
 
 int64_t cp_preprocess_frame_table_bytes(int32_t B) {
@@ -855,16 +720,11 @@ int cp_preprocess_slots_ragged_dev(const uint8_t* frames, const void* table, int
   if (!known_format(format) && format != CP_PIX_PER_FRAME)
     return fail(CP_ERR_INVALID, "cp_preprocess_slots_ragged_dev: unknown pixel format " + std::to_string(format));
   if (B <= 0 || dst_h <= 0 || dst_w <= 0) return fail(CP_ERR_INVALID, "cp_preprocess_slots_ragged_dev: bad shape");
-  const RaggedFrame* fr = (const RaggedFrame*)table;
-  const int blocks = preprocess_blocks((size_t)B * dst_h * dst_w);
-  cudaStream_t s = (cudaStream_t)stream_;
-  auto launch = [&](auto kernel) {
-    kernel<<<blocks, 256, 0, s>>>(frames, fr, out, prev, start, B, dst_h, dst_w, mean[0], mean[1], mean[2], stdv[0],
-                                  stdv[1], stdv[2]);
-  };
-  with_format<true>(format, [&](auto k) { launch(preprocess_slots_ragged_kernel<decltype(k)::value>); });
-  CP_LAUNCH_CHECK("preprocess_slots_ragged_kernel");
-  return CP_OK;
+  PreprocessArgs a = preprocess_args(frames, out, B, dst_h, dst_w, mean, stdv);
+  a.fr = (const RaggedFrame*)table;
+  a.start = start;
+  a.prev = prev;
+  return launch_preprocess(format, a, (cudaStream_t)stream_);
 }
 
 int cp_preprocess_slots_rows_dev(const uint8_t* frames, const void* table, int32_t format, const int32_t* rows, int32_t B,
@@ -876,16 +736,13 @@ int cp_preprocess_slots_rows_dev(const uint8_t* frames, const void* table, int32
   if (!known_format(format) && format != CP_PIX_PER_FRAME)
     return fail(CP_ERR_INVALID, "cp_preprocess_slots_rows_dev: unknown pixel format " + std::to_string(format));
   if (B <= 0 || dst_h <= 0 || dst_w <= 0) return fail(CP_ERR_INVALID, "cp_preprocess_slots_rows_dev: bad shape");
-  const RaggedFrame* fr = (const RaggedFrame*)table;
-  const int blocks = preprocess_blocks((size_t)B * dst_h * dst_w);
-  cudaStream_t s = (cudaStream_t)stream_;
-  auto launch = [&](auto kernel) {
-    kernel<<<blocks, 256, 0, s>>>(frames, fr, rows, start, store, out, prev, B, dst_h, dst_w, mean[0], mean[1], mean[2],
-                                  stdv[0], stdv[1], stdv[2]);
-  };
-  with_format<true>(format, [&](auto k) { launch(preprocess_slots_rows_kernel<decltype(k)::value>); });
-  CP_LAUNCH_CHECK("preprocess_slots_rows_kernel");
-  return CP_OK;
+  PreprocessArgs a = preprocess_args(frames, out, B, dst_h, dst_w, mean, stdv);
+  a.fr = (const RaggedFrame*)table;
+  a.rows = rows;
+  a.start = start;
+  a.store = store;
+  a.prev = prev;
+  return launch_preprocess(format, a, (cudaStream_t)stream_);
 }
 
 int cp_gather_rows_dev(const void* src, void* dst, int64_t row_bytes, int32_t n, const int32_t* map, void* stream_) {

@@ -18,8 +18,8 @@ import numpy as np
 import torch
 
 from . import _lib
-from .engine import (_YUV420, Engine, check_pixel_format, decode_params, decode_pnp, frame_layout, image_size, make_meta,
-                     preprocess, preprocess_formats, preprocess_ragged, preprocess_yuv420, slot_formats)
+from .engine import (Engine, check_pixel_format, decode_params, decode_pnp, frame_layout, image_size, make_meta,
+                     preprocess, preprocess_formats, slot_formats)
 from .model import _load_checkpoint, create_model, load_model
 from .tracker import Tracker, tracks_to_results
 
@@ -622,9 +622,8 @@ class ObjectPoseDetector(object):
             sh, sw = image_size(frames.shape[1:], pixel_format, "run_batch: each frame")
             fr = frames.to(dev, non_blocking=True).contiguous().reshape(-1)
             n = fr.numel() // max(B, 1)
-            run = preprocess_yuv420 if pixel_format in _YUV420 else preprocess_formats
-            x = run(fr, np.arange(B, dtype=np.int64) * n, [(sh, sw)] * B, pixel_format, self.opt.input_h,
-                    self.opt.input_w, self.opt.mean, self.opt.std)
+            x = preprocess_formats(fr, np.arange(B, dtype=np.int64) * n, [(sh, sw)] * B, pixel_format, self.opt.input_h,
+                                   self.opt.input_w, self.opt.mean, self.opt.std)
             c, s = np.array([sw / 2., sh / 2.], np.float32), float(max(sh, sw))
             iw, ih = sw, sh
         elif frames.dtype == torch.uint8:
@@ -648,9 +647,8 @@ class ObjectPoseDetector(object):
     def _ragged_input(self, frames, camera_matrix, pixel_format="bgr"):
         """Validated list of uint8 HWC frames (or frames of pixel_format: one name, or one per frame) -> (x [B,3,h,w]
         fp32 CUDA, meta rows [B,16] float64 host, trans_input [B,2,3] host).  The frames are copied into one device
-        buffer and pre-processed by one cp_preprocess_ragged (cp_preprocess_yuv420, cp_preprocess_formats for the camera
-        formats and for mixed formats) launch with the same fix_res affine (c = image centre, s = max side) and meta row
-        that pre_process / run() use."""
+        buffer and pre-processed by one cp_preprocess_formats launch with the same fix_res affine (c = image centre,
+        s = max side) and meta row that pre_process / run() use."""
         if getattr(self.opt, "fix_short", 0) > 0 or not getattr(self.opt, "fix_res", True):
             raise NotImplementedError("run_batch(list) pre-processes in the fix_res mode only")
         if float(self.scales[0]) != 1.0:
@@ -680,14 +678,7 @@ class ObjectPoseDetector(object):
                 self._affines[(h, w)] = affine_from_center_scale(c, sc, iw, ih)
             trans[b] = self._affines[(h, w)]
             meta[b] = make_meta(1, c, sc, w, h, cams[b]).numpy()[0]
-        one = fmts[0] if len(set(fmts)) == 1 else None        # one format: its launch, whatever form named it
-        if one == "bgr":
-            x = preprocess_ragged(self._packed, offs, hw, ih, iw, self.opt.mean, self.opt.std, trans_input=trans)
-        elif one in _YUV420:
-            x = preprocess_yuv420(self._packed, offs, hw, one, ih, iw, self.opt.mean, self.opt.std, trans_input=trans)
-        else:
-            x = preprocess_formats(self._packed, offs, hw, one or fmts, ih, iw, self.opt.mean, self.opt.std,
-                                   trans_input=trans)
+        x = preprocess_formats(self._packed, offs, hw, fmts, ih, iw, self.opt.mean, self.opt.std, trans_input=trans)
         return x, meta, trans
 
     def _meta_rows(self, meta):

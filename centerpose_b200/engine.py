@@ -508,34 +508,41 @@ def preprocess(frames_u8, dst_h, dst_w, mean, std, out=None, trans_input=None):
     return out
 
 
-def preprocess_ragged(packed_u8, offsets, src_hw, dst_h, dst_w, mean, std, out=None, trans_input=None):
-    """cp_preprocess_ragged: B frames of different sizes in one launch.  packed_u8: flat uint8 CUDA buffer holding frame b
-    (uint8 [src_hw[b][0], src_hw[b][1], 3]) at byte offsets[b] -> fp32 [B,3,dst_h,dst_w] CUDA, frame b bit for bit what
-    `preprocess` gives for it alone.  trans_input: optional [B,2,3] forward affines; default = each frame's fix_res affine."""
+def _preprocess_packed(who, packed_u8, offsets, src_hw, fmt, dst_h, dst_w, mean, std, out, trans_input):
+    """The call of cp_<who> on B frames packed into one buffer: (packed_u8, its bytes, offsets, src_hw, *fmt, out, B,
+    dst_h, dst_w, trans_input, mean, std, stream), fmt being the entry point's format argument, if it has one."""
     L = _lib.load()
     if not packed_u8.is_cuda or packed_u8.dtype != torch.uint8 or not packed_u8.is_contiguous():
-        raise RuntimeError("preprocess_ragged needs a contiguous uint8 CUDA buffer")
+        raise RuntimeError("%s needs a contiguous uint8 CUDA buffer" % who)
     offs = np.ascontiguousarray(offsets, np.int64).reshape(-1)
     hw = np.ascontiguousarray(src_hw, np.int32).reshape(-1, 2)
     B = offs.shape[0]
     if hw.shape[0] != B:
-        raise ValueError("preprocess_ragged: %d offsets for %d frame sizes" % (B, hw.shape[0]))
+        raise ValueError("%s: %d offsets for %d frame sizes" % (who, B, hw.shape[0]))
     if out is None:
         out = torch.empty((B, 3, dst_h, dst_w), dtype=torch.float32, device=packed_u8.device)
     tm = None
     if trans_input is not None:
         tr = np.ascontiguousarray(trans_input, np.float64).reshape(-1)
         if tr.shape[0] != 6 * B:
-            raise ValueError("preprocess_ragged: trans_input must hold %d 2x3 matrices" % B)
+            raise ValueError("%s: trans_input must hold %d 2x3 matrices" % (who, B))
         tm = tr.ctypes.data_as(ctypes.POINTER(ctypes.c_double))
     m = (ctypes.c_float * 3)(*[float(v) for v in mean])
     s = (ctypes.c_float * 3)(*[float(v) for v in std])
     with torch.cuda.device(packed_u8.device):
-        rc = L.cp_preprocess_ragged(_ptr(packed_u8), packed_u8.numel(), offs.ctypes.data_as(ctypes.POINTER(ctypes.c_int64)),
-                                    hw.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), _ptr(out), B, dst_h, dst_w, tm, m, s,
-                                    _stream())
-    _lib.check(rc, "cp_preprocess_ragged")
+        rc = getattr(L, "cp_" + who)(_ptr(packed_u8), packed_u8.numel(), offs.ctypes.data_as(ctypes.POINTER(ctypes.c_int64)),
+                                     hw.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), *fmt, _ptr(out), B, dst_h, dst_w,
+                                     tm, m, s, _stream())
+    _lib.check(rc, "cp_" + who)
     return out
+
+
+def preprocess_ragged(packed_u8, offsets, src_hw, dst_h, dst_w, mean, std, out=None, trans_input=None):
+    """cp_preprocess_ragged: B frames of different sizes in one launch.  packed_u8: flat uint8 CUDA buffer holding frame b
+    (uint8 [src_hw[b][0], src_hw[b][1], 3]) at byte offsets[b] -> fp32 [B,3,dst_h,dst_w] CUDA, frame b bit for bit what
+    `preprocess` gives for it alone.  trans_input: optional [B,2,3] forward affines; default = each frame's fix_res affine."""
+    return _preprocess_packed("preprocess_ragged", packed_u8, offsets, src_hw, (), dst_h, dst_w, mean, std, out,
+                              trans_input)
 
 
 _YUV420 = {"nv12": _lib.CP_PIX_NV12, "i420": _lib.CP_PIX_I420}
@@ -612,33 +619,12 @@ def preprocess_formats(packed_u8, offsets, src_hw, pixel_format, dst_h, dst_w, m
     names (one per frame).  packed_u8: flat uint8 CUDA buffer holding frame b (its pixel format's buffer of image size
     src_hw[b]) at byte offsets[b] -> fp32 [B,3,dst_h,dst_w] CUDA, frame b bit for bit what preprocess_ragged gives for
     cv2.cvtColor(frame) to BGR.  trans_input: optional [B,2,3] forward affines; default = each frame's fix_res affine."""
-    L = _lib.load()
-    offs = np.ascontiguousarray(offsets, np.int64).reshape(-1)
-    hw = np.ascontiguousarray(src_hw, np.int32).reshape(-1, 2)
-    B = offs.shape[0]
-    codes = np.array([_lib.PIXEL_FORMAT_CODES[f] for f in slot_formats(pixel_format, B, "preprocess_formats")],
-                     np.int32)
-    if not packed_u8.is_cuda or packed_u8.dtype != torch.uint8 or not packed_u8.is_contiguous():
-        raise RuntimeError("preprocess_formats needs a contiguous uint8 CUDA buffer")
-    if hw.shape[0] != B:
-        raise ValueError("preprocess_formats: %d offsets for %d frame sizes" % (B, hw.shape[0]))
-    if out is None:
-        out = torch.empty((B, 3, dst_h, dst_w), dtype=torch.float32, device=packed_u8.device)
-    tm = None
-    if trans_input is not None:
-        tr = np.ascontiguousarray(trans_input, np.float64).reshape(-1)
-        if tr.shape[0] != 6 * B:
-            raise ValueError("preprocess_formats: trans_input must hold %d 2x3 matrices" % B)
-        tm = tr.ctypes.data_as(ctypes.POINTER(ctypes.c_double))
-    m = (ctypes.c_float * 3)(*[float(v) for v in mean])
-    s = (ctypes.c_float * 3)(*[float(v) for v in std])
-    with torch.cuda.device(packed_u8.device):
-        rc = L.cp_preprocess_formats(_ptr(packed_u8), packed_u8.numel(), offs.ctypes.data_as(ctypes.POINTER(ctypes.c_int64)),
-                                     hw.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)),
-                                     codes.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), _ptr(out), B, dst_h, dst_w, tm,
-                                     m, s, _stream())
-    _lib.check(rc, "cp_preprocess_formats")
-    return out
+    _lib.load()
+    codes = np.array([_lib.PIXEL_FORMAT_CODES[f] for f in slot_formats(pixel_format, np.size(offsets),
+                                                                       "preprocess_formats")], np.int32)
+    return _preprocess_packed("preprocess_formats", packed_u8, offsets, src_hw,
+                              (codes.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)),), dst_h, dst_w, mean, std, out,
+                              trans_input)
 
 
 def preprocess_yuv420(packed_u8, offsets, src_hw, pixel_format, dst_h, dst_w, mean, std, out=None, trans_input=None):
@@ -646,32 +632,11 @@ def preprocess_yuv420(packed_u8, offsets, src_hw, pixel_format, dst_h, dst_w, me
     (uint8 [3H/2,W] in pixel_format "nv12" or "i420", (H, W) = src_hw[b], both even) at byte offsets[b] -> fp32
     [B,3,dst_h,dst_w] CUDA, frame b bit for bit what preprocess_ragged gives for cv2.cvtColor(frame, COLOR_YUV2BGR_*).
     trans_input: optional [B,2,3] forward affines; default = each frame's fix_res affine (that of `preprocess`)."""
-    L = _lib.load()
+    _lib.load()
     if pixel_format not in _YUV420:
         raise ValueError("preprocess_yuv420: pixel_format must be 'nv12' or 'i420', got %r" % (pixel_format,))
-    if not packed_u8.is_cuda or packed_u8.dtype != torch.uint8 or not packed_u8.is_contiguous():
-        raise RuntimeError("preprocess_yuv420 needs a contiguous uint8 CUDA buffer")
-    offs = np.ascontiguousarray(offsets, np.int64).reshape(-1)
-    hw = np.ascontiguousarray(src_hw, np.int32).reshape(-1, 2)
-    B = offs.shape[0]
-    if hw.shape[0] != B:
-        raise ValueError("preprocess_yuv420: %d offsets for %d frame sizes" % (B, hw.shape[0]))
-    if out is None:
-        out = torch.empty((B, 3, dst_h, dst_w), dtype=torch.float32, device=packed_u8.device)
-    tm = None
-    if trans_input is not None:
-        tr = np.ascontiguousarray(trans_input, np.float64).reshape(-1)
-        if tr.shape[0] != 6 * B:
-            raise ValueError("preprocess_yuv420: trans_input must hold %d 2x3 matrices" % B)
-        tm = tr.ctypes.data_as(ctypes.POINTER(ctypes.c_double))
-    m = (ctypes.c_float * 3)(*[float(v) for v in mean])
-    s = (ctypes.c_float * 3)(*[float(v) for v in std])
-    with torch.cuda.device(packed_u8.device):
-        rc = L.cp_preprocess_yuv420(_ptr(packed_u8), packed_u8.numel(), offs.ctypes.data_as(ctypes.POINTER(ctypes.c_int64)),
-                                    hw.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), _YUV420[pixel_format], _ptr(out), B,
-                                    dst_h, dst_w, tm, m, s, _stream())
-    _lib.check(rc, "cp_preprocess_yuv420")
-    return out
+    return _preprocess_packed("preprocess_yuv420", packed_u8, offsets, src_hw, (_YUV420[pixel_format],), dst_h, dst_w,
+                              mean, std, out, trans_input)
 
 
 def conv2d_nhwc(x, weight, bias=None, residual=None, stride=1, pad=0, relu=False, precision="fp32"):
