@@ -76,12 +76,12 @@ struct IgemmParams {
   int mask_is_logit;     // 1: apply sigmoid to channels 18..26
   int mode;
   const void* wgt_umma;  // tensor-core path: pre-swizzled weight tiles (igemm_umma.cu, conv_tma.cu, dcn_tma.cu), else null
+  // conv_tma / dcn_tma split-K workspace (plan-owned; null = no split-K): partial sums
+  float* splitk_ws;
+  size_t splitk_ws_floats;
   // conv_tma only: the per-head 1x1 convolutions fused into the epilogue of the merged heads 3x3 conv.  Head h owns the
   // output columns [h * fuse_hidden, (h + 1) * fuse_hidden); its 1x1 weights are [fuse_hidden][16] fp32 (rows = hidden
   // channel, 16 padded outputs), bias [16], output NCHW [B, fuse_cout[h], Hout, Wout].  fuse_n == 0: not fused.
-  // conv_tma split-K workspace (plan-owned; null = no split-K): partial sums
-  float* splitk_ws;
-  size_t splitk_ws_floats;
   int fuse_n, fuse_hidden;
   const float* fuse_w[16];
   const float* fuse_b[16];
@@ -161,6 +161,19 @@ int run_conv(IgemmParams& p, int32_t precision, const ConvPolicy& pol, cudaStrea
 // Split-K of the persistent TMA kernels: the largest divisor S of `slabs` such that tiles x S CTAs fit the SMs and their
 // partial sums (tile_floats each) fit the workspace; 1 = off.  CP_NO_SPLITK=1 turns it off; it is read at every launch.
 int splitk_factor(long long tiles, int slabs, int num_sms, size_t tile_floats, size_t ws_floats);
+// How a launch of conv_tma / dcn_tma sums the K slabs of its (m, n) tiles.
+struct KSplit {
+  int ksplit = 1;            // K segments per tile (1: one)
+  int sps = 0;               // slabs per segment
+  bool fold = false;         // one CTA per tile runs the segments back to back (the FOLD kernel instances)
+  long long total_tiles = 0; // tiles of the persistent grid: (m, n) tiles, times ksplit unless folded
+  unsigned grid = 0;         // CTAs: min(total_tiles, SMs)
+};
+// Batch-invariant plans (k.ksegments > 0) take the plan's segments, split over CTAs where the partial sums fit the
+// workspace and folded otherwise; other plans split as splitk_factor says.  can_split: the launch has split-K and fold
+// instances.  Fails (CP_ERR_INVALID, messages prefixed with `who`) where the segments do not fit the launch.
+int ksplit_for(const ConvKernel& k, long long mn_tiles, int slabs, size_t tile_floats, size_t ws_floats, bool can_split,
+               const char* who, KSplit* out);
 
 // wgmma tensor-core gather path (igemm_umma.cu).  prec: 0 = bf16, 1 = tf32 x 3 (fp32-equivalent)
 bool umma_supported(const IgemmParams& p, int prec);
@@ -272,10 +285,10 @@ inline int current_device_slot() {
   if (cudaGetDevice(&d) != cudaSuccess || d < 0 || d >= kMaxDevices) d = 0;
   return d;
 }
-template <typename T, int N = 1>
+template <typename T>
 struct PerDevice {
-  T v[kMaxDevices][N] = {};
-  T& here(int slot = 0) { return v[current_device_slot()][slot]; }
+  T v[kMaxDevices] = {};
+  T& here() { return v[current_device_slot()]; }
 };
 inline int device_sm_count(int* out) {
   static PerDevice<int> cache;
@@ -288,5 +301,27 @@ inline int device_sm_count(int* out) {
   *out = n;
   return CP_OK;
 }
+#ifdef __CUDACC__
+// A kernel instance and its opt-in to the 227 KB of dynamic shared memory of an SM, made once per device and instance:
+// opt_in_smem<Kernel> keeps its own per-device flag.  Null fn: no such instance.
+template <class Fn>
+struct SmemKernel {
+  Fn fn = nullptr;
+  int (*opt_in)() = nullptr;
+};
+template <auto Kernel>
+int opt_in_smem() {
+  static PerDevice<bool> configured;
+  if (!configured.here()) {
+    CP_CUDA_CHECK(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    configured.here() = true;
+  }
+  return CP_OK;
+}
+template <auto Kernel>
+SmemKernel<decltype(Kernel)> smem_kernel() {
+  return {Kernel, opt_in_smem<Kernel>};
+}
+#endif
 
 }  // namespace cp

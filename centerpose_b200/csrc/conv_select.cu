@@ -95,4 +95,25 @@ int splitk_factor(long long tiles, int slabs, int num_sms, size_t tile_floats, s
   return S;
 }
 
+int ksplit_for(const ConvKernel& k, long long mn_tiles, int slabs, size_t tile_floats, size_t ws_floats, bool can_split,
+               const char* who, KSplit* out) {
+  int num_sms = 0;
+  if (int rc = device_sm_count(&num_sms)) return rc;
+  KSplit r;
+  if (k.ksegments > 0) {
+    if (slabs % k.ksegments || (k.ksegments > 1 && !can_split))
+      return fail(CP_ERR_INVALID, std::string(who) + ": K segments do not fit the launch");
+    r.ksplit = k.ksegments;
+    r.fold = r.ksplit > 1 && (size_t)mn_tiles * r.ksplit * tile_floats > ws_floats;
+  } else {
+    r.ksplit = can_split ? splitk_factor(mn_tiles, slabs, num_sms, tile_floats, ws_floats) : 1;
+  }
+  r.sps = slabs / r.ksplit;
+  r.total_tiles = r.fold ? mn_tiles : mn_tiles * r.ksplit;
+  if (r.total_tiles >= (1ll << 31)) return fail(CP_ERR_INVALID, std::string(who) + ": too many tiles");
+  r.grid = (unsigned)(r.total_tiles < num_sms ? r.total_tiles : num_sms);
+  *out = r;
+  return CP_OK;
+}
+
 }  // namespace cp

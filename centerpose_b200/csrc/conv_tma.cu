@@ -35,6 +35,8 @@ constexpr int TM_THREADS_X3F = 640;   // + the fused 1x1 warpgroup
 constexpr uint32_t TM_HSLOT_BYTES = 128u * 32u * 4u;
 constexpr uint32_t TM_W1_BYTES = 128u * 16u * 4u;
 
+using namespace umma;
+
 struct TmaConvParams {
   CUtensorMap amap[4];
   int nsrc;
@@ -48,12 +50,7 @@ struct TmaConvParams {
   long long m_tiles;                    // number of 128-position tiles
   uint32_t slab_bytes, slab_stride;   // TMA transaction bytes, 1024-aligned stage stride
   int SA, SB;
-  const float* bias;
-  const float* residual;
-  int resStride, relu, res_after_relu;
-  float* out;
-  int outStride, out_nchw;
-  int round_tf32;     // round the stored outputs to tf32 (consumers feed them to the tf32 MMAs untouched)
+  EpiParams epi;      // round_tf32: the layers that read the outputs feed them to the tf32 MMAs untouched
   int cslab;          // channels per slab: 32 (128-byte rows, SWIZZLE_128B) or 16 (64-byte rows, SWIZZLE_64B; Cin = 16 layers)
   int x3;             // 3-term split (fp32-equivalent): hi/lo slabs + hi/lo weight tiles, BN <= 128
   int group;          // x3: K blocks per accumulation group (promoted into the fp32 sums after each group)
@@ -62,7 +59,7 @@ struct TmaConvParams {
   // CTA stores its promoted partial sums and conv_tma_splitk_finish adds them in split order (deterministic) and runs
   // the epilogue.  ksplit == 1: off.  Tile index = (m, n) tile * ksplit + split.
   int ksplit, sps;
-  float* part;          // [mn tiles][ksplit][BN / 4][tile_m] float4
+  float* part;          // split-K workspace (park_partial, umma_common.cuh)
   // fused per-head 1x1 (see IgemmParams): tph = N tiles per head, processed back to back by the same CTA
   int fuse, tph;
   const float* fuse_w[16];
@@ -75,8 +72,6 @@ struct TmaConvParams {
   long long wstride, tstride, tiles_per_model;
   int RS;             // x3 fused 1x1: slots of the hidden ring (1 or 2)
 };
-
-using namespace umma;
 
 struct TmaCtl {
   unsigned long long a_full[4], a_empty[4], a_split[4];
@@ -410,20 +405,7 @@ __global__ void __launch_bounds__(X3 ? (FUSE ? TM_THREADS_X3F : TM_THREADS_X3) :
     const uint32_t bar_a_empty = smem_u32(&ctl->a_empty[0]);
     const uint32_t bar_b_full = smem_u32(&ctl->b_full[0]), bar_b_empty = smem_u32(&ctl->b_empty[0]);
     const uint32_t a_lo_u = p.slab_stride >> 4, b_lo_u = ((uint32_t)BN * rowb) >> 4;
-    EpiParams ep;
-    ep.bias = p.bias;
-    ep.residual = p.residual;
-    ep.resStride = p.resStride;
-    ep.relu = p.relu;
-    ep.res_after_relu = p.res_after_relu;
-    ep.round_tf32 = p.round_tf32;
-    ep.out = p.out;
-    ep.outStride = p.outStride;
-    ep.out_nchw = p.out_nchw;
-    ep.Cout = p.Cout;
-    ep.CoutPad = p.CoutPad;
-    ep.H = p.H;
-    ep.W = p.W;
+    EpiParams ep = tile_epi(p);
     int sa = 0, sb = 0;
     uint32_t pa = 0, pb = 0;
     float acc[BN / 2];
@@ -521,7 +503,7 @@ __global__ void __launch_bounds__(X3 ? (FUSE ? TM_THREADS_X3F : TM_THREADS_X3) :
         // relu(conv + bias) of this warpgroup's 64 rows goes to the hidden ring, 32 columns per slot, 16-byte groups
         // XOR-swizzled by row & 7 (conflict-free float4 reads); the 1x1 warpgroup takes it from there
         const int fr0 = (wt >> 5) * 16 + ((wt & 31) >> 2), fcq = (wt & 3) * 2;     // accumulator fragment (drain_rows)
-        const float* b1 = p.bias + (MULTI ? (size_t)g.model * p.wstride : 0) + (size_t)g.n_tile * BN;
+        const float* b1 = p.epi.bias + (MULTI ? (size_t)g.model * p.wstride : 0) + (size_t)g.n_tile * BN;
         float* hring = reinterpret_cast<float*>(smem + (drain0 - smem_u32(smem)));        // hidden ring
         const uint32_t bar_h_full = smem_u32(&ctl->h_full[0]), bar_h_empty = smem_u32(&ctl->h_empty[0]);
         auto at = [&](int r, int col) { return r * 32 + ((((col >> 2) ^ r) & 7) << 2) + (col & 3); };
@@ -553,7 +535,7 @@ __global__ void __launch_bounds__(X3 ? (FUSE ? TM_THREADS_X3F : TM_THREADS_X3) :
       const int col_end = min(p.Cout, (g.n_tile + 1) * BN);
       const int head = FUSE ? g.n_tile / p.tph : 0, part = FUSE ? g.n_tile - head * p.tph : 0;
       const size_t wofs = MULTI ? (size_t)g.model * p.wstride : 0;      // this tile's model's biases and fused 1x1 weights
-      if (MULTI) ep.bias = p.bias + wofs;
+      if (MULTI) ep.bias = p.epi.bias + wofs;
       if (FUSE && part == 0) {
 #pragma unroll
         for (int j = 0; j < (FUSE ? 16 : 1); ++j) acc2[j] = 0.f;
@@ -561,8 +543,10 @@ __global__ void __launch_bounds__(X3 ? (FUSE ? TM_THREADS_X3F : TM_THREADS_X3) :
       auto fn = [&](int r, int cb, float (&v)[16]) {
         if (cb >= BN) return;
         if (!FUSE && KS_SPLIT > 1) {
-          // split-K: park the partial sums of this K range, [mn tile][split][float4 column group][row];
-          // conv_tma_splitk_finish adds the ranges in split order (a fixed summation order) and runs the epilogue
+          // split-K: park the partial sums of this K range in park_partial's layout (umma_common.cuh);
+          // conv_tma_splitk_finish adds the ranges in split order (a fixed summation order) and runs the epilogue.
+          // Written out here, not through park_partial: the call changes the register allocation of these instances,
+          // and the tf32 multi-model ones ran 1.7 % slower (H100 80GB HBM3, 700 W).
           const long long mn = tile / KS_SPLIT;
           const int ks = (int)(tile % KS_SPLIT);
           float4* mine = reinterpret_cast<float4*>(p.part) + (((size_t)mn * KS_SPLIT + ks) * (BN >> 2) + (cb >> 2)) * p.tile_m +
@@ -571,7 +555,7 @@ __global__ void __launch_bounds__(X3 ? (FUSE ? TM_THREADS_X3F : TM_THREADS_X3) :
           for (int q = 0; q < 4; ++q) __stcg(mine + (size_t)q * p.tile_m, make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]));
         } else if (FUSE) {
           // hidden = relu(conv3x3 + bias) never leaves the SM: multiply it with this head's 1x1 weights right here
-          const float* b1 = p.bias + wofs + (size_t)g.n_tile * BN + cb;
+          const float* b1 = p.epi.bias + wofs + (size_t)g.n_tile * BN + cb;
           const float4* w2 = reinterpret_cast<const float4*>(p.fuse_w[head] + wofs) + ((size_t)part * BN + cb) * 4;
 #pragma unroll
           for (int q = 0; q < 16; ++q) {
@@ -824,32 +808,28 @@ int tma_conv_encode(const IgemmParams& p, int Bmax, int cs, void* maps_out) {
   return CP_OK;
 }
 
-// FOLD (x3, not fused only): the K segments folded in one CTA per tile (batch-invariant plans)
-template <bool X3, bool FUSE, bool MULTI, bool FOLD = false>
-static int launch_conv_tma_kernel(const TmaConvParams& q, const cudaLaunchConfig_t& cfg0) {
-  void (*kern)(TmaConvParams) = nullptr;
-  switch (q.BN) {
-    case 16: kern = conv_tma_kernel<X3, FUSE, 16, MULTI, FOLD>; break;
-    case 32: kern = conv_tma_kernel<X3, FUSE, 32, MULTI, FOLD>; break;
-    case 64: kern = conv_tma_kernel<X3, FUSE, 64, MULTI, FOLD>; break;
-    case 128: kern = conv_tma_kernel<X3, FUSE, 128, MULTI, FOLD>; break;
-    default: return fail(CP_ERR_INVALID, "conv_tma: unsupported N tile");
+// The instance of one launch (null fn: no such instance).  FOLD (x3, not fused only): the K segments folded in one CTA
+// per tile.
+using ConvTmaKernel = SmemKernel<void (*)(TmaConvParams)>;
+template <bool X3, bool FUSE, bool MULTI, bool FOLD>
+static ConvTmaKernel conv_tma_kernel_bn(int BN) {
+  switch (BN) {
+    case 16: return smem_kernel<conv_tma_kernel<X3, FUSE, 16, MULTI, FOLD>>();
+    case 32: return smem_kernel<conv_tma_kernel<X3, FUSE, 32, MULTI, FOLD>>();
+    case 64: return smem_kernel<conv_tma_kernel<X3, FUSE, 64, MULTI, FOLD>>();
+    case 128: return smem_kernel<conv_tma_kernel<X3, FUSE, 128, MULTI, FOLD>>();
+    default: return {};
   }
-  static PerDevice<bool, 4> configured;
-  const int slot = q.BN == 128 ? 3 : (q.BN == 64 ? 2 : (q.BN == 32 ? 1 : 0));
-  if (!configured.here(slot)) {
-    CP_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    configured.here(slot) = true;
-  }
-  cudaLaunchConfig_t cfg = cfg0;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = g_pdl ? 1 : 0;
-  CP_CUDA_CHECK(cudaLaunchKernelEx(&cfg, kern, q));
-  CP_LAUNCH_CHECK("conv_tma_kernel");
-  return CP_OK;
+}
+static ConvTmaKernel conv_tma_kernel_for(int BN, bool x3, bool fuse, bool multi, bool fold) {
+  if (fold)
+    return !x3 || fuse ? ConvTmaKernel{}
+                       : (multi ? conv_tma_kernel_bn<true, false, true, true>(BN) : conv_tma_kernel_bn<true, false, false, true>(BN));
+  if (multi)
+    return x3 ? (fuse ? conv_tma_kernel_bn<true, true, true, false>(BN) : conv_tma_kernel_bn<true, false, true, false>(BN))
+              : (fuse ? conv_tma_kernel_bn<false, true, true, false>(BN) : conv_tma_kernel_bn<false, false, true, false>(BN));
+  return x3 ? (fuse ? conv_tma_kernel_bn<true, true, false, false>(BN) : conv_tma_kernel_bn<true, false, false, false>(BN))
+            : (fuse ? conv_tma_kernel_bn<false, true, false, false>(BN) : conv_tma_kernel_bn<false, false, false, false>(BN));
 }
 
 int launch_conv_tma(const IgemmParams& p, const void* maps, const ConvKernel& k, cudaStream_t stream, LaunchInfo* info) {
@@ -894,15 +874,7 @@ int launch_conv_tma(const IgemmParams& p, const void* maps, const ConvKernel& k,
   const uint32_t a_stage = q.slab_stride * (x3 ? 2u : 1u);
   size_t smem = 0;
   if (int rc = tma_smem_layout(a_stage, btile, q.k, x3 && p.fuse_n > 0, &q.SA, &q.SB, &q.RS, &smem)) return rc;
-  q.bias = p.bias;
-  q.residual = p.residual;
-  q.resStride = p.resStride;
-  q.relu = p.relu;
-  q.res_after_relu = p.res_after_relu;
-  q.out = p.out;
-  q.outStride = p.outStride;
-  q.out_nchw = p.out_nchw;
-  q.round_tf32 = k.round_out;
+  q.epi = epi_params(p, k.round_out);
   q.wtiles = (const unsigned char*)p.wgt_umma;
   if (p.fuse_n > 0) {
     if (p.fuse_hidden % q.BN || p.CoutPad != p.fuse_n * p.fuse_hidden || !p.relu || p.residual || (x3 && q.BN != 128))
@@ -919,56 +891,24 @@ int launch_conv_tma(const IgemmParams& p, const void* maps, const ConvKernel& k,
   q.m_tiles = (long long)m_tiles;
   q.part = p.splitk_ws;
   const long long mn = (long long)m_tiles * (p.CoutPad / q.BN);
-  const int nslab = q.Cin / q.cslab;
-  int num_sms = 0;
-  if (int rc = device_sm_count(&num_sms)) return rc;
   // split-K (tf32x3, plain epilogue): small feature maps give a persistent kernel fewer tiles than SMs while every tile
   // walks a long serial K loop (level5 at batch 1: 16 tiles x 144 K blocks).  Deal slab-aligned K ranges to more CTAs.
-  // Batch-invariant plans fix the segments by the layer's shape (k.ksegments) and split them only when their partial sums
-  // fit the workspace; otherwise one CTA per tile folds them (the FOLD instances of conv_tma_kernel), with the same bits.
-  const size_t tile_floats = (size_t)q.tile_m * q.BN;
-  bool fold = false;
-  if (k.ksegments > 0) {
-    if (nslab % k.ksegments || (k.ksegments > 1 && (!x3 || q.fuse)))
-      return fail(CP_ERR_INVALID, "conv_tma: K segments do not fit the launch");
-    q.ksplit = k.ksegments;
-    fold = q.ksplit > 1 && (size_t)mn * q.ksplit * tile_floats > p.splitk_ws_floats;
-  } else {
-    q.ksplit = x3 && !q.fuse ? splitk_factor(mn, nslab, num_sms, tile_floats, p.splitk_ws_floats) : 1;
-  }
-  q.sps = nslab / q.ksplit;
-  q.total_tiles = fold ? mn : mn * q.ksplit;
-  if (q.total_tiles >= (1ll << 31)) return fail(CP_ERR_INVALID, "conv_tma: too many tiles");
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)(q.total_tiles < num_sms ? q.total_tiles : num_sms));
-  cfg.blockDim = dim3(x3 ? (q.fuse ? TM_THREADS_X3F : TM_THREADS_X3) : TM_THREADS);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
+  KSplit ks;
+  if (int rc = ksplit_for(k, mn, q.Cin / q.cslab, (size_t)q.tile_m * q.BN, p.splitk_ws_floats, x3 && !q.fuse, "conv_tma", &ks))
+    return rc;
+  q.ksplit = ks.ksplit;
+  q.sps = ks.sps;
+  q.total_tiles = ks.total_tiles;
   // several models in the launch: the model-indexed instantiations; one model runs the one-model code unchanged
   const bool multi = p.B > q.ipm;
-  int rc;
-  if (fold)
-    rc = multi ? launch_conv_tma_kernel<true, false, true, true>(q, cfg) : launch_conv_tma_kernel<true, false, false, true>(q, cfg);
-  else if (multi)
-    rc = x3 ? (q.fuse ? launch_conv_tma_kernel<true, true, true>(q, cfg) : launch_conv_tma_kernel<true, false, true>(q, cfg))
-            : (q.fuse ? launch_conv_tma_kernel<false, true, true>(q, cfg) : launch_conv_tma_kernel<false, false, true>(q, cfg));
-  else
-    rc = x3 ? (q.fuse ? launch_conv_tma_kernel<true, true, false>(q, cfg) : launch_conv_tma_kernel<true, false, false>(q, cfg))
-            : (q.fuse ? launch_conv_tma_kernel<false, true, false>(q, cfg) : launch_conv_tma_kernel<false, false, false>(q, cfg));
-  if (rc) return rc;
-  if (info) {
-    info->BN = q.BN;
-    info->ksplit = q.ksplit;
-    info->grid = cfg.gridDim.x;
-    info->path = q.ksplit == 1 ? CP_KPATH_ONE : (fold ? CP_KPATH_FOLD : CP_KPATH_SPLIT);
-  }
-  if (q.ksplit > 1 && !fold) {
-    const long long threads = mn * (q.BN / 4) * q.tile_m;
-    CP_CUDA_CHECK(launch_kernel(multi ? conv_tma_splitk_finish<true> : conv_tma_splitk_finish<false>,
-                                dim3((unsigned)((threads + 255) / 256)), dim3(256), 0, stream, q, mn));
-    CP_LAUNCH_CHECK("conv_tma_splitk_finish");
-  }
-  return CP_OK;
+  const ConvTmaKernel kern = conv_tma_kernel_for(q.BN, x3, q.fuse, multi, ks.fold);
+  if (!kern.fn) return fail(CP_ERR_INVALID, "conv_tma: unsupported N tile");
+  if (int rc = kern.opt_in()) return rc;
+  CP_CUDA_CHECK(launch_kernel(kern.fn, dim3(ks.grid), dim3(x3 ? (q.fuse ? TM_THREADS_X3F : TM_THREADS_X3) : TM_THREADS), smem,
+                              stream, q));
+  CP_LAUNCH_CHECK("conv_tma_kernel");
+  return splitk_tail(ks, q, q.tile_m, mn, multi ? conv_tma_splitk_finish<true> : conv_tma_splitk_finish<false>, stream, info,
+                     "conv_tma");
 }
 
 }  // namespace cp

@@ -56,14 +56,10 @@ struct DcnTmaParams {
   long long total_tiles;             // m tiles x n tiles (n fastest)
   int SB;
   int AH;                            // A stages (1, 2 or 4)
-  const float* bias;
-  const float* residual;
-  int resStride, relu, res_after_relu;
-  float* out;
-  int outStride, out_nchw, round_tf32;
+  EpiParams epi;
   const unsigned char* wtiles;
   // split-K (small maps: fewer tiles than SMs): tile = (m, n) tile * ksplit + split; a split walks `sps` slabs, stores its
-  // partial sums to `part` ([mn tile][split][BN / 4][128 rows] float4) and dcn_tma_splitk_finish runs the epilogue
+  // partial sums to `part` (park_partial, umma_common.cuh) and dcn_tma_splitk_finish runs the epilogue
   int ksplit, sps;
   float* part;
   int ipm;                           // models (IgemmParams::ipm): image n takes model n / ipm's bias and weight tiles
@@ -380,20 +376,7 @@ __global__ void __launch_bounds__(DT_THREADS, 1) dcn_tma_kernel(const __grid_con
     asm volatile("setmaxnreg.inc.sync.aligned.u32 176;");
     const int c = warp >= 12 ? 1 : 0, wt = tid & 127;
     float* dstage = reinterpret_cast<float*>(smem + (drain0 - sbase)) + (size_t)c * (DRAIN_STAGE_BYTES / 4);
-    EpiParams ep;
-    ep.bias = p.bias;
-    ep.residual = p.residual;
-    ep.resStride = p.resStride;
-    ep.relu = p.relu;
-    ep.res_after_relu = p.res_after_relu;
-    ep.round_tf32 = p.round_tf32;
-    ep.out = p.out;
-    ep.outStride = p.outStride;
-    ep.out_nchw = p.out_nchw;
-    ep.Cout = p.Cout;
-    ep.CoutPad = p.CoutPad;
-    ep.H = p.H;
-    ep.W = p.W;
+    EpiParams ep = tile_epi(p);
     const uint32_t bar_a_full = smem_u32(&ctl->a_full[0]), bar_a_empty = smem_u32(&ctl->a_empty[0]);
     const uint32_t bar_b_full = smem_u32(&ctl->b_full[0]), bar_b_empty = smem_u32(&ctl->b_empty[0]);
     const uint32_t b_lo = ((uint32_t)BN * 64u) >> 4;
@@ -509,15 +492,13 @@ __global__ void __launch_bounds__(DT_THREADS, 1) dcn_tma_kernel(const __grid_con
       const int n = (int)(m_tile / p.tiles_per_image);
       const int pt = (int)(m_tile - (long long)n * p.tiles_per_image);
       const int col_end = min(p.Cout, (n_tile + 1) * BN);
-      if (MULTI) ep.bias = p.bias + (size_t)(n / p.ipm) * p.wstride;
+      if (MULTI) ep.bias = p.epi.bias + (size_t)(n / p.ipm) * p.wstride;
       auto fn = [&](int r, int cb0, float (&v)[16]) {
         if (cb0 >= BN) return;
         const int i = c * 64 + r;
         if (KS_SPLIT > 1) {
           // split-K: the finished columns of this position go to the workspace instead of through the epilogue
-          float4* part_row = reinterpret_cast<float4*>(p.part) + ((size_t)tile * (BN >> 2) + (cb0 >> 2)) * 128 + i;
-#pragma unroll
-          for (int q = 0; q < 4; ++q) __stcg(part_row + (size_t)q * 128, make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]));
+          park_partial<BN>(p.part, tile, cb0, i, DT_BM, v);
         } else {
           const int oy = (pt / p.tiles_x) * DT_PH + (i >> 4), ox = (pt % p.tiles_x) * DT_PW + (i & 15);
           const int m = (n * p.H + oy) * p.W + ox;
@@ -569,21 +550,24 @@ int dcn_tma_encode(const IgemmParams& p, int Bmax, void* map_out) {
   return tma_encode_nhwc_box(p.src[0], p.srcC[0], p.Win, p.Hin, Bmax, p.srcStride[0], DT_CS, DT_SW, DT_SH, 1, map_out);
 }
 
-// The instance of one launch (null: no such N tile).  FOLD: the K segments folded in one CTA per tile.
-using DcnTmaKernel = void (*)(DcnTmaParams);
-template <bool FOLD>
-static DcnTmaKernel dcn_tma_kernel_for(int BN, bool x3, bool multi) {
+// The instance of one launch (null fn: no such N tile).  FOLD: the K segments folded in one CTA per tile.
+using DcnTmaKernel = SmemKernel<void (*)(DcnTmaParams)>;
+template <bool X3, bool MULTI, bool FOLD>
+static DcnTmaKernel dcn_tma_kernel_bn(int BN) {
   switch (BN) {
-    case 16: return multi ? (x3 ? dcn_tma_kernel<true, 16, true, FOLD> : dcn_tma_kernel<false, 16, true, FOLD>)
-                          : (x3 ? dcn_tma_kernel<true, 16, false, FOLD> : dcn_tma_kernel<false, 16, false, FOLD>);
-    case 32: return multi ? (x3 ? dcn_tma_kernel<true, 32, true, FOLD> : dcn_tma_kernel<false, 32, true, FOLD>)
-                          : (x3 ? dcn_tma_kernel<true, 32, false, FOLD> : dcn_tma_kernel<false, 32, false, FOLD>);
-    case 64: return multi ? (x3 ? dcn_tma_kernel<true, 64, true, FOLD> : dcn_tma_kernel<false, 64, true, FOLD>)
-                          : (x3 ? dcn_tma_kernel<true, 64, false, FOLD> : dcn_tma_kernel<false, 64, false, FOLD>);
-    case 128: return multi ? (x3 ? dcn_tma_kernel<true, 128, true, FOLD> : dcn_tma_kernel<false, 128, true, FOLD>)
-                           : (x3 ? dcn_tma_kernel<true, 128, false, FOLD> : dcn_tma_kernel<false, 128, false, FOLD>);
-    default: return nullptr;
+    case 16: return smem_kernel<dcn_tma_kernel<X3, 16, MULTI, FOLD>>();
+    case 32: return smem_kernel<dcn_tma_kernel<X3, 32, MULTI, FOLD>>();
+    case 64: return smem_kernel<dcn_tma_kernel<X3, 64, MULTI, FOLD>>();
+    case 128: return smem_kernel<dcn_tma_kernel<X3, 128, MULTI, FOLD>>();
+    default: return {};
   }
+}
+static DcnTmaKernel dcn_tma_kernel_for(int BN, bool x3, bool multi, bool fold) {
+  if (fold)
+    return multi ? (x3 ? dcn_tma_kernel_bn<true, true, true>(BN) : dcn_tma_kernel_bn<false, true, true>(BN))
+                 : (x3 ? dcn_tma_kernel_bn<true, false, true>(BN) : dcn_tma_kernel_bn<false, false, true>(BN));
+  return multi ? (x3 ? dcn_tma_kernel_bn<true, true, false>(BN) : dcn_tma_kernel_bn<false, true, false>(BN))
+               : (x3 ? dcn_tma_kernel_bn<true, false, false>(BN) : dcn_tma_kernel_bn<false, false, false>(BN));
 }
 
 int launch_dcn_tma(const IgemmParams& p, const void* map, const ConvKernel& k, cudaStream_t stream, LaunchInfo* info) {
@@ -622,62 +606,27 @@ int launch_dcn_tma(const IgemmParams& p, const void* map, const ConvKernel& k, c
   if (fixed + 2 * (size_t)btile > budget) return fail(CP_ERR_INVALID, "dcn_tma: tile does not fit shared memory");
   q.SB = (int)((budget - fixed) / btile);
   if (q.SB > 8) q.SB = 8;
-  q.bias = p.bias;
-  q.residual = p.residual;
-  q.resStride = p.resStride;
-  q.relu = p.relu;
-  q.res_after_relu = p.res_after_relu;
-  q.out = p.out;
-  q.outStride = p.outStride;
-  q.out_nchw = p.out_nchw;
-  q.round_tf32 = k.round_out;
+  q.epi = epi_params(p, k.round_out);
   q.wtiles = (const unsigned char*)p.wgt_umma;
   q.ipm = model_ipm(p);
   q.wstride = p.wstride;
   q.tstride = p.tstride;
   const bool multi = p.B > q.ipm;      // several models: the model-indexed instantiations
   const size_t smem = fixed + (size_t)q.SB * btile;
-  int num_sms = 0;
-  if (int rc = device_sm_count(&num_sms)) return rc;
   // split-K: at batch 1 the 512 -> 256 DCN at 16 x 16 is 4 tiles of 288 K blocks; deal slab ranges to idle SMs.
-  // Batch-invariant plans fix the segments by the layer's shape (k.ksegments) and split them only when their partial sums
-  // fit the workspace; otherwise one CTA per tile folds them (the FOLD instances of dcn_tma_kernel), with the same bits.
-  const int nslab = p.Cin / DT_CS;
-  const size_t tile_floats = (size_t)DT_BM * q.BN;
-  bool fold = false;
+  KSplit ks;
+  if (int rc = ksplit_for(k, mn, p.Cin / DT_CS, (size_t)DT_BM * q.BN, p.splitk_ws_floats, true, "dcn_tma", &ks)) return rc;
+  q.ksplit = ks.ksplit;
+  q.sps = ks.sps;
+  q.total_tiles = ks.total_tiles;
   q.part = p.splitk_ws;
-  if (k.ksegments > 0) {
-    if (nslab % k.ksegments) return fail(CP_ERR_INVALID, "dcn_tma: K segments do not fit the launch");
-    q.ksplit = k.ksegments;
-    fold = q.ksplit > 1 && (size_t)mn * q.ksplit * tile_floats > p.splitk_ws_floats;
-  } else {
-    q.ksplit = splitk_factor(mn, nslab, num_sms, tile_floats, p.splitk_ws_floats);
-  }
-  q.sps = nslab / q.ksplit;
-  q.total_tiles = fold ? mn : mn * q.ksplit;
-  const DcnTmaKernel kern = fold ? dcn_tma_kernel_for<true>(q.BN, x3, multi) : dcn_tma_kernel_for<false>(q.BN, x3, multi);
-  if (!kern) return fail(CP_ERR_INVALID, "dcn_tma: unsupported N tile");
-  static PerDevice<bool, 32> configured;
-  const int slot = (fold ? 16 : 0) + (multi ? 8 : 0) + (x3 ? 4 : 0) + (q.BN == 128 ? 3 : (q.BN == 64 ? 2 : (q.BN == 32 ? 1 : 0)));
-  if (!configured.here(slot)) {
-    CP_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    configured.here(slot) = true;
-  }
-  const unsigned grid = (unsigned)(q.total_tiles < num_sms ? q.total_tiles : num_sms);
-  CP_CUDA_CHECK(launch_kernel(kern, dim3(grid), dim3(DT_THREADS), smem, stream, q));
+  const DcnTmaKernel kern = dcn_tma_kernel_for(q.BN, x3, multi, ks.fold);
+  if (!kern.fn) return fail(CP_ERR_INVALID, "dcn_tma: unsupported N tile");
+  if (int rc = kern.opt_in()) return rc;
+  CP_CUDA_CHECK(launch_kernel(kern.fn, dim3(ks.grid), dim3(DT_THREADS), smem, stream, q));
   CP_LAUNCH_CHECK("dcn_tma_kernel");
-  if (info) {
-    info->BN = q.BN;
-    info->ksplit = q.ksplit;
-    info->grid = grid;
-    info->path = q.ksplit == 1 ? CP_KPATH_ONE : (fold ? CP_KPATH_FOLD : CP_KPATH_SPLIT);
-  }
-  if (q.ksplit > 1 && !fold) {
-    const long long threads = mn * (q.BN / 4) * DT_BM;
-    CP_CUDA_CHECK(launch_kernel(multi ? dcn_tma_splitk_finish<true> : dcn_tma_splitk_finish<false>, dim3((unsigned)((threads + 255) / 256)), dim3(256), 0, stream, q, mn));
-    CP_LAUNCH_CHECK("dcn_tma_splitk_finish");
-  }
-  return CP_OK;
+  return splitk_tail(ks, q, DT_BM, mn, multi ? dcn_tma_splitk_finish<true> : dcn_tma_splitk_finish<false>, stream, info,
+                     "dcn_tma");
 }
 
 }  // namespace cp

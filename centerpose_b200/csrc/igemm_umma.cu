@@ -277,20 +277,9 @@ __global__ void __launch_bounds__(UM_THREADS, 1) igemm_umma_kernel(const IgemmPa
         }
       }
     }
-    EpiParams ep;
-    ep.bias = MULTI ? p.bias + (size_t)model * p.wstride : p.bias;
-    ep.residual = p.residual;
-    ep.resStride = p.resStride;
-    ep.relu = p.relu;
-    ep.res_after_relu = p.res_after_relu;
-    ep.round_tf32 = 0;
-    ep.out = p.out;
-    ep.outStride = p.outStride;
-    ep.out_nchw = p.out_nchw;
-    ep.Cout = p.Cout;
-    ep.CoutPad = p.CoutPad;
-    ep.H = p.Hout;
-    ep.W = p.Wout;
+    const float* bias = MULTI ? p.bias + (size_t)model * p.wstride : p.bias;
+    EpiParams ep = epi_params(p, false);
+    ep.bias = bias;
     const int col_end = min(p.Cout, (n_tile + 1) * BN);
     float* dstage = reinterpret_cast<float*>(smem + (tiles0 - smem_u32(smem)) + (size_t)STAGES * stage_bytes) +
                     (size_t)c * (DRAIN_STAGE_BYTES / 4);
@@ -408,22 +397,16 @@ int launch_pack_umma_weight(const float* src, int ld, int Kreal, int Cout, int C
 template <int PREC, int BN, bool MULTI>
 static int launch_igemm_umma_bn(const IgemmParams& p, int stages, size_t smem, int nacc, cudaStream_t stream,
                                 LaunchInfo* info) {
-  void (*kern)(const IgemmParams, const int, const int) =
-      (p.mode == IGEMM_DCN)      ? igemm_umma_kernel<PREC, IGEMM_DCN, BN, MULTI>
-      : (p.mode == IGEMM_DECONV) ? igemm_umma_kernel<PREC, IGEMM_DECONV, BN, MULTI>
-                                 : igemm_umma_kernel<PREC, IGEMM_NHWC_VEC, BN, MULTI>;
-  static PerDevice<bool, 3> configured;
-  const int slot = p.mode == IGEMM_DCN ? 1 : (p.mode == IGEMM_DECONV ? 2 : 0);
-  if (!configured.here(slot)) {
-    CP_CUDA_CHECK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
-    configured.here(slot) = true;
-  }
+  const auto kern = (p.mode == IGEMM_DCN)      ? smem_kernel<igemm_umma_kernel<PREC, IGEMM_DCN, BN, MULTI>>()
+                    : (p.mode == IGEMM_DECONV) ? smem_kernel<igemm_umma_kernel<PREC, IGEMM_DECONV, BN, MULTI>>()
+                                               : smem_kernel<igemm_umma_kernel<PREC, IGEMM_NHWC_VEC, BN, MULTI>>();
+  if (int rc = kern.opt_in()) return rc;
   IgemmParams q = p;
   q.ipm = model_ipm(p);
   const bool deconv = p.mode == IGEMM_DECONV;
   const int Mm = q.ipm * (deconv ? p.Hin * p.Win : p.Hout * p.Wout);
   dim3 grid((unsigned)((size_t)(p.CoutPad / BN) * ((Mm + UM_BM - 1) / UM_BM) * (p.B / q.ipm)), deconv ? 4 : 1);
-  CP_CUDA_CHECK(launch_kernel(kern, grid, dim3(UM_THREADS), smem, stream, q, stages, nacc));
+  CP_CUDA_CHECK(launch_kernel(kern.fn, grid, dim3(UM_THREADS), smem, stream, q, stages, nacc));
   CP_LAUNCH_CHECK("igemm_umma_kernel");
   if (info) {
     info->BN = BN;

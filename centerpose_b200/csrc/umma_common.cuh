@@ -5,6 +5,8 @@
 #include <stdint.h>
 #include <stdio.h>
 
+#include "common.cuh"
+
 namespace cp {
 namespace umma {
 
@@ -340,6 +342,25 @@ struct EpiParams {
   int outStride, out_nchw;
   int Cout, CoutPad, H, W;   // Cout/H/W: NCHW addressing; CoutPad: length of the bias vector
 };
+// The epilogue of a convolution launch.  round_out: round the stored outputs to tf32.
+__host__ __device__ __forceinline__ EpiParams epi_params(const IgemmParams& p, bool round_out) {
+  return {p.bias, p.residual, p.resStride, p.relu, p.res_after_relu, round_out, p.out, p.outStride, p.out_nchw,
+          p.Cout, p.CoutPad, p.Hout, p.Wout};
+}
+// The epilogue of a conv_tma / dcn_tma launch, its output geometry taken from the kernel's tile geometry: the epilogue
+// and the tile code then read each value from one parameter word (reading the copies in p.epi as well costs the
+// consumers instructions and registers).  So p.epi.Cout, CoutPad, H and W are not read on these kernels.  They hold the
+// same values: both kernels take only stride-1 convolutions padded by k / 2 (tma_conv_supported, dcn_tma_supported),
+// whose Hout / Wout (epi_params) equal the Hin / Win of the tile geometry.
+template <class Params>
+__device__ __forceinline__ EpiParams tile_epi(const Params& p) {
+  EpiParams e = p.epi;
+  e.Cout = p.Cout;
+  e.CoutPad = p.CoutPad;
+  e.H = p.H;
+  e.W = p.W;
+  return e;
+}
 
 template <int NV>
 __device__ __forceinline__ void epilogue_row(const EpiParams& e, float (&vv)[NV], bool valid, int m, int n, int oy, int ox,
@@ -387,10 +408,20 @@ __device__ __forceinline__ void epilogue_row(const EpiParams& e, float (&vv)[NV]
   }
 }
 
+// Split-K, first half (dcn_tma_kernel; conv_tma_kernel writes the same layout itself): the CTA of K segment `split`
+// of an (m, n) tile parks the partial sums v of columns col0 .. col0 + 15 of tile row `row` in the workspace,
+// [mn tile][split][BN / 4][rows] float4 (row-fastest: coalesced).  vtile = mn tile * ksplit + split.
+template <int BN>
+__device__ __forceinline__ void park_partial(float* part, long long vtile, int col0, int row, int rows, const float (&v)[16]) {
+  float4* dst = reinterpret_cast<float4*>(part) + ((size_t)vtile * (BN >> 2) + (col0 >> 2)) * rows + row;
+#pragma unroll
+  for (int q = 0; q < 4; ++q) __stcg(dst + (size_t)q * rows, make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]));
+}
+
 // Split-K, second half (conv_tma_splitk_finish, dcn_tma_splitk_finish): one thread per (tile row i, 4 columns) of an
-// (m, n) tile adds the ksplit partial sums ([mn tile][split][BN / 4][rows] float4, row-fastest: coalesced) in split
-// order and runs the epilogue.  row_at(mn, i, &n, &oy, &ox) maps the row to its output position (false: none).  MULTI
-// (several models in the launch): image n takes the bias of model n / p.ipm.
+// (m, n) tile adds the ksplit partial sums park_partial left in split order and runs the epilogue.  row_at(mn, i, &n,
+// &oy, &ox) maps the row to its output position (false: none).  MULTI (several models in the launch): image n takes the
+// bias of model n / p.ipm.
 template <bool MULTI, class Params, class RowAt>
 __device__ __forceinline__ void splitk_finish(const Params& p, int rows, long long mn_tiles, RowAt row_at) {
   griddep_launch_dependents();
@@ -413,10 +444,29 @@ __device__ __forceinline__ void splitk_finish(const Params& p, int rows, long lo
   int n, oy, ox;
   if (!row_at(mn, i, &n, &oy, &ox)) return;
   const int n_tile = (int)(mn % (p.CoutPad / p.BN));
-  const EpiParams e{MULTI ? p.bias + (size_t)(n / p.ipm) * p.wstride : p.bias, p.residual, p.resStride, p.relu, p.res_after_relu, p.round_tf32, p.out, p.outStride, p.out_nchw,
-                    p.Cout, p.CoutPad, p.H, p.W};
+  EpiParams e = tile_epi(p);
+  if (MULTI) e.bias = p.epi.bias + (size_t)(n / p.ipm) * p.wstride;
   float v[4] = {a.x, a.y, a.z, a.w};
   epilogue_row<4>(e, v, true, (n * p.H + oy) * p.W + ox, n, oy, ox, n_tile * p.BN + c4 * 4, min(p.Cout, (n_tile + 1) * p.BN));
+}
+
+// The host side of a conv_tma / dcn_tma launch after its main kernel: reports the launch and, where it split K over
+// CTAs, adds the parked partial sums with `finish` (the launch's splitk_finish instance).
+template <class Params>
+int splitk_tail(const KSplit& ks, const Params& q, int rows, long long mn_tiles, void (*finish)(Params, long long),
+                cudaStream_t s, LaunchInfo* info, const char* who) {
+  if (info) {
+    info->BN = q.BN;
+    info->ksplit = ks.ksplit;
+    info->grid = ks.grid;
+    info->path = ks.ksplit == 1 ? CP_KPATH_ONE : (ks.fold ? CP_KPATH_FOLD : CP_KPATH_SPLIT);
+  }
+  if (ks.ksplit > 1 && !ks.fold) {
+    const long long threads = mn_tiles * (q.BN / 4) * rows;
+    CP_CUDA_CHECK(launch_kernel(finish, dim3((unsigned)((threads + 255) / 256)), dim3(256), 0, s, q, mn_tiles));
+    CP_LAUNCH_CHECK(std::string(who) + "_splitk_finish");
+  }
+  return CP_OK;
 }
 
 // Row-wise drain of a warpgroup's 64 x BN wgmma accumulator: 32 columns at a time go through `stage` (64 x 33 floats of
