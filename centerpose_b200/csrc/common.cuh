@@ -1,5 +1,6 @@
 // Shared declarations for libcenterpose_b200.so (sm_90a only).
 #pragma once
+#include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -227,7 +228,7 @@ int tma_cslab(const IgemmParams& p, int x3);     // channels per activation slab
 int launch_pack_tma_weight(const float* src_k_by_ld, int ld, int Cin, int taps, int Cout, int CoutPad, int x3, int cslab,
                            int bn, void* dst, cudaStream_t s);
 int tma_encode_nhwc_box(const float* base, int C, int W, int H, int B, int strideFloats, int boxC, int boxW, int boxH,
-                        int swizzle64, void* map_out /* 128 bytes, 64-byte aligned */);
+                        CUtensorMapSwizzle swizzle, void* map_out /* 128 bytes, 64-byte aligned */);
 int tma_conv_encode(const IgemmParams& p, int Bmax, int cslab, void* maps_out /* 4 x 128 bytes */);
 int launch_conv_tma(const IgemmParams& p, const void* maps, const ConvKernel& k, cudaStream_t stream, LaunchInfo* info);
 long long conv_tma_image_tiles(const IgemmParams& p, int BN);     // (m, n) tiles of one image of one model

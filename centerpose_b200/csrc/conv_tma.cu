@@ -70,7 +70,7 @@ struct TmaConvParams {
   // of them over its ipm images) so that no tile mixes two models' weights.
   int ipm;
   long long wstride, tstride, tiles_per_model;
-  int RS;             // x3 fused 1x1: slots of the hidden ring (1 or 2)
+  int RS;             // x3 fused 1x1: slots of the hidden ring (1 or 2: a power of two, Ring::at)
 };
 
 struct TmaCtl {
@@ -175,7 +175,12 @@ __global__ void __launch_bounds__(X3 ? (FUSE ? TM_THREADS_X3F : TM_THREADS_X3) :
   const long long tph = FUSE ? p.tph : 1;
   auto tile_at = [&](long long it) { return ((long long)blockIdx.x + (it / tph) * gridDim.x) * tph + (it % tph); };
 
+  // The rings (each role walks its own copy): slabs, weight tiles, x3 fused: the hidden chunks (one definition for both
+  // sides).  x3: the splitters hand each slab stage on through a_split, 128 arrivals.
+  const Ring h{ctl->h_full, ctl->h_empty, p.RS};
   if (tid == 0) {
+    // Written out, not through ring_init: with it the MULTI BN = 32 instances change register allocation (98 registers
+    // in tf32, 12/16 B of spill in x3 fused).
     for (int s = 0; s < p.SA; ++s) {
       mbar_init(smem_u32(&ctl->a_full[s]), 1);
       mbar_init(smem_u32(&ctl->a_empty[s]), 2);     // one arrival per consumer warpgroup
@@ -207,8 +212,7 @@ __global__ void __launch_bounds__(X3 ? (FUSE ? TM_THREADS_X3F : TM_THREADS_X3) :
     if (warp == 0) {
       // ===================== activation slabs via TMA =====================
       if (lane == 0) {
-        int stage = 0;
-        uint32_t phase = 0;
+        Ring a{ctl->a_full, ctl->a_empty, p.SA};
         for (long long it = 0, tile = tile_at(0); tile < total_tiles; tile = tile_at(++it)) {
           const TileGeo g = decode_tile<MULTI>(p, tile / KS_SPLIT, n_tiles);
           const int s_begin = (int)(tile % KS_SPLIT) * sps;
@@ -218,18 +222,14 @@ __global__ void __launch_bounds__(X3 ? (FUSE ? TM_THREADS_X3F : TM_THREADS_X3) :
               cb += p.srcC[src];
               ++src;
             }
-            mbar_wait(smem_u32(&ctl->a_empty[stage]), phase ^ 1u);
-            const uint32_t bar = smem_u32(&ctl->a_full[stage]);
-            mbar_arrive_expect_tx(bar, p.slab_bytes);
-            const uint32_t dst = slabs0 + (uint32_t)stage * a_stage;
+            a.wait_empty();
+            a.arrive_full_tx(p.slab_bytes);
+            const uint32_t dst = slabs0 + (uint32_t)a.stage * a_stage;
             if (p.k == 3)
-              tma_load_4d(dst, &p.amap[src], s * p.cslab - cb, -1, g.r_lo - 1, g.img, bar);
+              tma_load_4d(dst, &p.amap[src], s * p.cslab - cb, -1, g.r_lo - 1, g.img, a.full_bar());
             else
-              tma_load_2d(dst, &p.amap[src], s * p.cslab - cb, (int)g.pos0, bar);
-            if (++stage == p.SA) {
-              stage = 0;
-              phase ^= 1u;
-            }
+              tma_load_2d(dst, &p.amap[src], s * p.cslab - cb, (int)g.pos0, a.full_bar());
+            a.advance();
           }
         }
       }
@@ -237,8 +237,7 @@ __global__ void __launch_bounds__(X3 ? (FUSE ? TM_THREADS_X3F : TM_THREADS_X3) :
     } else if (warp == 1) {
       // ===================== weight tiles =====================
       if (lane == 0) {
-        int stage = 0;
-        uint32_t phase = 0;
+        Ring b{ctl->b_full, ctl->b_empty, p.SB};
         for (long long it = 0, tile = tile_at(0); tile < total_tiles; tile = tile_at(++it)) {
           const unsigned char* wsrc;
           if constexpr (MULTI) {
@@ -249,16 +248,7 @@ __global__ void __launch_bounds__(X3 ? (FUSE ? TM_THREADS_X3F : TM_THREADS_X3) :
             const int n_tile = (int)((tile / KS_SPLIT) % n_tiles);
             wsrc = p.wtiles + ((size_t)n_tile * KB_all + (size_t)(tile % KS_SPLIT) * KB) * btile_bytes;
           }
-          for (int kb = 0; kb < KB; ++kb) {
-            mbar_wait(smem_u32(&ctl->b_empty[stage]), phase ^ 1u);
-            const uint32_t bar = smem_u32(&ctl->b_full[stage]);
-            mbar_arrive_expect_tx(bar, btile_bytes);
-            bulk_g2s(btiles0 + (uint32_t)stage * btile_bytes, wsrc + (size_t)kb * btile_bytes, btile_bytes, bar);
-            if (++stage == p.SB) {
-              stage = 0;
-              phase ^= 1u;
-            }
-          }
+          produce_weight_tiles(b, btiles0, btile_bytes, wsrc, KB);
         }
       }
       __syncwarp();
@@ -273,7 +263,6 @@ __global__ void __launch_bounds__(X3 ? (FUSE ? TM_THREADS_X3F : TM_THREADS_X3) :
     // the hidden ring, then the staged 1x1 weights, take the place of the consumers' staging buffers
     const float* hring = reinterpret_cast<const float*>(smem + (drain0 - smem_u32(smem)));
     float4* w1 = reinterpret_cast<float4*>(smem + (drain0 - smem_u32(smem)) + (size_t)p.RS * TM_HSLOT_BYTES);
-    const uint32_t bar_h_full = smem_u32(&ctl->h_full[0]), bar_h_empty = smem_u32(&ctl->h_empty[0]);
     auto at = [&](int r, int col) { return r * 32 + ((((col >> 2) ^ r) & 7) << 2) + (col & 3); };
     // the tile's 1x1 weights as float4 (hidden k, outputs 4 q .. 4 q + 3) at (4 k + q) ^ (k & 16 ? 4 : 0): rows k and
     // k ^ 1 trade places in the upper half of every 32, so the two hidden halves of a warp read different banks
@@ -284,8 +273,7 @@ __global__ void __launch_bounds__(X3 ? (FUSE ? TM_THREADS_X3F : TM_THREADS_X3) :
                           (size_t)part * BN * 4;
       for (int i = wt; i < BN * 4; i += 128) w1[i ^ (((i >> 2) & 16) ? 4 : 0)] = __ldg(src + i);
     };
-    int rs = 0;
-    uint32_t rp = 0;
+    Ring hr = h;
     float acc2[32];
     long long it = 0, tile = tile_at(0);
     if (tile < total_tiles) stage_w1(tile);
@@ -299,8 +287,8 @@ __global__ void __launch_bounds__(X3 ? (FUSE ? TM_THREADS_X3F : TM_THREADS_X3) :
       }
 #pragma unroll 1
       for (int c0 = 0; c0 < BN; c0 += 32) {
-        mbar_wait(bar_h_full + 8u * (uint32_t)rs, rp);
-        const float* hs = hring + (size_t)rs * (TM_HSLOT_BYTES / 4);
+        hr.wait_full();
+        const float* hs = hring + (size_t)hr.stage * (TM_HSLOT_BYTES / 4);
 #pragma unroll
         for (int m4 = 0; m4 < 4; ++m4) {
           const int k0 = 16 * hh + 4 * m4;          // hidden channels c0 + k0 .. + 3
@@ -325,11 +313,8 @@ __global__ void __launch_bounds__(X3 ? (FUSE ? TM_THREADS_X3F : TM_THREADS_X3) :
             }
           }
         }
-        mbar_arrive(bar_h_empty + 8u * (uint32_t)rs);
-        if (++rs == p.RS) {
-          rs = 0;
-          rp ^= 1u;
-        }
+        hr.arrive_empty();
+        hr.advance();
       }
       if (part == p.tph - 1) {
         // the two hidden halves of a (row, output) are in lanes that differ in bit 1
@@ -362,13 +347,12 @@ __global__ void __launch_bounds__(X3 ? (FUSE ? TM_THREADS_X3F : TM_THREADS_X3) :
     asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(REG_SPLIT));
     // ===================== hi / lo splitters (x3): slab -> tf32-exact hi (in place) + lo slab =====================
     const int st = tid - 384;
-    int stage = 0;
-    uint32_t phase = 0;
+    Ring split{ctl->a_full, ctl->a_split, p.SA};     // the splitters take a full slab stage and release it into a_split
     const uint32_t nchunk = p.slab_bytes >> 4;
     for (long long it = 0, tile = tile_at(0); tile < total_tiles; tile = tile_at(++it)) {
       for (int s = 0; s < sps; ++s) {
-        mbar_wait(smem_u32(&ctl->a_full[stage]), phase);
-        const uint32_t hi = slabs0 + (uint32_t)stage * a_stage;
+        split.wait_full();
+        const uint32_t hi = slabs0 + (uint32_t)split.stage * a_stage;
         const uint32_t lo = hi + p.slab_stride;
         for (uint32_t c0 = st; c0 < nchunk; c0 += 128 * 4) {
           float4 v[4];
@@ -389,11 +373,8 @@ __global__ void __launch_bounds__(X3 ? (FUSE ? TM_THREADS_X3F : TM_THREADS_X3) :
           }
         }
         fence_proxy_async_smem();
-        mbar_arrive(smem_u32(&ctl->a_split[stage]));
-        if (++stage == p.SA) {
-          stage = 0;
-          phase ^= 1u;
-        }
+        split.arrive_empty();
+        split.advance();
       }
     }
   } else {
@@ -401,13 +382,10 @@ __global__ void __launch_bounds__(X3 ? (FUSE ? TM_THREADS_X3F : TM_THREADS_X3) :
     // ===================== consumers: warpgroup c multiplies rows [64 c, 64 c + 64) of every tile =====================
     const int c = (warp - 4) >> 2, wt = tid & 127;
     float* dstage = reinterpret_cast<float*>(smem + (drain0 - smem_u32(smem))) + (size_t)c * (DRAIN_STAGE_BYTES / 4);
-    const uint32_t bar_a = smem_u32(X3 ? &ctl->a_split[0] : &ctl->a_full[0]);
-    const uint32_t bar_a_empty = smem_u32(&ctl->a_empty[0]);
-    const uint32_t bar_b_full = smem_u32(&ctl->b_full[0]), bar_b_empty = smem_u32(&ctl->b_empty[0]);
+    // x3: a slab stage is full once the splitters are done with it
+    Ring a{X3 ? ctl->a_split : ctl->a_full, ctl->a_empty, p.SA}, b{ctl->b_full, ctl->b_empty, p.SB};
     const uint32_t a_lo_u = p.slab_stride >> 4, b_lo_u = ((uint32_t)BN * rowb) >> 4;
     EpiParams ep = tile_epi(p);
-    int sa = 0, sb = 0;
-    uint32_t pa = 0, pb = 0;
     float acc[BN / 2];
     float sums[X3 ? BN / 2 : 1];
     float tot[FOLD ? BN / 2 : 1];        // fold: the running total of the finished K segments
@@ -433,11 +411,11 @@ __global__ void __launch_bounds__(X3 ? (FUSE ? TM_THREADS_X3F : TM_THREADS_X3) :
       const int group = X3 ? p.group : 1;
       const bool overlap = X3 && p.SA > 1;
       int tap = 0;
-      // retire the K block before position (sb, sa, tap): its weight stage, and its slab stage when it was a slab's last tap
+      // retire the K block before position (b, a, tap): its weight stage, and its slab stage when it was a slab's last tap
       auto release_prev = [&]() {
         if (wt == 0) {
-          mbar_arrive(bar_b_empty + 8u * (uint32_t)(sb == 0 ? p.SB - 1 : sb - 1));
-          if (tap == 0) mbar_arrive(bar_a_empty + 8u * (uint32_t)(sa == 0 ? p.SA - 1 : sa - 1));
+          b.arrive_empty(b.prev());
+          if (tap == 0) a.arrive_empty(a.prev());
         }
       };
       const int KB_seg = FOLD ? p.sps * taps : KB;       // K blocks of one segment
@@ -445,12 +423,12 @@ __global__ void __launch_bounds__(X3 ? (FUSE ? TM_THREADS_X3F : TM_THREADS_X3) :
         for (int kb0 = 0; kb0 < KB_seg; kb0 += group) {
           const int n_kb = min(group, KB_seg - kb0);
           for (int i = 0; i < n_kb; ++i) {
-            if (tap == 0) mbar_wait(bar_a + 8u * (uint32_t)sa, pa);
+            if (tap == 0) a.wait_full();
             const int ky = tap / 3, kx = tap - ky * 3;
             const uint32_t arow = row0 + (p.k == 3 ? (uint32_t)(ky * p.Wt + kx) : 0u);
-            mbar_wait(bar_b_full + 8u * (uint32_t)sb, pb);
-            const uint64_t da = make_desc(slabs0 + (uint32_t)sa * a_stage + arow * rowb, p.cslab);
-            const uint64_t db = make_desc(btiles0 + (uint32_t)sb * btile_bytes, p.cslab);
+            b.wait_full();
+            const uint64_t da = make_desc(slabs0 + (uint32_t)a.stage * a_stage + arow * rowb, p.cslab);
+            const uint64_t db = make_desc(btiles0 + (uint32_t)b.stage * btile_bytes, p.cslab);
             const bool fresh = X3 ? i == 0 : kb0 == 0;
             if (p.cslab == 32)
               mma_kblock_issue<BN, X3, false, 4>(acc, da, db, a_lo_u, b_lo_u, fresh);
@@ -460,16 +438,10 @@ __global__ void __launch_bounds__(X3 ? (FUSE ? TM_THREADS_X3F : TM_THREADS_X3) :
               wg_wait<1>();
               release_prev();
             }
-            if (++sb == p.SB) {
-              sb = 0;
-              pb ^= 1u;
-            }
+            b.advance();
             if (++tap == taps) {
               tap = 0;
-              if (++sa == p.SA) {
-                sa = 0;
-                pa ^= 1u;
-              }
+              a.advance();
             }
             if (!overlap) {
               wg_wait<0>();
@@ -505,14 +477,12 @@ __global__ void __launch_bounds__(X3 ? (FUSE ? TM_THREADS_X3F : TM_THREADS_X3) :
         const int fr0 = (wt >> 5) * 16 + ((wt & 31) >> 2), fcq = (wt & 3) * 2;     // accumulator fragment (drain_rows)
         const float* b1 = p.epi.bias + (MULTI ? (size_t)g.model * p.wstride : 0) + (size_t)g.n_tile * BN;
         float* hring = reinterpret_cast<float*>(smem + (drain0 - smem_u32(smem)));        // hidden ring
-        const uint32_t bar_h_full = smem_u32(&ctl->h_full[0]), bar_h_empty = smem_u32(&ctl->h_empty[0]);
         auto at = [&](int r, int col) { return r * 32 + ((((col >> 2) ^ r) & 7) << 2) + (col & 3); };
 #pragma unroll
         for (int c0 = 0; c0 < BN; c0 += 32) {
-          const uint32_t chunk = (uint32_t)it * (BN / 32) + c0 / 32;       // chunks so far: ring slot and phase
-          const uint32_t rs = chunk % p.RS, rp = (chunk / p.RS) & 1u;
-          mbar_wait(bar_h_empty + 8u * rs, rp ^ 1u);
-          float* hs = hring + (size_t)rs * (TM_HSLOT_BYTES / 4) + c * 64 * 32;
+          const Ring hc = h.at((uint32_t)it * (BN / 32) + c0 / 32);       // chunks so far: ring slot and phase
+          hc.wait_empty();
+          float* hs = hring + (size_t)hc.stage * (TM_HSLOT_BYTES / 4) + c * 64 * 32;
 #pragma unroll
           for (int j = 0; j < BN / 8; ++j) {
             if (j * 8 >= c0 && j * 8 < c0 + 32) {
@@ -524,7 +494,7 @@ __global__ void __launch_bounds__(X3 ? (FUSE ? TM_THREADS_X3F : TM_THREADS_X3) :
               hs[at(fr0 + 8, col + 1)] = fmaxf(sums[X3 ? 4 * j + 3 : 0] + by, 0.f);
             }
           }
-          mbar_arrive(bar_h_full + 8u * rs);
+          hc.arrive_full();
         }
         continue;
       }
@@ -758,9 +728,9 @@ int launch_pack_tma_weight(const float* src, int ld, int Cin, int taps, int Cout
   return CP_OK;
 }
 
-// One 4-D fp32 NHWC tensor map {C, W, H, B} with box {boxC, boxW, boxH, 1}, un-swizzled or SWIZZLE_64B (dcn_tma.cu slabs).
+// One 4-D fp32 NHWC tensor map {C, W, H, B} with box {boxC, boxW, boxH, 1} (conv_tma 3x3 and dcn_tma slabs).
 int tma_encode_nhwc_box(const float* base, int C, int W, int H, int B, int strideFloats, int boxC, int boxW, int boxH,
-                        int swizzle64, void* map_out) {
+                        CUtensorMapSwizzle swizzle, void* map_out) {
   EncodeTiledFn enc = get_encode();
   if (!enc) return fail(CP_ERR_CUDA, "cuTensorMapEncodeTiled entry point not available");
   cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
@@ -768,8 +738,7 @@ int tma_encode_nhwc_box(const float* base, int C, int W, int H, int B, int strid
   cuuint32_t box[4] = {(cuuint32_t)boxC, (cuuint32_t)boxW, (cuuint32_t)boxH, 1};
   cuuint32_t es[4] = {1, 1, 1, 1};
   CUresult r = enc(reinterpret_cast<CUtensorMap*>(map_out), CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void*)base, dims, strides, box,
-                   es, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_NONE,
-                   CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                   es, CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                    CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) return fail(CP_ERR_CUDA, "cuTensorMapEncodeTiled failed with code " + std::to_string((int)r));
   return CP_OK;
@@ -784,25 +753,17 @@ int tma_conv_encode(const IgemmParams& p, int Bmax, int cs, void* maps_out) {
   const int boxh = tma_boxh(Wt);
   const CUtensorMapSwizzle swz = cs == 32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B;
   for (int s = 0; s < p.nsrc; ++s) {
-    CUresult r;
     if (p.kh == 3) {
-      cuuint64_t dims[4] = {(cuuint64_t)p.srcC[s], (cuuint64_t)p.Win, (cuuint64_t)p.Hin, (cuuint64_t)Bmax};
-      cuuint64_t strides[3] = {(cuuint64_t)p.srcStride[s] * 4, (cuuint64_t)p.Win * p.srcStride[s] * 4,
-                               (cuuint64_t)p.Hin * p.Win * p.srcStride[s] * 4};
-      cuuint32_t box[4] = {(cuuint32_t)cs, (cuuint32_t)Wt, (cuuint32_t)boxh, 1};
-      cuuint32_t es[4] = {1, 1, 1, 1};
-      r = enc(&maps[s], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, (void*)p.src[s], dims, strides, box, es,
-              CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    } else {
-      cuuint64_t dims[2] = {(cuuint64_t)p.srcC[s], (cuuint64_t)Bmax * p.Hin * p.Win};
-      cuuint64_t strides[1] = {(cuuint64_t)p.srcStride[s] * 4};
-      cuuint32_t box[2] = {(cuuint32_t)cs, (cuuint32_t)TM_BM};
-      cuuint32_t es[2] = {1, 1};
-      r = enc(&maps[s], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)p.src[s], dims, strides, box, es,
-              CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+      if (int rc = tma_encode_nhwc_box(p.src[s], p.srcC[s], p.Win, p.Hin, Bmax, p.srcStride[s], cs, Wt, boxh, swz, &maps[s]))
+        return rc;
+      continue;
     }
+    cuuint64_t dims[2] = {(cuuint64_t)p.srcC[s], (cuuint64_t)Bmax * p.Hin * p.Win};
+    cuuint64_t strides[1] = {(cuuint64_t)p.srcStride[s] * 4};
+    cuuint32_t box[2] = {(cuuint32_t)cs, (cuuint32_t)TM_BM};
+    cuuint32_t es[2] = {1, 1};
+    CUresult r = enc(&maps[s], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, (void*)p.src[s], dims, strides, box, es,
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, swz, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return fail(CP_ERR_CUDA, "cuTensorMapEncodeTiled failed with code " + std::to_string((int)r));
   }
   return CP_OK;

@@ -141,23 +141,16 @@ __global__ void __launch_bounds__(DT_THREADS, 1) dcn_tma_kernel(const __grid_con
   const int KB_all = (p.Cin / DT_CS) * 9;
   const int KS_SPLIT = FOLD ? 1 : p.ksplit;
   const long long total_tiles = p.total_tiles;
-  const uint32_t ah_log = (uint32_t)(31 - __clz(p.AH));      // K block n uses A stage n % AH, in round n / AH
+  // The A ring is indexed by the K-block count: K block n uses A stage n % AH, in round n / AH.  It stays written out
+  // (not Ring::at): through the ring type, the tf32 BN = 128 FOLD instance spills 16 B.
+  const uint32_t ah_log = (uint32_t)(31 - __clz(p.AH));
 
+  // The rings (each role walks its own copy): slabs, sampling records, A tiles, weight tiles
   if (tid == 0) {
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(smem_u32(&ctl->s_full[s]), 1);
-      mbar_init(smem_u32(&ctl->s_empty[s]), 4);             // one arrival per gather warp
-      mbar_init(smem_u32(&ctl->c_full[s]), 2);              // one arrival per record warp (2, 3)
-      mbar_init(smem_u32(&ctl->c_empty[s]), 4);
-    }
-    for (int s = 0; s < p.AH; ++s) {
-      mbar_init(smem_u32(&ctl->a_full[s]), 4);              // written by the four gather warps
-      mbar_init(smem_u32(&ctl->a_empty[s]), 8);             // released by every consumer warp
-    }
-    for (int s = 0; s < p.SB; ++s) {
-      mbar_init(smem_u32(&ctl->b_full[s]), 1);
-      mbar_init(smem_u32(&ctl->b_empty[s]), 2);
-    }
+    ring_init({ctl->s_full, ctl->s_empty, 2}, 1, 4);     // empty: one arrival per gather warp
+    ring_init({ctl->c_full, ctl->c_empty, 2}, 2, 4);     // full: one arrival per record warp (2, 3)
+    ring_init({ctl->a_full, ctl->a_empty, p.AH}, 4, 8);  // full: the four gather warps; empty: every consumer warp
+    ring_init({ctl->b_full, ctl->b_empty, p.SB}, 1, 2);
     fence_mbar_init();
   }
   __syncthreads();
@@ -171,8 +164,7 @@ __global__ void __launch_bounds__(DT_THREADS, 1) dcn_tma_kernel(const __grid_con
     if (warp == 0) {
       // ===================== slabs via TMA =====================
       if (lane == 0) {
-        int stage = 0;
-        uint32_t phase = 0;
+        Ring slabs{ctl->s_full, ctl->s_empty, 2};
         for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
           const long long m_tile = (tile / KS_SPLIT) / n_tiles;
           const int s0 = (int)(tile % KS_SPLIT) * nslab;
@@ -180,15 +172,11 @@ __global__ void __launch_bounds__(DT_THREADS, 1) dcn_tma_kernel(const __grid_con
           const int pt = (int)(m_tile - (long long)img * p.tiles_per_image);
           const int y0 = (pt / p.tiles_x) * DT_PH, x0 = (pt % p.tiles_x) * DT_PW;
           for (int s = 0; s < nslab; ++s) {
-            mbar_wait(smem_u32(&ctl->s_empty[stage]), phase ^ 1u);
-            const uint32_t bar = smem_u32(&ctl->s_full[stage]);
-            mbar_arrive_expect_tx(bar, DT_SLAB_BYTES);
-            tma_load_4d(slabs0 + (uint32_t)stage * DT_SLAB_BYTES, &p.amap, (s0 + s) * DT_CS, x0 - DT_HALO, y0 - DT_HALO, img,
-                        bar);
-            if (++stage == 2) {
-              stage = 0;
-              phase ^= 1u;
-            }
+            slabs.wait_empty();
+            slabs.arrive_full_tx(DT_SLAB_BYTES);
+            tma_load_4d(slabs0 + (uint32_t)slabs.stage * DT_SLAB_BYTES, &p.amap, (s0 + s) * DT_CS, x0 - DT_HALO, y0 - DT_HALO,
+                        img, slabs.full_bar());
+            slabs.advance();
           }
         }
       }
@@ -197,47 +185,33 @@ __global__ void __launch_bounds__(DT_THREADS, 1) dcn_tma_kernel(const __grid_con
       // ===================== sampling records: thread t writes positions t and t + 64 of every tile into the record
       // buffer the gather freed last (double-buffered), while the gather and the consumers work on the tile before
       const int rt = tid - 64;
-      int cb = 0;
-      uint32_t pc = 0;
+      Ring recs{ctl->c_full, ctl->c_empty, 2};
       for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         const long long m_tile = (tile / KS_SPLIT) / n_tiles;
         const int img = (int)(m_tile / p.tiles_per_image);
         const int pt = (int)(m_tile - (long long)img * p.tiles_per_image);
         const int y0 = (pt / p.tiles_x) * DT_PH, x0 = (pt % p.tiles_x) * DT_PW;
-        mbar_wait(smem_u32(&ctl->c_empty[cb]), pc ^ 1u);
+        recs.wait_empty();
 #pragma unroll 1
         for (int i = rt; i < DT_BM; i += 64) {
           const int oy = y0 + (i >> 4), ox = x0 + (i & 15);
           coef_row(p, p.offmask + ((size_t)((size_t)img * p.H + oy) * p.W + ox) * p.omStride, oy, ox, y0 - DT_HALO,
-                   x0 - DT_HALO, coef0 + (uint32_t)cb * DT_COEF_BYTES + (uint32_t)i * 144u);
+                   x0 - DT_HALO, coef0 + (uint32_t)recs.stage * DT_COEF_BYTES + (uint32_t)i * 144u);
         }
         __syncwarp();
-        if (lane == 0) mbar_arrive(smem_u32(&ctl->c_full[cb]));
-        if (++cb == 2) {
-          cb = 0;
-          pc ^= 1u;
-        }
+        if (lane == 0) recs.arrive_full();
+        recs.advance();
       }
     } else if (warp == 1) {
       // ===================== weight tiles =====================
       if (lane == 0) {
-        int stage = 0;
-        uint32_t phase = 0;
+        Ring b{ctl->b_full, ctl->b_empty, p.SB};
         for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
           const int n_tile = (int)((tile / KS_SPLIT) % n_tiles);
           const int model = MULTI ? (int)((tile / KS_SPLIT) / n_tiles / p.tiles_per_image) / p.ipm : 0;
           const unsigned char* wsrc = p.wtiles + (size_t)model * p.tstride +
                                       ((size_t)n_tile * KB_all + (size_t)(tile % KS_SPLIT) * KB) * btile_bytes;
-          for (int kb = 0; kb < KB; ++kb) {
-            mbar_wait(smem_u32(&ctl->b_empty[stage]), phase ^ 1u);
-            const uint32_t bar = smem_u32(&ctl->b_full[stage]);
-            mbar_arrive_expect_tx(bar, btile_bytes);
-            bulk_g2s(btiles0 + (uint32_t)stage * btile_bytes, wsrc + (size_t)kb * btile_bytes, btile_bytes, bar);
-            if (++stage == p.SB) {
-              stage = 0;
-              phase ^= 1u;
-            }
-          }
+          produce_weight_tiles(b, btiles0, btile_bytes, wsrc, KB);
         }
       }
       __syncwarp();
@@ -251,15 +225,14 @@ __global__ void __launch_bounds__(DT_THREADS, 1) dcn_tma_kernel(const __grid_con
     const int row = gt & 127;
     const uint32_t a_row = atiles0 + (uint32_t)(row >> 3) * 512u + (uint32_t)(row & 7) * 64u;
     const uint32_t asw = (uint32_t)(row >> 1) & 3u;
-    int ss = 0, cb = 0;
-    uint32_t ps = 0, pc = 0;
+    Ring slabs{ctl->s_full, ctl->s_empty, 2}, recs{ctl->c_full, ctl->c_empty, 2};
     uint32_t cnt = 0;                      // K blocks produced
     for (long long tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
       const long long m_tile = (tile / KS_SPLIT) / n_tiles;
       const int s0 = (int)(tile % KS_SPLIT) * nslab;
       const int img = (int)(m_tile / p.tiles_per_image);
-      mbar_wait(smem_u32(&ctl->c_full[cb]), pc);
-      const uint32_t crow = coef0 + (uint32_t)cb * DT_COEF_BYTES + (uint32_t)row * 144u;
+      recs.wait_full();
+      const uint32_t crow = coef0 + (uint32_t)recs.stage * DT_COEF_BYTES + (uint32_t)row * 144u;
       const float* gimg = p.src + (size_t)img * p.H * p.W * p.srcStride;
       int cur = -1;
       uint32_t slab = 0;
@@ -269,14 +242,11 @@ __global__ void __launch_bounds__(DT_THREADS, 1) dcn_tma_kernel(const __grid_con
         if (s != cur) {
           if (cur >= 0) {                     // done with the previous slab
             __syncwarp();
-            if (lane == 0) mbar_arrive(smem_u32(&ctl->s_empty[ss]));
-            if (++ss == 2) {
-              ss = 0;
-              ps ^= 1u;
-            }
+            if (lane == 0) slabs.arrive_empty();
+            slabs.advance();
           }
-          mbar_wait(smem_u32(&ctl->s_full[ss]), ps);
-          slab = slabs0 + (uint32_t)ss * DT_SLAB_BYTES;
+          slabs.wait_full();
+          slab = slabs0 + (uint32_t)slabs.stage * DT_SLAB_BYTES;
           cur = s;
         }
         const float4 rec = rec_next;
@@ -359,17 +329,11 @@ __global__ void __launch_bounds__(DT_THREADS, 1) dcn_tma_kernel(const __grid_con
       }
       __syncwarp();
       if (lane == 0) {
-        mbar_arrive(smem_u32(&ctl->s_empty[ss]));       // last slab of the tile
-        mbar_arrive(smem_u32(&ctl->c_empty[cb]));
+        slabs.arrive_empty();       // last slab of the tile
+        recs.arrive_empty();
       }
-      if (++ss == 2) {
-        ss = 0;
-        ps ^= 1u;
-      }
-      if (++cb == 2) {
-        cb = 0;
-        pc ^= 1u;
-      }
+      slabs.advance();
+      recs.advance();
     }
   } else {
     // ===================== consumers: warpgroup c multiplies rows [64 c, 64 c + 64) of every tile =====================
@@ -377,11 +341,10 @@ __global__ void __launch_bounds__(DT_THREADS, 1) dcn_tma_kernel(const __grid_con
     const int c = warp >= 12 ? 1 : 0, wt = tid & 127;
     float* dstage = reinterpret_cast<float*>(smem + (drain0 - sbase)) + (size_t)c * (DRAIN_STAGE_BYTES / 4);
     EpiParams ep = tile_epi(p);
-    const uint32_t bar_a_full = smem_u32(&ctl->a_full[0]), bar_a_empty = smem_u32(&ctl->a_empty[0]);
-    const uint32_t bar_b_full = smem_u32(&ctl->b_full[0]), bar_b_empty = smem_u32(&ctl->b_empty[0]);
     const uint32_t b_lo = ((uint32_t)BN * 64u) >> 4;
-    int sb = 0;
-    uint32_t pb = 0, cnt = 0;
+    const uint32_t bar_a_full = smem_u32(&ctl->a_full[0]), bar_a_empty = smem_u32(&ctl->a_empty[0]);
+    Ring b{ctl->b_full, ctl->b_empty, p.SB};
+    uint32_t cnt = 0;
     // K block n's A stage: this warpgroup's half once it is written; each warp releases it on its own
     auto a_wait = [&](uint32_t n) {
       const uint32_t sa = n & (uint32_t)(p.AH - 1);
@@ -394,16 +357,13 @@ __global__ void __launch_bounds__(DT_THREADS, 1) dcn_tma_kernel(const __grid_con
     };
     // the next weight stage: waits for it, returns its descriptor and its index (for the release)
     auto b_wait = [&](int& st) {
-      mbar_wait(bar_b_full + 8u * (uint32_t)sb, pb);
-      st = sb;
-      if (++sb == p.SB) {
-        sb = 0;
-        pb ^= 1u;
-      }
+      b.wait_full();
+      st = b.stage;
+      b.advance();
       return make_desc(btiles0 + (uint32_t)st * btile_bytes, DT_CS);
     };
     auto b_release = [&](int st) {
-      if (wt == 0) mbar_arrive(bar_b_empty + 8u * (uint32_t)st);
+      if (wt == 0) b.arrive_empty(st);
     };
     float acc[BN / 2];
     float sums[X3 ? BN / 2 : 1];
@@ -547,7 +507,8 @@ long long dcn_tma_image_tiles(const IgemmParams& p, int BN) {
 }
 
 int dcn_tma_encode(const IgemmParams& p, int Bmax, void* map_out) {
-  return tma_encode_nhwc_box(p.src[0], p.srcC[0], p.Win, p.Hin, Bmax, p.srcStride[0], DT_CS, DT_SW, DT_SH, 1, map_out);
+  return tma_encode_nhwc_box(p.src[0], p.srcC[0], p.Win, p.Hin, Bmax, p.srcStride[0], DT_CS, DT_SW, DT_SH,
+                             CU_TENSOR_MAP_SWIZZLE_64B, map_out);
 }
 
 // The instance of one launch (null fn: no such N tile).  FOLD: the K segments folded in one CTA per tile.

@@ -79,11 +79,11 @@ __global__ void __launch_bounds__(UM_THREADS, 1) igemm_umma_kernel(const IgemmPa
   const int K = p.kh * p.kw * p.Cin;
   const int KB = (K + T::kElems - 1) / T::kElems;
 
+  // one ring of (A tile, weight tile) stages; full: every gather thread + the weight copy's expect_tx arrival, empty:
+  // one arrival per consumer warpgroup
+  Ring ring{ctl->full, ctl->empty, STAGES};
   if (tid == 0) {
-    for (int s = 0; s < STAGES; ++s) {
-      mbar_init(smem_u32(&ctl->full[s]), UM_PROD_WARPS * 32 + 1);      // + the weight copy's expect_tx arrival
-      mbar_init(smem_u32(&ctl->empty[s]), 2);                          // one arrival per consumer warpgroup
-    }
+    ring_init(ring, UM_PROD_WARPS * 32 + 1, 2);
     fence_mbar_init();
   }
   __syncthreads();
@@ -114,8 +114,6 @@ __global__ void __launch_bounds__(UM_THREADS, 1) igemm_umma_kernel(const IgemmPa
       int cur_tap = -1;
       constexpr int F4 = T::kChunkCh / 4;     // float4 loads per chunk (2 for bf16, 1 for tf32)
 
-      int stage = 0;
-      uint32_t phase = 0;
       for (int kb = 0; kb < KB; ++kb) {
         // ---- issue every global load of this thread's 4 chunks first (memory-level parallelism) ...
         float4 ld[4][MODE == IGEMM_DCN ? 4 * F4 : F4];
@@ -189,13 +187,13 @@ __global__ void __launch_bounds__(UM_THREADS, 1) igemm_umma_kernel(const IgemmPa
           }
         }
         // ---- ... then wait for the stage, convert and store into the swizzled K-major tile
-        mbar_wait(smem_u32(&ctl->empty[stage]), phase ^ 1u);
+        ring.wait_empty();
         if (tid == 0) {
-          const uint32_t bar = smem_u32(&ctl->full[stage]);
-          mbar_arrive_expect_tx(bar, b_tile_bytes);
-          bulk_g2s(tiles0 + (uint32_t)stage * stage_bytes + A_TILE_BYTES, wsrc + (size_t)kb * b_tile_bytes, b_tile_bytes, bar);
+          ring.arrive_full_tx(b_tile_bytes);
+          bulk_g2s(tiles0 + (uint32_t)ring.stage * stage_bytes + A_TILE_BYTES, wsrc + (size_t)kb * b_tile_bytes, b_tile_bytes,
+                   ring.full_bar());
         }
-        const uint32_t a_dst = tiles0 + (uint32_t)stage * stage_bytes + row_off;
+        const uint32_t a_dst = tiles0 + (uint32_t)ring.stage * stage_bytes + row_off;
 #pragma unroll
         for (int qi = 0; qi < 4; ++qi) {
           float v[8];
@@ -232,11 +230,8 @@ __global__ void __launch_bounds__(UM_THREADS, 1) igemm_umma_kernel(const IgemmPa
             st_shared_v4f(a_dst + coff, v[0], v[1], v[2], v[3]);
         }
         fence_proxy_async_smem();
-        mbar_arrive(smem_u32(&ctl->full[stage]));
-        if (++stage == STAGES) {
-          stage = 0;
-          phase ^= 1u;
-        }
+        ring.arrive_full();
+        ring.advance();
       }
     }
 
@@ -250,23 +245,18 @@ __global__ void __launch_bounds__(UM_THREADS, 1) igemm_umma_kernel(const IgemmPa
     for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
 #pragma unroll
     for (int j = 0; j < (X3 ? BN / 2 : 1); ++j) sums[j] = 0.f;
-    int stage = 0;
-    uint32_t phase = 0;
     int gk = 0;                              // tf32x3: K block inside its accumulation group
     for (int kb = 0; kb < KB; ++kb) {
-      mbar_wait(smem_u32(&ctl->full[stage]), phase);
-      const uint32_t a_tile = tiles0 + (uint32_t)stage * stage_bytes + (uint32_t)c * 64u * ROW_BYTES;
-      const uint64_t db = make_desc(tiles0 + (uint32_t)stage * stage_bytes + A_TILE_BYTES, 32);
+      ring.wait_full();
+      const uint32_t a_tile = tiles0 + (uint32_t)ring.stage * stage_bytes + (uint32_t)c * 64u * ROW_BYTES;
+      const uint64_t db = make_desc(tiles0 + (uint32_t)ring.stage * stage_bytes + A_TILE_BYTES, 32);
       // tf32x3: NACC K blocks are chained in the accumulator, then added into round-to-nearest fp32 sums
       if (X3)
         mma_kblock_x3<BN, 4>(acc, a_tile, wt, db, ((uint32_t)BN * ROW_BYTES) >> 4, gk == 0);
       else
         mma_kblock<BN, false, true, 4>(acc, make_desc(a_tile, 32), db, 0, 0, kb == 0);
-      if (wt == 0) mbar_arrive(smem_u32(&ctl->empty[stage]));
-      if (++stage == STAGES) {
-        stage = 0;
-        phase ^= 1u;
-      }
+      if (wt == 0) ring.arrive_empty();
+      ring.advance();
       if (X3) {
         if (gk == NACC - 1 || kb == KB - 1) {
 #pragma unroll

@@ -53,6 +53,54 @@ __device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t
                "l"(src), "r"(bytes), "r"(bar)
                : "memory");
 }
+// A ring of n shared-memory stages between producer and consumer roles, seen through its full and empty mbarriers
+// (one of each per stage); the protocol is DESIGN.md §4, "mbarrier rings".  A role walks the stages in
+// order: `stage` is its current one and `phase` flips at every wrap.  A ring is a view: the x3 consumers of conv_tma
+// see the slab ring through its split barriers.  Rings indexed by a running count k use at(k) (n a power of two).
+struct Ring {
+  unsigned long long *full, *empty;
+  int n;
+  int stage = 0;
+  uint32_t phase = 0;
+
+  __device__ __forceinline__ uint32_t full_bar() const { return smem_u32(full + stage); }
+  __device__ __forceinline__ void wait_full() const { mbar_wait(full_bar(), phase); }
+  __device__ __forceinline__ void wait_empty() const { mbar_wait(smem_u32(empty + stage), phase ^ 1u); }
+  __device__ __forceinline__ void arrive_full() const { mbar_arrive(full_bar()); }
+  __device__ __forceinline__ void arrive_full_tx(uint32_t bytes) const { mbar_arrive_expect_tx(full_bar(), bytes); }
+  __device__ __forceinline__ void arrive_empty(int s) const { mbar_arrive(smem_u32(empty + s)); }
+  __device__ __forceinline__ void arrive_empty() const { arrive_empty(stage); }
+  __device__ __forceinline__ void advance() {
+    if (++stage == n) {
+      stage = 0;
+      phase ^= 1u;
+    }
+  }
+  __device__ __forceinline__ int prev() const { return stage == 0 ? n - 1 : stage - 1; }
+  // slot and parity of the k-th use of a ring of n stages, n a power of two: what stage and phase are after k advances
+  static __device__ __forceinline__ uint32_t slot(uint32_t k, int n) { return k & (uint32_t)(n - 1); }
+  static __device__ __forceinline__ uint32_t parity(uint32_t k, int n) { return (k & (uint32_t)n) ? 1u : 0u; }
+  __device__ __forceinline__ Ring at(uint32_t k) const { return {full, empty, n, (int)slot(k, n), parity(k, n)}; }
+};
+// Initialises a ring's barriers: a stage is full after `full_arrivals` arrivals, empty after `empty_arrivals`.
+__device__ __forceinline__ void ring_init(const Ring& r, uint32_t full_arrivals, uint32_t empty_arrivals) {
+  for (int s = 0; s < r.n; ++s) {
+    mbar_init(smem_u32(r.full + s), full_arrivals);
+    mbar_init(smem_u32(r.empty + s), empty_arrivals);
+  }
+}
+// Streams the KB weight tiles of one output tile, btile_bytes each from `src` on, into the stages of ring b (stage s at
+// tiles0 + s btile_bytes) with cp.async.bulk: the weight-tile producer warp of conv_tma and dcn_tma.
+__device__ __forceinline__ void produce_weight_tiles(Ring& b, uint32_t tiles0, uint32_t btile_bytes, const unsigned char* src,
+                                                     int KB) {
+  for (int kb = 0; kb < KB; ++kb) {
+    b.wait_empty();
+    b.arrive_full_tx(btile_bytes);
+    bulk_g2s(tiles0 + (uint32_t)b.stage * btile_bytes, src + (size_t)kb * btile_bytes, btile_bytes, b.full_bar());
+    b.advance();
+  }
+}
+
 // named barrier of the 128 threads of one warpgroup (ids 1 .. 15; 0 is __syncthreads)
 __device__ __forceinline__ void wg_bar_sync(int id) { asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory"); }
 
