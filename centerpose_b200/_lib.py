@@ -62,13 +62,16 @@ EXPORTS = [
     "cp_preprocess_frame_table_bytes", "cp_preprocess_frame_table", "cp_preprocess_slots_ragged_dev",
     "cp_preprocess_slots_rows_dev", "cp_gather_rows_dev", "cp_tracker_render_dev2", "cp_tracker_step_dev",
     "cp_preprocess_formats", "cp_preprocess_frame_table_formats", "cp_plan_op_ksegments", "cp_plan_ksegments",
+    "cp_preprocess_remap", "cp_preprocess_frame_table_maps",
 ]
 
 # cp_pixel_format; "bgr" is the interleaved uint8 [H,W,3] input of every other pre-process entry point.  The camera
-# formats carry ffmpeg's pix_fmt names; CP_PIX_PER_FRAME launches a frame table of per-frame formats.
+# formats carry ffmpeg's pix_fmt names; CP_PIX_PER_FRAME launches a frame table of per-frame formats, and CP_PIX_REMAP
+# OR-ed into either launches a table with coordinate maps (cp_preprocess_frame_table_maps).
 CP_PIX_NV12, CP_PIX_I420, CP_PIX_BGR = 0, 1, 2
 CP_PIX_RGB24, CP_PIX_RGBA, CP_PIX_BGRA, CP_PIX_YUYV422, CP_PIX_UYVY422 = 16, 17, 18, 32, 33
 CP_PIX_PER_FRAME = 64
+CP_PIX_REMAP = 128
 PIXEL_FORMATS = ("bgr", "nv12", "i420", "rgb24", "rgba", "bgra", "yuyv422", "uyvy422")
 PIXEL_FORMAT_CODES = {"bgr": CP_PIX_BGR, "nv12": CP_PIX_NV12, "i420": CP_PIX_I420, "rgb24": CP_PIX_RGB24,
                       "rgba": CP_PIX_RGBA, "bgra": CP_PIX_BGRA, "yuyv422": CP_PIX_YUYV422, "uyvy422": CP_PIX_UYVY422}
@@ -234,6 +237,11 @@ def load():
                                         ctypes.POINTER(ctypes.c_float), vp]
     L.cp_preprocess_frame_table_formats.argtypes = [i64, ctypes.POINTER(i64), ctypes.POINTER(i32), ctypes.POINTER(i32),
                                                     i32, i32, i32, ctypes.POINTER(ctypes.c_double), vp, vp]
+    L.cp_preprocess_remap.argtypes = [vp, i64, ctypes.POINTER(i64), ctypes.POINTER(i32), ctypes.POINTER(i32),
+                                      ctypes.POINTER(vp), vp, i32, i32, i32, ctypes.POINTER(ctypes.c_double),
+                                      ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_float), vp]
+    L.cp_preprocess_frame_table_maps.argtypes = [i64, ctypes.POINTER(i64), ctypes.POINTER(i32), i32, ctypes.POINTER(i32),
+                                                 ctypes.POINTER(vp), i32, i32, i32, ctypes.POINTER(ctypes.c_double), vp, vp]
     L.cp_tracker_create.argtypes = [ctypes.POINTER(CpTrackerConfig), ctypes.POINTER(vp)]
     L.cp_tracker_destroy.argtypes = [vp]
     L.cp_tracker_reset.argtypes = [vp, i32, vp]

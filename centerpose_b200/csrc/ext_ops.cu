@@ -12,6 +12,8 @@
 //                        cp_preprocess_slots_rows_dev that of the live slots of a step with idle slots (a table may hold
 //                        one format per frame: cp_preprocess_frame_table_formats, launched as CP_PIX_PER_FRAME);
 //   cp_gather_rows_dev -- a row gather through a device map, the graph-safe reordering of per-slot rows.
+#include <climits>
+#include <cstring>
 #include <type_traits>
 #include <vector>
 
@@ -34,20 +36,37 @@ struct WarpM {
   double m[6];
 };
 
-// one output pixel (x, y) of a [sh, sw] frame under the inverted matrix W, all three channels.  The source pixels come
-// from `px`: px.taps(iy, ix, in-frame flags) sees the 2 x 2 taps (iy, ix) .. (iy + 1, ix + 1) once, then px(k, yy, xx, c)
-// is channel c (B, G, R) of in-frame tap k = 2 (yy - iy) + (xx - ix) as an integer 0..255.  Taps outside the frame are
-// the border value 0 and are never fetched.  Channel c's value goes to out[c * plane], then to prev(c, value), the
-// previous-frame write of the launch's mode (preprocess_kernel).
-template <class Fetch, class Prev>
-__device__ __forceinline__ void warp_walk(Fetch px, float* __restrict__ out, size_t plane, int sh, int sw, int x,
-                                          int y, const WarpM& W, const float* mean, const float* stdv, Prev prev) {
+// The source position of output pixel (x, y) under the inverted matrix W in 1/32 pixels, warpAffine's coordinate
+// generator.
+__device__ __forceinline__ int2 affine_pos(const WarpM& W, int x, int y) {
   // unfused double arithmetic (the host code OpenCV runs here has no FMA contraction)
   const int X0 = __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(W.m[1], (double)y), W.m[2]), 1024.0)) + 16;
   const int Y0 = __double2int_rn(__dmul_rn(__dadd_rn(__dmul_rn(W.m[4], (double)y), W.m[5]), 1024.0)) + 16;
   const int ad = __double2int_rn(__dmul_rn(__dmul_rn(W.m[0], (double)x), 1024.0));
   const int bd = __double2int_rn(__dmul_rn(__dmul_rn(W.m[3], (double)x), 1024.0));
-  const int X = (X0 + ad) >> 5, Y = (Y0 + bd) >> 5;
+  return make_int2((X0 + ad) >> 5, (Y0 + bd) >> 5);
+}
+
+// The source position of a coordinate-map entry m = (map x, map y) in 1/32 pixels, cv2.remap's generator for float
+// maps (imgwarp.cpp RemapInvoker, INTER_LINEAR): cvRound(m * INTER_TAB_SIZE) of the float32 product.  cvRound is the
+// x86 conversion, whose result for NaN, +-inf and products beyond the int range is INT_MIN; that lands far outside the
+// frame, so the pixel is the border value 0.  (__float2int_rn would give 0 for NaN and saturate the others, which
+// samples inside the frame.)
+__device__ __forceinline__ int cv_round32(float v) {
+  const float p = __fmul_rn(v, 32.f);
+  return p >= -2147483648.f && p < 2147483648.f ? __float2int_rn(p) : INT_MIN;
+}
+__device__ __forceinline__ int2 map_pos(float2 m) { return make_int2(cv_round32(m.x), cv_round32(m.y)); }
+
+// one output pixel of a [sh, sw] frame whose source position is (X, Y) in 1/32 pixels (affine_pos or map_pos), all
+// three channels.  The source pixels come from `px`: px.taps(iy, ix, in-frame flags) sees the 2 x 2 taps (iy, ix) ..
+// (iy + 1, ix + 1) once, then px(k, yy, xx, c) is channel c (B, G, R) of in-frame tap k = 2 (yy - iy) + (xx - ix) as
+// an integer 0..255.  Taps outside the frame are the border value 0 and are never fetched.  Channel c's value goes to
+// out[c * plane], then to prev(c, value), the previous-frame write of the launch's mode (preprocess_kernel).
+template <class Fetch, class Prev>
+__device__ __forceinline__ void warp_walk(Fetch px, float* __restrict__ out, size_t plane, int sh, int sw, int2 pos,
+                                          const float* mean, const float* stdv, Prev prev) {
+  const int X = pos.x, Y = pos.y;
   int ix = X >> 5, iy = Y >> 5;
   // saturate_cast<short> of the integer coordinates (only matters for absurd scales; keeps the restatement exact)
   ix = max(-32768, min(32767, ix));
@@ -173,16 +192,26 @@ struct RaggedFrame {
 // offset, so its entries are RaggedFrames of the same 64 bytes and a walk still reads one entry per output pixel.
 constexpr int kFormatShift = 56;
 constexpr long long kOffsetMask = (1ll << kFormatShift) - 1;
+// A mapped frame (a table of cp_preprocess_frame_table_maps, launched with CP_PIX_REMAP) sets bit 6 of that byte, above
+// every format, and keeps the device address of its coordinate map, float2 [dh, dw], in the bits of W.m[0]; the rest
+// of W is unused.  Unmapped frames of the same table keep their affine.
+constexpr long long kMappedFlag = 1ll << (kFormatShift + 6);
+__device__ __forceinline__ const float2* frame_map(const RaggedFrame& f) {
+  return reinterpret_cast<const float2*>(__double_as_longlong(f.W.m[0]));
+}
 
-// walk(fetch) with the tap fetch of frame f in format kFormat; CP_PIX_PER_FRAME: in the format its entry holds.  The
-// format is uniform across a frame, so the branch costs a frame's threads nothing but the switch.
-template <int kFormat, class Walk>
+// walk(fetch) with the tap fetch of frame f in the format of launch code kCode (a cp_pixel_format or CP_PIX_PER_FRAME,
+// with or without CP_PIX_REMAP); CP_PIX_PER_FRAME: in the format its entry holds.  The format is uniform across a frame,
+// so the branch costs a frame's threads nothing but the switch.  Only the CP_PIX_REMAP instances mask the mapped flag.
+template <int kCode, class Walk>
 __device__ __forceinline__ void frame_walk(const uint8_t* __restrict__ frames, const RaggedFrame& f, Walk walk) {
+  constexpr bool kRemap = kCode & CP_PIX_REMAP;
+  constexpr int kFormat = kCode & ~CP_PIX_REMAP;
   if constexpr (kFormat != CP_PIX_PER_FRAME) {
-    walk(make_fetch<kFormat>(frames + f.offset, f.sh, f.sw));
+    walk(make_fetch<kFormat>(frames + (kRemap ? f.offset & kOffsetMask : f.offset), f.sh, f.sw));
   } else {
     const uint8_t* img = frames + (f.offset & kOffsetMask);
-    switch ((int)(f.offset >> kFormatShift)) {
+    switch (kRemap ? (int)((f.offset & ~kMappedFlag) >> kFormatShift) : (int)(f.offset >> kFormatShift)) {
       case CP_PIX_NV12: walk(make_fetch<CP_PIX_NV12>(img, f.sh, f.sw)); break;
       case CP_PIX_I420: walk(make_fetch<CP_PIX_I420>(img, f.sh, f.sw)); break;
       case CP_PIX_BGR: walk(make_fetch<CP_PIX_BGR>(img, f.sh, f.sw)); break;
@@ -218,9 +247,11 @@ enum PrevMode { kNoPrev, kTwin, kExchange };
 
 // B rows of [3, dh, dw]: row n is frame n (uniform) or the frame of slot s through the table (kTable), in format
 // kFormat (CP_PIX_PER_FRAME: each table entry's own).  Every thread is one output pixel of one row, grid-stride, and
-// reads and writes only its own elements.
+// reads and writes only its own elements.  kFormat | CP_PIX_REMAP (table form only): a mapped entry takes its source
+// position from its coordinate map at the output pixel, an unmapped one from its affine.
 template <int kFormat, bool kTable, PrevMode kMode>
 __global__ void preprocess_kernel(const PreprocessArgs a) {
+  static_assert(kTable || !(kFormat & CP_PIX_REMAP), "coordinate maps come through a frame table");
   const size_t plane = (size_t)a.dh * a.dw, total = (size_t)a.B * plane;
   for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
     const int x = (int)(i % a.dw);
@@ -239,8 +270,18 @@ __global__ void preprocess_kernel(const PreprocessArgs a) {
     const bool start = kMode != kNoPrev && a.start && a.start[s];
     float* prev = a.prev + o;
     float* store = a.store + (size_t)s * 3 * plane + px;
+    // a mapped launch reads the map before the format switch; the others generate the affine position inside it
+    int2 mapped{};
+    if constexpr ((kFormat & CP_PIX_REMAP) != 0)
+      mapped = f.offset & kMappedFlag ? map_pos(frame_map(f)[px]) : affine_pos(f.W, x, y);
     frame_walk<kFormat>(a.frames, f, [&](auto fetch) {
-      warp_walk(fetch, a.out + o, plane, f.sh, f.sw, x, y, f.W, a.mean, a.stdv, [&](int c, float v) {
+      const int2 pos = [&] {
+        if constexpr ((kFormat & CP_PIX_REMAP) != 0)
+          return mapped;
+        else
+          return affine_pos(f.W, x, y);
+      }();
+      warp_walk(fetch, a.out + o, plane, f.sh, f.sw, pos, a.mean, a.stdv, [&](int c, float v) {
         if constexpr (kMode == kTwin) {
           if (start) prev[c * plane] = v;
         } else if constexpr (kMode == kExchange) {
@@ -313,10 +354,16 @@ bool known_format(int format) {
          format == CP_PIX_BGRA || is_yuv422(format);
 }
 
+// a launch code of a frame table: a cp_pixel_format or CP_PIX_PER_FRAME, either with or without CP_PIX_REMAP
+bool table_code(int code) {
+  const int format = code & ~CP_PIX_REMAP;
+  return code >= 0 && (known_format(format) || format == CP_PIX_PER_FRAME);
+}
+
 // f(std::integral_constant<int, format>) for a format chosen at run time (one of cp_pixel_format or
 // CP_PIX_PER_FRAME), already checked
 template <class F>
-void with_format(int format, F f) {
+void with_base_format(int format, F f) {
   switch (format) {
     case CP_PIX_NV12: f(std::integral_constant<int, CP_PIX_NV12>{}); break;
     case CP_PIX_I420: f(std::integral_constant<int, CP_PIX_I420>{}); break;
@@ -328,6 +375,16 @@ void with_format(int format, F f) {
     case CP_PIX_UYVY422: f(std::integral_constant<int, CP_PIX_UYVY422>{}); break;
     default: f(std::integral_constant<int, CP_PIX_PER_FRAME>{});
   }
+}
+
+// with_base_format for a launch code, already checked: a table code with CP_PIX_REMAP gives its own constant
+template <class F>
+void with_format(int code, F f) {
+  if (code & CP_PIX_REMAP)
+    with_base_format(code & ~CP_PIX_REMAP,
+                     [&](auto k) { f(std::integral_constant<int, decltype(k)::value | CP_PIX_REMAP>{}); });
+  else
+    with_base_format(code, f);
 }
 
 // the arguments every form of preprocess_kernel takes; the entry points fill in the frame source and previous frame
@@ -346,11 +403,11 @@ PreprocessArgs preprocess_args(const uint8_t* frames, float* out, int B, int dh,
   return a;
 }
 
-// enqueues preprocess_kernel in `format`: the table form when a.fr is set (which may also be CP_PIX_PER_FRAME and
-// take the store exchange, with rows), else the uniform form; the previous-frame mode is the one a's pointers select
+// enqueues preprocess_kernel in `format`: the table form when a.fr is set (which may also be CP_PIX_PER_FRAME, carry
+// CP_PIX_REMAP and take the store exchange, with rows), else the uniform form; the previous-frame mode is the one a's
+// pointers select
 int launch_preprocess(int format, const PreprocessArgs& a, cudaStream_t s) {
-  if (a.fr ? !known_format(format) && format != CP_PIX_PER_FRAME || (a.store && !a.rows)
-           : !known_format(format) || a.store)
+  if (a.fr ? !table_code(format) || (a.store && !a.rows) : !known_format(format) || a.store)
     return fail(CP_ERR_INVALID, "preprocess_kernel: no instance for pixel format " + std::to_string(format) +
                                     (a.fr ? " over a frame table" : " over a uniform batch") +
                                     (a.store ? " with a store" : ""));
@@ -365,7 +422,7 @@ int launch_preprocess(int format, const PreprocessArgs& a, cudaStream_t s) {
         preprocess_kernel<kFormat, true, kTwin><<<blocks, 256, 0, s>>>(a);
       else
         preprocess_kernel<kFormat, true, kExchange><<<blocks, 256, 0, s>>>(a);
-    } else if constexpr (kFormat != CP_PIX_PER_FRAME) {
+    } else if constexpr (kFormat != CP_PIX_PER_FRAME && !(kFormat & CP_PIX_REMAP)) {
       if (mode == kNoPrev)
         preprocess_kernel<kFormat, false, kNoPrev><<<blocks, 256, 0, s>>>(a);
       else
@@ -378,13 +435,15 @@ int launch_preprocess(int format, const PreprocessArgs& a, cudaStream_t s) {
 
 // The per-frame parameters of a ragged batch, checked against the packed buffer before any work is enqueued.  Frame b
 // is in `format` (a cp_pixel_format), or in formats[b] when `formats` (host int32 [B]) is given; then each entry's
-// offset also carries the frame's format (kFormatShift), for a CP_PIX_PER_FRAME launch.
+// offset also carries the frame's format (kFormatShift), for a CP_PIX_PER_FRAME launch.  maps (host, B device
+// pointers, or NULL): frame b with maps[b] set is a mapped entry (kMappedFlag), for a CP_PIX_REMAP launch.
 int ragged_frames(const char* who, int64_t frames_bytes, const int64_t* offsets, const int32_t* src_hw, int B, int dst_h,
-                  int dst_w, const double* trans_input, int format, const int32_t* formats, std::vector<RaggedFrame>& fr) {
+                  int dst_w, const double* trans_input, int format, const int32_t* formats, std::vector<RaggedFrame>& fr,
+                  const float* const* maps = nullptr) {
   const std::string w0 = who;
-  if (formats && frames_bytes > kOffsetMask)
+  if ((formats || maps) && frames_bytes > kOffsetMask)
     return fail(CP_ERR_INVALID, w0 + ": a " + std::to_string(frames_bytes) + "-byte buffer is too large for per-frame "
-                                "formats");
+                                "formats or maps");
   fr.resize(B);
   for (int b = 0; b < B; ++b) {
     const int h = src_hw[2 * b], w = src_hw[2 * b + 1];
@@ -412,6 +471,13 @@ int ragged_frames(const char* who, int64_t frames_bytes, const int64_t* offsets,
     fr[b].offset = formats ? offsets[b] | (long long)fmt << kFormatShift : offsets[b];
     fr[b].sh = h;
     fr[b].sw = w;
+    if (maps && maps[b]) {
+      if ((uintptr_t)maps[b] % alignof(float2))
+        return fail(CP_ERR_INVALID, w0 + ": the map of frame " + std::to_string(b) + " is not 8-byte aligned");
+      const long long addr = (long long)(uintptr_t)maps[b];
+      std::memcpy(&fr[b].W.m[0], &addr, sizeof addr);
+      fr[b].offset |= kMappedFlag;
+    }
   }
   return CP_OK;
 }
@@ -435,9 +501,9 @@ int launch_ragged(const char* who, int format, const std::vector<RaggedFrame>& f
 // checks a frame table's frames (ragged_frames) and writes it to `table`
 int upload_frame_table(const char* who, int64_t frames_bytes, const int64_t* offsets, const int32_t* src_hw, int format,
                        const int32_t* formats, int B, int dst_h, int dst_w, const double* trans_input, void* table,
-                       void* stream_) {
+                       void* stream_, const float* const* maps = nullptr) {
   std::vector<RaggedFrame> fr;
-  int rc = ragged_frames(who, frames_bytes, offsets, src_hw, B, dst_h, dst_w, trans_input, format, formats, fr);
+  int rc = ragged_frames(who, frames_bytes, offsets, src_hw, B, dst_h, dst_w, trans_input, format, formats, fr, maps);
   if (rc) return rc;
   // a build-time call: the copy is complete when it returns, so `fr` may go out of scope
   cudaStream_t s = (cudaStream_t)stream_;
@@ -655,6 +721,24 @@ int cp_preprocess_formats(const uint8_t* frames, int64_t frames_bytes, const int
                        (cudaStream_t)stream_);
 }
 
+int cp_preprocess_remap(const uint8_t* frames, int64_t frames_bytes, const int64_t* offsets, const int32_t* src_hw,
+                        const int32_t* formats, const float* const* maps, float* out, int32_t B, int32_t dst_h,
+                        int32_t dst_w, const double* trans_input, const float mean[3], const float stdv[3],
+                        void* stream_) {
+  if (!frames || !offsets || !src_hw || !formats || !maps || !out || !mean || !stdv)
+    return fail(CP_ERR_INVALID, "cp_preprocess_remap: null argument");
+  if (B <= 0 || dst_h <= 0 || dst_w <= 0 || frames_bytes <= 0) return fail(CP_ERR_INVALID, "cp_preprocess_remap: bad shape");
+  int format = formats[0];
+  for (int b = 1; b < B; ++b)
+    if (formats[b] != format) format = CP_PIX_PER_FRAME;
+  std::vector<RaggedFrame> fr;
+  int rc = ragged_frames("cp_preprocess_remap", frames_bytes, offsets, src_hw, B, dst_h, dst_w, trans_input, format,
+                         format == CP_PIX_PER_FRAME ? formats : nullptr, fr, maps);
+  if (rc) return rc;
+  return launch_ragged("cp_preprocess_remap", format | CP_PIX_REMAP, fr,
+                       preprocess_args(frames, out, B, dst_h, dst_w, mean, stdv), (cudaStream_t)stream_);
+}
+
 int cp_preprocess_slots_dev(const uint8_t* frames, int32_t format, int32_t B, int32_t src_h, int32_t src_w,
                             int32_t dst_h, int32_t dst_w, const double* trans_input, const float mean[3],
                             const float stdv[3], const int32_t* start, float* out, float* prev, void* stream_) {
@@ -711,13 +795,27 @@ int cp_preprocess_frame_table_formats(int64_t frames_bytes, const int64_t* offse
                             B, dst_h, dst_w, trans_input, table, stream_);
 }
 
+int cp_preprocess_frame_table_maps(int64_t frames_bytes, const int64_t* offsets, const int32_t* src_hw, int32_t format,
+                                   const int32_t* formats, const float* const* maps, int32_t B, int32_t dst_h,
+                                   int32_t dst_w, const double* trans_input, void* table, void* stream_) {
+  if (!offsets || !src_hw || !maps || !table) return fail(CP_ERR_INVALID, "cp_preprocess_frame_table_maps: null argument");
+  if (B <= 0 || dst_h <= 0 || dst_w <= 0 || frames_bytes <= 0)
+    return fail(CP_ERR_INVALID, "cp_preprocess_frame_table_maps: bad shape");
+  if (format == CP_PIX_PER_FRAME ? !formats : !known_format(format) || formats)
+    return fail(CP_ERR_INVALID, "cp_preprocess_frame_table_maps: format " + std::to_string(format) +
+                                    (formats ? " with per-frame formats (they take CP_PIX_PER_FRAME)"
+                                             : " (a cp_pixel_format, or CP_PIX_PER_FRAME with per-frame formats)"));
+  return upload_frame_table("cp_preprocess_frame_table_maps", frames_bytes, offsets, src_hw, format, formats, B, dst_h,
+                            dst_w, trans_input, table, stream_, maps);
+}
+
 int cp_preprocess_slots_ragged_dev(const uint8_t* frames, const void* table, int32_t format, int32_t B, int32_t dst_h,
                                    int32_t dst_w, const float mean[3], const float stdv[3], const int32_t* start,
                                    float* out, float* prev, void* stream_) {
   if (!frames || !table || !out || !mean || !stdv)
     return fail(CP_ERR_INVALID, "cp_preprocess_slots_ragged_dev: null argument");
   if (!start != !prev) return fail(CP_ERR_INVALID, "cp_preprocess_slots_ragged_dev: start and prev go together");
-  if (!known_format(format) && format != CP_PIX_PER_FRAME)
+  if (!table_code(format))
     return fail(CP_ERR_INVALID, "cp_preprocess_slots_ragged_dev: unknown pixel format " + std::to_string(format));
   if (B <= 0 || dst_h <= 0 || dst_w <= 0) return fail(CP_ERR_INVALID, "cp_preprocess_slots_ragged_dev: bad shape");
   PreprocessArgs a = preprocess_args(frames, out, B, dst_h, dst_w, mean, stdv);
@@ -733,7 +831,7 @@ int cp_preprocess_slots_rows_dev(const uint8_t* frames, const void* table, int32
   if (!frames || !table || !rows || !out || !mean || !stdv)
     return fail(CP_ERR_INVALID, "cp_preprocess_slots_rows_dev: null argument");
   if (!store != !prev) return fail(CP_ERR_INVALID, "cp_preprocess_slots_rows_dev: store and prev go together");
-  if (!known_format(format) && format != CP_PIX_PER_FRAME)
+  if (!table_code(format))
     return fail(CP_ERR_INVALID, "cp_preprocess_slots_rows_dev: unknown pixel format " + std::to_string(format));
   if (B <= 0 || dst_h <= 0 || dst_w <= 0) return fail(CP_ERR_INVALID, "cp_preprocess_slots_rows_dev: bad shape");
   PreprocessArgs a = preprocess_args(frames, out, B, dst_h, dst_w, mean, stdv);

@@ -19,7 +19,8 @@ import torch
 
 from . import _lib
 from .engine import (Engine, check_pixel_format, decode_params, decode_pnp, frame_layout, image_size, make_meta,
-                     preprocess, preprocess_formats, slot_formats)
+                     preprocess, preprocess_formats, preprocess_remap, slot_formats)
+from .lens import MapCache, slot_distortions, undistorted_cameras
 from .model import _load_checkpoint, create_model, load_model
 from .tracker import Tracker, tracks_to_results
 
@@ -207,6 +208,7 @@ class ObjectPoseDetector(object):
         self._meta_dev = None
         self._packed = None            # run_batch(list): device buffer the ragged frames are packed into
         self._affines = {}             # (h, w) -> fix_res trans_input of that frame size
+        self._maps = MapCache()        # run_batch(distortion=): the device map of each camera
 
     def _to_device(self, t):
         """base_detector.py:41,436: everything the network touches lives on opt.device (always CUDA here)."""
@@ -547,7 +549,7 @@ class ObjectPoseDetector(object):
 
     # ------------------------------------------------------------------ batched API (not in the reference)
     def run_batch(self, frames, camera_matrix, pre_images=None, pre_hms=None, pre_hm_hp=None, to_host=True, track=False,
-                  out=None, pre_dets=None, frame_ids=None, new_video=None, pixel_format="bgr"):
+                  out=None, pre_dets=None, frame_ids=None, new_video=None, pixel_format="bgr", distortion=None):
         """frames: uint8 [B,H,W,3] (numpy / pinned CPU tensor / CUDA tensor) or a
         pre-processed fp32 [B,3,h,w] CUDA tensor.  One native cp_infer call for the
         whole batch.  Returns (poses [B,K,192], n_valid [B]) -- on the host when
@@ -578,22 +580,33 @@ class ObjectPoseDetector(object):
         ([B,H,W,4]) and "yuyv422" / "uyvy422" ([B,H,W,2], W even) are converted the same way, each bit for bit its
         cv2.cvtColor to BGR (COLOR_RGB2BGR, _RGBA2BGR, _BGRA2BGR, COLOR_YUV2BGR_YUYV, _UYVY).  With a list of frames,
         pixel_format may also be a list of one name per frame or slot (cameras of different kinds); a list of one name
-        repeated is that name."""
+        repeated is that name.
+
+        distortion: the lens distortion of the cameras (lens.LensDistortion), one for every camera or a list of one per
+        frame or slot, None for an undistorted camera.  A distorted camera's frames are undistorted inside the
+        pre-process: its network input is, bit for bit, the normalised cv2.remap of the BGR frame through
+        lens.undistort_map (built once per camera and kept on the device), and its meta row carries the
+        new_camera_matrix K_new, so records are in the pixels of the undistorted image of camera K_new and poses in the
+        camera frame.  Every result then equals that of the same call on those fp32 inputs with camera_matrix K_new.
+        The array form goes through a frame table (cp_preprocess_remap) only when some camera is distorted.  Refused:
+        distortion with pre-processed fp32 frames, and with the keep_res / fix_short pre-process."""
         if track and not getattr(self.opt, "tracking_task", False):
             raise ValueError("run_batch(track=True) needs a tracking model (opt.tracking_task)")
         if isinstance(frames, (list, tuple)):
             if pre_images is not None or pre_hms is not None or pre_hm_hp is not None:
                 raise ValueError("run_batch(list): the previous frames and heat maps are kept per slot (track=True)")
             if track:
-                return self._run_slots(frames, camera_matrix, to_host, out, pre_dets, frame_ids, new_video, pixel_format)
+                return self._run_slots(frames, camera_matrix, to_host, out, pre_dets, frame_ids, new_video, pixel_format,
+                                       distortion)
             if new_video is not None or pre_dets is not None or frame_ids is not None:
                 raise ValueError("run_batch(list): new_video / pre_dets / frame_ids need track=True")
+            dists = slot_distortions(distortion, len(frames))
             check_frames(frames, allow_idle=False, pixel_format=pixel_format)
-            x, meta, _ = self._ragged_input(frames, camera_matrix, pixel_format)
+            x, meta, _ = self._ragged_input(frames, camera_matrix, pixel_format, dists)
         else:
             if new_video is not None:
                 raise ValueError("run_batch: new_video needs a list of slot frames")
-            x, meta, c, s = self._array_input(frames, camera_matrix, pixel_format)
+            x, meta, c, s = self._array_input(frames, camera_matrix, pixel_format, distortion)
             B = x.shape[0]
             if track:
                 pre_dets = self._slot_pre_dets(pre_dets, B)
@@ -606,13 +619,16 @@ class ObjectPoseDetector(object):
                                       n_valid=out[1] if out is not None else None)
         return _returned((poses, n_valid), to_host)
 
-    def _array_input(self, frames, camera_matrix, pixel_format="bgr"):
+    def _array_input(self, frames, camera_matrix, pixel_format="bgr", distortion=None):
         """run_batch's array form: uint8 [B,H,W,3] frames, frames of another pixel_format (uint8 [B,3H/2,W], [B,H,W,C]) (or
         pre-processed fp32 [B,3,h,w]) -> (x [B,3,h,w] fp32 CUDA, meta rows [B,16] float64 host, c, s) with the fix_res
-        affine of the image size."""
+        affine of the image size; with a distorted camera (distortion), through _remap_input."""
         dev = self.opt.device
         if isinstance(frames, np.ndarray):
             frames = torch.from_numpy(frames)
+        dists = slot_distortions(distortion, frames.shape[0] if frames.dim() else 0)
+        if dists is not None:
+            return self._remap_input(frames, camera_matrix, pixel_format, dists)
         if check_pixel_format(pixel_format) != "bgr":
             layout = frame_layout(pixel_format)
             if frames.dtype != torch.uint8 or frames.dim() != layout.count(",") + 2:
@@ -643,12 +659,46 @@ class ObjectPoseDetector(object):
             raise NotImplementedError("run_batch pre-processes at scale 1; use run() for test_scales[0] != 1")
         return x, meta, c, s
 
+    def _remap_input(self, frames, camera_matrix, pixel_format, dists):
+        """_array_input with distorted cameras: the uint8 frames of one size as a frame table, one cp_preprocess_remap
+        launch (unmapped frames under the fix_res affine of the size, as the array form without distortion)."""
+        self._check_undistort(pixel_format)
+        if frames.dtype != torch.uint8:
+            raise ValueError("run_batch: distortion undistorts camera frames (uint8); pre-processed fp32 input has no "
+                             "frame to remap, got %s" % frames.dtype)
+        layout = frame_layout(pixel_format)
+        if frames.dim() != layout.count(",") + 2:
+            raise ValueError("run_batch: %s frames are uint8 [B,%s, got %s" % (pixel_format, layout[1:], tuple(frames.shape)))
+        B = frames.shape[0]
+        sh, sw = image_size(frames.shape[1:], pixel_format, "run_batch: each frame")
+        cams = camera_per_frame(camera_matrix, B)
+        ih, iw = self.opt.input_h, self.opt.input_w
+        maps = self._maps.maps(dists, cams, [(sh, sw)] * B, (ih, iw), self.opt.device)
+        fr = frames.to(self.opt.device, non_blocking=True).contiguous().reshape(-1)
+        n = fr.numel() // max(B, 1)
+        x = preprocess_remap(fr, np.arange(B, dtype=np.int64) * n, [(sh, sw)] * B, pixel_format, maps, ih, iw,
+                             self.opt.mean, self.opt.std)
+        c, s = np.array([sw / 2., sh / 2.], np.float32), float(max(sh, sw))
+        meta = make_meta(B, c, s, sw, sh, undistorted_cameras(dists, cams)).numpy()
+        return x, meta, c, s
+
+    def _check_undistort(self, pixel_format):
+        """Refuses, before any device work, what the undistorting pre-process does not take."""
+        if getattr(self.opt, "fix_short", 0) > 0 or not getattr(self.opt, "fix_res", True):
+            raise NotImplementedError("run_batch: distortion undistorts into the fix_res input; the keep_res and "
+                                      "fix_short pre-process take no distortion")
+        if float(self.scales[0]) != 1.0:
+            raise NotImplementedError("run_batch pre-processes at scale 1; use run() for test_scales[0] != 1")
+        if not isinstance(pixel_format, (list, tuple)):
+            check_pixel_format(pixel_format)
+
     # ------------------------------------------------------------------ ragged batches (lists of frames)
-    def _ragged_input(self, frames, camera_matrix, pixel_format="bgr"):
+    def _ragged_input(self, frames, camera_matrix, pixel_format="bgr", dists=None):
         """Validated list of uint8 HWC frames (or frames of pixel_format: one name, or one per frame) -> (x [B,3,h,w]
         fp32 CUDA, meta rows [B,16] float64 host, trans_input [B,2,3] host).  The frames are copied into one device
         buffer and pre-processed by one cp_preprocess_formats launch with the same fix_res affine (c = image centre,
-        s = max side) and meta row that pre_process / run() use."""
+        s = max side) and meta row that pre_process / run() use.  dists (slot_distortions, one per frame): one
+        cp_preprocess_remap launch instead, the distorted frames through their maps and with K_new in their meta rows."""
         if getattr(self.opt, "fix_short", 0) > 0 or not getattr(self.opt, "fix_res", True):
             raise NotImplementedError("run_batch(list) pre-processes in the fix_res mode only")
         if float(self.scales[0]) != 1.0:
@@ -656,6 +706,8 @@ class ObjectPoseDetector(object):
         B = len(frames)
         cams = camera_per_frame(camera_matrix, B)
         fmts = slot_formats(pixel_format, B)
+        if dists is not None:
+            self._check_undistort(pixel_format)
         dev = self.opt.device
         ih, iw = self.opt.input_h, self.opt.input_w
         ts, hw, offs, off = [], np.zeros((B, 2), np.int32), np.zeros(B, np.int64), 0
@@ -677,8 +729,14 @@ class ObjectPoseDetector(object):
             if (h, w) not in self._affines:
                 self._affines[(h, w)] = affine_from_center_scale(c, sc, iw, ih)
             trans[b] = self._affines[(h, w)]
-            meta[b] = make_meta(1, c, sc, w, h, cams[b]).numpy()[0]
-        x = preprocess_formats(self._packed, offs, hw, fmts, ih, iw, self.opt.mean, self.opt.std, trans_input=trans)
+            meta[b] = make_meta(1, c, sc, w, h, cams[b] if dists is None else undistorted_cameras(dists[b:b + 1],
+                                                                                                 cams[b:b + 1])).numpy()[0]
+        if dists is None:
+            x = preprocess_formats(self._packed, offs, hw, fmts, ih, iw, self.opt.mean, self.opt.std, trans_input=trans)
+        else:
+            maps = self._maps.maps(dists, cams, [tuple(v) for v in hw], (ih, iw), dev)
+            x = preprocess_remap(self._packed, offs, hw, fmts, maps, ih, iw, self.opt.mean, self.opt.std,
+                                 trans_input=trans)
         return x, meta, trans
 
     def _meta_rows(self, meta):
@@ -690,7 +748,8 @@ class ObjectPoseDetector(object):
             self._meta_key = key
         return self._meta_dev
 
-    def _run_slots(self, frames, camera_matrix, to_host, out, pre_dets, frame_ids, new_video, pixel_format="bgr"):
+    def _run_slots(self, frames, camera_matrix, to_host, out, pre_dets, frame_ids, new_video, pixel_format="bgr",
+                   distortion=None):
         """run_batch(list, track=True): frames[i] is the next frame of the video in slot i, or None when slot i is idle
         this step (its tracker stream is not stepped and keeps its state).  new_video[i] marks the first frame of a
         video in slot i, which then behaves exactly like the first run() call of a fresh detector: the stream is reset,
@@ -700,6 +759,9 @@ class ObjectPoseDetector(object):
         Returns (tracks [S,T,320], n_tracks [S]) for the S slots, idle slots with n_tracks 0 and zero rows; out:
         optional (tracks, n_tracks) CUDA tensors of those shapes to write into."""
         S = len(frames)
+        dists = slot_distortions(distortion, S)
+        if dists is not None:
+            self._check_undistort(pixel_format)
         check_frames(frames, allow_idle=True, pixel_format=pixel_format)
         cams = camera_per_frame(camera_matrix, S)
         new_video = check_slot_list(new_video, S, "new_video", bool)
@@ -713,7 +775,8 @@ class ObjectPoseDetector(object):
             return _returned(out, to_host)
         fmts = slot_formats(pixel_format, S)
         x, meta, trans = self._ragged_input([frames[i] for i in live], np.stack([cams[i] for i in live]),
-                                            [fmts[i] for i in live])
+                                            [fmts[i] for i in live],
+                                            slot_distortions([dists[i] for i in live], len(live)) if dists else None)
         return self._track_step(S, live, x, self._meta_rows(meta), trans, new_video, pre_dets, frame_ids, to_host, out)
 
     # ---- what a tracking step does per category: one category here; MultiCategoryTracker runs several through the
@@ -868,17 +931,17 @@ class MultiCategoryDetector(ObjectPoseDetector):
             self._eng = eng
         return eng
 
-    def run_batch(self, frames, camera_matrix, to_host=True, out=None, pixel_format="bgr"):
+    def run_batch(self, frames, camera_matrix, to_host=True, out=None, pixel_format="bgr", distortion=None):
         """run_batch of ObjectPoseDetector (a uint8 [B,H,W,3] array, or a list of mixed-size frames with one camera or
-        one per frame; YUV 4:2:0 and camera formats with pixel_format, a list of names with a list of frames, as there)
-        for every category: the frames are
-        pre-processed once.  Returns (poses [M,B,K,192], n_valid [M,B]) in `categories` order, also for M = 1; out:
+        one per frame; YUV 4:2:0 and camera formats with pixel_format, a list of names with a list of frames, and lens
+        distortion with distortion, as there) for every category: the frames are pre-processed once.  Returns (poses [M,B,K,192], n_valid [M,B]) in `categories` order, also for M = 1; out:
         optional (poses, n_valid) CUDA tensors of those shapes to write into."""
         if isinstance(frames, (list, tuple)):
+            dists = slot_distortions(distortion, len(frames))
             check_frames(frames, allow_idle=False, pixel_format=pixel_format)
-            x, meta, _ = self._ragged_input(frames, camera_matrix, pixel_format)
+            x, meta, _ = self._ragged_input(frames, camera_matrix, pixel_format, dists)
         else:
-            x, meta, _, _ = self._array_input(frames, camera_matrix, pixel_format)
+            x, meta, _, _ = self._array_input(frames, camera_matrix, pixel_format, distortion)
         eng = self.engine(x.shape[0], x.shape[2], x.shape[3])
         if len(self._prms) > 1:
             _, poses, n_valid = eng.infer(x, self._meta_rows(meta), self._prms,
@@ -919,7 +982,7 @@ class MultiCategoryTracker(MultiCategoryDetector):
             self.tracker = None
 
     def run_batch(self, frames, camera_matrix, new_video=None, pre_dets=None, frame_ids=None, to_host=True, out=None,
-                  pixel_format="bgr"):
+                  pixel_format="bgr", distortion=None):
         """The next frame of every slot, for every category.  frames: uint8 [S,H,W,3] (every slot steps), or a list of S
         uint8 [H_s,W_s,3] frames of mixed sizes where None idles a slot this step, with camera_matrix [3,3] or one per
         slot.  new_video[i]: slot i starts a new video (every category).  pre_dets: None, or a mapping category -> per
@@ -927,12 +990,14 @@ class MultiCategoryTracker(MultiCategoryDetector):
         Returns (tracks [M,S,T,320], n_tracks [M,S]) in `categories` order (idle slots: n_tracks 0, zero rows), on the
         host when `to_host`; out: optional (tracks, n_tracks) CUDA tensors of those shapes to write into.
         pixel_format "nv12" / "i420": YUV 4:2:0 frames, uint8 [S,3H/2,W] or [3H_s/2,W_s]; the camera formats and one name
-        per slot with a list of frames as in ObjectPoseDetector.run_batch."""
+        per slot with a list of frames, and distortion (one LensDistortion, or one per slot), as in
+        ObjectPoseDetector.run_batch."""
         if isinstance(frames, (list, tuple)):
-            return self._run_slots(frames, camera_matrix, to_host, out, pre_dets, frame_ids, new_video, pixel_format)
+            return self._run_slots(frames, camera_matrix, to_host, out, pre_dets, frame_ids, new_video, pixel_format,
+                                   distortion)
         if new_video is not None:
             raise ValueError("run_batch: new_video needs a list of slot frames")
-        x, meta, c, s = self._array_input(frames, camera_matrix, pixel_format)
+        x, meta, c, s = self._array_input(frames, camera_matrix, pixel_format, distortion)
         S = x.shape[0]
         pre_dets = self._slot_pre_dets(pre_dets, S)
         frame_ids = check_slot_list(frame_ids, S, "frame_ids")

@@ -627,6 +627,40 @@ def preprocess_formats(packed_u8, offsets, src_hw, pixel_format, dst_h, dst_w, m
                               trans_input)
 
 
+def map_pointers(maps, n, dst_h, dst_w, device, who):
+    """The host array of n device pointers of cp_preprocess_remap / cp_preprocess_frame_table_maps: maps is a list of n
+    float32 [dst_h, dst_w, 2] contiguous CUDA tensors on `device` (lens.undistort_map's layout), None for a frame that
+    keeps its affine.  The caller keeps the tensors alive while a launch can read them."""
+    maps = list(maps)
+    if len(maps) != n:
+        raise ValueError("%s: %d maps for %d frames" % (who, len(maps), n))
+    device = torch.device(device)
+    if device.type == "cuda" and device.index is None:
+        device = torch.device("cuda", torch.cuda.current_device())
+    for b, m in enumerate(maps):
+        if m is not None and (not torch.is_tensor(m) or m.dtype != torch.float32 or tuple(m.shape) != (dst_h, dst_w, 2)
+                              or m.device != device or not m.is_contiguous()):
+            raise ValueError("%s: map %d must be a contiguous float32 [%d,%d,2] tensor on %s, got %s"
+                             % (who, b, dst_h, dst_w, device, (m.dtype, tuple(m.shape), str(m.device))
+                                if torch.is_tensor(m) else type(m).__name__))
+    return (ctypes.c_void_p * n)(*[None if m is None else m.data_ptr() for m in maps])
+
+
+def preprocess_remap(packed_u8, offsets, src_hw, pixel_format, maps, dst_h, dst_w, mean, std, out=None,
+                     trans_input=None):
+    """cp_preprocess_remap: preprocess_formats with a coordinate map per frame (lens distortion).  maps: one float32
+    [dst_h, dst_w, 2] CUDA tensor per frame, or None for a frame that keeps its affine (trans_input[b], or its fix_res
+    affine).  A mapped frame's output is bit for bit cv2.remap(cv2.cvtColor(frame) to BGR, map x, map y, INTER_LINEAR,
+    BORDER_CONSTANT, 0), normalised."""
+    _lib.load()
+    B = int(np.size(offsets))
+    codes = np.array([_lib.PIXEL_FORMAT_CODES[f] for f in slot_formats(pixel_format, B, "preprocess_remap")], np.int32)
+    ptrs = map_pointers(maps, B, dst_h, dst_w, packed_u8.device, "preprocess_remap")
+    return _preprocess_packed("preprocess_remap", packed_u8, offsets, src_hw,
+                              (codes.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)), ptrs), dst_h, dst_w, mean, std,
+                              out, trans_input)
+
+
 def preprocess_yuv420(packed_u8, offsets, src_hw, pixel_format, dst_h, dst_w, mean, std, out=None, trans_input=None):
     """cp_preprocess_yuv420: preprocess_ragged for YUV 4:2:0 frames.  packed_u8: flat uint8 CUDA buffer holding frame b
     (uint8 [3H/2,W] in pixel_format "nv12" or "i420", (H, W) = src_hw[b], both even) at byte offsets[b] -> fp32

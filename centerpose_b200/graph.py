@@ -59,15 +59,20 @@ class _SlotGraph(object):
         eng.load_state_dict(m.state_dict())
         return eng, decode_params(det.opt, test_scale=1.0), None
 
-    def _build(self, det, slots, frame_hw, camera_matrix, pixel_format, idle_slots=False):
+    def _build(self, det, slots, frame_hw, camera_matrix, pixel_format, idle_slots=False, distortion=None):
         """Checks, buffers and the captured steps; everything that refuses comes before any device work."""
         from .detector import affine_from_center_scale, camera_per_frame
-        from .engine import check_pixel_format, frame_shape, make_meta, slot_formats
+        from .engine import check_pixel_format, frame_shape, make_meta, map_pointers, slot_formats
+        from .lens import slot_distortions, undistort_map, undistorted_cameras
         who, opt = type(self).__name__, det.opt
         self._refuse(opt, who)
         S = int(slots)
         if S < 1:
             raise ValueError("%s: slots must be >= 1, got %d" % (who, S))
+        dists = slot_distortions(distortion, S, who)
+        if dists is not None and (getattr(opt, "fix_short", 0) > 0 or not getattr(opt, "fix_res", True)):
+            raise NotImplementedError("%s: distortion undistorts into the fix_res input; the keep_res and fix_short "
+                                      "pre-process take no distortion" % who)
         sizes, self.per_slot = _frame_sizes(frame_hw, S, who)
         self.idle_slots = bool(idle_slots)
         if isinstance(pixel_format, (list, tuple)) and not self.per_slot:
@@ -78,6 +83,10 @@ class _SlotGraph(object):
         self.pixel_format = fmts[0] if len(set(fmts)) == 1 else fmts
         shapes = [frame_shape(h, w, f) for (h, w), f in zip(sizes, fmts)]
         cams = np.stack(camera_per_frame(camera_matrix, S))
+        if dists is not None:                             # every map is built now, on the host, before device work
+            host_maps = [None if d is None else undistort_map(d, cams[b], sizes[b if self.per_slot else 0],
+                                                              (opt.input_h, opt.input_w)) for b, d in enumerate(dists)]
+            cams = undistorted_cameras(dists, cams)       # the meta rows carry K_new
         if self.per_slot:
             self.frame_hw, self.frame_shape = sizes, shapes
         else:
@@ -102,7 +111,9 @@ class _SlotGraph(object):
         self._std = (ctypes.c_float * 3)(*[float(v) for v in opt.std])
         mixed = isinstance(self.pixel_format, list)       # per-slot formats: a table of them, one per-frame launch
         self._fmt = _lib.CP_PIX_PER_FRAME if mixed else _lib.PIXEL_FORMAT_CODES[self.pixel_format]
-        if self.per_slot or self.idle_slots:                # a frame table (with idle slots: of S equal sizes too)
+        # a frame table with one frame_hw per slot, idle slots or lens distortion (with one frame_hw: S equal sizes)
+        self._table = self.per_slot or self.idle_slots or dists is not None
+        if self._table:
             n = [int(np.prod(s)) for s in self._slot_shapes]
             offs = np.concatenate([[0], np.cumsum(n)[:-1]]).astype(np.int64)
             self.frames = torch.zeros((int(sum(n)),), dtype=torch.uint8, device=dev)
@@ -112,7 +123,17 @@ class _SlotGraph(object):
             p64, p32 = offs.ctypes.data_as(ctypes.POINTER(ctypes.c_int64)), hw.ctypes.data_as(ctypes.POINTER(ctypes.c_int32))
             ptr = trans.ctypes.data_as(ctypes.POINTER(ctypes.c_double))
             with torch.cuda.device(dev):
-                if mixed:
+                if dists is not None:
+                    # the maps live as long as the graph that reads them
+                    self._maps = [None if m is None else torch.from_numpy(m).to(dev) for m in host_maps]
+                    codes = np.array([_lib.PIXEL_FORMAT_CODES[f] for f in fmts], np.int32) if mixed else None
+                    _lib.check(L.cp_preprocess_frame_table_maps(
+                        self.frames.numel(), p64, p32, self._fmt,
+                        None if codes is None else codes.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)),
+                        map_pointers(self._maps, S, ih, iw, dev, who), S, ih, iw, ptr, _ptr(self.table), _stream()),
+                        "cp_preprocess_frame_table_maps")
+                    self._fmt |= _lib.CP_PIX_REMAP
+                elif mixed:
                     codes = np.array([_lib.PIXEL_FORMAT_CODES[f] for f in fmts], np.int32)
                     _lib.check(L.cp_preprocess_frame_table_formats(self.frames.numel(), p64, p32,
                                                                    codes.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)),
@@ -166,7 +187,7 @@ class _SlotGraph(object):
         """The pre-process of every slot into out [S,3,h,w]; with start flags, a starting slot's input also goes to
         prev."""
         L, S, (ih, iw) = self.L, self.slots, out.shape[2:]
-        if self.per_slot:
+        if self._table:
             _lib.check(L.cp_preprocess_slots_ragged_dev(_ptr(self.frames), _ptr(self.table), self._fmt, S, ih, iw,
                                                         self._mean, self._std, _ptr(start), _ptr(out), _ptr(prev),
                                                         _stream()), "cp_preprocess_slots_ragged_dev")
@@ -266,7 +287,7 @@ class _SlotGraph(object):
         if self.idle_slots:
             return self._call_rows(frames, start)
         with torch.cuda.device(self.device):
-            for dst, f in zip(self._slot_frames if self.per_slot else [self.frames], frames):
+            for dst, f in zip(self._slot_frames if self.per_slot else [self.frames.view(self.frame_shape)], frames):
                 dst.copy_(f, non_blocking=True)
             if start is not None:
                 # one flag per tracker stream, the same in every category; a pageable source: staged before copy_
@@ -332,17 +353,22 @@ class DetectGraph(_SlotGraph):
     cameras, scattered to their slots: an idle slot comes back with n_valid 0 and zero rows, and an all-idle call returns
     zeros and launches nothing.  One step is captured per live count L = 1..S (the network runs at batch L, as in
     run_batch, and split-K makes batch-L bits differ from batch-S bits); a call is one copy per live frame, one copy of an
-    int32 control block (the row / slot maps) and one graph launch."""
+    int32 control block (the row / slot maps) and one graph launch.
+
+    distortion: the lens distortion of the cameras (lens.LensDistortion), one for every slot or a list of one per slot
+    (None: an undistorted camera), as run_batch(distortion=) takes it.  The maps (lens.undistort_map) and a frame table
+    with them are built with the graph, which then always pre-processes through the table; every step is bit for bit
+    run_batch(..., distortion=) on the same frames."""
 
     _host_list = "run_batch(list) of the live frames"
 
-    def __init__(self, det, slots, frame_hw, camera_matrix, pixel_format="bgr", idle_slots=False):
+    def __init__(self, det, slots, frame_hw, camera_matrix, pixel_format="bgr", idle_slots=False, distortion=None):
         from .detector import MultiCategoryDetector, ObjectPoseDetector
         if isinstance(det, MultiCategoryDetector):
             raise NotImplementedError("DetectGraph detects one category; several run through a MultiCategoryDetectGraph")
         if not isinstance(det, ObjectPoseDetector):
             raise NotImplementedError("DetectGraph takes an ObjectPoseDetector, got %s" % type(det).__name__)
-        self._build(det, slots, frame_hw, camera_matrix, pixel_format, idle_slots)
+        self._build(det, slots, frame_hw, camera_matrix, pixel_format, idle_slots, distortion)
 
     def _refuse(self, opt, who):
         if getattr(opt, "tracking_task", False):
@@ -411,7 +437,7 @@ class MultiCategoryDetectGraph(DetectGraph):
 
     _host_list = "MultiCategoryDetector.run_batch(list) of the live frames"
 
-    def __init__(self, mdet, slots, frame_hw, camera_matrix, pixel_format="bgr", idle_slots=False):
+    def __init__(self, mdet, slots, frame_hw, camera_matrix, pixel_format="bgr", idle_slots=False, distortion=None):
         from .detector import MultiCategoryDetector, MultiCategoryTracker
         if isinstance(mdet, MultiCategoryTracker):
             raise ValueError("MultiCategoryDetectGraph needs a MultiCategoryDetector; a MultiCategoryTracker runs "
@@ -419,4 +445,4 @@ class MultiCategoryDetectGraph(DetectGraph):
         if not isinstance(mdet, MultiCategoryDetector):
             raise NotImplementedError("MultiCategoryDetectGraph takes a MultiCategoryDetector; one category's "
                                       "ObjectPoseDetector goes to DetectGraph")
-        self._build(mdet, slots, frame_hw, camera_matrix, pixel_format, idle_slots)
+        self._build(mdet, slots, frame_hw, camera_matrix, pixel_format, idle_slots, distortion)

@@ -29,6 +29,9 @@ per-rank records are all-gathered (one NCCL call per batch, `dist.PoseBuffer`) b
 Both take `pixel_format="nv12"` or `"i420"` for YUV 4:2:0 frames as video decoders give them (uint8 [3H/2,W] per
 frame, H and W even): they are uploaded as they are, half the bytes of BGR, and converted inside the pre-process
 kernel; the results equal those of the same frames converted by cv2.cvtColor and submitted as BGR.
+
+Both take `distortion=` (lens.LensDistortion, one for every camera or one per frame / slot) for cameras with lens
+distortion: the frames are undistorted inside the pre-process exactly as run_batch(distortion=) does.
 """
 import collections
 
@@ -38,6 +41,7 @@ import torch
 from . import _lib
 from .dist import PoseBuffer, shard_range, slot_layout
 from .engine import check_pixel_format, frame_shape
+from .lens import slot_distortions
 
 
 class _Slot(object):
@@ -53,11 +57,12 @@ class _Slot(object):
 
 class BatchPipeline(object):
     """height, width: the image size of every frame; pixel_format "bgr" (frames uint8 [B,H,W,3]), "nv12" or "i420"
-    (uint8 [B,3H/2,W])."""
+    (uint8 [B,3H/2,W]); distortion: one LensDistortion for every frame, or a list of one per frame of a batch."""
 
     def __init__(self, det, batch, height, width, camera_matrix, world=1, depth=2, to_host=True, group=None,
-                 pixel_format="bgr"):
+                 pixel_format="bgr", distortion=None):
         self.pixel_format = check_pixel_format(pixel_format)
+        self.distortion = slot_distortions(distortion, int(batch), "BatchPipeline")
         shape = frame_shape(int(height), int(width), pixel_format)
         self.det, self.cam, self.depth, self.to_host, self.group = det, camera_matrix, int(depth), to_host, group
         self.device = torch.device(det.opt.device)
@@ -102,7 +107,7 @@ class BatchPipeline(object):
         if slot.used:
             compute.wait_event(slot.side_done)           # the slot's previous gather / download have read its records
         self.det.run_batch(slot.u8, self.cam, to_host=False, out=(slot.pbuf.poses, slot.pbuf.n_valid),
-                           pixel_format=self.pixel_format)
+                           pixel_format=self.pixel_format, distortion=self.distortion)
         slot.compute_done.record(compute)
         slot.used = True
         # the all-gather and the download run on a side stream: the next batch's kernels neither queue behind the copy nor
@@ -157,10 +162,13 @@ class TrackPipeline(object):
     (through pinned staging) on a copy stream while step i computes, and the track records of step i are read back one
     submit later.  With world > 1 (under torchrun) rank `rank` runs the slots shard_range(slots, rank, world) and one
     all-gather per step collects everyone's records (`dist.slot_layout`).  pixel_format "nv12" / "i420": every frame is
-    YUV 4:2:0, uint8 [3H/2,W]."""
+    YUV 4:2:0, uint8 [3H/2,W].  distortion: one LensDistortion for every slot, or a list of one per slot (None: an
+    undistorted camera); a camera changed by submit(camera_matrix=) gets its own map (built once, then cached)."""
 
-    def __init__(self, det, slots, camera_matrix, world=1, rank=0, depth=2, to_host=True, group=None, pixel_format="bgr"):
+    def __init__(self, det, slots, camera_matrix, world=1, rank=0, depth=2, to_host=True, group=None, pixel_format="bgr",
+                 distortion=None):
         self.pixel_format = check_pixel_format(pixel_format)
+        self.distortion = slot_distortions(distortion, int(slots), "TrackPipeline")
         self.det, self.depth, self.to_host, self.group = det, int(depth), to_host, group
         self.device = torch.device(det.opt.device)
         if self.device.type != "cuda":
@@ -236,7 +244,8 @@ class TrackPipeline(object):
             self.det.run_batch(dev_frames, self.cams[self.lo:self.hi], to_host=False, track=True,
                                out=(st.buf.poses[:n], st.buf.n_valid[:n]), new_video=self._local(new_video, "new_video"),
                                pre_dets=self._local(pre_dets, "pre_dets"), frame_ids=self._local(frame_ids, "frame_ids"),
-                               pixel_format=self.pixel_format)
+                               pixel_format=self.pixel_format,
+                               distortion=None if self.distortion is None else self.distortion[self.lo:self.hi])
         st.compute_done.record(compute)
         st.used = True
         with torch.cuda.stream(self.side_stream):

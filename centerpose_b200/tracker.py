@@ -388,17 +388,22 @@ class TrackGraph(_SlotGraph):
     returns zeros and launches nothing.  One step is captured per live count L = 1..S (the network runs at batch L, as
     in run_batch), so building costs S warm-up steps and S captures; a call is one copy per live frame, one copy of an
     int32 control block (start flags and the row / stream maps) and one graph launch.  Each slot's previous frame is
-    kept in a per-slot store that the pre-process exchanges in place."""
+    kept in a per-slot store that the pre-process exchanges in place.
+
+    distortion: the lens distortion of the cameras, one lens.LensDistortion for every slot or one per slot (None: an
+    undistorted camera), as run_batch(track=True, distortion=) takes it.  The maps and a frame table with them are
+    built with the graph, which then always pre-processes through the table; every step is bit for bit
+    run_batch(..., track=True, distortion=) on the same frames."""
 
     _host_step = "run_batch(track=True)"              # where what the graph refuses runs
     _host_list = "run_batch(list, track=True)"
 
-    def __init__(self, det, slots, frame_hw, camera_matrix, pixel_format="bgr", idle_slots=False):
+    def __init__(self, det, slots, frame_hw, camera_matrix, pixel_format="bgr", idle_slots=False, distortion=None):
         from .detector import ObjectPoseDetector
         if not isinstance(det, ObjectPoseDetector) or det._track_categories() is not None:
             raise NotImplementedError("TrackGraph tracks one category; several run through MultiCategoryTracker.run_batch "
                                       "or a MultiCategoryTrackGraph")
-        self._build(det, slots, frame_hw, camera_matrix, pixel_format, idle_slots)
+        self._build(det, slots, frame_hw, camera_matrix, pixel_format, idle_slots, distortion)
 
     def _refuse(self, opt, who):
         if not getattr(opt, "tracking_task", False):
@@ -527,7 +532,7 @@ class MultiCategoryTrackGraph(TrackGraph):
     _host_step = "MultiCategoryTracker.run_batch"
     _host_list = "MultiCategoryTracker.run_batch(list)"
 
-    def __init__(self, trk, slots, frame_hw, camera_matrix, pixel_format="bgr", idle_slots=False):
+    def __init__(self, trk, slots, frame_hw, camera_matrix, pixel_format="bgr", idle_slots=False, distortion=None):
         from .detector import MultiCategoryDetector, MultiCategoryTracker
         if not isinstance(trk, MultiCategoryTracker):
             if isinstance(trk, MultiCategoryDetector):
@@ -535,4 +540,4 @@ class MultiCategoryTrackGraph(TrackGraph):
                                  "tracking model")
             raise NotImplementedError("MultiCategoryTrackGraph takes a MultiCategoryTracker; one category's "
                                       "ObjectPoseDetector goes to TrackGraph")
-        self._build(trk, slots, frame_hw, camera_matrix, pixel_format, idle_slots)
+        self._build(trk, slots, frame_hw, camera_matrix, pixel_format, idle_slots, distortion)

@@ -675,7 +675,10 @@ enum cp_pixel_format {
   CP_PIX_YUYV422 = 32,   /* [H, W, 2], W even, Y0 U Y1 V per pixel pair (V4L2 YUYV, GStreamer YUY2): COLOR_YUV2BGR_YUYV */
   CP_PIX_UYVY422 = 33,   /* [H, W, 2], W even, U Y0 V Y1 per pixel pair (V4L2 / GStreamer UYVY): COLOR_YUV2BGR_UYVY */
   /* not a frame format: a launch over a table of per-frame formats (cp_preprocess_frame_table_formats) */
-  CP_PIX_PER_FRAME = 64
+  CP_PIX_PER_FRAME = 64,
+  /* not a frame format: OR-ed into a format or CP_PIX_PER_FRAME, the launch code of a table with coordinate maps
+   * (cp_preprocess_frame_table_maps) */
+  CP_PIX_REMAP = 128
 };
 /* cp_preprocess_ragged on YUV 4:2:0 frames: frame b is [src_hw[b][0] * 3 / 2, src_hw[b][1]] uint8 in `format`, i.e.
  * src_hw[b][0] * src_hw[b][1] * 3 / 2 bytes starting `offsets[b]` bytes into `frames`; src_hw holds the IMAGE sizes
@@ -745,6 +748,29 @@ int cp_preprocess_slots_ragged_dev(const uint8_t* frames, const void* table, int
 int cp_preprocess_frame_table_formats(int64_t frames_bytes, const int64_t* offsets, const int32_t* src_hw,
                                       const int32_t* formats, int32_t B, int32_t dst_h, int32_t dst_w,
                                       const double* trans_input, void* table, void* stream);
+/* Lens distortion: frames resampled through a coordinate map instead of an affine.  maps is a HOST array of B DEVICE
+ * pointers (8-byte aligned); maps[b] is float32 [dst_h, dst_w, 2], the (x, y) source position in frame b of every
+ * output pixel, e.g. cv2.initUndistortRectifyMap(K, D, None, [A; 0 0 1] @ K_new, (dst_w, dst_h), CV_32FC1) stacked on
+ * the last axis.  maps[b] NULL: frame b keeps its affine (trans_input[b], or its fix_res affine when trans_input is
+ * NULL).  A mapped frame's output is, bit for bit, cv2.remap(cv2.cvtColor(frame) to BGR, map x, map y, INTER_LINEAR,
+ * BORDER_CONSTANT, 0), then normalised as every pre-process; map entries that are NaN, +-inf or beyond the int range
+ * give the border value 0, as cv2.remap.  The caller owns the maps: they must hold their values and stay allocated
+ * until every launch that reads them has finished (for a table, as long as the table is launched).
+ *   - cp_preprocess_remap: cp_preprocess_formats with maps; the table is uploaded per call.
+ *   - cp_preprocess_frame_table_maps: a frame table of cp_preprocess_frame_table_bytes(B) bytes, built as
+ *     cp_preprocess_frame_table (format a cp_pixel_format, formats NULL) or cp_preprocess_frame_table_formats (format
+ *     CP_PIX_PER_FRAME, formats HOST int32 [B]), with the same checks.  Mapped and unmapped frames may share it.  It is
+ *     launched by cp_preprocess_slots_ragged_dev and cp_preprocess_slots_rows_dev with the launch code
+ *     format | CP_PIX_REMAP (and only so); an unmapped frame's output is then bit for bit that of the table without
+ *     maps.
+ * Null pointers, B <= 0, a format / formats pair other than those above, a map that is not 8-byte aligned and every
+ * check of the tables without maps return CP_ERR_INVALID before any work. */
+int cp_preprocess_remap(const uint8_t* frames, int64_t frames_bytes, const int64_t* offsets, const int32_t* src_hw,
+                        const int32_t* formats, const float* const* maps, float* out, int32_t B, int32_t dst_h,
+                        int32_t dst_w, const double* trans_input, const float mean[3], const float std[3], void* stream);
+int cp_preprocess_frame_table_maps(int64_t frames_bytes, const int64_t* offsets, const int32_t* src_hw, int32_t format,
+                                   const int32_t* formats, const float* const* maps, int32_t B, int32_t dst_h,
+                                   int32_t dst_w, const double* trans_input, void* table, void* stream);
 /* The pre-process of one tracking step in which only some of the S slots of a cp_preprocess_frame_table have a frame,
  * safe to capture in a CUDA graph.  Row n of the B live rows is slot rows[n]: out[n] (device fp32 [B,3,dst_h,dst_w]) is
  * bit for bit what cp_preprocess_slots_ragged_dev gives for that slot's frame.  rows (int32 [B]), start (int32 [S], per
