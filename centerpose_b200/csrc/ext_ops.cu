@@ -605,7 +605,8 @@ int cp_dcn_v2_forward_ex(const float* input, const float* weight, const float* b
     return fail(CP_ERR_INVALID, "cp_dcn_v2_forward: null argument");
   if (B <= 0 || C <= 0 || H <= 0 || W <= 0 || Co <= 0) return fail(CP_ERR_INVALID, "cp_dcn_v2_forward: bad shape");
   cudaStream_t s = (cudaStream_t)stream_;
-  const int Cp = round_up(C, 16);
+  // zero channels pad C to a whole K block of dcn_tma (16) and, in bf16, to the 32-channel span of a gather thread
+  const int Cp = round_up(C, precision == CP_PREC_BF16 ? 32 : 16);
   const int CoPad = conv_cout_pad(Co);
   const size_t npix = (size_t)B * H * W;
   const size_t n_x = npix * Cp, n_om = npix * 32, n_w = (size_t)9 * Cp * CoPad, n_b = CoPad;

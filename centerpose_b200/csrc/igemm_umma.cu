@@ -205,8 +205,8 @@ __global__ void __launch_bounds__(UM_THREADS, 1) igemm_umma_kernel(const IgemmPa
               for (int h4 = 0; h4 < F4; ++h4) {
                 const float4 c1 = ld[qi][0 * F4 + h4], c2 = ld[qi][1 * F4 + h4], c3 = ld[qi][2 * F4 + h4],
                              c4 = ld[qi][3 * F4 + h4];
-                // NOTE: w1..w4 / mk belong to the tap of the LAST chunk decoded above; chunks of one thread share a
-                // tap whenever Cin is a multiple of the thread's 4-chunk span (all DCN layers: Cin % 64 == 0)
+                // w1..w4 / mk belong to the tap of the LAST chunk decoded above: the chunks of one thread share a
+                // tap because umma_supported requires Cin to be a multiple of the thread's 4-chunk span
                 v[h4 * 4 + 0] = (w1 * c1.x + w2 * c2.x + w3 * c3.x + w4 * c4.x) * mk;
                 v[h4 * 4 + 1] = (w1 * c1.y + w2 * c2.y + w3 * c3.y + w4 * c4.y) * mk;
                 v[h4 * 4 + 2] = (w1 * c1.z + w2 * c2.z + w3 * c3.z + w4 * c4.z) * mk;
@@ -355,6 +355,8 @@ bool umma_supported(const IgemmParams& p, int prec) {
     return false;
   const int ch = prec == 0 ? 8 : 4;
   if (p.Cin % ch) return false;
+  // DCN: a gather thread blends its four chunks with the sampling weights of one tap, so they must not straddle two
+  if (p.mode == IGEMM_DCN && p.Cin % (4 * ch)) return false;
   for (int s = 0; s < p.nsrc; ++s)
     if (p.srcC[s] % ch || p.srcStride[s] % 4) return false;
   return umma_tile_n(p.CoutPad, prec) != 0;
