@@ -70,11 +70,17 @@ EXPORTS = [
 # OR-ed into either launches a table with coordinate maps (cp_preprocess_frame_table_maps).
 CP_PIX_NV12, CP_PIX_I420, CP_PIX_BGR = 0, 1, 2
 CP_PIX_RGB24, CP_PIX_RGBA, CP_PIX_BGRA, CP_PIX_YUYV422, CP_PIX_UYVY422 = 16, 17, 18, 32, 33
+CP_PIX_GRAY, CP_PIX_BAYER_RGGB8, CP_PIX_BAYER_BGGR8, CP_PIX_BAYER_GBRG8, CP_PIX_BAYER_GRBG8 = 48, 49, 50, 51, 52
 CP_PIX_PER_FRAME = 64
 CP_PIX_REMAP = 128
+# the colour formats, and the sensor formats: one uint8 [H,W] plane per frame, mono or a Bayer mosaic named after its
+# pixels (0,0) (0,1) / (1,0) (1,1) as ffmpeg, V4L2 and ROS name it
 PIXEL_FORMATS = ("bgr", "nv12", "i420", "rgb24", "rgba", "bgra", "yuyv422", "uyvy422")
+SENSOR_FORMATS = ("gray", "bayer_rggb8", "bayer_bggr8", "bayer_gbrg8", "bayer_grbg8")
 PIXEL_FORMAT_CODES = {"bgr": CP_PIX_BGR, "nv12": CP_PIX_NV12, "i420": CP_PIX_I420, "rgb24": CP_PIX_RGB24,
-                      "rgba": CP_PIX_RGBA, "bgra": CP_PIX_BGRA, "yuyv422": CP_PIX_YUYV422, "uyvy422": CP_PIX_UYVY422}
+                      "rgba": CP_PIX_RGBA, "bgra": CP_PIX_BGRA, "yuyv422": CP_PIX_YUYV422, "uyvy422": CP_PIX_UYVY422,
+                      "gray": CP_PIX_GRAY, "bayer_rggb8": CP_PIX_BAYER_RGGB8, "bayer_bggr8": CP_PIX_BAYER_BGGR8,
+                      "bayer_gbrg8": CP_PIX_BAYER_GBRG8, "bayer_grbg8": CP_PIX_BAYER_GRBG8}
 
 # cp_plan_create_ex / cp_plan_memory flags
 CP_PLAN_REUSE_ACTIVATIONS = 1

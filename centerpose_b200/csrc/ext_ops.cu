@@ -6,7 +6,8 @@
 //                        (reference: detectors/base_detector.py:91-148, fix_res branch); cp_preprocess_ragged does
 //                        the same for frames of different sizes in one launch, and cp_preprocess_yuv420 for NV12 / I420
 //                        frames (the colour conversion of cv2.cvtColor fused into the warp's tap fetch), and
-//                        cp_preprocess_formats for the camera formats (RGB24, RGBA, BGRA, YUYV, UYVY), one per frame;
+//                        cp_preprocess_formats for the camera formats (RGB24, RGBA, BGRA, YUYV, UYVY, gray and the
+//                        Bayer mosaics), one per frame;
 //                        cp_preprocess_slots_dev is the graph-safe form for one tracking step of a uniform batch, and
 //                        cp_preprocess_slots_ragged_dev (over a cp_preprocess_frame_table) that of slots of mixed sizes,
 //                        cp_preprocess_slots_rows_dev that of the live slots of a step with idle slots (a table may hold
@@ -161,12 +162,70 @@ struct YuvFetch {
   }
 };
 
+// Bayer mosaics [sh, sw] (sh, sw >= 3) demosaiced per tap to the BGR that cv2.cvtColor's bilinear COLOR_Bayer??2BGR
+// gives, restated bit for bit (tests/bayer_ref.py, pinned against cv2).  The four patterns are one fetch with a phase
+// (py, px): pixel (y, x) of the frame's pattern is pixel (y + py, x + px) of R G / G B, so rggb is (0, 0), grbg (0, 1),
+// gbrg (1, 0) and bggr (1, 1).  An interior pixel keeps its own channel and takes
+//   at R or B: G = (N + S + W + E + 2) >> 2, the other chroma = (NW + NE + SW + SE + 2) >> 2;
+//   at G: the chroma of its row's other sites = (W + E + 1) >> 1, that of its column's = (N + S + 1) >> 1;
+// and an in-frame border pixel (y, x) takes the BGR of interior pixel (clamp(y, 1, sh - 2), clamp(x, 1, sw - 2)).
+// The clamped 3 x 3 neighbourhoods of the four taps lie in one window of at most 4 x 4 bytes, read once; every in-frame
+// tap is demosaiced from it before the first channel is written, taps outside stay BGR 0.
+struct BayerFetch {
+  const uint8_t* __restrict__ img;
+  int sh, sw;
+  int py, px;
+  int b[4], g[4], r[4];
+  __device__ __forceinline__ void taps(int iy, int ix, bool in00, bool in01, bool in10, bool in11) {
+    const bool in[4] = {in00, in01, in10, in11};
+#pragma unroll
+    for (int k = 0; k < 4; ++k) b[k] = g[k] = r[k] = 0;
+    if (!(in00 || in01 || in10 || in11)) return;
+    // the clamped centres of the tap rows and columns; the window starts one row and column before the first
+    const int cy0 = max(1, min(sh - 2, iy)), cy1 = max(1, min(sh - 2, iy + 1));
+    const int cx0 = max(1, min(sw - 2, ix)), cx1 = max(1, min(sw - 2, ix + 1));
+    const int r0 = cy0 - 1, c0 = cx0 - 1;
+    // rows r0 .. r0 + 3, bytes c0 .. c0 + 3 (byte j of a word is column c0 + j); the fourth row and column are needed
+    // only where they are in the frame, so their reads are clamped into it
+    uint32_t win[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const uint8_t* __restrict__ row = img + (size_t)min(r0 + j, sh - 1) * sw + c0;
+      win[j] = row[0] | (uint32_t)row[1] << 8 | (uint32_t)row[2] << 16 | (uint32_t)row[min(3, sw - 1 - c0)] << 24;
+    }
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      if (!in[k]) continue;
+      const int cy = k >> 1 ? cy1 : cy0, cx = k & 1 ? cx1 : cx0;
+      const bool down = cy != cy0;                     // the neighbourhood's rows are window rows 1..3, else 0..2
+      const int sh8 = 8 * (cx - c0 - 1);               // and its columns start at byte cx - c0 - 1
+      const uint32_t N = (down ? win[1] : win[0]) >> sh8, C = (down ? win[2] : win[1]) >> sh8,
+                     S = (down ? win[3] : win[2]) >> sh8;
+      const int n_w = N & 255, n = N >> 8 & 255, n_e = N >> 16 & 255, w = C & 255, c = C >> 8 & 255, e = C >> 16 & 255,
+                s_w = S & 255, s = S >> 8 & 255, s_e = S >> 16 & 255;
+      const bool even_row = ((cy + py) & 1) == 0, chroma = ((cy + py + cx + px) & 1) == 0;
+      // own: the chroma of the row's colour (R on an R G row), other: the other chroma
+      const int own = chroma ? c : (w + e + 1) >> 1;
+      const int other = chroma ? (n_w + n_e + s_w + s_e + 2) >> 2 : (n + s + 1) >> 1;
+      g[k] = chroma ? (n + s + w + e + 2) >> 2 : c;
+      r[k] = even_row ? own : other;
+      b[k] = even_row ? other : own;
+    }
+  }
+  __device__ __forceinline__ int operator()(int k, int, int, int c) const { return c == 0 ? b[k] : (c == 1 ? g[k] : r[k]); }
+};
+__device__ __forceinline__ BayerFetch bayer_fetch(const uint8_t* __restrict__ img, int sh, int sw, int format) {
+  return BayerFetch{img, sh, sw, format == CP_PIX_BAYER_BGGR8 || format == CP_PIX_BAYER_GBRG8,
+                    format == CP_PIX_BAYER_BGGR8 || format == CP_PIX_BAYER_GRBG8};
+}
+
 // The bytes of one sh x sw frame in a cp_pixel_format (0 for CP_PIX_PER_FRAME or an unknown value).
 __host__ __device__ constexpr size_t frame_bytes(int format, size_t sh, size_t sw) {
   return format == CP_PIX_NV12 || format == CP_PIX_I420     ? sh * sw * 3 / 2
          : format == CP_PIX_BGR || format == CP_PIX_RGB24    ? sh * sw * 3
          : format == CP_PIX_RGBA || format == CP_PIX_BGRA    ? sh * sw * 4
          : format == CP_PIX_YUYV422 || format == CP_PIX_UYVY422 ? sh * sw * 2
+         : format >= CP_PIX_GRAY && format <= CP_PIX_BAYER_GRBG8 ? sh * sw
                                                              : 0;
 }
 
@@ -177,6 +236,10 @@ __device__ __forceinline__ auto make_fetch(const uint8_t* __restrict__ img, int 
     return PackedFetch<kFormat == CP_PIX_BGR ? 3 : 4, 0, 1, 2>{img, sw};
   else if constexpr (kFormat == CP_PIX_RGB24 || kFormat == CP_PIX_RGBA)
     return PackedFetch<kFormat == CP_PIX_RGB24 ? 3 : 4, 2, 1, 0>{img, sw};
+  else if constexpr (kFormat == CP_PIX_GRAY)
+    return PackedFetch<1, 0, 0, 0>{img, sw};           // COLOR_GRAY2BGR: B = G = R = Y
+  else if constexpr (kFormat >= CP_PIX_BAYER_RGGB8 && kFormat <= CP_PIX_BAYER_GRBG8)
+    return bayer_fetch(img, sh, sw, kFormat);
   else
     return YuvFetch<kFormat>{img, sh, sw};
 }
@@ -211,7 +274,8 @@ __device__ __forceinline__ void frame_walk(const uint8_t* __restrict__ frames, c
     walk(make_fetch<kFormat>(frames + (kRemap ? f.offset & kOffsetMask : f.offset), f.sh, f.sw));
   } else {
     const uint8_t* img = frames + (f.offset & kOffsetMask);
-    switch (kRemap ? (int)((f.offset & ~kMappedFlag) >> kFormatShift) : (int)(f.offset >> kFormatShift)) {
+    const int format = kRemap ? (int)((f.offset & ~kMappedFlag) >> kFormatShift) : (int)(f.offset >> kFormatShift);
+    switch (format) {
       case CP_PIX_NV12: walk(make_fetch<CP_PIX_NV12>(img, f.sh, f.sw)); break;
       case CP_PIX_I420: walk(make_fetch<CP_PIX_I420>(img, f.sh, f.sw)); break;
       case CP_PIX_BGR: walk(make_fetch<CP_PIX_BGR>(img, f.sh, f.sw)); break;
@@ -219,7 +283,13 @@ __device__ __forceinline__ void frame_walk(const uint8_t* __restrict__ frames, c
       case CP_PIX_RGBA: walk(make_fetch<CP_PIX_RGBA>(img, f.sh, f.sw)); break;
       case CP_PIX_BGRA: walk(make_fetch<CP_PIX_BGRA>(img, f.sh, f.sw)); break;
       case CP_PIX_YUYV422: walk(make_fetch<CP_PIX_YUYV422>(img, f.sh, f.sw)); break;
-      default: walk(make_fetch<CP_PIX_UYVY422>(img, f.sh, f.sw)); break;
+      case CP_PIX_UYVY422: walk(make_fetch<CP_PIX_UYVY422>(img, f.sh, f.sw)); break;
+      case CP_PIX_GRAY: walk(make_fetch<CP_PIX_GRAY>(img, f.sh, f.sw)); break;
+      case CP_PIX_BAYER_RGGB8:
+      case CP_PIX_BAYER_BGGR8:
+      case CP_PIX_BAYER_GBRG8:
+      case CP_PIX_BAYER_GRBG8: walk(bayer_fetch(img, f.sh, f.sw, format)); break;   // one walk, the phase at run time
+      default: break;                                  // no table the host builds holds another value
     }
   }
 }
@@ -349,9 +419,10 @@ int preprocess_blocks(size_t total) {
 
 bool is_yuv420(int format) { return format == CP_PIX_NV12 || format == CP_PIX_I420; }
 bool is_yuv422(int format) { return format == CP_PIX_YUYV422 || format == CP_PIX_UYVY422; }
+bool is_bayer(int format) { return format >= CP_PIX_BAYER_RGGB8 && format <= CP_PIX_BAYER_GRBG8; }
 bool known_format(int format) {
   return format == CP_PIX_BGR || is_yuv420(format) || format == CP_PIX_RGB24 || format == CP_PIX_RGBA ||
-         format == CP_PIX_BGRA || is_yuv422(format);
+         format == CP_PIX_BGRA || is_yuv422(format) || format == CP_PIX_GRAY || is_bayer(format);
 }
 
 // a launch code of a frame table: a cp_pixel_format or CP_PIX_PER_FRAME, either with or without CP_PIX_REMAP
@@ -373,6 +444,11 @@ void with_base_format(int format, F f) {
     case CP_PIX_BGRA: f(std::integral_constant<int, CP_PIX_BGRA>{}); break;
     case CP_PIX_YUYV422: f(std::integral_constant<int, CP_PIX_YUYV422>{}); break;
     case CP_PIX_UYVY422: f(std::integral_constant<int, CP_PIX_UYVY422>{}); break;
+    case CP_PIX_GRAY: f(std::integral_constant<int, CP_PIX_GRAY>{}); break;
+    case CP_PIX_BAYER_RGGB8: f(std::integral_constant<int, CP_PIX_BAYER_RGGB8>{}); break;
+    case CP_PIX_BAYER_BGGR8: f(std::integral_constant<int, CP_PIX_BAYER_BGGR8>{}); break;
+    case CP_PIX_BAYER_GBRG8: f(std::integral_constant<int, CP_PIX_BAYER_GBRG8>{}); break;
+    case CP_PIX_BAYER_GRBG8: f(std::integral_constant<int, CP_PIX_BAYER_GRBG8>{}); break;
     default: f(std::integral_constant<int, CP_PIX_PER_FRAME>{});
   }
 }
@@ -452,10 +528,12 @@ int ragged_frames(const char* who, int64_t frames_bytes, const int64_t* offsets,
       return fail(CP_ERR_INVALID, w0 + ": frame " + std::to_string(b) + " has unknown pixel format " +
                                       std::to_string(fmt));
     const bool yuv = is_yuv420(fmt);
-    if (h <= 0 || w <= 0 || (yuv && (h % 2 || w % 2)) || (is_yuv422(fmt) && w % 2))
+    if (h <= 0 || w <= 0 || (yuv && (h % 2 || w % 2)) || (is_yuv422(fmt) && w % 2) ||
+        (is_bayer(fmt) && (h < 3 || w < 3)))
       return fail(CP_ERR_INVALID, w0 + ": frame " + std::to_string(b) + " has size " + std::to_string(h) + " x " +
                                       std::to_string(w) + (yuv ? " (YUV 4:2:0 needs even sizes)"
-                                                               : is_yuv422(fmt) ? " (YUV 4:2:2 needs an even width)" : ""));
+                                                           : is_yuv422(fmt) ? " (YUV 4:2:2 needs an even width)"
+                                                           : is_bayer(fmt) ? " (a Bayer mosaic needs at least 3 x 3)" : ""));
     const int64_t bytes = (int64_t)frame_bytes(fmt, h, w);
     if (offsets[b] < 0 || offsets[b] > frames_bytes || bytes > frames_bytes - offsets[b])
       return fail(CP_ERR_INVALID, w0 + ": frame " + std::to_string(b) + " (" + std::to_string(h) + " x " +
@@ -754,6 +832,9 @@ int cp_preprocess_slots_dev(const uint8_t* frames, int32_t format, int32_t B, in
                                     std::to_string(src_h) + " x " + std::to_string(src_w));
   if (is_yuv422(format) && src_w % 2)
     return fail(CP_ERR_INVALID, "cp_preprocess_slots_dev: YUV 4:2:2 frames need an even width, got " +
+                                    std::to_string(src_h) + " x " + std::to_string(src_w));
+  if (is_bayer(format) && (src_h < 3 || src_w < 3))
+    return fail(CP_ERR_INVALID, "cp_preprocess_slots_dev: Bayer mosaics need at least 3 x 3, got " +
                                     std::to_string(src_h) + " x " + std::to_string(src_w));
   double T[6];
   if (trans_input)

@@ -578,7 +578,10 @@ class ObjectPoseDetector(object):
         result equals, bit for bit, that of the same call on cv2.cvtColor(frame, COLOR_YUV2BGR_NV12 / _I420).  c, s and
         the meta rows come from the image size (H, W).  The camera formats "rgb24" (uint8 [B,H,W,3]), "rgba" / "bgra"
         ([B,H,W,4]) and "yuyv422" / "uyvy422" ([B,H,W,2], W even) are converted the same way, each bit for bit its
-        cv2.cvtColor to BGR (COLOR_RGB2BGR, _RGBA2BGR, _BGRA2BGR, COLOR_YUV2BGR_YUYV, _UYVY).  With a list of frames,
+        cv2.cvtColor to BGR (COLOR_RGB2BGR, _RGBA2BGR, _BGRA2BGR, COLOR_YUV2BGR_YUYV, _UYVY).  So are the sensor
+        formats, one uint8 plane per frame ([B,H,W] or a list of [H_b,W_b]): "gray" (COLOR_GRAY2BGR) and the Bayer
+        mosaics "bayer_rggb8" / "bayer_bggr8" / "bayer_gbrg8" / "bayer_grbg8" (H and W at least 3), named after their
+        top-left 2 x 2 block and demosaiced as cv2's bilinear COLOR_BayerBG2BGR / _RG / _GR / _GB.  With a list of frames,
         pixel_format may also be a list of one name per frame or slot (cameras of different kinds); a list of one name
         repeated is that name.
 
@@ -989,8 +992,8 @@ class MultiCategoryTracker(MultiCategoryDetector):
         slot list of meta['pre_dets'] lists (None = that slot is not seeded); frame_ids: per slot meta['id'].
         Returns (tracks [M,S,T,320], n_tracks [M,S]) in `categories` order (idle slots: n_tracks 0, zero rows), on the
         host when `to_host`; out: optional (tracks, n_tracks) CUDA tensors of those shapes to write into.
-        pixel_format "nv12" / "i420": YUV 4:2:0 frames, uint8 [S,3H/2,W] or [3H_s/2,W_s]; the camera formats and one name
-        per slot with a list of frames, and distortion (one LensDistortion, or one per slot), as in
+        pixel_format "nv12" / "i420": YUV 4:2:0 frames, uint8 [S,3H/2,W] or [3H_s/2,W_s]; the camera and sensor
+        formats, one name per slot with a list of frames, and distortion (one LensDistortion, or one per slot), as in
         ObjectPoseDetector.run_batch."""
         if isinstance(frames, (list, tuple)):
             return self._run_slots(frames, camera_matrix, to_host, out, pre_dets, frame_ids, new_video, pixel_format,

@@ -546,22 +546,32 @@ def preprocess_ragged(packed_u8, offsets, src_hw, dst_h, dst_w, mean, std, out=N
 
 
 _YUV420 = {"nv12": _lib.CP_PIX_NV12, "i420": _lib.CP_PIX_I420}
-# the buffer of one H x W image in each pixel_format: [3H/2,W] for YUV 4:2:0, else [H,W,C]
-_LAYOUT = {"bgr": "[H,W,3]", "nv12": "[3H/2,W]", "i420": "[3H/2,W]", "rgb24": "[H,W,3]", "rgba": "[H,W,4]",
-           "bgra": "[H,W,4]", "yuyv422": "[H,W,2]", "uyvy422": "[H,W,2]"}
+# the buffer of one H x W image in each pixel_format: [3H/2,W] for YUV 4:2:0, [H,W] for the sensor formats, else
+# [H,W,C]
+_LAYOUT = dict({"bgr": "[H,W,3]", "nv12": "[3H/2,W]", "i420": "[3H/2,W]", "rgb24": "[H,W,3]", "rgba": "[H,W,4]",
+                "bgra": "[H,W,4]", "yuyv422": "[H,W,2]", "uyvy422": "[H,W,2]"},
+               **{f: "[H,W]" for f in _lib.SENSOR_FORMATS})
 _CHANNELS = {"bgr": 3, "rgb24": 3, "rgba": 4, "bgra": 4, "yuyv422": 2, "uyvy422": 2}
+_ALL_FORMATS = _lib.PIXEL_FORMATS + _lib.SENSOR_FORMATS
+
+
+def _min_side(pixel_format):
+    """The least height and width of a frame in a sensor format: a Bayer mosaic's demosaic needs 3 x 3 pixels."""
+    return 3 if pixel_format.startswith("bayer_") else 1
 
 
 def check_pixel_format(pixel_format):
     """pixel_format (cp_pixel_format): "bgr" (uint8 [H,W,3], cv2.imread's), "nv12" or "i420" (uint8 [3H/2,W], H and W
-    even), or a camera format named as ffmpeg's pix_fmt: "rgb24" ([H,W,3]), "rgba" / "bgra" ([H,W,4], alpha ignored),
-    "yuyv422" / "uyvy422" ([H,W,2] packed YUV 4:2:2, W even).  One name; a list (one per camera) goes through
-    slot_formats where frames come as a list."""
+    even), a camera format named as ffmpeg's pix_fmt: "rgb24" ([H,W,3]), "rgba" / "bgra" ([H,W,4], alpha ignored),
+    "yuyv422" / "uyvy422" ([H,W,2] packed YUV 4:2:2, W even), or a sensor format, one [H,W] plane: "gray" (mono) or a
+    Bayer mosaic "bayer_rggb8" / "bayer_bggr8" / "bayer_gbrg8" / "bayer_grbg8" (H and W at least 3), demosaiced as
+    cv2's bilinear COLOR_Bayer??2BGR.  One name; a list (one per camera) goes through slot_formats where frames come as
+    a list."""
     if isinstance(pixel_format, (list, tuple)):
         raise ValueError("pixel_format must be one name here, got a list %r; one name per camera goes with a list of "
                          "frames (run_batch(list), a graph built with one frame_hw per slot)" % (list(pixel_format),))
-    if pixel_format not in _lib.PIXEL_FORMATS:
-        raise ValueError("pixel_format must be one of %s, got %r" % (", ".join(_lib.PIXEL_FORMATS), pixel_format))
+    if pixel_format not in _ALL_FORMATS:
+        raise ValueError("pixel_format must be one of %s, got %r" % (", ".join(_ALL_FORMATS), pixel_format))
     return pixel_format
 
 
@@ -573,9 +583,9 @@ def slot_formats(pixel_format, n, who="run_batch"):
         raise ValueError("%s: pixel_format is one name or one per frame, got %d names for %d frames"
                          % (who, len(pixel_format), n))
     for f in pixel_format:
-        if isinstance(f, (list, tuple)) or f not in _lib.PIXEL_FORMATS:
+        if isinstance(f, (list, tuple)) or f not in _ALL_FORMATS:
             raise ValueError("pixel_format must be one of %s, got %r in %r"
-                             % (", ".join(_lib.PIXEL_FORMATS), f, list(pixel_format)))
+                             % (", ".join(_ALL_FORMATS), f, list(pixel_format)))
     return list(pixel_format)
 
 
@@ -586,8 +596,14 @@ def frame_layout(pixel_format):
 
 def frame_shape(h, w, pixel_format):
     """The buffer shape of one h x w image in pixel_format: [h,w,3] for "bgr" / "rgb24", [h,w,4] for "rgba" / "bgra",
-    [h,w,2] for "yuyv422" / "uyvy422" (w even), [3h/2,w] for "nv12" / "i420" (h and w even); else ValueError."""
-    c = _CHANNELS.get(check_pixel_format(pixel_format))
+    [h,w,2] for "yuyv422" / "uyvy422" (w even), [3h/2,w] for "nv12" / "i420" (h and w even), [h,w] for "gray" and the
+    Bayer mosaics (h and w at least 3); else ValueError."""
+    if check_pixel_format(pixel_format) in _lib.SENSOR_FORMATS:
+        m = _min_side(pixel_format)
+        if h < m or w < m:
+            raise ValueError("%s frames need at least %d x %d pixels; got %d x %d" % (pixel_format, m, m, h, w))
+        return (int(h), int(w))
+    c = _CHANNELS.get(pixel_format)
     if c is not None:
         if c == 2 and (w % 2 or h < 1 or w < 2):
             raise ValueError("%s frames need an even, positive width; got %d x %d" % (pixel_format, h, w))
@@ -601,7 +617,13 @@ def image_size(shape, pixel_format, what="frame"):
     """(H, W) of the image a buffer of `shape` holds in pixel_format; ValueError (naming the expected shape) when the
     shape is not one of that format."""
     shape = tuple(int(v) for v in shape)
-    c = _CHANNELS.get(check_pixel_format(pixel_format))
+    if check_pixel_format(pixel_format) in _lib.SENSOR_FORMATS:
+        m = _min_side(pixel_format)
+        if len(shape) != 2 or shape[0] < m or shape[1] < m:
+            raise ValueError("%s has shape %s, expected a %s frame [H,W]%s" % (what, shape, pixel_format,
+                                                                              " with H and W at least 3" if m > 1 else ""))
+        return shape
+    c = _CHANNELS.get(pixel_format)
     if c is not None:
         if len(shape) != 3 or shape[2] != c or shape[0] < 1 or shape[1] < 1 or (c == 2 and shape[1] % 2):
             raise ValueError("%s has shape %s, expected %s[H,W,%d]%s" % (what, shape, "" if c == 3 else "a %s frame "

@@ -343,7 +343,8 @@ class DetectGraph(_SlotGraph):
     MultiCategoryDetectGraph.
 
     frame_hw, camera_matrix, pixel_format and the frames of a call are those of TrackGraph: one (H, W) for every slot
-    (frames uint8 [S,H,W,3], or [S,3H/2,W] for "nv12" / "i420", [S,H,W,C] for a camera format) or a list of S sizes (a
+    (frames uint8 [S,H,W,3], or [S,3H/2,W] for "nv12" / "i420", [S,H,W,C] for a camera format, [S,H,W] for "gray" and
+    the Bayer mosaics) or a list of S sizes (a
     list of S frames, packed into one device buffer and pre-processed through a frame table built now; pixel_format may
     then be a list of one name per slot); [3,3] or [S,3,3] cameras.  Frames may be in pinned host memory (keep them
     unchanged until the step's outputs are read) or on the device.

@@ -28,7 +28,9 @@ per-rank records are all-gathered (one NCCL call per batch, `dist.PoseBuffer`) b
 
 Both take `pixel_format="nv12"` or `"i420"` for YUV 4:2:0 frames as video decoders give them (uint8 [3H/2,W] per
 frame, H and W even): they are uploaded as they are, half the bytes of BGR, and converted inside the pre-process
-kernel; the results equal those of the same frames converted by cv2.cvtColor and submitted as BGR.
+kernel; the results equal those of the same frames converted by cv2.cvtColor and submitted as BGR.  The camera and
+sensor formats of engine.check_pixel_format work the same way; a Bayer mosaic or "gray" frame is uint8 [H,W], a third
+of the bytes of BGR.
 
 Both take `distortion=` (lens.LensDistortion, one for every camera or one per frame / slot) for cameras with lens
 distortion: the frames are undistorted inside the pre-process exactly as run_batch(distortion=) does.

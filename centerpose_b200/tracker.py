@@ -370,8 +370,9 @@ class TrackGraph(_SlotGraph):
 
     frame_hw: one (H, W) for every slot, or a list of S (H_s, W_s).  camera_matrix: [3,3] for every slot or [S,3,3].
       - One size: a call takes the frames as one array, uint8 [S,H,W,3] for pixel_format "bgr", [S,3H/2,W] for "nv12" /
-        "i420" (H, W even), [S,H,W,C] for a camera format ("rgb24", "rgba", "bgra", "yuyv422", "uyvy422"); one copy
-        and the uniform pre-process (cp_preprocess_slots_dev).
+        "i420" (H, W even), [S,H,W,C] for a camera format ("rgb24", "rgba", "bgra", "yuyv422", "uyvy422"), [S,H,W] for
+        a sensor format ("gray", "bayer_rggb8", "bayer_bggr8", "bayer_gbrg8", "bayer_grbg8"); one copy and the uniform
+        pre-process (cp_preprocess_slots_dev).
       - One size per slot: a call takes a list of S frames, uint8 [H_s,W_s,3] or [3H_s/2,W_s] (...), each copied into
         its own region of one packed device buffer; the step is that of run_batch(list, track=True) with every slot
         present, the pre-process reading a frame table built once now (cp_preprocess_slots_ragged_dev).  pixel_format

@@ -674,6 +674,15 @@ enum cp_pixel_format {
   CP_PIX_BGRA = 18,      /* [H, W, 4] B G R A, alpha ignored: COLOR_BGRA2BGR */
   CP_PIX_YUYV422 = 32,   /* [H, W, 2], W even, Y0 U Y1 V per pixel pair (V4L2 YUYV, GStreamer YUY2): COLOR_YUV2BGR_YUYV */
   CP_PIX_UYVY422 = 33,   /* [H, W, 2], W even, U Y0 V Y1 per pixel pair (V4L2 / GStreamer UYVY): COLOR_YUV2BGR_UYVY */
+  /* Sensor formats: one uint8 [H, W] plane per frame.  A Bayer mosaic is named after its pixels (0,0) (0,1) / (1,0)
+   * (1,1) as ffmpeg, V4L2 and ROS name it; cv2 names the same mosaic after the block at (1,1), so the codes cross.  The
+   * demosaic is cv2's bilinear one (an in-frame border pixel takes the BGR of the nearest interior pixel); a mosaic needs
+   * at least 3 x 3 pixels (cv2 gives a black image below that; these refuse it). */
+  CP_PIX_GRAY = 48,          /* Y (ROS mono8, V4L2 GREY, GStreamer GRAY8): COLOR_GRAY2BGR, B = G = R = Y */
+  CP_PIX_BAYER_RGGB8 = 49,   /* R G / G B (V4L2 RGGB): COLOR_BayerBG2BGR */
+  CP_PIX_BAYER_BGGR8 = 50,   /* B G / G R (V4L2 BA81): COLOR_BayerRG2BGR */
+  CP_PIX_BAYER_GBRG8 = 51,   /* G B / R G (V4L2 GBRG): COLOR_BayerGR2BGR */
+  CP_PIX_BAYER_GRBG8 = 52,   /* G R / B G (V4L2 GRBG): COLOR_BayerGB2BGR */
   /* not a frame format: a launch over a table of per-frame formats (cp_preprocess_frame_table_formats) */
   CP_PIX_PER_FRAME = 64,
   /* not a frame format: OR-ed into a format or CP_PIX_PER_FRAME, the launch code of a table with coordinate maps
@@ -693,24 +702,25 @@ int cp_preprocess_yuv420(const uint8_t* frames, int64_t frames_bytes, const int6
                          const float mean[3], const float std[3], void* stream);
 /* cp_preprocess_ragged with one pixel format per frame: frame b is in formats[b] (HOST int32 [B], any cp_pixel_format
  * but CP_PIX_PER_FRAME), its buffer shape given by that format and the image size src_hw[b] = (H, W) (4:2:0: both even;
- * 4:2:2: W even).  Frame b's output equals, bit for bit, cp_preprocess_ragged on cv2.cvtColor(frame) to BGR with the
- * same trans_input (NULL: each frame's fix_res affine).  One launch: one format's walk when every frame has it, else a
- * walk that reads each frame's format from the per-frame parameters.  An unknown format, a size its format cannot have
- * or a frame that does not fit inside frames_bytes at its format's size returns CP_ERR_INVALID before any work is
- * enqueued. */
+ * 4:2:2: W even; a Bayer mosaic: both at least 3).  Frame b's output equals, bit for bit, cp_preprocess_ragged on
+ * cv2.cvtColor(frame) to BGR with the same trans_input (NULL: each frame's fix_res affine).  One launch: one format's
+ * walk when every frame has it, else a walk that reads each frame's format from the per-frame parameters.  An unknown
+ * format, a size its format cannot have or a frame that does not fit inside frames_bytes at its format's size returns
+ * CP_ERR_INVALID before any work is enqueued. */
 int cp_preprocess_formats(const uint8_t* frames, int64_t frames_bytes, const int64_t* offsets, const int32_t* src_hw,
                           const int32_t* formats, float* out, int32_t B, int32_t dst_h, int32_t dst_w,
                           const double* trans_input, const float mean[3], const float std[3], void* stream);
 
 /* The pre-process of one tracking step of B video slots, safe to capture in a CUDA graph: it reads no host memory and
- * allocates nothing once enqueued, so a replay runs it with the arguments it was captured with.  frames: device uint8,
- * B frames of one image size (src_h, src_w) in `format` (cp_pixel_format; YUV 4:2:0 needs an even size), frame b at byte
- * b * (bytes of one frame).  trans_input: HOST row-major 2x3 forward affine for every frame, read before the call
- * returns (NULL: the fix_res affine of the size, as cp_preprocess).  out: device fp32 [B,3,dst_h,dst_w], frame b bit for
- * bit what cp_preprocess_affine (BGR), cp_preprocess_yuv420 (NV12 / I420) or cp_preprocess_formats gives for it.  start: device int32 [B] read
- * when the kernel runs, or NULL; where start[b] != 0 frame b's output is written to prev[b] (device fp32
- * [B,3,dst_h,dst_w]) as well: a slot whose video starts with this frame takes it as its previous frame.  start and prev
- * are both given or both NULL.  Bad arguments return CP_ERR_INVALID before any work is enqueued. */
+ * allocates nothing once enqueued, so a replay runs it with the arguments it was captured with.  frames: device uint8, B
+ * frames of one image size (src_h, src_w) in `format` (cp_pixel_format; YUV 4:2:0 needs an even size, a Bayer mosaic at
+ * least 3 x 3), frame b at byte b * (bytes of one frame).  trans_input: HOST row-major 2x3 forward affine for every
+ * frame, read before the call returns (NULL: the fix_res affine of the size, as cp_preprocess).  out: device fp32
+ * [B,3,dst_h,dst_w], frame b bit for bit what cp_preprocess_affine (BGR), cp_preprocess_yuv420 (NV12 / I420) or
+ * cp_preprocess_formats gives for it.  start: device int32 [B] read when the kernel runs, or NULL; where start[b] != 0
+ * frame b's output is written to prev[b] (device fp32 [B,3,dst_h,dst_w]) as well: a slot whose video starts with this
+ * frame takes it as its previous frame.  start and prev are both given or both NULL.  Bad arguments return CP_ERR_INVALID
+ * before any work is enqueued. */
 int cp_preprocess_slots_dev(const uint8_t* frames, int32_t format, int32_t B, int32_t src_h, int32_t src_w,
                             int32_t dst_h, int32_t dst_w, const double* trans_input, const float mean[3],
                             const float std[3], const int32_t* start, float* out, float* prev, void* stream);
@@ -741,10 +751,10 @@ int cp_preprocess_slots_ragged_dev(const uint8_t* frames, const void* table, int
                                    float* out, float* prev, void* stream);
 /* A frame table with one pixel format per frame (cameras of different kinds in one step): cp_preprocess_frame_table
  * with formats[b] (HOST int32 [B], any cp_pixel_format but CP_PIX_PER_FRAME) for frame b, checked the same way (an
- * unknown format, an odd width in 4:2:2 or odd size in 4:2:0, a frame overrunning frames_bytes at its format's size
- * return CP_ERR_INVALID before any work).  The table has cp_preprocess_frame_table_bytes(B) bytes and is launched by
- * cp_preprocess_slots_ragged_dev and cp_preprocess_slots_rows_dev with format CP_PIX_PER_FRAME (and only so): frame b's
- * output is then bit for bit what the launch of a one-format table gives for it. */
+ * unknown format, an odd width in 4:2:2 or odd size in 4:2:0, a mosaic below 3 x 3, a frame overrunning frames_bytes at
+ * its format's size return CP_ERR_INVALID before any work).  The table has cp_preprocess_frame_table_bytes(B) bytes
+ * and is launched by cp_preprocess_slots_ragged_dev and cp_preprocess_slots_rows_dev with format CP_PIX_PER_FRAME
+ * (and only so): frame b's output is then bit for bit what the launch of a one-format table gives for it. */
 int cp_preprocess_frame_table_formats(int64_t frames_bytes, const int64_t* offsets, const int32_t* src_hw,
                                       const int32_t* formats, int32_t B, int32_t dst_h, int32_t dst_w,
                                       const double* trans_input, void* table, void* stream);
