@@ -62,7 +62,7 @@ EXPORTS = [
     "cp_preprocess_frame_table_bytes", "cp_preprocess_frame_table", "cp_preprocess_slots_ragged_dev",
     "cp_preprocess_slots_rows_dev", "cp_gather_rows_dev", "cp_tracker_render_dev2", "cp_tracker_step_dev",
     "cp_preprocess_formats", "cp_preprocess_frame_table_formats", "cp_plan_op_ksegments", "cp_plan_ksegments",
-    "cp_preprocess_remap", "cp_preprocess_frame_table_maps",
+    "cp_preprocess_remap", "cp_preprocess_frame_table_maps", "cp_preprocess_resize_affine",
 ]
 
 # cp_pixel_format; "bgr" is the interleaved uint8 [H,W,3] input of every other pre-process entry point.  The camera
@@ -221,6 +221,8 @@ def load():
                                 ctypes.POINTER(ctypes.c_float), vp]
     L.cp_preprocess_affine.argtypes = [vp, vp, i32, i32, i32, i32, i32, ctypes.POINTER(ctypes.c_double),
                                        ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_float), vp]
+    L.cp_preprocess_resize_affine.argtypes = [vp, vp, i32, i32, i32, i32, i32, i32, i32, ctypes.POINTER(ctypes.c_double),
+                                              ctypes.POINTER(ctypes.c_float), ctypes.POINTER(ctypes.c_float), vp]
     L.cp_preprocess_ragged.argtypes = [vp, i64, ctypes.POINTER(i64), ctypes.POINTER(i32), vp, i32, i32, i32,
                                        ctypes.POINTER(ctypes.c_double), ctypes.POINTER(ctypes.c_float),
                                        ctypes.POINTER(ctypes.c_float), vp]

@@ -7,7 +7,8 @@
 //                        the same for frames of different sizes in one launch, and cp_preprocess_yuv420 for NV12 / I420
 //                        frames (the colour conversion of cv2.cvtColor fused into the warp's tap fetch), and
 //                        cp_preprocess_formats for the camera formats (RGB24, RGBA, BGRA, YUYV, UYVY, gray and the
-//                        Bayer mosaics), one per frame;
+//                        Bayer mosaics), one per frame; cp_preprocess_resize_affine for a frame first resized by
+//                        cv2.resize at a test scale (fused into the warp's tap fetch);
 //                        cp_preprocess_slots_dev is the graph-safe form for one tracking step of a uniform batch, and
 //                        cp_preprocess_slots_ragged_dev (over a cp_preprocess_frame_table) that of slots of mixed sizes,
 //                        cp_preprocess_slots_rows_dev that of the live slots of a step with idle slots (a table may hold
@@ -219,6 +220,65 @@ __device__ __forceinline__ BayerFetch bayer_fetch(const uint8_t* __restrict__ im
                     format == CP_PIX_BAYER_BGGR8 || format == CP_PIX_BAYER_GRBG8};
 }
 
+// A BGR frame [sh, sw] served as cv2.resize(frame, (rw, rh)) (INTER_LINEAR) gives it, restated bit for bit (OpenCV
+// resize.cpp, INTER_RESIZE_COEF_BITS = 11; tests/resize_ref.py, pinned against cv2): the walk runs over the [rh, rw]
+// resized image, and every in-frame tap is resized from its 2 x 2 source pixels once, before the first channel is
+// written; taps outside stay BGR 0.  Per axis, with cv2's inverse scale (the host's 1 / (dst / src) in double),
+// destination index d takes f = (float)((d + 0.5) scale - 0.5), s = floor(f), f -= s and the weights
+// a0 = rne((1 - f) 2048), a1 = rne(f 2048) (float32 products).  Across, s < 0 or s >= sw - 1 puts s at the nearest
+// column with weights (2048, 0), and S = src[s] a0 + src[s + 1] a1.  Down, f is kept and the rows s and s + 1 are each
+// clamped into the frame (clamping f as across is off by one on the first and last rows of an upscale); the pixel is
+// sat((((b0 (S0 >> 4)) >> 16) + ((b1 (S1 >> 4)) >> 16) + 2) >> 2), cv2's VResizeLinear<uchar>.
+struct ResizeFetch {
+  const uint8_t* __restrict__ img;
+  int sh, sw;                          // the source frame
+  double scale_x, scale_y;
+  int bgr[4][3];
+  // the first source index of destination index d on an axis of inverse scale `scale`, and its two weights
+  static __device__ __forceinline__ int axis(int d, double scale, int& a0, int& a1) {
+    // unfused double arithmetic, as in the host code
+    float f = __double2float_rn(__dsub_rn(__dmul_rn(__dadd_rn((double)d, 0.5), scale), 0.5));
+    const float s = floorf(f);
+    f = __fsub_rn(f, s);
+    a0 = __float2int_rn(__fmul_rn(__fsub_rn(1.f, f), 2048.f));
+    a1 = __float2int_rn(__fmul_rn(f, 2048.f));
+    return (int)s;
+  }
+  __device__ __forceinline__ void taps(int iy, int ix, bool in00, bool in01, bool in10, bool in11) {
+    const bool in[4] = {in00, in01, in10, in11};
+    int x0[2], x1[2], a0[2], a1[2], y0[2], y1[2], b0[2], b1[2];   // [j]: column ix + j, row iy + j
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      int s = axis(ix + j, scale_x, a0[j], a1[j]);
+      if (s < 0 || s >= sw - 1) {
+        s = s < 0 ? 0 : sw - 1;
+        a0[j] = 2048;
+        a1[j] = 0;
+      }
+      x0[j] = s * 3;
+      x1[j] = min(s + 1, sw - 1) * 3;
+      s = axis(iy + j, scale_y, b0[j], b1[j]);
+      y0[j] = max(0, min(sh - 1, s));
+      y1[j] = max(0, min(sh - 1, s + 1));
+    }
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      bgr[k][0] = bgr[k][1] = bgr[k][2] = 0;
+      if (!in[k]) continue;
+      const int j = k >> 1, i = k & 1;
+      const uint8_t* __restrict__ r0 = img + (size_t)y0[j] * sw * 3;
+      const uint8_t* __restrict__ r1 = img + (size_t)y1[j] * sw * 3;
+#pragma unroll
+      for (int c = 0; c < 3; ++c) {
+        const int S0 = r0[x0[i] + c] * a0[i] + r0[x1[i] + c] * a1[i];
+        const int S1 = r1[x0[i] + c] * a0[i] + r1[x1[i] + c] * a1[i];
+        bgr[k][c] = max(0, min(255, (((b0[j] * (S0 >> 4)) >> 16) + ((b1[j] * (S1 >> 4)) >> 16) + 2) >> 2));
+      }
+    }
+  }
+  __device__ __forceinline__ int operator()(int k, int, int, int c) const { return bgr[k][c]; }
+};
+
 // The bytes of one sh x sw frame in a cp_pixel_format (0 for CP_PIX_PER_FRAME or an unknown value).
 __host__ __device__ constexpr size_t frame_bytes(int format, size_t sh, size_t sw) {
   return format == CP_PIX_NV12 || format == CP_PIX_I420     ? sh * sw * 3 / 2
@@ -308,7 +368,13 @@ struct PreprocessArgs {
   float* store;              // beginning a video); else the exchange (the live rows name distinct slots)
   float* prev;
   float* out;
+  int rh, rw;                // kResizeBgr: the size the frame is resized to, and cv2's inverse scales of the two axes
+  double scale_x, scale_y;
 };
+
+// The launch code of cp_preprocess_resize_affine (internal, not a cp_pixel_format): the uniform form over BGR frames
+// served through ResizeFetch, without previous frames.
+constexpr int kResizeBgr = 256 | CP_PIX_BGR;
 
 // The previous-frame writes of a launch (PreprocessArgs): none; the twin, prev[n] = the value where start[s] is set;
 // the exchange, prev[n] = start[s] ? value : store[s], then store[s] = value.  The mode is a template parameter, so a
@@ -318,7 +384,8 @@ enum PrevMode { kNoPrev, kTwin, kExchange };
 // B rows of [3, dh, dw]: row n is frame n (uniform) or the frame of slot s through the table (kTable), in format
 // kFormat (CP_PIX_PER_FRAME: each table entry's own).  Every thread is one output pixel of one row, grid-stride, and
 // reads and writes only its own elements.  kFormat | CP_PIX_REMAP (table form only): a mapped entry takes its source
-// position from its coordinate map at the output pixel, an unmapped one from its affine.
+// position from its coordinate map at the output pixel, an unmapped one from its affine.  kResizeBgr (uniform form):
+// frame n is BGR [a.sh, a.sw] and the walk runs over its resize to [a.rh, a.rw] (ResizeFetch).
 template <int kFormat, bool kTable, PrevMode kMode>
 __global__ void preprocess_kernel(const PreprocessArgs a) {
   static_assert(kTable || !(kFormat & CP_PIX_REMAP), "coordinate maps come through a frame table");
@@ -333,6 +400,8 @@ __global__ void preprocess_kernel(const PreprocessArgs a) {
     if constexpr (kTable) {
       if (kMode == kExchange || a.rows) s = a.rows[n];      // the exchange is the rows form's only
       f = a.fr[s];
+    } else if constexpr (kFormat == kResizeBgr) {
+      f = RaggedFrame{a.W, (long long)n * a.sh * a.sw * 3, a.rh, a.rw};   // the walk's frame is the resized image
     } else {
       f = RaggedFrame{a.W, (long long)(n * frame_bytes(kFormat, a.sh, a.sw)), a.sh, a.sw};
     }
@@ -344,7 +413,7 @@ __global__ void preprocess_kernel(const PreprocessArgs a) {
     int2 mapped{};
     if constexpr ((kFormat & CP_PIX_REMAP) != 0)
       mapped = f.offset & kMappedFlag ? map_pos(frame_map(f)[px]) : affine_pos(f.W, x, y);
-    frame_walk<kFormat>(a.frames, f, [&](auto fetch) {
+    const auto walk = [&](auto fetch) {
       const int2 pos = [&] {
         if constexpr ((kFormat & CP_PIX_REMAP) != 0)
           return mapped;
@@ -359,7 +428,11 @@ __global__ void preprocess_kernel(const PreprocessArgs a) {
           store[c * plane] = v;
         }
       });
-    });
+    };
+    if constexpr (kFormat == kResizeBgr)
+      walk(ResizeFetch{a.frames + f.offset, a.sh, a.sw, a.scale_x, a.scale_y});
+    else
+      frame_walk<kFormat>(a.frames, f, walk);
   }
 }
 
@@ -481,13 +554,18 @@ PreprocessArgs preprocess_args(const uint8_t* frames, float* out, int B, int dh,
 
 // enqueues preprocess_kernel in `format`: the table form when a.fr is set (which may also be CP_PIX_PER_FRAME, carry
 // CP_PIX_REMAP and take the store exchange, with rows), else the uniform form; the previous-frame mode is the one a's
-// pointers select
+// pointers select; kResizeBgr: its one instance, uniform without previous frames
 int launch_preprocess(int format, const PreprocessArgs& a, cudaStream_t s) {
+  const int blocks = preprocess_blocks((size_t)a.B * a.dh * a.dw);
+  if (format == kResizeBgr && !a.fr && !a.prev) {
+    preprocess_kernel<kResizeBgr, false, kNoPrev><<<blocks, 256, 0, s>>>(a);
+    CP_LAUNCH_CHECK("preprocess_kernel");
+    return CP_OK;
+  }
   if (a.fr ? !table_code(format) || (a.store && !a.rows) : !known_format(format) || a.store)
     return fail(CP_ERR_INVALID, "preprocess_kernel: no instance for pixel format " + std::to_string(format) +
                                     (a.fr ? " over a frame table" : " over a uniform batch") +
                                     (a.store ? " with a store" : ""));
-  const int blocks = preprocess_blocks((size_t)a.B * a.dh * a.dw);
   const PrevMode mode = !a.prev ? kNoPrev : !a.store ? kTwin : kExchange;
   with_format(format, [&](auto k) {
     constexpr int kFormat = decltype(k)::value;
@@ -744,6 +822,31 @@ int cp_preprocess_affine(const uint8_t* frames, float* out, int32_t B, int32_t s
   a.sh = src_h;
   a.sw = src_w;
   return launch_preprocess(CP_PIX_BGR, a, (cudaStream_t)stream_);
+}
+
+int cp_preprocess_resize_affine(const uint8_t* frames, float* out, int32_t B, int32_t src_h, int32_t src_w, int32_t rs_h,
+                                int32_t rs_w, int32_t dst_h, int32_t dst_w, const double trans_input[6],
+                                const float mean[3], const float stdv[3], void* stream_) {
+  if (!frames || !out || !mean || !stdv || !trans_input)
+    return fail(CP_ERR_INVALID, "cp_preprocess_resize_affine: null argument");
+  if (B <= 0 || src_h <= 0 || src_w <= 0 || rs_h <= 0 || rs_w <= 0 || dst_h <= 0 || dst_w <= 0)
+    return fail(CP_ERR_INVALID, "cp_preprocess_resize_affine: bad shape (B " + std::to_string(B) + ", frame " +
+                                    std::to_string(src_h) + " x " + std::to_string(src_w) + ", resized " +
+                                    std::to_string(rs_h) + " x " + std::to_string(rs_w) + ", output " +
+                                    std::to_string(dst_h) + " x " + std::to_string(dst_w) + ")");
+  // cv2.resize copies a frame of the same size
+  if (rs_h == src_h && rs_w == src_w)
+    return cp_preprocess_affine(frames, out, B, src_h, src_w, dst_h, dst_w, trans_input, mean, stdv, stream_);
+  PreprocessArgs a = preprocess_args(frames, out, B, dst_h, dst_w, mean, stdv);
+  a.W = invert_affine(trans_input);
+  a.sh = src_h;
+  a.sw = src_w;
+  a.rh = rs_h;
+  a.rw = rs_w;
+  // cv2's inverse scales: 1 / inv_scale with inv_scale = dst / src, in double
+  a.scale_x = 1. / ((double)rs_w / src_w);
+  a.scale_y = 1. / ((double)rs_h / src_h);
+  return launch_preprocess(kResizeBgr, a, (cudaStream_t)stream_);
 }
 
 // the fix_res affine of the frame size (fix_res_affine above)

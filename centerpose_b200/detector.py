@@ -2,12 +2,15 @@
 /root/reference/src/lib/detectors/{base_detector,object_pose,detector_factory}.py.
 
 `run()` keeps the reference's one-image semantics and its 12-key return dict
-(base_detector.py:390-772): load -> pre_process (cv2, identical to the
-reference) -> network -> decode -> post_process -> merge -> PnP.  Everything
-after pre_process runs in libcenterpose_b200.so; the only host work left is
-rebuilding the reference's Python result structures from the fixed-shape pose
-records (`records_to_results`).  `run_batch()` is the batched entry point the
-reference does not have (B = 32 / 256 configurations of BASELINE.json).
+(base_detector.py:390-772): load -> pre_process -> network -> decode ->
+post_process -> merge -> PnP.  A uint8 BGR image is uploaded once and
+pre-processed on the device at every test scale, bit for bit what the cv2 code
+of `pre_process` gives (which stays, as the public method and for pre-processed
+input); everything after it runs in libcenterpose_b200.so too.  The only host
+work left is rebuilding the reference's Python result structures from the
+fixed-shape pose records (`records_to_results`).  `run_batch()` is the batched
+entry point the reference does not have (B = 32 / 256 configurations of
+BASELINE.json).
 """
 import copy
 import json
@@ -209,6 +212,8 @@ class ObjectPoseDetector(object):
         self._packed = None            # run_batch(list): device buffer the ragged frames are packed into
         self._affines = {}             # (h, w) -> fix_res trans_input of that frame size
         self._maps = MapCache()        # run_batch(distortion=): the device map of each camera
+        self._stage = None             # run(): the pinned staging buffer and the device buffer of the frame
+        self._frame_dev = None
 
     def _to_device(self, t):
         """base_detector.py:41,436: everything the network touches lives on opt.device (always CUDA here)."""
@@ -217,7 +222,17 @@ class ObjectPoseDetector(object):
     # base_detector.py:91-148 -- the reference's cv2 pre-processing (host side), all three modes
     def pre_process(self, image, scale, input_meta={}):
         import cv2
-        height, width = image.shape[0:2]
+        (new_height, new_width), meta = self._pre_meta(image.shape[0], image.shape[1], scale, input_meta)
+        inp_height, inp_width = meta["inp_height"], meta["inp_width"]
+        resized = cv2.resize(image, (new_width, new_height))
+        inp = cv2.warpAffine(resized, meta["trans_input"], (inp_width, inp_height), flags=cv2.INTER_LINEAR)
+        inp = ((inp / 255. - self.mean) / self.std).astype(np.float32)
+        images = torch.from_numpy(inp.transpose(2, 0, 1).reshape(1, 3, inp_height, inp_width))
+        return images, meta
+
+    def _pre_meta(self, height, width, scale, input_meta):
+        """The geometry of pre_process for a height x width frame at `scale`, in each mode: ((new_height, new_width), the
+        size cv2.resize takes the frame to; meta, with pre_dets / camera_matrix / id copied from input_meta)."""
         new_height = int(height * scale)
         new_width = int(width * scale)
         if self.opt.fix_short > 0:
@@ -243,16 +258,42 @@ class ObjectPoseDetector(object):
         out_height = inp_height // self.opt.down_ratio
         out_width = inp_width // self.opt.down_ratio
         trans_output = affine_from_center_scale(c, s0, out_width, out_height)
-        resized = cv2.resize(image, (new_width, new_height))
-        inp = cv2.warpAffine(resized, trans_input, (inp_width, inp_height), flags=cv2.INTER_LINEAR)
-        inp = ((inp / 255. - self.mean) / self.std).astype(np.float32)
-        images = torch.from_numpy(inp.transpose(2, 0, 1).reshape(1, 3, inp_height, inp_width))
         meta = {"c": c, "s": s, "height": height, "width": width, "out_height": out_height,
                 "out_width": out_width, "inp_height": inp_height, "inp_width": inp_width,
                 "trans_input": trans_input, "trans_output": trans_output}
         for k in ("pre_dets", "camera_matrix", "id"):
             if k in input_meta:
                 meta[k] = input_meta[k]
+        return (new_height, new_width), meta
+
+    def _device_frame(self, image):
+        """run()'s frame on the device, or None for the host pre_process: a uint8 [H,W,3] numpy image is uploaded once
+        per call, as [1,H,W,3], through a pinned staging buffer into a device buffer, both kept and grown (run()
+        synchronises before it returns, so both are free again at the next call).  A test scale that resizes the frame
+        below 1 px is refused first."""
+        if not (isinstance(image, np.ndarray) and image.dtype == np.uint8 and image.ndim == 3 and image.shape[2] == 3):
+            return None
+        h, w = image.shape[:2]
+        for scale in self.scales:
+            if int(h * scale) < 1 or int(w * scale) < 1:
+                raise ValueError("run: test scale %g resizes the %d x %d frame to %d x %d pixels"
+                                 % (scale, h, w, int(h * scale), int(w * scale)))
+        n = image.size
+        if self._stage is None or self._stage.numel() < n:
+            self._stage = torch.empty((n,), dtype=torch.uint8, pin_memory=True)
+            self._frame_dev = torch.empty((n,), dtype=torch.uint8, device=self.opt.device)
+        np.copyto(self._stage[:n].numpy().reshape(image.shape), image)
+        frame = self._frame_dev[:n]
+        frame.copy_(self._stage[:n], non_blocking=True)
+        return frame.view((1,) + image.shape)
+
+    def _device_pre_process(self, frame, scale, input_meta):
+        """pre_process on the device of the uploaded frame ([1,H,W,3] uint8 CUDA, _device_frame): the same images (here
+        a [1,3,inp_height,inp_width] CUDA tensor) and meta, bit for bit -- cv2.resize fused into the warp
+        (cp_preprocess_resize_affine) in all three modes."""
+        (new_height, new_width), meta = self._pre_meta(frame.shape[1], frame.shape[2], scale, input_meta)
+        images = preprocess(frame, meta["inp_height"], meta["inp_width"], self.opt.mean, self.opt.std,
+                            trans_input=meta["trans_input"], resize_hw=(new_height, new_width))
         return images, meta
 
     def _track_policy(self, start, frame_id, pre_dets):
@@ -308,9 +349,12 @@ class ObjectPoseDetector(object):
                 "camera_matrix": np.eye(3)}
 
     def run(self, image_or_path_or_tensor, filename=None, meta_inp={}, preprocessed_flag=False):
-        """base_detector.py:390-772.  One image per call, the reference's 12-key return dict.  After pre_process
-        everything runs in libcenterpose_b200.so; post_process / merge_outputs / PnP are part of the fused decode call,
-        so their stamps are 0 and `dec` carries the whole post-network stage."""
+        """base_detector.py:390-772.  One image per call, the reference's 12-key return dict.  A uint8 [H,W,3] image
+        (passed, or read from a path) is uploaded once and pre-processed on the device at every test scale
+        (_device_frame, _device_pre_process: bit for bit pre_process, so `pre` covers the upload and the launches);
+        pre-processed input and other dtypes or shapes go through pre_process on the host.  After that everything runs
+        in libcenterpose_b200.so; post_process / merge_outputs / PnP are part of the fused decode call, so their stamps
+        are 0 and `dec` carries the whole post-network stage."""
         import cv2
         load_time, pre_time, net_time, dec_time, post_time = 0, 0, 0, 0, 0
         merge_time, track_time, pnp_time, tot_time = 0, 0, 0, 0
@@ -331,6 +375,9 @@ class ObjectPoseDetector(object):
             pre_processed = True
         loaded_time = time.time()
         load_time += loaded_time - start_time
+        # a uint8 BGR frame goes to the device once and every scale pre-processes it there; `pre` covers the upload
+        frame = None if pre_processed else self._device_frame(image)
+        pre_time += time.time() - loaded_time
 
         # base_detector.py:421-497: one pass per test scale.  merge_outputs (object_pose.py:184-197) reads detections[0],
         # i.e. only the FIRST scale contributes results (with the soft-NMS forced on when several scales are listed); the
@@ -338,7 +385,9 @@ class ObjectPoseDetector(object):
         first = None
         for si, scale in enumerate(self.scales):
             scale_start_time = time.time()
-            if not pre_processed:
+            if frame is not None:
+                images, meta = self._device_pre_process(frame, scale, meta_inp)
+            elif not pre_processed:
                 images, meta = self.pre_process(image, scale, meta_inp)
             else:
                 images = torch.from_numpy(np.expand_dims(image, axis=0))

@@ -487,12 +487,16 @@ class InferGraph(object):
         return self.poses, self.n_valid
 
 
-def preprocess(frames_u8, dst_h, dst_w, mean, std, out=None, trans_input=None):
+def preprocess(frames_u8, dst_h, dst_w, mean, std, out=None, trans_input=None, resize_hw=None):
     """cp_preprocess: uint8 [B,H,W,3] CUDA -> fp32 [B,3,dst_h,dst_w] CUDA (bit-exact cv2.warpAffine + normalise).
-    trans_input: optional 2x3 forward affine (meta['trans_input']); default = the fix_res affine of the frame size."""
+    trans_input: optional 2x3 forward affine (meta['trans_input']); default = the fix_res affine of the frame size.
+    resize_hw: (rh, rw) to warp cv2.resize(frame, (rw, rh)) instead of the frame, as pre_process does at a test scale
+    (cp_preprocess_resize_affine); trans_input then maps the resized image and must be given."""
     L = _lib.load()
     if not frames_u8.is_cuda or frames_u8.dtype != torch.uint8:
         raise RuntimeError("preprocess needs a uint8 CUDA tensor")
+    if resize_hw is not None and trans_input is None:
+        raise ValueError("preprocess: resize_hw needs the trans_input of the resized image")
     B, sh, sw, _ = frames_u8.shape
     if out is None:
         out = torch.empty((B, 3, dst_h, dst_w), dtype=torch.float32, device=frames_u8.device)
@@ -501,7 +505,12 @@ def preprocess(frames_u8, dst_h, dst_w, mean, std, out=None, trans_input=None):
     with torch.cuda.device(frames_u8.device):
         if trans_input is not None:
             tm = (ctypes.c_double * 6)(*[float(v) for v in np.asarray(trans_input, np.float64).reshape(-1)])
-            rc = L.cp_preprocess_affine(_ptr(frames_u8.contiguous()), _ptr(out), B, sh, sw, dst_h, dst_w, tm, m, s, _stream())
+            if resize_hw is not None:
+                rc = L.cp_preprocess_resize_affine(_ptr(frames_u8.contiguous()), _ptr(out), B, sh, sw, int(resize_hw[0]),
+                                                   int(resize_hw[1]), dst_h, dst_w, tm, m, s, _stream())
+            else:
+                rc = L.cp_preprocess_affine(_ptr(frames_u8.contiguous()), _ptr(out), B, sh, sw, dst_h, dst_w, tm, m, s,
+                                            _stream())
         else:
             rc = L.cp_preprocess(_ptr(frames_u8.contiguous()), _ptr(out), B, sh, sw, dst_h, dst_w, m, s, _stream())
     _lib.check(rc, "cp_preprocess")

@@ -33,7 +33,8 @@
  *       utils/pnp/cuboid_pnp_shell.py:11-93, utils/pnp/cuboid_pnp_solver.py:91-239
  *   cp_infer
  *       detectors/base_detector.py:473-654 (process -> post_process -> merge -> PnP)
- *   cp_preprocess / cp_preprocess_affine / cp_preprocess_ragged / cp_preprocess_yuv420 / cp_preprocess_formats
+ *   cp_preprocess / cp_preprocess_affine / cp_preprocess_ragged / cp_preprocess_yuv420 / cp_preprocess_formats /
+ *   cp_preprocess_resize_affine
  *       detectors/base_detector.py:91-148 pre_process (resize + affine warp + normalise)
  */
 #ifndef CENTERPOSE_B200_H_
@@ -645,6 +646,14 @@ int cp_preprocess(const uint8_t* frames, float* out, int32_t B, int32_t src_h, i
  * meta['trans_input'] (source frame -> network input), e.g. for fix_short / keep_res or rotated crops. */
 int cp_preprocess_affine(const uint8_t* frames, float* out, int32_t B, int32_t src_h, int32_t src_w, int32_t dst_h,
                          int32_t dst_w, const double trans_input[6], const float mean[3], const float std[3], void* stream);
+/* cp_preprocess_affine of each frame resized first, as pre_process does at a test scale (base_detector.py:94-96,
+ * :128): out = (warpAffine(cv2.resize(frame, (rs_w, rs_h)), trans_input, (dst_w, dst_h)) / 255 - mean) / std, bit for
+ * bit.  The resize is cv2's INTER_LINEAR for 8-bit frames (11-bit integer weights), computed per tap inside the warp,
+ * so the resized frame is never stored.  rs_h x rs_w == src_h x src_w makes exactly the launch of
+ * cp_preprocess_affine (cv2.resize copies such a frame).  Any size <= 0 returns CP_ERR_INVALID before any work. */
+int cp_preprocess_resize_affine(const uint8_t* frames, float* out, int32_t B, int32_t src_h, int32_t src_w,
+                                int32_t rs_h, int32_t rs_w, int32_t dst_h, int32_t dst_w, const double trans_input[6],
+                                const float mean[3], const float std[3], void* stream);
 /* A ragged batch in one launch: B frames of different sizes packed into one device buffer.  Frame b is uint8
  * [src_hw[b][0], src_hw[b][1], 3] starting `offsets[b]` bytes into `frames` (frames_bytes long); out: device fp32 NCHW
  * [B,3,dst_h,dst_w].  offsets (int64 [B]), src_hw (int32 [B,2]) and trans_input (double [B,6], row-major 2x3 forward
