@@ -63,6 +63,7 @@ EXPORTS = [
     "cp_preprocess_slots_rows_dev", "cp_gather_rows_dev", "cp_tracker_render_dev2", "cp_tracker_step_dev",
     "cp_preprocess_formats", "cp_preprocess_frame_table_formats", "cp_plan_op_ksegments", "cp_plan_ksegments",
     "cp_preprocess_remap", "cp_preprocess_frame_table_maps", "cp_preprocess_resize_affine",
+    "cp_jpeg_parse", "cp_jpeg_workspace_bytes", "cp_jpeg_decode", "cp_jpeg_last_rounds",
 ]
 
 # cp_pixel_format; "bgr" is the interleaved uint8 [H,W,3] input of every other pre-process entry point.  The camera
@@ -82,6 +83,16 @@ PIXEL_FORMAT_CODES = {"bgr": CP_PIX_BGR, "nv12": CP_PIX_NV12, "i420": CP_PIX_I42
                       "gray": CP_PIX_GRAY, "bayer_rggb8": CP_PIX_BAYER_RGGB8, "bayer_bggr8": CP_PIX_BAYER_BGGR8,
                       "bayer_gbrg8": CP_PIX_BAYER_GBRG8, "bayer_grbg8": CP_PIX_BAYER_GRBG8}
 
+# cp_jpeg_refusal: why cp_jpeg_parse refuses a file; cp_jpeg_error: the bits of a frame's error word after cp_jpeg_decode
+JPEG_REFUSALS = {0: "ok", 1: "not a JPEG file", 2: "truncated header", 3: "progressive JPEG", 4: "lossless JPEG",
+                 5: "arithmetic coding", 6: "samples other than 8 bits", 7: "not 1 or 3 components",
+                 8: "more than one scan", 9: "height set by a DNL marker", 10: "unsupported chroma sampling",
+                 11: "RGB-coded JPEG", 12: "missing or malformed DQT / DHT", 13: "malformed header",
+                 14: "more than 2^30 pixels"}
+JPEG_ERR_CODE, JPEG_ERR_RUN, JPEG_ERR_SHORT, JPEG_ERR_RESTART = 1, 2, 4, 8
+JPEG_ERRORS = {JPEG_ERR_CODE: "invalid Huffman code", JPEG_ERR_RUN: "AC run past coefficient 63",
+               JPEG_ERR_SHORT: "restart segment ends early", JPEG_ERR_RESTART: "missing or misnumbered RST marker"}
+
 # cp_plan_create_ex / cp_plan_memory flags
 CP_PLAN_REUSE_ACTIVATIONS = 1
 CP_PLAN_MULTI_TRACK = 2
@@ -96,6 +107,19 @@ FAM_MAXPOOL, FAM_UPADD, FAM_GN_RELU, FAM_GRU = 7, 8, 9, 10
 FAMILY_NAMES = {FAM_NONE: "fused", FAM_IGEMM_FP32: "igemm_fp32", FAM_STEM: "stem", FAM_CONV3_C16: "conv3_c16",
                 FAM_IGEMM_UMMA: "igemm_umma", FAM_CONV_TMA: "conv_tma", FAM_DCN_TMA: "dcn_tma", FAM_MAXPOOL: "maxpool",
                 FAM_UPADD: "upadd", FAM_GN_RELU: "gn_relu", FAM_GRU: "gru"}
+
+
+class CpJpegHuff(ctypes.Structure):
+    _fields_ = [("look", ctypes.c_uint16 * 512), ("maxcode", ctypes.c_int32 * 18), ("valoffset", ctypes.c_int32 * 18),
+                ("vals", ctypes.c_uint8 * 256)]
+
+
+class CpJpegHeader(ctypes.Structure):
+    _fields_ = ([(n, ctypes.c_int32) for n in ("status", "width", "height", "out_h", "out_w", "orientation", "ncomp",
+                                                "hmax", "vmax", "mcux", "mcuy", "blocks_per_mcu", "restart_interval")] +
+                [("scan_begin", ctypes.c_int64), ("scan_end", ctypes.c_int64), ("comp_h", ctypes.c_int32 * 3),
+                 ("comp_v", ctypes.c_int32 * 3), ("quant", (ctypes.c_int16 * 64) * 3), ("dc", CpJpegHuff * 3),
+                 ("ac", CpJpegHuff * 3)])
 
 
 class CpOpStat(ctypes.Structure):
@@ -281,10 +305,15 @@ def load():
     L.cp_plan_op_ksegments.argtypes = [vp, i32, ctypes.POINTER(i32), ctypes.POINTER(i32), ctypes.POINTER(i32)]
     L.cp_plan_ksegments.argtypes = [ctypes.POINTER(CpConfig), i32, ctypes.c_uint32, ctypes.POINTER(i32), i32,
                                     ctypes.POINTER(i32)]
+    L.cp_jpeg_parse.argtypes = [vp, i64, ctypes.POINTER(CpJpegHeader)]
+    L.cp_jpeg_workspace_bytes.argtypes = [ctypes.POINTER(CpJpegHeader), i32]
+    L.cp_jpeg_workspace_bytes.restype = ctypes.c_size_t
+    L.cp_jpeg_decode.argtypes = [ctypes.POINTER(CpJpegHeader), i32, vp, vp, vp, vp, vp, ctypes.c_size_t, vp, i32, vp]
+    L.cp_jpeg_last_rounds.argtypes = []
     for name in EXPORTS:
         fn = getattr(L, name)
         if name not in ("cp_version", "cp_last_error", "cp_plan_bytes", "cp_plan_forward_launches",
-                        "cp_decode_workspace_bytes", "cp_preprocess_frame_table_bytes"):
+                        "cp_decode_workspace_bytes", "cp_preprocess_frame_table_bytes", "cp_jpeg_workspace_bytes"):
             fn.restype = ctypes.c_int
     _lib = L
     return L

@@ -12,7 +12,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libcenterpose_b200.so")
-SOURCES = ["plan.cu", "igemm_fp32.cu", "elementwise.cu", "decode.cu", "ext_ops.cu", "conv_select.cu", "igemm_umma.cu", "stem_conv.cu", "conv_tma.cu", "dcn_tma.cu", "tracker.cu", "dcn_bwd.cu"]
+SOURCES = ["plan.cu", "igemm_fp32.cu", "elementwise.cu", "decode.cu", "ext_ops.cu", "conv_select.cu", "igemm_umma.cu", "stem_conv.cu", "conv_tma.cu", "dcn_tma.cu", "tracker.cu", "dcn_bwd.cu", "jpeg.cu"]
 def _headers():
     """Every header a .cu may include: editing shared code (umma_common.cuh, pose_core.h ...) must rebuild the objects."""
     hs = sorted(f for f in os.listdir(CSRC) if f.endswith((".cuh", ".h")))

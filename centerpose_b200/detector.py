@@ -21,8 +21,9 @@ import numpy as np
 import torch
 
 from . import _lib
-from .engine import (Engine, check_pixel_format, decode_params, decode_pnp, frame_layout, image_size, make_meta,
-                     preprocess, preprocess_formats, preprocess_remap, slot_formats)
+from .engine import (JPEG, Engine, check_pixel_format, decode_params, decode_pnp, frame_layout, image_size, is_jpeg,
+                     jpeg_bytes, jpeg_decode, jpeg_error_text, jpeg_parse, make_meta, preprocess, preprocess_formats,
+                     preprocess_remap, slot_formats)
 from .lens import MapCache, slot_distortions, undistorted_cameras
 from .model import _load_checkpoint, create_model, load_model
 from .tracker import Tracker, tracks_to_results
@@ -127,6 +128,45 @@ def camera_per_frame(camera_matrix, B):
     return list(cam)
 
 
+class JpegFrame:
+    """An encoded JPEG frame of run_batch(list, pixel_format="jpeg"): its bytes (uint8 numpy) and parsed header; shape is
+    that of the decoded BGR image (after the EXIF orientation)."""
+
+    def __init__(self, data, header):
+        self.data, self.header = data, header
+        self.shape = (header.out_h, header.out_w, 3)
+
+
+def jpeg_frames(frames, pixel_format):
+    """run_batch(list) with pixel_format "jpeg" (or a list naming it for some frames): each such frame (bytes, a 1-D uint8
+    numpy array or CPU tensor; None for an idle slot) parsed into a JpegFrame, its format replaced by "bgr".  A refused
+    header raises ValueError naming the frame and the reason, before any device work.  Other calls are returned as
+    they are."""
+    names = list(pixel_format) if isinstance(pixel_format, (list, tuple)) else [pixel_format] * len(frames)
+    if JPEG not in [f for f in names if isinstance(f, str)]:
+        return frames, pixel_format
+    if len(names) != len(frames):
+        raise ValueError("run_batch: pixel_format is one name or one per frame, got %d names for %d frames"
+                         % (len(names), len(frames)))
+    frames = list(frames)
+    for b, f in enumerate(frames):
+        if names[b] != JPEG:
+            continue
+        names[b] = "bgr"
+        if f is None:
+            continue
+        data = jpeg_bytes(f)
+        if data is None:
+            raise TypeError("run_batch: frame %d is a %s; pixel_format \"jpeg\" takes encoded bytes, a 1-D uint8 numpy "
+                            "array or CPU tensor" % (b, type(f).__name__))
+        h = jpeg_parse(data)
+        if h.status:
+            raise ValueError("run_batch: frame %d is a JPEG the device decoder does not take: %s"
+                             % (b, _lib.JPEG_REFUSALS.get(h.status, h.status)))
+        frames[b] = JpegFrame(data, h)
+    return frames, names
+
+
 def check_frames(frames, allow_idle, pixel_format="bgr"):
     """The frames of a ragged batch: uint8 [H,W,3] numpy arrays or tensors, or the buffers of another pixel_format
     (engine.check_pixel_format), one name for every frame or a list with one per frame (None = an idle slot when
@@ -140,6 +180,8 @@ def check_frames(frames, allow_idle, pixel_format="bgr"):
         if f is None:
             if not allow_idle:
                 raise ValueError("run_batch: frame %d is None (idle slots need track=True)" % b)
+            continue
+        if isinstance(f, JpegFrame):
             continue
         if not isinstance(f, (np.ndarray, torch.Tensor)):
             raise TypeError("run_batch: frame %d is a %s, not a numpy array or tensor" % (b, type(f).__name__))
@@ -214,6 +256,7 @@ class ObjectPoseDetector(object):
         self._maps = MapCache()        # run_batch(distortion=): the device map of each camera
         self._stage = None             # run(): the pinned staging buffer and the device buffer of the frame
         self._frame_dev = None
+        self._jpeg_dev = None          # run(): the device copy of a JPEG file's bytes
 
     def _to_device(self, t):
         """base_detector.py:41,436: everything the network touches lives on opt.device (always CUDA here)."""
@@ -266,6 +309,13 @@ class ObjectPoseDetector(object):
                 meta[k] = input_meta[k]
         return (new_height, new_width), meta
 
+    def _check_scales(self, h, w):
+        """A test scale that resizes the h x w frame below 1 px is refused before any device work."""
+        for scale in self.scales:
+            if int(h * scale) < 1 or int(w * scale) < 1:
+                raise ValueError("run: test scale %g resizes the %d x %d frame to %d x %d pixels"
+                                 % (scale, h, w, int(h * scale), int(w * scale)))
+
     def _device_frame(self, image):
         """run()'s frame on the device, or None for the host pre_process: a uint8 [H,W,3] numpy image is uploaded once
         per call, as [1,H,W,3], through a pinned staging buffer into a device buffer, both kept and grown (run()
@@ -273,19 +323,36 @@ class ObjectPoseDetector(object):
         below 1 px is refused first."""
         if not (isinstance(image, np.ndarray) and image.dtype == np.uint8 and image.ndim == 3 and image.shape[2] == 3):
             return None
-        h, w = image.shape[:2]
-        for scale in self.scales:
-            if int(h * scale) < 1 or int(w * scale) < 1:
-                raise ValueError("run: test scale %g resizes the %d x %d frame to %d x %d pixels"
-                                 % (scale, h, w, int(h * scale), int(w * scale)))
+        self._check_scales(*image.shape[:2])
         n = image.size
-        if self._stage is None or self._stage.numel() < n:
+        if self._stage is None or self._stage.numel() < n or self._frame_dev.numel() < n:
             self._stage = torch.empty((n,), dtype=torch.uint8, pin_memory=True)
             self._frame_dev = torch.empty((n,), dtype=torch.uint8, device=self.opt.device)
         np.copyto(self._stage[:n].numpy().reshape(image.shape), image)
         frame = self._frame_dev[:n]
         frame.copy_(self._stage[:n], non_blocking=True)
         return frame.view((1,) + image.shape)
+
+    def _device_jpeg(self, data, header):
+        """run()'s frame decoded on the device from the bytes of a supported JPEG (cp_jpeg_decode, bit for bit
+        cv2.imread): the bytes go up once through the pinned staging buffer, the decoded frame lands in the device frame
+        buffer as [1,H,W,3].  None when the bitstream is corrupt (the frame's error word, read back once): run() then
+        decodes on the host as before."""
+        h, w = header.out_h, header.out_w
+        self._check_scales(h, w)
+        n, m = len(data), h * w * 3
+        if self._stage is None or self._stage.numel() < n:
+            self._stage = torch.empty((n,), dtype=torch.uint8, pin_memory=True)
+        if self._frame_dev is None or self._frame_dev.numel() < m:
+            self._frame_dev = torch.empty((m,), dtype=torch.uint8, device=self.opt.device)
+        if self._jpeg_dev is None or self._jpeg_dev.numel() < n:
+            self._jpeg_dev = torch.empty((n,), dtype=torch.uint8, device=self.opt.device)
+        np.copyto(self._stage[:n].numpy(), data)
+        self._jpeg_dev[:n].copy_(self._stage[:n], non_blocking=True)
+        errors = jpeg_decode([header], self._jpeg_dev, [0], self._frame_dev, [0])
+        if int(errors.item()):
+            return None
+        return self._frame_dev[:m].view(1, h, w, 3)
 
     def _device_pre_process(self, frame, scale, input_meta):
         """pre_process on the device of the uploaded frame ([1,H,W,3] uint8 CUDA, _device_frame): the same images (here
@@ -364,19 +431,48 @@ class ObjectPoseDetector(object):
                                       "state once per scale, base_detector.py:440-449)")
         start_time = time.time()
         pre_processed = preprocessed_flag
-        if isinstance(image_or_path_or_tensor, np.ndarray):
+        encoded = None              # the bytes of a JPEG file or of encoded input, decoded on the device
+        from_path = type(image_or_path_or_tensor) == type("")   # before `filename` may replace it (a label, not a file)
+        if isinstance(image_or_path_or_tensor, (bytes, bytearray)) or (
+                isinstance(image_or_path_or_tensor, np.ndarray) and image_or_path_or_tensor.ndim == 1
+                and image_or_path_or_tensor.dtype == np.uint8):
+            encoded, image = jpeg_bytes(image_or_path_or_tensor), None
+            if filename is not None:
+                image_or_path_or_tensor = filename
+        elif isinstance(image_or_path_or_tensor, np.ndarray):
             image = image_or_path_or_tensor
             if filename is not None:
                 image_or_path_or_tensor = filename
         elif type(image_or_path_or_tensor) == type(""):
-            image = cv2.imread(image_or_path_or_tensor)
+            image = None
+            try:
+                with open(image_or_path_or_tensor, "rb") as fp:
+                    head = fp.read(3)
+                    if is_jpeg(head):
+                        encoded = np.frombuffer(head + fp.read(), np.uint8)
+            except OSError:
+                pass
+            if encoded is None:
+                image = cv2.imread(image_or_path_or_tensor)
         else:
             image = image_or_path_or_tensor["image"][0].numpy()
             pre_processed = True
         loaded_time = time.time()
         load_time += loaded_time - start_time
-        # a uint8 BGR frame goes to the device once and every scale pre-processes it there; `pre` covers the upload
-        frame = None if pre_processed else self._device_frame(image)
+        # a uint8 BGR frame goes to the device once and every scale pre-processes it there; `pre` covers the upload.
+        # A supported JPEG is decoded there instead (bit for bit cv2.imread); a refused or corrupt one is decoded by cv2.
+        frame = None
+        if encoded is not None:
+            header = jpeg_parse(encoded) if is_jpeg(encoded) else None
+            if header is not None and header.status == 0:
+                frame = self._device_jpeg(encoded, header)
+            if frame is None:
+                image = cv2.imread(image_or_path_or_tensor) if from_path else cv2.imdecode(encoded, cv2.IMREAD_COLOR)
+            else:
+                debug = int(getattr(self.opt, "debug", 0) or 0)
+                image = frame[0].cpu().numpy() if debug >= 1 else None
+        if frame is None and not pre_processed:
+            frame = self._device_frame(image)
         pre_time += time.time() - loaded_time
 
         # base_detector.py:421-497: one pass per test scale.  merge_outputs (object_pose.py:184-197) reads detections[0],
@@ -653,6 +749,7 @@ class ObjectPoseDetector(object):
             if new_video is not None or pre_dets is not None or frame_ids is not None:
                 raise ValueError("run_batch(list): new_video / pre_dets / frame_ids need track=True")
             dists = slot_distortions(distortion, len(frames))
+            frames, pixel_format = jpeg_frames(frames, pixel_format)
             check_frames(frames, allow_idle=False, pixel_format=pixel_format)
             x, meta, _ = self._ragged_input(frames, camera_matrix, pixel_format, dists)
         else:
@@ -768,11 +865,13 @@ class ObjectPoseDetector(object):
             ts.append(t)
             hw[b] = image_size(t.shape, fmts[b])
             offs[b] = off
-            off += t.numel()
+            off += int(np.prod(t.shape))
         if self._packed is None or self._packed.numel() < off or self._packed.device != torch.device(dev):
             self._packed = torch.empty((max(off, 1),), dtype=torch.uint8, device=dev)
         for t, o in zip(ts, offs):
-            self._packed[o:o + t.numel()].copy_(t.reshape(-1), non_blocking=True)
+            if not isinstance(t, JpegFrame):
+                self._packed[o:o + t.numel()].copy_(t.reshape(-1), non_blocking=True)
+        self._decode_jpegs(frames, offs)
         trans = np.zeros((B, 2, 3), np.float64)
         meta = np.zeros((B, _lib.CP_META_DOUBLES), np.float64)
         for b in range(B):
@@ -790,6 +889,21 @@ class ObjectPoseDetector(object):
             x = preprocess_remap(self._packed, offs, hw, fmts, maps, ih, iw, self.opt.mean, self.opt.std,
                                  trans_input=trans)
         return x, meta, trans
+
+    def _decode_jpegs(self, frames, offs):
+        """The JpegFrames among frames decoded by one cp_jpeg_decode, frame b into self._packed at offs[b] as BGR.  A
+        corrupt bitstream raises ValueError naming the frame (one small copy back of the error words)."""
+        idx = [b for b, f in enumerate(frames) if isinstance(f, JpegFrame)]
+        if not idx:
+            return
+        data = np.concatenate([frames[b].data for b in idx])
+        starts = np.cumsum([0] + [len(frames[b].data) for b in idx[:-1]])
+        enc = torch.from_numpy(data).to(self.opt.device, non_blocking=True)
+        errors = jpeg_decode([frames[b].header for b in idx], enc, starts, self._packed, [offs[b] for b in idx])
+        bad = errors.cpu().numpy()
+        for k, b in enumerate(idx):
+            if bad[k]:
+                raise ValueError("run_batch: frame %d is a corrupt JPEG (%s)" % (b, jpeg_error_text(bad[k])))
 
     def _meta_rows(self, meta):
         """Host meta rows -> a device tensor, uploaded again only when the rows change (a fixed frame size and camera
@@ -812,6 +926,7 @@ class ObjectPoseDetector(object):
         optional (tracks, n_tracks) CUDA tensors of those shapes to write into."""
         S = len(frames)
         dists = slot_distortions(distortion, S)
+        frames, pixel_format = jpeg_frames(frames, pixel_format)
         if dists is not None:
             self._check_undistort(pixel_format)
         check_frames(frames, allow_idle=True, pixel_format=pixel_format)
@@ -990,6 +1105,7 @@ class MultiCategoryDetector(ObjectPoseDetector):
         optional (poses, n_valid) CUDA tensors of those shapes to write into."""
         if isinstance(frames, (list, tuple)):
             dists = slot_distortions(distortion, len(frames))
+            frames, pixel_format = jpeg_frames(frames, pixel_format)
             check_frames(frames, allow_idle=False, pixel_format=pixel_format)
             x, meta, _ = self._ragged_input(frames, camera_matrix, pixel_format, dists)
         else:

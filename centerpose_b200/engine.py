@@ -517,6 +517,59 @@ def preprocess(frames_u8, dst_h, dst_w, mean, std, out=None, trans_input=None, r
     return out
 
 
+def is_jpeg(data):
+    """True for encoded bytes that start like a JPEG file (FF D8 FF)."""
+    return len(data) >= 3 and bytes(data[:3]) == b"\xff\xd8\xff"
+
+
+def jpeg_bytes(frame):
+    """An encoded JPEG as run_batch(pixel_format="jpeg") takes it (bytes, a 1-D uint8 numpy array or CPU tensor) ->
+    a contiguous uint8 numpy array, or None for anything else."""
+    if isinstance(frame, (bytes, bytearray, memoryview)):
+        return np.frombuffer(frame, np.uint8)
+    if isinstance(frame, np.ndarray) and frame.dtype == np.uint8 and frame.ndim == 1:
+        return np.ascontiguousarray(frame)
+    if isinstance(frame, torch.Tensor) and frame.dtype == torch.uint8 and frame.dim() == 1 and not frame.is_cuda:
+        return frame.contiguous().numpy()
+    return None
+
+
+def jpeg_parse(data):
+    """cp_jpeg_parse of one encoded file (a uint8 numpy array) -> its CpJpegHeader; header.status is 0 for a supported
+    file, else the cp_jpeg_refusal (_lib.JPEG_REFUSALS names it)."""
+    L = _lib.load()
+    h = _lib.CpJpegHeader()
+    L.cp_jpeg_parse(data.ctypes.data_as(ctypes.c_void_p), len(data), ctypes.byref(h))
+    return h
+
+
+def jpeg_decode(headers, bytes_u8, byte_offsets, out_u8, out_offsets, subseq_words=0):
+    """cp_jpeg_decode: the parsed JPEGs whose files start byte_offsets[b] into bytes_u8 (uint8 CUDA) decoded, bit for
+    bit cv2.imdecode, into uint8 BGR [out_h, out_w, 3] at out_offsets[b] of out_u8 (uint8 CUDA).  Returns the int32 CUDA
+    error word of each frame (0: decoded exactly; else _lib.JPEG_ERR_* bits)."""
+    L = _lib.load()
+    B = len(headers)
+    hs = (_lib.CpJpegHeader * B)(*headers)
+    dev = bytes_u8.device
+    ws_bytes = L.cp_jpeg_workspace_bytes(hs, B)
+    if ws_bytes == 0:
+        _lib.check(-1, "cp_jpeg_workspace_bytes")
+    ws = torch.empty((ws_bytes,), dtype=torch.uint8, device=dev)
+    errors = torch.empty((B,), dtype=torch.int32, device=dev)
+    bo = (ctypes.c_int64 * B)(*[int(v) for v in byte_offsets])
+    oo = (ctypes.c_int64 * B)(*[int(v) for v in out_offsets])
+    with torch.cuda.device(dev):
+        rc = L.cp_jpeg_decode(hs, B, _ptr(bytes_u8), bo, _ptr(out_u8), oo, _ptr(ws), ctypes.c_size_t(ws_bytes),
+                              _ptr(errors), int(subseq_words), _stream())
+    _lib.check(rc, "cp_jpeg_decode")
+    return errors
+
+
+def jpeg_error_text(word):
+    """The cp_jpeg_error bits of a frame's error word, in words."""
+    return ", ".join(v for k, v in sorted(_lib.JPEG_ERRORS.items()) if int(word) & k)
+
+
 def _preprocess_packed(who, packed_u8, offsets, src_hw, fmt, dst_h, dst_w, mean, std, out, trans_input):
     """The call of cp_<who> on B frames packed into one buffer: (packed_u8, its bytes, offsets, src_hw, *fmt, out, B,
     dst_h, dst_w, trans_input, mean, std, stream), fmt being the entry point's format argument, if it has one."""
@@ -564,6 +617,16 @@ _CHANNELS = {"bgr": 3, "rgb24": 3, "rgba": 4, "bgra": 4, "yuyv422": 2, "uyvy422"
 _ALL_FORMATS = _lib.PIXEL_FORMATS + _lib.SENSOR_FORMATS
 
 
+# encoded JPEG frames: not a cp_pixel_format (the pre-process never sees one); run_batch(list) decodes them to BGR first
+JPEG = "jpeg"
+
+
+def _refuse_jpeg(pixel_format):
+    if isinstance(pixel_format, str) and pixel_format == JPEG:
+        raise ValueError("pixel_format \"jpeg\" takes encoded JPEG frames, which have no fixed shape to stage or capture: "
+                         "pass them as a list to run_batch(list, pixel_format=\"jpeg\")")
+
+
 def _min_side(pixel_format):
     """The least height and width of a frame in a sensor format: a Bayer mosaic's demosaic needs 3 x 3 pixels."""
     return 3 if pixel_format.startswith("bayer_") else 1
@@ -579,6 +642,7 @@ def check_pixel_format(pixel_format):
     if isinstance(pixel_format, (list, tuple)):
         raise ValueError("pixel_format must be one name here, got a list %r; one name per camera goes with a list of "
                          "frames (run_batch(list), a graph built with one frame_hw per slot)" % (list(pixel_format),))
+    _refuse_jpeg(pixel_format)
     if pixel_format not in _ALL_FORMATS:
         raise ValueError("pixel_format must be one of %s, got %r" % (", ".join(_ALL_FORMATS), pixel_format))
     return pixel_format
@@ -592,6 +656,7 @@ def slot_formats(pixel_format, n, who="run_batch"):
         raise ValueError("%s: pixel_format is one name or one per frame, got %d names for %d frames"
                          % (who, len(pixel_format), n))
     for f in pixel_format:
+        _refuse_jpeg(f)
         if isinstance(f, (list, tuple)) or f not in _ALL_FORMATS:
             raise ValueError("pixel_format must be one of %s, got %r in %r"
                              % (", ".join(_ALL_FORMATS), f, list(pixel_format)))

@@ -36,6 +36,8 @@
  *   cp_preprocess / cp_preprocess_affine / cp_preprocess_ragged / cp_preprocess_yuv420 / cp_preprocess_formats /
  *   cp_preprocess_resize_affine
  *       detectors/base_detector.py:91-148 pre_process (resize + affine warp + normalise)
+ *   cp_jpeg_parse / cp_jpeg_decode
+ *       detectors/base_detector.py:412 cv2.imread of run()'s image path (libjpeg-turbo's baseline decoder)
  */
 #ifndef CENTERPOSE_B200_H_
 #define CENTERPOSE_B200_H_
@@ -807,6 +809,76 @@ int cp_preprocess_slots_rows_dev(const uint8_t* frames, const void* table, int32
  * the kernel runs, WITHOUT checking: the caller guarantees every map[i] is below the rows of src.  Bad arguments return
  * CP_ERR_INVALID before any work is enqueued. */
 int cp_gather_rows_dev(const void* src, void* dst, int64_t row_bytes, int32_t n, const int32_t* map, void* stream);
+
+/* ---- JPEG decode (jpeg.cu) -------------------------------------------------
+ * Baseline sequential JPEG (SOF0 / SOF1, 8-bit, one interleaved scan of 1 or 3 components, luma sampling 1x1, 2x1,
+ * 1x2, 2x2 or 4x1 with chroma 1x1, any restart interval, 8- or 16-bit DQT, DHT present or absent -- absent tables are
+ * the standard ones of T.81 Annex K.3, as MJPEG frames need) decoded on the device into uint8 BGR [H, W, 3], bit for bit
+ * cv2.imdecode(bytes, IMREAD_COLOR): libjpeg-turbo's integer pipeline (islow IDCT, fancy chroma up-sampling, the
+ * jdcolor.c fixed-point YCbCr -> BGR) and the EXIF orientation applied as cv2 applies it.  Everything else is refused by
+ * cp_jpeg_parse with a cp_jpeg_refusal before any device work. */
+enum cp_jpeg_refusal {
+  CP_JPEG_OK = 0,
+  CP_JPEG_NOT_JPEG = 1,       /* no SOI */
+  CP_JPEG_TRUNCATED = 2,      /* the headers end before the scan */
+  CP_JPEG_PROGRESSIVE = 3,    /* SOF2 / SOF6 / SOF10 / SOF14 */
+  CP_JPEG_LOSSLESS = 4,       /* SOF3 / SOF7 / SOF11 / SOF15 */
+  CP_JPEG_ARITHMETIC = 5,     /* SOF9 (and the other arithmetic SOFs), DAC */
+  CP_JPEG_PRECISION = 6,      /* samples other than 8 bits */
+  CP_JPEG_COMPONENTS = 7,     /* not 1 or 3 components */
+  CP_JPEG_MULTI_SCAN = 8,     /* a scan without every component, or a second scan */
+  CP_JPEG_DNL = 9,            /* the height comes from a DNL marker */
+  CP_JPEG_SAMPLING = 10,      /* another sampling layout */
+  CP_JPEG_RGB = 11,           /* RGB-coded (Adobe transform 0, or component ids 'R' 'G' 'B') */
+  CP_JPEG_BAD_TABLE = 12,     /* a missing or malformed DQT / DHT */
+  CP_JPEG_BAD_HEADER = 13,    /* any other malformed header */
+  CP_JPEG_TOO_LARGE = 14      /* more than 2^30 pixels (cv2.imread refuses them too, CV_IO_MAX_IMAGE_PIXELS) */
+};
+#define CP_JPEG_MAX_COMPONENTS 3
+/* One Huffman table, derived on the host: look[code of the next 9 bits] = (length << 8) | symbol for codes of at most
+ * 9 bits (0 otherwise); longer codes through libjpeg's maxcode / valoffset (maxcode[l] = -1: no code of length l). */
+typedef struct cp_jpeg_huff {
+  uint16_t look[512];
+  int32_t maxcode[18];
+  int32_t valoffset[18];
+  uint8_t vals[256];
+} cp_jpeg_huff;
+/* What cp_jpeg_parse reads from a file.  width x height is the coded frame, out_h x out_w the decoded image after the
+ * EXIF orientation (1..8).  The scan's entropy-coded bytes are [scan_begin, scan_end) of the file. */
+typedef struct cp_jpeg_header {
+  int32_t status;                 /* cp_jpeg_refusal */
+  int32_t width, height, out_h, out_w, orientation;
+  int32_t ncomp;                  /* 1 (gray) or 3 (YCbCr) */
+  int32_t hmax, vmax;             /* luma sampling; 1 x 1 for gray */
+  int32_t mcux, mcuy, blocks_per_mcu, restart_interval;
+  int64_t scan_begin, scan_end;
+  int32_t comp_h[CP_JPEG_MAX_COMPONENTS], comp_v[CP_JPEG_MAX_COMPONENTS];
+  int16_t quant[CP_JPEG_MAX_COMPONENTS][64];          /* natural order, as the IDCT multiplies (libjpeg's short) */
+  cp_jpeg_huff dc[CP_JPEG_MAX_COMPONENTS], ac[CP_JPEG_MAX_COMPONENTS];
+} cp_jpeg_header;
+/* Host only, no GPU: parses the n bytes of a JPEG file and fills *h.  Returns 0 when the file is supported, else
+ * CP_ERR_INVALID with the reason in h->status (and cp_last_error). */
+int cp_jpeg_parse(const uint8_t* bytes, int64_t n, cp_jpeg_header* h);
+/* Device workspace bytes cp_jpeg_decode needs for these B parsed headers at any subseq_words; 0 for bad arguments. */
+size_t cp_jpeg_workspace_bytes(const cp_jpeg_header* headers, int32_t B);
+/* Decodes B parsed JPEGs in one launch per phase.  headers: HOST [B]; file b's bytes start byte_offsets[b] (HOST int64)
+ * into the DEVICE buffer d_bytes; its BGR image (uint8 [out_h, out_w, 3]) is written at DEVICE d_bgr + out_offsets[b]
+ * (HOST int64).  d_errors: DEVICE int32 [B], set to 0 for a frame decoded exactly and to a cp_jpeg_error mask for a
+ * corrupt stream; every read is bounded by its restart segment, so a corrupt frame touches nothing but its error word
+ * and its own output.  subseq_words: the length in 32-bit words of the subsequences of the parallel Huffman decode (0
+ * = the library's default).  The call waits on `stream` once per synchronisation round of the Huffman decode.  Bad
+ * arguments (a refused header, a small workspace) return CP_ERR_INVALID before any work. */
+enum cp_jpeg_error {
+  CP_JPEG_ERR_CODE = 1,       /* a Huffman code that is in no table */
+  CP_JPEG_ERR_RUN = 2,        /* an AC run past coefficient 63 */
+  CP_JPEG_ERR_SHORT = 4,      /* a restart segment ends before its MCU count */
+  CP_JPEG_ERR_RESTART = 8     /* a missing or misnumbered RST marker */
+};
+int cp_jpeg_decode(const cp_jpeg_header* headers, int32_t B, const uint8_t* d_bytes, const int64_t* byte_offsets,
+                   uint8_t* d_bgr, const int64_t* out_offsets, void* workspace, size_t ws_bytes, int32_t* d_errors,
+                   int32_t subseq_words, void* stream);
+/* The synchronisation rounds the last cp_jpeg_decode of this thread took (1 when every subsequence started exact). */
+int cp_jpeg_last_rounds(void);
 
 /* ---- misc ------------------------------------------------------------------ */
 int cp_version(void);
