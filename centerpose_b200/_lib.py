@@ -64,6 +64,8 @@ EXPORTS = [
     "cp_preprocess_formats", "cp_preprocess_frame_table_formats", "cp_plan_op_ksegments", "cp_plan_ksegments",
     "cp_preprocess_remap", "cp_preprocess_frame_table_maps", "cp_preprocess_resize_affine",
     "cp_jpeg_parse", "cp_jpeg_workspace_bytes", "cp_jpeg_decode", "cp_jpeg_last_rounds",
+    "cp_jpeg_slots_workspace_bytes", "cp_jpeg_slots_block_bytes", "cp_jpeg_slots_prepare", "cp_jpeg_decode_slots_dev",
+    "cp_jpeg_mask_counts_dev",
 ]
 
 # cp_pixel_format; "bgr" is the interleaved uint8 [H,W,3] input of every other pre-process entry point.  The camera
@@ -89,9 +91,10 @@ JPEG_REFUSALS = {0: "ok", 1: "not a JPEG file", 2: "truncated header", 3: "progr
                  8: "more than one scan", 9: "height set by a DNL marker", 10: "unsupported chroma sampling",
                  11: "RGB-coded JPEG", 12: "missing or malformed DQT / DHT", 13: "malformed header",
                  14: "more than 2^30 pixels"}
-JPEG_ERR_CODE, JPEG_ERR_RUN, JPEG_ERR_SHORT, JPEG_ERR_RESTART = 1, 2, 4, 8
+JPEG_ERR_CODE, JPEG_ERR_RUN, JPEG_ERR_SHORT, JPEG_ERR_RESTART, JPEG_ERR_SYNC = 1, 2, 4, 8, 16
 JPEG_ERRORS = {JPEG_ERR_CODE: "invalid Huffman code", JPEG_ERR_RUN: "AC run past coefficient 63",
-               JPEG_ERR_SHORT: "restart segment ends early", JPEG_ERR_RESTART: "missing or misnumbered RST marker"}
+               JPEG_ERR_SHORT: "restart segment ends early", JPEG_ERR_RESTART: "missing or misnumbered RST marker",
+               JPEG_ERR_SYNC: "Huffman synchronisation timed out"}
 
 # cp_plan_create_ex / cp_plan_memory flags
 CP_PLAN_REUSE_ACTIVATIONS = 1
@@ -310,10 +313,20 @@ def load():
     L.cp_jpeg_workspace_bytes.restype = ctypes.c_size_t
     L.cp_jpeg_decode.argtypes = [ctypes.POINTER(CpJpegHeader), i32, vp, vp, vp, vp, vp, ctypes.c_size_t, vp, i32, vp]
     L.cp_jpeg_last_rounds.argtypes = []
+    L.cp_jpeg_slots_workspace_bytes.argtypes = [i32, ctypes.POINTER(i32), ctypes.POINTER(i64), i32]
+    L.cp_jpeg_slots_workspace_bytes.restype = ctypes.c_size_t
+    L.cp_jpeg_slots_block_bytes.argtypes = [i32]
+    L.cp_jpeg_slots_block_bytes.restype = ctypes.c_size_t
+    L.cp_jpeg_slots_prepare.argtypes = [i32, ctypes.POINTER(i32), ctypes.POINTER(i64), i32, ctypes.POINTER(CpJpegHeader),
+                                        ctypes.POINTER(i64), ctypes.POINTER(i64), vp]
+    L.cp_jpeg_decode_slots_dev.argtypes = [vp, i32, ctypes.POINTER(i32), ctypes.POINTER(i64), i32, vp, vp, vp,
+                                           ctypes.c_size_t, vp, vp]
+    L.cp_jpeg_mask_counts_dev.argtypes = [vp, vp, i32, i32, vp, vp]
     for name in EXPORTS:
         fn = getattr(L, name)
         if name not in ("cp_version", "cp_last_error", "cp_plan_bytes", "cp_plan_forward_launches",
-                        "cp_decode_workspace_bytes", "cp_preprocess_frame_table_bytes", "cp_jpeg_workspace_bytes"):
+                        "cp_decode_workspace_bytes", "cp_preprocess_frame_table_bytes", "cp_jpeg_workspace_bytes",
+                        "cp_jpeg_slots_workspace_bytes", "cp_jpeg_slots_block_bytes"):
             fn.restype = ctypes.c_int
     _lib = L
     return L

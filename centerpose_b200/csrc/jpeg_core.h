@@ -347,6 +347,42 @@ JPG_HD void pixel(const cp_jpeg_header& h, const uint8_t* const* planes, const i
   bgr[2] = (uint8_t)clampi(Y + cr_r(cr), 0, 255);
 }
 
+// ---------------------------------------------------------------- the capacity of a slot of one decoded size
+// Upper bounds on what one frame needs in the decode workspace, for every supported file that decodes to out_h x out_w
+// (the coded frame in either orientation, any sampling, gray included, any restart interval) in at most max_bytes
+// bytes, at `words` 32-bit words per subsequence: its compacted scan bytes, restart segments (at most one per MCU),
+// subsequences, blocks and component-plane bytes.  A plane holds whole blocks, so the plane bytes are 64 per block.
+struct SlotCap {
+  int64_t comp, nseg, nsub, nblocks, nplane;
+};
+
+// What one parsed frame needs, in the same terms (jpeg.cu's workspace layouts size by it).
+JPG_HD SlotCap frame_need(const cp_jpeg_header& h, int words) {
+  const int64_t nraw = h.scan_end - h.scan_begin, nmcu = (int64_t)h.mcux * h.mcuy;
+  SlotCap c{nraw + 8, h.restart_interval ? (nmcu + h.restart_interval - 1) / h.restart_interval : 1, 0,
+            nmcu * h.blocks_per_mcu, 0};
+  c.nsub = (nraw * 8 + 32 * words - 1) / (32 * words) + c.nseg;
+  for (int k = 0; k < h.ncomp; ++k) c.nplane += (int64_t)plane_w(h, k) * plane_h(h, k);
+  return c;
+}
+
+JPG_HD SlotCap slot_capacity(int out_h, int out_w, int64_t max_bytes, int words) {
+  SlotCap c{max_bytes + 8, 0, 0, 0, 0};
+  const int hs[6] = {1, 2, 1, 2, 4, 1}, vs[6] = {1, 1, 2, 2, 1, 1};      // luma 1x1 2x1 1x2 2x2 4x1, then gray
+  for (int o = 0; o < 2; ++o) {
+    const int64_t w = o ? out_h : out_w, h = o ? out_w : out_h;
+    for (int k = 0; k < 6; ++k) {
+      const int64_t nmcu = ((w + 8 * hs[k] - 1) / (8 * hs[k])) * ((h + 8 * vs[k] - 1) / (8 * vs[k]));
+      const int64_t nb = k == 5 ? nmcu : nmcu * (hs[k] * vs[k] + 2);
+      if (nmcu > c.nseg) c.nseg = nmcu;
+      if (nb > c.nblocks) c.nblocks = nb;
+    }
+  }
+  c.nsub = (max_bytes * 8 + 32 * words - 1) / (32 * words) + c.nseg;
+  c.nplane = c.nblocks * 64;
+  return c;
+}
+
 // ---------------------------------------------------------------- host: the header parser
 // T.81 Annex K.3 (Tables K.3 - K.6), the tables libjpeg-turbo installs in slots 0 (luma) and 1 (chroma) of each class
 // when a file defines none there (MJPEG).  bits[l] = number of codes of length l (1..16).

@@ -621,10 +621,18 @@ _ALL_FORMATS = _lib.PIXEL_FORMATS + _lib.SENSOR_FORMATS
 JPEG = "jpeg"
 
 
+# an MJPEG camera: encoded baseline JPEG frames of one decoded size, which the live-video graphs decode (graph.py)
+MJPEG = "mjpeg"
+
+
 def _refuse_jpeg(pixel_format):
     if isinstance(pixel_format, str) and pixel_format == JPEG:
         raise ValueError("pixel_format \"jpeg\" takes encoded JPEG frames, which have no fixed shape to stage or capture: "
                          "pass them as a list to run_batch(list, pixel_format=\"jpeg\")")
+    if isinstance(pixel_format, str) and pixel_format == MJPEG:
+        raise ValueError("pixel_format \"mjpeg\" is an MJPEG camera of one frame size, decoded inside the live-video "
+                         "graphs (DetectGraph, TrackGraph and their multi-category forms); encoded frames of any size go "
+                         "as a list to run_batch(list, pixel_format=\"jpeg\")")
 
 
 def _min_side(pixel_format):

@@ -6,12 +6,13 @@ control copy and one replay).  A graph class defines its step: the opt it refuse
 (`_buffers`), the launches of a step (`_step`) and its outputs (`_out`).  `DetectGraph` / `MultiCategoryDetectGraph`
 here replay run_batch of a detection model; `TrackGraph` / `MultiCategoryTrackGraph` (tracker.py) the tracking step."""
 import ctypes
+import warnings
 
 import numpy as np
 import torch
 
 from . import _lib
-from .engine import _ptr, _stream
+from .engine import MJPEG, _ptr, _stream
 
 
 def _frame_sizes(frame_hw, S, who):
@@ -34,6 +35,7 @@ class _SlotGraph(object):
     _refuse(opt, who), _buffers(opt, meta, trans), _steps(), _step(p) and set self._out in _buffers."""
 
     _host_list = "run_batch(list)"                    # where idle slots and mixed sizes run without a graph
+    _mjpeg = ()                                       # the "mjpeg" slots, whose step decodes their frames first
 
     def _refuse(self, opt, who):
         """Raise for an opt the step does not take, before any device work."""
@@ -59,7 +61,8 @@ class _SlotGraph(object):
         eng.load_state_dict(m.state_dict())
         return eng, decode_params(det.opt, test_scale=1.0), None
 
-    def _build(self, det, slots, frame_hw, camera_matrix, pixel_format, idle_slots=False, distortion=None):
+    def _build(self, det, slots, frame_hw, camera_matrix, pixel_format, idle_slots=False, distortion=None,
+               max_frame_bytes=None):
         """Checks, buffers and the captured steps; everything that refuses comes before any device work."""
         from .detector import affine_from_center_scale, camera_per_frame
         from .engine import check_pixel_format, frame_shape, make_meta, map_pointers, slot_formats
@@ -78,6 +81,14 @@ class _SlotGraph(object):
         if isinstance(pixel_format, (list, tuple)) and not self.per_slot:
             raise ValueError("%s: one pixel_format per slot goes with one frame_hw per slot; with one frame_hw every "
                              "slot takes one name, got %r" % (who, list(pixel_format)))
+        # "mjpeg" slots are BGR slots whose frames the step decodes first; no other code learns the name
+        names = list(pixel_format) if isinstance(pixel_format, (list, tuple)) else [pixel_format] * S
+        self._mjpeg = [b for b, f in enumerate(names) if isinstance(f, str) and f == MJPEG] if len(names) == S else []
+        if self._mjpeg:
+            shown = pixel_format
+            pixel_format = (["bgr" if b in self._mjpeg else f for b, f in enumerate(names)]
+                            if isinstance(pixel_format, (list, tuple)) else "bgr")
+        max_bytes = self._max_frame_bytes(max_frame_bytes, sizes if self.per_slot else sizes * S, who)
         fmts = slot_formats(pixel_format, S, who) if self.per_slot else [check_pixel_format(pixel_format)]
         # one name repeated is that name: the same table, launches and bits
         self.pixel_format = fmts[0] if len(set(fmts)) == 1 else fmts
@@ -111,6 +122,8 @@ class _SlotGraph(object):
         self._std = (ctypes.c_float * 3)(*[float(v) for v in opt.std])
         mixed = isinstance(self.pixel_format, list)       # per-slot formats: a table of them, one per-frame launch
         self._fmt = _lib.CP_PIX_PER_FRAME if mixed else _lib.PIXEL_FORMAT_CODES[self.pixel_format]
+        if self._mjpeg:
+            self.pixel_format = shown if isinstance(shown, str) or len(set(shown)) > 1 else shown[0]
         # a frame table with one frame_hw per slot, idle slots or lens distortion (with one frame_hw: S equal sizes)
         self._table = self.per_slot or self.idle_slots or dists is not None
         if self._table:
@@ -144,6 +157,9 @@ class _SlotGraph(object):
                                                            _ptr(self.table), _stream()), "cp_preprocess_frame_table")
         else:
             self.frames = torch.zeros(self.frame_shape, dtype=torch.uint8, device=dev)
+            offs = np.arange(S, dtype=np.int64) * int(np.prod(shapes[0]))
+        if self._mjpeg:
+            self._jpeg_buffers(max_bytes, offs)
         if self.idle_slots:
             # one int32 control block per call (_control): start flags [M*S], rows [S] (the slot of each live row), ids
             # [M*S] (the row m * S + slot of each live row of each category) and inv [M*S] (the live row of each
@@ -181,6 +197,112 @@ class _SlotGraph(object):
 
     def _warmed(self):
         """After the warm-up steps, before the capture."""
+
+    # ---- MJPEG slots -------------------------------------------------------------------------------------------------
+    def _max_frame_bytes(self, max_frame_bytes, sizes, who):
+        """The encoded bytes each slot takes: max_frame_bytes (one int or one per slot), by default H * W * 3."""
+        if max_frame_bytes is None:
+            return [h * w * 3 for h, w in sizes]
+        if not self._mjpeg:
+            raise ValueError("%s: max_frame_bytes caps the encoded frames of \"mjpeg\" slots, and no slot is one"
+                             % who)
+        per = list(max_frame_bytes) if isinstance(max_frame_bytes, (list, tuple, np.ndarray)) else \
+            [max_frame_bytes] * len(sizes)
+        if len(per) != len(sizes) or any(int(v) != v or not 1 <= int(v) < 1 << 28 for v in per):
+            raise ValueError("%s: max_frame_bytes is one int or one per slot, each 1 .. 2^28 - 1, got %r"
+                             % (who, max_frame_bytes))
+        return [int(v) for v in per]
+
+    def _jpeg_buffers(self, max_bytes, offs):
+        """The slot decode's sizes, device block, encoded-byte buffer, workspace and error words; the block starts with
+        every slot skipped."""
+        L, S, dev = self.L, self.slots, self.device
+        self._jhw = np.ascontiguousarray(self._slot_hw, np.int32)
+        self._jmax = np.ascontiguousarray(max_bytes, np.int64)
+        self._jbyte_offs = np.concatenate([[0], np.cumsum(self._jmax)[:-1]]).astype(np.int64)
+        self._jout = np.ascontiguousarray(offs, np.int64)
+        self._jblock_host = np.zeros(int(L.cp_jpeg_slots_block_bytes(S)), np.uint8)
+        ws = L.cp_jpeg_slots_workspace_bytes(S, self._jhw.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)),
+                                             self._jmax.ctypes.data_as(ctypes.POINTER(ctypes.c_int64)), 0)
+        if ws == 0:
+            _lib.check(-1, "cp_jpeg_slots_workspace_bytes")
+        self._jws = torch.empty((int(ws),), dtype=torch.uint8, device=dev)
+        self._jbytes = torch.zeros((int(self._jmax.sum()),), dtype=torch.uint8, device=dev)
+        self._jblock = torch.zeros((self._jblock_host.size,), dtype=torch.uint8, device=dev)
+        self.decode_errors = torch.zeros((S,), dtype=torch.int32, device=dev)
+        self._prepare([None] * S)
+        self._jblock.copy_(torch.from_numpy(self._jblock_host))
+
+    def _encoded(self, b, f):
+        """The encoded frame of MJPEG slot b, checked on the host: (its bytes as a CPU tensor, its CpJpegHeader)."""
+        from .engine import jpeg_bytes, jpeg_parse
+        who = type(self).__name__
+        if torch.is_tensor(f) and f.is_cuda:
+            raise ValueError("%s: slot %d is an \"mjpeg\" slot, whose header is parsed on the host: pass its frame "
+                             "from host memory, not as a CUDA tensor" % (who, b))
+        data = jpeg_bytes(f)
+        if data is None:
+            raise ValueError("%s: slot %d is an \"mjpeg\" slot: its frame is the encoded bytes (bytes, a 1-D uint8 "
+                             "numpy array or CPU tensor), got %s" % (who, b, type(f).__name__))
+        if len(data) > self._jmax[b]:
+            raise ValueError("%s: slot %d takes encoded frames of at most max_frame_bytes = %d bytes, got %d"
+                             % (who, b, self._jmax[b], len(data)))
+        h = jpeg_parse(data)
+        if h.status:
+            raise ValueError("%s: slot %d is a JPEG the device decoder does not take: %s"
+                             % (who, b, _lib.JPEG_REFUSALS.get(h.status, h.status)))
+        if (h.out_h, h.out_w) != tuple(self._slot_hw[b]):
+            raise ValueError("%s: slot %d decodes to %d x %d, its frame_hw is %s"
+                             % (who, b, h.out_h, h.out_w, tuple(self._slot_hw[b])))
+        if torch.is_tensor(f):
+            return f.contiguous(), h
+        with warnings.catch_warnings():                  # read-only bytes: only ever the source of a copy
+            warnings.simplefilter("ignore")
+            return torch.from_numpy(data), h
+
+    def _prepare(self, encoded):
+        """cp_jpeg_slots_prepare of one call into the host block: encoded[s] is (bytes, header) or None (skipped)."""
+        S = self.slots
+        hs = (_lib.CpJpegHeader * S)()
+        nbytes = np.zeros(S, np.int64)
+        for s, e in enumerate(encoded):
+            if e is not None:
+                hs[s], nbytes[s] = e[1], e[0].numel()
+        p64 = ctypes.POINTER(ctypes.c_int64)
+        _lib.check(self.L.cp_jpeg_slots_prepare(S, self._jhw.ctypes.data_as(ctypes.POINTER(ctypes.c_int32)),
+                                                self._jmax.ctypes.data_as(p64), 0, hs, nbytes.ctypes.data_as(p64),
+                                                self._jout.ctypes.data_as(p64),
+                                                self._jblock_host.ctypes.data_as(ctypes.c_void_p)),
+                   "cp_jpeg_slots_prepare")
+
+    def _upload_encoded(self, frames):
+        """The block and the encoded frames of one call copied in (before the replay); returns frames with the MJPEG
+        slots' entries None, so that only the other slots' frames are copied as they are."""
+        enc = [frames[b] if b in self._mjpeg else None for b in range(self.slots)]
+        self._prepare(enc)
+        # pageable sources are staged before copy_ returns, without waiting for the device
+        self._jblock.copy_(torch.from_numpy(self._jblock_host), non_blocking=True)
+        for b, e in enumerate(enc):
+            if e is not None:
+                o = int(self._jbyte_offs[b])
+                self._jbytes[o:o + e[0].numel()].copy_(e[0], non_blocking=True)
+        return [None if b in self._mjpeg else f for b, f in enumerate(frames)]
+
+    def _decode(self):
+        """The slot decode of a step, ahead of the pre-process: every live MJPEG slot's BGR frame into its region."""
+        if self._mjpeg:
+            p32, p64 = ctypes.POINTER(ctypes.c_int32), ctypes.POINTER(ctypes.c_int64)
+            _lib.check(self.L.cp_jpeg_decode_slots_dev(
+                _ptr(self._jblock), self.slots, self._jhw.ctypes.data_as(p32), self._jmax.ctypes.data_as(p64), 0,
+                _ptr(self._jbytes), _ptr(self.frames), _ptr(self._jws), ctypes.c_size_t(self._jws.numel()),
+                _ptr(self.decode_errors), _stream()), "cp_jpeg_decode_slots_dev")
+
+    def _mask(self, n_valid, n, rows=None):
+        """n_valid of a step's n rows zeroed for every slot (rows[r], or r) whose frame did not decode exactly."""
+        if self._mjpeg:
+            _lib.check(self.L.cp_jpeg_mask_counts_dev(_ptr(self.decode_errors), _ptr(rows), n,
+                                                      self.streams // self.slots, _ptr(n_valid), _stream()),
+                       "cp_jpeg_mask_counts_dev")
 
     # ---- launches the steps share ------------------------------------------------------------------------------------
     def _preprocess(self, out, start=None, prev=None):
@@ -239,6 +361,11 @@ class _SlotGraph(object):
         """The frames of one call, checked against the slots' shapes: one tensor, or one per slot (with idle slots: one
         per slot, None for an idle one)."""
         who = type(self).__name__
+        if self._mjpeg and (not isinstance(frames, (list, tuple)) or len(frames) != self.slots):
+            what = "%d entries" % len(frames) if isinstance(frames, (list, tuple)) else type(frames).__name__
+            raise ValueError("%s has \"mjpeg\" slots: frames is a list of %d entries, the encoded bytes of each "
+                             "\"mjpeg\" slot%s, got %s" % (who, self.slots, " (None for an idle slot)"
+                                                             if self.idle_slots else "", what))
         if self.idle_slots and not isinstance(frames, (list, tuple)):
             if self.per_slot or not (torch.is_tensor(frames) or isinstance(frames, np.ndarray)):
                 raise ValueError("%s was built with idle slots: frames is a list of %d frames (None for an idle slot)%s, "
@@ -250,7 +377,7 @@ class _SlotGraph(object):
                                                                                  self.pixel_format, frames.dtype,
                                                                                  tuple(frames.shape)))
             return list(frames)                         # every slot live
-        if not self.per_slot and not self.idle_slots:
+        if not self.per_slot and not self.idle_slots and not self._mjpeg:
             if isinstance(frames, np.ndarray):
                 frames = torch.from_numpy(frames)
             if not torch.is_tensor(frames) or frames.dtype != torch.uint8 or tuple(frames.shape) != self.frame_shape:
@@ -271,6 +398,9 @@ class _SlotGraph(object):
                     continue
                 raise ValueError("%s steps every slot: slot %d is idle; idle slots run through %s"
                                  % (who, b, self._host_list))
+            if b in self._mjpeg:
+                out.append(self._encoded(b, f))
+                continue
             if isinstance(f, np.ndarray):
                 f = torch.from_numpy(f)
             if not torch.is_tensor(f) or f.dtype != torch.uint8 or tuple(f.shape) != self._slot_shapes[b]:
@@ -287,8 +417,11 @@ class _SlotGraph(object):
         if self.idle_slots:
             return self._call_rows(frames, start)
         with torch.cuda.device(self.device):
+            if self._mjpeg:
+                frames = self._upload_encoded(frames)
             for dst, f in zip(self._slot_frames if self.per_slot else [self.frames.view(self.frame_shape)], frames):
-                dst.copy_(f, non_blocking=True)
+                if f is not None:
+                    dst.copy_(f, non_blocking=True)
             if start is not None:
                 # one flag per tracker stream, the same in every category; a pageable source: staged before copy_
                 # returns, without waiting for the device
@@ -314,8 +447,11 @@ class _SlotGraph(object):
             else:
                 start = np.array([i in live and (bool(start[i]) or not self._started[i]) for i in range(self.slots)],
                                  np.int32)
+            if self._mjpeg:
+                frames = self._upload_encoded(frames)
             for i in live:
-                self._slot_frames[i].copy_(frames[i], non_blocking=True)
+                if frames[i] is not None:
+                    self._slot_frames[i].copy_(frames[i], non_blocking=True)
             # a pageable source: staged before copy_ returns, without waiting for the device
             self.ctrl.copy_(torch.from_numpy(self._control(live, start)), non_blocking=True)
             self.graphs[len(live) - 1].replay()
@@ -359,17 +495,25 @@ class DetectGraph(_SlotGraph):
     distortion: the lens distortion of the cameras (lens.LensDistortion), one for every slot or a list of one per slot
     (None: an undistorted camera), as run_batch(distortion=) takes it.  The maps (lens.undistort_map) and a frame table
     with them are built with the graph, which then always pre-processes through the table; every step is bit for bit
-    run_batch(..., distortion=) on the same frames."""
+    run_batch(..., distortion=) on the same frames.
+
+    pixel_format "mjpeg" (one name, or in a per-slot list): an MJPEG camera, encoded baseline JPEG frames of the slot's
+    decoded size (bytes, a 1-D uint8 numpy array or CPU tensor); a call then takes a list of S entries.  The step
+    decodes them on the device first (cp_jpeg_decode_slots_dev) and is bit for bit run_batch(list,
+    pixel_format="jpeg").  max_frame_bytes (one int or one per slot, default H * W * 3) caps a slot's encoded size.  A
+    frame the header parser refuses, of another decoded size or over max_frame_bytes is a ValueError naming the slot;
+    a bitstream error sets the slot's word in decode_errors (int32 [S], device) and its n_valid to 0 for that step."""
 
     _host_list = "run_batch(list) of the live frames"
 
-    def __init__(self, det, slots, frame_hw, camera_matrix, pixel_format="bgr", idle_slots=False, distortion=None):
+    def __init__(self, det, slots, frame_hw, camera_matrix, pixel_format="bgr", idle_slots=False, distortion=None,
+                 max_frame_bytes=None):
         from .detector import MultiCategoryDetector, ObjectPoseDetector
         if isinstance(det, MultiCategoryDetector):
             raise NotImplementedError("DetectGraph detects one category; several run through a MultiCategoryDetectGraph")
         if not isinstance(det, ObjectPoseDetector):
             raise NotImplementedError("DetectGraph takes an ObjectPoseDetector, got %s" % type(det).__name__)
-        self._build(det, slots, frame_hw, camera_matrix, pixel_format, idle_slots, distortion)
+        self._build(det, slots, frame_hw, camera_matrix, pixel_format, idle_slots, distortion, max_frame_bytes)
 
     def _refuse(self, opt, who):
         if getattr(opt, "tracking_task", False):
@@ -401,18 +545,22 @@ class DetectGraph(_SlotGraph):
         with torch.cuda.device(self.device):
             if self.idle_slots:
                 return self._step_rows(p)
+            self._decode()
             self._preprocess(self.x)
             self.eng.infer(self.x, self.meta, self.prm, poses=self.poses, n_valid=self.n_valid)
+            self._mask(self.n_valid, self.slots)
 
     def _step_rows(self, n):
         """A step of n live slots: the row-mapped pre-process, the gather of the live rows' meta rows, the network at
         batch n into the compact rows and their scatter to the slots (zeros for idle slots).  Which slots are live is
         data in the control block; n fixes the shapes."""
         MS = self.streams
+        self._decode()
         self._preprocess_rows(n, self.x)
         self._gather(self.meta, self.meta_rows, n, self.rows)
         self.eng.infer(self.x[:n], self.meta_rows[:n], self.prm, poses=self._rows_view(self.poses_rows, n),
                        n_valid=self._rows_view(self.n_valid_rows, n))
+        self._mask(self._rows_view(self.n_valid_rows, n), n, self.rows)
         rec = self.poses.shape[-2:]
         self._gather(self.poses_rows.view((MS,) + rec), self.poses.view((MS,) + rec), MS, self.inv)
         self._gather(self.n_valid_rows.view(MS, 1), self.n_valid.view(MS, 1), MS, self.inv)
@@ -438,7 +586,8 @@ class MultiCategoryDetectGraph(DetectGraph):
 
     _host_list = "MultiCategoryDetector.run_batch(list) of the live frames"
 
-    def __init__(self, mdet, slots, frame_hw, camera_matrix, pixel_format="bgr", idle_slots=False, distortion=None):
+    def __init__(self, mdet, slots, frame_hw, camera_matrix, pixel_format="bgr", idle_slots=False, distortion=None,
+                 max_frame_bytes=None):
         from .detector import MultiCategoryDetector, MultiCategoryTracker
         if isinstance(mdet, MultiCategoryTracker):
             raise ValueError("MultiCategoryDetectGraph needs a MultiCategoryDetector; a MultiCategoryTracker runs "
@@ -446,4 +595,4 @@ class MultiCategoryDetectGraph(DetectGraph):
         if not isinstance(mdet, MultiCategoryDetector):
             raise NotImplementedError("MultiCategoryDetectGraph takes a MultiCategoryDetector; one category's "
                                       "ObjectPoseDetector goes to DetectGraph")
-        self._build(mdet, slots, frame_hw, camera_matrix, pixel_format, idle_slots, distortion)
+        self._build(mdet, slots, frame_hw, camera_matrix, pixel_format, idle_slots, distortion, max_frame_bytes)

@@ -399,12 +399,13 @@ class TrackGraph(_SlotGraph):
     _host_step = "run_batch(track=True)"              # where what the graph refuses runs
     _host_list = "run_batch(list, track=True)"
 
-    def __init__(self, det, slots, frame_hw, camera_matrix, pixel_format="bgr", idle_slots=False, distortion=None):
+    def __init__(self, det, slots, frame_hw, camera_matrix, pixel_format="bgr", idle_slots=False, distortion=None,
+                 max_frame_bytes=None):
         from .detector import ObjectPoseDetector
         if not isinstance(det, ObjectPoseDetector) or det._track_categories() is not None:
             raise NotImplementedError("TrackGraph tracks one category; several run through MultiCategoryTracker.run_batch "
                                       "or a MultiCategoryTrackGraph")
-        self._build(det, slots, frame_hw, camera_matrix, pixel_format, idle_slots, distortion)
+        self._build(det, slots, frame_hw, camera_matrix, pixel_format, idle_slots, distortion, max_frame_bytes)
 
     def _refuse(self, opt, who):
         if not getattr(opt, "tracking_task", False):
@@ -463,11 +464,13 @@ class TrackGraph(_SlotGraph):
         MS, (ih, iw), cur, prev = self.streams, self.x[p].shape[2:], self.x[p], self.x[1 - p]
         with torch.cuda.device(self.device):
             _lib.check(L.cp_tracker_reset_dev(h, MS, _ptr(self.start), st), "cp_tracker_reset_dev")
+            self._decode()
             self._preprocess(cur, self.start, prev)
             _lib.check(L.cp_tracker_render_dev(h, MS, _ptr(self.meta_all), _ptr(self.trans), ih, iw, _ptr(self.modes),
                                                _ptr(self.pre_hm), _ptr(self.pre_hm_hp), st), "cp_tracker_render_dev")
             self.eng.infer(cur, self.meta, self.prm, prev, self.pre_hm, self.pre_hm_hp, poses=self.poses,
                            n_valid=self.n_valid)
+            self._mask(self.n_valid, self.slots)
             _lib.check(L.cp_tracker_step(h, MS, _ptr(self.poses), _ptr(self.n_valid), self.poses.shape[-2],
                                          _ptr(self.meta_all), _ptr(self.tracks), _ptr(self.n_tracks), st), "cp_tracker_step")
 
@@ -483,6 +486,7 @@ class TrackGraph(_SlotGraph):
         poses, n_valid = self._rows_view(self.poses, n), self._rows_view(self.n_valid, n)
         with torch.cuda.device(self.device):
             _lib.check(L.cp_tracker_reset_dev(h, MS, _ptr(self.start), st), "cp_tracker_reset_dev")
+            self._decode()
             self._preprocess_rows(n, cur, self.start, self.store, prev)
             self._gather(self.meta, self.meta_rows, n, self.rows)
             self._gather(self.meta_all, self.meta_trk, Mn, self.ids)
@@ -492,6 +496,7 @@ class TrackGraph(_SlotGraph):
                        "cp_tracker_render_dev2")
             self.eng.infer(cur[:n], self.meta_rows[:n], self.prm, prev[:n], pre_hm, pre_hm_hp, poses=poses,
                            n_valid=n_valid)
+            self._mask(n_valid, n, self.rows)
             _lib.check(L.cp_tracker_step_dev(h, Mn, _ptr(self.ids), _ptr(poses), _ptr(n_valid), poses.shape[-2],
                                              _ptr(self.meta_trk), _ptr(self.tracks_rows), _ptr(self.n_tracks_rows), st),
                        "cp_tracker_step_dev")
@@ -533,7 +538,8 @@ class MultiCategoryTrackGraph(TrackGraph):
     _host_step = "MultiCategoryTracker.run_batch"
     _host_list = "MultiCategoryTracker.run_batch(list)"
 
-    def __init__(self, trk, slots, frame_hw, camera_matrix, pixel_format="bgr", idle_slots=False, distortion=None):
+    def __init__(self, trk, slots, frame_hw, camera_matrix, pixel_format="bgr", idle_slots=False, distortion=None,
+                 max_frame_bytes=None):
         from .detector import MultiCategoryDetector, MultiCategoryTracker
         if not isinstance(trk, MultiCategoryTracker):
             if isinstance(trk, MultiCategoryDetector):
@@ -541,4 +547,4 @@ class MultiCategoryTrackGraph(TrackGraph):
                                  "tracking model")
             raise NotImplementedError("MultiCategoryTrackGraph takes a MultiCategoryTracker; one category's "
                                       "ObjectPoseDetector goes to TrackGraph")
-        self._build(trk, slots, frame_hw, camera_matrix, pixel_format, idle_slots, distortion)
+        self._build(trk, slots, frame_hw, camera_matrix, pixel_format, idle_slots, distortion, max_frame_bytes)

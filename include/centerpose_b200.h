@@ -872,13 +872,45 @@ enum cp_jpeg_error {
   CP_JPEG_ERR_CODE = 1,       /* a Huffman code that is in no table */
   CP_JPEG_ERR_RUN = 2,        /* an AC run past coefficient 63 */
   CP_JPEG_ERR_SHORT = 4,      /* a restart segment ends before its MCU count */
-  CP_JPEG_ERR_RESTART = 8     /* a missing or misnumbered RST marker */
+  CP_JPEG_ERR_RESTART = 8,    /* a missing or misnumbered RST marker */
+  CP_JPEG_ERR_SYNC = 16       /* cp_jpeg_decode_slots_dev: a CTA waited about a second for its predecessor's state */
 };
 int cp_jpeg_decode(const cp_jpeg_header* headers, int32_t B, const uint8_t* d_bytes, const int64_t* byte_offsets,
                    uint8_t* d_bgr, const int64_t* out_offsets, void* workspace, size_t ws_bytes, int32_t* d_errors,
                    int32_t subseq_words, void* stream);
 /* The synchronisation rounds the last cp_jpeg_decode of this thread took (1 when every subsequence started exact). */
 int cp_jpeg_last_rounds(void);
+
+/* The slot decode, safe to capture in a CUDA graph: S slots of fixed decoded size hw[s] = (out_h, out_w) (HOST int32
+ * [S][2], after the EXIF orientation), each taking one encoded frame of at most max_bytes[s] bytes (HOST int64 [S]) per
+ * call.  Every grid and workspace offset depends only on S, hw, max_bytes and subseq_words; what changes per frame
+ * (sampling, quality, tables, restart interval, orientation, length) is read on the device from a control block.  A
+ * call: cp_jpeg_slots_prepare fills the block on the host, the caller copies it to a DEVICE buffer of
+ * cp_jpeg_slots_block_bytes(S) bytes and slot s's file to d_bytes + the sum of max_bytes[0..s-1], and the captured
+ * cp_jpeg_decode_slots_dev decodes.  The result is bit for bit cp_jpeg_decode's (cv2.imdecode's) at any
+ * subseq_words. */
+/* Device workspace bytes of these slots at subseq_words (0 = the default); 0 for bad arguments.  Host only. */
+size_t cp_jpeg_slots_workspace_bytes(int32_t S, const int32_t* hw, const int64_t* max_bytes, int32_t subseq_words);
+/* Bytes of the control block of S slots: S cp_jpeg_header, then the per-slot jobs (256-byte aligned); 0 for S <= 0. */
+size_t cp_jpeg_slots_block_bytes(int32_t S);
+/* Host only, no GPU: fills host_block (cp_jpeg_slots_block_bytes(S) bytes) for one call.  headers[s]: slot s's file
+ * parsed by cp_jpeg_parse; nbytes[s]: its length, 0 to skip the slot this call (its header in the block is zeroed, its
+ * output is not written and its error word is 0); out_offsets[s]: where its BGR image [out_h, out_w, 3] goes in d_bgr.
+ * A live slot whose header is refused, decodes to another size than hw[s], or has more than max_bytes[s] bytes (or a
+ * scan past nbytes[s]) returns CP_ERR_INVALID naming the slot, and the block is left as it was. */
+int cp_jpeg_slots_prepare(int32_t S, const int32_t* hw, const int64_t* max_bytes, int32_t subseq_words,
+                          const cp_jpeg_header* headers, const int64_t* nbytes, const int64_t* out_offsets,
+                          void* host_block);
+/* Decodes the slots of the DEVICE block d_block with no host round trip: one launch per phase over capacity-sized
+ * grids, the Huffman synchronisation in one chained launch.  d_errors: DEVICE int32 [S], each slot's cp_jpeg_error mask
+ * (0 for a skipped slot).  A corrupt frame touches nothing but its own error word, workspace regions and output. */
+int cp_jpeg_decode_slots_dev(const void* d_block, int32_t S, const int32_t* hw, const int64_t* max_bytes,
+                             int32_t subseq_words, const uint8_t* d_bytes, uint8_t* d_bgr, void* workspace,
+                             size_t ws_bytes, int32_t* d_errors, void* stream);
+/* Safe to capture: d_n_valid[m * n + r] = 0 for m < M, r < n when d_errors[slot] != 0, slot = d_rows[r] (DEVICE int32
+ * [n]) or r when d_rows is NULL.  A slot whose frame did not decode exactly detects nothing. */
+int cp_jpeg_mask_counts_dev(const int32_t* d_errors, const int32_t* d_rows, int32_t n, int32_t M, int32_t* d_n_valid,
+                            void* stream);
 
 /* ---- misc ------------------------------------------------------------------ */
 int cp_version(void);
