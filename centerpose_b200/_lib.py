@@ -72,18 +72,25 @@ EXPORTS = [
 # formats carry ffmpeg's pix_fmt names; CP_PIX_PER_FRAME launches a frame table of per-frame formats, and CP_PIX_REMAP
 # OR-ed into either launches a table with coordinate maps (cp_preprocess_frame_table_maps).
 CP_PIX_NV12, CP_PIX_I420, CP_PIX_BGR = 0, 1, 2
+CP_PIX_NV21, CP_PIX_YV12, CP_PIX_NV12_FULL, CP_PIX_I420_FULL, CP_PIX_NV21_FULL, CP_PIX_YV12_FULL = 10, 11, 12, 13, 14, 15
 CP_PIX_RGB24, CP_PIX_RGBA, CP_PIX_BGRA, CP_PIX_YUYV422, CP_PIX_UYVY422 = 16, 17, 18, 32, 33
 CP_PIX_GRAY, CP_PIX_BAYER_RGGB8, CP_PIX_BAYER_BGGR8, CP_PIX_BAYER_GBRG8, CP_PIX_BAYER_GRBG8 = 48, 49, 50, 51, 52
 CP_PIX_PER_FRAME = 64
 CP_PIX_REMAP = 128
 # the colour formats, and the sensor formats: one uint8 [H,W] plane per frame, mono or a Bayer mosaic named after its
-# pixels (0,0) (0,1) / (1,0) (1,1) as ffmpeg, V4L2 and ROS name it
+# pixels (0,0) (0,1) / (1,0) (1,1) as ffmpeg, V4L2 and ROS name it; the phone formats: YUV 4:2:0 as Android and ARKit
+# give it, NV21 / YV12 (chroma swapped) in limited range and all four 4:2:0 layouts in full range ("_full", JFIF)
 PIXEL_FORMATS = ("bgr", "nv12", "i420", "rgb24", "rgba", "bgra", "yuyv422", "uyvy422")
 SENSOR_FORMATS = ("gray", "bayer_rggb8", "bayer_bggr8", "bayer_gbrg8", "bayer_grbg8")
+PHONE_FORMATS = ("nv21", "yv12", "nv12_full", "nv21_full", "i420_full", "yv12_full")
 PIXEL_FORMAT_CODES = {"bgr": CP_PIX_BGR, "nv12": CP_PIX_NV12, "i420": CP_PIX_I420, "rgb24": CP_PIX_RGB24,
                       "rgba": CP_PIX_RGBA, "bgra": CP_PIX_BGRA, "yuyv422": CP_PIX_YUYV422, "uyvy422": CP_PIX_UYVY422,
                       "gray": CP_PIX_GRAY, "bayer_rggb8": CP_PIX_BAYER_RGGB8, "bayer_bggr8": CP_PIX_BAYER_BGGR8,
-                      "bayer_gbrg8": CP_PIX_BAYER_GBRG8, "bayer_grbg8": CP_PIX_BAYER_GRBG8}
+                      "bayer_gbrg8": CP_PIX_BAYER_GBRG8, "bayer_grbg8": CP_PIX_BAYER_GRBG8,
+                      "nv21": CP_PIX_NV21, "yv12": CP_PIX_YV12, "nv12_full": CP_PIX_NV12_FULL,
+                      "nv21_full": CP_PIX_NV21_FULL, "i420_full": CP_PIX_I420_FULL, "yv12_full": CP_PIX_YV12_FULL}
+# every 4:2:0 format, uint8 [3H/2,W] with H and W even
+YUV420_FORMATS = ("nv12", "i420") + PHONE_FORMATS
 
 # cp_jpeg_refusal: why cp_jpeg_parse refuses a file; cp_jpeg_error: the bits of a frame's error word after cp_jpeg_decode
 JPEG_REFUSALS = {0: "ok", 1: "not a JPEG file", 2: "truncated header", 3: "progressive JPEG", 4: "lossless JPEG",

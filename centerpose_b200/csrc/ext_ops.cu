@@ -4,8 +4,8 @@
 //                        (reference: DCNv2/src/cuda/dcn_v2_cuda.cu:42-172).
 //   cp_preprocess     -- batched uint8 HWC frames -> normalised fp32 NCHW network input
 //                        (reference: detectors/base_detector.py:91-148, fix_res branch); cp_preprocess_ragged does
-//                        the same for frames of different sizes in one launch, and cp_preprocess_yuv420 for NV12 / I420
-//                        frames (the colour conversion of cv2.cvtColor fused into the warp's tap fetch), and
+//                        the same for frames of different sizes in one launch, and cp_preprocess_yuv420 for YUV 4:2:0
+//                        frames (NV12 / I420, NV21 / YV12, each in limited or full range; the colour conversion of cv2.cvtColor fused into the warp's tap fetch), and
 //                        cp_preprocess_formats for the camera formats (RGB24, RGBA, BGRA, YUYV, UYVY, gray and the
 //                        Bayer mosaics), one per frame; cp_preprocess_resize_affine for a frame first resized by
 //                        cv2.resize at a test scale (fused into the warp's tap fetch);
@@ -116,14 +116,18 @@ struct PackedFetch {
 //   B = sat((y + 2116026 u) >> 20), G = sat((y - 852492 v - 409993 u) >> 20), R = sat((y + 1673527 v) >> 20)
 // 4:2:0 (COLOR_YUV2BGR_NV12 / _I420) [3 sh / 2, sw] (sh, sw even): the Y plane [sh, sw] comes first; then NV12: U, V
 // interleaved, row yy / 2, bytes (xx & ~1) and (xx | 1); I420: the U plane [sh/2, sw/2], then the V plane [sh/2, sw/2].
+// kVFirst swaps the chroma: V, U interleaved (NV21, COLOR_YUV2BGR_NV21) or the V plane first (YV12, COLOR_YUV2BGR_YV12).
+// kFull: full range (JFIF), with no cv2 4:2:0 code: the same 2x2 chroma, then cv2's COLOR_YCrCb2BGR in 14-bit fixed
+// point (tests/phone_ref.py, pinned against cv2 on every (Y, Cr, Cb)):
+//   B = sat(Y + ((29049 u + 2^13) >> 14)), G = sat(Y + ((-11698 v - 5636 u + 2^13) >> 14)), R = sat(Y + ((22987 v + 2^13) >> 14))
 // Packed 4:2:2 (COLOR_YUV2BGR_YUYV / _UYVY) [sh, sw, 2] (sw even): the pixel pair (xx & ~1, xx | 1) of a row is 4 bytes,
 // Y0 U Y1 V (YUYV) or U Y0 V Y1 (UYVY), one U, V for both pixels.  Every in-frame tap is read and converted once, before
 // the first channel is written; taps outside stay BGR 0, warpAffine's border of the converted image.
-template <int kFormat>
+template <int kLayout, bool kVFirst = false, bool kFull = false>
 struct YuvFetch {
   const uint8_t* __restrict__ img;
   int sh, sw;
-  int yv[4], u[4], v[4];      // per tap: max(Y - 16, 0) * 1220542 + 2^19, U - 128, V - 128
+  int yv[4], u[4], v[4];      // per tap: max(Y - 16, 0) * 1220542 + 2^19 (kFull: Y), U - 128, V - 128
   __device__ __forceinline__ void taps(int iy, int ix, bool in00, bool in01, bool in10, bool in11) {
     const bool in[4] = {in00, in01, in10, in11};
 #pragma unroll
@@ -132,34 +136,44 @@ struct YuvFetch {
       if (!in[k]) continue;
       const int yy = iy + (k >> 1), xx = ix + (k & 1);
       int Y, U, V;
-      if constexpr (kFormat == CP_PIX_NV12 || kFormat == CP_PIX_I420) {
+      if constexpr (kLayout == CP_PIX_NV12 || kLayout == CP_PIX_I420) {
         const uint8_t* __restrict__ chroma = img + (size_t)sh * sw;
-        if constexpr (kFormat == CP_PIX_NV12) {
+        if constexpr (kLayout == CP_PIX_NV12) {
           const size_t o = (size_t)(yy >> 1) * sw + (xx & ~1);
-          U = chroma[o];
-          V = chroma[o + 1];
+          U = chroma[o + kVFirst];
+          V = chroma[o + !kVFirst];
         } else {
           const size_t o = (size_t)(yy >> 1) * (sw >> 1) + (xx >> 1);
-          U = chroma[o];
-          V = chroma[(size_t)(sh >> 1) * (sw >> 1) + o];
+          if constexpr (kVFirst) {
+            V = chroma[o];
+            U = chroma[(size_t)(sh >> 1) * (sw >> 1) + o];
+          } else {
+            U = chroma[o];
+            V = chroma[(size_t)(sh >> 1) * (sw >> 1) + o];
+          }
         }
         Y = img[(size_t)yy * sw + xx];
       } else {
-        constexpr int kY = kFormat == CP_PIX_YUYV422 ? 0 : 1, kU = 1 - kY;    // byte of Y0 and of U in a pair
+        constexpr int kY = kLayout == CP_PIX_YUYV422 ? 0 : 1, kU = 1 - kY;    // byte of Y0 and of U in a pair
         const uint8_t* __restrict__ pair = img + ((size_t)yy * sw + (xx & ~1)) * 2;
         Y = pair[kY + 2 * (xx & 1)];
         U = pair[kU];
         V = pair[kU + 2];
       }
-      yv[k] = max(Y - 16, 0) * 1220542 + (1 << 19);
+      yv[k] = kFull ? Y : max(Y - 16, 0) * 1220542 + (1 << 19);
       u[k] = U - 128;
       v[k] = V - 128;
     }
   }
   __device__ __forceinline__ int operator()(int k, int, int, int c) const {
-    const int t = c == 0 ? yv[k] + 2116026 * u[k]
-                         : (c == 1 ? yv[k] - 852492 * v[k] - 409993 * u[k] : yv[k] + 1673527 * v[k]);
-    return max(0, min(255, t >> 20));
+    if constexpr (kFull) {
+      const int t = c == 0 ? 29049 * u[k] : (c == 1 ? -11698 * v[k] - 5636 * u[k] : 22987 * v[k]);
+      return max(0, min(255, yv[k] + ((t + (1 << 13)) >> 14)));
+    } else {
+      const int t = c == 0 ? yv[k] + 2116026 * u[k]
+                           : (c == 1 ? yv[k] - 852492 * v[k] - 409993 * u[k] : yv[k] + 1673527 * v[k]);
+      return max(0, min(255, t >> 20));
+    }
   }
 };
 
@@ -279,9 +293,14 @@ struct ResizeFetch {
   __device__ __forceinline__ int operator()(int k, int, int, int c) const { return bgr[k][c]; }
 };
 
+// The eight 4:2:0 codes: NV12, I420, and 8 plus the bits 1 (planar), 2 (V first) and 4 (full range) for the others.
+__host__ __device__ constexpr bool is_yuv420(int format) {
+  return format == CP_PIX_NV12 || format == CP_PIX_I420 || (format >= CP_PIX_NV21 && format <= CP_PIX_YV12_FULL);
+}
+
 // The bytes of one sh x sw frame in a cp_pixel_format (0 for CP_PIX_PER_FRAME or an unknown value).
 __host__ __device__ constexpr size_t frame_bytes(int format, size_t sh, size_t sw) {
-  return format == CP_PIX_NV12 || format == CP_PIX_I420     ? sh * sw * 3 / 2
+  return is_yuv420(format)                                 ? sh * sw * 3 / 2
          : format == CP_PIX_BGR || format == CP_PIX_RGB24    ? sh * sw * 3
          : format == CP_PIX_RGBA || format == CP_PIX_BGRA    ? sh * sw * 4
          : format == CP_PIX_YUYV422 || format == CP_PIX_UYVY422 ? sh * sw * 2
@@ -300,6 +319,8 @@ __device__ __forceinline__ auto make_fetch(const uint8_t* __restrict__ img, int 
     return PackedFetch<1, 0, 0, 0>{img, sw};           // COLOR_GRAY2BGR: B = G = R = Y
   else if constexpr (kFormat >= CP_PIX_BAYER_RGGB8 && kFormat <= CP_PIX_BAYER_GRBG8)
     return bayer_fetch(img, sh, sw, kFormat);
+  else if constexpr (is_yuv420(kFormat))
+    return YuvFetch<kFormat & 1 ? CP_PIX_I420 : CP_PIX_NV12, (kFormat & 2) != 0, (kFormat & 4) != 0>{img, sh, sw};
   else
     return YuvFetch<kFormat>{img, sh, sw};
 }
@@ -338,6 +359,12 @@ __device__ __forceinline__ void frame_walk(const uint8_t* __restrict__ frames, c
     switch (format) {
       case CP_PIX_NV12: walk(make_fetch<CP_PIX_NV12>(img, f.sh, f.sw)); break;
       case CP_PIX_I420: walk(make_fetch<CP_PIX_I420>(img, f.sh, f.sw)); break;
+      case CP_PIX_NV21: walk(make_fetch<CP_PIX_NV21>(img, f.sh, f.sw)); break;
+      case CP_PIX_YV12: walk(make_fetch<CP_PIX_YV12>(img, f.sh, f.sw)); break;
+      case CP_PIX_NV12_FULL: walk(make_fetch<CP_PIX_NV12_FULL>(img, f.sh, f.sw)); break;
+      case CP_PIX_I420_FULL: walk(make_fetch<CP_PIX_I420_FULL>(img, f.sh, f.sw)); break;
+      case CP_PIX_NV21_FULL: walk(make_fetch<CP_PIX_NV21_FULL>(img, f.sh, f.sw)); break;
+      case CP_PIX_YV12_FULL: walk(make_fetch<CP_PIX_YV12_FULL>(img, f.sh, f.sw)); break;
       case CP_PIX_BGR: walk(make_fetch<CP_PIX_BGR>(img, f.sh, f.sw)); break;
       case CP_PIX_RGB24: walk(make_fetch<CP_PIX_RGB24>(img, f.sh, f.sw)); break;
       case CP_PIX_RGBA: walk(make_fetch<CP_PIX_RGBA>(img, f.sh, f.sw)); break;
@@ -490,7 +517,6 @@ int preprocess_blocks(size_t total) {
   return blocks;
 }
 
-bool is_yuv420(int format) { return format == CP_PIX_NV12 || format == CP_PIX_I420; }
 bool is_yuv422(int format) { return format == CP_PIX_YUYV422 || format == CP_PIX_UYVY422; }
 bool is_bayer(int format) { return format >= CP_PIX_BAYER_RGGB8 && format <= CP_PIX_BAYER_GRBG8; }
 bool known_format(int format) {
@@ -511,6 +537,12 @@ void with_base_format(int format, F f) {
   switch (format) {
     case CP_PIX_NV12: f(std::integral_constant<int, CP_PIX_NV12>{}); break;
     case CP_PIX_I420: f(std::integral_constant<int, CP_PIX_I420>{}); break;
+    case CP_PIX_NV21: f(std::integral_constant<int, CP_PIX_NV21>{}); break;
+    case CP_PIX_YV12: f(std::integral_constant<int, CP_PIX_YV12>{}); break;
+    case CP_PIX_NV12_FULL: f(std::integral_constant<int, CP_PIX_NV12_FULL>{}); break;
+    case CP_PIX_I420_FULL: f(std::integral_constant<int, CP_PIX_I420_FULL>{}); break;
+    case CP_PIX_NV21_FULL: f(std::integral_constant<int, CP_PIX_NV21_FULL>{}); break;
+    case CP_PIX_YV12_FULL: f(std::integral_constant<int, CP_PIX_YV12_FULL>{}); break;
     case CP_PIX_BGR: f(std::integral_constant<int, CP_PIX_BGR>{}); break;
     case CP_PIX_RGB24: f(std::integral_constant<int, CP_PIX_RGB24>{}); break;
     case CP_PIX_RGBA: f(std::integral_constant<int, CP_PIX_RGBA>{}); break;
@@ -876,7 +908,7 @@ int cp_preprocess_yuv420(const uint8_t* frames, int64_t frames_bytes, const int6
                          const float mean[3], const float stdv[3], void* stream_) {
   if (!frames || !offsets || !src_hw || !out || !mean || !stdv) return fail(CP_ERR_INVALID, "cp_preprocess_yuv420: null argument");
   if (B <= 0 || dst_h <= 0 || dst_w <= 0 || frames_bytes <= 0) return fail(CP_ERR_INVALID, "cp_preprocess_yuv420: bad shape");
-  if (format != CP_PIX_NV12 && format != CP_PIX_I420)
+  if (!is_yuv420(format))
     return fail(CP_ERR_INVALID, "cp_preprocess_yuv420: unknown pixel format " + std::to_string(format));
   std::vector<RaggedFrame> fr;
   int rc = ragged_frames("cp_preprocess_yuv420", frames_bytes, offsets, src_hw, B, dst_h, dst_w, trans_input, format,

@@ -726,7 +726,10 @@ class ObjectPoseDetector(object):
         cv2.cvtColor to BGR (COLOR_RGB2BGR, _RGBA2BGR, _BGRA2BGR, COLOR_YUV2BGR_YUYV, _UYVY).  So are the sensor
         formats, one uint8 plane per frame ([B,H,W] or a list of [H_b,W_b]): "gray" (COLOR_GRAY2BGR) and the Bayer
         mosaics "bayer_rggb8" / "bayer_bggr8" / "bayer_gbrg8" / "bayer_grbg8" (H and W at least 3), named after their
-        top-left 2 x 2 block and demosaiced as cv2's bilinear COLOR_BayerBG2BGR / _RG / _GR / _GB.  With a list of frames,
+        top-left 2 x 2 block and demosaiced as cv2's bilinear COLOR_BayerBG2BGR / _RG / _GR / _GB.  So are the phone
+        formats, 4:2:0 like "nv12": "nv21" / "yv12" (COLOR_YUV2BGR_NV21 / _YV12) and the full-range "nv12_full" /
+        "nv21_full" / "i420_full" / "yv12_full" (each pixel takes its 2 x 2 block's Cb, Cr, then COLOR_YCrCb2BGR, as
+        ARKit and Android cameras deliver them; engine.check_pixel_format).  With a list of frames,
         pixel_format may also be a list of one name per frame or slot (cameras of different kinds); a list of one name
         repeated is that name.
 

@@ -607,14 +607,21 @@ def preprocess_ragged(packed_u8, offsets, src_hw, dst_h, dst_w, mean, std, out=N
                               trans_input)
 
 
-_YUV420 = {"nv12": _lib.CP_PIX_NV12, "i420": _lib.CP_PIX_I420}
+_YUV420 = {f: _lib.PIXEL_FORMAT_CODES[f] for f in _lib.YUV420_FORMATS}
 # the buffer of one H x W image in each pixel_format: [3H/2,W] for YUV 4:2:0, [H,W] for the sensor formats, else
 # [H,W,C]
-_LAYOUT = dict({"bgr": "[H,W,3]", "nv12": "[3H/2,W]", "i420": "[3H/2,W]", "rgb24": "[H,W,3]", "rgba": "[H,W,4]",
-                "bgra": "[H,W,4]", "yuyv422": "[H,W,2]", "uyvy422": "[H,W,2]"},
-               **{f: "[H,W]" for f in _lib.SENSOR_FORMATS})
+_LAYOUT = dict({"bgr": "[H,W,3]", "rgb24": "[H,W,3]", "rgba": "[H,W,4]", "bgra": "[H,W,4]", "yuyv422": "[H,W,2]",
+                "uyvy422": "[H,W,2]"}, **{f: "[H,W]" for f in _lib.SENSOR_FORMATS},
+               **{f: "[3H/2,W]" for f in _lib.YUV420_FORMATS})
 _CHANNELS = {"bgr": 3, "rgb24": 3, "rgba": 4, "bgra": 4, "yuyv422": 2, "uyvy422": 2}
-_ALL_FORMATS = _lib.PIXEL_FORMATS + _lib.SENSOR_FORMATS
+_ALL_FORMATS = _lib.PIXEL_FORMATS + _lib.SENSOR_FORMATS + _lib.PHONE_FORMATS
+
+
+def _unknown_format(f, names=None):
+    """The ValueError of an unknown pixel_format f (in the list `names`, when given)."""
+    return ValueError("pixel_format must be one of %s, got %r%s; phone cameras also give %s"
+                      % (", ".join(_lib.PIXEL_FORMATS + _lib.SENSOR_FORMATS), f,
+                         "" if names is None else " in %r" % (list(names),), ", ".join(_lib.PHONE_FORMATS)))
 
 
 # encoded JPEG frames: not a cp_pixel_format (the pre-process never sees one); run_batch(list) decodes them to BGR first
@@ -645,14 +652,16 @@ def check_pixel_format(pixel_format):
     even), a camera format named as ffmpeg's pix_fmt: "rgb24" ([H,W,3]), "rgba" / "bgra" ([H,W,4], alpha ignored),
     "yuyv422" / "uyvy422" ([H,W,2] packed YUV 4:2:2, W even), or a sensor format, one [H,W] plane: "gray" (mono) or a
     Bayer mosaic "bayer_rggb8" / "bayer_bggr8" / "bayer_gbrg8" / "bayer_grbg8" (H and W at least 3), demosaiced as
-    cv2's bilinear COLOR_Bayer??2BGR.  One name; a list (one per camera) goes through slot_formats where frames come as
-    a list."""
+    cv2's bilinear COLOR_Bayer??2BGR, or a phone format, YUV 4:2:0 [3H/2,W] as Android and ARKit give it: "nv21" /
+    "yv12" (the chroma of NV12 / I420 swapped, COLOR_YUV2BGR_NV21 / _YV12) and "nv12_full" / "nv21_full" /
+    "i420_full" / "yv12_full" (full range, JFIF: each pixel takes its 2x2 block's Cb, Cr, then COLOR_YCrCb2BGR).  One
+    name; a list (one per camera) goes through slot_formats where frames come as a list."""
     if isinstance(pixel_format, (list, tuple)):
         raise ValueError("pixel_format must be one name here, got a list %r; one name per camera goes with a list of "
                          "frames (run_batch(list), a graph built with one frame_hw per slot)" % (list(pixel_format),))
     _refuse_jpeg(pixel_format)
     if pixel_format not in _ALL_FORMATS:
-        raise ValueError("pixel_format must be one of %s, got %r" % (", ".join(_ALL_FORMATS), pixel_format))
+        raise _unknown_format(pixel_format)
     return pixel_format
 
 
@@ -666,8 +675,7 @@ def slot_formats(pixel_format, n, who="run_batch"):
     for f in pixel_format:
         _refuse_jpeg(f)
         if isinstance(f, (list, tuple)) or f not in _ALL_FORMATS:
-            raise ValueError("pixel_format must be one of %s, got %r in %r"
-                             % (", ".join(_ALL_FORMATS), f, list(pixel_format)))
+            raise _unknown_format(f, pixel_format)
     return list(pixel_format)
 
 
@@ -678,8 +686,8 @@ def frame_layout(pixel_format):
 
 def frame_shape(h, w, pixel_format):
     """The buffer shape of one h x w image in pixel_format: [h,w,3] for "bgr" / "rgb24", [h,w,4] for "rgba" / "bgra",
-    [h,w,2] for "yuyv422" / "uyvy422" (w even), [3h/2,w] for "nv12" / "i420" (h and w even), [h,w] for "gray" and the
-    Bayer mosaics (h and w at least 3); else ValueError."""
+    [h,w,2] for "yuyv422" / "uyvy422" (w even), [3h/2,w] for "nv12" / "i420" and the phone formats (h and w even),
+    [h,w] for "gray" and the Bayer mosaics (h and w at least 3); else ValueError."""
     if check_pixel_format(pixel_format) in _lib.SENSOR_FORMATS:
         m = _min_side(pixel_format)
         if h < m or w < m:
@@ -767,12 +775,14 @@ def preprocess_remap(packed_u8, offsets, src_hw, pixel_format, maps, dst_h, dst_
 
 def preprocess_yuv420(packed_u8, offsets, src_hw, pixel_format, dst_h, dst_w, mean, std, out=None, trans_input=None):
     """cp_preprocess_yuv420: preprocess_ragged for YUV 4:2:0 frames.  packed_u8: flat uint8 CUDA buffer holding frame b
-    (uint8 [3H/2,W] in pixel_format "nv12" or "i420", (H, W) = src_hw[b], both even) at byte offsets[b] -> fp32
-    [B,3,dst_h,dst_w] CUDA, frame b bit for bit what preprocess_ragged gives for cv2.cvtColor(frame, COLOR_YUV2BGR_*).
+    (uint8 [3H/2,W] in pixel_format "nv12", "i420" or a phone format (check_pixel_format), (H, W) = src_hw[b], both
+    even) at byte offsets[b] -> fp32 [B,3,dst_h,dst_w] CUDA, frame b bit for bit what preprocess_ragged gives for the
+    frame converted to BGR (cv2.cvtColor(frame, COLOR_YUV2BGR_*), or the full-range rule of check_pixel_format).
     trans_input: optional [B,2,3] forward affines; default = each frame's fix_res affine (that of `preprocess`)."""
     _lib.load()
     if pixel_format not in _YUV420:
-        raise ValueError("preprocess_yuv420: pixel_format must be 'nv12' or 'i420', got %r" % (pixel_format,))
+        raise ValueError("preprocess_yuv420: pixel_format must be 'nv12' or 'i420', or a phone format (%s), got %r"
+                         % (", ".join(_lib.PHONE_FORMATS), pixel_format))
     return _preprocess_packed("preprocess_yuv420", packed_u8, offsets, src_hw, (_YUV420[pixel_format],), dst_h, dst_w,
                               mean, std, out, trans_input)
 

@@ -118,6 +118,7 @@ class _SlotGraph(object):
             meta[b] = make_meta(1, c, sc, w, h, cams[b]).numpy()[0]
             trans[b] = affine_from_center_scale(c, sc, iw, ih).reshape(6)
         self.meta = torch.from_numpy(meta).to(dev)                   # the network's rows, one per frame
+        self._meta_host, self._distorted = meta, dists is not None    # what a per-step camera_matrix starts from
         self._mean = (ctypes.c_float * 3)(*[float(v) for v in opt.mean])
         self._std = (ctypes.c_float * 3)(*[float(v) for v in opt.std])
         mixed = isinstance(self.pixel_format, list)       # per-slot formats: a table of them, one per-frame launch
@@ -351,6 +352,49 @@ class _SlotGraph(object):
         inv[ids[:M * n]] = np.arange(M * n, dtype=np.int32)
         return np.concatenate([np.tile(start, M), rows, ids, inv]).astype(np.int32)
 
+    def _camera_rows(self, camera_matrix):
+        """The meta rows of a call's camera_matrix ([3,3] for every slot or [S,3,3], a numpy array or a CPU tensor):
+        every slot's row with its camera fields replaced, or None when it is None.  Refused before any device work: a
+        graph built with distortion= (its undistortion maps were built from the build-time cameras), another shape, a
+        non-finite value, a CUDA tensor."""
+        if camera_matrix is None:
+            return None
+        who, S = type(self).__name__, self.slots
+        if self._distorted:
+            raise ValueError("%s was built with distortion=: its undistortion maps come from the cameras it was built "
+                             "with, so it takes no per-step camera_matrix; build a graph for the new cameras" % who)
+        if torch.is_tensor(camera_matrix):
+            if camera_matrix.device.type != "cpu":
+                raise ValueError("%s: camera_matrix is read on the host: pass a numpy array or a CPU tensor, got a "
+                                 "tensor on %s" % (who, camera_matrix.device))
+            camera_matrix = camera_matrix.numpy()
+        try:
+            cam = np.asarray(camera_matrix, np.float64)
+        except (TypeError, ValueError):
+            cam = None
+        if cam is None or cam.shape not in ((3, 3), (S, 3, 3)):
+            raise ValueError("%s: camera_matrix must be [3,3] or one [3,3] per slot ([%d,3,3]), got %s"
+                             % (who, S, type(camera_matrix).__name__ if cam is None else cam.shape))
+        if not np.isfinite(cam).all():
+            raise ValueError("%s: camera_matrix holds a non-finite value" % who)
+        rows = self._meta_host.copy()
+        rows[:, 5:14] = np.broadcast_to(cam.reshape(-1, 9), (S, 9))
+        return rows
+
+    def _camera_meta(self):
+        """The device meta rows a per-step camera replaces: the network's rows (a tracking graph's also hold the tracker
+        streams' rows, one per category)."""
+        return self.meta
+
+    def _set_cameras(self, rows):
+        """One copy of the meta rows `rows` (_camera_rows) to the device, on the current stream ahead of the replay;
+        they stay in force until the next camera_matrix."""
+        dst = self._camera_meta()
+        src = np.tile(rows, (dst.shape[0] // self.slots, 1))
+        # a pageable source: staged before copy_ returns, without waiting for the device
+        dst.copy_(torch.from_numpy(src), non_blocking=True)
+        self._meta_host = rows
+
     def reset(self):
         """Forget every slot's tracks and previous frame: the next call starts a video in every slot (with idle slots:
         each slot's next live frame starts its video)."""
@@ -411,9 +455,12 @@ class _SlotGraph(object):
             out.append(f)
         return out
 
-    def _replay(self, frames, start=None):
-        """Copies the checked frames of a call (and, when given, the start flags: int32 [S]) and replays the step; with
-        idle slots, _call_rows.  Returns self._out."""
+    def _replay(self, frames, start=None, cameras=None):
+        """Copies the checked frames of a call (and, when given, the start flags: int32 [S], and the meta rows of a
+        camera_matrix: _camera_rows) and replays the step; with idle slots, _call_rows.  Returns self._out."""
+        if cameras is not None:
+            with torch.cuda.device(self.device):
+                self._set_cameras(cameras)
         if self.idle_slots:
             return self._call_rows(frames, start)
         with torch.cuda.device(self.device):
@@ -565,14 +612,18 @@ class DetectGraph(_SlotGraph):
         self._gather(self.poses_rows.view((MS,) + rec), self.poses.view((MS,) + rec), MS, self.inv)
         self._gather(self.n_valid_rows.view(MS, 1), self.n_valid.view(MS, 1), MS, self.inv)
 
-    def __call__(self, frames, new_video=None, pre_dets=None):
+    def __call__(self, frames, new_video=None, pre_dets=None, camera_matrix=None):
         """The next frame of every camera -> (poses [S,K,192], n_valid [S]) ([M,S,...] in MultiCategoryDetectGraph):
         views of the graph's own buffers, overwritten by the next call.  frames: one array (one frame_hw) or a list of
-        one frame per slot (one frame_hw per slot, or idle slots: None for an idle camera)."""
+        one frame per slot (one frame_hw per slot, or idle slots: None for an idle camera).  camera_matrix: None (the
+        cameras in force), or [3,3] / [S,3,3] (numpy or a CPU tensor), the cameras of this step and the later ones
+        (cameras whose intrinsics change with focus, as phones report them per frame); every step is run_batch with the
+        cameras in force.  A graph built with distortion= refuses it."""
         if new_video is not None or pre_dets is not None:
             raise ValueError("%s keeps nothing from one frame to the next: new_video and pre_dets are tracking "
                              "arguments (TrackGraph, run_batch(track=True))" % type(self).__name__)
-        return self._replay(self._frames(frames))
+        frames = self._frames(frames)
+        return self._replay(frames, cameras=self._camera_rows(camera_matrix))
 
 
 class MultiCategoryDetectGraph(DetectGraph):

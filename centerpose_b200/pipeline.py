@@ -30,7 +30,8 @@ Both take `pixel_format="nv12"` or `"i420"` for YUV 4:2:0 frames as video decode
 frame, H and W even): they are uploaded as they are, half the bytes of BGR, and converted inside the pre-process
 kernel; the results equal those of the same frames converted by cv2.cvtColor and submitted as BGR.  The camera and
 sensor formats of engine.check_pixel_format work the same way; a Bayer mosaic or "gray" frame is uint8 [H,W], a third
-of the bytes of BGR.
+of the bytes of BGR, and a phone format ("nv21", "yv12", "nv12_full", "nv21_full", "i420_full", "yv12_full") is 4:2:0
+like "nv12".
 
 Both take `distortion=` (lens.LensDistortion, one for every camera or one per frame / slot) for cameras with lens
 distortion: the frames are undistorted inside the pre-process exactly as run_batch(distortion=) does.

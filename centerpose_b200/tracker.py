@@ -371,7 +371,8 @@ class TrackGraph(_SlotGraph):
     frame_hw: one (H, W) for every slot, or a list of S (H_s, W_s).  camera_matrix: [3,3] for every slot or [S,3,3].
       - One size: a call takes the frames as one array, uint8 [S,H,W,3] for pixel_format "bgr", [S,3H/2,W] for "nv12" /
         "i420" (H, W even), [S,H,W,C] for a camera format ("rgb24", "rgba", "bgra", "yuyv422", "uyvy422"), [S,H,W] for
-        a sensor format ("gray", "bayer_rggb8", "bayer_bggr8", "bayer_gbrg8", "bayer_grbg8"); one copy and the uniform
+        a sensor format ("gray", "bayer_rggb8", "bayer_bggr8", "bayer_gbrg8", "bayer_grbg8"), [S,3H/2,W] for a phone
+        format ("nv21", "yv12", "nv12_full", "nv21_full", "i420_full", "yv12_full"); one copy and the uniform
         pre-process (cp_preprocess_slots_dev).
       - One size per slot: a call takes a list of S frames, uint8 [H_s,W_s,3] or [3H_s/2,W_s] (...), each copied into
         its own region of one packed device buffer; the step is that of run_batch(list, track=True) with every slot
@@ -425,7 +426,11 @@ class TrackGraph(_SlotGraph):
         S, MS, dev = self.slots, self.streams, self.device
         M, ih, iw = MS // S, opt.input_h, opt.input_w
         self.tracker = Tracker(opt, streams=S, device=dev, categories=self.categories)
-        self.meta_all = self.meta if M == 1 else torch.from_numpy(np.tile(meta, (M, 1))).to(dev)
+        if M > 1:                                        # the network's rows are category 0's: one buffer to update
+            self.meta_all = torch.from_numpy(np.tile(meta, (M, 1))).to(dev)
+            self.meta = self.meta_all[:S]
+        else:
+            self.meta_all = self.meta
         self.trans = torch.from_numpy(np.tile(trans, (M, 1))).to(dev)
         mode = _lib.RENDER_EMPTY if getattr(opt, "empty_pre_hm", False) else _lib.RENDER_TRACKS
         self.modes = torch.full((MS,), mode, dtype=torch.int32, device=dev)
@@ -449,6 +454,9 @@ class TrackGraph(_SlotGraph):
             self.tracks_rows, self.n_tracks_rows = torch.zeros_like(self.tracks), torch.zeros_like(self.n_tracks)
         out_lead = (S,) if self.categories is None else (M, S)
         self._out = (self.tracks.view(out_lead + self.tracks.shape[1:]), self.n_tracks.view(out_lead))
+
+    def _camera_meta(self):
+        return self.meta_all
 
     def _warmed(self):
         if self.idle_slots:                      # the warm-ups stepped every stream: start from nothing
@@ -503,11 +511,13 @@ class TrackGraph(_SlotGraph):
             self._gather(self.tracks_rows, self.tracks, MS, self.inv)
             self._gather(self.n_tracks_rows.view(MS, 1), self.n_tracks.view(MS, 1), MS, self.inv)
 
-    def __call__(self, frames, new_video=None, pre_dets=None):
+    def __call__(self, frames, new_video=None, pre_dets=None, camera_matrix=None):
         """The next frame of every slot -> (tracks [S,T,320], n_tracks [S]) ([M,S,...] in MultiCategoryTrackGraph):
         views of the graph's own buffers, overwritten by the next call.  frames: one array (one frame_hw) or a list of
         one frame per slot (one frame_hw per slot).  new_video: None or one bool per slot (slot i starts a new video
-        with this frame)."""
+        with this frame).  camera_matrix: None (the cameras in force), or [3,3] / [S,3,3] (numpy or a CPU tensor), the
+        cameras of this step and the later ones, read by the network's PnP and the tracker's alike; every step is
+        run_batch(track=True) with the cameras in force.  A graph built with distortion= refuses it."""
         who = type(self).__name__
         if pre_dets is not None:
             raise NotImplementedError("%s does not seed tracks; pre_dets seeding runs through %s" % (who, self._host_step))
@@ -518,7 +528,7 @@ class TrackGraph(_SlotGraph):
             if len(new_video) != self.slots:
                 raise ValueError("%s: %d new_video entries for %d slots" % (who, len(new_video), self.slots))
             start |= np.array(new_video, np.int32)
-        return self._replay(frames, start)
+        return self._replay(frames, start, self._camera_rows(camera_matrix))
 
 
 class MultiCategoryTrackGraph(TrackGraph):

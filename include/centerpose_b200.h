@@ -668,12 +668,24 @@ int cp_preprocess_ragged(const uint8_t* frames, int64_t frames_bytes, const int6
                          const float mean[3], const float std[3], void* stream);
 
 /* YUV 4:2:0 frames as video decoders and cameras produce them, in cv2's layouts: one uint8 [3H/2, W] buffer per frame,
- * the Y plane [H, W] first, then
+ * H and W even, the Y plane [H, W] first, then
  *   CP_PIX_NV12: interleaved chroma rows [H/2, W], U at even and V at odd bytes (NVDEC's and most cameras' output);
- *   CP_PIX_I420: the U plane [H/2, W/2], then the V plane [H/2, W/2] (ffmpeg's yuv420p). */
+ *   CP_PIX_I420: the U plane [H/2, W/2], then the V plane [H/2, W/2] (ffmpeg's yuv420p).
+ * Phone cameras give the same two layouts with the chroma swapped, and in full range.  Those codes are 8 plus three
+ * bits: 1 the planar layout (I420), 2 V before U, 4 full range; 8 and 9 are not formats.  Limited range (BT.601, Y in
+ * 16..235) is cv2's COLOR_YUV2BGR_* conversion.  Full range (JFIF: Y, Cb, Cr in 0..255) has no 4:2:0 code in cv2; it
+ * is each pixel taking the Cb, Cr of its 2x2 block, then cv2.cvtColor([Y, Cr, Cb], COLOR_YCrCb2BGR), which is exactly
+ *   R = sat(Y + ((Cr' 22987 + 2^13) >> 14)), G = sat(Y + ((Cr' -11698 + Cb' -5636 + 2^13) >> 14)),
+ *   B = sat(Y + ((Cb' 29049 + 2^13) >> 14)), with Cr' = Cr - 128, Cb' = Cb - 128 and an arithmetic shift. */
 enum cp_pixel_format {
   CP_PIX_NV12 = 0,
   CP_PIX_I420 = 1,
+  CP_PIX_NV21 = 10,         /* NV12 with V at even and U at odd bytes (Android's Camera1 default): COLOR_YUV2BGR_NV21 */
+  CP_PIX_YV12 = 11,         /* the V plane, then the U plane (Android's YV12): COLOR_YUV2BGR_YV12 */
+  CP_PIX_NV12_FULL = 12,    /* NV12 in full range (ARKit's 420YpCbCr8BiPlanarFullRange) */
+  CP_PIX_I420_FULL = 13,    /* I420 in full range (ffmpeg's yuvj420p) */
+  CP_PIX_NV21_FULL = 14,    /* NV21 in full range (Android's camera HAL: JFIF) */
+  CP_PIX_YV12_FULL = 15,    /* YV12 in full range */
   CP_PIX_BGR = 2,  /* interleaved uint8 [H, W, 3]; taken by cp_preprocess_slots_dev and cp_preprocess_slots_ragged_dev
                     * (cp_preprocess_yuv420 refuses it) */
   /* Camera formats, ffmpeg's pix_fmt names; one uint8 [H, W, C] buffer per frame.  Each is converted to BGR inside the
@@ -700,12 +712,13 @@ enum cp_pixel_format {
    * (cp_preprocess_frame_table_maps) */
   CP_PIX_REMAP = 128
 };
-/* cp_preprocess_ragged on YUV 4:2:0 frames: frame b is [src_hw[b][0] * 3 / 2, src_hw[b][1]] uint8 in `format`, i.e.
- * src_hw[b][0] * src_hw[b][1] * 3 / 2 bytes starting `offsets[b]` bytes into `frames`; src_hw holds the IMAGE sizes
- * (H, W), which must be even.  Frame b's output equals, bit for bit, cp_preprocess_ragged on
- * cv2.cvtColor(frame, COLOR_YUV2BGR_NV12 / COLOR_YUV2BGR_I420) with the same trans_input (NULL: each frame's fix_res
- * affine).  The conversion (BT.601 limited range, 20-bit fixed point, one U, V per 2x2 block, as cv2) runs inside the
- * warp on the four taps of every output pixel; taps outside the frame are BGR 0, like warpAffine's border.  An odd size,
+/* cp_preprocess_ragged on YUV 4:2:0 frames: frame b is [src_hw[b][0] * 3 / 2, src_hw[b][1]] uint8 in `format` (any of
+ * the eight 4:2:0 codes), i.e. src_hw[b][0] * src_hw[b][1] * 3 / 2 bytes starting `offsets[b]` bytes into `frames`;
+ * src_hw holds the IMAGE sizes (H, W), which must be even.  Frame b's output equals, bit for bit, cp_preprocess_ragged on
+ * the frame converted to BGR as the format's comment says (cv2.cvtColor(frame, COLOR_YUV2BGR_NV12 / _I420 / _NV21 /
+ * _YV12) in limited range) with the same trans_input (NULL: each frame's fix_res affine).  The conversion (one U, V per
+ * 2x2 block, as cv2; BT.601 limited range in 20-bit fixed point, or full range in 14-bit) runs inside the warp on the
+ * four taps of every output pixel; taps outside the frame are BGR 0, like warpAffine's border.  An odd size,
  * an unknown format or a frame that does not fit inside frames_bytes returns CP_ERR_INVALID before any work is enqueued.
  * A uniform batch is the case of equal sizes. */
 int cp_preprocess_yuv420(const uint8_t* frames, int64_t frames_bytes, const int64_t* offsets, const int32_t* src_hw,
@@ -727,7 +740,7 @@ int cp_preprocess_formats(const uint8_t* frames, int64_t frames_bytes, const int
  * frames of one image size (src_h, src_w) in `format` (cp_pixel_format; YUV 4:2:0 needs an even size, a Bayer mosaic at
  * least 3 x 3), frame b at byte b * (bytes of one frame).  trans_input: HOST row-major 2x3 forward affine for every
  * frame, read before the call returns (NULL: the fix_res affine of the size, as cp_preprocess).  out: device fp32
- * [B,3,dst_h,dst_w], frame b bit for bit what cp_preprocess_affine (BGR), cp_preprocess_yuv420 (NV12 / I420) or
+ * [B,3,dst_h,dst_w], frame b bit for bit what cp_preprocess_affine (BGR), cp_preprocess_yuv420 (the 4:2:0 formats) or
  * cp_preprocess_formats gives for it.  start: device int32 [B] read when the kernel runs, or NULL; where start[b] != 0
  * frame b's output is written to prev[b] (device fp32 [B,3,dst_h,dst_w]) as well: a slot whose video starts with this
  * frame takes it as its previous frame.  start and prev are both given or both NULL.  Bad arguments return CP_ERR_INVALID
@@ -749,8 +762,8 @@ int cp_preprocess_slots_dev(const uint8_t* frames, int32_t format, int32_t B, in
  *   - cp_preprocess_slots_ragged_dev, the captured call: frames (a device buffer of at least frames_bytes bytes, laid out
  *     as the table says), the table and start are device memory read when the kernel runs, nothing is allocated and no
  *     host memory is read after the call returns.  `format` must be the one the table was built for.  out: device fp32
- *     [B,3,dst_h,dst_w], frame b bit for bit what cp_preprocess_ragged (CP_PIX_BGR) or cp_preprocess_yuv420 (NV12 /
- *     I420) gives for it with the same offsets, sizes and affines.  start / prev as in cp_preprocess_slots_dev: where
+ *     [B,3,dst_h,dst_w], frame b bit for bit what cp_preprocess_ragged (CP_PIX_BGR) or cp_preprocess_yuv420 (the
+ *     4:2:0 formats) gives for it with the same offsets, sizes and affines.  start / prev as in cp_preprocess_slots_dev: where
  *     start[b] != 0 frame b's output is written to prev[b] as well, other rows of prev are not touched; both given or
  *     both NULL.  Bad arguments return CP_ERR_INVALID before any work is enqueued. */
 int64_t cp_preprocess_frame_table_bytes(int32_t B);
